@@ -18,6 +18,7 @@
  *   wn_postprocess_u8     hubconf.py:24-34         ten2arr_noeinops (clip, *255, truncate, NCHW->NHWC)
  *   wn_enhance_u8         hubconf.py:85-94 + net.py:99-108: preprocess -> model -> postprocess
  *                         (the per-frame body of inference.py:261-323)
+ *   wn_enhance_u8_tiled   the same, computed in overlapping windows: bounded workspace for images of any size
  *   wn_forward_train /    train.py:108 `out = model(...)` and train.py:130-131 `loss.backward()`
  *   wn_backward           (autograd through net.py:99-108)
  *
@@ -38,7 +39,7 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 3
+#define WN_ABI_VERSION 4
 
 #define WN_OK 0
 #define WN_E_INVALID (-1)   /* bad argument (NULL pointer, non-positive size, unknown mode) */
@@ -148,6 +149,25 @@ size_t wn_enhance_workspace_bytes(int n, int h, int w, int mode);
 int wn_enhance_u8(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, float* out_f32_or_null,
                   int n, int height, int width, int mode, void* workspace, size_t workspace_bytes,
                   void* stream);
+
+/*
+ * wn_enhance_u8 with a workspace that does not grow with the image: the same bits, computed in windows.
+ * wn_enhance_u8 runs whole images per pass (~1.9 KB of workspace per pixel, so one 45 MP photo needs more than
+ * an 80 GB card).  Every output pixel depends on the input within 13 pixels, so each image is cut into balanced
+ * output tiles of at most tile_h x tile_w, each computed from a window that extends it by up to 13 pixels per side
+ * (clamped into the image; all windows of a call have one size).  The statistics of the preprocess (white balance,
+ * CLAHE) are taken over the full images.  A pass runs as many windows as fit in max_pass_pixels (0 = 8 Mi pixels;
+ * at least one window); the workspace is that pass plus ~84 KB per image of LUTs, whatever the image size.  With
+ * tile 998 x 998 a window is at most 1024 x 1024.  The result equals wn_enhance_u8's bit for bit.
+ * Tensor-core modes only (WN_MODE_FP32_SIMT: WN_E_UNSUPPORTED); no peer outputs.  max_pass_pixels is this call's
+ * own argument (wn_set_chunk_pixels does not apply), so that the workspace function and the call agree.
+ * The workspace function returns 0 for arguments the call rejects.
+ */
+size_t wn_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
+                                        int mode);
+int wn_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, float* out_f32_or_null,
+                        int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels,
+                        int mode, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * wn_enhance_u8 with the all-gather of the output fused into the kernel that produces it (SURVEY 8e: the one

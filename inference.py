@@ -107,6 +107,9 @@ def main():
     ap.add_argument("--name", type=str, help="(Optional) Subfolder name to save under `./output`.")
     ap.add_argument("--show-split", action="store_true", default=False,
                     help="(Optional) Left/right of output is original/processed, with a before/after watermark.")
+    ap.add_argument("--tile", type=int, default=None,
+                    help="(Optional) Compute each image in overlapping tiles of at most N x N output pixels: the same "
+                         "result with GPU memory that does not grow with the image size (e.g. 998 for large photos).")
     args = ap.parse_args()
     assert args.source is not None, "No input image/video specified in --source!"
     if not torch.cuda.is_available():
@@ -114,7 +117,7 @@ def main():
     print("Using device: cuda")
     import cv2  # file / codec I/O only
 
-    enhancer = Enhancer(load_model(args.weights))
+    enhancer = Enhancer(load_model(args.weights), tile=args.tile)
     source = Path(args.source)
     assert source.exists(), f"{args.source} does not exist!"
     files = [source] if not source.is_dir() else [

@@ -19,7 +19,7 @@ MODE_BF16_FP8 = 2
 MODE_DEFAULT = -1
 NUM_PARAMS = 34
 NUM_TIMING_SLOTS = 23
-ABI_VERSION = 3
+ABI_VERSION = 4
 PEER_HANDLE_BYTES = 64  # WN_PEER_HANDLE_BYTES
 MAX_PEERS = 15          # WN_MAX_PEERS
 
@@ -48,6 +48,9 @@ _SIGNATURES = {
                               c_void_p, c_size_t, c_void_p]),
     "wn_enhance_u8_peers": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_int, c_int, c_int, c_int,
                                     c_int, c_void_p, c_size_t, c_void_p]),
+    "wn_enhance_tiled_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong, c_int]),
+    "wn_enhance_u8_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                    ctypes.c_longlong, c_int, c_void_p, c_size_t, c_void_p]),
     "wn_launch_count": (c_uint64, [c_void_p]),
     "wn_submodule_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "wn_confidence_maps": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p,

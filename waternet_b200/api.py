@@ -43,16 +43,25 @@ class Enhancer:
     For small frames the ~15 kernel launches of one enhance call cost more host time than the GPU
     needs to run them; with ``cuda_graph=True`` (default for batches up to ``GRAPH_MAX_PIXELS``) the
     launch sequence is captured once per input shape into a CUDA graph and replayed.
+
+    ``tile``: ``None`` runs whole images per pass (``Engine.enhance``).  An int or (h, w) runs the tiled forward
+    (``Engine.enhance_tiled``: the same bits, with a workspace that does not grow with the image size -- for photos
+    and frames too large for one pass) one image per pipelined pass, so that image i+1's copy-in runs under image
+    i's kernels; it never captures a graph.  Tensor-core precisions only.
     """
 
     GRAPH_MAX_PIXELS = 1 << 20
 
-    def __init__(self, model, device=None, precision: Optional[str] = None, cuda_graph: bool = True, depth: int = 2):
+    def __init__(self, model, device=None, precision: Optional[str] = None, cuda_graph: bool = True, depth: int = 2,
+                 tile=None):
         if device is not None:
             model = model.to(device)
         self.model = model
         self.engine: Engine = model.engine()  # raises without CUDA: there is no CPU path
         self.mode = model._mode() if precision is None else MODES[precision]
+        self.tile = None if tile is None else Engine._tile_hw(tile)
+        if self.tile is not None and self.mode == _lib.MODE_FP32_SIMT:
+            raise ValueError("tile: the tiled forward runs in the tensor-core precisions only, not fp32")
         self.cuda_graph = cuda_graph
         self._slots: List[_Slot] = [_Slot() for _ in range(max(1, depth))]
         self._next = 0
@@ -84,6 +93,9 @@ class Enhancer:
         """preprocess -> forward -> ten2arr of images [a, b) of the slot (graph replay when small)."""
         src, dst = slot.dev_in[a:b], slot.dev_out[a:b]
         shape = tuple(slot.dev_in.shape)
+        if self.tile is not None:
+            eng.enhance_tiled(src, tile=self.tile, mode=self.mode, out_u8=dst)
+            return
         if peer_out or not (self.cuda_graph and whole and shape[0] * shape[1] * shape[2] <= self.GRAPH_MAX_PIXELS):
             eng.enhance(src, mode=self.mode, out_u8=dst, peer_out=peer_out)
             return
@@ -120,6 +132,8 @@ class Enhancer:
         """
         if pin_in.dtype != torch.uint8 or pin_in.dim() != 4 or pin_in.shape[3] != 3 or pin_in.shape != pin_out.shape:
             raise ValueError(f"expected uint8 (N,H,W,3) pinned tensors of one shape, got {tuple(pin_in.shape)}")
+        if exchange is not None and self.tile is not None:
+            raise ValueError("exchange: the fused multi-GPU exchange is not available with tile")
         eng = self.model.engine()  # re-packs if the parameters changed since the last call (no-op otherwise)
         dev = eng.device
         slot = self._slots[self._next % len(self._slots)]
@@ -140,7 +154,7 @@ class Enhancer:
             slot.done = torch.cuda.Event()
             slot.done.record(cur)
             return slot
-        nb = eng.chunk_images(n, h, w)
+        nb = 1 if self.tile is not None else eng.chunk_images(n, h, w)
         self._s_in.wait_stream(cur)   # whatever the caller enqueued before (e.g. filling pin_in on the device side)
         self._s_out.wait_stream(cur)
         for a in range(0, n, nb):

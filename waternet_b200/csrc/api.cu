@@ -327,6 +327,47 @@ int wn_enhance_u8_peers(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, flo
   return mirror_u8(h, out_nhwc, peers, (size_t)n * height * width * 3, nullptr, (cudaStream_t)stream);
 }
 
+size_t wn_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
+                                        int mode) {
+  const int m = resolve_mode(mode);
+  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) return 0;
+  return umma_enhance_tiled_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels);
+}
+
+int wn_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, float* out_f32_or_null, int n,
+                        int height, int width, int tile_h, int tile_w, long long max_pass_pixels, int mode,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h || !rgb || !out_nhwc || !workspace) {
+    set_error("wn_enhance_u8_tiled: null argument");
+    return WN_E_INVALID;
+  }
+  if (n <= 0 || height <= 0 || width <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
+    set_error("wn_enhance_u8_tiled: bad shape n=%d h=%d w=%d tile=%dx%d max_pass_pixels=%lld", n, height, width,
+              tile_h, tile_w, max_pass_pixels);
+    return WN_E_INVALID;
+  }
+  const int m = resolve_mode(mode);
+  if (m == WN_MODE_FP32_SIMT) {
+    set_error("wn_enhance_u8_tiled: the tiled forward runs in the tensor-core modes only, not WN_MODE_FP32_SIMT");
+    return WN_E_UNSUPPORTED;
+  }
+  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) {
+    set_error("wn_enhance_u8_tiled: unknown mode %d", mode);
+    return WN_E_INVALID;
+  }
+  if (!h->packed) {
+    set_error("wn_enhance_u8_tiled: wn_pack_weights has not been called");
+    return WN_E_STATE;
+  }
+  if ((size_t)height * width > (size_t)0x7fffffff / 3 || n > 65535) {
+    set_error("image too large: n=%d h=%d w=%d", n, height, width);
+    return WN_E_UNSUPPORTED;
+  }
+  DeviceGuard guard(h->device);
+  return umma_enhance_u8_tiled(h, rgb, out_nhwc, out_f32_or_null, n, height, width, tile_h, tile_w, max_pass_pixels,
+                               workspace, workspace_bytes, (cudaStream_t)stream, m == WN_MODE_BF16_FP8 ? 1 : 0);
+}
+
 // ---- the reference's callable sub-modules (net.py:45-56 ConfidenceMapGenerator.forward, :75-80 Refiner.forward)
 size_t wn_submodule_workspace_bytes(int n, int h, int w, int mode) {
   if (n <= 0 || h <= 0 || w <= 0) return 0;

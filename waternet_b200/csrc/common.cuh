@@ -6,6 +6,7 @@
 #include <stdio.h>
 
 #include "../../include/waternet_b200.h"
+#include "tiling.cuh"
 
 namespace wn {
 
@@ -136,6 +137,13 @@ int resize_u8(wn_handle* h, const uint8_t* const* src, const int* src_h, const i
 // (8 bf16 levels 0..255: plane 0 = x.rgb wb.rgb he.rg, plane 1 = he.b gc.rgb 0 0 0 0)
 int preprocess_u8_planes(wn_handle* h, const uint8_t* rgb, int n, int height, int width, uint4* planes,
                          void* workspace, size_t workspace_bytes, cudaStream_t stream);
+// the same split in two for the tiled forward: the statistics and LUTs of all n images once, then the operand planes
+// of `count` windows (win0, win0 + 1, ...) of `tiles` per pass, read from the full images at image coordinates
+// (workspace: that of preprocess_u8_luts, untouched in between)
+int preprocess_u8_luts(wn_handle* h, const uint8_t* rgb, int n, int height, int width, void* workspace,
+                       size_t workspace_bytes, cudaStream_t stream);
+int preprocess_u8_window_planes(wn_handle* h, const uint8_t* rgb, int n, const TileGeom& tiles, long long win0,
+                                int count, uint4* planes, void* workspace, cudaStream_t stream);
 
 // conv_simt.cu
 int simt_pack_weights(wn_handle* h, const float* const* params, cudaStream_t stream);
@@ -175,6 +183,8 @@ struct FwdOpts {
   uint8_t* out_u8 = nullptr;   // the last launch also writes ten2arr(out) as uint8 NHWC
   PeerOut peers = {};          // ... and the same bytes to every peer address (offsets as out_u8)
   int stack = kStackAll;       // kStackCmg: stop after the confidence maps; kStackRefiners: refiners only
+  const TileGeom* tiles = nullptr;  // tiled forward: image n of the batch is window win0 + n of these tiles, and the
+  long long win0 = 0;               // last launch stores its kept rectangle into out / out_u8 at image coordinates
 };
 int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out, int n,
                         int height, int width, const FwdBuffers& b, cudaStream_t stream,
@@ -196,6 +206,11 @@ int mirror_u8(wn_handle* h, const uint8_t* src, const PeerOut& peers, size_t byt
 int umma_enhance_u8(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* out_f32, int n, int height,
                     int width, void* workspace, size_t workspace_bytes, cudaStream_t stream, int scheme,
                     const PeerOut& peers = PeerOut());
+// 0 when the arguments are out of range (tiles < 1, an image over the preprocess limit)
+size_t umma_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels);
+int umma_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* out_f32, int n, int height,
+                          int width, int tile_h, int tile_w, long long max_pass_pixels, void* workspace,
+                          size_t workspace_bytes, cudaStream_t stream, int scheme);
 int umma_f8_overflowed(const wn_handle* h);
 
 // conv_bwd.cu

@@ -333,6 +333,11 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
     a.out_u8 = o.out_u8;
     a.cm = o.stack == kStackRefiners ? nullptr : b.cm;
     a.refined_out = b.refined;
+    if (o.tiles) {
+      a.tiled = 1;
+      a.tiles = *o.tiles;
+      a.win0 = o.win0;
+    }
   };
   const bool want_cmg = o.stack != kStackRefiners, want_ref = o.stack != kStackCmg;
   // fp8-correction scheme (inference): the tensor-bound layers replace the two bf16 correction passes by one
@@ -532,6 +537,63 @@ int umma_enhance_u8(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* ou
     o.peers.n = peers.n;
     for (int k = 0; k < peers.n; k++) o.peers.p[k] = peers.p[k] + (size_t)n0 * H * W * 3;
     rc = umma_pass(h, no_in, none, out_f32 ? out_f32 + (size_t)n0 * 3 * H * W : nullptr, cur, H, W, b, stream, o);
+    if (rc) return rc;
+  }
+  return mirror_overflow(h, scheme, stream);
+}
+
+// The tiled form (tiling.cuh): the statistics and LUTs of all n images once, then per pass a batch of equally sized
+// windows runs through the same ten launches (and range guard) as a batch of images, and the last launch stores
+// each window's kept rectangle into the full-image outputs.  Workspace: one pass of windows plus the per-image
+// LUTs, independent of the image size.  The geometry is arithmetic on the window index: nothing is copied from the
+// host, so the call stays stream-ordered and can be captured in a graph.
+size_t umma_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels) {
+  if (n <= 0 || h <= 0 || w <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) return 0;
+  if ((size_t)h * w > (size_t)0x7fffffff / 3 || n > 65535) return 0;
+  const TileGeom g = tile_geom(h, w, tile_h, tile_w);
+  const long long p = tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels);
+  return (size_t)p * g.win_h * g.win_w * kUmmaBytesPerPixel + 4096 + (preprocess_workspace_bytes(n, h, w) + 255) / 256 * 256 +
+         1024;
+}
+
+int umma_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* out_f32, int n, int H, int W,
+                          int tile_h, int tile_w, long long max_pass_pixels, void* workspace, size_t workspace_bytes,
+                          cudaStream_t stream, int scheme) {
+  if (!h->umma) {
+    set_error("tensor-core weights have not been packed");
+    return WN_E_STATE;
+  }
+  const size_t need = umma_enhance_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels);
+  if (workspace_bytes < need) {
+    set_error("tiled enhance workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  int rc = get_encoder();
+  if (rc) return rc;
+  scheme = effective_scheme(h, scheme);
+  const TileGeom g = tile_geom(H, W, tile_h, tile_w);
+  const long long total = (long long)n * g.ny * g.nx;
+  const long long per_pass = tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels);
+  uint8_t* pre_ws = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
+  const size_t pre_b = (preprocess_workspace_bytes(n, H, W) + 255) / 256 * 256;
+  void* fwd_ws = pre_ws + pre_b;
+  if ((rc = preprocess_u8_luts(h, rgb, n, H, W, pre_ws, pre_b, stream))) return rc;
+  const int64_t none[4][4] = {};
+  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (long long w0 = 0; w0 < total; w0 += per_pass) {
+    const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
+    FwdBuffers b = carve(fwd_ws, cur, g.win_h, g.win_w);
+    WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));
+    rc = preprocess_u8_window_planes(h, rgb, n, g, w0, cur, b.act0, pre_ws, stream);
+    if (rc) return rc;
+    FwdOpts o;
+    o.scheme = scheme;
+    o.packed = true;
+    o.hi_only = true;
+    o.out_u8 = out_u8;
+    o.tiles = &g;
+    o.win0 = w0;
+    rc = umma_pass(h, no_in, none, out_f32, cur, g.win_h, g.win_w, b, stream, o);
     if (rc) return rc;
   }
   return mirror_overflow(h, scheme, stream);

@@ -323,11 +323,14 @@ __device__ __forceinline__ void store_level_planes(uint4* planes, size_t n, size
   p[plane] = make_uint4(bf16_levels2(lv[8], lv[9]), bf16_levels2(lv[10], lv[11]), 0u, 0u);
 }
 
-template <bool VEC4>
+// WIN (the tiled forward): blockIdx.y is window win0 + blockIdx.y of `tiles`; the kernel writes that window's operand
+// planes (out.planes only), reading the full image and interpolating its CLAHE tiles at image coordinates
+template <bool VEC4, bool WIN = false>
 __global__ void __launch_bounds__(256)
 apply_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw,
              const Tables* __restrict__ tables, const uint8_t* __restrict__ clahe_lut,
-             const uint8_t* __restrict__ wb_lut, ApplyOut out, int iters) {
+             const uint8_t* __restrict__ wb_lut, ApplyOut out, int iters, TileGeom tiles, long long win0) {
+  static_assert(!(VEC4 && WIN), "the windowed form has no vector path");
   __shared__ __align__(16) uint8_t s_clahe[64 * 256];
   __shared__ __align__(16) uint8_t s_wb[768];
   __shared__ __align__(16) uint8_t s_gamma[256];
@@ -337,7 +340,9 @@ apply_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw,
   __shared__ int16_t s_ytab[256];
   __shared__ int16_t s_fytab[256];
   __shared__ float s_div[256];
-  const int tid = threadIdx.x, n = blockIdx.y;
+  TileWindow win = {};
+  if constexpr (WIN) win = tile_window(tiles, win0 + blockIdx.y);
+  const int tid = threadIdx.x, n = WIN ? win.img : blockIdx.y;
   {
     const uint4* src = reinterpret_cast<const uint4*>(clahe_lut + (size_t)n * 64 * 256);
     uint4* dst = reinterpret_cast<uint4*>(s_clahe);
@@ -423,6 +428,19 @@ apply_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw,
         q[1] = (uint32_t)a1[1] | ((uint32_t)a1[2] << 8) | ((uint32_t)a2[0] << 16) | ((uint32_t)a2[1] << 24);
         q[2] = (uint32_t)a2[2] | ((uint32_t)a3[0] << 8) | ((uint32_t)a3[1] << 16) | ((uint32_t)a3[2] << 24);
       }
+    }
+  } else if constexpr (WIN) {
+    // pixel pix of the window is image pixel (ys + y, xs + x); planes [window of the pass][2][win_h * win_w]
+    const int wplane = tiles.win_h * tiles.win_w;
+    for (int it = 0; it < iters; it++) {
+      const int pix = (blockIdx.x * iters + it) * 256 + tid;
+      if (pix >= wplane) break;
+      const int wy = pix / tiles.win_w;
+      const int ipix = (win.ys + wy) * W + win.xs + (pix - wy * tiles.win_w);
+      const uint8_t* p = rgb + ((size_t)n * plane + ipix) * 3;
+      int lv[12];
+      one_pixel(ipix, p[0], p[1], p[2], lv);
+      store_level_planes(out.planes, blockIdx.y, wplane, pix, lv);
     }
   } else {
     for (int it = 0; it < iters; it++) {
@@ -556,9 +574,26 @@ int preprocess_u8_planes(wn_handle* h, const uint8_t* rgb, int n, int H, int W, 
                         workspace, workspace_bytes, stream, 0);
 }
 
-static int preprocess_run(wn_handle* h, const uint8_t* rgb, int n, int H, int W, float* x, float* wb,
-                          float* he, float* gc, uint8_t* wb_u8, uint8_t* he_u8, uint8_t* gc_u8, uint4* planes,
-                          void* workspace, size_t workspace_bytes, cudaStream_t stream, int gray) {
+struct PreBufs {
+  uint32_t* tile_hist;
+  uint32_t* rgb_hist;
+  uint8_t* clahe_lut;
+  uint8_t* wb_lut;
+};
+static PreBufs pre_carve(void* workspace, int n) {
+  PreBufs b;
+  uint8_t* ws = (uint8_t*)workspace;
+  b.tile_hist = (uint32_t*)ws;
+  ws += align_up((size_t)n * 64 * 256 * 4, 256);
+  b.rgb_hist = (uint32_t*)ws;
+  ws += align_up((size_t)n * 768 * 4, 256);
+  b.clahe_lut = ws;
+  ws += align_up((size_t)n * 64 * 256, 256);
+  b.wb_lut = ws;
+  return b;
+}
+
+static int preprocess_check(int n, int H, int W, size_t workspace_bytes) {
   if (workspace_bytes < preprocess_workspace_bytes(n, H, W)) {
     set_error("preprocess workspace too small: %zu < %zu", workspace_bytes,
               preprocess_workspace_bytes(n, H, W));
@@ -568,16 +603,14 @@ static int preprocess_run(wn_handle* h, const uint8_t* rgb, int n, int H, int W,
     set_error("image too large: n=%d h=%d w=%d", n, H, W);
     return WN_E_UNSUPPORTED;
   }
-  PreGeom g = geometry(H, W);
-  uint8_t* ws = (uint8_t*)workspace;
-  uint32_t* tile_hist = (uint32_t*)ws;
-  ws += align_up((size_t)n * 64 * 256 * 4, 256);
-  uint32_t* rgb_hist = (uint32_t*)ws;
-  ws += align_up((size_t)n * 768 * 4, 256);
-  uint8_t* clahe_lut = ws;
-  ws += align_up((size_t)n * 64 * 256, 256);
-  uint8_t* wb_lut = ws;
+  return WN_OK;
+}
 
+// passes 1 and 2: per-image histograms -> CLAHE and white-balance LUTs in the workspace
+static int preprocess_luts(wn_handle* h, const uint8_t* rgb, int n, int H, int W, const PreGeom& g, const PreBufs& b,
+                           cudaStream_t stream, int gray) {
+  uint32_t* tile_hist = b.tile_hist;
+  uint32_t* rgb_hist = b.rgb_hist;
   size_t hist_bytes = align_up((size_t)n * 64 * 256 * 4, 256) + (size_t)n * 768 * 4;
   WN_CUDA(cudaMemsetAsync(tile_hist, 0, hist_bytes, stream));
   // ~4K pixels per CTA keeps the grid well above two CTAs per SM even for one 1080p image
@@ -596,9 +629,24 @@ static int preprocess_run(wn_handle* h, const uint8_t* rgb, int n, int H, int W,
   {
   TimedScope ts(h, kSlotLuts, stream);
   luts_kernel<<<dim3(65, n), 256, 0, stream>>>(tile_hist, rgb_hist, H * W, g.clip, g.lut_scale,
-                                               clahe_lut, wb_lut, gray);
+                                               b.clahe_lut, b.wb_lut, gray);
   WN_LAUNCH_CHECK(h);
   }
+  return WN_OK;
+}
+
+static int preprocess_run(wn_handle* h, const uint8_t* rgb, int n, int H, int W, float* x, float* wb,
+                          float* he, float* gc, uint8_t* wb_u8, uint8_t* he_u8, uint8_t* gc_u8, uint4* planes,
+                          void* workspace, size_t workspace_bytes, cudaStream_t stream, int gray) {
+  int rc = preprocess_check(n, H, W, workspace_bytes);
+  if (rc) return rc;
+  PreGeom g = geometry(H, W);
+  const PreBufs b = pre_carve(workspace, n);
+  rc = preprocess_luts(h, rgb, n, H, W, g, b, stream, gray);
+  if (rc) return rc;
+  const uint8_t* clahe_lut = b.clahe_lut;
+  const uint8_t* wb_lut = b.wb_lut;
+  const TileGeom untiled = {};
   ApplyOut ao;
   ao.f32[0] = x; ao.f32[1] = wb; ao.f32[2] = he; ao.f32[3] = gc;
   ao.u8[0] = wb_u8; ao.u8[1] = he_u8; ao.u8[2] = gc_u8;
@@ -612,13 +660,39 @@ static int preprocess_run(wn_handle* h, const uint8_t* rgb, int n, int H, int W,
     const int iters = apply_iters((long long)n * H * W / 4, h->sm_count);
     const int per_cta = 256 * iters * 4;
     apply_kernel<true><<<dim3((H * W + per_cta - 1) / per_cta, n), 256, 0, stream>>>(rgb, H, W, g.th, g.tw, h->d_tables,
-                                                                                   clahe_lut, wb_lut, ao, iters);
+                                                                                   clahe_lut, wb_lut, ao, iters,
+                                                                                   untiled, 0);
   } else {
     const int iters = apply_iters((long long)n * H * W, h->sm_count);
     const int per_cta = 256 * iters;
     apply_kernel<false><<<dim3((H * W + per_cta - 1) / per_cta, n), 256, 0, stream>>>(rgb, H, W, g.th, g.tw, h->d_tables,
-                                                                                    clahe_lut, wb_lut, ao, iters);
+                                                                                    clahe_lut, wb_lut, ao, iters,
+                                                                                    untiled, 0);
   }
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+
+int preprocess_u8_luts(wn_handle* h, const uint8_t* rgb, int n, int H, int W, void* workspace, size_t workspace_bytes,
+                       cudaStream_t stream) {
+  const int rc = preprocess_check(n, H, W, workspace_bytes);
+  if (rc) return rc;
+  return preprocess_luts(h, rgb, n, H, W, geometry(H, W), pre_carve(workspace, n), stream, 0);
+}
+
+int preprocess_u8_window_planes(wn_handle* h, const uint8_t* rgb, int n, const TileGeom& tiles, long long win0,
+                                int count, uint4* planes, void* workspace, cudaStream_t stream) {
+  const PreGeom g = geometry(tiles.H, tiles.W);
+  const PreBufs b = pre_carve(workspace, n);
+  ApplyOut ao;
+  memset(&ao, 0, sizeof(ao));
+  ao.planes = planes;
+  TimedScope ts(h, kSlotApply, stream);
+  const int wplane = tiles.win_h * tiles.win_w;
+  const int iters = apply_iters((long long)count * wplane, h->sm_count);
+  const int per_cta = 256 * iters;
+  apply_kernel<false, true><<<dim3((wplane + per_cta - 1) / per_cta, count), 256, 0, stream>>>(
+      rgb, tiles.H, tiles.W, g.th, g.tw, h->d_tables, b.clahe_lut, b.wb_lut, ao, iters, tiles, win0);
   WN_LAUNCH_CHECK(h);
   return WN_OK;
 }

@@ -1,0 +1,71 @@
+// Window geometry of the tiled forward (wn_enhance_u8_tiled).  The apply kernel, the gate epilogue and the host
+// planner all call these functions: this is the only place that knows the rule.
+//
+// Every output pixel of WaterNet depends on the input within kTileHalo pixels (the eight cmg convolutions have
+// radii 3+2+1+0+3+2+1+1; the refiners need 6, the gate is per pixel).  An image is cut into balanced output tiles
+// of at most tile_h x tile_w; tile (i, j) keeps rows [i*th, min(H, (i+1)*th)) and is computed from a window of
+// win_h x win_w image pixels around it, clamped into the image.  All windows of a call have the same size, every
+// window edge inside the image is at least kTileHalo pixels from the kept rectangle, and a window edge on the
+// image border sees the same zero padding as the untiled forward: every kept pixel sees the operands it sees
+// untiled (DESIGN.md "Tiled enhance").
+#pragma once
+
+namespace wn {
+
+constexpr int kTileHalo = 13;
+
+struct TileGeom {
+  int H, W;          // image
+  int th, tw;        // kept tile (balanced: <= the requested tile)
+  int ny, nx;        // tiles per image column / row
+  int win_h, win_w;  // window
+};
+
+// tile_h, tile_w >= 1 and H, W >= 1 (checked by the callers)
+__host__ __device__ inline TileGeom tile_geom(int H, int W, int tile_h, int tile_w) {
+  TileGeom g;
+  g.H = H;
+  g.W = W;
+  g.ny = (H + tile_h - 1) / tile_h;
+  g.nx = (W + tile_w - 1) / tile_w;
+  g.th = (H + g.ny - 1) / g.ny;  // (ny - 1) * th < H: no tile is empty
+  g.tw = (W + g.nx - 1) / g.nx;
+  g.win_h = g.th + 2 * kTileHalo < H ? g.th + 2 * kTileHalo : H;
+  g.win_w = g.tw + 2 * kTileHalo < W ? g.tw + 2 * kTileHalo : W;
+  return g;
+}
+
+// window `win` of a call, numbered (image, tile row, tile column): its image, its origin and its kept rectangle
+// [ky0, ky1) x [kx0, kx1), all in image coordinates
+struct TileWindow {
+  int img, ys, xs, ky0, ky1, kx0, kx1;
+};
+
+__host__ __device__ inline int tile_clamp(int v, int lo, int hi) { return v < lo ? lo : v > hi ? hi : v; }
+
+__host__ __device__ inline TileWindow tile_window(const TileGeom& g, long long win) {
+  const long long per_image = (long long)g.ny * g.nx;
+  TileWindow t;
+  t.img = (int)(win / per_image);
+  const int r = (int)(win - t.img * per_image);
+  const int i = r / g.nx, j = r - i * g.nx;
+  t.ky0 = i * g.th;
+  t.kx0 = j * g.tw;
+  t.ky1 = t.ky0 + g.th < g.H ? t.ky0 + g.th : g.H;
+  t.kx1 = t.kx0 + g.tw < g.W ? t.kx0 + g.tw : g.W;
+  t.ys = tile_clamp(t.ky0 - kTileHalo, 0, g.H - g.win_h);
+  t.xs = tile_clamp(t.kx0 - kTileHalo, 0, g.W - g.win_w);
+  return t;
+}
+
+// windows per pass: as many as fit in max_pass_pixels (at least one, at most all of them and at most 65535, the
+// grid limit of the per-window apply kernel)
+__host__ __device__ inline long long tile_pass_windows(const TileGeom& g, int n, long long max_pass_pixels) {
+  const long long total = (long long)n * g.ny * g.nx;
+  long long p = max_pass_pixels / ((long long)g.win_h * g.win_w);
+  if (p > total) p = total;
+  if (p > 65535) p = 65535;
+  return p < 1 ? 1 : p;
+}
+
+}  // namespace wn

@@ -191,6 +191,11 @@ struct ConvArgs {
   // conditional launch: when non-null and *run_if == 0 the kernel returns at once (the bf16x3 re-run of a
   // batch is enqueued unconditionally behind the fp8-correction pass and only does work if the flag is up)
   const int* run_if;
+  // kEpiGate of the tiled forward (tiled != 0): image n of the launch is window win0 + n of `tiles`; only the
+  // pixels of its kept rectangle are stored, into out_f32 / out_u8 of the full images at image coordinates
+  int tiled;
+  long long win0;
+  TileGeom tiles;
 };
 
 __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b) {
@@ -302,12 +307,22 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
 #pragma unroll
         for (int c = 0; c < 3; c++)
           v[c] = __fadd_rn(__fadd_rn(__fmul_rn(r[c], c0), __fmul_rn(r[3 + c], c1)), __fmul_rn(r[6 + c], c2));
+        size_t oo = o, ohw = hw, o8 = ((size_t)n * hw + pix) * 3;
+        if (g.tiled) {  // window pixel -> image pixel; the halo around the kept rectangle is not stored
+          const TileWindow t = tile_window(g.tiles, g.win0 + n);
+          const int y = t.ys + gy, x = t.xs + gx;
+          if (y < t.ky0 || y >= t.ky1 || x < t.kx0 || x >= t.kx1) return;
+          ohw = (size_t)g.tiles.H * g.tiles.W;
+          const size_t ipix = (size_t)y * g.tiles.W + x;
+          oo = (size_t)t.img * 3 * ohw + ipix;
+          o8 = ((size_t)t.img * ohw + ipix) * 3;
+        }
         if (g.out_f32) {
 #pragma unroll
-          for (int c = 0; c < 3; c++) g.out_f32[o + c * hw] = v[c];
+          for (int c = 0; c < 3; c++) g.out_f32[oo + c * ohw] = v[c];
         }
         if (g.out_u8) {  // ten2arr (hubconf.py:24-34): clip to [0,1], *255, truncate; NHWC
-          uint8_t* q = g.out_u8 + ((size_t)n * hw + pix) * 3;
+          uint8_t* q = g.out_u8 + o8;
 #pragma unroll
           for (int c = 0; c < 3; c++) q[c] = (uint8_t)(int)__fmul_rn(fminf(fmaxf(v[c], 0.0f), 1.0f), 255.0f);
         }

@@ -53,6 +53,25 @@ def new_engine(device=None) -> "Engine":
     return Engine(_require_cuda(device))
 
 
+TILE_HALO = 13  # receptive-field radius of WaterNet (csrc/tiling.cuh kTileHalo)
+
+
+def tile_geometry(h: int, w: int, tile_h: int, tile_w: int) -> dict:
+    """The window rule of wn_enhance_u8_tiled (csrc/tiling.cuh) restated for callers that plan or check a tiled
+    call: balanced tile size and count per axis, window size, and each window's origin and kept rectangle."""
+    def axis(size, tile):
+        count = -(-size // tile)
+        t = -(-size // count)
+        win = min(size, t + 2 * TILE_HALO)
+        spans = [(i * t, min(size, (i + 1) * t)) for i in range(count)]
+        starts = [min(max(k0 - TILE_HALO, 0), size - win) for k0, _ in spans]
+        return t, count, win, spans, starts
+    th, ny, win_h, rows, ys = axis(h, tile_h)
+    tw, nx, win_w, cols, xs = axis(w, tile_w)
+    return {"th": th, "tw": tw, "ny": ny, "nx": nx, "win_h": win_h, "win_w": win_w,
+            "windows": [(ys[i], xs[j], rows[i], cols[j]) for i in range(ny) for j in range(nx)]}
+
+
 def _stream_ptr(device: torch.device) -> ctypes.c_void_p:
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -368,12 +387,7 @@ class Engine:
         _lib.check(rc, "wn_postprocess_u8")
         return res
 
-    def enhance(self, rgb_u8: torch.Tensor, mode: int = _lib.MODE_DEFAULT, out_u8: Optional[torch.Tensor] = None,
-                out_f32: Optional[torch.Tensor] = None, peer_out=()) -> torch.Tensor:
-        """preprocess -> forward -> postprocess on uint8 (N,H,W,3) CUDA input; returns uint8 NHWC.
-
-        ``peer_out``: device addresses (ints) inside other ranks' buffers (``dist.PeerGather.peer_addresses``) that
-        receive the same bytes as ``out_u8`` from the kernel that writes it (wn_enhance_u8_peers)."""
+    def _enhance_args(self, rgb_u8, out_u8, out_f32):
         if rgb_u8.dtype != torch.uint8 or rgb_u8.dim() != 4 or rgb_u8.shape[3] != 3:
             raise ValueError(f"expected uint8 (N,H,W,3), got {rgb_u8.dtype} {tuple(rgb_u8.shape)}")
         rgb_u8 = rgb_u8.to(self.device).contiguous()
@@ -387,6 +401,16 @@ class Engine:
         if out_f32 is not None and (out_f32.dtype != torch.float32 or tuple(out_f32.shape) != (n, 3, h, w)
                                     or not out_f32.is_contiguous() or out_f32.device != rgb_u8.device):
             raise ValueError(f"out_f32 must be a contiguous float32 {(n, 3, h, w)} tensor on {rgb_u8.device}")
+        return rgb_u8, out_u8
+
+    def enhance(self, rgb_u8: torch.Tensor, mode: int = _lib.MODE_DEFAULT, out_u8: Optional[torch.Tensor] = None,
+                out_f32: Optional[torch.Tensor] = None, peer_out=()) -> torch.Tensor:
+        """preprocess -> forward -> postprocess on uint8 (N,H,W,3) CUDA input; returns uint8 NHWC.
+
+        ``peer_out``: device addresses (ints) inside other ranks' buffers (``dist.PeerGather.peer_addresses``) that
+        receive the same bytes as ``out_u8`` from the kernel that writes it (wn_enhance_u8_peers)."""
+        rgb_u8, out_u8 = self._enhance_args(rgb_u8, out_u8, out_f32)
+        n, h, w, _ = rgb_u8.shape
         if out_u8.numel() == 0:
             return out_u8
         ws = self._workspace("enhance", self.lib.wn_enhance_workspace_bytes(n, h, w, mode))
@@ -396,4 +420,40 @@ class Engine:
                                               None if out_f32 is None else out_f32.data_ptr(), peers, len(peer_out),
                                               n, h, w, mode, ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
         _lib.check(rc, "wn_enhance_u8_peers")
+        return out_u8
+
+    DEFAULT_TILE = (998, 998)  # a window (tile + 13 pixels of context per side) of at most 1024 x 1024
+
+    @staticmethod
+    def _tile_hw(tile) -> Tuple[int, int]:
+        th, tw = (tile, tile) if isinstance(tile, (int, np.integer)) else tuple(tile)
+        if int(th) < 1 or int(tw) < 1:
+            raise ValueError(f"tile must be at least 1 x 1, got {tile!r}")
+        return int(th), int(tw)
+
+    def tiled_workspace_bytes(self, n: int, h: int, w: int, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
+                              max_pass_pixels: int = 0) -> int:
+        """Workspace of one ``enhance_tiled`` call (wn_enhance_tiled_workspace_bytes); 0 for rejected arguments."""
+        th, tw = self._tile_hw(tile)
+        return int(self.lib.wn_enhance_tiled_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels), mode))
+
+    def enhance_tiled(self, rgb_u8: torch.Tensor, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
+                      out_u8: Optional[torch.Tensor] = None, out_f32: Optional[torch.Tensor] = None,
+                      max_pass_pixels: int = 0) -> torch.Tensor:
+        """``enhance`` computed in overlapping windows (wn_enhance_u8_tiled): the same bits, with a workspace that
+        does not grow with the image size.  ``tile``: the largest output tile, an int or (h, w); ``max_pass_pixels``:
+        window pixels per pass (0 = 8 Mi).  Tensor-core modes only."""
+        th, tw = self._tile_hw(tile)
+        rgb_u8, out_u8 = self._enhance_args(rgb_u8, out_u8, out_f32)
+        n, h, w, _ = rgb_u8.shape
+        if out_u8.numel() == 0:
+            return out_u8
+        nbytes = self.lib.wn_enhance_tiled_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels), mode)
+        ws = self._workspace("enhance", nbytes)
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_enhance_u8_tiled(self.handle, rgb_u8.data_ptr(), out_u8.data_ptr(),
+                                              None if out_f32 is None else out_f32.data_ptr(), n, h, w, th, tw,
+                                              int(max_pass_pixels), mode, ws.data_ptr(), ws.numel(),
+                                              _stream_ptr(self.device))
+        _lib.check(rc, "wn_enhance_u8_tiled")
         return out_u8
