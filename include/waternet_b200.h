@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 4
+#define WN_ABI_VERSION 5
 
 #define WN_OK 0
 #define WN_E_INVALID (-1)   /* bad argument (NULL pointer, non-positive size, unknown mode) */
@@ -223,12 +223,6 @@ int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const 
                            const float* gc, const int64_t in_strides[4][4], int n, int height,
                            int width, int mode, int layer, float* dst, void* workspace,
                            size_t workspace_bytes, void* stream);
-
-/*
- * Debug switches of the tensor-core path.  No flag is defined at present: every value leaves the computation
- * unchanged (kept for ABI stability).
- */
-int wn_debug_set_flags(wn_handle* h, int flags);
 
 /* Number of kernels the library has launched on this handle since creation. */
 uint64_t wn_launch_count(const wn_handle* h);

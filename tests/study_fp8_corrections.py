@@ -21,7 +21,7 @@ import torch.nn.functional as F
 from oracle import forward as ofw
 from oracle import preprocess as opre
 
-# the layers the library runs with the fp8 correction pass (conv_umma.cu: has_f8_form)
+# the layers the library runs with the fp8 correction pass (conv_umma.cu: the f8 column of kSpecs)
 LIBRARY_F8_LAYERS = {"cmg.conv2", "cmg.conv3", "cmg.conv5", "cmg.conv6", "cmg.conv7",
                      "wb_refiner.conv2", "ce_refiner.conv2", "gc_refiner.conv2"}
 

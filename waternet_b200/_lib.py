@@ -19,7 +19,7 @@ MODE_BF16_FP8 = 2
 MODE_DEFAULT = -1
 NUM_PARAMS = 34
 NUM_TIMING_SLOTS = 23
-ABI_VERSION = 4
+ABI_VERSION = 5
 PEER_HANDLE_BYTES = 64  # WN_PEER_HANDLE_BYTES
 MAX_PEERS = 15          # WN_MAX_PEERS
 
@@ -67,7 +67,6 @@ _SIGNATURES = {
     "wn_memcpy_async": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
     "wn_stream_write_value32": (c_int, [c_void_p, c_void_p, ctypes.c_uint32]),
     "wn_stream_wait_value32": (c_int, [c_void_p, c_void_p, ctypes.c_uint32]),
-    "wn_debug_set_flags": (c_int, [c_void_p, c_int]),
     "wn_train_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "wn_forward_train": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p,
                                  c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),

@@ -465,15 +465,6 @@ int wn_f8_overflowed(const wn_handle* h) { return h ? umma_f8_overflowed(h) : 0;
 
 uint64_t wn_launch_count(const wn_handle* h) { return h ? h->launches : 0; }
 
-int wn_debug_set_flags(wn_handle* h, int flags) {
-  if (!h) {
-    set_error("wn_debug_set_flags: null handle");
-    return WN_E_INVALID;
-  }
-  h->dbg_flags = flags;
-  return WN_OK;
-}
-
 size_t wn_train_workspace_bytes(int n, int h, int w) {
   if (n <= 0 || h <= 0 || w <= 0) return 0;
   return train_workspace_bytes_padded(n, h, w);

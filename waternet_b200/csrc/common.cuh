@@ -91,7 +91,6 @@ struct wn_handle {
   int sm_count;
   wn::Timing* timing;
   wn::UmmaBwd* bwd;
-  int dbg_flags;  // wn_debug_set_flags (no switch is defined at present); 0 in normal use
   long long chunk_pixels;  // cap on pixels per pass of the tensor-core forward (0 = default, wn_set_chunk_pixels)
 };
 

@@ -334,24 +334,29 @@ input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, I
 // ------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------
+// The backward of each forward convolution (the refiners' side by side).
 enum DgradLayer { kD8 = 0, kD7, kD6, kD5, kD4, kD3, kD2, kDR3, kDR2, kD1, kDR1, kNumDgrad };
+// Data gradient (UmmaCfg): ks, kpad = K = forward Cout (padded), npad = N per block = forward Cin, nblk, concat, tps.
+// Weight gradient (WgradCfg): nci = forward input channels (padded), tpg = taps per CTA group.  conv = the cmg
+// convolution (-1: refiner conv2 / conv3, -2: refiner conv1).
 struct DgradSpec {
-  int ks, kpad, npad, nblk, concat, conv;  // K = forward Cout (padded), N per block = forward Cin
+  int ks, kpad, npad, nblk, concat, tps, nci, tpg, conv;
 };
-static const DgradSpec kDSpecs[kNumDgrad] = {
-    {3, 16, 64, 1, 1, 7},
-    {3, 64, 64, 1, 1, 6},
-    {5, 64, 64, 1, 1, 5},
-    {7, 64, 64, 1, 1, 4},
-    {1, 64, 128, 1, 0, 3},
-    {3, 128, 128, 1, 0, 2},
-    {5, 128, 128, 1, 0, 1},
-    {3, 16, 96, 1, 0, -1},
-    {5, 96, 32, 3, 1, -1},
-    // gradients with respect to the packed 16-channel input (only when an input image requires grad):
+static constexpr DgradSpec kDSpecs[kNumDgrad] = {
+    // ks kpad npad nblk concat tps nci tpg conv
+    {3, 16, 64, 1, 1, 9, 64, 4, 7},       // kD8
+    {3, 64, 64, 1, 1, 9, 64, 4, 6},       // kD7
+    {5, 64, 64, 1, 1, 5, 64, 4, 5},       // kD6
+    {7, 64, 64, 1, 1, 7, 64, 4, 4},       // kD5
+    {1, 64, 128, 1, 0, 1, 128, 1, 3},     // kD4
+    {3, 128, 128, 1, 0, 3, 128, 2, 2},    // kD3
+    {5, 128, 128, 1, 0, 5, 128, 2, 1},    // kD2
+    {3, 16, 96, 1, 0, 9, 96, 2, -1},      // kDR3
+    {5, 96, 32, 3, 1, 5, 96, 2, -1},      // kDR2
+    // data gradients with respect to the packed 16-channel input (only when an input image requires grad):
     // from cmg.conv1 (K = 128) and from the three refiner conv1 (K = 96); 32 rows, 12 real
-    {7, 128, 32, 1, 1, 0},
-    {7, 96, 32, 1, 1, -2}};
+    {7, 128, 32, 1, 1, 7, 16, 16, 0},     // kD1
+    {7, 96, 32, 1, 1, 7, 16, 16, -2}};    // kDR1
 
 struct UmmaBwd {
   uint8_t* stages[kNumDgrad];
@@ -504,11 +509,12 @@ static int make_plane_tmap(CUtensorMap* tm, void* base, int planes_total, int N,
   return WN_OK;
 }
 
-// dense[tap][128][NCI] += sum_px g[px][co] * a[px + tap][ci]
-template <int KS, int NCI, int TPG>
+// dense[tap][128][nci] += sum_px g[px][co] * a[px + tap][ci]
+template <int LI>
 static int launch_wgrad(wn_handle* h, uint4* gplanes, int co_valid, uint4* aplanes, float* dense, float* partial, int n,
                         int H, int W, cudaStream_t stream) {
-  using C = WgradCfg<KS, NCI, TPG>;
+  constexpr DgradSpec s = kDSpecs[LI];
+  using C = WgradCfg<s.ks, s.nci, s.tpg>;
   const int co_planes = (co_valid + 7) / 8;
   const int planes_half = (co_valid + 15) / 16 * 2;  // gradient buffers hold a multiple of 16 channels
   CUtensorMap tg, ta;
@@ -529,12 +535,13 @@ static int launch_wgrad(wn_handle* h, uint4* gplanes, int co_valid, uint4* aplan
   if (splits > tiles) splits = tiles;
   if (splits < 1) splits = 1;
   if (splits * C::NGROUPS > kPartialSlots) splits = kPartialSlots / C::NGROUPS;
-  static_assert((size_t)TPG * 128 * NCI * sizeof(float) <= kPartialSlotBytes, "partial-sum slot");
-  auto kern = wgrad_umma_kernel<KS, NCI, TPG>;
+  static_assert((size_t)s.tpg * 128 * s.nci * sizeof(float) <= kPartialSlotBytes, "partial-sum slot");
+  auto kern = wgrad_umma_kernel<s.ks, s.nci, s.tpg>;
   WN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
   kern<<<dim3(C::NGROUPS, (unsigned)splits), kWgradThreads, C::SMEM_BYTES, stream>>>(tg, ta, a);
   WN_LAUNCH_CHECK(h);
-  reduce_wgrad_kernel<<<256, 256, 0, stream>>>(partial, dense, KS * KS, TPG, C::NGROUPS, (int)splits, NCI, co_valid);
+  reduce_wgrad_kernel<<<256, 256, 0, stream>>>(partial, dense, s.ks * s.ks, s.tpg, C::NGROUPS, (int)splits, s.nci,
+                                               co_valid);
   WN_LAUNCH_CHECK(h);
   return WN_OK;
 }
@@ -556,14 +563,11 @@ static int bias_grad(wn_handle* h, const uint4* gplanes, int planes_half, int co
   return WN_OK;
 }
 
-template <int KS, int KPAD, int NPAD, int CONCAT = 0, int NBLK = 1, int TPS = 1>
-static int launch_dgrad(wn_handle* h, int li, uint4* g_in, uint4* g_out, int out_channels, const uint4* saved,
-                        int n, int H, int W, cudaStream_t stream) {
-  const DgradSpec& s = kDSpecs[li];
-  if (s.ks != KS || s.kpad != KPAD || s.npad != NPAD || s.concat != CONCAT || s.nblk != NBLK) {
-    set_error("internal: dgrad launch %d does not match its packed weights", li);
-    return WN_E_STATE;
-  }
+template <int LI>
+static int launch_dgrad(wn_handle* h, uint4* g_in, uint4* g_out, const uint4* saved, int n, int H, int W,
+                        cudaStream_t stream) {
+  constexpr DgradSpec s = kDSpecs[LI];
+  constexpr int out_channels = s.npad * s.nblk;
   ConvArgs a;
   memset(&a, 0, sizeof(a));
   a.N = n; a.H = H; a.W = W;
@@ -573,8 +577,28 @@ static int launch_dgrad(wn_handle* h, int li, uint4* g_in, uint4* g_out, int out
   a.cout = out_channels;
   a.mask_base = saved;  // nullptr: no ReLU in front (network input)
   a.mask_planes_half = out_channels / 8;
-  return launch_conv<KS, KPAD, NPAD, kEpiDgrad, CONCAT, NBLK, TPS>(h, kSlotGate, h->bwd->stages[li],
-                                                                         h->bwd->zero_bias, g_in, a, stream);
+  return launch_conv<s.ks, s.kpad, s.npad, kEpiDgrad, s.concat, s.nblk, s.tps>(h, kSlotGate, h->bwd->stages[LI],
+                                                                              h->bwd->zero_bias, g_in, a, stream);
+}
+
+// Backward of one cmg convolution from g, the gradient with respect to its output: its weight and bias gradients,
+// then, when g_dst is given, the gradient with respect to its input into g_dst.  Its input is the saved activation
+// a[conv], whose zeros gate that gradient (ReLU'); conv 0 reads act0 instead, the images * 255 with no ReLU.
+template <int LI>
+static int cmg_conv_backward(wn_handle* h, const TrainBuffers& t, float* const* grads, uint4* g, uint4* g_dst, int n,
+                             int H, int W, cudaStream_t stream) {
+  constexpr DgradSpec s = kDSpecs[LI];
+  static_assert(s.conv >= 0, "not a cmg convolution");
+  const LayerDesc& d = kCmg[s.conv];
+  uint4* act = s.conv ? t.f.a[s.conv] : t.f.act0;
+  int rc;
+  if ((rc = launch_wgrad<LI>(h, g, d.cout, act, t.dense, t.partial, n, H, W, stream))) return rc;
+  if ((rc = extract(h, t.dense, grads[2 * s.conv], d.cout, d.cin, s.ks, s.nci, 0, d.cin, 0, 0,
+                    s.conv ? 1.f : 1.f / 255.f, stream)))
+    return rc;
+  if ((rc = bias_grad(h, g, (d.cout + 15) / 16 * 2, d.cout, grads[2 * s.conv + 1], t.partial, n, H * W, stream)))
+    return rc;
+  return g_dst ? launch_dgrad<LI>(h, g, g_dst, s.conv ? act : nullptr, n, H, W, stream) : WN_OK;
 }
 
 int backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n, int H,
@@ -595,52 +619,19 @@ int backward(wn_handle* h, const float* grad_out, float* const* grads, float* co
   gate_bwd_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(grad_out, t.f.cm, t.f.refined, t.g8, t.gr3, hw);
   WN_LAUNCH_CHECK(h);
 
-  // ---- confidence-map stack: conv8 ... conv1 ---------------------------------------------
-  // conv8 (64 -> 3, 3x3): g = g8 (16-channel planes, 3 valid), a = a7
-  if ((rc = launch_wgrad<3, 64, 4>(h, t.g8, 3, t.f.a[7], t.dense, t.partial, n, H, W, stream))) return rc;
-  if ((rc = extract(h, t.dense, gw(7), 3, 64, 3, 64, 0, 64, 0, 0, 1.f, stream))) return rc;
-  if ((rc = bias_grad(h, t.g8, 2, 3, gb(7), t.partial, n, hw, stream))) return rc;
-  if ((rc = launch_dgrad<3, 16, 64, 1, 1, 9>(h, kD8, t.g8, t.ga, 64, t.f.a[7], n, H, W, stream))) return rc;
-  // conv7 (64 -> 64, 3x3): g = ga
-  if ((rc = launch_wgrad<3, 64, 4>(h, t.ga, 64, t.f.a[6], t.dense, t.partial, n, H, W, stream))) return rc;
-  if ((rc = extract(h, t.dense, gw(6), 64, 64, 3, 64, 0, 64, 0, 0, 1.f, stream))) return rc;
-  if ((rc = bias_grad(h, t.ga, 8, 64, gb(6), t.partial, n, hw, stream))) return rc;
-  if ((rc = launch_dgrad<3, 64, 64, 1, 1, 9>(h, kD7, t.ga, t.gb, 64, t.f.a[6], n, H, W, stream))) return rc;
-  // conv6 (5x5): g = gb
-  if ((rc = launch_wgrad<5, 64, 4>(h, t.gb, 64, t.f.a[5], t.dense, t.partial, n, H, W, stream))) return rc;
-  if ((rc = extract(h, t.dense, gw(5), 64, 64, 5, 64, 0, 64, 0, 0, 1.f, stream))) return rc;
-  if ((rc = bias_grad(h, t.gb, 8, 64, gb(5), t.partial, n, hw, stream))) return rc;
-  if ((rc = launch_dgrad<5, 64, 64, 1, 1, 5>(h, kD6, t.gb, t.ga, 64, t.f.a[5], n, H, W, stream))) return rc;
-  // conv5 (7x7): g = ga
-  if ((rc = launch_wgrad<7, 64, 4>(h, t.ga, 64, t.f.a[4], t.dense, t.partial, n, H, W, stream))) return rc;
-  if ((rc = extract(h, t.dense, gw(4), 64, 64, 7, 64, 0, 64, 0, 0, 1.f, stream))) return rc;
-  if ((rc = bias_grad(h, t.ga, 8, 64, gb(4), t.partial, n, hw, stream))) return rc;
-  if ((rc = launch_dgrad<7, 64, 64, 1, 1, 7>(h, kD5, t.ga, t.gb, 64, t.f.a[4], n, H, W, stream))) return rc;
-  // conv4 (128 -> 64, 1x1): g = gb (64), a = a3 (128)
-  if ((rc = launch_wgrad<1, 128, 1>(h, t.gb, 64, t.f.a[3], t.dense, t.partial, n, H, W, stream))) return rc;
-  if ((rc = extract(h, t.dense, gw(3), 64, 128, 1, 128, 0, 128, 0, 0, 1.f, stream))) return rc;
-  if ((rc = bias_grad(h, t.gb, 8, 64, gb(3), t.partial, n, hw, stream))) return rc;
-  if ((rc = launch_dgrad<1, 64, 128, 0, 1, 1>(h, kD4, t.gb, t.ga, 128, t.f.a[3], n, H, W, stream))) return rc;
-  // conv3 (128 -> 128, 3x3): g = ga
-  if ((rc = launch_wgrad<3, 128, 2>(h, t.ga, 128, t.f.a[2], t.dense, t.partial, n, H, W, stream))) return rc;
-  if ((rc = extract(h, t.dense, gw(2), 128, 128, 3, 128, 0, 128, 0, 0, 1.f, stream))) return rc;
-  if ((rc = bias_grad(h, t.ga, 16, 128, gb(2), t.partial, n, hw, stream))) return rc;
-  if ((rc = launch_dgrad<3, 128, 128, 0, 1, 3>(h, kD3, t.ga, t.gb, 128, t.f.a[2], n, H, W, stream))) return rc;
-  // conv2 (5x5): g = gb
-  if ((rc = launch_wgrad<5, 128, 2>(h, t.gb, 128, t.f.a[1], t.dense, t.partial, n, H, W, stream))) return rc;
-  if ((rc = extract(h, t.dense, gw(1), 128, 128, 5, 128, 0, 128, 0, 0, 1.f, stream))) return rc;
-  if ((rc = bias_grad(h, t.gb, 16, 128, gb(1), t.partial, n, hw, stream))) return rc;
-  if ((rc = launch_dgrad<5, 128, 128, 0, 1, 5>(h, kD2, t.gb, t.ga, 128, t.f.a[1], n, H, W, stream))) return rc;
-  // conv1 (12 -> 128, 7x7): g = ga, a = act0 (holds v*255 -> scale the gradient back)
-  if ((rc = launch_wgrad<7, 16, 16>(h, t.ga, 128, t.f.act0, t.dense, t.partial, n, H, W, stream))) return rc;
-  if ((rc = extract(h, t.dense, gw(0), 128, 12, 7, 16, 0, 12, 0, 0, 1.f / 255.f, stream))) return rc;
-  if ((rc = bias_grad(h, t.ga, 16, 128, gb(0), t.partial, n, hw, stream))) return rc;
-  if (input_grads) {  // d/d(packed input) from cmg.conv1: ga (128) -> g8 region reused as a 32-channel buffer
-    if ((rc = launch_dgrad<7, 128, 32, 1, 1, 7>(h, kD1, t.ga, t.gin_a, 32, nullptr, n, H, W, stream))) return rc;
-  }
+  // ---- confidence-map stack: conv8 ... conv1, the gradient ping-ponging between ga and gb ----------
+  // conv8's output gradient g8 has 16-channel planes, 3 valid; conv1's input gradient only when asked for
+  if ((rc = cmg_conv_backward<kD8>(h, t, grads, t.g8, t.ga, n, H, W, stream))) return rc;
+  if ((rc = cmg_conv_backward<kD7>(h, t, grads, t.ga, t.gb, n, H, W, stream))) return rc;
+  if ((rc = cmg_conv_backward<kD6>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
+  if ((rc = cmg_conv_backward<kD5>(h, t, grads, t.ga, t.gb, n, H, W, stream))) return rc;
+  if ((rc = cmg_conv_backward<kD4>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
+  if ((rc = cmg_conv_backward<kD3>(h, t, grads, t.ga, t.gb, n, H, W, stream))) return rc;
+  if ((rc = cmg_conv_backward<kD2>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
+  if ((rc = cmg_conv_backward<kD1>(h, t, grads, t.ga, input_grads ? t.gin_a : nullptr, n, H, W, stream))) return rc;
 
   // ---- refiners: conv3, conv2, conv1 (three side by side) ---------------------------------
-  if ((rc = launch_wgrad<3, 96, 2>(h, t.gr3, 9, t.f.r[2], t.dense, t.partial, n, H, W, stream))) return rc;
+  if ((rc = launch_wgrad<kDR3>(h, t.gr3, 9, t.f.r[2], t.dense, t.partial, n, H, W, stream))) return rc;
   for (int r = 0; r < 3; r++) {
     if ((rc = extract(h, t.dense, gw(8 + 3 * r + 2), 3, 32, 3, 96, 3 * r, 32, 32 * r, 0, 1.f, stream))) return rc;
   }
@@ -651,8 +642,8 @@ int backward(wn_handle* h, const float* grad_out, float* const* grads, float* co
     for (int r = 0; r < 3; r++)
       WN_CUDA(cudaMemcpyAsync(gb(8 + 3 * r + 2), tmp + 3 * r, 3 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   }
-  if ((rc = launch_dgrad<3, 16, 96, 0, 1, 9>(h, kDR3, t.gr3, t.gra, 96, t.f.r[2], n, H, W, stream))) return rc;
-  if ((rc = launch_wgrad<5, 96, 2>(h, t.gra, 96, t.f.r[1], t.dense, t.partial, n, H, W, stream))) return rc;
+  if ((rc = launch_dgrad<kDR3>(h, t.gr3, t.gra, t.f.r[2], n, H, W, stream))) return rc;
+  if ((rc = launch_wgrad<kDR2>(h, t.gra, 96, t.f.r[1], t.dense, t.partial, n, H, W, stream))) return rc;
   {
     float* tmp = t.dense + (size_t)25 * 128 * 96;
     if ((rc = bias_grad(h, t.gra, 12, 96, tmp, t.partial, n, hw, stream))) return rc;
@@ -661,8 +652,8 @@ int backward(wn_handle* h, const float* grad_out, float* const* grads, float* co
       WN_CUDA(cudaMemcpyAsync(gb(8 + 3 * r + 1), tmp + 32 * r, 32 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
     }
   }
-  if ((rc = launch_dgrad<5, 96, 32, 1, 3, 5>(h, kDR2, t.gra, t.grb, 96, t.f.r[1], n, H, W, stream))) return rc;
-  if ((rc = launch_wgrad<7, 16, 16>(h, t.grb, 96, t.f.act0, t.dense, t.partial, n, H, W, stream))) return rc;
+  if ((rc = launch_dgrad<kDR2>(h, t.gra, t.grb, t.f.r[1], n, H, W, stream))) return rc;
+  if ((rc = launch_wgrad<kDR1>(h, t.grb, 96, t.f.act0, t.dense, t.partial, n, H, W, stream))) return rc;
   {
     float* tmp = t.dense + (size_t)49 * 128 * 16;
     if ((rc = bias_grad(h, t.grb, 12, 96, tmp, t.partial, n, hw, stream))) return rc;
@@ -673,7 +664,7 @@ int backward(wn_handle* h, const float* grad_out, float* const* grads, float* co
     }
   }
   if (input_grads) {
-    if ((rc = launch_dgrad<7, 96, 32, 1, 1, 7>(h, kDR1, t.grb, t.gin_b, 32, nullptr, n, H, W, stream))) return rc;
+    if ((rc = launch_dgrad<kDR1>(h, t.grb, t.gin_b, nullptr, n, H, W, stream))) return rc;
     InputGrads ig;
     for (int i = 0; i < 4; i++) ig.p[i] = input_grads[i];
     input_grads_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(t.gin_a, t.gin_b, ig, hw);

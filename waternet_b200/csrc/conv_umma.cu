@@ -81,23 +81,31 @@ enum UmmaLayer {
   kR3,        // three refiner conv3 as block-diagonal 96 -> 9 (pad 16), ReLU, gated sum
   kNumUmmaLayers
 };
+// Everything a layer's launches and packed weights depend on (UmmaCfg in umma_conv.cuh).  npad = output columns
+// per diagonal block; concat = CONCAT of the bf16x3 form, set where the a_hi x [w_hi | w_lo] product fits one wgmma
+// (N = 2 * NPAD <= 256); slot = timing slot, the state-dict index of the layer's (first) convolution; f8 = the layer
+// has an fp8-correction form (UmmaCfg FMT bit 0, the tensor-bound layers), which uses CONCAT 0.
 struct UmmaLayerSpec {
-  int ks, cinpad, npad, cout, slot, concat, nblk;  // npad = output columns per diagonal block
+  int ks, cinpad, npad, epi, concat, nblk, tps, slot;
+  bool f8;
 };
-// CONCAT where the a_hi x [w_hi | w_lo] product fits one wgmma (N = 2 * NPAD <= 256)
-static const UmmaLayerSpec kSpecs[kNumUmmaLayers] = {
-    {7, 16, 224, 224, 0, 0, 1},
-    {5, 128, 128, 128, 1, 0, 1},
-    {3, 128, 128, 128, 2, 0, 1},
-    {1, 128, 64, 64, 3, 1, 1},
-    {7, 64, 64, 64, 4, 1, 1},
-    {5, 64, 64, 64, 5, 1, 1},
-    {3, 64, 64, 64, 6, 1, 1},
-    {3, 64, 16, 3, 7, 1, 1},
-    {5, 96, 32, 96, 9, 1, 3},
-    {3, 96, 16, 9, 10, 1, 1}};
+static constexpr UmmaLayerSpec kSpecs[kNumUmmaLayers] = {
+    // ks cinpad npad epi       concat nblk tps slot f8
+    {7, 16, 224, kEpiAct, 0, 1, 1, 0, false},     // kL1
+    {5, 128, 128, kEpiAct, 0, 1, 5, 1, true},     // kC2
+    {3, 128, 128, kEpiAct, 0, 1, 3, 2, true},     // kC3
+    {1, 128, 64, kEpiAct, 1, 1, 1, 3, false},     // kC4
+    {7, 64, 64, kEpiAct, 1, 1, 7, 4, true},       // kC5
+    {5, 64, 64, kEpiAct, 1, 1, 5, 5, true},       // kC6
+    {3, 64, 64, kEpiAct, 1, 1, 9, 6, true},       // kC7
+    {3, 64, 16, kEpiSigmoid, 1, 1, 9, 7, false},  // kC8
+    {5, 96, 32, kEpiAct, 1, 3, 5, 9, true},       // kR2
+    {3, 96, 16, kEpiGate, 1, 1, 9, 10, false}};   // kR3
 
-static int spec_slot(int li) { return kSpecs[li].slot; }
+// In the fp8-correction scheme a layer writes the hi + fp8-planes format (FMT bit 1) when its consumers read it with
+// their fp8 form.  L1 feeds C2 and R2; every other layer feeds the next one, except the last layer of each stack.
+static_assert(kSpecs[kC2].f8 == kSpecs[kR2].f8, "L1 writes one format for both of its consumers");
+static constexpr bool writes_f8(int li) { return li != kC8 && li != kR3 && kSpecs[li + 1].f8; }
 
 // out -> every peer address (the uint8 output of the last launch, the range guard's re-run -- then conditional on
 // *run_if like every launch of that chain)
@@ -122,10 +130,8 @@ int mirror_u8(wn_handle* h, const uint8_t* src, const PeerOut& peers, size_t byt
   return WN_OK;
 }
 
-// layers that have an fp8-correction form (UmmaCfg FMT bit 0): the tensor-bound layers
-static bool has_f8_form(int li) { return li == kC2 || li == kC3 || li == kC5 || li == kC6 || li == kC7 || li == kR2; }
 struct UmmaWeights {
-  uint8_t* stages8[kNumUmmaLayers];  // fp8-correction weight images (has_f8_form layers)
+  uint8_t* stages8[kNumUmmaLayers];  // fp8-correction weight images (layers with an fp8 form)
   float* scale8[kNumUmmaLayers];     // {ws, 2^-9 / ws, max|w|, -}
   int* overflow_dev;                 // sticky: an activation left the e4m3 range in the fp8-correction mode
   int* overflow_host;                // pinned mirror, refreshed at the end of every forward of that mode
@@ -142,7 +148,7 @@ int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t str
   for (int i = 0; i < kNumUmmaLayers; i++) {  // (re)allocate whatever an earlier, failed call left unallocated
     if (!h->umma->stages[i]) WN_CUDA(cudaMalloc(&h->umma->stages[i], stage_bytes_total(kSpecs[i])));
     if (!h->umma->bias[i]) WN_CUDA(cudaMalloc(&h->umma->bias[i], kSpecs[i].npad * kSpecs[i].nblk * sizeof(float)));
-    if (has_f8_form(i)) {
+    if (kSpecs[i].f8) {
       if (!h->umma->stages8[i]) WN_CUDA(cudaMalloc(&h->umma->stages8[i], stage_bytes_total(kSpecs[i])));
       if (!h->umma->scale8[i]) WN_CUDA(cudaMalloc(&h->umma->scale8[i], 4 * sizeof(float)));
     }
@@ -188,7 +194,7 @@ int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t str
     pack_stages_kernel<<<256, 256, 0, stream>>>(u->dense, (__nv_bfloat16*)u->stages[li], s.npad, s.cinpad, kk,
                                                 s.concat, s.nblk);
     WN_LAUNCH_CHECK(h);
-    if (has_f8_form(li)) {
+    if (s.f8) {
       WN_CUDA(cudaMemsetAsync(u->scale8[li], 0, 4 * sizeof(float), stream));
       f8_absmax_kernel<<<64, 256, 0, stream>>>(u->dense, (size_t)rows * s.cinpad * kk, u->scale8[li]);
       WN_LAUNCH_CHECK(h);
@@ -239,25 +245,21 @@ size_t umma_forward_workspace_bytes(int n, int h, int w) {
   return nb * h * w * kUmmaBytesPerPixel + nb * h * 64 + 4096;
 }
 
-template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0>
-static int launch_umma(wn_handle* h, int li, void* in_base, ConvArgs a, cudaStream_t stream) {
-  const UmmaLayerSpec& spec = kSpecs[li];
-  if constexpr ((FMT & kFmtOut8) != 0) a.f8_overflow = h->umma->overflow_dev;
-  if constexpr ((FMT & kFmtIn8) != 0) {  // fp8-correction form: its own weight images, [hi | fp8] layout
-    if (spec.ks != KS || spec.cinpad != CIN_PAD || spec.npad != NPAD || spec.nblk != NBLK || !has_f8_form(li)) {
-      set_error("internal: fp8 launch configuration of layer %d does not match its packed weights", li);
-      return WN_E_STATE;
-    }
-    a.f8_scale = h->umma->scale8[li] + 1;
-    return launch_conv<KS, CIN_PAD, NPAD, EPI, 0, NBLK, TPS, FMT>(h, spec.slot, h->umma->stages8[li], h->umma->bias[li],
-                                                                  in_base, a, stream);
+// Launch layer LI in the fp8-correction scheme (f8) or in bf16x3.  A layer's fp8 form reads its own weight images,
+// in the [hi | fp8] layout.
+template <int LI>
+static int launch_layer(wn_handle* h, bool f8, void* in_base, ConvArgs a, cudaStream_t stream) {
+  constexpr UmmaLayerSpec s = kSpecs[LI];
+  const UmmaWeights* u = h->umma;
+  if (f8) {
+    constexpr int FMT = (s.f8 ? kFmtIn8 : 0) | (writes_f8(LI) ? kFmtOut8 : 0);
+    if constexpr ((FMT & kFmtOut8) != 0) a.f8_overflow = u->overflow_dev;
+    if constexpr (s.f8) a.f8_scale = u->scale8[LI] + 1;
+    return launch_conv<s.ks, s.cinpad, s.npad, s.epi, (s.f8 ? 0 : s.concat), s.nblk, s.tps, FMT>(
+        h, s.slot, s.f8 ? u->stages8[LI] : u->stages[LI], u->bias[LI], in_base, a, stream);
   }
-  if (spec.ks != KS || spec.cinpad != CIN_PAD || spec.npad != NPAD || spec.concat != CONCAT || spec.nblk != NBLK) {
-    set_error("internal: launch configuration of layer %d does not match its packed weights", li);
-    return WN_E_STATE;
-  }
-  return launch_conv<KS, CIN_PAD, NPAD, EPI, CONCAT, NBLK, TPS, FMT>(h, spec.slot, h->umma->stages[li], h->umma->bias[li],
-                                                                     in_base, a, stream);
+  return launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps>(h, s.slot, u->stages[LI], u->bias[LI],
+                                                                             in_base, a, stream);
 }
 
 // bf16 hi/lo planes -> fp32 NCHW (test aid)
@@ -314,10 +316,18 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   a.N = n; a.H = H; a.W = W;
   a.run_if = o.run_if;
   int rc;
-  auto dump = [&](int layer, const uint4* buf, int channels, int f8 = 0) -> bool {
-    if (dbg_layer != layer) return false;
-    decode_planes_kernel<<<dim3((H * W + 255) / 256, channels / 8, n), 256, 0, stream>>>(buf, dbg_dst, channels / 8,
-                                                                                     H * W, f8);
+  // fp8-correction scheme (inference): the tensor-bound layers replace the two bf16 correction passes by one
+  // fp8 MMA (UmmaCfg FMT); a layer whose consumer is such a layer writes the hi + fp8-planes format
+  const bool f8 = o.scheme == 1;
+  // after layer li's launch: decode its output (a.dst0) when it is the one wn_debug_forward_layer asks for.  That
+  // call numbers an output by its convolution in state-dict order, the layer's timing slot; L1's second output
+  // (a.dst1) is the refiners' conv1, number 8.
+  auto dump = [&](int li) -> bool {
+    const bool second = li == kL1 && dbg_layer == 8;
+    if (dbg_layer != kSpecs[li].slot && !second) return false;
+    const ActDst& d = second ? a.dst1 : a.dst0;
+    decode_planes_kernel<<<dim3((H * W + 255) / 256, d.planes_half, n), 256, 0, stream>>>(d.base, dbg_dst, d.planes_half,
+                                                                                      H * W, f8 && writes_f8(li));
     h->launches++;
     return true;
   };
@@ -340,63 +350,45 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
     }
   };
   const bool want_cmg = o.stack != kStackRefiners, want_ref = o.stack != kStackCmg;
-  // fp8-correction scheme (inference): the tensor-bound layers replace the two bf16 correction passes by one
-  // fp8 MMA (UmmaCfg FMT); a layer whose consumer is such a layer writes the hi + fp8-planes format
-  const bool f8 = o.scheme == 1;
-  constexpr int IN8 = kFmtIn8, OUT8 = kFmtOut8;
   // L1: 16 -> 128 (cmg) + 96 (refiners)
   act(b.a[1], 128, b.r[1], 96);
   a.skip_lo = b.exact_flag;
   a.a_hi_only = o.hi_only ? 1 : 0;
-  rc = f8 ? launch_umma<7, 16, 224, kEpiAct, 0, 1, 1, OUT8>(h, kL1, b.act0, a, stream)
-          : launch_umma<7, 16, 224, kEpiAct, 0, 1, 1>(h, kL1, b.act0, a, stream);
-  if (rc) return rc;
+  if ((rc = launch_layer<kL1>(h, f8, b.act0, a, stream))) return rc;
   a.skip_lo = nullptr;
   a.a_hi_only = 0;
-  if (dump(0, b.a[1], 128, f8) || dump(8, b.r[1], 96, f8)) return WN_OK;
+  if (dump(kL1)) return WN_OK;
   if (want_cmg) {
     act(b.a[2], 128, nullptr, 0);
-    rc = f8 ? launch_umma<5, 128, 128, kEpiAct, 0, 1, 5, IN8 | OUT8>(h, kC2, b.a[1], a, stream)
-            : launch_umma<5, 128, 128, kEpiAct, 0, 1, 5>(h, kC2, b.a[1], a, stream);
-    if (rc) return rc;
-    if (dump(1, b.a[2], 128, f8)) return WN_OK;
+    if ((rc = launch_layer<kC2>(h, f8, b.a[1], a, stream))) return rc;
+    if (dump(kC2)) return WN_OK;
     act(b.a[3], 128, nullptr, 0);
-    rc = f8 ? launch_umma<3, 128, 128, kEpiAct, 0, 1, 3, IN8>(h, kC3, b.a[2], a, stream)
-            : launch_umma<3, 128, 128, kEpiAct, 0, 1, 3>(h, kC3, b.a[2], a, stream);
-    if (rc) return rc;
-    if (dump(2, b.a[3], 128)) return WN_OK;
+    if ((rc = launch_layer<kC3>(h, f8, b.a[2], a, stream))) return rc;
+    if (dump(kC3)) return WN_OK;
     act(b.a[4], 64, nullptr, 0);
-    rc = f8 ? launch_umma<1, 128, 64, kEpiAct, 1, 1, 1, OUT8>(h, kC4, b.a[3], a, stream)
-            : launch_umma<1, 128, 64, kEpiAct, 1, 1, 1>(h, kC4, b.a[3], a, stream);
-    if (rc) return rc;
-    if (dump(3, b.a[4], 64, f8)) return WN_OK;
+    if ((rc = launch_layer<kC4>(h, f8, b.a[3], a, stream))) return rc;
+    if (dump(kC4)) return WN_OK;
     act(b.a[5], 64, nullptr, 0);
-    rc = f8 ? launch_umma<7, 64, 64, kEpiAct, 0, 1, 7, IN8 | OUT8>(h, kC5, b.a[4], a, stream)
-            : launch_umma<7, 64, 64, kEpiAct, 1, 1, 7>(h, kC5, b.a[4], a, stream);
-    if (rc) return rc;
-    if (dump(4, b.a[5], 64, f8)) return WN_OK;
+    if ((rc = launch_layer<kC5>(h, f8, b.a[4], a, stream))) return rc;
+    if (dump(kC5)) return WN_OK;
     act(b.a[6], 64, nullptr, 0);
-    rc = f8 ? launch_umma<5, 64, 64, kEpiAct, 0, 1, 5, IN8 | OUT8>(h, kC6, b.a[5], a, stream)
-            : launch_umma<5, 64, 64, kEpiAct, 1, 1, 5>(h, kC6, b.a[5], a, stream);
-    if (rc) return rc;
-    if (dump(5, b.a[6], 64, f8)) return WN_OK;
+    if ((rc = launch_layer<kC6>(h, f8, b.a[5], a, stream))) return rc;
+    if (dump(kC6)) return WN_OK;
     act(b.a[7], 64, nullptr, 0);
-    rc = f8 ? launch_umma<3, 64, 64, kEpiAct, 0, 1, 9, IN8>(h, kC7, b.a[6], a, stream)
-            : launch_umma<3, 64, 64, kEpiAct, 1, 1, 9>(h, kC7, b.a[6], a, stream);
-    if (rc) return rc;
-    if (dump(6, b.a[7], 64)) return WN_OK;
-    a.out_f32 = dbg_layer == 7 ? dbg_dst : b.cm;
-    if ((rc = launch_umma<3, 64, 16, kEpiSigmoid, 1, 1, 9>(h, kC8, b.a[7], a, stream))) return rc;
-    if (dbg_layer == 7) return WN_OK;
+    if ((rc = launch_layer<kC7>(h, f8, b.a[6], a, stream))) return rc;
+    if (dump(kC7)) return WN_OK;
+    // the confidence maps are fp32: a dump of them is written in place of b.cm
+    const bool dump_maps = dbg_layer == kSpecs[kC8].slot;
+    a.out_f32 = dump_maps ? dbg_dst : b.cm;
+    if ((rc = launch_layer<kC8>(h, f8, b.a[7], a, stream))) return rc;
+    if (dump_maps) return WN_OK;
   }
   if (!want_ref) return WN_OK;
   act(b.r[2], 96, nullptr, 0);
-  rc = f8 ? launch_umma<5, 96, 32, kEpiAct, 0, 3, 5, IN8>(h, kR2, b.r[1], a, stream)
-          : launch_umma<5, 96, 32, kEpiAct, 1, 3, 5>(h, kR2, b.r[1], a, stream);
-  if (rc) return rc;
-  if (dump(9, b.r[2], 96)) return WN_OK;
+  if ((rc = launch_layer<kR2>(h, f8, b.r[1], a, stream))) return rc;
+  if (dump(kR2)) return WN_OK;
   last();
-  if ((rc = launch_umma<3, 96, 16, kEpiGate, 1, 1, 9>(h, kR3, b.r[2], a, stream))) return rc;
+  if ((rc = launch_layer<kR3>(h, f8, b.r[2], a, stream))) return rc;
   return o.out_u8 ? mirror_u8(h, o.out_u8, o.peers, (size_t)n * H * W * 3, o.run_if, stream) : WN_OK;
 }
 

@@ -6,7 +6,6 @@ libwaternet_b200.so.
 from __future__ import annotations
 
 import ctypes
-import os
 import threading
 from typing import Dict, Optional, Sequence, Tuple
 
@@ -83,10 +82,6 @@ class Engine:
         handle = ctypes.c_void_p()
         _lib.check(self.lib.wn_create(device.index, ctypes.byref(handle)), "wn_create")
         self.handle = handle
-        # bring-up / A-B switches of the conv pipeline (wn_debug_set_flags): 256 / 512 = conv3+conv4 / conv7+conv8 unfused
-        flags = int(os.environ.get("WATERNET_B200_DEBUG_FLAGS", "0"), 0)
-        if flags:
-            _lib.check(self.lib.wn_debug_set_flags(handle, flags), "wn_debug_set_flags")
         self._ws = _ws_pool.setdefault(device.index, {})
         self._weights_key = None
         self._weights_keepalive = None
@@ -118,10 +113,6 @@ class Engine:
     def set_chunk_pixels(self, max_pixels: int) -> None:
         """Lower the per-pass pixel cap (0 = default 8 Mi); tests force the multi-pass path with it."""
         _lib.check(self.lib.wn_set_chunk_pixels(self.handle, int(max_pixels)), "wn_set_chunk_pixels")
-
-    def set_debug_flags(self, flags: int) -> None:
-        """wn_debug_set_flags: bits 0-3 switch pipeline pieces off (results wrong), bit 8 runs conv3 / conv4 unfused."""
-        _lib.check(self.lib.wn_debug_set_flags(self.handle, int(flags)), "wn_debug_set_flags")
 
     def f8_overflowed(self) -> bool:
         """True once the fp8-correction mode saw an activation beyond the e4m3 range.  The batch that did was
