@@ -19,6 +19,7 @@
  *   wn_enhance_u8         hubconf.py:85-94 + net.py:99-108: preprocess -> model -> postprocess
  *                         (the per-frame body of inference.py:261-323)
  *   wn_enhance_u8_tiled   the same, computed in overlapping windows: bounded workspace for images of any size
+ *   wn_enhance_u8_ragged  the same for n images of n sizes in one call (inference.py --source <directory>)
  *   wn_forward_train /    train.py:108 `out = model(...)` and train.py:130-131 `loss.backward()`
  *   wn_backward           (autograd through net.py:99-108)
  *
@@ -39,7 +40,7 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 5
+#define WN_ABI_VERSION 6
 
 #define WN_OK 0
 #define WN_E_INVALID (-1)   /* bad argument (NULL pointer, non-positive size, unknown mode) */
@@ -168,6 +169,32 @@ size_t wn_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int til
 int wn_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, float* out_f32_or_null,
                         int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels,
                         int mode, void* workspace, size_t workspace_bytes, void* stream);
+
+/*
+ * A ragged batch: n images, each of its own size, enhanced in one call (a directory of photos).  Image i is cut into
+ * exactly the windows wn_enhance_u8_tiled would use for it alone (tile_h x tile_w; a small image is one window).
+ * The windows of all images are sorted by shape and packed into passes of equally sized slots, each window at its
+ * slot's top-left, with the slot pixels outside it held at zero; a pass holds at most max_pass_pixels slot pixels
+ * (0 = 8 Mi; at least one window), at most 65535 windows, and -- when it holds more than one -- at most 25 % of
+ * zero padding.  The outputs of image i equal, bit for bit, what wn_enhance_u8 returns for image i alone, in both
+ * tensor-core modes, provided the e4m3 range guard stays down: the guard's flag is sticky, so once a pass raises it,
+ * that pass and every later one are recomputed with the bf16x3 kernels, including images that did not raise it.
+ * Workspace: the largest pass (~1.9 KB per slot pixel) plus ~84 KB of LUTs per image plus the window table; it does
+ * not grow with any image's size.  images_host is a HOST array of n entries with device pointers; out_f32 may be
+ * NULL per image.  Tensor-core modes only (WN_MODE_FP32_SIMT: WN_E_UNSUPPORTED); no peer outputs.  The call copies
+ * its plan to the device from pageable host memory once, so it cannot be captured in a CUDA graph.
+ * The workspace function returns 0 for arguments the call rejects.
+ */
+typedef struct {
+  const uint8_t* rgb;  /* device, HWC uint8 (height, width, 3), contiguous */
+  uint8_t* out_u8;     /* device, HWC uint8, same size */
+  float* out_f32;      /* device, fp32 NCHW (1, 3, height, width), or NULL */
+  int height, width;
+} wn_ragged_image;
+size_t wn_enhance_ragged_workspace_bytes(const int* heights_host, const int* widths_host, int n, int tile_h,
+                                         int tile_w, long long max_pass_pixels, int mode);
+int wn_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images_host, int n, int tile_h, int tile_w,
+                         long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * wn_enhance_u8 with the all-gather of the output fused into the kernel that produces it (SURVEY 8e: the one

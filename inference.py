@@ -1,6 +1,7 @@
 """Enhance images / videos (same CLI and output layout as the reference's inference.py).
 
     python inference.py --source <image|video|directory> [--weights W] [--name NAME] [--show-split]
+                        [--tile N] [--batch N]
 
 Every frame goes uint8 -> GPU (preprocess, gated-fusion forward, uint8 postprocess) -> uint8
 through ``waternet_b200.api.Enhancer``; video frames are processed in small batches.  File and
@@ -61,6 +62,16 @@ def run_image(cv2, enhancer, path, savedir, show_split):
     cv2.imwrite(os.fspath(savedir / path.name), split_view(cv2, bgr, out_bgr) if show_split else out_bgr)
 
 
+def run_images(cv2, enhancer, paths, savedir, show_split):
+    """Several still images of their own sizes in one ragged call (``--batch``); written as run_image writes them."""
+    bgrs = [cv2.imread(os.fspath(p)) for p in paths]
+    outs = enhancer.enhance_many([np.ascontiguousarray(b[..., ::-1]) for b in bgrs])
+    savedir.mkdir(parents=True, exist_ok=True)
+    for path, bgr, out in zip(paths, bgrs, outs):
+        out_bgr = np.ascontiguousarray(out[..., ::-1])
+        cv2.imwrite(os.fspath(savedir / path.name), split_view(cv2, bgr, out_bgr) if show_split else out_bgr)
+
+
 def run_video(cv2, enhancer, path, savedir, show_split):
     cap = cv2.VideoCapture(os.fspath(path))
     fps = int(cap.get(cv2.CAP_PROP_FPS))
@@ -110,7 +121,11 @@ def main():
     ap.add_argument("--tile", type=int, default=None,
                     help="(Optional) Compute each image in overlapping tiles of at most N x N output pixels: the same "
                          "result with GPU memory that does not grow with the image size (e.g. 998 for large photos).")
+    ap.add_argument("--batch", type=int, default=1,
+                    help="(Optional) Enhance the still images of a directory N at a time, each at its own size, in "
+                         "one GPU call per group (the same result; --tile sets the tile of that call).")
     args = ap.parse_args()
+    assert args.batch >= 1, "--batch must be at least 1"
     assert args.source is not None, "No input image/video specified in --source!"
     if not torch.cuda.is_available():
         raise SystemExit("inference.py needs a CUDA device (H100); waternet_b200 has no CPU path")
@@ -126,11 +141,20 @@ def main():
     outdir = ROOT / "output"
     outdir.mkdir(exist_ok=True)
     savedir = outdir / args.name if args.name is not None else next_run_dir(outdir)
+    pending = []  # still images waiting for a group of --batch
     for f in files:
         if f.suffix.lower() in IM_SUFFIXES:
-            run_image(cv2, enhancer, f, savedir, args.show_split)
+            if args.batch == 1:
+                run_image(cv2, enhancer, f, savedir, args.show_split)
+                continue
+            pending.append(f)
+            if len(pending) == args.batch:
+                run_images(cv2, enhancer, pending, savedir, args.show_split)
+                pending = []
         elif f.suffix.lower() in VID_SUFFIXES:
             run_video(cv2, enhancer, f, savedir, args.show_split)
+    if pending:
+        run_images(cv2, enhancer, pending, savedir, args.show_split)
     print(f"Saved output to {savedir}!")
 
 

@@ -19,9 +19,15 @@ MODE_BF16_FP8 = 2
 MODE_DEFAULT = -1
 NUM_PARAMS = 34
 NUM_TIMING_SLOTS = 23
-ABI_VERSION = 5
+ABI_VERSION = 6
 PEER_HANDLE_BYTES = 64  # WN_PEER_HANDLE_BYTES
 MAX_PEERS = 15          # WN_MAX_PEERS
+
+
+class RaggedImage(ctypes.Structure):
+    """wn_ragged_image: one image of a ragged batch (device pointers)."""
+    _fields_ = [("rgb", c_void_p), ("out_u8", c_void_p), ("out_f32", c_void_p), ("height", c_int), ("width", c_int)]
+
 
 # name -> (restype, argtypes); mirrors include/waternet_b200.h one to one
 _SIGNATURES = {
@@ -51,6 +57,10 @@ _SIGNATURES = {
     "wn_enhance_tiled_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong, c_int]),
     "wn_enhance_u8_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                     ctypes.c_longlong, c_int, c_void_p, c_size_t, c_void_p]),
+    "wn_enhance_ragged_workspace_bytes": (c_size_t, [POINTER(c_int), POINTER(c_int), c_int, c_int, c_int,
+                                                     ctypes.c_longlong, c_int]),
+    "wn_enhance_u8_ragged": (c_int, [c_void_p, POINTER(RaggedImage), c_int, c_int, c_int, ctypes.c_longlong, c_int,
+                                     c_void_p, c_size_t, c_void_p]),
     "wn_launch_count": (c_uint64, [c_void_p]),
     "wn_submodule_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "wn_confidence_maps": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p,

@@ -67,6 +67,7 @@ class Enhancer:
         self._next = 0
         self._pin_in = None
         self._pin_out = None
+        self._pin_many = None  # enhance_many's staging buffers (in, out), grown to the largest call
         dev = self.engine.device
         self._s_in = torch.cuda.Stream(dev)
         self._s_out = torch.cuda.Stream(dev)
@@ -87,6 +88,42 @@ class Enhancer:
         self.enhance_pinned(self._pin_in, self._pin_out)
         out = self._pin_out.numpy().copy()
         return out[0] if single else out
+
+    def enhance_many(self, images) -> list:
+        """A list of uint8 HWC images, each of its own size (a directory of photos), enhanced in one ragged call
+        (``Engine.enhance_ragged`` with ``tile``, or ``Engine.DEFAULT_TILE`` when that is None): one copy in through
+        a pinned staging buffer of the total size, one call, one copy out.  Returns the list of enhanced images; each
+        equals what ``self(image)`` returns.  Tensor-core precisions only."""
+        if self.mode == _lib.MODE_FP32_SIMT:
+            raise ValueError("enhance_many: ragged batches run in the tensor-core precisions only, not fp32")
+        arrs = [np.asarray(a) for a in images]
+        for i, a in enumerate(arrs):
+            if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+                raise ValueError(f"image {i}: expected uint8 HWC RGB, got {a.dtype} {a.shape}")
+        offs = np.cumsum([0] + [a.size for a in arrs]).tolist()
+        total = offs[-1]
+        if total == 0:
+            return [a.copy() for a in arrs]
+        if self._pin_many is None or self._pin_many[0].numel() < total:
+            self._pin_many = (torch.empty(total, dtype=torch.uint8).pin_memory(),
+                              torch.empty(total, dtype=torch.uint8).pin_memory())
+        pin_in, pin_out = self._pin_many
+        for a, o in zip(arrs, offs):
+            pin_in.numpy()[o:o + a.size] = a.reshape(-1)
+        eng = self.model.engine()  # re-packs if the parameters changed since the last call (no-op otherwise)
+        dev = eng.device
+        dev_in = torch.empty(total, dtype=torch.uint8, device=dev)
+        dev_out = torch.empty(total, dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):  # the copies and the call on the device's current stream
+            dev_in.copy_(pin_in[:total], non_blocking=True)
+            views = [(dev_in[o:o + a.size].view(a.shape), dev_out[o:o + a.size].view(a.shape))
+                     for a, o in zip(arrs, offs)]
+            eng.enhance_ragged([v for v, _ in views], tile=self.tile or Engine.DEFAULT_TILE, mode=self.mode,
+                               out_u8=[v for _, v in views])
+            pin_out[:total].copy_(dev_out, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+        out = pin_out.numpy()
+        return [out[o:o + a.size].reshape(a.shape).copy() for a, o in zip(arrs, offs)]
 
     # ---- kernels of one pass --------------------------------------------------------------------
     def _run_kernels(self, eng: Engine, slot: _Slot, a: int, b: int, whole: bool, peer_out=()) -> None:

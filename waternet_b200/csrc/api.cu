@@ -368,6 +368,73 @@ int wn_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, flo
                                workspace, workspace_bytes, (cudaStream_t)stream, m == WN_MODE_BF16_FP8 ? 1 : 0);
 }
 
+// the argument checks the ragged call and its workspace function share (the image pointers aside)
+static int ragged_check(const char* what, int n, int tile_h, int tile_w, long long max_pass_pixels, int mode) {
+  if (n <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
+    set_error("%s: bad shape n=%d tile=%dx%d max_pass_pixels=%lld", what, n, tile_h, tile_w, max_pass_pixels);
+    return WN_E_INVALID;
+  }
+  if (n > 65535) {
+    set_error("%s: too many images: n=%d", what, n);
+    return WN_E_UNSUPPORTED;
+  }
+  const int m = resolve_mode(mode);
+  if (m == WN_MODE_FP32_SIMT) {
+    set_error("%s: ragged batches run in the tensor-core modes only, not WN_MODE_FP32_SIMT", what);
+    return WN_E_UNSUPPORTED;
+  }
+  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) {
+    set_error("%s: unknown mode %d", what, mode);
+    return WN_E_INVALID;
+  }
+  return WN_OK;
+}
+static int ragged_check_size(const char* what, int i, int height, int width) {
+  if (height <= 0 || width <= 0) {
+    set_error("%s: bad size of image %d: h=%d w=%d", what, i, height, width);
+    return WN_E_INVALID;
+  }
+  if ((size_t)height * width > (size_t)0x7fffffff / 3) {
+    set_error("image too large: image %d h=%d w=%d", i, height, width);
+    return WN_E_UNSUPPORTED;
+  }
+  return WN_OK;
+}
+
+size_t wn_enhance_ragged_workspace_bytes(const int* heights_host, const int* widths_host, int n, int tile_h,
+                                         int tile_w, long long max_pass_pixels, int mode) {
+  const char* what = "wn_enhance_ragged_workspace_bytes";
+  if (!heights_host || !widths_host || ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode)) return 0;
+  for (int i = 0; i < n; i++)
+    if (ragged_check_size(what, i, heights_host[i], widths_host[i])) return 0;
+  return umma_enhance_ragged_workspace_bytes(heights_host, widths_host, n, tile_h, tile_w, max_pass_pixels);
+}
+
+int wn_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images_host, int n, int tile_h, int tile_w,
+                         long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* what = "wn_enhance_u8_ragged";
+  if (!h || !images_host || !workspace) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  int rc = ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode);
+  if (rc) return rc;
+  for (int i = 0; i < n; i++) {
+    if (!images_host[i].rgb || !images_host[i].out_u8) {
+      set_error("%s: null image pointer (image %d)", what, i);
+      return WN_E_INVALID;
+    }
+    if ((rc = ragged_check_size(what, i, images_host[i].height, images_host[i].width))) return rc;
+  }
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  return umma_enhance_u8_ragged(h, images_host, n, tile_h, tile_w, max_pass_pixels, workspace, workspace_bytes,
+                                (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0);
+}
+
 // ---- the reference's callable sub-modules (net.py:45-56 ConfidenceMapGenerator.forward, :75-80 Refiner.forward)
 size_t wn_submodule_workspace_bytes(int n, int h, int w, int mode) {
   if (n <= 0 || h <= 0 || w <= 0) return 0;

@@ -143,6 +143,23 @@ int preprocess_u8_luts(wn_handle* h, const uint8_t* rgb, int n, int height, int 
                        size_t workspace_bytes, cudaStream_t stream);
 int preprocess_u8_window_planes(wn_handle* h, const uint8_t* rgb, int n, const TileGeom& tiles, long long win0,
                                 int count, uint4* planes, void* workspace, cudaStream_t stream);
+// ... and for a ragged batch, where every image has its own size: the preprocess geometry of one image (CLAHE tile,
+// clip limit, LUT scale, histogram slabs), the statistics and LUTs of all n images from their device table (one
+// stats and one LUT launch), then the operand planes of `count` windows in slots of slot_h x slot_w (zeros outside
+// each window's valid extent).  Workspace: that of preprocess_workspace_bytes(n, ...), untouched in between.
+struct RaggedImage {
+  const uint8_t* rgb;
+  int H, W;
+  int th, tw, clip;          // CLAHE tile and clip limit (PreGeom)
+  int rows_per_slab, slabs;  // stats grid: slabs of tile rows per CLAHE tile
+  float lut_scale;
+};
+static_assert(sizeof(RaggedImage) == 40, "RaggedImage: engine.RAGGED_IMAGE_BYTES restates this size");
+RaggedImage ragged_image(const uint8_t* rgb, int height, int width);
+int preprocess_u8_ragged_luts(wn_handle* h, int n, const RaggedImage* imgs, int max_slabs, void* workspace,
+                              cudaStream_t stream);
+int preprocess_u8_ragged_planes(wn_handle* h, int n, const RaggedImage* imgs, const RaggedWindow* wins, int count,
+                                int slot_h, int slot_w, uint4* planes, void* workspace, cudaStream_t stream);
 
 // conv_simt.cu
 int simt_pack_weights(wn_handle* h, const float* const* params, cudaStream_t stream);
@@ -184,6 +201,8 @@ struct FwdOpts {
   int stack = kStackAll;       // kStackCmg: stop after the confidence maps; kStackRefiners: refiners only
   const TileGeom* tiles = nullptr;  // tiled forward: image n of the batch is window win0 + n of these tiles, and the
   long long win0 = 0;               // last launch stores its kept rectangle into out / out_u8 at image coordinates
+  const RaggedWindow* rwin = nullptr;  // ragged pass (device table): image n of the batch is window rwin[n] in its
+                                       // slot; every layer masks it, the last launch stores into its own image
 };
 int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out, int n,
                         int height, int width, const FwdBuffers& b, cudaStream_t stream,
@@ -210,6 +229,12 @@ size_t umma_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int t
 int umma_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* out_f32, int n, int height,
                           int width, int tile_h, int tile_w, long long max_pass_pixels, void* workspace,
                           size_t workspace_bytes, cudaStream_t stream, int scheme);
+// the arguments are checked by the caller (api.cu)
+size_t umma_enhance_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
+                                           long long max_pass_pixels);
+int umma_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images, int n, int tile_h, int tile_w,
+                           long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream,
+                           int scheme);
 int umma_f8_overflowed(const wn_handle* h);
 
 // conv_bwd.cu

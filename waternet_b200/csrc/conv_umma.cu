@@ -246,20 +246,27 @@ size_t umma_forward_workspace_bytes(int n, int h, int w) {
 }
 
 // Launch layer LI in the fp8-correction scheme (f8) or in bf16x3.  A layer's fp8 form reads its own weight images,
-// in the [hi | fp8] layout.
-template <int LI>
-static int launch_layer(wn_handle* h, bool f8, void* in_base, ConvArgs a, cudaStream_t stream) {
+// in the [hi | fp8] layout.  A pass of a ragged batch (a.rwin) runs the RAG instantiations of the layers that mask
+// (kEpiAct) or store per window (kEpiGate); the confidence maps are per pixel and need neither.
+template <int LI, bool RAG>
+static int launch_layer_as(wn_handle* h, bool f8, void* in_base, ConvArgs a, cudaStream_t stream) {
   constexpr UmmaLayerSpec s = kSpecs[LI];
+  constexpr bool R = RAG && s.epi != kEpiSigmoid;
   const UmmaWeights* u = h->umma;
   if (f8) {
     constexpr int FMT = (s.f8 ? kFmtIn8 : 0) | (writes_f8(LI) ? kFmtOut8 : 0);
     if constexpr ((FMT & kFmtOut8) != 0) a.f8_overflow = u->overflow_dev;
     if constexpr (s.f8) a.f8_scale = u->scale8[LI] + 1;
-    return launch_conv<s.ks, s.cinpad, s.npad, s.epi, (s.f8 ? 0 : s.concat), s.nblk, s.tps, FMT>(
+    return launch_conv<s.ks, s.cinpad, s.npad, s.epi, (s.f8 ? 0 : s.concat), s.nblk, s.tps, FMT, R>(
         h, s.slot, s.f8 ? u->stages8[LI] : u->stages[LI], u->bias[LI], in_base, a, stream);
   }
-  return launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps>(h, s.slot, u->stages[LI], u->bias[LI],
-                                                                             in_base, a, stream);
+  return launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps, 0, R>(h, s.slot, u->stages[LI],
+                                                                                 u->bias[LI], in_base, a, stream);
+}
+template <int LI>
+static int launch_layer(wn_handle* h, bool f8, void* in_base, ConvArgs a, cudaStream_t stream) {
+  return a.rwin ? launch_layer_as<LI, true>(h, f8, in_base, a, stream)
+                : launch_layer_as<LI, false>(h, f8, in_base, a, stream);
 }
 
 // bf16 hi/lo planes -> fp32 NCHW (test aid)
@@ -315,6 +322,7 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   memset(&a, 0, sizeof(a));
   a.N = n; a.H = H; a.W = W;
   a.run_if = o.run_if;
+  a.rwin = o.rwin;
   int rc;
   // fp8-correction scheme (inference): the tensor-bound layers replace the two bf16 correction passes by one
   // fp8 MMA (UmmaCfg FMT); a layer whose consumer is such a layer writes the hi + fp8-planes format
@@ -586,6 +594,102 @@ int umma_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, flo
     o.tiles = &g;
     o.win0 = w0;
     rc = umma_pass(h, no_in, none, out_f32, cur, g.win_h, g.win_w, b, stream, o);
+    if (rc) return rc;
+  }
+  return mirror_overflow(h, scheme, stream);
+}
+
+// The ragged form (tiling.cuh ragged_plan): the statistics and LUTs of all n images in one launch each, then per
+// pass a batch of slots runs through the same ten launches (and range guard) as a batch of images; each window's
+// valid extent is masked and its kept rectangle stored into its own image.  The plan (per-image geometry and one
+// descriptor per window) is copied into the workspace once per call, so the call cannot be captured in a graph.
+// Workspace: the largest pass plus the per-image LUTs plus the table, independent of the image sizes.
+static size_t align256(size_t v) { return (v + 255) / 256 * 256; }
+static size_t ragged_table_bytes(int n, size_t windows) {
+  return align256(align256((size_t)n * sizeof(RaggedImage)) + windows * sizeof(RaggedWindow));
+}
+static long long ragged_pass_pixels(long long max_pass_pixels) {
+  return max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels;
+}
+static size_t ragged_workspace(int n, const std::vector<RaggedWindow>& wins, const std::vector<RaggedPass>& passes) {
+  long long px = 0;
+  for (const RaggedPass& p : passes) {
+    const long long v = (long long)p.count * p.slot_h * p.slot_w;
+    px = v > px ? v : px;
+  }
+  return (size_t)px * kUmmaBytesPerPixel + 4096 + (preprocess_workspace_bytes(n, 1, 1) + 255) / 256 * 256 +
+         ragged_table_bytes(n, wins.size()) + 1024;
+}
+
+size_t umma_enhance_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
+                                           long long max_pass_pixels) {
+  std::vector<RaggedWindow> wins;
+  std::vector<RaggedPass> passes;
+  ragged_plan(hs, ws, n, tile_h, tile_w, ragged_pass_pixels(max_pass_pixels), &wins, &passes);
+  return ragged_workspace(n, wins, passes);
+}
+
+int umma_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images, int n, int tile_h, int tile_w,
+                           long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream,
+                           int scheme) {
+  if (!h->umma) {
+    set_error("tensor-core weights have not been packed");
+    return WN_E_STATE;
+  }
+  std::vector<int> hs(n), ws(n);
+  for (int i = 0; i < n; i++) {
+    hs[i] = images[i].height;
+    ws[i] = images[i].width;
+  }
+  std::vector<RaggedWindow> wins;
+  std::vector<RaggedPass> passes;
+  ragged_plan(hs.data(), ws.data(), n, tile_h, tile_w, ragged_pass_pixels(max_pass_pixels), &wins, &passes);
+  const size_t need = ragged_workspace(n, wins, passes);
+  if (workspace_bytes < need) {
+    set_error("ragged enhance workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  int rc = get_encoder();
+  if (rc) return rc;
+  scheme = effective_scheme(h, scheme);
+  // workspace: [LUTs of the n images][table: n RaggedImage | windows][one pass]
+  uint8_t* pre_ws = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
+  const size_t pre_b = (preprocess_workspace_bytes(n, 1, 1) + 255) / 256 * 256;
+  uint8_t* table = pre_ws + pre_b;
+  const size_t img_b = align256((size_t)n * sizeof(RaggedImage));
+  void* fwd_ws = table + ragged_table_bytes(n, wins.size());
+  std::vector<uint8_t> host(img_b + wins.size() * sizeof(RaggedWindow));
+  RaggedImage* imgs = reinterpret_cast<RaggedImage*>(host.data());
+  int max_slabs = 1;
+  for (int i = 0; i < n; i++) {
+    imgs[i] = ragged_image(images[i].rgb, images[i].height, images[i].width);
+    max_slabs = imgs[i].slabs > max_slabs ? imgs[i].slabs : max_slabs;
+  }
+  for (RaggedWindow& w : wins) {
+    w.rgb = images[w.img].rgb;
+    w.out_u8 = images[w.img].out_u8;
+    w.out_f32 = images[w.img].out_f32;
+  }
+  memcpy(host.data() + img_b, wins.data(), wins.size() * sizeof(RaggedWindow));
+  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
+  WN_CUDA(cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
+  const RaggedImage* d_imgs = reinterpret_cast<const RaggedImage*>(table);
+  const RaggedWindow* d_wins = reinterpret_cast<const RaggedWindow*>(table + img_b);
+  if ((rc = preprocess_u8_ragged_luts(h, n, d_imgs, max_slabs, pre_ws, stream))) return rc;
+  const int64_t none[4][4] = {};
+  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (const RaggedPass& p : passes) {
+    FwdBuffers b = carve(fwd_ws, p.count, p.slot_h, p.slot_w);
+    WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));
+    rc = preprocess_u8_ragged_planes(h, n, d_imgs, d_wins + p.first, p.count, p.slot_h, p.slot_w, b.act0, pre_ws,
+                                     stream);
+    if (rc) return rc;
+    FwdOpts o;
+    o.scheme = scheme;
+    o.packed = true;
+    o.hi_only = true;
+    o.rwin = d_wins + p.first;
+    rc = umma_pass(h, no_in, none, nullptr, p.count, p.slot_h, p.slot_w, b, stream, o);
     if (rc) return rc;
   }
   return mirror_overflow(h, scheme, stream);

@@ -128,13 +128,26 @@ __device__ __forceinline__ int reflect101(int p, int len) {
 // ---------------------------------------------------------------------------
 constexpr int kStatsThreads = 256;
 
+// RAG (ragged batches): image n = blockIdx.z takes its pointer and geometry from imgs[n]; the grid is sized for the
+// image with the most slabs, and the surplus slabs of the others exit
+template <bool RAG = false>
 __global__ void __launch_bounds__(kStatsThreads)
 stats_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw, int rows_per_slab,
              const Tables* __restrict__ tables, uint32_t* __restrict__ tile_hist,
-             uint32_t* __restrict__ rgb_hist) {
+             uint32_t* __restrict__ rgb_hist, const RaggedImage* __restrict__ imgs) {
   __shared__ uint32_t s_hist[4][256];  // 0: L of this tile, 1..3: R, G, B
   __shared__ uint16_t s_gtab[256];
   __shared__ uint16_t s_ctab[3072];
+  if constexpr (RAG) {
+    const RaggedImage im = imgs[blockIdx.z];
+    if ((int)blockIdx.y >= im.slabs) return;
+    rgb = im.rgb;
+    H = im.H;
+    W = im.W;
+    th = im.th;
+    tw = im.tw;
+    rows_per_slab = im.rows_per_slab;
+  }
   const int tid = threadIdx.x;
   for (int i = tid; i < 1024; i += kStatsThreads) (&s_hist[0][0])[i] = 0;
   for (int i = tid; i < 256; i += kStatsThreads) s_gtab[i] = tables->gtab[i];
@@ -145,7 +158,7 @@ stats_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw, int 
   const int n = blockIdx.z;
   const int r0 = blockIdx.y * rows_per_slab;
   const int r1 = min(r0 + rows_per_slab, th);
-  const uint8_t* img = rgb + (size_t)n * H * W * 3;
+  const uint8_t* img = RAG ? rgb : rgb + (size_t)n * H * W * 3;
   const int count = (r1 - r0) * tw;
   for (int i = tid; i < count; i += kStatsThreads) {
     int rr = i / tw;
@@ -217,15 +230,22 @@ __device__ double np_quantile_from_cum(const uint32_t* cum, int n, double q) {
   return res;
 }
 
+// RAG: image n = blockIdx.y takes its pixel count, clip limit and LUT scale from imgs[n]
+template <bool RAG = false>
 __global__ void __launch_bounds__(256)
 luts_kernel(const uint32_t* __restrict__ tile_hist, const uint32_t* __restrict__ rgb_hist,
             int npix, int clip, float lut_scale, uint8_t* __restrict__ clahe_lut,
-            uint8_t* __restrict__ wb_lut, int gray) {
+            uint8_t* __restrict__ wb_lut, int gray, const RaggedImage* __restrict__ imgs) {
   __shared__ uint32_t s_warp[8];
   __shared__ uint32_t s_cum[3][256];
   __shared__ unsigned long long s_sum[3];
   __shared__ uint32_t s_red;
   const int tid = threadIdx.x, n = blockIdx.y;
+  if constexpr (RAG) {
+    npix = imgs[n].H * imgs[n].W;
+    clip = imgs[n].clip;
+    lut_scale = imgs[n].lut_scale;
+  }
   if (blockIdx.x < 64) {
     // OpenCV CLAHE_CalcLut_Body: clip, redistribute the excess, prefix-sum, scale.
     const int tile = blockIdx.x;
@@ -324,13 +344,16 @@ __device__ __forceinline__ void store_level_planes(uint4* planes, size_t n, size
 }
 
 // WIN (the tiled forward): blockIdx.y is window win0 + blockIdx.y of `tiles`; the kernel writes that window's operand
-// planes (out.planes only), reading the full image and interpolating its CLAHE tiles at image coordinates
-template <bool VEC4, bool WIN = false>
+// planes (out.planes only), reading the full image and interpolating its CLAHE tiles at image coordinates.
+// RAG (ragged batches): blockIdx.y is window wins[blockIdx.y], in a slot of tiles.win_h x tiles.win_w; the image and
+// its geometry come from the descriptors, and slot pixels outside the window's valid extent get zero planes.
+template <bool VEC4, bool WIN = false, bool RAG = false>
 __global__ void __launch_bounds__(256)
 apply_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw,
              const Tables* __restrict__ tables, const uint8_t* __restrict__ clahe_lut,
-             const uint8_t* __restrict__ wb_lut, ApplyOut out, int iters, TileGeom tiles, long long win0) {
-  static_assert(!(VEC4 && WIN), "the windowed form has no vector path");
+             const uint8_t* __restrict__ wb_lut, ApplyOut out, int iters, TileGeom tiles, long long win0,
+             const RaggedImage* __restrict__ imgs, const RaggedWindow* __restrict__ wins) {
+  static_assert(!(VEC4 && WIN) && !(VEC4 && RAG) && !(WIN && RAG), "one windowed form, without a vector path");
   __shared__ __align__(16) uint8_t s_clahe[64 * 256];
   __shared__ __align__(16) uint8_t s_wb[768];
   __shared__ __align__(16) uint8_t s_gamma[256];
@@ -342,7 +365,17 @@ apply_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw,
   __shared__ float s_div[256];
   TileWindow win = {};
   if constexpr (WIN) win = tile_window(tiles, win0 + blockIdx.y);
-  const int tid = threadIdx.x, n = WIN ? win.img : blockIdx.y;
+  RaggedWindow rw = {};
+  if constexpr (RAG) {
+    rw = wins[blockIdx.y];
+    const RaggedImage im = imgs[rw.img];
+    rgb = im.rgb;
+    H = im.H;
+    W = im.W;
+    th = im.th;
+    tw = im.tw;
+  }
+  const int tid = threadIdx.x, n = WIN ? win.img : RAG ? rw.img : blockIdx.y;
   {
     const uint4* src = reinterpret_cast<const uint4*>(clahe_lut + (size_t)n * 64 * 256);
     uint4* dst = reinterpret_cast<uint4*>(s_clahe);
@@ -440,6 +473,21 @@ apply_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw,
       const uint8_t* p = rgb + ((size_t)n * plane + ipix) * 3;
       int lv[12];
       one_pixel(ipix, p[0], p[1], p[2], lv);
+      store_level_planes(out.planes, blockIdx.y, wplane, pix, lv);
+    }
+  } else if constexpr (RAG) {
+    // slot pixel (sy, sx) is image pixel (ys + sy, xs + sx) inside the valid extent; planes [slot][2][slot pixels]
+    const int wplane = tiles.win_h * tiles.win_w;
+    for (int it = 0; it < iters; it++) {
+      const int pix = (blockIdx.x * iters + it) * 256 + tid;
+      if (pix >= wplane) break;
+      const int sy = pix / tiles.win_w, sx = pix - sy * tiles.win_w;
+      int lv[12] = {};  // zero operands outside the window: what the tiled call's TMA reads beyond its window
+      if (sy < rw.vh && sx < rw.vw) {
+        const int ipix = (rw.ys + sy) * W + rw.xs + sx;
+        const uint8_t* p = rgb + (size_t)ipix * 3;
+        one_pixel(ipix, p[0], p[1], p[2], lv);
+      }
       store_level_planes(out.planes, blockIdx.y, wplane, pix, lv);
     }
   } else {
@@ -623,13 +671,13 @@ static int preprocess_luts(wn_handle* h, const uint8_t* rgb, int n, int H, int W
   TimedScope ts(h, kSlotStats, stream);
   stats_kernel<<<dim3(64, slabs, n), kStatsThreads, 0, stream>>>(rgb, H, W, g.th, g.tw,
                                                                   rows_per_slab, h->d_tables,
-                                                                  tile_hist, rgb_hist);
+                                                                  tile_hist, rgb_hist, nullptr);
   WN_LAUNCH_CHECK(h);
   }
   {
   TimedScope ts(h, kSlotLuts, stream);
   luts_kernel<<<dim3(65, n), 256, 0, stream>>>(tile_hist, rgb_hist, H * W, g.clip, g.lut_scale,
-                                               b.clahe_lut, b.wb_lut, gray);
+                                               b.clahe_lut, b.wb_lut, gray, nullptr);
   WN_LAUNCH_CHECK(h);
   }
   return WN_OK;
@@ -661,13 +709,13 @@ static int preprocess_run(wn_handle* h, const uint8_t* rgb, int n, int H, int W,
     const int per_cta = 256 * iters * 4;
     apply_kernel<true><<<dim3((H * W + per_cta - 1) / per_cta, n), 256, 0, stream>>>(rgb, H, W, g.th, g.tw, h->d_tables,
                                                                                    clahe_lut, wb_lut, ao, iters,
-                                                                                   untiled, 0);
+                                                                                   untiled, 0, nullptr, nullptr);
   } else {
     const int iters = apply_iters((long long)n * H * W, h->sm_count);
     const int per_cta = 256 * iters;
     apply_kernel<false><<<dim3((H * W + per_cta - 1) / per_cta, n), 256, 0, stream>>>(rgb, H, W, g.th, g.tw, h->d_tables,
                                                                                     clahe_lut, wb_lut, ao, iters,
-                                                                                    untiled, 0);
+                                                                                    untiled, 0, nullptr, nullptr);
   }
   WN_LAUNCH_CHECK(h);
   return WN_OK;
@@ -692,7 +740,62 @@ int preprocess_u8_window_planes(wn_handle* h, const uint8_t* rgb, int n, const T
   const int iters = apply_iters((long long)count * wplane, h->sm_count);
   const int per_cta = 256 * iters;
   apply_kernel<false, true><<<dim3((wplane + per_cta - 1) / per_cta, count), 256, 0, stream>>>(
-      rgb, tiles.H, tiles.W, g.th, g.tw, h->d_tables, b.clahe_lut, b.wb_lut, ao, iters, tiles, win0);
+      rgb, tiles.H, tiles.W, g.th, g.tw, h->d_tables, b.clahe_lut, b.wb_lut, ao, iters, tiles, win0, nullptr, nullptr);
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+
+// the stats grid of one image, as preprocess_luts sizes it
+RaggedImage ragged_image(const uint8_t* rgb, int H, int W) {
+  const PreGeom g = geometry(H, W);
+  RaggedImage r;
+  r.rgb = rgb;
+  r.H = H;
+  r.W = W;
+  r.th = g.th;
+  r.tw = g.tw;
+  r.clip = g.clip;
+  r.lut_scale = g.lut_scale;
+  int slabs = (g.th * g.tw + 4095) / 4096;
+  if (slabs > g.th) slabs = g.th;
+  if (slabs < 1) slabs = 1;
+  r.rows_per_slab = (g.th + slabs - 1) / slabs;
+  r.slabs = (g.th + r.rows_per_slab - 1) / r.rows_per_slab;
+  return r;
+}
+
+int preprocess_u8_ragged_luts(wn_handle* h, int n, const RaggedImage* imgs, int max_slabs, void* workspace,
+                              cudaStream_t stream) {
+  const PreBufs b = pre_carve(workspace, n);
+  WN_CUDA(cudaMemsetAsync(b.tile_hist, 0, align_up((size_t)n * 64 * 256 * 4, 256) + (size_t)n * 768 * 4, stream));
+  {
+  TimedScope ts(h, kSlotStats, stream);
+  stats_kernel<true><<<dim3(64, max_slabs, n), kStatsThreads, 0, stream>>>(nullptr, 0, 0, 0, 0, 0, h->d_tables,
+                                                                          b.tile_hist, b.rgb_hist, imgs);
+  WN_LAUNCH_CHECK(h);
+  }
+  TimedScope ts(h, kSlotLuts, stream);
+  luts_kernel<true><<<dim3(65, n), 256, 0, stream>>>(b.tile_hist, b.rgb_hist, 0, 0, 0.f, b.clahe_lut, b.wb_lut, 0,
+                                                     imgs);
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+
+int preprocess_u8_ragged_planes(wn_handle* h, int n, const RaggedImage* imgs, const RaggedWindow* wins, int count,
+                                int slot_h, int slot_w, uint4* planes, void* workspace, cudaStream_t stream) {
+  const PreBufs b = pre_carve(workspace, n);
+  ApplyOut ao;
+  memset(&ao, 0, sizeof(ao));
+  ao.planes = planes;
+  TileGeom slot = {};
+  slot.win_h = slot_h;
+  slot.win_w = slot_w;
+  TimedScope ts(h, kSlotApply, stream);
+  const int wplane = slot_h * slot_w;
+  const int iters = apply_iters((long long)count * wplane, h->sm_count);
+  const int per_cta = 256 * iters;
+  apply_kernel<false, false, true><<<dim3((wplane + per_cta - 1) / per_cta, count), 256, 0, stream>>>(
+      nullptr, 0, 0, 0, 0, h->d_tables, b.clahe_lut, b.wb_lut, ao, iters, slot, 0, imgs, wins);
   WN_LAUNCH_CHECK(h);
   return WN_OK;
 }

@@ -10,6 +10,11 @@
 // untiled (DESIGN.md "Tiled enhance").
 #pragma once
 
+#include <stdint.h>
+
+#include <algorithm>
+#include <vector>
+
 namespace wn {
 
 constexpr int kTileHalo = 13;
@@ -66,6 +71,86 @@ __host__ __device__ inline long long tile_pass_windows(const TileGeom& g, int n,
   if (p > total) p = total;
   if (p > 65535) p = 65535;
   return p < 1 ? 1 : p;
+}
+
+// ---- ragged batches (wn_enhance_u8_ragged): n images of their own sizes in one call ----
+// Image i is cut into exactly the windows wn_enhance_u8_tiled would use for it alone (tile_geom / tile_window).  The
+// windows of all images are sorted by shape and packed into passes; a pass runs as a batch of equally sized *slots*
+// (the per-axis maximum of its windows), each window at its slot's top-left.  Slot pixels beyond a window's valid
+// extent vh x vw are stored as zeros by every layer (the windowed apply kernel and the kEpiAct epilogues), so that
+// each window sees the same zero padding as the tiled call (DESIGN.md "Ragged batches").
+struct RaggedWindow {
+  const uint8_t* rgb;      // the image, HWC uint8
+  uint8_t* out_u8;         // its HWC uint8 output
+  float* out_f32;          // its fp32 NCHW output, or null
+  int img, H, W;           // image index and size
+  int ys, xs;              // window origin in the image
+  int vh, vw;              // valid extent: the window's size
+  int ky0, ky1, kx0, kx1;  // kept rectangle, image coordinates
+  int pad_;
+};
+static_assert(sizeof(RaggedWindow) == 72, "RaggedWindow: engine.RAGGED_WINDOW_BYTES restates this size");
+
+struct RaggedPass {
+  long long first;  // first window (index into the sorted table)
+  int count;        // windows
+  int slot_h, slot_w;
+};
+
+// max_pass_pixels > 0; the caller has checked n, the sizes and the tile.  Windows go into *wins in pass order
+// (shape sorted: taller first, then wider, then image and window order) with their pointers left null.  A window
+// joins the open pass unless that would break one of its limits: count x slot pixels <= max_pass_pixels, at most
+// 65535 windows (the grid limit of the apply kernel), and masked padding at most a quarter of the slot pixels.
+inline void ragged_plan(const int* hs, const int* ws, int n, int tile_h, int tile_w, long long max_pass_pixels,
+                        std::vector<RaggedWindow>* wins, std::vector<RaggedPass>* passes) {
+  wins->clear();
+  passes->clear();
+  for (int i = 0; i < n; i++) {
+    const TileGeom g = tile_geom(hs[i], ws[i], tile_h, tile_w);
+    for (long long k = 0; k < (long long)g.ny * g.nx; k++) {
+      const TileWindow t = tile_window(g, k);
+      RaggedWindow r = {};
+      r.img = i;
+      r.H = g.H;
+      r.W = g.W;
+      r.ys = t.ys;
+      r.xs = t.xs;
+      r.vh = g.win_h;
+      r.vw = g.win_w;
+      r.ky0 = t.ky0;
+      r.ky1 = t.ky1;
+      r.kx0 = t.kx0;
+      r.kx1 = t.kx1;
+      wins->push_back(r);
+    }
+  }
+  std::stable_sort(wins->begin(), wins->end(), [](const RaggedWindow& a, const RaggedWindow& b) {
+    return a.vh != b.vh ? a.vh > b.vh : a.vw > b.vw;
+  });
+  RaggedPass p = {0, 0, 0, 0};
+  long long valid = 0;
+  for (size_t k = 0; k < wins->size(); k++) {
+    const RaggedWindow& w = (*wins)[k];
+    if (p.count > 0) {
+      const long long cnt = p.count + 1;
+      const long long slot = (long long)(p.slot_h > w.vh ? p.slot_h : w.vh) * (p.slot_w > w.vw ? p.slot_w : w.vw);
+      const long long v = valid + (long long)w.vh * w.vw;
+      if (cnt <= 65535 && cnt * slot <= max_pass_pixels && 4 * (cnt * slot - v) <= cnt * slot) {
+        p.count++;
+        p.slot_h = p.slot_h > w.vh ? p.slot_h : w.vh;
+        p.slot_w = p.slot_w > w.vw ? p.slot_w : w.vw;
+        valid = v;
+        continue;
+      }
+      passes->push_back(p);
+    }
+    p.first = (long long)k;
+    p.count = 1;
+    p.slot_h = w.vh;
+    p.slot_w = w.vw;
+    valid = (long long)w.vh * w.vw;
+  }
+  if (p.count > 0) passes->push_back(p);
 }
 
 }  // namespace wn

@@ -196,6 +196,10 @@ struct ConvArgs {
   int tiled;
   long long win0;
   TileGeom tiles;
+  // ragged batches (kernel template RAG): image n of the launch is window rwin[n] at the slot's top-left.  kEpiAct
+  // stores zeros at slot pixels outside its valid extent; kEpiGate stores its kept rectangle into that window's
+  // image (its own out_f32 / out_u8 and width)
+  const RaggedWindow* rwin;
 };
 
 __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b) {
@@ -212,9 +216,11 @@ __device__ __forceinline__ void split_bf16x2(float f0, float f1, uint32_t& hi, u
 }
 
 // Epilogue of 16 consecutive output channels [ch, ch + 16) of one pixel; f = the raw sums (scaled in the fp8 scheme).
-template <int EPI, bool OUT8>
+// RAG: `valid` is false at slot pixels outside the window's valid extent, where kEpiAct stores zeros (hi, lo and
+// fp8 planes alike; they cannot raise the e4m3 flag).
+template <int EPI, bool OUT8, bool RAG = false>
 __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bias, const float* f, int ch, int n,
-                                           int gx, int gy) {
+                                           int gx, int gy, bool valid = true) {
   const size_t hw = (size_t)g.H * g.W;
   const size_t pix = (size_t)gy * g.W + gx;
   if constexpr (EPI == kEpiAct || EPI == kEpiDgrad) {
@@ -230,6 +236,7 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
 #pragma unroll
         for (int t = 0; t < 4; t++) {
           v[t] = fmaxf(f[j + t] + s_bias[ch + j + t], 0.f);
+          if constexpr (RAG) v[t] = valid ? v[t] : 0.f;
           vmax = fmaxf(vmax, v[t]);
         }
 #pragma unroll
@@ -276,6 +283,10 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
           } else {
             f0 = fmaxf(f[q + j] + s_bias[c + j], 0.f);
             f1 = fmaxf(f[q + j + 1] + s_bias[c + j + 1], 0.f);
+            if constexpr (RAG) {
+              f0 = valid ? f0 : 0.f;
+              f1 = valid ? f1 : 0.f;
+            }
           }
           split_bf16x2(f0, f1, hi[j >> 1], lo[j >> 1]);
         }
@@ -308,7 +319,18 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
         for (int c = 0; c < 3; c++)
           v[c] = __fadd_rn(__fadd_rn(__fmul_rn(r[c], c0), __fmul_rn(r[3 + c], c1)), __fmul_rn(r[6 + c], c2));
         size_t oo = o, ohw = hw, o8 = ((size_t)n * hw + pix) * 3;
-        if (g.tiled) {  // window pixel -> image pixel; the halo around the kept rectangle is not stored
+        float* out_f32 = g.out_f32;
+        uint8_t* out_u8 = g.out_u8;
+        if constexpr (RAG) {  // slot pixel -> pixel of the window's own image; only the kept rectangle is stored
+          const RaggedWindow& t = g.rwin[n];
+          const int y = t.ys + gy, x = t.xs + gx;
+          if (y < t.ky0 || y >= t.ky1 || x < t.kx0 || x >= t.kx1) return;
+          ohw = (size_t)t.H * t.W;
+          oo = (size_t)y * t.W + x;
+          o8 = oo * 3;
+          out_f32 = t.out_f32;
+          out_u8 = t.out_u8;
+        } else if (g.tiled) {  // window pixel -> image pixel; the halo around the kept rectangle is not stored
           const TileWindow t = tile_window(g.tiles, g.win0 + n);
           const int y = t.ys + gy, x = t.xs + gx;
           if (y < t.ky0 || y >= t.ky1 || x < t.kx0 || x >= t.kx1) return;
@@ -317,12 +339,12 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
           oo = (size_t)t.img * 3 * ohw + ipix;
           o8 = ((size_t)t.img * ohw + ipix) * 3;
         }
-        if (g.out_f32) {
+        if (out_f32) {
 #pragma unroll
-          for (int c = 0; c < 3; c++) g.out_f32[oo + c * ohw] = v[c];
+          for (int c = 0; c < 3; c++) out_f32[oo + c * ohw] = v[c];
         }
-        if (g.out_u8) {  // ten2arr (hubconf.py:24-34): clip to [0,1], *255, truncate; NHWC
-          uint8_t* q = g.out_u8 + o8;
+        if (out_u8) {  // ten2arr (hubconf.py:24-34): clip to [0,1], *255, truncate; NHWC
+          uint8_t* q = out_u8 + o8;
 #pragma unroll
           for (int c = 0; c < 3; c++) q[c] = (uint8_t)(int)__fmul_rn(fminf(fmaxf(v[c], 0.0f), 1.0f), 255.0f);
         }
@@ -331,12 +353,14 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
   }
 }
 
-template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT, int NBLK, int TPS, int FMT = 0>
+// RAG: a pass of a ragged batch (ConvArgs::rwin)
+template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT, int NBLK, int TPS, int FMT = 0, bool RAG = false>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) {
   using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT>;
   constexpr bool F8IN = C::F8IN, DUAL = C::DUAL, OUT8 = (FMT & kFmtOut8) != 0;
   static_assert(!OUT8 || EPI == kEpiAct, "fp8 planes are written by the activation epilogue only");
+  static_assert(!RAG || EPI == kEpiAct || EPI == kEpiGate, "ragged passes mask activations and store the gate");
   if (g.run_if != nullptr && *reinterpret_cast<const volatile int*>(g.run_if) == 0) return;  // whole grid alike
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -485,6 +509,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     const int m = wg * 64 + r;
     const int gx = tx * kTileW + (m & 7), gy = ty * kTileH + (m >> 3);
     const bool inside = gx < g.W && gy < g.H;
+    bool valid = true;
+    if constexpr (RAG) valid = gx < g.rwin[n].vw && gy < g.rwin[n].vh;
     constexpr int NCH = NBLK * NPAD;
 #pragma unroll
     for (int ch0 = 0; ch0 < NCH; ch0 += 32) {
@@ -515,7 +541,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
           const float4 x = s[q];
           f[4 * q] = x.x; f[4 * q + 1] = x.y; f[4 * q + 2] = x.z; f[4 * q + 3] = x.w;
         }
-        epilogue16<EPI, OUT8>(g, s_bias, f, cb, n, gx, gy);
+        epilogue16<EPI, OUT8, RAG>(g, s_bias, f, cb, n, gx, gy, valid);
       }
       wg_bar(1 + wg);
     }
@@ -676,7 +702,8 @@ static int make_tmap(CUtensorMap* tm, void* base, int planes_total, int N, int H
 }
 
 // Launch one convolution.  `slot` is the timing slot (common.cuh).  One persistent CTA per SM (shared-memory footprint).
-template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0>
+template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0,
+          bool RAG = false>
 static int launch_conv(wn_handle* h, int slot, const uint8_t* wpk, const float* bias, void* in_base, ConvArgs a,
                        cudaStream_t stream) {
   using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT>;
@@ -691,7 +718,7 @@ static int launch_conv(wn_handle* h, int slot, const uint8_t* wpk, const float* 
   a.tiles_x = (a.W + kTileW - 1) / kTileW;
   a.tiles_y = (a.H + kTileH - 1) / kTileH;
   const long long tiles = (long long)a.tiles_x * a.tiles_y * a.N;
-  auto kern = conv_umma_kernel<KS, CIN_PAD, NPAD, EPI, CONCAT, NBLK, TPS, FMT>;
+  auto kern = conv_umma_kernel<KS, CIN_PAD, NPAD, EPI, CONCAT, NBLK, TPS, FMT, RAG>;
   WN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
   TimedScope ts(h, slot, stream);
   const int grid = (int)(tiles < h->sm_count ? tiles : h->sm_count);

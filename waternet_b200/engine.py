@@ -71,6 +71,40 @@ def tile_geometry(h: int, w: int, tile_h: int, tile_w: int) -> dict:
             "windows": [(ys[i], xs[j], rows[i], cols[j]) for i in range(ny) for j in range(nx)]}
 
 
+DEFAULT_PASS_PIXELS = 8 << 20  # max_pass_pixels = 0
+RAGGED_WINDOW_BYTES = 72       # csrc/tiling.cuh RaggedWindow: one descriptor per window
+RAGGED_IMAGE_BYTES = 40        # csrc/common.cuh RaggedImage: one per image
+
+
+def ragged_plan(sizes, tile_h: int, tile_w: int, max_pass_pixels: int = 0) -> list:
+    """The pass plan of wn_enhance_u8_ragged (csrc/tiling.cuh ragged_plan) restated for callers that plan or check
+    a ragged call.  ``sizes``: [(h, w), ...].  Returns the passes in order, each a dict with ``slot`` (h, w) and
+    ``windows``: dicts with the image index ``img``, origin ``ys``, ``xs``, valid extent ``vh``, ``vw`` and kept
+    ``rows`` (ky0, ky1) and ``cols`` (kx0, kx1)."""
+    limit = max_pass_pixels or DEFAULT_PASS_PIXELS
+    wins = []
+    for i, (h, w) in enumerate(sizes):
+        g = tile_geometry(h, w, tile_h, tile_w)
+        wins += [{"img": i, "ys": ys, "xs": xs, "vh": g["win_h"], "vw": g["win_w"], "rows": rows, "cols": cols}
+                 for ys, xs, rows, cols in g["windows"]]
+    wins.sort(key=lambda r: (-r["vh"], -r["vw"]))  # stable: image and window order within a shape
+    passes, cur, valid = [], None, 0
+    for r in wins:
+        if cur is not None:
+            cnt = len(cur["windows"]) + 1
+            sh, sw = max(cur["slot"][0], r["vh"]), max(cur["slot"][1], r["vw"])
+            v = valid + r["vh"] * r["vw"]
+            if cnt <= 65535 and cnt * sh * sw <= limit and 4 * (cnt * sh * sw - v) <= cnt * sh * sw:
+                cur["windows"].append(r)
+                cur["slot"], valid = (sh, sw), v
+                continue
+            passes.append(cur)
+        cur, valid = {"slot": (r["vh"], r["vw"]), "windows": [r]}, r["vh"] * r["vw"]
+    if cur is not None:
+        passes.append(cur)
+    return passes
+
+
 def _stream_ptr(device: torch.device) -> ctypes.c_void_p:
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -448,3 +482,52 @@ class Engine:
                                               _stream_ptr(self.device))
         _lib.check(rc, "wn_enhance_u8_tiled")
         return out_u8
+
+    def ragged_workspace_bytes(self, sizes, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
+                               max_pass_pixels: int = 0) -> int:
+        """Workspace of one ``enhance_ragged`` call over images of ``sizes`` [(h, w), ...]
+        (wn_enhance_ragged_workspace_bytes); 0 for rejected arguments."""
+        th, tw = self._tile_hw(tile)
+        n = len(sizes)
+        hs = (ctypes.c_int * max(1, n))(*[int(h) for h, _ in sizes])
+        ws = (ctypes.c_int * max(1, n))(*[int(w) for _, w in sizes])
+        return int(self.lib.wn_enhance_ragged_workspace_bytes(hs, ws, n, th, tw, int(max_pass_pixels), mode))
+
+    def enhance_ragged(self, images: Sequence[torch.Tensor], tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
+                       out_u8: Optional[Sequence[torch.Tensor]] = None,
+                       out_f32: Optional[Sequence[Optional[torch.Tensor]]] = None,
+                       max_pass_pixels: int = 0) -> list:
+        """``enhance`` of n uint8 (H_i,W_i,3) CUDA images of their own sizes in one call (wn_enhance_u8_ragged).
+        Each image's outputs equal, bit for bit, ``enhance`` of that image alone (while the e4m3 range guard stays
+        down).  ``tile`` and ``max_pass_pixels`` as in ``enhance_tiled``.  ``out_u8`` / ``out_f32``: optional lists of
+        per-image outputs, uint8 (H_i,W_i,3) and float32 (1,3,H_i,W_i); an ``out_f32`` entry may be None.  Returns the
+        list of uint8 outputs.  Tensor-core modes only."""
+        th, tw = self._tile_hw(tile)
+        n = len(images)
+        if out_u8 is not None and len(out_u8) != n or out_f32 is not None and len(out_f32) != n:
+            raise ValueError(f"out_u8 / out_f32 must hold one entry per image ({n})")
+        srcs, outs = [], []
+        for i, img in enumerate(images):
+            if img.dim() != 3:
+                raise ValueError(f"image {i}: expected uint8 (H,W,3), got {img.dtype} {tuple(img.shape)}")
+            src, dst = self._enhance_args(img[None], None if out_u8 is None else out_u8[i][None],
+                                          None if out_f32 is None else out_f32[i])
+            srcs.append(src[0])
+            outs.append(dst[0] if out_u8 is None else out_u8[i])
+        entries = []
+        for i, (src, dst) in enumerate(zip(srcs, outs)):
+            if src.numel() == 0:  # zero-pixel images: empty outputs, no library call
+                continue
+            f32 = None if out_f32 is None else out_f32[i]
+            entries.append(_lib.RaggedImage(src.data_ptr(), dst.data_ptr(), None if f32 is None else f32.data_ptr(),
+                                            src.shape[0], src.shape[1]))
+        if not entries:
+            return outs
+        nbytes = self.ragged_workspace_bytes([(e.height, e.width) for e in entries], (th, tw), mode, max_pass_pixels)
+        ws = self._workspace("enhance", nbytes)
+        table = (_lib.RaggedImage * len(entries))(*entries)
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_enhance_u8_ragged(self.handle, table, len(entries), th, tw, int(max_pass_pixels), mode,
+                                               ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
+        _lib.check(rc, "wn_enhance_u8_ragged")
+        return outs
