@@ -14,6 +14,8 @@
  *   wn_forward            waternet/net.py:99-108   WaterNet.forward(x, wb, ce, gc)
  *   wn_confidence_maps    waternet/net.py:45-56    ConfidenceMapGenerator.forward(x, wb, ce, gc)
  *   wn_refine             waternet/net.py:75-80    Refiner.forward(x, xbar)
+ *   wn_forward_tiled,     the same three, computed in overlapping windows: bounded workspace for images of any size
+ *   wn_confidence_maps_tiled, wn_refine_tiled
  *   wn_resize_u8          waternet/training_utils.py:94-107  cv2.resize + BGR2RGB of the dataset items
  *   wn_postprocess_u8     hubconf.py:24-34         ten2arr_noeinops (clip, *255, truncate, NCHW->NHWC)
  *   wn_enhance_u8         hubconf.py:85-94 + net.py:99-108: preprocess -> model -> postprocess
@@ -40,7 +42,7 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 6
+#define WN_ABI_VERSION 7
 
 #define WN_OK 0
 #define WN_E_INVALID (-1)   /* bad argument (NULL pointer, non-positive size, unknown mode) */
@@ -139,6 +141,37 @@ int wn_confidence_maps(wn_handle* h, const float* x, const float* wb, const floa
 int wn_refine(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
               float* out, int n, int height, int width, int mode, void* workspace, size_t workspace_bytes,
               void* stream);
+
+/*
+ * wn_forward, wn_confidence_maps and wn_refine with a workspace that does not grow with the image: the same bits,
+ * computed in windows.  The untiled calls run whole images per pass (~1.9 KB of workspace per pixel, so one 45 MP
+ * photo needs more than an 80 GB card).  Each image is cut into the windows of wn_enhance_u8_tiled (balanced output
+ * tiles of at most tile_h x tile_w, each computed from a window up to 13 pixels larger per side, clamped into the
+ * image); a pass runs as many windows as fit in max_pass_pixels (0 = 8 Mi pixels; at least one window).  The first
+ * layer drops its a_lo pass when every input value of the call is an 8-bit level (u/255), as wn_forward does for a
+ * batch it runs in one pass; the results then equal those of the untiled calls bit for bit.  Inputs and strides as
+ * wn_forward / wn_refine; the outputs are fp32 contiguous NCHW (N,3,H,W).
+ * Workspace: wn_forward_tiled_workspace_bytes for wn_forward_tiled, wn_submodule_tiled_workspace_bytes for the two
+ * sub-modules (one pass of windows, ~1.9 KB per window pixel, plus 36 B per window pixel for the sub-modules),
+ * whatever the image size.  Tensor-core modes only (WN_MODE_FP32_SIMT: WN_E_UNSUPPORTED); the size limits of
+ * wn_enhance_u8_tiled.  max_pass_pixels is this call's own argument (wn_set_chunk_pixels does not apply).  Nothing
+ * is copied from the host, so a call can be captured in a CUDA graph.  The workspace functions return 0 for
+ * arguments the calls reject.
+ */
+size_t wn_forward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
+                                        int mode);
+int wn_forward_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                     const int64_t in_strides[4][4], float* out, int n, int height, int width, int tile_h, int tile_w,
+                     long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream);
+size_t wn_submodule_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
+                                          int mode);
+int wn_confidence_maps_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                             const int64_t in_strides[4][4], float* out_maps, int n, int height, int width, int tile_h,
+                             int tile_w, long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes,
+                             void* stream);
+int wn_refine_tiled(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
+                    float* out, int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels,
+                    int mode, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * preprocess -> forward -> postprocess without leaving the device.  In the tensor-core modes nothing fp32 is

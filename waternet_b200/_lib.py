@@ -19,7 +19,7 @@ MODE_BF16_FP8 = 2
 MODE_DEFAULT = -1
 NUM_PARAMS = 34
 NUM_TIMING_SLOTS = 23
-ABI_VERSION = 6
+ABI_VERSION = 7
 PEER_HANDLE_BYTES = 64  # WN_PEER_HANDLE_BYTES
 MAX_PEERS = 15          # WN_MAX_PEERS
 
@@ -67,6 +67,16 @@ _SIGNATURES = {
                                    c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "wn_refine": (c_int, [c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int64), c_void_p, c_int, c_int, c_int,
                           c_int, c_void_p, c_size_t, c_void_p]),
+    "wn_forward_tiled_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong, c_int]),
+    "wn_forward_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p,
+                                 c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong, c_int, c_void_p, c_size_t,
+                                 c_void_p]),
+    "wn_submodule_tiled_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong, c_int]),
+    "wn_confidence_maps_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64),
+                                         c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong, c_int,
+                                         c_void_p, c_size_t, c_void_p]),
+    "wn_refine_tiled": (c_int, [c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int64), c_void_p, c_int, c_int, c_int,
+                                c_int, c_int, ctypes.c_longlong, c_int, c_void_p, c_size_t, c_void_p]),
     "wn_forward_chunk_images": (c_int, [c_void_p, c_int, c_int, c_int]),
     "wn_set_chunk_pixels": (c_int, [c_void_p, ctypes.c_longlong]),
     "wn_f8_overflowed": (c_int, [c_void_p]),

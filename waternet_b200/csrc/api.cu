@@ -514,6 +514,105 @@ int wn_refine(wn_handle* h, int which, const float* x, const float* xbar, const 
   return WN_OK;
 }
 
+// ---- the tiled forward of fp32 tensors (WaterNet.forward and its sub-modules, in windows)
+// the argument checks the tiled forward calls and their workspace functions share (pointers aside)
+static int forward_tiled_check(const char* what, int n, int height, int width, int tile_h, int tile_w,
+                               long long max_pass_pixels, int mode) {
+  if (n <= 0 || height <= 0 || width <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
+    set_error("%s: bad shape n=%d h=%d w=%d tile=%dx%d max_pass_pixels=%lld", what, n, height, width, tile_h, tile_w,
+              max_pass_pixels);
+    return WN_E_INVALID;
+  }
+  const int m = resolve_mode(mode);
+  if (m == WN_MODE_FP32_SIMT) {
+    set_error("%s: the tiled forward runs in the tensor-core modes only, not WN_MODE_FP32_SIMT", what);
+    return WN_E_UNSUPPORTED;
+  }
+  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) {
+    set_error("%s: unknown mode %d", what, mode);
+    return WN_E_INVALID;
+  }
+  if ((size_t)height * width > (size_t)0x7fffffff / 3 || n > 65535) {
+    set_error("image too large: n=%d h=%d w=%d", n, height, width);
+    return WN_E_UNSUPPORTED;
+  }
+  return WN_OK;
+}
+
+size_t wn_forward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
+                                        int mode) {
+  if (forward_tiled_check("wn_forward_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels, mode)) return 0;
+  return umma_forward_tiled_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels, false);
+}
+
+size_t wn_submodule_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
+                                          int mode) {
+  if (forward_tiled_check("wn_submodule_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels, mode))
+    return 0;
+  return umma_forward_tiled_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels, true);
+}
+
+// the checks and the call shared by the three entry points; `what` names the entry point
+static int forward_tiled(const char* what, wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out,
+                         int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels, int mode,
+                         void* workspace, size_t workspace_bytes, void* stream, int stack, int which) {
+  int rc = forward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels, mode);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  return umma_forward_tiled(h, in, st, out, n, height, width, tile_h, tile_w, max_pass_pixels, workspace,
+                            workspace_bytes, (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0,
+                            stack, which);
+}
+
+int wn_forward_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                     const int64_t in_strides[4][4], float* out, int n, int height, int width, int tile_h, int tile_w,
+                     long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h || !x || !wb || !he || !gc || !in_strides || !out || !workspace) {
+    set_error("wn_forward_tiled: null argument");
+    return WN_E_INVALID;
+  }
+  const float* in[4] = {x, wb, he, gc};
+  return forward_tiled("wn_forward_tiled", h, in, in_strides, out, n, height, width, tile_h, tile_w, max_pass_pixels,
+                       mode, workspace, workspace_bytes, stream, kStackAll, 0);
+}
+
+int wn_confidence_maps_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                             const int64_t in_strides[4][4], float* out_maps, int n, int height, int width, int tile_h,
+                             int tile_w, long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes,
+                             void* stream) {
+  if (!h || !x || !wb || !he || !gc || !in_strides || !out_maps || !workspace) {
+    set_error("wn_confidence_maps_tiled: null argument");
+    return WN_E_INVALID;
+  }
+  const float* in[4] = {x, wb, he, gc};
+  return forward_tiled("wn_confidence_maps_tiled", h, in, in_strides, out_maps, n, height, width, tile_h, tile_w,
+                       max_pass_pixels, mode, workspace, workspace_bytes, stream, kStackCmg, 0);
+}
+
+int wn_refine_tiled(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
+                    float* out, int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels,
+                    int mode, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h || !x || !xbar || !in_strides || !out || !workspace) {
+    set_error("wn_refine_tiled: null argument");
+    return WN_E_INVALID;
+  }
+  if (which < 0 || which > 2) {
+    set_error("wn_refine_tiled: which must be 0, 1 or 2, got %d", which);
+    return WN_E_INVALID;
+  }
+  // as wn_refine: refiner r sees cat[x, input r+1], so xbar goes to every slot
+  const float* in[4] = {x, xbar, xbar, xbar};
+  int64_t st[4][4];
+  for (int t = 0; t < 4; t++)
+    for (int k = 0; k < 4; k++) st[t][k] = in_strides[t == 0 ? 0 : 1][k];
+  return forward_tiled("wn_refine_tiled", h, in, st, out, n, height, width, tile_h, tile_w, max_pass_pixels, mode,
+                       workspace, workspace_bytes, stream, kStackRefiners, which);
+}
+
 int wn_set_chunk_pixels(wn_handle* h, long long max_pixels) {
   if (!h || max_pixels < 0) {
     set_error("wn_set_chunk_pixels: bad argument");

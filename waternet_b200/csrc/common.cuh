@@ -219,6 +219,13 @@ int umma_chunk_images(const wn_handle* h, int n, int height, int width);
 int umma_forward(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], float* out,
                  int n, int height, int width, void* workspace, size_t workspace_bytes,
                  cudaStream_t stream, int scheme = 0, int stack = kStackAll, float* refined = nullptr);
+// the tiled forward of fp32 tensors (arguments checked by the caller, api.cu).  stack as umma_forward; the
+// sub-modules write `out` directly (kStackRefiners: refiner `which`) and need the `submodule` workspace
+size_t umma_forward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
+                                          bool submodule);
+int umma_forward_tiled(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], float* out, int n,
+                       int height, int width, int tile_h, int tile_w, long long max_pass_pixels, void* workspace,
+                       size_t workspace_bytes, cudaStream_t stream, int scheme, int stack = kStackAll, int which = 0);
 size_t umma_enhance_workspace_bytes(int n, int h, int w);
 int mirror_u8(wn_handle* h, const uint8_t* src, const PeerOut& peers, size_t bytes, const int* run_if, cudaStream_t stream);
 int umma_enhance_u8(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* out_f32, int n, int height,

@@ -35,14 +35,29 @@ struct PackInArgs {
   const float* p[4];
   long long s[4][4];
 };
+// FORM kPackImages: pixel blockIdx.x * 256 + tid of image blockIdx.y -> act0 planes, and the flag.
+// kPackWindows (tiled forward): pixel of window win0 + blockIdx.y of `tiles`, read at image coordinates -> that
+// window's act0 planes (blockIdx.y of the pass); the flag is not touched.
+// kPackFlag: the flag alone, over every pixel of every image (same grid as kPackImages), nothing is written.
+enum PackForm { kPackImages = 0, kPackWindows = 1, kPackFlag = 2 };
+template <int FORM = kPackImages>
 __global__ void __launch_bounds__(256) pack_inputs_kernel(PackInArgs a, uint4* __restrict__ out, int H, int W,
-                                                          int* __restrict__ exact_flag) {
-  const int n = blockIdx.y;
+                                                          int* __restrict__ exact_flag, TileGeom tiles, long long win0) {
   const int pix = blockIdx.x * 256 + threadIdx.x;
-  const int hw = H * W;
+  const int hw = FORM == kPackWindows ? tiles.win_h * tiles.win_w : H * W;
   bool exact = true;
   if (pix < hw) {
-    const int y = pix / W, x = pix - y * W;
+    int n = blockIdx.y, y, x;
+    if constexpr (FORM == kPackWindows) {
+      const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
+      const int wy = pix / tiles.win_w;
+      n = t.img;
+      y = t.ys + wy;
+      x = t.xs + (pix - wy * tiles.win_w);
+    } else {
+      y = pix / W;
+      x = pix - y * W;
+    }
     float v[16];
 #pragma unroll
     for (int t = 0; t < 4; t++)
@@ -54,19 +69,40 @@ __global__ void __launch_bounds__(256) pack_inputs_kernel(PackInArgs a, uint4* _
         if (fabsf(f - r) <= 6.103515625e-5f && r >= 0.f && r <= 255.f) f = r; else exact = false;
         v[t * 3 + c] = f;
       }
-    v[12] = v[13] = v[14] = v[15] = 0.f;
-    uint32_t hi[8], lo[8];
+    if constexpr (FORM != kPackFlag) {
+      v[12] = v[13] = v[14] = v[15] = 0.f;
+      uint32_t hi[8], lo[8];
 #pragma unroll
-    for (int j = 0; j < 16; j += 2) {
-      split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
+      for (int j = 0; j < 16; j += 2) {
+        split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
+      }
+      uint4* o = out + (size_t)blockIdx.y * 4 * hw + pix;  // planes: hi0, hi1, lo0, lo1
+      o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+      o[hw] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+      o[2 * (size_t)hw] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+      o[3 * (size_t)hw] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
     }
-    uint4* o = out + (size_t)n * 4 * hw + pix;  // planes: hi0, hi1, lo0, lo1
-    o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    o[hw] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-    o[2 * (size_t)hw] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-    o[3 * (size_t)hw] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
   }
-  if (!__syncthreads_and(exact) && threadIdx.x == 0) atomicExch(exact_flag, 0);
+  if constexpr (FORM != kPackWindows)
+    if (!__syncthreads_and(exact) && threadIdx.x == 0) atomicExch(exact_flag, 0);
+}
+
+// Sub-modules of the tiled forward: window blockIdx.y of the pass (window win0 + blockIdx.y of `tiles`) holds `cs`
+// fp32 planes of win_h x win_w; channels [c0, c0 + c) of its kept rectangle are stored into dst, contiguous NCHW
+// (N, c, H, W), at image coordinates.
+__global__ void __launch_bounds__(256) store_kept_kernel(const float* __restrict__ src, int cs, int c0, int c,
+                                                         float* __restrict__ dst, TileGeom tiles, long long win0) {
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  const int hw = tiles.win_h * tiles.win_w;
+  if (pix >= hw) return;
+  const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
+  const int wy = pix / tiles.win_w;
+  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
+  if (y < t.ky0 || y >= t.ky1 || x < t.kx0 || x >= t.kx1) return;
+  const size_t ihw = (size_t)tiles.H * tiles.W;
+  const float* s = src + ((size_t)blockIdx.y * cs + c0) * hw + pix;
+  float* d = dst + (size_t)t.img * c * ihw + (size_t)y * tiles.W + x;
+  for (int k = 0; k < c; k++) d[k * ihw] = s[(size_t)k * hw];
 }
 
 // ------------------------------------------------------------------------------------------
@@ -301,6 +337,15 @@ __global__ void decode_planes_kernel(const uint4* __restrict__ src, float* __res
   }
 }
 
+static PackInArgs pack_args(const float* const in[4], const int64_t st[4][4]) {
+  PackInArgs pa;
+  for (int t = 0; t < 4; t++) {
+    pa.p[t] = in[t];
+    for (int k = 0; k < 4; k++) pa.s[t][k] = st[t][k];
+  }
+  return pa;
+}
+
 // Where every layer's output lives.  Inference ping-pongs two buffers per stack; the training
 // forward (conv_bwd.cu) gives every activation its own buffer because the backward pass needs them.
 int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out, int n, int H,
@@ -308,14 +353,11 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   const int dbg_layer = o.dbg_layer;
   float* const dbg_dst = o.dbg_dst;
   if (!o.packed) {
-    PackInArgs pa;
-    for (int t = 0; t < 4; t++) {
-      pa.p[t] = in[t];
-      for (int k = 0; k < 4; k++) pa.s[t][k] = st[t][k];
-    }
+    const PackInArgs pa = pack_args(in, st);
     TimedScope ts(h, kSlotPack, stream);
     WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
-    pack_inputs_kernel<<<dim3((H * W + 255) / 256, n), 256, 0, stream>>>(pa, b.act0, H, W, b.exact_flag);
+    pack_inputs_kernel<kPackImages><<<dim3((H * W + 255) / 256, n), 256, 0, stream>>>(pa, b.act0, H, W, b.exact_flag,
+                                                                                       TileGeom(), 0);
     WN_LAUNCH_CHECK(h);
   }
   ConvArgs a;
@@ -691,6 +733,87 @@ int umma_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images, int n, i
     o.rwin = d_wins + p.first;
     rc = umma_pass(h, no_in, none, nullptr, p.count, p.slot_h, p.slot_w, b, stream, o);
     if (rc) return rc;
+  }
+  return mirror_overflow(h, scheme, stream);
+}
+
+// The tiled form of umma_forward (fp32 tensors in): the windows of tiling.cuh, one pass of them at a time through
+// the same ten launches and range guard.  The windowed packing kernel reads each window's operands at image
+// coordinates through the caller's strides.  Whether the first layer drops its a_lo pass is decided once for the
+// whole call, over every input pixel of the n images (kPackFlag), so it takes the path wn_forward takes when that
+// runs the batch in one pass.  The flag sits at the start of the workspace, outside the per-pass carve-up (whose
+// layout moves with the window count), and stays valid for the bf16x3 re-run of every pass.  kStackAll: the gate
+// epilogue stores each kept rectangle into `out`.  The sub-modules keep their result (the maps, or the three refined
+// images) in window layout and store_kept_kernel copies the kept rectangle of the wanted planes into `out`.
+// Workspace: [flag | refined images of one pass (sub-modules) | one pass], independent of the image size.  Nothing
+// is copied from the host: the call can be captured in a graph.
+size_t umma_forward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
+                                          bool submodule) {
+  const TileGeom g = tile_geom(h, w, tile_h, tile_w);
+  const size_t px = (size_t)tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels) *
+                    g.win_h * g.win_w;
+  return px * kUmmaBytesPerPixel + 4096 + 256 + (submodule ? align256(px * 9 * sizeof(float)) + 256 : 0);
+}
+
+int umma_forward_tiled(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], float* out, int n,
+                       int H, int W, int tile_h, int tile_w, long long max_pass_pixels, void* workspace,
+                       size_t workspace_bytes, cudaStream_t stream, int scheme, int stack, int which) {
+  if (!h->umma) {
+    set_error("tensor-core weights have not been packed");
+    return WN_E_STATE;
+  }
+  const bool sub = stack != kStackAll;
+  const size_t need = umma_forward_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels, sub);
+  if (workspace_bytes < need) {
+    set_error("tiled forward workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  int rc = get_encoder();
+  if (rc) return rc;
+  scheme = effective_scheme(h, scheme);
+  const TileGeom g = tile_geom(H, W, tile_h, tile_w);
+  const long long total = (long long)n * g.ny * g.nx;
+  const long long per_pass = tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels);
+  const size_t win_px = (size_t)g.win_h * g.win_w;
+  uint8_t* base = (uint8_t*)align256((uintptr_t)workspace);
+  int* exact = (int*)base;
+  float* refined = (float*)(base + 256);
+  void* fwd_ws = base + 256 + (sub ? align256(per_pass * win_px * 9 * sizeof(float)) : 0);
+  const PackInArgs pa = pack_args(in, in_strides);
+  {
+    TimedScope ts(h, kSlotPack, stream);
+    WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
+    pack_inputs_kernel<kPackFlag><<<dim3((H * W + 255) / 256, n), 256, 0, stream>>>(pa, nullptr, H, W, exact, g, 0);
+    WN_LAUNCH_CHECK(h);
+  }
+  for (long long w0 = 0; w0 < total; w0 += per_pass) {
+    const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
+    FwdBuffers b = carve(fwd_ws, cur, g.win_h, g.win_w);
+    b.exact_flag = exact;
+    {
+      TimedScope ts(h, kSlotPack, stream);
+      pack_inputs_kernel<kPackWindows><<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(
+          pa, b.act0, H, W, exact, g, w0);
+      WN_LAUNCH_CHECK(h);
+    }
+    FwdOpts o;
+    o.scheme = scheme;
+    o.packed = true;
+    o.stack = stack;
+    if (stack == kStackRefiners) b.refined = refined;
+    if (!sub) {
+      o.tiles = &g;
+      o.win0 = w0;
+    }
+    rc = umma_pass(h, in, in_strides, sub ? nullptr : out, cur, g.win_h, g.win_w, b, stream, o);
+    if (rc) return rc;
+    if (sub) {  // after the pass and its conditional bf16x3 re-run
+      TimedScope ts(h, kSlotGate, stream);
+      const bool maps = stack == kStackCmg;
+      store_kept_kernel<<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(
+          maps ? b.cm : refined, maps ? 3 : 9, maps ? 0 : 3 * which, 3, out, g, w0);
+      WN_LAUNCH_CHECK(h);
+    }
   }
   return mirror_overflow(h, scheme, stream);
 }

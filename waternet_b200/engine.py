@@ -483,6 +483,82 @@ class Engine:
         _lib.check(rc, "wn_enhance_u8_tiled")
         return out_u8
 
+    # ---- the tiled forward of fp32 tensors (wn_forward_tiled, wn_confidence_maps_tiled, wn_refine_tiled) ----------
+    def forward_tiled_workspace_bytes(self, n: int, h: int, w: int, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
+                                      max_pass_pixels: int = 0) -> int:
+        """Workspace of one ``forward_tiled`` call (wn_forward_tiled_workspace_bytes); 0 for rejected arguments."""
+        th, tw = self._tile_hw(tile)
+        return int(self.lib.wn_forward_tiled_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels), mode))
+
+    def submodule_tiled_workspace_bytes(self, n: int, h: int, w: int, tile=DEFAULT_TILE,
+                                        mode: int = _lib.MODE_DEFAULT, max_pass_pixels: int = 0) -> int:
+        """Workspace of one ``confidence_maps_tiled`` / ``refine_tiled`` call (wn_submodule_tiled_workspace_bytes);
+        0 for rejected arguments."""
+        th, tw = self._tile_hw(tile)
+        return int(self.lib.wn_submodule_tiled_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels), mode))
+
+    def forward_tiled(self, x, wb, he, gc, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
+                      out: Optional[torch.Tensor] = None, max_pass_pixels: int = 0) -> torch.Tensor:
+        """``forward`` computed in overlapping windows (wn_forward_tiled): the same bits when every input value is an
+        8-bit level or the untiled call runs the batch in one pass, with a workspace that does not grow with the
+        image size.  ``tile`` and ``max_pass_pixels`` as in ``enhance_tiled``.  Tensor-core modes only."""
+        th, tw = self._tile_hw(tile)
+        ins = self._check_inputs((x, wb, he, gc))
+        n, _, h, w = ins[0].shape
+        if out is None:
+            out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
+        elif (out.dtype != torch.float32 or tuple(out.shape) != (n, 3, h, w) or not out.is_contiguous()
+              or out.device != self.device):
+            raise ValueError(f"out must be a contiguous float32 {(n, 3, h, w)} tensor on {self.device}")
+        if out.numel() == 0:
+            return out
+        strides = (ctypes.c_int64 * 16)(*[s for t in ins for s in t.stride()])
+        ws = self._workspace("forward", self.forward_tiled_workspace_bytes(n, h, w, (th, tw), mode, max_pass_pixels))
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_forward_tiled(self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(),
+                                           ins[3].data_ptr(), strides, out.data_ptr(), n, h, w, th, tw,
+                                           int(max_pass_pixels), mode, ws.data_ptr(), ws.numel(),
+                                           _stream_ptr(self.device))
+        _lib.check(rc, "wn_forward_tiled")
+        return out
+
+    def confidence_maps_tiled(self, x, wb, he, gc, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
+                              max_pass_pixels: int = 0) -> torch.Tensor:
+        """``confidence_maps`` computed in overlapping windows (wn_confidence_maps_tiled)."""
+        th, tw = self._tile_hw(tile)
+        ins = self._check_inputs((x, wb, he, gc))
+        n, _, h, w = ins[0].shape
+        out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
+        if out.numel() == 0:
+            return out
+        strides = (ctypes.c_int64 * 16)(*[s for t in ins for s in t.stride()])
+        ws = self._workspace("forward", self.submodule_tiled_workspace_bytes(n, h, w, (th, tw), mode, max_pass_pixels))
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_confidence_maps_tiled(self.handle, ins[0].data_ptr(), ins[1].data_ptr(),
+                                                   ins[2].data_ptr(), ins[3].data_ptr(), strides, out.data_ptr(), n,
+                                                   h, w, th, tw, int(max_pass_pixels), mode, ws.data_ptr(),
+                                                   ws.numel(), _stream_ptr(self.device))
+        _lib.check(rc, "wn_confidence_maps_tiled")
+        return out
+
+    def refine_tiled(self, which: int, x, xbar, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
+                     max_pass_pixels: int = 0) -> torch.Tensor:
+        """``refine`` computed in overlapping windows (wn_refine_tiled)."""
+        th, tw = self._tile_hw(tile)
+        ins = self._check_inputs((x, xbar))
+        n, _, h, w = ins[0].shape
+        out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
+        if out.numel() == 0:
+            return out
+        strides = (ctypes.c_int64 * 8)(*[s for t in ins for s in t.stride()])
+        ws = self._workspace("forward", self.submodule_tiled_workspace_bytes(n, h, w, (th, tw), mode, max_pass_pixels))
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_refine_tiled(self.handle, int(which), ins[0].data_ptr(), ins[1].data_ptr(), strides,
+                                          out.data_ptr(), n, h, w, th, tw, int(max_pass_pixels), mode, ws.data_ptr(),
+                                          ws.numel(), _stream_ptr(self.device))
+        _lib.check(rc, "wn_refine_tiled")
+        return out
+
     def ragged_workspace_bytes(self, sizes, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
                                max_pass_pixels: int = 0) -> int:
         """Workspace of one ``enhance_ragged`` call over images of ``sizes`` [(h, w), ...]

@@ -37,15 +37,16 @@ def ten2arr_noeinops(ten: torch.Tensor) -> np.ndarray:
     return eng.postprocess(ten.to(eng.device)).cpu().numpy()
 
 
-def waternet(pretrained: bool = True, device=None):
+def waternet(pretrained: bool = True, device=None, tile=None):
     """Returns ``(preprocess, postprocess, model)`` -- the order ``hubconf.py:96`` returns.
 
     ``preprocess(rgb_arr)``: HWC (or NHWC) uint8 array -> ``(rgb, wb, he, gc)`` fp32
     (N,3,H,W) tensors on the device (``hubconf.py:85-91``).  ``postprocess(out)``:
-    model output -> uint8 NHWC array (``hubconf.py:93-94``).
+    model output -> uint8 NHWC array (``hubconf.py:93-94``).  ``tile`` sets ``model.tile``
+    (e.g. 998): the model then runs in overlapping windows, so that images of any size fit.
     """
     eng = get_engine(device)
-    model = WaterNet()
+    model = WaterNet(tile=tile)
     if pretrained is True:
         ckpt = torch.hub.load_state_dict_from_url(DEFAULT_CKPT_URL, progress=False, check_hash=True)
         model.load_state_dict(ckpt)

@@ -25,7 +25,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib
-from .engine import new_engine
+from .engine import Engine, new_engine
 
 MODES = {"default": _lib.MODE_DEFAULT, "fp32": _lib.MODE_FP32_SIMT, "bf16x3": _lib.MODE_BF16X3,
          "bf16_fp8": _lib.MODE_BF16_FP8}
@@ -35,6 +35,16 @@ MODES = {"default": _lib.MODE_DEFAULT, "fp32": _lib.MODE_FP32_SIMT, "bf16x3": _l
 # Kept outside the module so that copy.deepcopy / pickling of a model never touches a C handle.
 _model_engines = weakref.WeakKeyDictionary()
 _model_engines_lock = threading.Lock()
+
+
+def _checked_tile(tile, mode: int):
+    """``tile`` as (h, w), or None for whole images per pass.  The tiled forward runs on the tensor cores only."""
+    if tile is None:
+        return None
+    if mode == _lib.MODE_FP32_SIMT:
+        raise ValueError("tile: the tiled forward runs on the tensor cores only, and precision='fp32' is the CUDA-core "
+                         "mode; use precision='default' or 'bf16x3', or tile=None")
+    return Engine._tile_hw(tile)
 
 
 def _param_version(p) -> int:
@@ -103,11 +113,13 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
     ``WaterNet`` it runs with the parent's packed state dict (``wn_confidence_maps`` / ``wn_refine``); a
     free-standing instance packs its own tensors into the state-dict slots of its kind, zeros elsewhere.
     Sub-module calls are inference entry points: with autograd recording they evaluate the torch graph instead
-    (the fused training path is ``WaterNet.forward``).
+    (the fused training path is ``WaterNet.forward``).  Bound to a ``WaterNet`` a stack follows the parent's
+    ``precision`` and ``tile``; a free-standing one uses its own attributes.
     """
 
     spec: List[tuple] = []
     precision = "default"
+    tile = None
 
     def __init__(self):
         super().__init__()
@@ -144,15 +156,18 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
             self.__dict__["_parent_ref"] = ref
 
     def _mode_and_engine(self, x, zero_layout):
-        """(mode, engine with the right state dict packed, slot).  zero_layout(own) -> the 34-tensor list of a
-        free-standing stack."""
+        """(mode, engine with the right state dict packed, slot, tile or None).  zero_layout(own) -> the 34-tensor
+        list of a free-standing stack."""
         parent = self._parent_ref() if self._parent_ref is not None else None
         if parent is not None:
-            return parent._mode(), parent._engine_with_weights(x), self._slot
+            mode = parent._mode()
+            return mode, parent._engine_with_weights(x), self._slot, _checked_tile(parent.tile, mode)
         if self.precision not in MODES:
             raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(MODES)}")
+        mode = MODES[self.precision]
+        tile = _checked_tile(self.tile, mode)
         own = self._own_params()
-        return MODES[self.precision], self._engine_for(x, zero_layout(own)), 0
+        return mode, self._engine_for(x, zero_layout(own)), 0, tile
 
     @staticmethod
     def _needs_graph(tensors, params):
@@ -184,9 +199,12 @@ class ConfidenceMapGenerator(_ConvStack):
         if self._needs_graph((x, wb, ce, gc), self._own_params()):
             maps = self._graph(x, wb, ce, gc)
         else:
-            mode, eng, _ = self._mode_and_engine(
+            mode, eng, _, tile = self._mode_and_engine(
                 x, lambda own: own + 3 * _zeros_like_spec(REFINER_SPEC, own[0]))
-            maps = eng.confidence_maps(x, wb, ce, gc, mode)
+            if tile is None:
+                maps = eng.confidence_maps(x, wb, ce, gc, mode)
+            else:
+                maps = eng.confidence_maps_tiled(x, wb, ce, gc, tile, mode)
         return torch.split(maps, [1, 1, 1], dim=1)
 
 
@@ -204,9 +222,11 @@ class Refiner(_ConvStack):
     def forward(self, x, xbar):
         if self._needs_graph((x, xbar), self._own_params()):
             return self._graph(x, xbar)
-        mode, eng, slot = self._mode_and_engine(
+        mode, eng, slot, tile = self._mode_and_engine(
             x, lambda own: _zeros_like_spec(CMG_SPEC, own[0]) + own + 2 * _zeros_like_spec(REFINER_SPEC, own[0]))
-        return eng.refine(slot, x, xbar, mode)
+        if tile is None:
+            return eng.refine(slot, x, xbar, mode)
+        return eng.refine_tiled(slot, x, xbar, tile, mode)
 
 
 class _KernelForward(torch.autograd.Function):
@@ -267,15 +287,26 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
     the two correction terms of the heavy layers as one fp8 MMA; ~4e-4 of the fp32 result, inside the 1e-3
     parity bar), ``"bf16x3"`` (all three terms in bf16, ~3e-5; what training always uses),
     ``"fp32"`` (CUDA-core fp32 FMA).
+
+    ``tile``: None (whole images per pass, ~1.9 KB of workspace per pixel) or the largest output tile, an int or
+    (h, w), e.g. 998.  When set, inference calls of the model and of its ``cmg`` and refiners run in overlapping
+    windows (``wn_forward_tiled``): the same bits as untiled, with a workspace that does not grow with the image
+    size (~15 GB at tile 998 for a 45 MP photo, which does not fit on an 80 GB card untiled).  Tensor-core
+    precisions only.  A call that records an autograd graph (training) ignores ``tile`` and runs as without it.
     """
 
-    def __init__(self, precision: str = "default"):
+    tile = None  # models pickled before the attribute existed
+
+    def __init__(self, precision: str = "default", tile=None):
         super().__init__()
         self.cmg = ConfidenceMapGenerator()
         self.wb_refiner = Refiner()
         self.ce_refiner = Refiner()
         self.gc_refiner = Refiner()
         self.precision = precision
+        self.tile = tile
+        if tile is not None:
+            _checked_tile(tile, self._mode())
         self._bind_children()
 
     def _bind_children(self) -> None:
@@ -343,6 +374,9 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
             return self._engine_with_weights(x).forward(x, wb, ce, gc, mode)
         needs_graph = torch.is_grad_enabled() and (
             any(t.requires_grad for t in (x, wb, ce, gc)) or any(p.requires_grad for p in self.parameters()))
-        if needs_graph:
+        if needs_graph:  # tile does not apply: training keeps every activation of whole images
             return _KernelForward.apply(self, mode, x, wb, ce, gc, *self.parameters())
+        tile = _checked_tile(self.tile, mode)
+        if tile is not None:
+            return self._engine_with_weights(x).forward_tiled(x, wb, ce, gc, tile, mode)
         return self._kernel_forward(x, wb, ce, gc, mode)
