@@ -252,7 +252,8 @@ int wn_enhance_u8_peers(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, flo
  * and OVERWRITES the 34 gradient tensors `grads` (device pointers, same order, shapes and layout as
  * `params` of wn_pack_weights).  input_grads is NULL or four device pointers to fp32 contiguous
  * (N,3,H,W) tensors that receive d(loss)/d(x), d/d(wb), d/d(he), d/d(gc).
- * The workspace must stay untouched between the two calls; n*h*w <= 8 Mi pixels per call.
+ * The workspace must stay untouched between the two calls; n*h*w <= 8 Mi pixels and n <= 65535 images per call
+ * (wn_train_workspace_bytes returns 0 beyond that).
  */
 size_t wn_train_workspace_bytes(int n, int h, int w);
 int wn_forward_train(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,

@@ -63,6 +63,9 @@ def test_null_arguments_are_rejected_without_a_gpu(lib):
     assert lib.wn_preprocess_workspace_bytes(2, 112, 112) > 0
     assert lib.wn_submodule_workspace_bytes(2, 112, 112, -1) > lib.wn_forward_workspace_bytes(2, 112, 112, -1)
     assert lib.wn_enhance_workspace_bytes(2, 112, 112, -1) > 0
+    assert lib.wn_train_workspace_bytes(65535, 1, 1) > 0
+    assert lib.wn_train_workspace_bytes(65536, 1, 1) == 0   # at most 65535 images per training call
+    assert lib.wn_train_workspace_bytes(0, 8, 8) == 0
     assert lib.wn_forward_chunk_images(None, 4, 8, 8) == 0 and lib.wn_f8_overflowed(None) == 0
     assert lib.wn_set_chunk_pixels(None, 0) != 0
 

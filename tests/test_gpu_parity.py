@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from conftest import golden_files, load_golden
+from grad_reference import reference
 from oracle import forward as ofw
 from oracle import preprocess as opre
 
@@ -298,32 +299,6 @@ def test_training_step_gradients_match_torch_graph():
     assert rel(g1r, m64.gc_refiner.conv3.bias.grad) < 2e-2
 
 
-def _fp64_grads(sd, ins, target):
-    """Ground truth: float64 autograd through the functional oracle graph."""
-    import torch.nn.functional as F
-    params = {k: v.double().clone().requires_grad_(True) for k, v in sd.items()}
-    x, wb, he, gc = leaves = [t.double().clone().requires_grad_(True) for t in ins]
-
-    def conv(prefix, t, k):
-        return F.conv2d(t, params[prefix + ".weight"], params[prefix + ".bias"], padding=k // 2)
-
-    out = torch.cat([x, wb, he, gc], 1)
-    for name, _, _, k in ofw.CMG_LAYERS[:-1]:
-        out = F.relu(conv(f"cmg.{name}", out, k))
-    cm = torch.sigmoid(conv("cmg.conv8", out, 3))
-    total = 0
-    for r, (ref, other) in enumerate(zip(ofw.REFINERS, (wb, he, gc))):
-        t = torch.cat([x, other], 1)
-        for name, _, _, k in ofw.REFINER_LAYERS:
-            t = F.relu(conv(f"{ref}.{name}", t, k))
-        total = total + t * cm[:, r:r + 1]
-    loss = F.mse_loss(total, target.double())
-    loss.backward()
-    grads = {k: v.grad for k, v in params.items()}
-    grads["__inputs__"] = [t.grad for t in leaves]
-    return total.detach(), grads
-
-
 @pytest.mark.parametrize("shape", [(2, 24, 24), (1, 37, 53), (3, 16, 40)])
 def test_native_backward_matches_fp64_autograd(shape):
     """wn_forward_train + wn_backward: all 34 parameter gradients against float64 autograd."""
@@ -337,11 +312,11 @@ def test_native_backward_matches_fp64_autograd(shape):
     out = m(*[t.cuda() for t in ins])
     assert out.grad_fn is not None
     torch.nn.functional.mse_loss(out, target.cuda()).backward()
-    ref_out, ref = _fp64_grads(sd, ins, target)
-    _assert_close(out.detach().cpu().numpy(), ref_out.numpy())
+    ref = reference(sd, ins, target=target, magnitude=False)
+    _assert_close(out.detach().cpu().numpy(), ref.out.numpy())
     worst = 0.0
     for (name, p) in m.named_parameters():
-        g, r = p.grad.double().cpu(), ref[name]
+        g, r = p.grad.double().cpu(), ref.grads[name]
         rel = ((g - r).norm() / r.norm().clamp_min(1e-30)).item()
         worst = max(worst, rel)
         assert rel < 2e-3, f"{name}: relative gradient error {rel:.2e}"
@@ -385,16 +360,16 @@ def _input_grad_case(sd, needs, n=2, h=29, w=43):
     cu = [t.cuda().requires_grad_(need) for t, need in zip(ins, needs)]
     out = m(*cu)
     torch.nn.functional.mse_loss(out, target.cuda()).backward()
-    ref_out, ref = _fp64_grads(sd, ins, target)
-    _assert_close(out.detach().cpu().numpy(), ref_out.numpy())
+    ref = reference(sd, ins, target=target, magnitude=False)
+    _assert_close(out.detach().cpu().numpy(), ref.out.numpy())
     rels = []
-    for t, need, r in zip(cu, needs, ref["__inputs__"]):
+    for t, need, r in zip(cu, needs, ref.input_grads):
         if not need:
             assert t.grad is None
             continue
         assert t.grad.shape == r.shape
         rels.append(((t.grad.double().cpu() - r).norm() / r.norm()).item())
-    prels = {name: ((p.grad.double().cpu() - ref[name]).norm() / ref[name].norm().clamp_min(1e-30)).item()
+    prels = {name: ((p.grad.double().cpu() - ref.grads[name]).norm() / ref.grads[name].norm().clamp_min(1e-30)).item()
              for name, p in m.named_parameters()}
     return rels, prels
 

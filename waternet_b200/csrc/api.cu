@@ -632,7 +632,7 @@ int wn_f8_overflowed(const wn_handle* h) { return h ? umma_f8_overflowed(h) : 0;
 uint64_t wn_launch_count(const wn_handle* h) { return h ? h->launches : 0; }
 
 size_t wn_train_workspace_bytes(int n, int h, int w) {
-  if (n <= 0 || h <= 0 || w <= 0) return 0;
+  if (n <= 0 || h <= 0 || w <= 0 || n > 65535) return 0;
   return train_workspace_bytes_padded(n, h, w);
 }
 
@@ -647,6 +647,10 @@ int wn_forward_train(wn_handle* h, const float* x, const float* wb, const float*
   if (!h->packed) {
     set_error("wn_forward_train: wn_pack_weights has not been called");
     return WN_E_STATE;
+  }
+  if (n > 65535) {  // one image per grid row of the per-pixel kernels
+    set_error("wn_forward_train: at most 65535 images per call, got n=%d", n);
+    return WN_E_UNSUPPORTED;
   }
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
@@ -668,6 +672,10 @@ int wn_backward(wn_handle* h, const float* grad_out, float* const* grads, float*
   if (!h->packed) {
     set_error("wn_backward: wn_pack_weights has not been called");
     return WN_E_STATE;
+  }
+  if (n > 65535) {
+    set_error("wn_backward: at most 65535 images per call, got n=%d", n);
+    return WN_E_UNSUPPORTED;
   }
   if (input_grads)
     for (int i = 0; i < 4; i++)

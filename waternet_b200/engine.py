@@ -265,12 +265,13 @@ class Engine:
 
     # ---- training step (wn_forward_train / wn_backward) ---------------------------------------
     TRAIN_MAX_PIXELS = 8 << 20
+    TRAIN_MAX_IMAGES = 65535
 
     def forward_train(self, x, wb, he, gc):
         """Tensor-core forward that keeps every activation.  Returns (out, saved workspaces).
 
-        wn_forward_train takes at most TRAIN_MAX_PIXELS per call; a larger batch runs as several calls over slices
-        of the batch, each with its own workspace (~5.6 KB per pixel in total, like the reference's autograd graph)."""
+        wn_forward_train takes at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES per call; a larger batch runs as several
+        calls over slices of the batch, each with its own workspace (~5.6 KB per pixel in total, like the reference's autograd graph)."""
         ins = self._check_inputs((x, wb, he, gc))
         n, _, h, w = ins[0].shape
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
@@ -281,7 +282,7 @@ class Engine:
                 f"a forward pass that keeps its activations for autograd holds ~5.6 KB per pixel: one {h}x{w} image "
                 f"exceeds the {self.TRAIN_MAX_PIXELS >> 20} Mi-pixel limit of wn_forward_train.  For inference wrap the "
                 "call in torch.no_grad()")
-        per = max(1, self.TRAIN_MAX_PIXELS // (h * w))
+        per = min(self.TRAIN_MAX_IMAGES, max(1, self.TRAIN_MAX_PIXELS // (h * w)))
         saved = []
         for a in range(0, n, per):
             b = min(n, a + per)
