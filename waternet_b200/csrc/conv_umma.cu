@@ -19,8 +19,8 @@
 // out-of-image pixels come back as zeros from the TMA (padding="same").
 //
 // One persistent CTA per SM, warp-specialised:
-//   warps 0-7  two consumer warpgroups: each issues the m64 wgmmas of half of the 8x16-pixel tile
-//              (accumulators in registers) and then runs the epilogue of those 64 pixels
+//   warps 0-7  two consumer warpgroups: each issues the m64 wgmmas of half of the 8x16- or 16x16-pixel tile
+//              (accumulators in registers; kSpecs mw, ng) and then runs the epilogue of those pixels
 //              (registers -> shared-memory transpose -> bias/act -> bf16 hi/lo planes or fp32)
 //   warp 8     A producer (TMA halo tiles, one 16-channel chunk per stage)
 //   warp 9     B producer (bulk copies of pre-packed weight stages, 1-9 taps of a chunk per stage)
@@ -120,23 +120,26 @@ enum UmmaLayer {
 // Everything a layer's launches and packed weights depend on (UmmaCfg in umma_conv.cuh).  npad = output columns
 // per diagonal block; concat = CONCAT of the bf16x3 form, set where the a_hi x [w_hi | w_lo] product fits one wgmma
 // (N = 2 * NPAD <= 256); slot = timing slot, the state-dict index of the layer's (first) convolution; f8 = the layer
-// has an fp8-correction form (UmmaCfg FMT bit 0, the tensor-bound layers), which uses CONCAT 0.
+// has an fp8-correction form (UmmaCfg FMT bit 0, the tensor-bound layers), which uses CONCAT 0.  mw = m64 blocks per
+// warpgroup (2: 16 x 16-pixel tiles, which halve the weight bytes streamed per pixel) and ng = column groups of npad /
+// ng channels each (UmmaCfg MW, NG): at mw = 2 the accumulators of both blocks must fit in 128 registers per thread.
 struct UmmaLayerSpec {
   int ks, cinpad, npad, epi, concat, nblk, tps, slot;
   bool f8;
+  int mw, ng;
 };
 static constexpr UmmaLayerSpec kSpecs[kNumUmmaLayers] = {
-    // ks cinpad npad epi       concat nblk tps slot f8
-    {7, 16, 224, kEpiAct, 0, 1, 1, 0, false},     // kL1
-    {5, 128, 128, kEpiAct, 0, 1, 5, 1, true},     // kC2
-    {3, 128, 128, kEpiAct, 0, 1, 3, 2, true},     // kC3
-    {1, 128, 64, kEpiAct, 1, 1, 1, 3, false},     // kC4
-    {7, 64, 64, kEpiAct, 1, 1, 7, 4, true},       // kC5
-    {5, 64, 64, kEpiAct, 1, 1, 5, 5, true},       // kC6
-    {3, 64, 64, kEpiAct, 1, 1, 9, 6, true},       // kC7
-    {3, 64, 16, kEpiSigmoid, 1, 1, 9, 7, false},  // kC8
-    {5, 96, 32, kEpiAct, 1, 3, 5, 9, true},       // kR2
-    {3, 96, 16, kEpiGate, 1, 1, 9, 10, false}};   // kR3
+    // ks cinpad npad epi       concat nblk tps slot f8  mw ng
+    {7, 16, 224, kEpiAct, 0, 1, 1, 0, false, 1, 1},     // kL1
+    {5, 128, 128, kEpiAct, 0, 1, 5, 1, true, 1, 1},     // kC2
+    {3, 128, 128, kEpiAct, 0, 1, 3, 2, true, 1, 1},     // kC3
+    {1, 128, 64, kEpiAct, 1, 1, 1, 3, false, 1, 1},     // kC4
+    {7, 64, 64, kEpiAct, 1, 1, 7, 4, true, 2, 1},       // kC5
+    {5, 64, 64, kEpiAct, 1, 1, 5, 5, true, 2, 1},       // kC6
+    {3, 64, 64, kEpiAct, 1, 1, 9, 6, true, 2, 1},       // kC7
+    {3, 64, 16, kEpiSigmoid, 1, 1, 9, 7, false, 1, 1},  // kC8
+    {5, 96, 32, kEpiAct, 1, 3, 5, 9, true, 1, 1},       // kR2
+    {3, 96, 16, kEpiGate, 1, 1, 9, 10, false, 1, 1}};   // kR3
 
 // In the fp8-correction scheme a layer writes the hi + fp8-planes format (FMT bit 1) when its consumers read it with
 // their fp8 form.  L1 feeds C2 and R2; every other layer feeds the next one, except the last layer of each stack.
@@ -227,18 +230,25 @@ int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t str
       for (int r = 0; r < 3 && !rc; r++) rc = scatter(8 + 3 * r + 2, 3, 32, 3 * r, 32, 32 * r, 0);
     }
     if (rc) return rc;
-    pack_stages_kernel<<<256, 256, 0, stream>>>(u->dense, (__nv_bfloat16*)u->stages[li], s.npad, s.cinpad, kk,
-                                                s.concat, s.nblk);
-    WN_LAUNCH_CHECK(h);
+    // each column group's stages are contiguous: group g holds dense rows [g * gw, (g + 1) * gw)
+    const int gw = s.npad / s.ng;
+    const size_t group_bytes = stage_bytes_total(s) / s.ng;
+    for (int g = 0; g < s.ng; g++) {
+      pack_stages_kernel<<<256, 256, 0, stream>>>(u->dense, (__nv_bfloat16*)(u->stages[li] + g * group_bytes), gw,
+                                                  s.cinpad, kk, s.concat, s.nblk, g * gw);
+      WN_LAUNCH_CHECK(h);
+    }
     if (s.f8) {
       WN_CUDA(cudaMemsetAsync(u->scale8[li], 0, 4 * sizeof(float), stream));
       f8_absmax_kernel<<<64, 256, 0, stream>>>(u->dense, (size_t)rows * s.cinpad * kk, u->scale8[li]);
       WN_LAUNCH_CHECK(h);
       f8_scale_finish_kernel<<<1, 1, 0, stream>>>(u->scale8[li]);
       WN_LAUNCH_CHECK(h);
-      pack_stages_f8_kernel<<<256, 256, 0, stream>>>(u->dense, u->stages8[li], u->scale8[li], s.npad, s.cinpad, kk,
-                                                     s.nblk);
-      WN_LAUNCH_CHECK(h);
+      for (int g = 0; g < s.ng; g++) {
+        pack_stages_f8_kernel<<<256, 256, 0, stream>>>(u->dense, u->stages8[li] + g * group_bytes, u->scale8[li], gw,
+                                                       s.cinpad, kk, s.nblk, g * gw);
+        WN_LAUNCH_CHECK(h);
+      }
     }
   }
   return WN_OK;
@@ -289,15 +299,16 @@ static int launch_layer_as(wn_handle* h, bool f8, void* in_base, ConvArgs a, cud
   constexpr UmmaLayerSpec s = kSpecs[LI];
   constexpr bool R = RAG && s.epi != kEpiSigmoid;
   const UmmaWeights* u = h->umma;
+  constexpr int GW = s.npad / s.ng;  // channels per column group
   if (f8) {
     constexpr int FMT = (s.f8 ? kFmtIn8 : 0) | (writes_f8(LI) ? kFmtOut8 : 0);
     if constexpr ((FMT & kFmtOut8) != 0) a.f8_overflow = u->overflow_dev;
     if constexpr (s.f8) a.f8_scale = u->scale8[LI] + 1;
-    return launch_conv<s.ks, s.cinpad, s.npad, s.epi, (s.f8 ? 0 : s.concat), s.nblk, s.tps, FMT, R>(
+    return launch_conv<s.ks, s.cinpad, GW, s.epi, (s.f8 ? 0 : s.concat), s.nblk, s.tps, FMT, R, s.mw, s.ng>(
         h, s.slot, s.f8 ? u->stages8[LI] : u->stages[LI], u->bias[LI], in_base, a, stream);
   }
-  return launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps, 0, R>(h, s.slot, u->stages[LI],
-                                                                                 u->bias[LI], in_base, a, stream);
+  return launch_conv<s.ks, s.cinpad, GW, s.epi, s.concat, s.nblk, s.tps, 0, R, s.mw, s.ng>(
+      h, s.slot, u->stages[LI], u->bias[LI], in_base, a, stream);
 }
 template <int LI>
 static int launch_layer(wn_handle* h, bool f8, void* in_base, ConvArgs a, cudaStream_t stream) {

@@ -89,9 +89,9 @@ __device__ __forceinline__ uint16_t pack_e4m3x2(float f0, float f1) {
 // kEpiDgrad (backward): no bias; zero where the saved forward activation is zero (ReLU'), -> planes.
 enum Epilogue { kEpiAct = 0, kEpiSigmoid = 1, kEpiGate = 2, kEpiDgrad = 3 };
 
-// One CTA tile = 8 x 16 pixels = M 128: warpgroup w computes rows 64w..64w+63 (pixel rows 8w..8w+7) with
-// m64nNk16 wgmma, accumulators in registers, and then runs the epilogue of those rows itself.
-constexpr int kTileW = 8, kTileH = 16;
+// One CTA tile = (8 * MW) x 16 pixels: warpgroup w computes pixel rows 8w..8w+7 as MW m64 blocks (block b = tile
+// columns 8b..8b+7) with m64nNk16 wgmma, accumulators in registers, and then runs the epilogue of those rows itself.
+constexpr int kTileH = 16;
 // warps 0-7: two consumer warpgroups (wgmma + epilogue); 8: A producer (TMA halo tiles); 9: B producer (weights)
 constexpr int kThreads = 320;
 constexpr int kWarpA = 8, kWarpB = 9;
@@ -115,12 +115,19 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 //        The fp8 product accumulates in registers of its own: Hopper's fp8 wgmma adds with fewer mantissa bits
 //        than fp32, which is harmless for the small correction terms but not for the main product.
 //        bit 1 (kFmtOut8): the epilogue writes that hi + fp8-planes format (its consumer has bit 0 set).
+// MW     m64 blocks per warpgroup: 1 = 8 x 16-pixel tile (M = 128), 2 = 16 x 16 (M = 256).  Every weight stage a
+//        CTA streams from L2 then serves twice the pixels.
+// NG     column groups: a CTA computes the NPAD output channels [g * NPAD, (g + 1) * NPAD) of column group g; the
+//        layer has NG * NPAD channels and each group's weight stages are packed contiguously.  Splitting the columns
+//        keeps MW = 2 within the registers of a wide layer, at the price of reading each halo tile once per group.
 constexpr int kFmtIn8 = 1, kFmtOut8 = 2;
-template <int KS, int CIN_PAD, int NPAD, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0>
+template <int KS, int CIN_PAD, int NPAD, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0, int MW = 1,
+          int NG = 1>
 struct UmmaCfg {
   static constexpr bool F8IN = (FMT & kFmtIn8) != 0;
   static constexpr bool DUAL = CONCAT != 0;  // two accumulator halves per block: [a x w_hi | a_hi x w_lo]
-  static constexpr int HALO_W = kTileW + KS - 1, HALO_H = kTileH + KS - 1;
+  static constexpr int TILE_W = 8 * MW;
+  static constexpr int HALO_W = TILE_W + KS - 1, HALO_H = kTileH + KS - 1;
   static constexpr int NCHUNK = CIN_PAD / 16;
   static constexpr int PLANE_BYTES = HALO_W * HALO_H * 16;
   static constexpr int A_STAGE = (4 * PLANE_BYTES + 1023) / 1024 * 1024;  // hi k0, hi k1, lo k0, lo k1
@@ -150,7 +157,11 @@ struct UmmaCfg {
   static_assert(NA >= 1, "halo tile does not fit in shared memory");
   static_assert(NCHUNK % NBLK == 0, "chunks must split evenly over the diagonal blocks");
   static_assert(NPAD % 16 == 0 && (DUAL ? 2 : 1) * NPAD <= 256, "invalid wgmma N");
-  static_assert(ACC + (F8IN ? ACC8 : 0) <= 128, "accumulators do not fit in registers");
+  static_assert(MW == 1 || MW == 2, "one or two m64 blocks per warpgroup");
+  static_assert(NG == 1 || NBLK == 1, "column groups of a block-diagonal layer");
+  static_assert(MW * (ACC + (F8IN ? ACC8 : 0)) <= 128, "accumulators do not fit in registers");
+  // full weight image of one column group: every (chunk, stage)
+  static constexpr size_t GROUP_BYTES = (size_t)NCHUNK * NSTAGE_PER_CHUNK * B_STAGE;
 };
 
 struct ActDst {
@@ -353,11 +364,13 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
   }
 }
 
-// RAG: a pass of a ragged batch (ConvArgs::rwin)
-template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT, int NBLK, int TPS, int FMT = 0, bool RAG = false>
+// RAG: a pass of a ragged batch (ConvArgs::rwin).  Work item t is pixel tile t / NG, column group t % NG, so the
+// groups of one pixel tile run on neighbouring CTAs at the same time and share its halo loads in L2.
+template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT, int NBLK, int TPS, int FMT = 0, bool RAG = false,
+          int MW = 1, int NG = 1>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) {
-  using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT>;
+  using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT, MW, NG>;
   constexpr bool F8IN = C::F8IN, DUAL = C::DUAL, OUT8 = (FMT & kFmtOut8) != 0;
   static_assert(!OUT8 || EPI == kEpiAct, "fp8 planes are written by the activation epilogue only");
   static_assert(!RAG || EPI == kEpiAct || EPI == kEpiGate, "ragged passes mask activations and store the gate");
@@ -373,16 +386,16 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
   uint64_t* b_full = a_empty + C::NA;
   uint64_t* b_empty = b_full + C::NB;
   float* s_bias = reinterpret_cast<float*>(tail + 512);
-  static_assert((2 * 6 + 2 * 8) * 8 <= 512 && NBLK * NPAD * 4 <= 2048 - 512, "barrier / bias area");
+  static_assert((2 * 6 + 2 * 8) * 8 <= 512 && NG * NBLK * NPAD * 4 <= 2048 - 512, "barrier / bias area");
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int num_tiles = g.tiles_x * g.tiles_y * g.N;
+  const int num_tiles = g.tiles_x * g.tiles_y * g.N * NG;
   if (tid == 0) {
     for (int i = 0; i < C::NA; i++) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], kConsumerWarps); }
     for (int i = 0; i < C::NB; i++) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], kConsumerWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  for (int i = tid; i < NBLK * NPAD; i += kThreads) s_bias[i] = g.bias[i];
+  for (int i = tid; i < NG * NBLK * NPAD; i += kThreads) s_bias[i] = g.bias[i];
   __syncthreads();
 
   if (warp == kWarpA) {
@@ -391,10 +404,11 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int n = tile / (g.tiles_x * g.tiles_y);
-        const int rem = tile - n * g.tiles_x * g.tiles_y;
+        const int pt = tile / NG;
+        const int n = pt / (g.tiles_x * g.tiles_y);
+        const int rem = pt - n * g.tiles_x * g.tiles_y;
         const int ty = rem / g.tiles_x, tx = rem - ty * g.tiles_x;
-        const int x0 = tx * kTileW - KS / 2, y0 = ty * kTileH - KS / 2;
+        const int x0 = tx * C::TILE_W - KS / 2, y0 = ty * kTileH - KS / 2;
         for (int c = 0; c < C::NCHUNK; c++) {
           mbar_wait(&a_empty[stage], phase ^ 1);
           uint8_t* dst = a_stages + stage * C::A_STAGE;
@@ -414,10 +428,11 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const uint8_t* wpk = g.wpk + (size_t)(tile % NG) * C::GROUP_BYTES;
         for (int it = 0; it < C::NCHUNK * C::NSTAGE_PER_CHUNK; it++) {
           mbar_wait(&b_empty[stage], phase ^ 1);
           mbar_expect_tx(&b_full[stage], C::B_STAGE);
-          bulk_load(b_stages + stage * C::B_STAGE, g.wpk + (size_t)it * C::B_STAGE, C::B_STAGE, &b_full[stage]);
+          bulk_load(b_stages + stage * C::B_STAGE, wpk + (size_t)it * C::B_STAGE, C::B_STAGE, &b_full[stage]);
           if (++stage == C::NB) { stage = 0; phase ^= 1; }
         }
       }
@@ -430,10 +445,11 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
   const bool skip_lo = (g.skip_lo != nullptr && *g.skip_lo != 0) || g.a_hi_only;
   const float dscale = F8IN ? *g.f8_scale : 1.f;
   // A operand: rows of the tile = pixels, 8 consecutive pixels of a halo row = one core matrix; this warpgroup's
-  // rows start 8 halo rows further.  K halves (channels 0-7 / 8-15 of the chunk) are one plane apart.
+  // rows start 8 halo rows further, its second m64 block 8 pixels (128 B) further along the same halo rows.  K halves
+  // (channels 0-7 / 8-15 of the chunk) are one plane apart.
   constexpr uint32_t kSboA = C::HALO_W * 16;
   constexpr uint32_t kLboB = (CONCAT ? 2 * NPAD : NPAD) * 16;
-  float acc[C::ACC], acc8[C::ACC8];
+  float acc[MW][C::ACC], acc8[MW][C::ACC8];
   int astage = 0, bstage = 0, pend_a = -1, pend_b = -1;
   uint32_t aphase = 0, bphase = 0;
   // a stage may be refilled once the wgmma groups reading it have completed: the release of a stage waits for
@@ -447,9 +463,12 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
   };
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
 #pragma unroll
-    for (int i = 0; i < C::ACC; i++) acc[i] = 0.f;
+    for (int mb = 0; mb < MW; mb++) {
 #pragma unroll
-    for (int i = 0; i < C::ACC8; i++) acc8[i] = 0.f;
+      for (int i = 0; i < C::ACC; i++) acc[mb][i] = 0.f;
+#pragma unroll
+      for (int i = 0; i < C::ACC8; i++) acc8[mb][i] = 0.f;
+    }
     // unrolled: the diagonal block a chunk feeds (which accumulator registers its wgmmas write) is a constant
 #pragma unroll
     for (int c = 0; c < C::NCHUNK; c++) {
@@ -466,23 +485,30 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
           const int ky = tap / KS, kx = tap - ky * KS;
           const uint32_t a_tap = a_base + (uint32_t)((ky * C::HALO_W + kx) * 16);
           const uint32_t b_tap = b_base + (uint32_t)(t * C::B_TAP);
-          const uint64_t a_hi = make_desc(a_tap, C::PLANE_BYTES, kSboA);
-          const uint64_t a_lo = make_desc(a_tap + 2 * C::PLANE_BYTES, C::PLANE_BYTES, kSboA);
+          // MW = 2: block mb is the same descriptor 8 pixels further, as an add to the start-address field (that of a
+          // shared-memory address never carries into the next field); fewer live descriptors than building each anew
+          const uint64_t a_hi0 = make_desc(a_tap, C::PLANE_BYTES, kSboA);
 #pragma unroll
-          for (int b = 0; b < NBLK; b++) {
-            if (NBLK > 1 && b != blk) continue;
-            float* d = acc + b * C::BLK_COLS / 2;
-            if constexpr (F8IN) {
-              // w_hi * ws * 2^9 (bf16, K = 16), then [e4m3(lo*2^9) | e4m3(v)] x [e4m3(w*ws) ; e4m3(w_lo*ws*2^9)] (K = 32)
-              wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, NPAD * 16, 128));
-              wgmma_e4m3<NPAD>(acc8 + b * C::BLK_COLS / 2, a_lo, make_desc(b_tap + NPAD * 32, NPAD * 16, 128));
-            } else if constexpr (CONCAT) {
-              wgmma_bf16<2 * NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));            // a_hi x [w_hi | w_lo]
-              if (!skip_lo) wgmma_bf16<NPAD>(d, a_lo, make_desc(b_tap, kLboB, 128));  // a_lo x w_hi
-            } else {
-              wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));                // a_hi x w_hi
-              if (!skip_lo) wgmma_bf16<NPAD>(d, a_lo, make_desc(b_tap, kLboB, 128));  // a_lo x w_hi
-              wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap + 2 * NPAD * 16, kLboB, 128));  // a_hi x w_lo
+          for (int mb = 0; mb < MW; mb++) {
+            const uint64_t a_hi = a_hi0 + mb * (128 >> 4);
+            const uint64_t a_lo = MW == 1 ? make_desc(a_tap + 2 * C::PLANE_BYTES, C::PLANE_BYTES, kSboA)
+                                          : a_hi + ((2 * C::PLANE_BYTES) >> 4);
+#pragma unroll
+            for (int b = 0; b < NBLK; b++) {
+              if (NBLK > 1 && b != blk) continue;
+              float* d = acc[mb] + b * C::BLK_COLS / 2;
+              if constexpr (F8IN) {
+                // w_hi * ws * 2^9 (bf16, K = 16), then [e4m3(lo*2^9) | e4m3(v)] x [e4m3(w*ws) ; e4m3(w_lo*ws*2^9)] (K = 32)
+                wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, NPAD * 16, 128));
+                wgmma_e4m3<NPAD>(acc8[mb] + b * C::BLK_COLS / 2, a_lo, make_desc(b_tap + NPAD * 32, NPAD * 16, 128));
+              } else if constexpr (CONCAT) {
+                wgmma_bf16<2 * NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));            // a_hi x [w_hi | w_lo]
+                if (!skip_lo) wgmma_bf16<NPAD>(d, a_lo, make_desc(b_tap, kLboB, 128));  // a_lo x w_hi
+              } else {
+                wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));                // a_hi x w_hi
+                if (!skip_lo) wgmma_bf16<NPAD>(d, a_lo, make_desc(b_tap, kLboB, 128));  // a_lo x w_hi
+                wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap + 2 * NPAD * 16, kLboB, 128));  // a_hi x w_lo
+              }
             }
           }
         }
@@ -498,52 +524,58 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     wg_wait<0>();
     release();
 
-    // ---- epilogue: 32 output channels at a time through shared memory.  The accumulator fragment gives a thread
-    // two channels of two rows per 8 columns; the epilogue wants a pixel's consecutive channels in one thread.
-    const int n = tile / (g.tiles_x * g.tiles_y);
-    const int rem = tile - n * g.tiles_x * g.tiles_y;
+    // ---- epilogue: one m64 block at a time, 32 output channels at a time through shared memory.  The accumulator
+    // fragment gives a thread two channels of two rows per 8 columns; the epilogue wants a pixel's consecutive
+    // channels in one thread.  Row r of block mb is pixel (8 mb + r % 8, 8 wg + r / 8) of the tile.
+    const int pt = tile / NG, c0 = (tile % NG) * NPAD;
+    const int n = pt / (g.tiles_x * g.tiles_y);
+    const int rem = pt - n * g.tiles_x * g.tiles_y;
     const int ty = rem / g.tiles_x, tx = rem - ty * g.tiles_x;
     float* stg = staging + wg * 64 * kStageLd;
     const int frow = (warp & 3) * 16 + (lane >> 2), fcol = (lane & 3) * 2;
     const int r = wtid & 63, half = wtid >> 6;
     const int m = wg * 64 + r;
-    const int gx = tx * kTileW + (m & 7), gy = ty * kTileH + (m >> 3);
-    const bool inside = gx < g.W && gy < g.H;
-    bool valid = true;
-    if constexpr (RAG) valid = gx < g.rwin[n].vw && gy < g.rwin[n].vh;
+    const int gy = ty * kTileH + (m >> 3);
     constexpr int NCH = NBLK * NPAD;
 #pragma unroll
-    for (int ch0 = 0; ch0 < NCH; ch0 += 32) {
+    for (int mb = 0; mb < MW; mb++) {
+      const int gx = tx * C::TILE_W + mb * 8 + (m & 7);
+      const bool inside = gx < g.W && gy < g.H;
+      bool valid = true;
+      if constexpr (RAG) valid = gx < g.rwin[n].vw && gy < g.rwin[n].vh;
 #pragma unroll
-      for (int j = 0; j < 4; j++) {
-        const int ch = ch0 + 8 * j;
-        if (ch < NCH) {
-          const int col = NBLK > 1 ? (ch / NPAD) * C::BLK_COLS + ch % NPAD : ch;
-          float v[4];
+      for (int ch0 = 0; ch0 < NCH; ch0 += 32) {
 #pragma unroll
-          for (int k = 0; k < 4; k++) {
-            v[k] = acc[col / 2 + k];
-            if constexpr (DUAL) v[k] += acc[(col + NPAD) / 2 + k];
-            if constexpr (F8IN) v[k] = (v[k] + acc8[col / 2 + k]) * dscale;
+        for (int j = 0; j < 4; j++) {
+          const int ch = ch0 + 8 * j;
+          if (ch < NCH) {
+            const int col = NBLK > 1 ? (ch / NPAD) * C::BLK_COLS + ch % NPAD : ch;
+            float v[4];
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+              v[k] = acc[mb][col / 2 + k];
+              if constexpr (DUAL) v[k] += acc[mb][(col + NPAD) / 2 + k];
+              if constexpr (F8IN) v[k] = (v[k] + acc8[mb][col / 2 + k]) * dscale;
+            }
+            float* s = stg + frow * kStageLd + 8 * j + fcol;
+            *reinterpret_cast<float2*>(s) = make_float2(v[0], v[1]);
+            *reinterpret_cast<float2*>(s + 8 * kStageLd) = make_float2(v[2], v[3]);
           }
-          float* s = stg + frow * kStageLd + 8 * j + fcol;
-          *reinterpret_cast<float2*>(s) = make_float2(v[0], v[1]);
-          *reinterpret_cast<float2*>(s + 8 * kStageLd) = make_float2(v[2], v[3]);
         }
-      }
-      wg_bar(1 + wg);
-      const int cb = ch0 + 16 * half;
-      if (cb < NCH && inside) {
-        float f[16];
-        const float4* s = reinterpret_cast<const float4*>(stg + r * kStageLd + 16 * half);
+        wg_bar(1 + wg);
+        const int cb = ch0 + 16 * half;
+        if (cb < NCH && inside) {
+          float f[16];
+          const float4* s = reinterpret_cast<const float4*>(stg + r * kStageLd + 16 * half);
 #pragma unroll
-        for (int q = 0; q < 4; q++) {
-          const float4 x = s[q];
-          f[4 * q] = x.x; f[4 * q + 1] = x.y; f[4 * q + 2] = x.z; f[4 * q + 3] = x.w;
+          for (int q = 0; q < 4; q++) {
+            const float4 x = s[q];
+            f[4 * q] = x.x; f[4 * q + 1] = x.y; f[4 * q + 2] = x.z; f[4 * q + 3] = x.w;
+          }
+          epilogue16<EPI, OUT8, RAG>(g, s_bias, f, c0 + cb, n, gx, gy, valid);
         }
-        epilogue16<EPI, OUT8, RAG>(g, s_bias, f, cb, n, gx, gy, valid);
+        wg_bar(1 + wg);
       }
-      wg_bar(1 + wg);
     }
   }
 }
@@ -569,8 +601,9 @@ static __global__ void scatter_bias_kernel(const float* __restrict__ src, float*
 }
 // dense fp32 [nblk*npad][cinpad][kk] -> weight stages, one per (chunk, tap), holding the rows of the
 // diagonal block the chunk feeds:  concat ? [k8][hi rows | lo rows][8] : [hi|lo][k8][rows][8]   (bf16)
+// row_off: the stages of one column group (UmmaCfg NG) hold dense rows [row_off, row_off + npad)
 static __global__ void pack_stages_kernel(const float* __restrict__ dense, __nv_bfloat16* __restrict__ out, int npad,
-                                   int cinpad, int kk, int concat, int nblk) {
+                                   int cinpad, int kk, int concat, int nblk, int row_off = 0) {
   const int nchunk = cinpad / 16, cpb = nchunk / nblk;
   const size_t total = (size_t)nchunk * kk * 2 * 2 * npad * 8;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -590,7 +623,7 @@ static __global__ void pack_stages_kernel(const float* __restrict__ dense, __nv_
     int tap = (int)(r % kk);
     int chunk = (int)(r / kk);
     int cin = chunk * 16 + k8 * 8 + e;
-    int row = (chunk / cpb) * npad + nrow;
+    int row = row_off + (chunk / cpb) * npad + nrow;
     float w = dense[((size_t)row * cinpad + cin) * kk + tap];
     __nv_bfloat16 hi = __float2bfloat16_rn(w);
     out[i] = split == 0 ? hi : __float2bfloat16_rn(w - __bfloat162float(hi));
@@ -601,7 +634,8 @@ static __global__ void pack_stages_kernel(const float* __restrict__ dense, __nv_
 // fp8 correction scheme (UmmaCfg FMT bit 0): per (chunk, tap):
 //   part 0  [k8 0|1][rows][8 bf16]            w_hi * ws * 2^9              (K = 16 bf16 MMA)
 //   part 1  [k16 0|1][rows][16 fp8 (e4m3)]    w * ws  |  w_lo * ws * 2^9   (K = 32 fp8 MMA)
-// with rows = npad.  scale[0] = ws (a power of two placing max|w| in [112, 224]),
+// with rows = npad (dense rows from row_off on: one column group).  scale[0] = ws (a power of two placing max|w| in
+// [112, 224] over the whole layer),
 // scale[1] = 2^-9 / ws (what the epilogue multiplies the second accumulator with); scale[2] = max|w|.
 // scale[2] (as unsigned bits) accumulates max|w| over the grid (bit patterns of non-negative floats are
 // ordered like the floats); f8_scale_finish_kernel turns it into scale[0], scale[1].
@@ -625,7 +659,8 @@ static __global__ void f8_scale_finish_kernel(float* __restrict__ scale) {
   scale[1] = 1.f / (512.f * ws);
 }
 static __global__ void pack_stages_f8_kernel(const float* __restrict__ dense, uint8_t* __restrict__ out,
-                                             const float* __restrict__ scale, int npad, int cinpad, int kk, int nblk) {
+                                             const float* __restrict__ scale, int npad, int cinpad, int kk, int nblk,
+                                             int row_off) {
   const int nchunk = cinpad / 16, cpb = nchunk / nblk, rows = npad;
   const size_t tap_bytes = (size_t)rows * 64;
   const float ws = scale[0];
@@ -637,7 +672,7 @@ static __global__ void pack_stages_f8_kernel(const float* __restrict__ dense, ui
     const int row = (int)(r % rows); r /= rows;
     const int tap = (int)(r % kk);
     const int chunk = (int)(r / kk);
-    const int wrow = (chunk / cpb) * npad + row;
+    const int wrow = row_off + (chunk / cpb) * npad + row;
     float w[2], wl[2];
     uint16_t hb[2];
 #pragma unroll
@@ -703,10 +738,10 @@ static int make_tmap(CUtensorMap* tm, void* base, int planes_total, int N, int H
 
 // Launch one convolution.  `slot` is the timing slot (common.cuh).  One persistent CTA per SM (shared-memory footprint).
 template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0,
-          bool RAG = false>
+          bool RAG = false, int MW = 1, int NG = 1>
 static int launch_conv(wn_handle* h, int slot, const uint8_t* wpk, const float* bias, void* in_base, ConvArgs a,
                        cudaStream_t stream) {
-  using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT>;
+  using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT, MW, NG>;
   int rc = get_encoder();
   if (rc) return rc;
   CUtensorMap tm;
@@ -715,10 +750,10 @@ static int launch_conv(wn_handle* h, int slot, const uint8_t* wpk, const float* 
   a.wpk = wpk;
   a.bias = bias;
   a.in_planes_half = CIN_PAD / 8;
-  a.tiles_x = (a.W + kTileW - 1) / kTileW;
+  a.tiles_x = (a.W + C::TILE_W - 1) / C::TILE_W;
   a.tiles_y = (a.H + kTileH - 1) / kTileH;
-  const long long tiles = (long long)a.tiles_x * a.tiles_y * a.N;
-  auto kern = conv_umma_kernel<KS, CIN_PAD, NPAD, EPI, CONCAT, NBLK, TPS, FMT, RAG>;
+  const long long tiles = (long long)a.tiles_x * a.tiles_y * a.N * NG;
+  auto kern = conv_umma_kernel<KS, CIN_PAD, NPAD, EPI, CONCAT, NBLK, TPS, FMT, RAG, MW, NG>;
   WN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
   TimedScope ts(h, slot, stream);
   const int grid = (int)(tiles < h->sm_count ? tiles : h->sm_count);
