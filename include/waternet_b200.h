@@ -24,6 +24,7 @@
  *   wn_enhance_u8_ragged  the same for n images of n sizes in one call (inference.py --source <directory>)
  *   wn_forward_train /    train.py:108 `out = model(...)` and train.py:130-131 `loss.backward()`
  *   wn_backward           (autograd through net.py:99-108)
+ *   wn_backward_tiled     the same gradients from the inputs alone, recomputed in overlapping windows
  *
  * Conventions: every data pointer is a DEVICE pointer on the handle's device
  * unless its name ends in _host; the caller owns every buffer (the handle only
@@ -42,7 +43,7 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 7
+#define WN_ABI_VERSION 8
 
 #define WN_OK 0
 #define WN_E_INVALID (-1)   /* bad argument (NULL pointer, non-positive size, unknown mode) */
@@ -261,6 +262,28 @@ int wn_forward_train(wn_handle* h, const float* x, const float* wb, const float*
                      void* train_workspace, size_t workspace_bytes, void* stream);
 int wn_backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n,
                 int height, int width, void* train_workspace, size_t workspace_bytes, void* stream);
+
+/*
+ * The windowed recompute backward: the gradients wn_backward gives, from the four inputs alone, in memory that does
+ * not grow with the image size.  The images are cut into the windows of wn_forward_tiled (tile_h x tile_w output
+ * tiles, 13 pixels of context per side).  For each pass of windows the call recomputes the training forward (the
+ * WN_MODE_BF16X3 arithmetic, the first layer's exact-levels decision taken over all input pixels, as
+ * wn_forward_tiled takes it) and runs the backward pass with d(loss)/d(out) taken inside each window's kept
+ * rectangle and 0 elsewhere.  The result equals the untiled gradients up to the order of the fp32 sums.
+ *   - x, wb, he, gc, in_strides: as wn_forward_tiled.  grad_out: fp32 contiguous (N,3,H,W) of the full images.
+ *   - grads, input_grads: as wn_backward, overwritten.
+ *   - max_pass_pixels: window pixels per pass, 0 = 2 Mi (~11.8 GB of workspace); at most 8 Mi, and a single window
+ *     may not exceed 8 Mi pixels either.  n <= 65535 and h * w <= 715,827,882 as the tiled forward.
+ *   - Deterministic, no atomics.  Input gradients are added window by window in window order, so they do not depend
+ *     on max_pass_pixels; the parameter gradients do (through the pixel split of the weight-gradient GEMMs).
+ *   - Nothing is copied from the host: a call can be captured in a CUDA graph.
+ * wn_backward_tiled_workspace_bytes returns 0 for every argument set the call rejects.
+ */
+size_t wn_backward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels);
+int wn_backward_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                      const int64_t in_strides[4][4], const float* grad_out, float* const* grads,
+                      float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
+                      long long max_pass_pixels, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * Per-kernel device timing (measurement aid for bench.py, off by default).  When on, every

@@ -688,6 +688,69 @@ int wn_backward(wn_handle* h, const float* grad_out, float* const* grads, float*
                   (cudaStream_t)stream);
 }
 
+// the argument checks wn_backward_tiled and its workspace function share (pointers aside)
+static int backward_tiled_check(const char* what, int n, int height, int width, int tile_h, int tile_w,
+                                long long max_pass_pixels) {
+  if (n <= 0 || height <= 0 || width <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
+    set_error("%s: bad shape n=%d h=%d w=%d tile=%dx%d max_pass_pixels=%lld", what, n, height, width, tile_h, tile_w,
+              max_pass_pixels);
+    return WN_E_INVALID;
+  }
+  if ((size_t)height * width > (size_t)0x7fffffff / 3 || n > 65535) {
+    set_error("image too large: n=%d h=%d w=%d", n, height, width);
+    return WN_E_UNSUPPORTED;
+  }
+  if (max_pass_pixels > kTrainMaxPixels) {
+    set_error("%s: max_pass_pixels=%lld exceeds the %lld pixels of one training pass", what, max_pass_pixels,
+              kTrainMaxPixels);
+    return WN_E_UNSUPPORTED;
+  }
+  const TileGeom g = tile_geom(height, width, tile_h, tile_w);
+  if ((long long)g.win_h * g.win_w > kTrainMaxPixels) {
+    set_error("%s: a %dx%d window exceeds the %lld pixels of one training pass; use a smaller tile", what, g.win_h,
+              g.win_w, kTrainMaxPixels);
+    return WN_E_UNSUPPORTED;
+  }
+  return WN_OK;
+}
+
+size_t wn_backward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels) {
+  if (backward_tiled_check("wn_backward_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels)) return 0;
+  return backward_tiled_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels);
+}
+
+int wn_backward_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                      const int64_t in_strides[4][4], const float* grad_out, float* const* grads,
+                      float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
+                      long long max_pass_pixels, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* what = "wn_backward_tiled";
+  if (!h || !x || !wb || !he || !gc || !in_strides || !grad_out || !grads || !workspace) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  for (int i = 0; i < WN_NUM_PARAMS; i++)
+    if (!grads[i]) {
+      set_error("%s: grads[%d] is NULL", what, i);
+      return WN_E_INVALID;
+    }
+  if (input_grads)
+    for (int i = 0; i < 4; i++)
+      if (!input_grads[i]) {
+        set_error("%s: input_grads[%d] is NULL", what, i);
+        return WN_E_INVALID;
+      }
+  int rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  const float* in[4] = {x, wb, he, gc};
+  return backward_tiled(h, in, in_strides, grad_out, grads, input_grads, n, height, width, tile_h, tile_w,
+                        max_pass_pixels, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const float* he,
                            const float* gc, const int64_t in_strides[4][4], int n, int height,
                            int width, int mode, int layer, float* dst, void* workspace,

@@ -244,7 +244,17 @@ int umma_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images, int n, i
                            int scheme);
 int umma_f8_overflowed(const wn_handle* h);
 
+// conv_umma.cu: the two packing steps of the tiled forward, shared with the windowed backward.  The exact-levels
+// flag over every input pixel of the n images (*flag is set to 1, then cleared unless all are 8-bit levels), and the
+// act0 planes of `count` windows (win0, win0 + 1, ...) of `tiles`, read at image coordinates.
+int pack_exact_flag(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], int* flag, int n,
+                    int height, int width, const TileGeom& tiles, cudaStream_t stream);
+int pack_input_windows(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], uint4* act0, int height,
+                       int width, const TileGeom& tiles, long long win0, int count, cudaStream_t stream);
+
 // conv_bwd.cu
+constexpr long long kTrainMaxPixels = 8ll << 20;  // pixels of one training pass (activations kept: ~5.6 KB each)
+constexpr long long kTiledTrainPassPixels = 2ll << 20;  // wn_backward_tiled: window pixels per pass by default
 int bwd_pack_weights(wn_handle* h, const float* const* params, cudaStream_t stream);
 void bwd_free(wn_handle* h);
 size_t train_workspace_bytes_padded(int n, int h, int w);
@@ -252,5 +262,10 @@ int forward_train(wn_handle* h, const float* const in[4], const int64_t in_strid
                   int height, int width, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 int backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n,
              int height, int width, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+// the windowed recompute backward; arguments checked by the caller (api.cu)
+size_t backward_tiled_workspace_bytes(int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels);
+int backward_tiled(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], const float* grad_out,
+                   float* const* grads, float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
+                   long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace wn

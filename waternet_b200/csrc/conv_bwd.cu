@@ -242,18 +242,13 @@ __global__ void extract_wgrad_kernel(const float* __restrict__ dense, float* __r
 //   g_zr3[3r+c] = g_out[c] * cm[r]            where refined[3r+c] > 0
 //   g_z8[r]     = (sum_c g_out[c] * refined[3r+c]) * cm[r] * (1 - cm[r])
 // Both are written as 16-channel gradient planes (bf16 hi/lo), unused channels zero.
-__global__ void __launch_bounds__(256)
-gate_bwd_kernel(const float* __restrict__ g_out, const float* __restrict__ cm, const float* __restrict__ refined,
-                uint4* __restrict__ g8, uint4* __restrict__ gr3, int hw) {
-  const int n = blockIdx.y;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  float go[3], c[3], v8[16], v9[16];
+// go: d(loss)/d(out) at pixel pix of image n of the batch
+__device__ __forceinline__ void gate_bwd_pixel(const float* go, const float* __restrict__ cm,
+                                               const float* __restrict__ refined, uint4* __restrict__ g8,
+                                               uint4* __restrict__ gr3, int n, int pix, int hw) {
+  float c[3], v8[16], v9[16];
 #pragma unroll
-  for (int k = 0; k < 3; k++) {
-    go[k] = g_out[((size_t)n * 3 + k) * hw + pix];
-    c[k] = cm[((size_t)n * 3 + k) * hw + pix];
-  }
+  for (int k = 0; k < 3; k++) c[k] = cm[((size_t)n * 3 + k) * hw + pix];
 #pragma unroll
   for (int j = 0; j < 16; j++) v8[j] = v9[j] = 0.f;
 #pragma unroll
@@ -283,6 +278,39 @@ gate_bwd_kernel(const float* __restrict__ g_out, const float* __restrict__ cm, c
   store(gr3, v9);
 }
 
+__global__ void __launch_bounds__(256)
+gate_bwd_kernel(const float* __restrict__ g_out, const float* __restrict__ cm, const float* __restrict__ refined,
+                uint4* __restrict__ g8, uint4* __restrict__ gr3, int hw) {
+  const int n = blockIdx.y;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  float go[3];
+#pragma unroll
+  for (int k = 0; k < 3; k++) go[k] = g_out[((size_t)n * 3 + k) * hw + pix];
+  gate_bwd_pixel(go, cm, refined, g8, gr3, n, pix, hw);
+}
+
+// The windowed form (wn_backward_tiled): window blockIdx.y of the pass is window win0 + blockIdx.y of `tiles`.
+// d(loss)/d(out) is read from the full images (contiguous NCHW) at the window's kept pixels and is 0 elsewhere, so
+// every window back-propagates only the output pixels it owns.
+__global__ void __launch_bounds__(256)
+gate_bwd_tiled_kernel(const float* __restrict__ g_out, const float* __restrict__ cm, const float* __restrict__ refined,
+                      uint4* __restrict__ g8, uint4* __restrict__ gr3, TileGeom tiles, long long win0) {
+  const int hw = tiles.win_h * tiles.win_w;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
+  const int wy = pix / tiles.win_w;
+  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
+  const bool kept = y >= t.ky0 && y < t.ky1 && x >= t.kx0 && x < t.kx1;
+  const size_t ihw = (size_t)tiles.H * tiles.W;
+  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
+  float go[3];
+#pragma unroll
+  for (int k = 0; k < 3; k++) go[k] = kept ? g_out[o + k * ihw] : 0.f;
+  gate_bwd_pixel(go, cm, refined, g8, gr3, blockIdx.y, pix, hw);
+}
+
 // data-gradient weights: dense_d[row_off + c][col(o)][kk-1-t] = W[o][c][t]   (transpose + spatial flip)
 // input channel c lands in row  row_off + c  (c < split)  or  row_off + c + shift  (c >= split)
 __global__ void scatter_weights_T_kernel(const float* __restrict__ src, float* __restrict__ dense, int co, int ci,
@@ -302,12 +330,9 @@ __global__ void scatter_weights_T_kernel(const float* __restrict__ src, float* _
 struct InputGrads {
   float* p[4];
 };
-__global__ void __launch_bounds__(256)
-input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, InputGrads out, int hw) {
-  const int n = blockIdx.y;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  float v[16];
+// v[3t + c] = d(loss)/d(input t, channel c) at pixel pix of image n of the batch
+__device__ __forceinline__ void input_grads_pixel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, int n,
+                                                  int pix, int hw, float* v) {
 #pragma unroll
   for (int j = 0; j < 16; j++) v[j] = 0.f;
   const uint4* bufs[2] = {ga, gb};
@@ -325,10 +350,79 @@ input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, I
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(256)
+input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, InputGrads out, int hw) {
+  const int n = blockIdx.y;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  float v[16];
+  input_grads_pixel(ga, gb, n, pix, hw, v);
 #pragma unroll
   for (int t = 0; t < 4; t++)
 #pragma unroll
     for (int c = 0; c < 3; c++) out.p[t][((size_t)n * 3 + c) * hw + pix] = v[t * 3 + c];
+}
+
+// The windowed form (wn_backward_tiled): add the input gradients of the pass's windows (w0, w0 + 1, ...) into the
+// four full (N,3,H,W) images.  Thread (blockIdx.y, pix) is pixel pix of window w0 + blockIdx.y.  Of the windows of
+// this pass that contain its image pixel (tile_cover), only the first does the work: it adds their contributions
+// one at a time in ascending window index to what earlier passes left there.  No atomics, and the order of the
+// additions at a pixel is the window order whatever the pass size.
+__global__ void __launch_bounds__(256)
+fold_input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, InputGrads out, TileGeom tiles,
+                        long long w0, int count) {
+  const int hw = tiles.win_h * tiles.win_w;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const long long me = w0 + blockIdx.y;
+  const TileWindow t = tile_window(tiles, me);
+  const int wy = pix / tiles.win_w;
+  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
+  const TileCover c = tile_cover(tiles, y, x);
+  const long long img0 = (long long)t.img * tiles.ny * tiles.nx;
+  long long first = -1;
+  for (int i = c.i0; i <= c.i1 && first < 0; i++)
+    for (int j = c.j0; j <= c.j1; j++) {
+      const long long k = img0 + (long long)i * tiles.nx + j;
+      if (k >= w0 && k < w0 + count) {
+        first = k;
+        break;
+      }
+    }
+  if (first != me) return;
+  const size_t ihw = (size_t)tiles.H * tiles.W;
+  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
+  float acc[12];
+#pragma unroll
+  for (int q = 0; q < 4; q++)
+#pragma unroll
+    for (int ch = 0; ch < 3; ch++) acc[q * 3 + ch] = out.p[q][o + ch * ihw];
+  for (int i = c.i0; i <= c.i1; i++)
+    for (int j = c.j0; j <= c.j1; j++) {
+      const long long k = img0 + (long long)i * tiles.nx + j;
+      if (k < w0 || k >= w0 + count) continue;
+      const TileWindow u = tile_window(tiles, k);
+      float v[16];
+      input_grads_pixel(ga, gb, (int)(k - w0), (y - u.ys) * tiles.win_w + (x - u.xs), hw, v);
+#pragma unroll
+      for (int q = 0; q < 12; q++) acc[q] += v[q];
+    }
+#pragma unroll
+  for (int q = 0; q < 4; q++)
+#pragma unroll
+    for (int ch = 0; ch < 3; ch++) out.p[q][o + ch * ihw] = acc[q * 3 + ch];
+}
+
+// dst.p[k][i] += src.p[k][i] for the 34 parameter gradients; blockIdx.y = k
+struct ParamGrads {
+  float* p[WN_NUM_PARAMS];
+  int size[WN_NUM_PARAMS];
+};
+__global__ void __launch_bounds__(256) add_param_grads_kernel(ParamGrads dst, ParamGrads src) {
+  const int k = blockIdx.y;
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < dst.size[k]; i += gridDim.x * 256) dst.p[k][i] += src.p[k][i];
 }
 
 // ------------------------------------------------------------------------------------------
@@ -434,7 +528,6 @@ static constexpr size_t kPartialBytes = kPartialSlots * kPartialSlotBytes;
 //                  gradient ping-pong 512 + 512 + 384 + 384 | 16-channel gradients 64 + 64
 static constexpr size_t kTrainBytesPerPixel =
     64 + 3 * 512 + 4 * 256 + 2 * 384 + 12 + 36 + 2 * 512 + 2 * 384 + 2 * 64 + 2 * 128;  // + two 32-ch input-gradient buffers
-static constexpr long long kTrainMaxPixels = 8ll << 20;
 
 size_t train_workspace_bytes(int n, int h, int w) {
   return (size_t)n * h * w * kTrainBytesPerPixel + kDenseBytes + kPartialBytes + 8192;
@@ -601,23 +694,15 @@ static int cmg_conv_backward(wn_handle* h, const TrainBuffers& t, float* const* 
   return g_dst ? launch_dgrad<LI>(h, g, g_dst, s.conv ? act : nullptr, n, H, W, stream) : WN_OK;
 }
 
-int backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n, int H,
-             int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (!h->bwd) {
-    set_error("backward weights have not been packed");
-    return WN_E_STATE;
-  }
-  int rc = check_train_args(n, H, W, workspace_bytes);
-  if (rc) return rc;
-  if ((rc = get_encoder())) return rc;
-  TrainBuffers t;
-  carve(&t, workspace, (size_t)n * H * W);
+// The backward pass of a batch whose forward activations are in t and whose output gradient planes (gate_bwd_kernel)
+// are in t.g8 / t.gr3: the 34 parameter gradients into grads (overwritten) and, when want_input_grads, the data
+// gradients of the packed 16-channel input into t.gin_a (cmg.conv1) and t.gin_b (the refiners' conv1).
+static int backward_layers(wn_handle* h, const TrainBuffers& t, float* const* grads, bool want_input_grads, int n,
+                           int H, int W, cudaStream_t stream) {
+  int rc;
   const int hw = H * W;
   auto gw = [&](int conv) { return grads[2 * conv]; };
   auto gb = [&](int conv) { return grads[2 * conv + 1]; };
-
-  gate_bwd_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(grad_out, t.f.cm, t.f.refined, t.g8, t.gr3, hw);
-  WN_LAUNCH_CHECK(h);
 
   // ---- confidence-map stack: conv8 ... conv1, the gradient ping-ponging between ga and gb ----------
   // conv8's output gradient g8 has 16-channel planes, 3 valid; conv1's input gradient only when asked for
@@ -628,7 +713,8 @@ int backward(wn_handle* h, const float* grad_out, float* const* grads, float* co
   if ((rc = cmg_conv_backward<kD4>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
   if ((rc = cmg_conv_backward<kD3>(h, t, grads, t.ga, t.gb, n, H, W, stream))) return rc;
   if ((rc = cmg_conv_backward<kD2>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
-  if ((rc = cmg_conv_backward<kD1>(h, t, grads, t.ga, input_grads ? t.gin_a : nullptr, n, H, W, stream))) return rc;
+  if ((rc = cmg_conv_backward<kD1>(h, t, grads, t.ga, want_input_grads ? t.gin_a : nullptr, n, H, W, stream)))
+    return rc;
 
   // ---- refiners: conv3, conv2, conv1 (three side by side) ---------------------------------
   if ((rc = launch_wgrad<kDR3>(h, t.gr3, 9, t.f.r[2], t.dense, t.partial, n, H, W, stream))) return rc;
@@ -663,12 +749,138 @@ int backward(wn_handle* h, const float* grad_out, float* const* grads, float* co
       WN_CUDA(cudaMemcpyAsync(gb(8 + 3 * r), tmp + 32 * r, 32 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
     }
   }
+  if (want_input_grads) return launch_dgrad<kDR1>(h, t.grb, t.gin_b, nullptr, n, H, W, stream);
+  return WN_OK;
+}
+
+int backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n, int H,
+             int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!h->bwd) {
+    set_error("backward weights have not been packed");
+    return WN_E_STATE;
+  }
+  int rc = check_train_args(n, H, W, workspace_bytes);
+  if (rc) return rc;
+  if ((rc = get_encoder())) return rc;
+  TrainBuffers t;
+  carve(&t, workspace, (size_t)n * H * W);
+  const int hw = H * W;
+
+  gate_bwd_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(grad_out, t.f.cm, t.f.refined, t.g8, t.gr3, hw);
+  WN_LAUNCH_CHECK(h);
+  if ((rc = backward_layers(h, t, grads, input_grads != nullptr, n, H, W, stream))) return rc;
   if (input_grads) {
-    if ((rc = launch_dgrad<kDR1>(h, t.grb, t.gin_b, nullptr, n, H, W, stream))) return rc;
     InputGrads ig;
     for (int i = 0; i < 4; i++) ig.p[i] = input_grads[i];
     input_grads_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(t.gin_a, t.gin_b, ig, hw);
     WN_LAUNCH_CHECK(h);
+  }
+  return WN_OK;
+}
+
+// ---- windowed recompute backward (wn_backward_tiled, DESIGN.md "Windowed backward") -------------------------------
+// The windows of tiling.cuh, one pass of them at a time: recompute the training forward of the pass, then run the
+// backward pass above on its windows as a batch, each window's output gradient taken from grad_out inside its kept
+// rectangle and 0 elsewhere.  Because no pixel more than kTileHalo from a kept pixel gets a gradient, each window's
+// contribution equals that of its kept pixels in the untiled backward.  The first pass writes the parameter
+// gradients, every later pass writes them into a scratch copy and adds that in (pass order).  Input gradients are
+// zeroed, then folded in window order.  Workspace: [flag | scratch parameter gradients | one pass of training
+// buffers], independent of the image size.  Nothing is copied from the host.
+static void param_grad_sizes(int* size) {
+  for (int c = 0; c < 8; c++) {
+    size[2 * c] = kCmg[c].cout * kCmg[c].cin * kCmg[c].ks * kCmg[c].ks;
+    size[2 * c + 1] = kCmg[c].cout;
+  }
+  for (int r = 0; r < 3; r++)
+    for (int i = 0; i < 3; i++) {
+      const int conv = 8 + 3 * r + i;
+      size[2 * conv] = kRef[i].cout * kRef[i].cin * kRef[i].ks * kRef[i].ks;
+      size[2 * conv + 1] = kRef[i].cout;
+    }
+}
+
+static size_t param_grads_bytes() {
+  int size[WN_NUM_PARAMS];
+  param_grad_sizes(size);
+  size_t b = 0;
+  for (int k = 0; k < WN_NUM_PARAMS; k++) b += ((size_t)size[k] * sizeof(float) + 255) / 256 * 256;
+  return b;
+}
+
+static long long tiled_train_pass(const TileGeom& g, int n, long long max_pass_pixels) {
+  return tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kTiledTrainPassPixels);
+}
+
+size_t backward_tiled_workspace_bytes(int n, int H, int W, int tile_h, int tile_w, long long max_pass_pixels) {
+  const TileGeom g = tile_geom(H, W, tile_h, tile_w);
+  const long long p = tiled_train_pass(g, n, max_pass_pixels);
+  return 256 + param_grads_bytes() + train_workspace_bytes_padded((int)p, g.win_h, g.win_w) + 256;
+}
+
+int backward_tiled(wn_handle* h, const float* const in[4], const int64_t st[4][4], const float* grad_out,
+                   float* const* grads, float* const* input_grads, int n, int H, int W, int tile_h, int tile_w,
+                   long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!h->bwd || !h->umma) {
+    set_error("backward weights have not been packed");
+    return WN_E_STATE;
+  }
+  const size_t need = backward_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels);
+  if (workspace_bytes < need) {
+    set_error("tiled backward workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  int rc = get_encoder();
+  if (rc) return rc;
+  const TileGeom g = tile_geom(H, W, tile_h, tile_w);
+  const long long total = (long long)n * g.ny * g.nx;
+  const long long per_pass = tiled_train_pass(g, n, max_pass_pixels);
+  const size_t win_px = (size_t)g.win_h * g.win_w;
+  uint8_t* base = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
+  int* exact = (int*)base;
+  ParamGrads dst, part;
+  param_grad_sizes(dst.size);
+  uint8_t* p = base + 256;
+  for (int k = 0; k < WN_NUM_PARAMS; k++) {
+    dst.p[k] = grads[k];
+    part.p[k] = (float*)p;
+    part.size[k] = dst.size[k];
+    p += ((size_t)dst.size[k] * sizeof(float) + 255) / 256 * 256;
+  }
+  void* pass_ws = p;
+  const size_t pass_bytes = workspace_bytes - (size_t)(p - (uint8_t*)workspace);
+  InputGrads ig;
+  if (input_grads)
+    for (int i = 0; i < 4; i++) {
+      ig.p[i] = input_grads[i];
+      WN_CUDA(cudaMemsetAsync(ig.p[i], 0, (size_t)n * 3 * H * W * sizeof(float), stream));
+    }
+  // the first layer drops its a_lo pass exactly when the forward that produced the output did (wn_forward_tiled)
+  if ((rc = pack_exact_flag(h, in, st, exact, n, H, W, g, stream))) return rc;
+  for (long long w0 = 0; w0 < total; w0 += per_pass) {
+    const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
+    if ((rc = check_train_args(cur, g.win_h, g.win_w, pass_bytes))) return rc;
+    TrainBuffers t;
+    carve(&t, pass_ws, (size_t)cur * win_px);
+    t.f.exact_flag = exact;
+    if ((rc = pack_input_windows(h, in, st, t.f.act0, H, W, g, w0, cur, stream))) return rc;
+    FwdOpts o;  // the bf16x3 scheme; the backward needs cm and refined, not the output
+    o.packed = true;
+    if ((rc = umma_forward_layers(h, in, st, nullptr, cur, g.win_h, g.win_w, t.f, stream, o))) return rc;
+    gate_bwd_tiled_kernel<<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(
+        grad_out, t.f.cm, t.f.refined, t.g8, t.gr3, g, w0);
+    WN_LAUNCH_CHECK(h);
+    if ((rc = backward_layers(h, t, w0 == 0 ? grads : part.p, input_grads != nullptr, cur, g.win_h, g.win_w,
+                              stream)))
+      return rc;
+    if (w0 > 0) {
+      add_param_grads_kernel<<<dim3(64, WN_NUM_PARAMS), 256, 0, stream>>>(dst, part);
+      WN_LAUNCH_CHECK(h);
+    }
+    if (input_grads) {
+      fold_input_grads_kernel<<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(t.gin_a, t.gin_b, ig,
+                                                                                                g, w0, cur);
+      WN_LAUNCH_CHECK(h);
+    }
   }
   return WN_OK;
 }

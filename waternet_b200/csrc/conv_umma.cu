@@ -758,6 +758,26 @@ int umma_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images, int n, i
 // images) in window layout and store_kept_kernel copies the kept rectangle of the wanted planes into `out`.
 // Workspace: [flag | refined images of one pass (sub-modules) | one pass], independent of the image size.  Nothing
 // is copied from the host: the call can be captured in a graph.
+int pack_exact_flag(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], int* flag, int n, int H,
+                    int W, const TileGeom& tiles, cudaStream_t stream) {
+  TimedScope ts(h, kSlotPack, stream);
+  WN_CUDA(cudaMemsetAsync(flag, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
+  pack_inputs_kernel<kPackFlag><<<dim3((H * W + 255) / 256, n), 256, 0, stream>>>(pack_args(in, in_strides), nullptr,
+                                                                                  H, W, flag, tiles, 0);
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+
+int pack_input_windows(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], uint4* act0, int H,
+                       int W, const TileGeom& tiles, long long win0, int count, cudaStream_t stream) {
+  TimedScope ts(h, kSlotPack, stream);
+  const size_t win_px = (size_t)tiles.win_h * tiles.win_w;
+  pack_inputs_kernel<kPackWindows><<<dim3((unsigned)((win_px + 255) / 256), count), 256, 0, stream>>>(
+      pack_args(in, in_strides), act0, H, W, nullptr, tiles, win0);
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+
 size_t umma_forward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
                                           bool submodule) {
   const TileGeom g = tile_geom(h, w, tile_h, tile_w);
@@ -790,23 +810,12 @@ int umma_forward_tiled(wn_handle* h, const float* const in[4], const int64_t in_
   int* exact = (int*)base;
   float* refined = (float*)(base + 256);
   void* fwd_ws = base + 256 + (sub ? align256(per_pass * win_px * 9 * sizeof(float)) : 0);
-  const PackInArgs pa = pack_args(in, in_strides);
-  {
-    TimedScope ts(h, kSlotPack, stream);
-    WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
-    pack_inputs_kernel<kPackFlag><<<dim3((H * W + 255) / 256, n), 256, 0, stream>>>(pa, nullptr, H, W, exact, g, 0);
-    WN_LAUNCH_CHECK(h);
-  }
+  if ((rc = pack_exact_flag(h, in, in_strides, exact, n, H, W, g, stream))) return rc;
   for (long long w0 = 0; w0 < total; w0 += per_pass) {
     const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
     FwdBuffers b = carve(fwd_ws, cur, g.win_h, g.win_w);
     b.exact_flag = exact;
-    {
-      TimedScope ts(h, kSlotPack, stream);
-      pack_inputs_kernel<kPackWindows><<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(
-          pa, b.act0, H, W, exact, g, w0);
-      WN_LAUNCH_CHECK(h);
-    }
+    if ((rc = pack_input_windows(h, in, in_strides, b.act0, H, W, g, w0, cur, stream))) return rc;
     FwdOpts o;
     o.scheme = scheme;
     o.packed = true;

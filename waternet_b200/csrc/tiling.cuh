@@ -63,6 +63,28 @@ __host__ __device__ inline TileWindow tile_window(const TileGeom& g, long long w
   return t;
 }
 
+// The windows whose extent contains image pixel (y, x): tile rows [i0, i1] x tile columns [j0, j1] of its image, the
+// window numbering of tile_window (row-major).  Window i starts at ys(i) = clamp(i*th - kTileHalo, 0, H - win_h),
+// which does not decrease with i, so the windows containing a row form one run: i1 is the last with ys(i) <= y, i0
+// the first with ys(i) + win_h > y.  Every pixel lies in its own tile's window, so the run is never empty.  Tiles
+// smaller than 2 * kTileHalo put a pixel in three or more windows per axis; when win_h == H every window contains it.
+struct TileCover {
+  int i0, i1, j0, j1;
+};
+
+__host__ __device__ inline void tile_cover_axis(int v, int size, int t, int count, int win, int* lo, int* hi) {
+  *hi = v >= size - win ? count - 1 : (v + kTileHalo) / t < count - 1 ? (v + kTileHalo) / t : count - 1;
+  const int first = v - win + 1;  // ys(i) >= first
+  *lo = first <= 0 ? 0 : (first + kTileHalo + t - 1) / t;
+}
+
+__host__ __device__ inline TileCover tile_cover(const TileGeom& g, int y, int x) {
+  TileCover c;
+  tile_cover_axis(y, g.H, g.th, g.ny, g.win_h, &c.i0, &c.i1);
+  tile_cover_axis(x, g.W, g.tw, g.nx, g.win_w, &c.j0, &c.j1);
+  return c;
+}
+
 // windows per pass: as many as fit in max_pass_pixels (at least one, at most all of them and at most 65535, the
 // grid limit of the per-window apply kernel)
 __host__ __device__ inline long long tile_pass_windows(const TileGeom& g, int n, long long max_pass_pixels) {

@@ -71,7 +71,22 @@ def tile_geometry(h: int, w: int, tile_h: int, tile_w: int) -> dict:
             "windows": [(ys[i], xs[j], rows[i], cols[j]) for i in range(ny) for j in range(nx)]}
 
 
+def covering_windows(g: dict, y: int, x: int) -> Tuple[range, range]:
+    """The windows whose extent contains pixel (y, x) of an image with ``tile_geometry`` ``g``: (tile rows, tile
+    columns), as ranges (csrc/tiling.cuh tile_cover, which the windowed backward folds input gradients by).  A
+    window's origin does not decrease along an axis, so the windows containing a row form one run."""
+    def axis(v, size, t, count, win):
+        hi = count - 1 if v >= size - win else min(count - 1, (v + TILE_HALO) // t)
+        first = v - win + 1  # origin >= first
+        lo = 0 if first <= 0 else -(-(first + TILE_HALO) // t)
+        return range(lo, hi + 1)
+    h = g["windows"][-1][2][1]
+    w = g["windows"][-1][3][1]
+    return axis(y, h, g["th"], g["ny"], g["win_h"]), axis(x, w, g["tw"], g["nx"], g["win_w"])
+
+
 DEFAULT_PASS_PIXELS = 8 << 20  # max_pass_pixels = 0
+TRAIN_PASS_PIXELS = 2 << 20    # max_pass_pixels = 0 of the windowed backward (wn_backward_tiled)
 RAGGED_WINDOW_BYTES = 72       # csrc/tiling.cuh RaggedWindow: one descriptor per window
 RAGGED_IMAGE_BYTES = 40        # csrc/common.cuh RaggedImage: one per image
 
@@ -608,3 +623,44 @@ class Engine:
                                                ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
         _lib.check(rc, "wn_enhance_u8_ragged")
         return outs
+
+    # ---- windowed recompute backward (wn_backward_tiled) -------------------------------------------
+    def backward_tiled_workspace_bytes(self, n: int, h: int, w: int, tile=DEFAULT_TILE, max_pass_pixels: int = 0) -> int:
+        """Workspace of one ``backward_tiled`` call (wn_backward_tiled_workspace_bytes); 0 for rejected arguments."""
+        th, tw = self._tile_hw(tile)
+        return int(self.lib.wn_backward_tiled_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels)))
+
+    def backward_tiled(self, grad_out: torch.Tensor, inputs, shapes, tile=DEFAULT_TILE, want_input_grads: bool = False,
+                       max_pass_pixels: int = 0):
+        """The gradients of ``backward`` from the four input images alone (wn_backward_tiled): the training forward
+        is recomputed in the overlapping windows of ``forward_tiled``, one pass of windows at a time, so no
+        activation outlives the call and the workspace does not grow with the image size.  ``max_pass_pixels``:
+        window pixels per pass (0 = 2 Mi, ~11.8 GB).  The workspace is allocated for this call only."""
+        th, tw = self._tile_hw(tile)
+        ins = self._check_inputs(inputs)
+        g = grad_out.detach().to(self.device, torch.float32).contiguous()
+        n, _, h, w = ins[0].shape
+        if tuple(g.shape) != (n, 3, h, w):
+            raise ValueError(f"grad_out must be {(n, 3, h, w)}, got {tuple(g.shape)}")
+        if g.numel() == 0:
+            grads = [torch.zeros(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
+            gin = [torch.zeros((n, 3, h, w), dtype=torch.float32, device=self.device) for _ in range(4)]
+            return (grads, gin) if want_input_grads else grads
+        grads = [torch.empty(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
+        gin = [torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) for _ in range(4)] \
+            if want_input_grads else None
+        nbytes = self.backward_tiled_workspace_bytes(n, h, w, (th, tw), max_pass_pixels)
+        if nbytes == 0:
+            raise _lib.WaterNetLibraryError(
+                f"wn_backward_tiled rejects n={n} h={h} w={w} tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        strides = (ctypes.c_int64 * 16)(*[s for t in ins for s in t.stride()])
+        arr = (ctypes.c_void_p * _lib.NUM_PARAMS)(*[t.data_ptr() for t in grads])
+        gin_arr = (ctypes.c_void_p * 4)(*[t.data_ptr() for t in gin]) if want_input_grads else None
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_backward_tiled(self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(),
+                                            ins[3].data_ptr(), strides, g.data_ptr(), arr, gin_arr, n, h, w, th, tw,
+                                            int(max_pass_pixels), ws.data_ptr(), ws.numel(),
+                                            _stream_ptr(self.device))
+        _lib.check(rc, "wn_backward_tiled")
+        return (grads, gin) if want_input_grads else grads

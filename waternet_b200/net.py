@@ -25,7 +25,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib
-from .engine import Engine, new_engine
+from .engine import TRAIN_PASS_PIXELS, Engine, new_engine
 
 MODES = {"default": _lib.MODE_DEFAULT, "fp32": _lib.MODE_FP32_SIMT, "bf16x3": _lib.MODE_BF16X3,
          "bf16_fp8": _lib.MODE_BF16_FP8}
@@ -45,6 +45,16 @@ def _checked_tile(tile, mode: int):
         raise ValueError("tile: the tiled forward runs on the tensor cores only, and precision='fp32' is the CUDA-core "
                          "mode; use precision='default' or 'bf16x3', or tile=None")
     return Engine._tile_hw(tile)
+
+
+def _checked_grad_tile(grad_tile, mode: int):
+    """``grad_tile`` as (h, w), or None for the untiled training path.  The windowed backward is tensor-core only."""
+    if grad_tile is None:
+        return None
+    if mode == _lib.MODE_FP32_SIMT:
+        raise ValueError("grad_tile: the windowed backward runs on the tensor cores only, and precision='fp32' is the "
+                         "CUDA-core mode; use precision='default' or 'bf16x3', or grad_tile=None")
+    return Engine._tile_hw(grad_tile)
 
 
 def _param_version(p) -> int:
@@ -232,14 +242,22 @@ class Refiner(_ConvStack):
 class _KernelForward(torch.autograd.Function):
     """Forward values and all gradients (34 parameters, and the four input images when they require
     grad) from the CUDA library (wn_forward_train / wn_backward).  Only the fp32 CUDA-core mode obtains
-    its gradients by re-evaluating the torch graph.
+    its gradients by re-evaluating the torch graph.  With ``grad_tile`` the forward keeps nothing but the four
+    inputs (wn_forward_tiled in the bf16x3 arithmetic of training) and the backward recomputes the activations
+    window by window (wn_backward_tiled); both hold at most one pass of TRAIN_PASS_PIXELS window pixels.
     """
 
     @staticmethod
-    def forward(ctx, model, mode, x, wb, ce, gc, *params):
+    def forward(ctx, model, mode, grad_tile, x, wb, ce, gc, *params):
         ctx.model = model
         ctx.native = mode != _lib.MODE_FP32_SIMT
+        ctx.grad_tile = grad_tile
         ctx.input_needs_grad = [t.requires_grad for t in (x, wb, ce, gc)]
+        if grad_tile is not None:
+            eng = model._engine_with_weights(x)
+            ctx.engine, ctx.weights_key = eng, eng._weights_key
+            ctx.save_for_backward(x, wb, ce, gc)
+            return eng.forward_tiled(x, wb, ce, gc, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS)
         if ctx.native:
             eng = model._engine_with_weights(x)
             out, ws = eng.forward_train(x, wb, ce, gc)
@@ -258,12 +276,17 @@ class _KernelForward(torch.autograd.Function):
             if eng._weights_key != ctx.weights_key:  # parameters changed between forward and backward
                 raise RuntimeError("model parameters were modified between forward and backward")
             want_in = any(ctx.input_needs_grad)
-            res = eng.backward(grad_out, ctx.saved_ws, [p.shape for p in params], want_input_grads=want_in)
+            shapes = [p.shape for p in params]
+            if ctx.grad_tile is not None:
+                res = eng.backward_tiled(grad_out, ctx.saved_tensors, shapes, ctx.grad_tile, want_input_grads=want_in,
+                                         max_pass_pixels=TRAIN_PASS_PIXELS)
+            else:
+                res = eng.backward(grad_out, ctx.saved_ws, shapes, want_input_grads=want_in)
+                ctx.saved_ws = None
             grads, gin = res if want_in else (res, [None] * 4)
-            ctx.saved_ws = None
             gpar = [g if p.requires_grad else None for g, p in zip(grads, params)]
             gin = [g if need else None for g, need in zip(gin, ctx.input_needs_grad)]
-            return (None, None, *gin, *gpar)
+            return (None, None, None, *gin, *gpar)
         x, wb, ce, gc = ctx.saved_tensors
         with torch.enable_grad():
             ins = [t.detach().requires_grad_(t.requires_grad) for t in (x, wb, ce, gc)]
@@ -273,7 +296,7 @@ class _KernelForward(torch.autograd.Function):
         it = iter(grads)
         gin = [next(it) if t.requires_grad else None for t in ins]
         gpar = [next(it) if p.requires_grad else None for p in params]
-        return (None, None, *gin, *gpar)
+        return (None, None, None, *gin, *gpar)
 
 
 class WaterNet(_PackedWeightsMixin, nn.Module):
@@ -293,11 +316,20 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
     windows (``wn_forward_tiled``): the same bits as untiled, with a workspace that does not grow with the image
     size (~15 GB at tile 998 for a 45 MP photo, which does not fit on an 80 GB card untiled).  Tensor-core
     precisions only.  A call that records an autograd graph (training) ignores ``tile`` and runs as without it.
+
+    ``grad_tile``: None (a call that records an autograd graph keeps every activation until backward, ~5.6 KB per
+    pixel, at most 8 Mi pixels per image) or the largest output tile of the windowed backward, an int or (h, w), e.g.
+    998.  When set, such a call keeps only its four inputs; its output is ``wn_forward_tiled`` in the bf16x3
+    arithmetic of training, and backward recomputes the activations window by window (``wn_backward_tiled``), in
+    about 12 GB whatever the image or batch size.  The gradients equal the untiled ones up to the order of fp32 sums.
+    It costs one more forward and the windows' overlap, so where the untiled path fits it is faster.  Tensor-core
+    precisions only.
     """
 
     tile = None  # models pickled before the attribute existed
+    grad_tile = None
 
-    def __init__(self, precision: str = "default", tile=None):
+    def __init__(self, precision: str = "default", tile=None, grad_tile=None):
         super().__init__()
         self.cmg = ConfidenceMapGenerator()
         self.wb_refiner = Refiner()
@@ -305,8 +337,11 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
         self.gc_refiner = Refiner()
         self.precision = precision
         self.tile = tile
+        self.grad_tile = grad_tile
         if tile is not None:
             _checked_tile(tile, self._mode())
+        if grad_tile is not None:
+            _checked_grad_tile(grad_tile, self._mode())
         self._bind_children()
 
     def _bind_children(self) -> None:
@@ -374,8 +409,9 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
             return self._engine_with_weights(x).forward(x, wb, ce, gc, mode)
         needs_graph = torch.is_grad_enabled() and (
             any(t.requires_grad for t in (x, wb, ce, gc)) or any(p.requires_grad for p in self.parameters()))
-        if needs_graph:  # tile does not apply: training keeps every activation of whole images
-            return _KernelForward.apply(self, mode, x, wb, ce, gc, *self.parameters())
+        if needs_graph:  # tile does not apply: training keeps every activation of whole images, unless grad_tile
+            grad_tile = _checked_grad_tile(self.grad_tile, mode)
+            return _KernelForward.apply(self, mode, grad_tile, x, wb, ce, gc, *self.parameters())
         tile = _checked_tile(self.tile, mode)
         if tile is not None:
             return self._engine_with_weights(x).forward_tiled(x, wb, ce, gc, tile, mode)
