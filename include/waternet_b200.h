@@ -25,6 +25,8 @@
  *   wn_forward_train /    train.py:108 `out = model(...)` and train.py:130-131 `loss.backward()`
  *   wn_backward           (autograd through net.py:99-108)
  *   wn_backward_tiled     the same gradients from the inputs alone, recomputed in overlapping windows
+ *   wn_confidence_maps_train / _backward, wn_refine_train / _backward
+ *                         the sub-modules under autograd (net.py:45-56, :75-80 with parameters that require grad)
  *
  * Conventions: every data pointer is a DEVICE pointer on the handle's device
  * unless its name ends in _host; the caller owns every buffer (the handle only
@@ -43,7 +45,7 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 8
+#define WN_ABI_VERSION 9
 
 #define WN_OK 0
 #define WN_E_INVALID (-1)   /* bad argument (NULL pointer, non-positive size, unknown mode) */
@@ -262,6 +264,35 @@ int wn_forward_train(wn_handle* h, const float* x, const float* wb, const float*
                      void* train_workspace, size_t workspace_bytes, void* stream);
 int wn_backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n,
                 int height, int width, void* train_workspace, size_t workspace_bytes, void* stream);
+
+/*
+ * The sub-modules under autograd (a ConfidenceMapGenerator or a Refiner trained on its own): the training step of
+ * wn_forward_train / wn_backward for one stack.
+ *   - The forward calls compute what wn_confidence_maps / wn_refine compute, in the WN_MODE_BF16X3 arithmetic of
+ *     wn_forward_train (the first layer drops its a_lo pass when every input value is an 8-bit level), and keep the
+ *     stack's activations in `ws`.  out_maps: the (N,3,H,W) maps; out: the refined image of refiner `which`
+ *     (0 = wb_refiner, 1 = ce_refiner, 2 = gc_refiner).  Inputs and strides as wn_confidence_maps / wn_refine.
+ *     A refiner's first layer is the refiners' conv1 alone: it does not pay for cmg.conv1.
+ *   - The backward calls consume that workspace and d(loss)/d(maps) or d(loss)/d(out) (fp32 contiguous NCHW).
+ *     grads has the WN_NUM_PARAMS layout of wn_backward; only the sub-module's own entries are written (overwritten):
+ *     0..15 for the cmg, 16 + 6 which .. 21 + 6 which for refiner `which`.  The other entries are ignored and may be
+ *     NULL.  input_grads is NULL or 4 pointers (cmg: x, wb, he, gc) or 2 (refiner: x, xbar) to fp32 contiguous
+ *     (N,3,H,W) tensors; any entry may be NULL.
+ *   - stack: 0 = confidence maps, 1 = refiner.  The workspace holds that stack's activations and gradients only
+ *     (~3.9 KB per pixel for the cmg, ~1.8 KB for a refiner, plus ~52 MB).  n*h*w <= 8 Mi pixels and n <= 65535
+ *     per call; wn_submodule_train_workspace_bytes returns 0 for arguments the calls reject.  The workspace must stay
+ *     untouched between the forward and the backward call of the same stack and `which`.
+ */
+size_t wn_submodule_train_workspace_bytes(int n, int h, int w, int stack);
+int wn_confidence_maps_train(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                             const int64_t in_strides[4][4], float* out_maps, int n, int height, int width, void* ws,
+                             size_t ws_bytes, void* stream);
+int wn_confidence_maps_backward(wn_handle* h, const float* grad_maps, float* const* grads, float* const* input_grads,
+                                int n, int height, int width, void* ws, size_t ws_bytes, void* stream);
+int wn_refine_train(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
+                    float* out, int n, int height, int width, void* ws, size_t ws_bytes, void* stream);
+int wn_refine_backward(wn_handle* h, int which, const float* grad_out, float* const* grads, float* const* input_grads,
+                       int n, int height, int width, void* ws, size_t ws_bytes, void* stream);
 
 /*
  * The windowed recompute backward: the gradients wn_backward gives, from the four inputs alone, in memory that does

@@ -19,7 +19,7 @@ MODE_BF16_FP8 = 2
 MODE_DEFAULT = -1
 NUM_PARAMS = 34
 NUM_TIMING_SLOTS = 23
-ABI_VERSION = 8
+ABI_VERSION = 9
 PEER_HANDLE_BYTES = 64  # WN_PEER_HANDLE_BYTES
 MAX_PEERS = 15          # WN_MAX_PEERS
 
@@ -92,7 +92,16 @@ _SIGNATURES = {
                                  c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "wn_backward": (c_int, [c_void_p, c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_int, c_void_p,
                             c_size_t, c_void_p]),
-    "wn_backward_tiled_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong]),
+    "wn_submodule_train_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "wn_confidence_maps_train": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p,
+                                         c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "wn_confidence_maps_backward": (c_int, [c_void_p, c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_int, c_int,
+                                            c_int, c_void_p, c_size_t, c_void_p]),
+    "wn_refine_train": (c_int, [c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int64), c_void_p, c_int, c_int, c_int,
+                                c_void_p, c_size_t, c_void_p]),
+    "wn_refine_backward": (c_int, [c_void_p, c_int, c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_int, c_int,
+                                   c_int, c_void_p, c_size_t, c_void_p]),
+    "wn_backward_tiled_workspace_bytes":(c_size_t, [c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong]),
     "wn_backward_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p,
                                   POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int,
                                   ctypes.c_longlong, c_void_p, c_size_t, c_void_p]),

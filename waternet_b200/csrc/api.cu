@@ -688,6 +688,113 @@ int wn_backward(wn_handle* h, const float* grad_out, float* const* grads, float*
                   (cudaStream_t)stream);
 }
 
+// ---- the sub-modules under autograd
+// the shape checks the four calls and the workspace function share; 0 = accepted
+static int submodule_train_check(const char* what, int n, int height, int width) {
+  if (n <= 0 || height <= 0 || width <= 0) {
+    set_error("%s: bad shape n=%d h=%d w=%d", what, n, height, width);
+    return WN_E_INVALID;
+  }
+  if (n > 65535 || (long long)n * height * width > kTrainMaxPixels) {
+    set_error("%s: at most 65535 images and %lld pixels per call, got n=%d h=%d w=%d", what, kTrainMaxPixels, n,
+              height, width);
+    return WN_E_UNSUPPORTED;
+  }
+  return WN_OK;
+}
+// the backward calls: the sub-module's own parameter gradients [first, first + count) must be given
+static int submodule_backward_check(const char* what, wn_handle* h, const float* grad, float* const* grads, int first,
+                                    int count, int n, int height, int width, void* ws) {
+  if (!h || !grad || !grads || !ws) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  for (int i = first; i < first + count; i++)
+    if (!grads[i]) {
+      set_error("%s: grads[%d] is NULL", what, i);
+      return WN_E_INVALID;
+    }
+  int rc = submodule_train_check(what, n, height, width);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  return WN_OK;
+}
+
+size_t wn_submodule_train_workspace_bytes(int n, int h, int w, int stack) {
+  if ((stack != 0 && stack != 1) || submodule_train_check("wn_submodule_train_workspace_bytes", n, h, w)) return 0;
+  return submodule_train_workspace_bytes(n, h, w, stack == 0 ? kStackCmg : kStackRefiners);
+}
+
+int wn_confidence_maps_train(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                             const int64_t in_strides[4][4], float* out_maps, int n, int height, int width, void* ws,
+                             size_t ws_bytes, void* stream) {
+  const char* what = "wn_confidence_maps_train";
+  if (!h || !x || !wb || !he || !gc || !in_strides || !out_maps || !ws) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  int rc = submodule_train_check(what, n, height, width);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  const float* in[4] = {x, wb, he, gc};
+  return confidence_maps_train(h, in, in_strides, out_maps, n, height, width, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+int wn_confidence_maps_backward(wn_handle* h, const float* grad_maps, float* const* grads, float* const* input_grads,
+                                int n, int height, int width, void* ws, size_t ws_bytes, void* stream) {
+  int rc = submodule_backward_check("wn_confidence_maps_backward", h, grad_maps, grads, 0, 16, n, height, width, ws);
+  if (rc) return rc;
+  DeviceGuard guard(h->device);
+  return confidence_maps_backward(h, grad_maps, grads, input_grads, n, height, width, ws, ws_bytes,
+                                  (cudaStream_t)stream);
+}
+
+int wn_refine_train(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
+                    float* out, int n, int height, int width, void* ws, size_t ws_bytes, void* stream) {
+  const char* what = "wn_refine_train";
+  if (which < 0 || which > 2) {
+    set_error("%s: which must be 0, 1 or 2, got %d", what, which);
+    return WN_E_INVALID;
+  }
+  if (!h || !x || !xbar || !in_strides || !out || !ws) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  int rc = submodule_train_check(what, n, height, width);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  // as wn_refine: refiner r sees cat[x, input r+1], so xbar goes to every slot
+  const float* in[4] = {x, xbar, xbar, xbar};
+  int64_t st[4][4];
+  for (int t = 0; t < 4; t++)
+    for (int k = 0; k < 4; k++) st[t][k] = in_strides[t == 0 ? 0 : 1][k];
+  return refine_train(h, which, in, st, out, n, height, width, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+int wn_refine_backward(wn_handle* h, int which, const float* grad_out, float* const* grads, float* const* input_grads,
+                       int n, int height, int width, void* ws, size_t ws_bytes, void* stream) {
+  const char* what = "wn_refine_backward";
+  if (which < 0 || which > 2) {
+    set_error("%s: which must be 0, 1 or 2, got %d", what, which);
+    return WN_E_INVALID;
+  }
+  int rc = submodule_backward_check(what, h, grad_out, grads, 16 + 6 * which, 6, n, height, width, ws);
+  if (rc) return rc;
+  DeviceGuard guard(h->device);
+  return refine_backward(h, which, grad_out, grads, input_grads, n, height, width, ws, ws_bytes, (cudaStream_t)stream);
+}
+
 // the argument checks wn_backward_tiled and its workspace function share (pointers aside)
 static int backward_tiled_check(const char* what, int n, int height, int width, int tile_h, int tile_w,
                                 long long max_pass_pixels) {

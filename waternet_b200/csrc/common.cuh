@@ -199,6 +199,7 @@ struct FwdOpts {
   uint8_t* out_u8 = nullptr;   // the last launch also writes ten2arr(out) as uint8 NHWC
   PeerOut peers = {};          // ... and the same bytes to every peer address (offsets as out_u8)
   int stack = kStackAll;       // kStackCmg: stop after the confidence maps; kStackRefiners: refiners only
+  bool refiner_l1 = false;     // kStackRefiners, bf16x3: the first layer is the refiners' conv1 alone (kRL1)
   const TileGeom* tiles = nullptr;  // tiled forward: image n of the batch is window win0 + n of these tiles, and the
   long long win0 = 0;               // last launch stores its kept rectangle into out / out_u8 at image coordinates
   const RaggedWindow* rwin = nullptr;  // ragged pass (device table): image n of the batch is window rwin[n] in its
@@ -262,6 +263,19 @@ int forward_train(wn_handle* h, const float* const in[4], const int64_t in_strid
                   int height, int width, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 int backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n,
              int height, int width, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+// The sub-modules under autograd (wn_confidence_maps_train / _backward, wn_refine_train / _backward); arguments
+// checked by the caller (api.cu).  stack: kStackCmg or kStackRefiners.  The workspace holds that stack's activations
+// and gradient buffers only.
+size_t submodule_train_workspace_bytes(int n, int height, int width, int stack);
+int confidence_maps_train(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], float* out_maps,
+                          int n, int height, int width, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int confidence_maps_backward(wn_handle* h, const float* grad_maps, float* const* grads, float* const* input_grads,
+                             int n, int height, int width, void* workspace, size_t workspace_bytes,
+                             cudaStream_t stream);
+int refine_train(wn_handle* h, int which, const float* const in[4], const int64_t in_strides[4][4], float* out, int n,
+                 int height, int width, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int refine_backward(wn_handle* h, int which, const float* grad_out, float* const* grads, float* const* input_grads,
+                    int n, int height, int width, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 // the windowed recompute backward; arguments checked by the caller (api.cu)
 size_t backward_tiled_workspace_bytes(int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels);
 int backward_tiled(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], const float* grad_out,

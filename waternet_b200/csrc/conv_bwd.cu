@@ -242,6 +242,20 @@ __global__ void extract_wgrad_kernel(const float* __restrict__ dense, float* __r
 //   g_zr3[3r+c] = g_out[c] * cm[r]            where refined[3r+c] > 0
 //   g_z8[r]     = (sum_c g_out[c] * refined[3r+c]) * cm[r] * (1 - cm[r])
 // Both are written as 16-channel gradient planes (bf16 hi/lo), unused channels zero.
+// 16 gradient values of pixel pix of image n -> a 16-channel gradient buffer (planes hi0, hi1, lo0, lo1)
+__device__ __forceinline__ void store_grad16(uint4* base, const float* v, int n, int pix, int hw) {
+  uint32_t hi[8], lo[8];
+#pragma unroll
+  for (int j = 0; j < 16; j += 2) {
+    split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
+  }
+  uint4* o = base + (size_t)n * 4 * hw + pix;
+  o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+  o[hw] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+  o[2 * (size_t)hw] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+  o[3 * (size_t)hw] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
+}
+
 // go: d(loss)/d(out) at pixel pix of image n of the batch
 __device__ __forceinline__ void gate_bwd_pixel(const float* go, const float* __restrict__ cm,
                                                const float* __restrict__ refined, uint4* __restrict__ g8,
@@ -262,20 +276,8 @@ __device__ __forceinline__ void gate_bwd_pixel(const float* go, const float* __r
     }
     v8[r] = dot * c[r] * (1.0f - c[r]);
   }
-  auto store = [&](uint4* base, const float* v) {
-    uint32_t hi[8], lo[8];
-#pragma unroll
-    for (int j = 0; j < 16; j += 2) {
-      split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
-    }
-    uint4* o = base + (size_t)n * 4 * hw + pix;  // planes: hi0, hi1, lo0, lo1
-    o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    o[hw] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-    o[2 * (size_t)hw] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-    o[3 * (size_t)hw] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-  };
-  store(g8, v8);
-  store(gr3, v9);
+  store_grad16(g8, v8, n, pix, hw);
+  store_grad16(gr3, v9, n, pix, hw);
 }
 
 __global__ void __launch_bounds__(256)
@@ -288,6 +290,48 @@ gate_bwd_kernel(const float* __restrict__ g_out, const float* __restrict__ cm, c
 #pragma unroll
   for (int k = 0; k < 3; k++) go[k] = g_out[((size_t)n * 3 + k) * hw + pix];
   gate_bwd_pixel(go, cm, refined, g8, gr3, n, pix, hw);
+}
+
+// The seeds of the sub-modules called on their own (wn_confidence_maps_backward, wn_refine_backward), as 16-channel
+// gradient planes like gate_bwd_kernel's.  maps = sigmoid(z_8):  g_z8[r] = d(map_r) * cm_r * (1 - cm_r).
+__global__ void __launch_bounds__(256)
+maps_bwd_kernel(const float* __restrict__ g_maps, const float* __restrict__ cm, uint4* __restrict__ g8, int hw) {
+  const int n = blockIdx.y;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  float v8[16];
+#pragma unroll
+  for (int j = 0; j < 16; j++) v8[j] = 0.f;
+#pragma unroll
+  for (int r = 0; r < 3; r++) {
+    const size_t o = ((size_t)n * 3 + r) * hw + pix;
+    const float c = cm[o];
+    v8[r] = g_maps[o] * c * (1.0f - c);
+  }
+  store_grad16(g8, v8, n, pix, hw);
+}
+
+// refiner `which` alone, out = relu(z_r3) of its three columns:  g_zr3[3 which + c] = d(out_c) where
+// refined[3 which + c] > 0; the other refiners' six columns are exactly 0, so nothing flows into their halves
+__global__ void __launch_bounds__(256)
+refine_bwd_kernel(const float* __restrict__ g_out, const float* __restrict__ refined, uint4* __restrict__ gr3,
+                  int which, int hw) {
+  const int n = blockIdx.y;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  float v9[16];
+#pragma unroll
+  for (int j = 0; j < 16; j++) v9[j] = 0.f;
+#pragma unroll
+  for (int r = 0; r < 3; r++) {
+    if (r != which) continue;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      const float rf = refined[((size_t)n * 9 + 3 * r + c) * hw + pix];
+      v9[3 * r + c] = rf > 0.f ? g_out[((size_t)n * 3 + c) * hw + pix] : 0.f;
+    }
+  }
+  store_grad16(gr3, v9, n, pix, hw);
 }
 
 // The windowed form (wn_backward_tiled): window blockIdx.y of the pass is window win0 + blockIdx.y of `tiles`.
@@ -363,6 +407,41 @@ input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, I
   for (int t = 0; t < 4; t++)
 #pragma unroll
     for (int c = 0; c < 3; c++) out.p[t][((size_t)n * 3 + c) * hw + pix] = v[t * 3 + c];
+}
+
+// The input gradients of a sub-module call, from the one 32-channel buffer its first layer wrote (the cmg: gin_a,
+// a refiner: gin_b): out.p[t] (NULL: skipped) receives packed channels 3 slot[t] .. 3 slot[t] + 2 (hi + lo).
+struct SubInputGrads {
+  float* p[4];
+  int slot[4];
+};
+__global__ void __launch_bounds__(256)
+submodule_input_grads_kernel(const uint4* __restrict__ g, SubInputGrads out, int hw) {
+  const int n = blockIdx.y;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  float v[16];
+#pragma unroll
+  for (int j = 0; j < 16; j++) v[j] = 0.f;
+#pragma unroll
+  for (int plane = 0; plane < 2; plane++)
+#pragma unroll
+    for (int half = 0; half < 2; half++) {
+      const uint4 q = g[((size_t)n * 8 + half * 4 + plane) * hw + pix];
+      const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+      for (int j = 0; j < 8; j++) v[plane * 8 + j] += __uint_as_float(((w[j >> 1] >> ((j & 1) * 16)) & 0xffffu) << 16);
+    }
+#pragma unroll
+  for (int t = 0; t < 4; t++) {
+    if (!out.p[t]) continue;
+#pragma unroll
+    for (int s = 0; s < 4; s++) {  // a constant index into v
+      if (s != out.slot[t]) continue;
+#pragma unroll
+      for (int c = 0; c < 3; c++) out.p[t][((size_t)n * 3 + c) * hw + pix] = v[3 * s + c];
+    }
+  }
 }
 
 // The windowed form (wn_backward_tiled): add the input gradients of the pass's windows (w0, w0 + 1, ...) into the
@@ -533,32 +612,52 @@ size_t train_workspace_bytes(int n, int h, int w) {
   return (size_t)n * h * w * kTrainBytesPerPixel + kDenseBytes + kPartialBytes + 8192;
 }
 
-static void carve(TrainBuffers* t, void* workspace, size_t px) {
-  uint8_t* ws = (uint8_t*)(((uintptr_t)workspace + 1023) / 1024 * 1024);
+// The buffers of one training pass of `stack` (FwdStack): kStackAll has all of them; a sub-module called on its own
+// (kStackCmg, kStackRefiners) leaves out the other stack's, which stay NULL.  Returns the bytes used from the
+// workspace's start, the 1 KiB alignment of the first region included.
+static size_t carve(TrainBuffers* t, void* workspace, size_t px, int stack = kStackAll) {
+  const uintptr_t start = (uintptr_t)workspace;
+  uintptr_t ws = (start + 1023) / 1024 * 1024;
   auto take = [&](size_t bytes) {
-    uint8_t* p = ws;
+    const uintptr_t p = ws;
     ws += (bytes + 1023) / 1024 * 1024;
-    return p;
+    return (void*)p;
   };
+  const bool cmg = stack != kStackRefiners, ref = stack != kStackCmg;
   memset(t, 0, sizeof(*t));
   t->f.act0 = (uint4*)take(px * 64);
-  for (int l = 1; l <= 3; l++) t->f.a[l] = (uint4*)take(px * 512);
-  for (int l = 4; l <= 7; l++) t->f.a[l] = (uint4*)take(px * 256);
-  t->f.r[1] = (uint4*)take(px * 384);
-  t->f.r[2] = (uint4*)take(px * 384);
-  t->f.cm = (float*)take(px * 12);
-  t->f.refined = (float*)take(px * 36);
+  if (cmg) {
+    for (int l = 1; l <= 3; l++) t->f.a[l] = (uint4*)take(px * 512);
+    for (int l = 4; l <= 7; l++) t->f.a[l] = (uint4*)take(px * 256);
+  }
+  if (ref) {
+    t->f.r[1] = (uint4*)take(px * 384);
+    t->f.r[2] = (uint4*)take(px * 384);
+  }
+  if (cmg) t->f.cm = (float*)take(px * 12);
+  if (ref) t->f.refined = (float*)take(px * 36);
   t->f.exact_flag = (int*)take(256);
-  t->ga = (uint4*)take(px * 512);
-  t->gb = (uint4*)take(px * 512);
-  t->gra = (uint4*)take(px * 384);
-  t->grb = (uint4*)take(px * 384);
-  t->g8 = (uint4*)take(px * 64);
-  t->gr3 = (uint4*)take(px * 64);
-  t->gin_a = (uint4*)take(px * 128);
-  t->gin_b = (uint4*)take(px * 128);
+  if (cmg) {
+    t->ga = (uint4*)take(px * 512);
+    t->gb = (uint4*)take(px * 512);
+  }
+  if (ref) {
+    t->gra = (uint4*)take(px * 384);
+    t->grb = (uint4*)take(px * 384);
+  }
+  if (cmg) t->g8 = (uint4*)take(px * 64);
+  if (ref) t->gr3 = (uint4*)take(px * 64);
+  if (cmg) t->gin_a = (uint4*)take(px * 128);
+  if (ref) t->gin_b = (uint4*)take(px * 128);
   t->dense = (float*)take(kDenseBytes);
   t->partial = (float*)take(kPartialBytes);
+  return (size_t)(ws - start);
+}
+
+// exactly what carve() takes of a workspace of any alignment
+size_t submodule_train_workspace_bytes(int n, int h, int w, int stack) {
+  TrainBuffers t;
+  return carve(&t, nullptr, (size_t)n * h * w, stack) + 1023;
 }
 
 static int check_train_args(int n, int H, int W, size_t bytes) {
@@ -694,18 +793,15 @@ static int cmg_conv_backward(wn_handle* h, const TrainBuffers& t, float* const* 
   return g_dst ? launch_dgrad<LI>(h, g, g_dst, s.conv ? act : nullptr, n, H, W, stream) : WN_OK;
 }
 
-// The backward pass of a batch whose forward activations are in t and whose output gradient planes (gate_bwd_kernel)
-// are in t.g8 / t.gr3: the 34 parameter gradients into grads (overwritten) and, when want_input_grads, the data
-// gradients of the packed 16-channel input into t.gin_a (cmg.conv1) and t.gin_b (the refiners' conv1).
-static int backward_layers(wn_handle* h, const TrainBuffers& t, float* const* grads, bool want_input_grads, int n,
-                           int H, int W, cudaStream_t stream) {
+// The two halves of the backward pass of a batch whose forward activations are in t.  The confidence-map half starts
+// from the gradient planes t.g8, the refiner half from t.gr3 (gate_bwd_kernel, or a sub-module's own seed).  Each
+// overwrites its stack's parameter gradients in grads (state-dict order) and, when want_input_grads, writes the data
+// gradient of the packed 16-channel input into t.gin_a (cmg.conv1) or t.gin_b (the refiners' conv1).
+static int backward_cmg(wn_handle* h, const TrainBuffers& t, float* const* grads, bool want_input_grads, int n, int H,
+                        int W, cudaStream_t stream) {
   int rc;
-  const int hw = H * W;
-  auto gw = [&](int conv) { return grads[2 * conv]; };
-  auto gb = [&](int conv) { return grads[2 * conv + 1]; };
-
-  // ---- confidence-map stack: conv8 ... conv1, the gradient ping-ponging between ga and gb ----------
-  // conv8's output gradient g8 has 16-channel planes, 3 valid; conv1's input gradient only when asked for
+  // conv8 ... conv1, the gradient ping-ponging between ga and gb.  conv8's output gradient g8 has 16-channel planes,
+  // 3 valid; conv1's input gradient only when asked for
   if ((rc = cmg_conv_backward<kD8>(h, t, grads, t.g8, t.ga, n, H, W, stream))) return rc;
   if ((rc = cmg_conv_backward<kD7>(h, t, grads, t.ga, t.gb, n, H, W, stream))) return rc;
   if ((rc = cmg_conv_backward<kD6>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
@@ -713,19 +809,27 @@ static int backward_layers(wn_handle* h, const TrainBuffers& t, float* const* gr
   if ((rc = cmg_conv_backward<kD4>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
   if ((rc = cmg_conv_backward<kD3>(h, t, grads, t.ga, t.gb, n, H, W, stream))) return rc;
   if ((rc = cmg_conv_backward<kD2>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
-  if ((rc = cmg_conv_backward<kD1>(h, t, grads, t.ga, want_input_grads ? t.gin_a : nullptr, n, H, W, stream)))
-    return rc;
+  return cmg_conv_backward<kD1>(h, t, grads, t.ga, want_input_grads ? t.gin_a : nullptr, n, H, W, stream);
+}
 
-  // ---- refiners: conv3, conv2, conv1 (three side by side) ---------------------------------
+// conv3, conv2, conv1 of the three refiners side by side.  which = -1: the gradients of all three; 0..2: of refiner
+// `which` alone (the launches are the same, only its weight and bias gradients are extracted)
+static int backward_refiners(wn_handle* h, const TrainBuffers& t, float* const* grads, int which,
+                             bool want_input_grads, int n, int H, int W, cudaStream_t stream) {
+  int rc;
+  const int hw = H * W;
+  const int r0 = which < 0 ? 0 : which, r1 = which < 0 ? 3 : which + 1;
+  auto gw = [&](int conv) { return grads[2 * conv]; };
+  auto gb = [&](int conv) { return grads[2 * conv + 1]; };
   if ((rc = launch_wgrad<kDR3>(h, t.gr3, 9, t.f.r[2], t.dense, t.partial, n, H, W, stream))) return rc;
-  for (int r = 0; r < 3; r++) {
+  for (int r = r0; r < r1; r++) {
     if ((rc = extract(h, t.dense, gw(8 + 3 * r + 2), 3, 32, 3, 96, 3 * r, 32, 32 * r, 0, 1.f, stream))) return rc;
   }
   {
     // the nine bias gradients sit in one 16-channel buffer: reduce once, then split per refiner
     float* tmp = t.dense + (size_t)9 * 128 * 96;
     if ((rc = bias_grad(h, t.gr3, 2, 9, tmp, t.partial, n, hw, stream))) return rc;
-    for (int r = 0; r < 3; r++)
+    for (int r = r0; r < r1; r++)
       WN_CUDA(cudaMemcpyAsync(gb(8 + 3 * r + 2), tmp + 3 * r, 3 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   }
   if ((rc = launch_dgrad<kDR3>(h, t.gr3, t.gra, t.f.r[2], n, H, W, stream))) return rc;
@@ -733,7 +837,7 @@ static int backward_layers(wn_handle* h, const TrainBuffers& t, float* const* gr
   {
     float* tmp = t.dense + (size_t)25 * 128 * 96;
     if ((rc = bias_grad(h, t.gra, 12, 96, tmp, t.partial, n, hw, stream))) return rc;
-    for (int r = 0; r < 3; r++) {
+    for (int r = r0; r < r1; r++) {
       if ((rc = extract(h, t.dense, gw(8 + 3 * r + 1), 32, 32, 5, 96, 32 * r, 32, 32 * r, 0, 1.f, stream))) return rc;
       WN_CUDA(cudaMemcpyAsync(gb(8 + 3 * r + 1), tmp + 32 * r, 32 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
     }
@@ -743,7 +847,7 @@ static int backward_layers(wn_handle* h, const TrainBuffers& t, float* const* gr
   {
     float* tmp = t.dense + (size_t)49 * 128 * 16;
     if ((rc = bias_grad(h, t.grb, 12, 96, tmp, t.partial, n, hw, stream))) return rc;
-    for (int r = 0; r < 3; r++) {
+    for (int r = r0; r < r1; r++) {
       // refiner r reads cat[x, input r+1]: channels 0..2 and 3(r+1)..3(r+1)+2 of the packed input
       if ((rc = extract(h, t.dense, gw(8 + 3 * r), 32, 6, 7, 16, 32 * r, 3, 0, 3 * (r + 1), 1.f / 255.f, stream))) return rc;
       WN_CUDA(cudaMemcpyAsync(gb(8 + 3 * r), tmp + 32 * r, 32 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
@@ -751,6 +855,14 @@ static int backward_layers(wn_handle* h, const TrainBuffers& t, float* const* gr
   }
   if (want_input_grads) return launch_dgrad<kDR1>(h, t.grb, t.gin_b, nullptr, n, H, W, stream);
   return WN_OK;
+}
+
+// The whole network: the 34 parameter gradients into grads (overwritten) and, when want_input_grads, t.gin_a and
+// t.gin_b
+static int backward_layers(wn_handle* h, const TrainBuffers& t, float* const* grads, bool want_input_grads, int n,
+                           int H, int W, cudaStream_t stream) {
+  int rc = backward_cmg(h, t, grads, want_input_grads, n, H, W, stream);
+  return rc ? rc : backward_refiners(h, t, grads, -1, want_input_grads, n, H, W, stream);
 }
 
 int backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n, int H,
@@ -773,6 +885,114 @@ int backward(wn_handle* h, const float* grad_out, float* const* grads, float* co
     InputGrads ig;
     for (int i = 0; i < 4; i++) ig.p[i] = input_grads[i];
     input_grads_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(t.gin_a, t.gin_b, ig, hw);
+    WN_LAUNCH_CHECK(h);
+  }
+  return WN_OK;
+}
+
+// ---- the sub-modules under autograd (wn_confidence_maps_train / _backward, wn_refine_train / _backward) -----------
+// The training forward of one stack (bf16x3 and the exact-levels flag, as forward_train; a refiner's first layer is
+// kRL1, the refiners' conv1 without cmg.conv1) keeps its activations in a workspace carved for that stack.  The
+// backward seeds that stack's half of the backward pass from d(maps) or d(out) and writes the sub-module's own
+// parameter gradients and, on request, the gradients of its own inputs.
+static int check_submodule_args(int n, int H, int W, int stack, size_t bytes) {
+  if ((long long)n * H * W > kTrainMaxPixels) {
+    set_error("training pass limited to %lld pixels per call (got %lld)", kTrainMaxPixels, (long long)n * H * W);
+    return WN_E_UNSUPPORTED;
+  }
+  const size_t need = submodule_train_workspace_bytes(n, H, W, stack);
+  if (bytes < need) {
+    set_error("sub-module training workspace too small: %zu < %zu", bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  return WN_OK;
+}
+
+static bool any_of4(float* const* p, int count) {
+  if (!p) return false;
+  for (int i = 0; i < count; i++)
+    if (p[i]) return true;
+  return false;
+}
+
+int confidence_maps_train(wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out_maps, int n,
+                          int H, int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  int rc = check_submodule_args(n, H, W, kStackCmg, workspace_bytes);
+  if (rc) return rc;
+  TrainBuffers t;
+  carve(&t, workspace, (size_t)n * H * W, kStackCmg);
+  FwdOpts o;
+  o.stack = kStackCmg;
+  if ((rc = umma_forward_layers(h, in, st, nullptr, n, H, W, t.f, stream, o))) return rc;
+  WN_CUDA(cudaMemcpyAsync(out_maps, t.f.cm, (size_t)n * 3 * H * W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  return WN_OK;
+}
+
+int confidence_maps_backward(wn_handle* h, const float* grad_maps, float* const* grads, float* const* input_grads,
+                             int n, int H, int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!h->bwd) {
+    set_error("backward weights have not been packed");
+    return WN_E_STATE;
+  }
+  int rc = check_submodule_args(n, H, W, kStackCmg, workspace_bytes);
+  if (rc) return rc;
+  if ((rc = get_encoder())) return rc;
+  TrainBuffers t;
+  carve(&t, workspace, (size_t)n * H * W, kStackCmg);
+  const int hw = H * W;
+  const bool want_in = any_of4(input_grads, 4);
+  maps_bwd_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(grad_maps, t.f.cm, t.g8, hw);
+  WN_LAUNCH_CHECK(h);
+  if ((rc = backward_cmg(h, t, grads, want_in, n, H, W, stream))) return rc;
+  if (want_in) {
+    SubInputGrads ig;
+    for (int i = 0; i < 4; i++) {  // cat[x, wb, he, gc]: image i is packed channels 3i..3i+2
+      ig.p[i] = input_grads[i];
+      ig.slot[i] = i;
+    }
+    submodule_input_grads_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(t.gin_a, ig, hw);
+    WN_LAUNCH_CHECK(h);
+  }
+  return WN_OK;
+}
+
+int refine_train(wn_handle* h, int which, const float* const in[4], const int64_t st[4][4], float* out, int n, int H,
+                 int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  int rc = check_submodule_args(n, H, W, kStackRefiners, workspace_bytes);
+  if (rc) return rc;
+  TrainBuffers t;
+  carve(&t, workspace, (size_t)n * H * W, kStackRefiners);
+  FwdOpts o;
+  o.stack = kStackRefiners;
+  o.refiner_l1 = true;
+  if ((rc = umma_forward_layers(h, in, st, nullptr, n, H, W, t.f, stream, o))) return rc;
+  const size_t img = (size_t)3 * H * W * sizeof(float);
+  WN_CUDA(cudaMemcpy2DAsync(out, img, t.f.refined + (size_t)which * 3 * H * W, 3 * img, img, n,
+                            cudaMemcpyDeviceToDevice, stream));
+  return WN_OK;
+}
+
+int refine_backward(wn_handle* h, int which, const float* grad_out, float* const* grads, float* const* input_grads,
+                    int n, int H, int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!h->bwd) {
+    set_error("backward weights have not been packed");
+    return WN_E_STATE;
+  }
+  int rc = check_submodule_args(n, H, W, kStackRefiners, workspace_bytes);
+  if (rc) return rc;
+  if ((rc = get_encoder())) return rc;
+  TrainBuffers t;
+  carve(&t, workspace, (size_t)n * H * W, kStackRefiners);
+  const int hw = H * W;
+  const bool want_in = any_of4(input_grads, 2);
+  refine_bwd_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(grad_out, t.f.refined, t.gr3, which, hw);
+  WN_LAUNCH_CHECK(h);
+  if ((rc = backward_refiners(h, t, grads, which, want_in, n, H, W, stream))) return rc;
+  if (want_in) {
+    // refiner `which` reads cat[x, input which+1] (the forward handed xbar to all three slots; the other refiners'
+    // seeds are zero, so their rows of the first layer's data gradient add exact zeros)
+    SubInputGrads ig = {{input_grads[0], input_grads[1], nullptr, nullptr}, {0, which + 1, 0, 0}};
+    submodule_input_grads_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(t.gin_b, ig, hw);
     WN_LAUNCH_CHECK(h);
   }
   return WN_OK;

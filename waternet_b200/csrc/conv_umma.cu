@@ -115,6 +115,7 @@ enum UmmaLayer {
   kC8,        // 64 -> 3 (pad 16), sigmoid
   kR2,        // three refiner conv2 as one block-diagonal 96 -> 96, 5x5
   kR3,        // three refiner conv3 as block-diagonal 96 -> 9 (pad 16), ReLU, gated sum
+  kRL1,       // the three refiner conv1 alone (16 -> 96, 7x7): the training forward of a refiner (bf16x3 only)
   kNumUmmaLayers
 };
 // Everything a layer's launches and packed weights depend on (UmmaCfg in umma_conv.cuh).  npad = output columns
@@ -139,12 +140,13 @@ static constexpr UmmaLayerSpec kSpecs[kNumUmmaLayers] = {
     {3, 64, 64, kEpiAct, 1, 1, 9, 6, true, 2, 1},       // kC7
     {3, 64, 16, kEpiSigmoid, 1, 1, 9, 7, false, 1, 1},  // kC8
     {5, 96, 32, kEpiAct, 1, 3, 5, 9, true, 1, 1},       // kR2
-    {3, 96, 16, kEpiGate, 1, 1, 9, 10, false, 1, 1}};   // kR3
+    {3, 96, 16, kEpiGate, 1, 1, 9, 10, false, 1, 1},    // kR3
+    {7, 16, 96, kEpiAct, 0, 1, 1, 8, false, 1, 1}};     // kRL1 (CONCAT 0 as kL1: the same sums per channel)
 
 // In the fp8-correction scheme a layer writes the hi + fp8-planes format (FMT bit 1) when its consumers read it with
 // their fp8 form.  L1 feeds C2 and R2; every other layer feeds the next one, except the last layer of each stack.
 static_assert(kSpecs[kC2].f8 == kSpecs[kR2].f8, "L1 writes one format for both of its consumers");
-static constexpr bool writes_f8(int li) { return li != kC8 && li != kR3 && kSpecs[li + 1].f8; }
+static constexpr bool writes_f8(int li) { return li < kR3 && li != kC8 && kSpecs[li + 1].f8; }
 
 // out -> every peer address (the uint8 output of the last launch, the range guard's re-run -- then conditional on
 // *run_if like every launch of that chain)
@@ -209,7 +211,7 @@ int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t str
     auto scatter = [&](int conv, int co, int ci, int row_off, int split, int base0, int base1) -> int {
       // the first layer consumes image levels 0..255 (see pack_inputs_kernel): fold the /255 into its weights
       scatter_weights_kernel<<<128, 256, 0, stream>>>(W(conv), u->dense, co, ci, kk, s.cinpad, row_off, split,
-                                                      base0, base1, li == kL1 ? 255.0f : 1.0f);
+                                                      base0, base1, li == kL1 || li == kRL1 ? 255.0f : 1.0f);
       WN_LAUNCH_CHECK(h);
       scatter_bias_kernel<<<1, 256, 0, stream>>>(B(conv), u->bias[li], co, row_off);
       WN_LAUNCH_CHECK(h);
@@ -226,6 +228,8 @@ int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t str
       rc = scatter(conv, d.cout, d.cin, 0, d.cin, 0, 0);
     } else if (li == kR2) {
       for (int r = 0; r < 3 && !rc; r++) rc = scatter(8 + 3 * r + 1, 32, 32, 32 * r, 32, 32 * r, 0);
+    } else if (li == kRL1) {  // kL1's refiner rows, from row 0
+      for (int r = 0; r < 3 && !rc; r++) rc = scatter(8 + 3 * r, 32, 6, 32 * r, 3, 0, 3 * (r + 1));
     } else {
       for (int r = 0; r < 3 && !rc; r++) rc = scatter(8 + 3 * r + 2, 3, 32, 3 * r, 32, 32 * r, 0);
     }
@@ -411,11 +415,19 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
     }
   };
   const bool want_cmg = o.stack != kStackRefiners, want_ref = o.stack != kStackCmg;
-  // L1: 16 -> 128 (cmg) + 96 (refiners)
-  act(b.a[1], 128, b.r[1], 96);
   a.skip_lo = b.exact_flag;
   a.a_hi_only = o.hi_only ? 1 : 0;
-  if ((rc = launch_layer<kL1>(h, f8, b.act0, a, stream))) return rc;
+  if (o.refiner_l1) {  // the refiners' conv1 alone, bf16x3 (the sums of kL1's refiner columns)
+    constexpr UmmaLayerSpec s = kSpecs[kRL1];
+    act(b.r[1], 96, nullptr, 0);
+    rc = launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps, 0, false, s.mw, s.ng>(
+        h, s.slot, h->umma->stages[kRL1], h->umma->bias[kRL1], b.act0, a, stream);
+    if (rc) return rc;
+  } else {
+    // L1: 16 -> 128 (cmg) + 96 (refiners); the training forward of the cmg alone has no r[1] and stores 128
+    act(b.a[1], 128, b.r[1], b.r[1] ? 96 : 0);
+    if ((rc = launch_layer<kL1>(h, f8, b.act0, a, stream))) return rc;
+  }
   a.skip_lo = nullptr;
   a.a_hi_only = 0;
   if (dump(kL1)) return WN_OK;

@@ -337,6 +337,95 @@ class Engine:
                 torch._foreach_add_(grads, part)
         return (grads, gin) if want_input_grads else grads
 
+    # ---- the sub-modules under autograd (wn_confidence_maps_train / _backward, wn_refine_train / _backward) --------
+    STACK_CMG, STACK_REFINER = 0, 1
+
+    def _submodule_train(self, stack: int, ins, call, what: str):
+        """The batch in slices of at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES, one workspace per slice, as
+        ``forward_train``.  call(slice inputs, strides, slice output, n, h, w, workspace) -> rc."""
+        n, _, h, w = ins[0].shape
+        out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
+        if out.numel() == 0:
+            return out, None
+        if h * w > self.TRAIN_MAX_PIXELS:
+            raise _lib.WaterNetLibraryError(
+                f"{what}: one {h}x{w} image exceeds the {self.TRAIN_MAX_PIXELS} pixels of one training call")
+        per = min(self.TRAIN_MAX_IMAGES, max(1, self.TRAIN_MAX_PIXELS // (h * w)))
+        saved = []
+        for a in range(0, n, per):
+            b = min(n, a + per)
+            part = [t[a:b] for t in ins]
+            strides = (ctypes.c_int64 * (4 * len(part)))(*[s for t in part for s in t.stride()])
+            nbytes = self.lib.wn_submodule_train_workspace_bytes(b - a, h, w, stack)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            with torch.cuda.device(self.device):
+                rc = call(part, strides, out[a:b], b - a, h, w, ws)
+            _lib.check(rc, what)
+            saved.append((a, b, ws))
+        return out, saved
+
+    def _submodule_backward(self, grad, saved, shapes, first: int, want_inputs, call, what: str):
+        """The parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) added in slice order, and
+        the input gradients asked for by ``want_inputs`` (None where not).  call(grad slice, grads array, input grads
+        array or None, n, h, w, workspace) -> rc."""
+        g = grad.detach().to(self.device, torch.float32).contiguous()
+        n, _, h, w = g.shape
+        saved = saved or []
+        make = torch.empty if saved else torch.zeros  # an empty batch has zero gradients
+        grads = [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
+        part = grads if len(saved) <= 1 else [torch.empty_like(t) for t in grads]
+        gin = [torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) if want else None
+               for want in want_inputs]
+        for i, (a, b, ws) in enumerate(saved):
+            arr = (ctypes.c_void_p * _lib.NUM_PARAMS)()
+            for k, t in enumerate(grads if i == 0 else part):
+                arr[first + k] = t.data_ptr()
+            gin_arr = None
+            if any(want_inputs):
+                gin_arr = (ctypes.c_void_p * len(gin))(*[None if t is None else t[a:b].data_ptr() for t in gin])
+            with torch.cuda.device(self.device):
+                rc = call(g[a:b].data_ptr(), arr, gin_arr, b - a, h, w, ws)
+            _lib.check(rc, what)
+            if i > 0:
+                torch._foreach_add_(grads, part)
+        return grads, gin
+
+    def confidence_maps_train(self, x, wb, he, gc):
+        """``confidence_maps`` in the bf16x3 arithmetic of training, keeping the activations of the cmg stack
+        (wn_confidence_maps_train).  Returns (maps, saved workspaces) for ``confidence_maps_backward``."""
+        ins = self._check_inputs((x, wb, he, gc))
+        stream = _stream_ptr(self.device)
+        return self._submodule_train(self.STACK_CMG, ins, lambda p, st, o, n, h, w, ws: self.lib.wn_confidence_maps_train(
+            self.handle, p[0].data_ptr(), p[1].data_ptr(), p[2].data_ptr(), p[3].data_ptr(), st, o.data_ptr(), n, h, w,
+            ws.data_ptr(), ws.numel(), stream), "wn_confidence_maps_train")
+
+    def confidence_maps_backward(self, grad_maps, saved, shapes, want_inputs=(False,) * 4):
+        """d(loss)/d(maps) + the workspaces of ``confidence_maps_train`` -> the 16 cmg parameter gradients
+        (state-dict order) and the gradients of x, wb, he, gc where ``want_inputs`` asks for them (else None)."""
+        stream = _stream_ptr(self.device)
+        return self._submodule_backward(grad_maps, saved, shapes, 0, want_inputs, lambda g, arr, gin, n, h, w, ws:
+                                        self.lib.wn_confidence_maps_backward(self.handle, g, arr, gin, n, h, w,
+                                                                             ws.data_ptr(), ws.numel(), stream),
+                                        "wn_confidence_maps_backward")
+
+    def refine_train(self, which: int, x, xbar):
+        """``refine`` in the bf16x3 arithmetic of training, keeping the activations of the refiner stack
+        (wn_refine_train).  Returns (out, saved workspaces) for ``refine_backward``."""
+        ins = self._check_inputs((x, xbar))
+        stream = _stream_ptr(self.device)
+        return self._submodule_train(self.STACK_REFINER, ins, lambda p, st, o, n, h, w, ws: self.lib.wn_refine_train(
+            self.handle, int(which), p[0].data_ptr(), p[1].data_ptr(), st, o.data_ptr(), n, h, w, ws.data_ptr(),
+            ws.numel(), stream), "wn_refine_train")
+
+    def refine_backward(self, which: int, grad_out, saved, shapes, want_inputs=(False, False)):
+        """d(loss)/d(out) + the workspaces of ``refine_train`` -> the 6 parameter gradients of refiner ``which``
+        (state-dict order) and the gradients of x, xbar where ``want_inputs`` asks for them (else None)."""
+        stream = _stream_ptr(self.device)
+        return self._submodule_backward(grad_out, saved, shapes, 16 + 6 * int(which), want_inputs,
+                                        lambda g, arr, gin, n, h, w, ws: self.lib.wn_refine_backward(
+                                            self.handle, int(which), g, arr, gin, n, h, w, ws.data_ptr(), ws.numel(),
+                                            stream), "wn_refine_backward")
+
     # ---- preprocess / postprocess ----------------------------------------------
     def preprocess(self, rgb_u8: torch.Tensor, tensors: bool = True, images: bool = False):
         """rgb_u8: uint8 (N,H,W,3) CUDA tensor.  Returns dict with the requested outputs.

@@ -13,6 +13,9 @@ reference's checkpoints load with strict ``load_state_dict`` and callers
   ``wn_backward``: tensor-core data-gradient and weight-gradient kernels), including
   gradients of the input images when they require grad.  Only the fp32 CUDA-core mode
   re-evaluates the network with torch ops for its backward pass.
+* The sub-modules (``model.cmg``, the refiners, free-standing instances) train on the library
+  the same way (``wn_confidence_maps_train`` / ``wn_refine_train`` and their backward), with
+  gradients for their own parameters and inputs only.
 """
 from __future__ import annotations
 
@@ -90,8 +93,10 @@ class _PackedWeightsMixin:
         self.invalidate_packed_weights()
         return out
 
-    def _engine_for(self, x, params):
-        """This module's private engine on x's device with ``params`` (34 tensors, state-dict order) packed."""
+    def _engine_for(self, x, params, key_params=None):
+        """This module's private engine on x's device with ``params`` (34 tensors, state-dict order) packed.  The
+        cache key is taken over ``key_params`` when given (a free-standing stack: its own parameters, not the zeros
+        that fill the other slots)."""
         if not x.is_cuda:
             raise _lib.WaterNetLibraryError(
                 f"{type(self).__name__}.forward got CPU tensors: waternet_b200 has no CPU path; move the model and "
@@ -103,7 +108,8 @@ class _PackedWeightsMixin:
             eng = per_dev.get(x.device.index)
             if eng is None:
                 eng = per_dev[x.device.index] = new_engine(x.device)
-        key = (getattr(self, "_pack_epoch", 0),) + tuple((p.data_ptr(), _param_version(p)) for p in params)
+        key = (getattr(self, "_pack_epoch", 0),) + tuple((p.data_ptr(), _param_version(p))
+                                                         for p in (params if key_params is None else key_params))
         eng.pack_weights(params, key=key)
         return eng
 
@@ -122,9 +128,14 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
     Like the reference's sub-modules (``net.py:45-56``, ``:75-80``) a stack can be called on its own.  Inside a
     ``WaterNet`` it runs with the parent's packed state dict (``wn_confidence_maps`` / ``wn_refine``); a
     free-standing instance packs its own tensors into the state-dict slots of its kind, zeros elsewhere.
-    Sub-module calls are inference entry points: with autograd recording they evaluate the torch graph instead
-    (the fused training path is ``WaterNet.forward``).  Bound to a ``WaterNet`` a stack follows the parent's
-    ``precision`` and ``tile``; a free-standing one uses its own attributes.
+    With autograd recording (a parameter or an input requires grad) a call on CUDA tensors in a tensor-core
+    precision trains natively: the forward runs in the bf16x3 arithmetic of training and keeps the stack's
+    activations (``wn_confidence_maps_train`` / ``wn_refine_train``), and backward gives the gradients of the stack's
+    own parameters and of its inputs (``wn_confidence_maps_backward`` / ``wn_refine_backward``).  Nothing reaches the
+    parent's other parameters.  Whole images per call (``tile`` and ``grad_tile`` do not apply), at most
+    ``Engine.TRAIN_MAX_PIXELS`` pixels per image; a batch over that runs in slices.  CPU tensors,
+    ``precision="fp32"`` and a larger image evaluate the torch graph instead.  Bound to a ``WaterNet`` a stack
+    follows the parent's ``precision`` and ``tile``; a free-standing one uses its own attributes.
     """
 
     spec: List[tuple] = []
@@ -177,11 +188,58 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
         mode = MODES[self.precision]
         tile = _checked_tile(self.tile, mode)
         own = self._own_params()
-        return mode, self._engine_for(x, zero_layout(own)), 0, tile
+        return mode, self._engine_for(x, zero_layout(own), key_params=own), 0, tile
+
+    def _train_engine(self, x):
+        """(engine with the right state dict packed, slot) for a call that records an autograd graph, or None where
+        the torch graph runs instead: CPU tensors, precision "fp32", or one image over Engine.TRAIN_MAX_PIXELS."""
+        if not x.is_cuda or x.shape[2] * x.shape[3] > Engine.TRAIN_MAX_PIXELS:
+            return None
+        parent = self._parent_ref() if self._parent_ref is not None else None
+        if parent is not None:
+            if parent._mode() == _lib.MODE_FP32_SIMT:
+                return None
+            return parent._engine_with_weights(x), self._slot
+        if self.precision not in MODES:
+            raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(MODES)}")
+        if MODES[self.precision] == _lib.MODE_FP32_SIMT:
+            return None
+        own = self._own_params()
+        return self._engine_for(x, self._zero_layout(own), key_params=own), 0
 
     @staticmethod
     def _needs_graph(tensors, params):
         return torch.is_grad_enabled() and (any(t.requires_grad for t in tensors) or any(p.requires_grad for p in params))
+
+
+class _SubmoduleForward(torch.autograd.Function):
+    """A sub-module called on its own under autograd: forward values and gradients from the CUDA library
+    (wn_confidence_maps_train / _backward for the cmg, wn_refine_train / _backward for a refiner), in the bf16x3
+    arithmetic of training.  It receives the stack's own 16 or 6 parameters, so autograd routes gradients to them and
+    to nothing else.  which: None for the cmg, else the refiner slot (0 wb, 1 ce, 2 gc) of the packed state dict."""
+
+    @staticmethod
+    def forward(ctx, eng, which, n_in, *tensors):
+        ins, params = tensors[:n_in], tensors[n_in:]
+        ctx.engine, ctx.which, ctx.n_in = eng, which, n_in
+        ctx.weights_key = eng._weights_key
+        ctx.shapes = [p.shape for p in params]
+        out, ctx.saved_ws = eng.confidence_maps_train(*ins) if which is None else eng.refine_train(which, *ins)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        eng = ctx.engine
+        if eng._weights_key != ctx.weights_key:
+            raise RuntimeError("sub-module parameters were modified between forward and backward")
+        need = ctx.needs_input_grad[3:]
+        want_in, want_par = need[:ctx.n_in], need[ctx.n_in:]
+        if ctx.which is None:
+            grads, gin = eng.confidence_maps_backward(grad, ctx.saved_ws, ctx.shapes, want_in)
+        else:
+            grads, gin = eng.refine_backward(ctx.which, grad, ctx.saved_ws, ctx.shapes, want_in)
+        ctx.saved_ws = None
+        return (None, None, None, *gin, *[g if w else None for g, w in zip(grads, want_par)])
 
 
 def _zeros_like_spec(spec, ref):
@@ -204,13 +262,20 @@ class ConfidenceMapGenerator(_ConvStack):
             out = F.relu(conv(out))
         return torch.sigmoid(layers[-1](out))
 
+    @staticmethod
+    def _zero_layout(own):
+        return own + 3 * _zeros_like_spec(REFINER_SPEC, own[0])
+
     def forward(self, x, wb, ce, gc):
         """Returns the three (N,1,H,W) maps ``out1, out2, out3`` like ``net.py:55-56``."""
         if self._needs_graph((x, wb, ce, gc), self._own_params()):
-            maps = self._graph(x, wb, ce, gc)
+            native = self._train_engine(x)
+            if native is None:
+                maps = self._graph(x, wb, ce, gc)
+            else:
+                maps = _SubmoduleForward.apply(native[0], None, 4, x, wb, ce, gc, *self._own_params())
         else:
-            mode, eng, _, tile = self._mode_and_engine(
-                x, lambda own: own + 3 * _zeros_like_spec(REFINER_SPEC, own[0]))
+            mode, eng, _, tile = self._mode_and_engine(x, self._zero_layout)
             if tile is None:
                 maps = eng.confidence_maps(x, wb, ce, gc, mode)
             else:
@@ -229,11 +294,18 @@ class Refiner(_ConvStack):
             out = F.relu(conv(out))
         return out
 
+    @staticmethod
+    def _zero_layout(own):  # a free-standing refiner runs in slot 0 (wb_refiner)
+        return _zeros_like_spec(CMG_SPEC, own[0]) + own + 2 * _zeros_like_spec(REFINER_SPEC, own[0])
+
     def forward(self, x, xbar):
         if self._needs_graph((x, xbar), self._own_params()):
-            return self._graph(x, xbar)
-        mode, eng, slot, tile = self._mode_and_engine(
-            x, lambda own: _zeros_like_spec(CMG_SPEC, own[0]) + own + 2 * _zeros_like_spec(REFINER_SPEC, own[0]))
+            native = self._train_engine(x)
+            if native is None:
+                return self._graph(x, xbar)
+            eng, slot = native
+            return _SubmoduleForward.apply(eng, slot, 2, x, xbar, *self._own_params())
+        mode, eng, slot, tile = self._mode_and_engine(x, self._zero_layout)
         if tile is None:
             return eng.refine(slot, x, xbar, mode)
         return eng.refine_tiled(slot, x, xbar, tile, mode)
