@@ -332,7 +332,8 @@ int wn_read_timings(wn_handle* h, float* ms, int* count);
  * Test aid: run wn_forward's layer chain in `mode` up to an intermediate activation and return it
  * as contiguous fp32 NCHW.  layer: 0..6 = output of cmg.conv1..conv7 (after ReLU), 7 = the three
  * sigmoid confidence maps, 8 = the three refiners' conv1 outputs concatenated (96 channels),
- * 9 = their conv2 outputs (96 channels).  dst must hold n*C*h*w floats.  Workspace as wn_forward.
+ * 9 = their conv2 outputs (96 channels), 10 = the three refined images (conv3 after ReLU, before the
+ * gate; 9 channels, 3r..3r+2 for refiner r).  dst must hold n*C*h*w floats.  Workspace as wn_forward.
  */
 int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const float* he,
                            const float* gc, const int64_t in_strides[4][4], int n, int height,

@@ -70,6 +70,19 @@ def test_null_arguments_are_rejected_without_a_gpu(lib):
     assert lib.wn_set_chunk_pixels(None, 0) != 0
 
 
+def test_debug_layer_bound(lib):
+    """wn_debug_forward_layer numbers the launch outputs 0..10 (10: the three refined images, Engine.LAYER_CHANNELS);
+    the layer is checked before anything else, so the bound shows without a device."""
+    from waternet_b200.engine import Engine
+    assert Engine.LAYER_CHANNELS == (128, 128, 128, 64, 64, 64, 64, 3, 96, 96, 9)
+    call = lambda layer: lib.wn_debug_forward_layer(None, None, None, None, None, None, 1, 1, 1, 0, layer, None, None,
+                                                    0, None)
+    for layer in (-1, 11):
+        assert call(layer) != 0 and b"not in 0..10" in lib.wn_last_error()
+    for layer in (0, 10):
+        assert call(layer) != 0 and b"bad argument" in lib.wn_last_error()
+
+
 def test_state_dict_is_reference_compatible():
     from waternet_b200.net import WaterNet
     m = WaterNet()

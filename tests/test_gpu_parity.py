@@ -1001,28 +1001,6 @@ def test_many_tiles_per_cta_default_mode():
         _assert_close(out, ofw.waternet_forward(sd, *ins, dtype=torch.float64).numpy())
 
 
-@pytest.mark.parametrize("precision", TC_MODES)
-def test_debug_layers_match_fp32_path(precision):
-    """wn_debug_forward_layer decodes every intermediate activation of the tensor-core chain (bf16 hi/lo planes, or
-    hi + fp8 planes where the consumer has an fp8 form); each matches the fp32 CUDA-core path's, at a ragged shape
-    and at one with many tiles per CTA."""
-    from waternet_b200 import _lib
-    m = _model(8, 3.0, precision)
-    eng = m.engine()
-    mode = m._mode()
-    for n, h, w in [(2, 37, 53), (1, 300, 500)]:
-        torch.manual_seed(h * w)
-        cu = [torch.rand(n, 3, h, w).cuda() for _ in range(4)]
-        errs = []
-        for layer in range(10):
-            want = eng.debug_layer(*cu, layer=layer, mode=_lib.MODE_FP32_SIMT).cpu().numpy().astype(np.float64)
-            got = eng.debug_layer(*cu, layer=layer, mode=mode).cpu().numpy()
-            assert got.shape == want.shape == (n, eng.LAYER_CHANNELS[layer], h, w)
-            errs.append(float(np.max(np.abs(got - want)) / np.max(np.abs(want))))
-        print(f"{precision} {(n, h, w)} max rel err per layer:", " ".join(f"{e:.2e}" for e in errs))
-        assert max(errs) <= REL_TOL, errs
-
-
 def test_native_backward_is_bit_reproducible():
     """The weight-gradient GEMM merges its per-CTA partial sums in a fixed order (no atomics): two backward passes
     over the same batch give bit-identical gradients."""

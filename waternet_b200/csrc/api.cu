@@ -862,7 +862,11 @@ int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const 
                            const float* gc, const int64_t in_strides[4][4], int n, int height,
                            int width, int mode, int layer, float* dst, void* workspace,
                            size_t workspace_bytes, void* stream) {
-  if (!h || !x || !wb || !he || !gc || !in_strides || !dst || !workspace || layer < 0 || layer > 9) {
+  if (layer < 0 || layer > 10) {
+    set_error("wn_debug_forward_layer: layer %d is not in 0..10", layer);
+    return WN_E_INVALID;
+  }
+  if (!h || !x || !wb || !he || !gc || !in_strides || !dst || !workspace) {
     set_error("wn_debug_forward_layer: bad argument");
     return WN_E_INVALID;
   }

@@ -356,6 +356,10 @@ static int simt_forward_chunk(wn_handle* h, const float* const in[4],
       continue;
     }
     if ((rc = run_conv(h, 8 + 3 * r + 2, r32b, refr, n, H, W, 1, stream))) return rc;
+    if (dbg_layer == 10)  // (N,3,H,W) -> channels 3r.. of (N,9,H,W)
+      WN_CUDA(cudaMemcpy2DAsync(dbg_dst + (size_t)r * 3 * plane, (size_t)9 * plane * sizeof(float), refr,
+                                (size_t)3 * plane * sizeof(float), (size_t)3 * plane * sizeof(float), n,
+                                cudaMemcpyDeviceToDevice, stream));
   }
   if (dbg_layer >= 0 || stack == kStackRefiners) return WN_OK;
   TimedScope ts(h, kSlotGate, stream);

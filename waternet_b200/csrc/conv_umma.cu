@@ -461,7 +461,16 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   if ((rc = launch_layer<kR2>(h, f8, b.r[1], a, stream))) return rc;
   if (dump(kR2)) return WN_OK;
   last();
+  // a dump of the refined images (number 10): the same launch with no gate, storing them alone
+  const bool dump_refined = dbg_layer == kSpecs[kR3].slot;
+  if (dump_refined) {
+    a.out_f32 = nullptr;
+    a.out_u8 = nullptr;
+    a.cm = nullptr;
+    a.refined_out = dbg_dst;
+  }
   if ((rc = launch_layer<kR3>(h, f8, b.r[2], a, stream))) return rc;
+  if (dump_refined) return WN_OK;
   return o.out_u8 ? mirror_u8(h, o.out_u8, o.peers, (size_t)n * H * W * 3, o.run_if, stream) : WN_OK;
 }
 

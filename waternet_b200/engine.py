@@ -262,7 +262,7 @@ class Engine:
         _lib.check(rc, "wn_refine")
         return out
 
-    LAYER_CHANNELS = (128, 128, 128, 64, 64, 64, 64, 3, 96, 96)
+    LAYER_CHANNELS = (128, 128, 128, 64, 64, 64, 64, 3, 96, 96, 9)
 
     def debug_layer(self, x, wb, he, gc, layer: int, mode: int) -> torch.Tensor:
         """Test aid (wn_debug_forward_layer): an intermediate activation as fp32 (N,C,H,W)."""
