@@ -27,6 +27,8 @@
  *   wn_backward_tiled     the same gradients from the inputs alone, recomputed in overlapping windows
  *   wn_confidence_maps_train / _backward, wn_refine_train / _backward
  *                         the sub-modules under autograd (net.py:45-56, :75-80 with parameters that require grad)
+ *   wn_confidence_maps_backward_tiled, wn_refine_backward_tiled
+ *                         their gradients from the inputs alone, recomputed in overlapping windows
  *
  * Conventions: every data pointer is a DEVICE pointer on the handle's device
  * unless its name ends in _host; the caller owns every buffer (the handle only
@@ -45,7 +47,7 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 9
+#define WN_ABI_VERSION 10
 
 #define WN_OK 0
 #define WN_E_INVALID (-1)   /* bad argument (NULL pointer, non-positive size, unknown mode) */
@@ -315,6 +317,33 @@ int wn_backward_tiled(wn_handle* h, const float* x, const float* wb, const float
                       const int64_t in_strides[4][4], const float* grad_out, float* const* grads,
                       float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
                       long long max_pass_pixels, void* workspace, size_t workspace_bytes, void* stream);
+
+/*
+ * The windowed recompute backward of one sub-module: the gradients wn_confidence_maps_backward / wn_refine_backward
+ * give, from the sub-module's inputs alone, in memory that does not grow with the image size.  The windows, the
+ * recomputed WN_MODE_BF16X3 training forward (of that stack alone, as wn_confidence_maps_train / wn_refine_train run
+ * it) and the exactness argument are those of wn_backward_tiled; a refiner's receptive-field radius (6) is within
+ * the windows' 13 pixels of context.
+ *   - x, wb, he, gc / x, xbar, in_strides: as wn_confidence_maps_tiled / wn_refine_tiled.  grad_maps / grad_out:
+ *     fp32 contiguous (N,3,H,W) of the full images.
+ *   - grads, input_grads: as wn_confidence_maps_backward / wn_refine_backward (only the stack's own entries of grads
+ *     are overwritten, the others may be NULL; input_grads NULL or 4 / 2 pointers, any of them NULL).
+ *   - max_pass_pixels and the size limits: as wn_backward_tiled.  stack: 0 = confidence maps, 1 = refiner.  At the
+ *     default pass of 2 Mi window pixels the workspace is at most ~8.1 GB for the cmg and ~3.9 GB for a refiner.
+ *   - Deterministic, no atomics; input gradients are folded in window order and do not depend on max_pass_pixels.
+ *   - Nothing is copied from the host: a call can be captured in a CUDA graph.
+ * wn_submodule_backward_tiled_workspace_bytes returns 0 for every argument set the calls reject.
+ */
+size_t wn_submodule_backward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w,
+                                                   long long max_pass_pixels, int stack);
+int wn_confidence_maps_backward_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                                      const int64_t in_strides[4][4], const float* grad_maps, float* const* grads,
+                                      float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
+                                      long long max_pass_pixels, void* workspace, size_t workspace_bytes, void* stream);
+int wn_refine_backward_tiled(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
+                             const float* grad_out, float* const* grads, float* const* input_grads, int n, int height,
+                             int width, int tile_h, int tile_w, long long max_pass_pixels, void* workspace,
+                             size_t workspace_bytes, void* stream);
 
 /*
  * Per-kernel device timing (measurement aid for bench.py, off by default).  When on, every

@@ -19,7 +19,7 @@ MODE_BF16_FP8 = 2
 MODE_DEFAULT = -1
 NUM_PARAMS = 34
 NUM_TIMING_SLOTS = 23
-ABI_VERSION = 9
+ABI_VERSION = 10
 PEER_HANDLE_BYTES = 64  # WN_PEER_HANDLE_BYTES
 MAX_PEERS = 15          # WN_MAX_PEERS
 
@@ -105,6 +105,14 @@ _SIGNATURES = {
     "wn_backward_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p,
                                   POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int,
                                   ctypes.c_longlong, c_void_p, c_size_t, c_void_p]),
+    "wn_submodule_backward_tiled_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong,
+                                                               c_int]),
+    "wn_confidence_maps_backward_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64),
+                                                  c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_int,
+                                                  c_int, c_int, ctypes.c_longlong, c_void_p, c_size_t, c_void_p]),
+    "wn_refine_backward_tiled": (c_int, [c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int64), c_void_p,
+                                         POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int,
+                                         ctypes.c_longlong, c_void_p, c_size_t, c_void_p]),
     "wn_debug_forward_layer": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int,
                                        c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "wn_enable_timing": (c_int, [c_void_p, c_int]),

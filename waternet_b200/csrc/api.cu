@@ -858,6 +858,77 @@ int wn_backward_tiled(wn_handle* h, const float* x, const float* wb, const float
                         max_pass_pixels, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
+// ---- the windowed recompute backward of one sub-module: the limits of wn_backward_tiled
+size_t wn_submodule_backward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w,
+                                                   long long max_pass_pixels, int stack) {
+  if ((stack != 0 && stack != 1) ||
+      backward_tiled_check("wn_submodule_backward_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels))
+    return 0;
+  return submodule_backward_tiled_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels,
+                                                  stack == 0 ? kStackCmg : kStackRefiners);
+}
+
+int wn_confidence_maps_backward_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
+                                      const int64_t in_strides[4][4], const float* grad_maps, float* const* grads,
+                                      float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
+                                      long long max_pass_pixels, void* workspace, size_t workspace_bytes,
+                                      void* stream) {
+  const char* what = "wn_confidence_maps_backward_tiled";
+  if (!h || !x || !wb || !he || !gc || !in_strides || !grad_maps || !grads || !workspace) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  for (int i = 0; i < 16; i++)
+    if (!grads[i]) {
+      set_error("%s: grads[%d] is NULL", what, i);
+      return WN_E_INVALID;
+    }
+  int rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  const float* in[4] = {x, wb, he, gc};
+  return submodule_backward_tiled(h, kStackCmg, 0, in, in_strides, grad_maps, grads, input_grads, n, height, width,
+                                  tile_h, tile_w, max_pass_pixels, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int wn_refine_backward_tiled(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
+                             const float* grad_out, float* const* grads, float* const* input_grads, int n, int height,
+                             int width, int tile_h, int tile_w, long long max_pass_pixels, void* workspace,
+                             size_t workspace_bytes, void* stream) {
+  const char* what = "wn_refine_backward_tiled";
+  if (which < 0 || which > 2) {
+    set_error("%s: which must be 0, 1 or 2, got %d", what, which);
+    return WN_E_INVALID;
+  }
+  if (!h || !x || !xbar || !in_strides || !grad_out || !grads || !workspace) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  for (int i = 16 + 6 * which; i < 22 + 6 * which; i++)
+    if (!grads[i]) {
+      set_error("%s: grads[%d] is NULL", what, i);
+      return WN_E_INVALID;
+    }
+  int rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  // as wn_refine_train: refiner r sees cat[x, input r+1], so xbar goes to every slot
+  const float* in[4] = {x, xbar, xbar, xbar};
+  int64_t st[4][4];
+  for (int t = 0; t < 4; t++)
+    for (int k = 0; k < 4; k++) st[t][k] = in_strides[t == 0 ? 0 : 1][k];
+  return submodule_backward_tiled(h, kStackRefiners, which, in, st, grad_out, grads, input_grads, n, height, width,
+                                  tile_h, tile_w, max_pass_pixels, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const float* he,
                            const float* gc, const int64_t in_strides[4][4], int n, int height,
                            int width, int mode, int layer, float* dst, void* workspace,

@@ -281,5 +281,14 @@ size_t backward_tiled_workspace_bytes(int n, int height, int width, int tile_h, 
 int backward_tiled(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], const float* grad_out,
                    float* const* grads, float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
                    long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+// ... of one sub-module (stack kStackCmg, or kStackRefiners with refiner `which`); arguments checked by the caller.
+// in: the stack's four packed inputs ({x, wb, he, gc}, or {x, xbar, xbar, xbar} for a refiner); grad: d(maps) or
+// d(out); grads: the 34-entry layout, the stack's own entries written; input_grads: NULL or 4 / 2 entries, any NULL
+size_t submodule_backward_tiled_workspace_bytes(int n, int height, int width, int tile_h, int tile_w,
+                                                long long max_pass_pixels, int stack);
+int submodule_backward_tiled(wn_handle* h, int stack, int which, const float* const in[4],
+                             const int64_t in_strides[4][4], const float* grad, float* const* grads,
+                             float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
+                             long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace wn

@@ -355,6 +355,65 @@ gate_bwd_tiled_kernel(const float* __restrict__ g_out, const float* __restrict__
   gate_bwd_pixel(go, cm, refined, g8, gr3, blockIdx.y, pix, hw);
 }
 
+// The windowed forms of maps_bwd_kernel / refine_bwd_kernel (wn_confidence_maps_backward_tiled,
+// wn_refine_backward_tiled), as gate_bwd_tiled_kernel is of gate_bwd_kernel: d(maps) or d(out) is read from the full
+// images (contiguous NCHW) at the window's kept pixels and is 0 elsewhere.
+__global__ void __launch_bounds__(256)
+maps_bwd_tiled_kernel(const float* __restrict__ g_maps, const float* __restrict__ cm, uint4* __restrict__ g8,
+                      TileGeom tiles, long long win0) {
+  const int hw = tiles.win_h * tiles.win_w;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
+  const int wy = pix / tiles.win_w;
+  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
+  const bool kept = y >= t.ky0 && y < t.ky1 && x >= t.kx0 && x < t.kx1;
+  const size_t ihw = (size_t)tiles.H * tiles.W;
+  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
+  float v8[16];
+#pragma unroll
+  for (int j = 0; j < 16; j++) v8[j] = 0.f;
+#pragma unroll
+  for (int r = 0; r < 3; r++) {
+    const float c = cm[((size_t)blockIdx.y * 3 + r) * hw + pix];
+    const float gm = kept ? g_maps[o + r * ihw] : 0.f;
+    v8[r] = gm * c * (1.0f - c);
+  }
+  store_grad16(g8, v8, blockIdx.y, pix, hw);
+}
+
+__global__ void __launch_bounds__(256)
+refine_bwd_tiled_kernel(const float* __restrict__ g_out, const float* __restrict__ refined, uint4* __restrict__ gr3,
+                        int which, TileGeom tiles, long long win0) {
+  const int hw = tiles.win_h * tiles.win_w;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
+  const int wy = pix / tiles.win_w;
+  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
+  const bool kept = y >= t.ky0 && y < t.ky1 && x >= t.kx0 && x < t.kx1;
+  const size_t ihw = (size_t)tiles.H * tiles.W;
+  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
+  float go[3], v9[16];
+#pragma unroll
+  for (int c = 0; c < 3; c++) go[c] = kept ? g_out[o + c * ihw] : 0.f;
+#pragma unroll
+  for (int j = 0; j < 16; j++) v9[j] = 0.f;
+#pragma unroll
+  for (int r = 0; r < 3; r++) {
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      float v = 0.f;
+      if (r == which) {
+        const float rf = refined[((size_t)blockIdx.y * 9 + 3 * r + c) * hw + pix];
+        v = rf > 0.f ? go[c] : 0.f;
+      }
+      v9[3 * r + c] = v;
+    }
+  }
+  store_grad16(gr3, v9, blockIdx.y, pix, hw);
+}
+
 // data-gradient weights: dense_d[row_off + c][col(o)][kk-1-t] = W[o][c][t]   (transpose + spatial flip)
 // input channel c lands in row  row_off + c  (c < split)  or  row_off + c + shift  (c >= split)
 __global__ void scatter_weights_T_kernel(const float* __restrict__ src, float* __restrict__ dense, int co, int ci,
@@ -492,6 +551,76 @@ fold_input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ 
   for (int q = 0; q < 4; q++)
 #pragma unroll
     for (int ch = 0; ch < 3; ch++) out.p[q][o + ch * ihw] = acc[q * 3 + ch];
+}
+
+// The windowed form of submodule_input_grads_kernel (wn_confidence_maps_backward_tiled, wn_refine_backward_tiled):
+// the one 32-channel buffer g of the pass's windows, folded into the full images out.p[t] (NULL: skipped) in the
+// order of fold_input_grads_kernel: the first covering window of the pass adds the contributions of all of them, in
+// ascending window index, to what earlier passes left.  No atomics.
+__device__ __forceinline__ void sub_input_grads_pixel(const uint4* __restrict__ g, int n, int pix, int hw, float* v) {
+#pragma unroll
+  for (int j = 0; j < 16; j++) v[j] = 0.f;
+#pragma unroll
+  for (int plane = 0; plane < 2; plane++)
+#pragma unroll
+    for (int half = 0; half < 2; half++) {
+      const uint4 q = g[((size_t)n * 8 + half * 4 + plane) * hw + pix];
+      const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+      for (int j = 0; j < 8; j++) v[plane * 8 + j] += __uint_as_float(((w[j >> 1] >> ((j & 1) * 16)) & 0xffffu) << 16);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+fold_submodule_input_grads_kernel(const uint4* __restrict__ g, SubInputGrads out, TileGeom tiles, long long w0,
+                                  int count) {
+  const int hw = tiles.win_h * tiles.win_w;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const long long me = w0 + blockIdx.y;
+  const TileWindow t = tile_window(tiles, me);
+  const int wy = pix / tiles.win_w;
+  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
+  const TileCover c = tile_cover(tiles, y, x);
+  const long long img0 = (long long)t.img * tiles.ny * tiles.nx;
+  long long first = -1;
+  for (int i = c.i0; i <= c.i1 && first < 0; i++)
+    for (int j = c.j0; j <= c.j1; j++) {
+      const long long k = img0 + (long long)i * tiles.nx + j;
+      if (k >= w0 && k < w0 + count) {
+        first = k;
+        break;
+      }
+    }
+  if (first != me) return;
+  const size_t ihw = (size_t)tiles.H * tiles.W;
+  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
+  float acc[12];
+#pragma unroll
+  for (int q = 0; q < 4; q++)
+#pragma unroll
+    for (int ch = 0; ch < 3; ch++) acc[q * 3 + ch] = out.p[q] ? out.p[q][o + ch * ihw] : 0.f;
+  for (int i = c.i0; i <= c.i1; i++)
+    for (int j = c.j0; j <= c.j1; j++) {
+      const long long k = img0 + (long long)i * tiles.nx + j;
+      if (k < w0 || k >= w0 + count) continue;
+      const TileWindow u = tile_window(tiles, k);
+      float v[16];
+      sub_input_grads_pixel(g, (int)(k - w0), (y - u.ys) * tiles.win_w + (x - u.xs), hw, v);
+#pragma unroll
+      for (int q = 0; q < 4; q++) {
+        const int s = out.slot[q];
+#pragma unroll
+        for (int ch = 0; ch < 3; ch++)  // constant indices into v
+          acc[q * 3 + ch] += s == 0 ? v[ch] : s == 1 ? v[3 + ch] : s == 2 ? v[6 + ch] : v[9 + ch];
+      }
+    }
+#pragma unroll
+  for (int q = 0; q < 4; q++) {
+    if (!out.p[q]) continue;
+#pragma unroll
+    for (int ch = 0; ch < 3; ch++) out.p[q][o + ch * ihw] = acc[q * 3 + ch];
+  }
 }
 
 // dst.p[k][i] += src.p[k][i] for the 34 parameter gradients; blockIdx.y = k
@@ -1099,6 +1228,119 @@ int backward_tiled(wn_handle* h, const float* const in[4], const int64_t st[4][4
     if (input_grads) {
       fold_input_grads_kernel<<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(t.gin_a, t.gin_b, ig,
                                                                                                 g, w0, cur);
+      WN_LAUNCH_CHECK(h);
+    }
+  }
+  return WN_OK;
+}
+
+// ---- windowed recompute backward of one sub-module (wn_confidence_maps_backward_tiled, wn_refine_backward_tiled) --
+// The pass loop of backward_tiled for one stack: the windows are those of the same rule (kTileHalo = 13 for both
+// stacks; a refiner's receptive-field radius is 6), each pass recomputes that stack's training forward (a refiner's
+// first layer is kRL1, as in refine_train), seeds it from d(maps) or d(out) inside the kept rectangles, runs that
+// stack's half of the backward and folds its input gradients.  Parameter gradients: the first pass writes the stack's
+// own entries of grads, every later pass writes a scratch copy of them that add_param_grads_kernel adds in.
+// Workspace: [flag | scratch copy of the stack's parameter gradients | one pass of carve(stack)].
+static void stack_params(int stack, int which, int* first, int* count) {
+  *first = stack == kStackCmg ? 0 : 16 + 6 * which;
+  *count = stack == kStackCmg ? 16 : 6;
+}
+
+static size_t stack_param_grads_bytes(int stack) {
+  int size[WN_NUM_PARAMS], first, count;
+  param_grad_sizes(size);
+  stack_params(stack, 0, &first, &count);  // the three refiners have the same shapes
+  size_t b = 0;
+  for (int k = first; k < first + count; k++) b += ((size_t)size[k] * sizeof(float) + 255) / 256 * 256;
+  return b;
+}
+
+size_t submodule_backward_tiled_workspace_bytes(int n, int H, int W, int tile_h, int tile_w, long long max_pass_pixels,
+                                                int stack) {
+  const TileGeom g = tile_geom(H, W, tile_h, tile_w);
+  const long long p = tiled_train_pass(g, n, max_pass_pixels);
+  return 256 + stack_param_grads_bytes(stack) + submodule_train_workspace_bytes((int)p, g.win_h, g.win_w, stack) + 256;
+}
+
+int submodule_backward_tiled(wn_handle* h, int stack, int which, const float* const in[4], const int64_t st[4][4],
+                             const float* grad, float* const* grads, float* const* input_grads, int n, int H, int W,
+                             int tile_h, int tile_w, long long max_pass_pixels, void* workspace, size_t workspace_bytes,
+                             cudaStream_t stream) {
+  if (!h->bwd || !h->umma) {
+    set_error("backward weights have not been packed");
+    return WN_E_STATE;
+  }
+  const size_t need = submodule_backward_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels, stack);
+  if (workspace_bytes < need) {
+    set_error("tiled sub-module backward workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  int rc = get_encoder();
+  if (rc) return rc;
+  const bool cmg = stack == kStackCmg;
+  const TileGeom g = tile_geom(H, W, tile_h, tile_w);
+  const long long total = (long long)n * g.ny * g.nx;
+  const long long per_pass = tiled_train_pass(g, n, max_pass_pixels);
+  const size_t win_px = (size_t)g.win_h * g.win_w;
+  uint8_t* base = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
+  int* exact = (int*)base;
+  int size[WN_NUM_PARAMS], first, count;
+  param_grad_sizes(size);
+  stack_params(stack, which, &first, &count);
+  // dst / part: the stack's own entries, compacted (add_param_grads_kernel grid y = count); later: the 34-entry
+  // layout the backward halves write, the own entries pointing at the scratch copy
+  ParamGrads dst, part;
+  float* later[WN_NUM_PARAMS] = {};
+  uint8_t* p = base + 256;
+  for (int k = 0; k < count; k++) {
+    dst.p[k] = grads[first + k];
+    part.p[k] = later[first + k] = (float*)p;
+    dst.size[k] = part.size[k] = size[first + k];
+    p += ((size_t)size[first + k] * sizeof(float) + 255) / 256 * 256;
+  }
+  void* pass_ws = p;
+  const size_t pass_bytes = workspace_bytes - (size_t)(p - (uint8_t*)workspace);
+  const int n_in = cmg ? 4 : 2;
+  bool want_in = false;
+  SubInputGrads ig = {{nullptr, nullptr, nullptr, nullptr}, {0, 0, 0, 0}};
+  for (int i = 0; i < n_in; i++) {
+    ig.p[i] = input_grads ? input_grads[i] : nullptr;
+    // cat[x, wb, he, gc]: image i is packed channels 3i..3i+2; refiner `which` reads cat[x, input which+1]
+    ig.slot[i] = cmg ? i : (i == 0 ? 0 : which + 1);
+    if (ig.p[i]) {
+      want_in = true;
+      WN_CUDA(cudaMemsetAsync(ig.p[i], 0, (size_t)n * 3 * H * W * sizeof(float), stream));
+    }
+  }
+  if ((rc = pack_exact_flag(h, in, st, exact, n, H, W, g, stream))) return rc;
+  for (long long w0 = 0; w0 < total; w0 += per_pass) {
+    const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
+    if ((rc = check_submodule_args(cur, g.win_h, g.win_w, stack, pass_bytes))) return rc;
+    TrainBuffers t;
+    carve(&t, pass_ws, (size_t)cur * win_px, stack);
+    t.f.exact_flag = exact;
+    if ((rc = pack_input_windows(h, in, st, t.f.act0, H, W, g, w0, cur, stream))) return rc;
+    FwdOpts o;
+    o.packed = true;
+    o.stack = stack;
+    o.refiner_l1 = !cmg;
+    if ((rc = umma_forward_layers(h, in, st, nullptr, cur, g.win_h, g.win_w, t.f, stream, o))) return rc;
+    const dim3 grid((unsigned)((win_px + 255) / 256), cur);
+    if (cmg)
+      maps_bwd_tiled_kernel<<<grid, 256, 0, stream>>>(grad, t.f.cm, t.g8, g, w0);
+    else
+      refine_bwd_tiled_kernel<<<grid, 256, 0, stream>>>(grad, t.f.refined, t.gr3, which, g, w0);
+    WN_LAUNCH_CHECK(h);
+    float* const* out = w0 == 0 ? grads : later;
+    rc = cmg ? backward_cmg(h, t, out, want_in, cur, g.win_h, g.win_w, stream)
+             : backward_refiners(h, t, out, which, want_in, cur, g.win_h, g.win_w, stream);
+    if (rc) return rc;
+    if (w0 > 0) {
+      add_param_grads_kernel<<<dim3(64, count), 256, 0, stream>>>(dst, part);
+      WN_LAUNCH_CHECK(h);
+    }
+    if (want_in) {
+      fold_submodule_input_grads_kernel<<<grid, 256, 0, stream>>>(cmg ? t.gin_a : t.gin_b, ig, g, w0, cur);
       WN_LAUNCH_CHECK(h);
     }
   }

@@ -753,3 +753,74 @@ class Engine:
                                             _stream_ptr(self.device))
         _lib.check(rc, "wn_backward_tiled")
         return (grads, gin) if want_input_grads else grads
+
+    # ---- windowed recompute backward of one sub-module (wn_confidence_maps_backward_tiled, wn_refine_backward_tiled) --
+    def submodule_backward_tiled_workspace_bytes(self, n: int, h: int, w: int, stack: int, tile=DEFAULT_TILE,
+                                                 max_pass_pixels: int = 0) -> int:
+        """Workspace of one ``confidence_maps_backward_tiled`` (stack 0) or ``refine_backward_tiled`` (stack 1) call
+        (wn_submodule_backward_tiled_workspace_bytes); 0 for rejected arguments."""
+        th, tw = self._tile_hw(tile)
+        return int(self.lib.wn_submodule_backward_tiled_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels),
+                                                                        int(stack)))
+
+    def _submodule_backward_tiled(self, stack: int, first: int, grad, ins, shapes, tile, want_inputs,
+                                  max_pass_pixels: int, call, what: str):
+        """The parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) and the input gradients
+        asked for by ``want_inputs`` (None where not), in one call with a workspace of its own.  call(strides, grad,
+        grads array, input grads array or None, n, h, w, th, tw, workspace) -> rc."""
+        th, tw = self._tile_hw(tile)
+        g = grad.detach().to(self.device, torch.float32).contiguous()
+        n, _, h, w = ins[0].shape
+        if tuple(g.shape) != (n, 3, h, w):
+            raise ValueError(f"the output gradient must be {(n, 3, h, w)}, got {tuple(g.shape)}")
+        make = torch.zeros if g.numel() == 0 else torch.empty  # an empty batch has zero gradients
+        grads = [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
+        gin = [make((n, 3, h, w), dtype=torch.float32, device=self.device) if want else None for want in want_inputs]
+        if g.numel() == 0:
+            return grads, gin
+        nbytes = self.submodule_backward_tiled_workspace_bytes(n, h, w, stack, (th, tw), max_pass_pixels)
+        if nbytes == 0:
+            raise _lib.WaterNetLibraryError(
+                f"{what} rejects n={n} h={h} w={w} tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        strides = (ctypes.c_int64 * (4 * len(ins)))(*[s for t in ins for s in t.stride()])
+        arr = (ctypes.c_void_p * _lib.NUM_PARAMS)()
+        for k, t in enumerate(grads):
+            arr[first + k] = t.data_ptr()
+        gin_arr = None
+        if any(want_inputs):
+            gin_arr = (ctypes.c_void_p * len(gin))(*[None if t is None else t.data_ptr() for t in gin])
+        with torch.cuda.device(self.device):
+            rc = call(strides, g.data_ptr(), arr, gin_arr, n, h, w, th, tw, ws)
+        _lib.check(rc, what)
+        return grads, gin
+
+    def confidence_maps_backward_tiled(self, grad_maps, inputs, shapes, tile=DEFAULT_TILE, want_inputs=(False,) * 4,
+                                       max_pass_pixels: int = 0):
+        """The gradients of ``confidence_maps_backward`` from the four input images alone
+        (wn_confidence_maps_backward_tiled): the cmg's training forward is recomputed in the overlapping windows of
+        ``confidence_maps_tiled``, one pass at a time, so no activation outlives the call and the workspace does not
+        grow with the image size.  ``max_pass_pixels``: window pixels per pass (0 = 2 Mi, ~8.1 GB).  Returns the 16
+        parameter gradients and the input gradients ``want_inputs`` asks for (else None).  The workspace is allocated
+        for this call only."""
+        ins = self._check_inputs(inputs)
+        stream = _stream_ptr(self.device)
+        mpp = int(max_pass_pixels)
+        return self._submodule_backward_tiled(
+            self.STACK_CMG, 0, grad_maps, ins, shapes, tile, want_inputs, mpp,
+            lambda st, g, arr, gin, n, h, w, th, tw, ws: self.lib.wn_confidence_maps_backward_tiled(
+                self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(), ins[3].data_ptr(), st, g, arr,
+                gin, n, h, w, th, tw, mpp, ws.data_ptr(), ws.numel(), stream), "wn_confidence_maps_backward_tiled")
+
+    def refine_backward_tiled(self, which: int, grad_out, inputs, shapes, tile=DEFAULT_TILE,
+                              want_inputs=(False, False), max_pass_pixels: int = 0):
+        """The gradients of ``refine_backward`` from x and xbar alone (wn_refine_backward_tiled), as
+        ``confidence_maps_backward_tiled`` (0 = 2 Mi window pixels per pass, ~3.8 GB)."""
+        ins = self._check_inputs(inputs)
+        stream = _stream_ptr(self.device)
+        mpp = int(max_pass_pixels)
+        return self._submodule_backward_tiled(
+            self.STACK_REFINER, 16 + 6 * int(which), grad_out, ins, shapes, tile, want_inputs, mpp,
+            lambda st, g, arr, gin, n, h, w, th, tw, ws: self.lib.wn_refine_backward_tiled(
+                self.handle, int(which), ins[0].data_ptr(), ins[1].data_ptr(), st, g, arr, gin, n, h, w, th, tw, mpp,
+                ws.data_ptr(), ws.numel(), stream), "wn_refine_backward_tiled")

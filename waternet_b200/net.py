@@ -15,7 +15,8 @@ reference's checkpoints load with strict ``load_state_dict`` and callers
   re-evaluates the network with torch ops for its backward pass.
 * The sub-modules (``model.cmg``, the refiners, free-standing instances) train on the library
   the same way (``wn_confidence_maps_train`` / ``wn_refine_train`` and their backward), with
-  gradients for their own parameters and inputs only.
+  gradients for their own parameters and inputs only; with ``grad_tile`` set their gradients are recomputed in
+  overlapping windows (``wn_confidence_maps_backward_tiled`` / ``wn_refine_backward_tiled``).
 """
 from __future__ import annotations
 
@@ -132,15 +133,21 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
     precision trains natively: the forward runs in the bf16x3 arithmetic of training and keeps the stack's
     activations (``wn_confidence_maps_train`` / ``wn_refine_train``), and backward gives the gradients of the stack's
     own parameters and of its inputs (``wn_confidence_maps_backward`` / ``wn_refine_backward``).  Nothing reaches the
-    parent's other parameters.  Whole images per call (``tile`` and ``grad_tile`` do not apply), at most
-    ``Engine.TRAIN_MAX_PIXELS`` pixels per image; a batch over that runs in slices.  CPU tensors,
-    ``precision="fp32"`` and a larger image evaluate the torch graph instead.  Bound to a ``WaterNet`` a stack
-    follows the parent's ``precision`` and ``tile``; a free-standing one uses its own attributes.
+    parent's other parameters.  Whole images per call (``tile`` does not apply), at most ``Engine.TRAIN_MAX_PIXELS``
+    pixels per image; a batch over that runs in slices.  CPU tensors, ``precision="fp32"`` and a larger image
+    evaluate the torch graph instead.
+    With ``grad_tile`` set (as ``WaterNet.grad_tile``) such a call keeps only its inputs: the forward is
+    ``wn_confidence_maps_tiled`` / ``wn_refine_tiled`` in the bf16x3 arithmetic of training, and backward recomputes
+    the stack's activations window by window (``wn_confidence_maps_backward_tiled`` / ``wn_refine_backward_tiled``),
+    in about 8 GB for the cmg and 4 GB for a refiner whatever the image or batch size, with no limit on the image
+    size.  Bound to a ``WaterNet`` a stack follows the parent's ``precision``, ``tile`` and ``grad_tile``; a
+    free-standing one uses its own attributes.
     """
 
     spec: List[tuple] = []
     precision = "default"
     tile = None
+    grad_tile = None
 
     def __init__(self):
         super().__init__()
@@ -190,10 +197,11 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
         own = self._own_params()
         return mode, self._engine_for(x, zero_layout(own), key_params=own), 0, tile
 
-    def _train_engine(self, x):
+    def _train_engine(self, x, any_size=False):
         """(engine with the right state dict packed, slot) for a call that records an autograd graph, or None where
-        the torch graph runs instead: CPU tensors, precision "fp32", or one image over Engine.TRAIN_MAX_PIXELS."""
-        if not x.is_cuda or x.shape[2] * x.shape[3] > Engine.TRAIN_MAX_PIXELS:
+        the torch graph runs instead: CPU tensors, precision "fp32", or one image over Engine.TRAIN_MAX_PIXELS (unless
+        ``any_size``: the windowed path)."""
+        if not x.is_cuda or (not any_size and x.shape[2] * x.shape[3] > Engine.TRAIN_MAX_PIXELS):
             return None
         parent = self._parent_ref() if self._parent_ref is not None else None
         if parent is not None:
@@ -207,6 +215,23 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
         own = self._own_params()
         return self._engine_for(x, self._zero_layout(own), key_params=own), 0
 
+    def _grad_tile(self):
+        """The windowed-backward tile of a call that records an autograd graph, as (h, w), or None: the parent's
+        ``grad_tile`` for a bound stack, else its own.  Refused with precision "fp32"."""
+        parent = self._parent_ref() if self._parent_ref is not None else None
+        if parent is not None:
+            return _checked_grad_tile(parent.grad_tile, parent._mode())
+        if self.precision not in MODES:
+            raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(MODES)}")
+        return _checked_grad_tile(self.grad_tile, MODES[self.precision])
+
+    def _train_call(self, x):
+        """(engine with the right state dict packed, slot, grad_tile or None) for a call that records an autograd
+        graph, or None where the torch graph runs instead.  With grad_tile any image size runs natively."""
+        grad_tile = self._grad_tile()
+        native = self._train_engine(x, any_size=grad_tile is not None)
+        return None if native is None else (*native, grad_tile)
+
     @staticmethod
     def _needs_graph(tensors, params):
         return torch.is_grad_enabled() and (any(t.requires_grad for t in tensors) or any(p.requires_grad for p in params))
@@ -216,14 +241,23 @@ class _SubmoduleForward(torch.autograd.Function):
     """A sub-module called on its own under autograd: forward values and gradients from the CUDA library
     (wn_confidence_maps_train / _backward for the cmg, wn_refine_train / _backward for a refiner), in the bf16x3
     arithmetic of training.  It receives the stack's own 16 or 6 parameters, so autograd routes gradients to them and
-    to nothing else.  which: None for the cmg, else the refiner slot (0 wb, 1 ce, 2 gc) of the packed state dict."""
+    to nothing else.  which: None for the cmg, else the refiner slot (0 wb, 1 ce, 2 gc) of the packed state dict.
+    With ``grad_tile`` the forward keeps nothing but the inputs (wn_confidence_maps_tiled / wn_refine_tiled in the
+    bf16x3 arithmetic of training) and the backward recomputes the stack's activations window by window
+    (wn_confidence_maps_backward_tiled / wn_refine_backward_tiled); both hold at most one pass of TRAIN_PASS_PIXELS
+    window pixels."""
 
     @staticmethod
-    def forward(ctx, eng, which, n_in, *tensors):
+    def forward(ctx, eng, which, grad_tile, n_in, *tensors):
         ins, params = tensors[:n_in], tensors[n_in:]
-        ctx.engine, ctx.which, ctx.n_in = eng, which, n_in
+        ctx.engine, ctx.which, ctx.n_in, ctx.grad_tile = eng, which, n_in, grad_tile
         ctx.weights_key = eng._weights_key
         ctx.shapes = [p.shape for p in params]
+        if grad_tile is not None:
+            ctx.save_for_backward(*ins)
+            if which is None:
+                return eng.confidence_maps_tiled(*ins, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS)
+            return eng.refine_tiled(which, *ins, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS)
         out, ctx.saved_ws = eng.confidence_maps_train(*ins) if which is None else eng.refine_train(which, *ins)
         return out
 
@@ -232,14 +266,22 @@ class _SubmoduleForward(torch.autograd.Function):
         eng = ctx.engine
         if eng._weights_key != ctx.weights_key:
             raise RuntimeError("sub-module parameters were modified between forward and backward")
-        need = ctx.needs_input_grad[3:]
+        need = ctx.needs_input_grad[4:]
         want_in, want_par = need[:ctx.n_in], need[ctx.n_in:]
-        if ctx.which is None:
+        if ctx.grad_tile is not None:
+            ins = ctx.saved_tensors
+            if ctx.which is None:
+                grads, gin = eng.confidence_maps_backward_tiled(grad, ins, ctx.shapes, ctx.grad_tile, want_in,
+                                                                max_pass_pixels=TRAIN_PASS_PIXELS)
+            else:
+                grads, gin = eng.refine_backward_tiled(ctx.which, grad, ins, ctx.shapes, ctx.grad_tile, want_in,
+                                                       max_pass_pixels=TRAIN_PASS_PIXELS)
+        elif ctx.which is None:
             grads, gin = eng.confidence_maps_backward(grad, ctx.saved_ws, ctx.shapes, want_in)
         else:
             grads, gin = eng.refine_backward(ctx.which, grad, ctx.saved_ws, ctx.shapes, want_in)
         ctx.saved_ws = None
-        return (None, None, None, *gin, *[g if w else None for g, w in zip(grads, want_par)])
+        return (None, None, None, None, *gin, *[g if w else None for g, w in zip(grads, want_par)])
 
 
 def _zeros_like_spec(spec, ref):
@@ -269,11 +311,12 @@ class ConfidenceMapGenerator(_ConvStack):
     def forward(self, x, wb, ce, gc):
         """Returns the three (N,1,H,W) maps ``out1, out2, out3`` like ``net.py:55-56``."""
         if self._needs_graph((x, wb, ce, gc), self._own_params()):
-            native = self._train_engine(x)
+            native = self._train_call(x)
             if native is None:
                 maps = self._graph(x, wb, ce, gc)
             else:
-                maps = _SubmoduleForward.apply(native[0], None, 4, x, wb, ce, gc, *self._own_params())
+                eng, _, grad_tile = native
+                maps = _SubmoduleForward.apply(eng, None, grad_tile, 4, x, wb, ce, gc, *self._own_params())
         else:
             mode, eng, _, tile = self._mode_and_engine(x, self._zero_layout)
             if tile is None:
@@ -300,11 +343,11 @@ class Refiner(_ConvStack):
 
     def forward(self, x, xbar):
         if self._needs_graph((x, xbar), self._own_params()):
-            native = self._train_engine(x)
+            native = self._train_call(x)
             if native is None:
                 return self._graph(x, xbar)
-            eng, slot = native
-            return _SubmoduleForward.apply(eng, slot, 2, x, xbar, *self._own_params())
+            eng, slot, grad_tile = native
+            return _SubmoduleForward.apply(eng, slot, grad_tile, 2, x, xbar, *self._own_params())
         mode, eng, slot, tile = self._mode_and_engine(x, self._zero_layout)
         if tile is None:
             return eng.refine(slot, x, xbar, mode)
@@ -395,7 +438,7 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
     arithmetic of training, and backward recomputes the activations window by window (``wn_backward_tiled``), in
     about 12 GB whatever the image or batch size.  The gradients equal the untiled ones up to the order of fp32 sums.
     It costs one more forward and the windows' overlap, so where the untiled path fits it is faster.  Tensor-core
-    precisions only.
+    precisions only.  Calls of ``cmg`` and the refiners on their own follow it as well (``_ConvStack``).
     """
 
     tile = None  # models pickled before the attribute existed
