@@ -22,8 +22,11 @@
  *                         (the per-frame body of inference.py:261-323)
  *   wn_enhance_u8_tiled   the same, computed in overlapping windows: bounded workspace for images of any size
  *   wn_enhance_u8_ragged  the same for n images of n sizes in one call (inference.py --source <directory>)
+ *   wn_forward_ragged     wn_forward for n images of n sizes in one call
  *   wn_forward_train /    train.py:108 `out = model(...)` and train.py:130-131 `loss.backward()`
  *   wn_backward           (autograd through net.py:99-108)
+ *   wn_forward_train_ragged / wn_backward_ragged
+ *                         the same for n images of n sizes in one call (a dataset without a fixed size)
  *   wn_backward_tiled     the same gradients from the inputs alone, recomputed in overlapping windows
  *   wn_confidence_maps_train / _backward, wn_refine_train / _backward
  *                         the sub-modules under autograd (net.py:45-56, :75-80 with parameters that require grad)
@@ -47,7 +50,7 @@
 extern "C" {
 #endif
 
-#define WN_ABI_VERSION 10
+#define WN_ABI_VERSION 11
 
 #define WN_OK 0
 #define WN_E_INVALID (-1)   /* bad argument (NULL pointer, non-positive size, unknown mode) */
@@ -235,6 +238,32 @@ int wn_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images_host, int n
                          long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * WaterNet.forward of a ragged batch of fp32 tensors: n images, each of its own size, in one call.  The windows,
+ * passes, limits and workspace bound of wn_enhance_u8_ragged (tile_h x tile_w windows, max_pass_pixels slot pixels
+ * per pass, 0 = 8 Mi, 25 % padding, 65535 windows per pass).  images_host is a HOST array of n descriptors with device
+ * pointers: the four inputs with their element strides (as in_strides of wn_forward; sN is not used) and the fp32
+ * contiguous (1,3,height,width) output.  Whether the first layer drops its a_lo pass is decided once over every input
+ * pixel of the n images, as wn_forward_tiled decides it.  The output of image i equals, bit for bit, what wn_forward
+ * returns for image i alone, in both tensor-core modes, while the e4m3 range guard stays down (the guard's flag is
+ * sticky, as in wn_enhance_u8_ragged).  Tensor-core modes only (WN_MODE_FP32_SIMT: WN_E_UNSUPPORTED).  The call copies
+ * its plan to the device from pageable host memory once, so it cannot be captured in a CUDA graph.  The workspace
+ * function returns 0 for arguments the call rejects.
+ */
+typedef struct {
+  const float* x;  /* device, fp32 (1,3,height,width) with the strides below */
+  const float* wb;
+  const float* he;
+  const float* gc;
+  int64_t in_strides[4][4]; /* {sN, sC, sH, sW} of x, wb, he, gc */
+  float* out;               /* device, fp32 contiguous (1,3,height,width) */
+  int height, width;
+} wn_ragged_tensors;
+size_t wn_forward_ragged_workspace_bytes(const int* heights_host, const int* widths_host, int n, int tile_h,
+                                         int tile_w, long long max_pass_pixels, int mode);
+int wn_forward_ragged(wn_handle* h, const wn_ragged_tensors* images_host, int n, int tile_h, int tile_w,
+                      long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * wn_enhance_u8 with the all-gather of the output fused into the kernel that produces it (SURVEY 8e: the one
  * exchange of the sharded path): the launch that writes out_nhwc stores the same bytes to peer_out[0..n_peers) --
  * addresses inside the other ranks' buffers, mapped with wn_peer_open (NVLink stores), each the start of where THIS
@@ -266,6 +295,31 @@ int wn_forward_train(wn_handle* h, const float* x, const float* wb, const float*
                      void* train_workspace, size_t workspace_bytes, void* stream);
 int wn_backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n,
                 int height, int width, void* train_workspace, size_t workspace_bytes, void* stream);
+
+/*
+ * The training step of a ragged batch: n images of their own sizes as ONE pass of n equally sized slots (the
+ * per-axis maximum of the sizes), each image at its slot's top-left; n * slot pixels <= 8 Mi and n <= 65535
+ * (wn_train_ragged_workspace_bytes returns 0 for every argument set the calls reject).
+ *   - wn_forward_train_ragged: wn_forward_train of every image (the WN_MODE_BF16X3 arithmetic; the exact-levels
+ *     decision over every input pixel of the n images), keeping the activations in `workspace`.  Descriptors as
+ *     wn_forward_ragged.  Slot pixels beyond an image are stored as zeros by every ReLU layer.
+ *   - wn_backward_ragged: consumes that workspace (untouched in between) and d(loss)/d(out) of every image.
+ *     heights_host / widths_host: the sizes of the forward call, in its order.  They fix where the call finds the
+ *     activations; the forward records its image count and slot in the workspace, and a backward whose sizes give
+ *     another count or slot stops with a device-side assertion (the CUDA context is then unusable).  grad_out_host: HOST array of n device
+ *     pointers to fp32 contiguous (1,3,H_i,W_i).  grads: as wn_backward, OVERWRITTEN with the gradients of the sum
+ *     of the n images' losses.  input_grads_host: NULL or a HOST array of 4n device pointers, image i's d/d(x),
+ *     d/d(wb), d/d(he), d/d(gc) at 4i .. 4i+3, fp32 contiguous (1,3,H_i,W_i); any entry may be NULL.
+ * Image i's output and input gradients equal those of wn_forward_train / wn_backward on image i alone bit for bit;
+ * the parameter gradients equal the sum of the per-image ones up to the order of the fp32 sums.  Both calls copy a
+ * small table from pageable host memory, so they cannot be captured in a CUDA graph.
+ */
+size_t wn_train_ragged_workspace_bytes(const int* heights_host, const int* widths_host, int n);
+int wn_forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images_host, int n, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int wn_backward_ragged(wn_handle* h, const int* heights_host, const int* widths_host, const float* const* grad_out_host,
+                       float* const* grads, float* const* input_grads_host, int n, void* workspace,
+                       size_t workspace_bytes, void* stream);
 
 /*
  * The sub-modules under autograd (a ConfidenceMapGenerator or a Refiner trained on its own): the training step of

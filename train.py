@@ -1,6 +1,7 @@
 """Train WaterNet (same CLI and artefacts as the reference's train.py; CUDA forward underneath).
 
     python train.py [--epochs 400] [--batch-size 16] [--height 112] [--width 112] [--weights W] [--seed S]
+    python train.py --native-size ...   every image at its own size (ragged batches, WaterNet.forward_many)
 
 Writes ``training/<n>/{last.pt, metrics-train.csv, metrics-val.csv, config.json}``.  Without the
 UIEB folders (``data/raw-890``, ``data/reference-890``) pass ``--synthetic`` for UIEB-shaped
@@ -37,7 +38,14 @@ def main():
                     help="(Optional) Compute the gradients in overlapping windows of N x N output pixels "
                          "(WaterNet.grad_tile): about 12 GB of activations whatever the image and batch size, for "
                          "about 1.5x the arithmetic.  Unset: whole images, ~5.6 KB per pixel")
+    ap.add_argument("--native-size", action="store_true",
+                    help="(Optional) Train every image at its own size: the dataset without --height/--width (UIEB: "
+                         "rounded down to a multiple of 32, as the reference does) and batches of differently sized "
+                         "images through WaterNet.forward_many.  With --synthetic: a mix of sizes around "
+                         "--height x --width")
     args = ap.parse_args()
+    if args.native_size and args.loader != "gpu":
+        raise SystemExit("--native-size needs --loader gpu (ragged batches are assembled on the device)")
     if args.seed is not None:
         torch.manual_seed(args.seed)
     if not torch.cuda.is_available():
@@ -51,15 +59,22 @@ def main():
     if args.synthetic or not raw_dir.exists():
         if not args.synthetic:
             print(f"{raw_dir} not found: falling back to --synthetic data")
-        dataset = SyntheticUIEB(890, args.height, args.width, seed=args.seed or 0, transform=aug)
+        sizes = None
+        if args.native_size:  # a mix of sizes around height x width, multiples of 16, at least 32
+            sizes = [(max(32, args.height + dh), max(32, args.width + dw))
+                     for dh, dw in ((0, 0), (32, -16), (-16, 32), (16, 16), (-32, 0))]
+        dataset = SyntheticUIEB(890, args.height, args.width, seed=args.seed or 0, transform=aug, sizes=sizes)
     else:
-        dataset = UIEBDataset(raw_dir, ref_dir, im_height=args.height, im_width=args.width,
+        size = (None, None) if args.native_size else (args.height, args.width)
+        dataset = UIEBDataset(raw_dir, ref_dir, im_height=size[0], im_width=size[1],
                               transform=aug if aug is not None else (lambda image, mask: {"image": image, "mask": mask}))
     n_val = 90 if len(dataset) >= 180 else max(1, len(dataset) // 10)
     train_set, val_set = torch.utils.data.random_split(dataset, [len(dataset) - n_val, n_val])
     if args.loader == "gpu":
-        train_loader = GpuBatchLoader(train_set, args.batch_size, device, augment=True, seed=args.seed)
-        val_loader = GpuBatchLoader(val_set, args.batch_size, device, augment=True, seed=args.seed)
+        train_loader = GpuBatchLoader(train_set, args.batch_size, device, augment=True, seed=args.seed,
+                                      ragged=args.native_size)
+        val_loader = GpuBatchLoader(val_set, args.batch_size, device, augment=True, seed=args.seed,
+                                    ragged=args.native_size)
     else:
         train_loader = torch.utils.data.DataLoader(train_set, batch_size=args.batch_size)
         val_loader = torch.utils.data.DataLoader(val_set, batch_size=args.batch_size)
@@ -86,7 +101,7 @@ def main():
         torch.save(model.state_dict(), savedir / "last.pt")
     T.save_metrics(savedir, train_hist, val_hist, {
         "epochs": args.epochs, "batch_size": args.batch_size, "im_height": args.height, "im_width": args.width,
-        "weights": args.weights})
+        "weights": args.weights, "native_size": args.native_size})
     print(f"Metrics and weights saved to {savedir}")
     print(f"Total time: {timer() - start}s")
 

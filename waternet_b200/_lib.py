@@ -19,7 +19,7 @@ MODE_BF16_FP8 = 2
 MODE_DEFAULT = -1
 NUM_PARAMS = 34
 NUM_TIMING_SLOTS = 23
-ABI_VERSION = 10
+ABI_VERSION = 11
 PEER_HANDLE_BYTES = 64  # WN_PEER_HANDLE_BYTES
 MAX_PEERS = 15          # WN_MAX_PEERS
 
@@ -27,6 +27,16 @@ MAX_PEERS = 15          # WN_MAX_PEERS
 class RaggedImage(ctypes.Structure):
     """wn_ragged_image: one image of a ragged batch (device pointers)."""
     _fields_ = [("rgb", c_void_p), ("out_u8", c_void_p), ("out_f32", c_void_p), ("height", c_int), ("width", c_int)]
+
+
+class RaggedTensors(ctypes.Structure):
+    """wn_ragged_tensors: the four fp32 inputs of one image of a ragged batch, their element strides (sN, sC, sH, sW
+    each), its fp32 contiguous (1,3,H,W) output and its size (device pointers)."""
+    _fields_ = [("x", c_void_p), ("wb", c_void_p), ("he", c_void_p), ("gc", c_void_p), ("in_strides", c_int64 * 16),
+                ("out", c_void_p), ("height", c_int), ("width", c_int)]
+
+
+RAGGED_TENSORS_BYTES = 176  # sizeof(wn_ragged_tensors), asserted in csrc/api.cu
 
 
 # name -> (restype, argtypes); mirrors include/waternet_b200.h one to one
@@ -113,6 +123,14 @@ _SIGNATURES = {
     "wn_refine_backward_tiled": (c_int, [c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int64), c_void_p,
                                          POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int,
                                          ctypes.c_longlong, c_void_p, c_size_t, c_void_p]),
+    "wn_forward_ragged_workspace_bytes": (c_size_t, [POINTER(c_int), POINTER(c_int), c_int, c_int, c_int,
+                                                     ctypes.c_longlong, c_int]),
+    "wn_forward_ragged": (c_int, [c_void_p, POINTER(RaggedTensors), c_int, c_int, c_int, ctypes.c_longlong, c_int,
+                                  c_void_p, c_size_t, c_void_p]),
+    "wn_train_ragged_workspace_bytes": (c_size_t, [POINTER(c_int), POINTER(c_int), c_int]),
+    "wn_forward_train_ragged": (c_int, [c_void_p, POINTER(RaggedTensors), c_int, c_void_p, c_size_t, c_void_p]),
+    "wn_backward_ragged": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_void_p), POINTER(c_void_p),
+                                   POINTER(c_void_p), c_int, c_void_p, c_size_t, c_void_p]),
     "wn_debug_forward_layer": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int,
                                        c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "wn_enable_timing": (c_int, [c_void_p, c_int]),

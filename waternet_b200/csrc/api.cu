@@ -435,6 +435,43 @@ int wn_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images_host, int n
                                 (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0);
 }
 
+static_assert(sizeof(wn_ragged_tensors) == 176, "wn_ragged_tensors: _lib.RAGGED_TENSORS_BYTES restates this size");
+
+size_t wn_forward_ragged_workspace_bytes(const int* heights_host, const int* widths_host, int n, int tile_h,
+                                         int tile_w, long long max_pass_pixels, int mode) {
+  const char* what = "wn_forward_ragged_workspace_bytes";
+  if (!heights_host || !widths_host || ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode)) return 0;
+  for (int i = 0; i < n; i++)
+    if (ragged_check_size(what, i, heights_host[i], widths_host[i])) return 0;
+  return umma_forward_ragged_workspace_bytes(heights_host, widths_host, n, tile_h, tile_w, max_pass_pixels);
+}
+
+int wn_forward_ragged(wn_handle* h, const wn_ragged_tensors* images_host, int n, int tile_h, int tile_w,
+                      long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* what = "wn_forward_ragged";
+  if (!h || !images_host || !workspace) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  int rc = ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode);
+  if (rc) return rc;
+  for (int i = 0; i < n; i++) {
+    const wn_ragged_tensors& t = images_host[i];
+    if (!t.x || !t.wb || !t.he || !t.gc || !t.out) {
+      set_error("%s: null image pointer (image %d)", what, i);
+      return WN_E_INVALID;
+    }
+    if ((rc = ragged_check_size(what, i, t.height, t.width))) return rc;
+  }
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  return umma_forward_ragged(h, images_host, n, tile_h, tile_w, max_pass_pixels, workspace, workspace_bytes,
+                             (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0);
+}
+
 // ---- the reference's callable sub-modules (net.py:45-56 ConfidenceMapGenerator.forward, :75-80 Refiner.forward)
 size_t wn_submodule_workspace_bytes(int n, int h, int w, int mode) {
   if (n <= 0 || h <= 0 || w <= 0) return 0;
@@ -686,6 +723,100 @@ int wn_backward(wn_handle* h, const float* grad_out, float* const* grads, float*
   DeviceGuard guard(h->device);
   return backward(h, grad_out, grads, input_grads, n, height, width, train_workspace, workspace_bytes,
                   (cudaStream_t)stream);
+}
+
+// ---- the ragged training step
+// the shape checks the two calls and the workspace function share; 0 = accepted
+static int train_ragged_check(const char* what, const int* hs, const int* ws, int n) {
+  if (n <= 0) {
+    set_error("%s: bad image count n=%d", what, n);
+    return WN_E_INVALID;
+  }
+  if (n > 65535) {
+    set_error("%s: at most 65535 images per call, got n=%d", what, n);
+    return WN_E_UNSUPPORTED;
+  }
+  int sh = 0, sw = 0;
+  for (int i = 0; i < n; i++) {
+    if (hs[i] <= 0 || ws[i] <= 0) {
+      set_error("%s: bad size of image %d: h=%d w=%d", what, i, hs[i], ws[i]);
+      return WN_E_INVALID;
+    }
+    sh = hs[i] > sh ? hs[i] : sh;
+    sw = ws[i] > sw ? ws[i] : sw;
+  }
+  if ((long long)n * sh * sw > kTrainMaxPixels) {
+    set_error("%s: %d slots of %dx%d exceed the %lld pixels of one training pass", what, n, sh, sw, kTrainMaxPixels);
+    return WN_E_UNSUPPORTED;
+  }
+  return WN_OK;
+}
+
+size_t wn_train_ragged_workspace_bytes(const int* heights_host, const int* widths_host, int n) {
+  if (!heights_host || !widths_host ||
+      train_ragged_check("wn_train_ragged_workspace_bytes", heights_host, widths_host, n))
+    return 0;
+  return train_ragged_workspace_bytes(heights_host, widths_host, n);
+}
+
+int wn_forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images_host, int n, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  const char* what = "wn_forward_train_ragged";
+  if (!h || !images_host || !workspace) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  if (n <= 0 || n > 65535) {
+    set_error("%s: 1..65535 images per call, got n=%d", what, n);
+    return n <= 0 ? WN_E_INVALID : WN_E_UNSUPPORTED;
+  }
+  std::vector<int> hs(n), ws(n);
+  for (int i = 0; i < n; i++) {
+    const wn_ragged_tensors& t = images_host[i];
+    if (!t.x || !t.wb || !t.he || !t.gc || !t.out) {
+      set_error("%s: null image pointer (image %d)", what, i);
+      return WN_E_INVALID;
+    }
+    hs[i] = t.height;
+    ws[i] = t.width;
+  }
+  int rc = train_ragged_check(what, hs.data(), ws.data(), n);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  return forward_train_ragged(h, images_host, n, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int wn_backward_ragged(wn_handle* h, const int* heights_host, const int* widths_host, const float* const* grad_out_host,
+                       float* const* grads, float* const* input_grads_host, int n, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+  const char* what = "wn_backward_ragged";
+  if (!h || !heights_host || !widths_host || !grad_out_host || !grads || !workspace) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  for (int i = 0; i < WN_NUM_PARAMS; i++)
+    if (!grads[i]) {
+      set_error("%s: grads[%d] is NULL", what, i);
+      return WN_E_INVALID;
+    }
+  int rc = train_ragged_check(what, heights_host, widths_host, n);
+  if (rc) return rc;
+  for (int i = 0; i < n; i++)
+    if (!grad_out_host[i]) {
+      set_error("%s: grad_out_host[%d] is NULL", what, i);
+      return WN_E_INVALID;
+    }
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  return backward_ragged(h, heights_host, widths_host, grad_out_host, grads, input_grads_host, n, workspace,
+                         workspace_bytes, (cudaStream_t)stream);
 }
 
 // ---- the sub-modules under autograd

@@ -253,6 +253,24 @@ int pack_exact_flag(wn_handle* h, const float* const in[4], const int64_t in_str
 int pack_input_windows(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], uint4* act0, int height,
                        int width, const TileGeom& tiles, long long win0, int count, cudaStream_t stream);
 
+// The ragged forms of the two packing steps (wn_forward_ragged, wn_forward_train_ragged).  imgs: one entry per image
+// (its four inputs and element strides), device table; wins: the `count` windows of one pass, device table, window k
+// in slot k at the slot's top-left.  With act0 NULL the call only clears *flag unless every input pixel of the
+// windows' valid extents is an 8-bit level; otherwise it writes the pass's act0 planes, zeros beyond each valid
+// extent, and leaves the flag alone.
+struct PackInArgs {
+  const float* p[4];
+  long long s[4][4];
+};
+int pack_input_ragged(wn_handle* h, const PackInArgs* imgs, const RaggedWindow* wins, int count, int slot_h,
+                      int slot_w, uint4* act0, int* flag, cudaStream_t stream);
+// wn_forward_ragged (arguments checked by the caller, api.cu): the windows and passes of ragged_plan
+size_t umma_forward_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
+                                           long long max_pass_pixels);
+int umma_forward_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, int tile_h, int tile_w,
+                        long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream,
+                        int scheme);
+
 // conv_bwd.cu
 constexpr long long kTrainMaxPixels = 8ll << 20;  // pixels of one training pass (activations kept: ~5.6 KB each)
 constexpr long long kTiledTrainPassPixels = 2ll << 20;  // wn_backward_tiled: window pixels per pass by default
@@ -290,5 +308,12 @@ int submodule_backward_tiled(wn_handle* h, int stack, int which, const float* co
                              const int64_t in_strides[4][4], const float* grad, float* const* grads,
                              float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
                              long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+// the ragged training step (wn_forward_train_ragged / wn_backward_ragged): the n images of one call as one pass of
+// slots of the per-axis maximum size; arguments checked by the caller (api.cu: n * slot pixels <= kTrainMaxPixels)
+size_t train_ragged_workspace_bytes(const int* hs, const int* ws, int n);
+int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, void* workspace, size_t workspace_bytes,
+                         cudaStream_t stream);
+int backward_ragged(wn_handle* h, const int* hs, const int* ws, const float* const* grad_out, float* const* grads,
+                    float* const* input_grads, int n, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace wn

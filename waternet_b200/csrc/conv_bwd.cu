@@ -14,6 +14,8 @@
 //   bias_grad_kernel     db[co] = sum_px g[px][co]
 //
 // All three GEMM-shaped pieces use the same bf16x3 split as the forward (gradient error ~1e-5).
+#include <assert.h>
+
 #include "umma_conv.cuh"
 
 namespace wn {
@@ -466,6 +468,58 @@ input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, I
   for (int t = 0; t < 4; t++)
 #pragma unroll
     for (int c = 0; c < 3; c++) out.p[t][((size_t)n * 3 + c) * hw + pix] = v[t * 3 + c];
+}
+
+// ---- the ragged training step (wn_forward_train_ragged / wn_backward_ragged): slot n of the pass holds image
+// wins[n].img at its top-left, valid extent wins[n].vh x wins[n].vw (the whole image).  Per image: d(loss)/d(out) and
+// the four input-gradient tensors (any may be null), fp32 contiguous (1,3,H,W).
+struct RaggedGrads {
+  const float* g_out;
+  float* in[4];
+};
+
+// The ragged form of gate_bwd_kernel: d(out) read at image coordinates inside the valid extent, 0 beyond it.  plan:
+// n, slot_h, slot_w as the forward call wrote them; the grid must be the same pass (gridDim.y = n slots).
+__global__ void __launch_bounds__(256)
+gate_bwd_ragged_kernel(const int* __restrict__ plan, const RaggedGrads* __restrict__ imgs, const RaggedWindow* __restrict__ wins,
+                       const float* __restrict__ cm, const float* __restrict__ refined, uint4* __restrict__ g8,
+                       uint4* __restrict__ gr3, int slot_h, int slot_w) {
+  assert(plan[0] == (int)gridDim.y && plan[1] == slot_h && plan[2] == slot_w);
+  const int hw = slot_h * slot_w;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const RaggedWindow& r = wins[blockIdx.y];
+  const int wy = pix / slot_w, wx = pix - wy * slot_w;
+  const bool valid = wy < r.vh && wx < r.vw;
+  const size_t ihw = (size_t)r.H * r.W;
+  const float* g = imgs[r.img].g_out + (size_t)(r.ys + wy) * r.W + (r.xs + wx);
+  float go[3];
+#pragma unroll
+  for (int k = 0; k < 3; k++) go[k] = valid ? g[k * ihw] : 0.f;
+  gate_bwd_pixel(go, cm, refined, g8, gr3, blockIdx.y, pix, hw);
+}
+
+// The ragged form of input_grads_kernel: only the valid extent of each slot is read (the input-gradient launches
+// have no ReLU mask, so gin_a / gin_b are not zero beyond it) and stored into the slot's image.
+__global__ void __launch_bounds__(256)
+input_grads_ragged_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb,
+                          const RaggedGrads* __restrict__ imgs, const RaggedWindow* __restrict__ wins, int slot_h,
+                          int slot_w) {
+  const int hw = slot_h * slot_w;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const RaggedWindow& r = wins[blockIdx.y];
+  const int wy = pix / slot_w, wx = pix - wy * slot_w;
+  if (wy >= r.vh || wx >= r.vw) return;
+  float v[16];
+  input_grads_pixel(ga, gb, blockIdx.y, pix, hw, v);
+  const size_t ihw = (size_t)r.H * r.W, o = (size_t)(r.ys + wy) * r.W + (r.xs + wx);
+  const RaggedGrads& d = imgs[r.img];
+#pragma unroll
+  for (int t = 0; t < 4; t++)
+    if (d.in[t])
+#pragma unroll
+      for (int c = 0; c < 3; c++) d.in[t][c * ihw + o] = v[t * 3 + c];
 }
 
 // The input gradients of a sub-module call, from the one 32-channel buffer its first layer wrote (the cmg: gin_a,
@@ -1014,6 +1068,142 @@ int backward(wn_handle* h, const float* grad_out, float* const* grads, float* co
     InputGrads ig;
     for (int i = 0; i < 4; i++) ig.p[i] = input_grads[i];
     input_grads_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(t.gin_a, t.gin_b, ig, hw);
+    WN_LAUNCH_CHECK(h);
+  }
+  return WN_OK;
+}
+
+// ---- the ragged training step ------------------------------------------------------------------------------------
+// The n images of a call run as one pass of n slots of the per-axis maximum size, image i in slot i at the top-left.
+// The forward masks every ReLU activation beyond each image (the RAG layers), and the backward seeds 0 there, so
+// every gradient plane a weight-gradient GEMM reads is 0 at masked pixels and adds exact zeros (DESIGN.md 4.10).
+// Workspace: [plan: n, slot_h, slot_w | windows | PackInArgs | RaggedGrads, one each per image][the training carve-up
+// of n slots].  The backward derives its carve-up from the sizes it is given; gate_bwd_ragged_kernel asserts that
+// they give the plan the forward wrote, so a backward with other sizes stops instead of reading the wrong activations.
+static void ragged_slot(const int* hs, const int* ws, int n, int* sh, int* sw) {
+  *sh = *sw = 0;
+  for (int i = 0; i < n; i++) {
+    *sh = hs[i] > *sh ? hs[i] : *sh;
+    *sw = ws[i] > *sw ? ws[i] : *sw;
+  }
+}
+static size_t align256b(size_t v) { return (v + 255) / 256 * 256; }
+static size_t ragged_train_table_bytes(int n) {
+  return align256b((size_t)n * sizeof(RaggedWindow)) + align256b((size_t)n * sizeof(PackInArgs)) +
+         align256b((size_t)n * sizeof(RaggedGrads));
+}
+
+size_t train_ragged_workspace_bytes(const int* hs, const int* ws, int n) {
+  int sh, sw;
+  ragged_slot(hs, ws, n, &sh, &sw);
+  return 256 + 256 + ragged_train_table_bytes(n) + train_workspace_bytes_padded(n, sh, sw);
+}
+
+// the table's three parts and the training buffers of a workspace of any alignment
+struct RaggedTrainLayout {
+  int* plan;  // n, slot_h, slot_w of the forward call
+  RaggedWindow* wins;
+  PackInArgs* imgs;
+  RaggedGrads* grads;
+  TrainBuffers t;
+};
+static RaggedTrainLayout ragged_train_layout(void* workspace, int n, int sh, int sw) {
+  RaggedTrainLayout l;
+  uint8_t* p = (uint8_t*)align256b((uintptr_t)workspace);
+  l.plan = (int*)p;
+  p += 256;
+  l.wins = (RaggedWindow*)p;
+  p += align256b((size_t)n * sizeof(RaggedWindow));
+  l.imgs = (PackInArgs*)p;
+  p += align256b((size_t)n * sizeof(PackInArgs));
+  l.grads = (RaggedGrads*)p;
+  p += align256b((size_t)n * sizeof(RaggedGrads));
+  carve(&l.t, p, (size_t)n * sh * sw);
+  return l;
+}
+
+int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, void* workspace, size_t workspace_bytes,
+                         cudaStream_t stream) {
+  std::vector<int> hs(n), ws(n);
+  for (int i = 0; i < n; i++) {
+    hs[i] = images[i].height;
+    ws[i] = images[i].width;
+  }
+  const size_t need = train_ragged_workspace_bytes(hs.data(), ws.data(), n);
+  if (workspace_bytes < need) {
+    set_error("ragged training workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  int sh, sw;
+  ragged_slot(hs.data(), ws.data(), n, &sh, &sw);
+  RaggedTrainLayout l = ragged_train_layout(workspace, n, sh, sw);
+  // host copy of the plan, the windows and the PackInArgs, contiguous as in the workspace
+  const size_t win_b = align256b((size_t)n * sizeof(RaggedWindow));
+  std::vector<uint8_t> host(256 + win_b + (size_t)n * sizeof(PackInArgs));
+  const int plan[3] = {n, sh, sw};
+  memcpy(host.data(), plan, sizeof(plan));
+  RaggedWindow* wins = reinterpret_cast<RaggedWindow*>(host.data() + 256);
+  PackInArgs* imgs = reinterpret_cast<PackInArgs*>(host.data() + 256 + win_b);
+  for (int i = 0; i < n; i++) {
+    const wn_ragged_tensors& d = images[i];
+    RaggedWindow r = {};
+    r.out_f32 = d.out;
+    r.img = i;
+    r.H = r.vh = r.ky1 = d.height;
+    r.W = r.vw = r.kx1 = d.width;
+    wins[i] = r;
+    const float* p[4] = {d.x, d.wb, d.he, d.gc};
+    for (int t = 0; t < 4; t++) {
+      imgs[i].p[t] = p[t];
+      for (int k = 0; k < 4; k++) imgs[i].s[t][k] = d.in_strides[t][k];
+    }
+  }
+  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
+  WN_CUDA(cudaMemcpyAsync(l.plan, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
+  int rc;
+  WN_CUDA(cudaMemsetAsync(l.t.f.exact_flag, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
+  if ((rc = pack_input_ragged(h, l.imgs, l.wins, n, sh, sw, nullptr, l.t.f.exact_flag, stream))) return rc;
+  if ((rc = pack_input_ragged(h, l.imgs, l.wins, n, sh, sw, l.t.f.act0, l.t.f.exact_flag, stream))) return rc;
+  FwdOpts o;
+  o.packed = true;
+  o.rwin = l.wins;
+  const int64_t none[4][4] = {};
+  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
+  return umma_forward_layers(h, no_in, none, nullptr, n, sh, sw, l.t.f, stream, o);
+}
+
+int backward_ragged(wn_handle* h, const int* hs, const int* ws, const float* const* grad_out, float* const* grads,
+                    float* const* input_grads, int n, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!h->bwd) {
+    set_error("backward weights have not been packed");
+    return WN_E_STATE;
+  }
+  const size_t need = train_ragged_workspace_bytes(hs, ws, n);
+  if (workspace_bytes < need) {
+    set_error("ragged training workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  int rc;
+  if ((rc = get_encoder())) return rc;
+  int sh, sw;
+  ragged_slot(hs, ws, n, &sh, &sw);
+  RaggedTrainLayout l = ragged_train_layout(workspace, n, sh, sw);
+  bool want_in = false;
+  std::vector<RaggedGrads> host(n);
+  for (int i = 0; i < n; i++) {
+    host[i].g_out = grad_out[i];
+    for (int t = 0; t < 4; t++) {
+      host[i].in[t] = input_grads ? input_grads[4 * i + t] : nullptr;
+      want_in = want_in || host[i].in[t];
+    }
+  }
+  WN_CUDA(cudaMemcpyAsync(l.grads, host.data(), (size_t)n * sizeof(RaggedGrads), cudaMemcpyHostToDevice, stream));
+  const dim3 grid((unsigned)(((size_t)sh * sw + 255) / 256), n);
+  gate_bwd_ragged_kernel<<<grid, 256, 0, stream>>>(l.plan, l.grads, l.wins, l.t.f.cm, l.t.f.refined, l.t.g8, l.t.gr3, sh, sw);
+  WN_LAUNCH_CHECK(h);
+  if ((rc = backward_layers(h, l.t, grads, want_in, n, sh, sw, stream))) return rc;
+  if (want_in) {
+    input_grads_ragged_kernel<<<grid, 256, 0, stream>>>(l.t.gin_a, l.t.gin_b, l.grads, l.wins, sh, sw);
     WN_LAUNCH_CHECK(h);
   }
   return WN_OK;

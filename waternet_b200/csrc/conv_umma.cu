@@ -31,10 +31,34 @@ namespace wn {
 // torch.cat([x, wb, ce, gc], 1) (net.py:46) -> act planes: 16 channels (12 + 4 zero), bf16 hi/lo of
 // v*255.  Inputs that came from 8-bit images (arr2ten: u/255) give integers 0..255, exact in the
 // 8-bit bf16 significand: then lo == 0 and the first layer can drop its a_lo pass (flag stays set).
-struct PackInArgs {
-  const float* p[4];
-  long long s[4][4];
-};
+// v[3t + c] = input t, channel c at (n, y, x), times 255; false unless all twelve are 8-bit levels
+__device__ __forceinline__ bool pack_pixel(const PackInArgs& a, int n, int y, int x, float* v) {
+  bool exact = true;
+#pragma unroll
+  for (int t = 0; t < 4; t++)
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      float f = __fmul_rn(a.p[t][n * a.s[t][0] + c * a.s[t][1] + y * a.s[t][2] + x * a.s[t][3]], 255.0f);
+      float r = rintf(f);
+      // (u/255)*255 lands within ~2e-5 of u; anything within 2^-14 of a level is treated as that level
+      if (fabsf(f - r) <= 6.103515625e-5f && r >= 0.f && r <= 255.f) f = r; else exact = false;
+      v[t * 3 + c] = f;
+    }
+  return exact;
+}
+// 16 channels -> the four operand planes hi0, hi1, lo0, lo1 of pixel o[0] (planes hw apart)
+__device__ __forceinline__ void store_packed(uint4* o, int hw, float* v) {
+  v[12] = v[13] = v[14] = v[15] = 0.f;
+  uint32_t hi[8], lo[8];
+#pragma unroll
+  for (int j = 0; j < 16; j += 2) {
+    split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
+  }
+  o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+  o[hw] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+  o[2 * (size_t)hw] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+  o[3 * (size_t)hw] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
+}
 // FORM kPackImages: pixel blockIdx.x * 256 + tid of image blockIdx.y -> act0 planes, and the flag.
 // kPackWindows (tiled forward): pixel of window win0 + blockIdx.y of `tiles`, read at image coordinates -> that
 // window's act0 planes (blockIdx.y of the pass); the flag is not touched.
@@ -59,31 +83,34 @@ __global__ void __launch_bounds__(256) pack_inputs_kernel(PackInArgs a, uint4* _
       x = pix - y * W;
     }
     float v[16];
-#pragma unroll
-    for (int t = 0; t < 4; t++)
-#pragma unroll
-      for (int c = 0; c < 3; c++) {
-        float f = __fmul_rn(a.p[t][n * a.s[t][0] + c * a.s[t][1] + y * a.s[t][2] + x * a.s[t][3]], 255.0f);
-        float r = rintf(f);
-        // (u/255)*255 lands within ~2e-5 of u; anything within 2^-14 of a level is treated as that level
-        if (fabsf(f - r) <= 6.103515625e-5f && r >= 0.f && r <= 255.f) f = r; else exact = false;
-        v[t * 3 + c] = f;
-      }
-    if constexpr (FORM != kPackFlag) {
-      v[12] = v[13] = v[14] = v[15] = 0.f;
-      uint32_t hi[8], lo[8];
-#pragma unroll
-      for (int j = 0; j < 16; j += 2) {
-        split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
-      }
-      uint4* o = out + (size_t)blockIdx.y * 4 * hw + pix;  // planes: hi0, hi1, lo0, lo1
-      o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-      o[hw] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-      o[2 * (size_t)hw] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-      o[3 * (size_t)hw] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-    }
+    exact = pack_pixel(a, n, y, x, v);
+    if constexpr (FORM != kPackFlag) store_packed(out + (size_t)blockIdx.y * 4 * hw + pix, hw, v);
   }
   if constexpr (FORM != kPackWindows)
+    if (!__syncthreads_and(exact) && threadIdx.x == 0) atomicExch(exact_flag, 0);
+}
+
+// The ragged form (pack_input_ragged): slot pixel blockIdx.x * 256 + tid of slot blockIdx.y, which holds window
+// wins[blockIdx.y] at its top-left.  Inside the window's valid extent the pixel is read at image coordinates through
+// its image's strides (64-bit offsets) with the arithmetic above; beyond it the planes are zeros.  FLAG: only the
+// exact-levels flag, over the valid extents, nothing is written.
+template <bool FLAG>
+__global__ void __launch_bounds__(256)
+pack_inputs_ragged_kernel(const PackInArgs* __restrict__ imgs, const RaggedWindow* __restrict__ wins,
+                          uint4* __restrict__ out, int slot_h, int slot_w, int* __restrict__ exact_flag) {
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  const int hw = slot_h * slot_w;
+  bool exact = true;
+  if (pix < hw) {
+    const RaggedWindow& r = wins[blockIdx.y];
+    const int wy = pix / slot_w, wx = pix - wy * slot_w;
+    float v[16];
+#pragma unroll
+    for (int j = 0; j < 12; j++) v[j] = 0.f;
+    if (wy < r.vh && wx < r.vw) exact = pack_pixel(imgs[r.img], 0, r.ys + wy, r.xs + wx, v);
+    if constexpr (!FLAG) store_packed(out + (size_t)blockIdx.y * 4 * hw + pix, hw, v);
+  }
+  if constexpr (FLAG)
     if (!__syncthreads_and(exact) && threadIdx.x == 0) atomicExch(exact_flag, 0);
 }
 
@@ -855,6 +882,108 @@ int umma_forward_tiled(wn_handle* h, const float* const in[4], const int64_t in_
           maps ? b.cm : refined, maps ? 3 : 9, maps ? 0 : 3 * which, 3, out, g, w0);
       WN_LAUNCH_CHECK(h);
     }
+  }
+  return mirror_overflow(h, scheme, stream);
+}
+
+int pack_input_ragged(wn_handle* h, const PackInArgs* imgs, const RaggedWindow* wins, int count, int slot_h,
+                      int slot_w, uint4* act0, int* flag, cudaStream_t stream) {
+  TimedScope ts(h, kSlotPack, stream);
+  const dim3 grid((unsigned)(((size_t)slot_h * slot_w + 255) / 256), count);
+  if (act0)
+    pack_inputs_ragged_kernel<false><<<grid, 256, 0, stream>>>(imgs, wins, act0, slot_h, slot_w, flag);
+  else
+    pack_inputs_ragged_kernel<true><<<grid, 256, 0, stream>>>(imgs, wins, nullptr, slot_h, slot_w, flag);
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+
+// The ragged form of umma_forward (fp32 tensors in, wn_forward_ragged): the windows and passes of ragged_plan, as
+// umma_enhance_u8_ragged runs them, with the operands read through each image's strides (pack_inputs_ragged_kernel)
+// instead of preprocessed from uint8.  The exact-levels flag is taken once over every input pixel of every image
+// before the first pass, as umma_forward_tiled takes it, and stays valid for the bf16x3 re-run of every pass.  The
+// gate epilogue stores each window's kept rectangle into its image's `out` (RaggedWindow::out_f32).  The plan (one
+// PackInArgs per image, one descriptor per window) is copied into the workspace once per call, so the call cannot be
+// captured in a graph.  Workspace: [flag | table | the largest pass].
+static size_t ragged_fp32_table_bytes(int n, size_t windows) {
+  return align256(align256((size_t)n * sizeof(PackInArgs)) + windows * sizeof(RaggedWindow));
+}
+static size_t ragged_fp32_workspace(int n, const std::vector<RaggedWindow>& wins,
+                                    const std::vector<RaggedPass>& passes) {
+  long long px = 0;
+  for (const RaggedPass& p : passes) {
+    const long long v = (long long)p.count * p.slot_h * p.slot_w;
+    px = v > px ? v : px;
+  }
+  return (size_t)px * kUmmaBytesPerPixel + 4096 + 256 + ragged_fp32_table_bytes(n, wins.size()) + 1024;
+}
+
+size_t umma_forward_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
+                                           long long max_pass_pixels) {
+  std::vector<RaggedWindow> wins;
+  std::vector<RaggedPass> passes;
+  ragged_plan(hs, ws, n, tile_h, tile_w, ragged_pass_pixels(max_pass_pixels), &wins, &passes);
+  return ragged_fp32_workspace(n, wins, passes);
+}
+
+int umma_forward_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, int tile_h, int tile_w,
+                        long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream,
+                        int scheme) {
+  if (!h->umma) {
+    set_error("tensor-core weights have not been packed");
+    return WN_E_STATE;
+  }
+  std::vector<int> hs(n), ws(n);
+  for (int i = 0; i < n; i++) {
+    hs[i] = images[i].height;
+    ws[i] = images[i].width;
+  }
+  std::vector<RaggedWindow> wins;
+  std::vector<RaggedPass> passes;
+  ragged_plan(hs.data(), ws.data(), n, tile_h, tile_w, ragged_pass_pixels(max_pass_pixels), &wins, &passes);
+  const size_t need = ragged_fp32_workspace(n, wins, passes);
+  if (workspace_bytes < need) {
+    set_error("ragged forward workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  int rc = get_encoder();
+  if (rc) return rc;
+  scheme = effective_scheme(h, scheme);
+  uint8_t* base = (uint8_t*)align256((uintptr_t)workspace);
+  int* exact = (int*)base;
+  uint8_t* table = base + 256;
+  const size_t img_b = align256((size_t)n * sizeof(PackInArgs));
+  void* fwd_ws = table + ragged_fp32_table_bytes(n, wins.size());
+  std::vector<uint8_t> host(img_b + wins.size() * sizeof(RaggedWindow));
+  PackInArgs* imgs = reinterpret_cast<PackInArgs*>(host.data());
+  for (int i = 0; i < n; i++) {
+    const wn_ragged_tensors& t = images[i];
+    const float* in[4] = {t.x, t.wb, t.he, t.gc};
+    imgs[i] = pack_args(in, t.in_strides);
+  }
+  for (RaggedWindow& w : wins) w.out_f32 = images[w.img].out;
+  memcpy(host.data() + img_b, wins.data(), wins.size() * sizeof(RaggedWindow));
+  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
+  WN_CUDA(cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
+  const PackInArgs* d_imgs = reinterpret_cast<const PackInArgs*>(table);
+  const RaggedWindow* d_wins = reinterpret_cast<const RaggedWindow*>(table + img_b);
+  WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
+  for (const RaggedPass& p : passes)
+    if ((rc = pack_input_ragged(h, d_imgs, d_wins + p.first, p.count, p.slot_h, p.slot_w, nullptr, exact, stream)))
+      return rc;
+  const int64_t none[4][4] = {};
+  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (const RaggedPass& p : passes) {
+    FwdBuffers b = carve(fwd_ws, p.count, p.slot_h, p.slot_w);
+    b.exact_flag = exact;
+    if ((rc = pack_input_ragged(h, d_imgs, d_wins + p.first, p.count, p.slot_h, p.slot_w, b.act0, exact, stream)))
+      return rc;
+    FwdOpts o;
+    o.scheme = scheme;
+    o.packed = true;
+    o.rwin = d_wins + p.first;
+    rc = umma_pass(h, no_in, none, nullptr, p.count, p.slot_h, p.slot_w, b, stream, o);
+    if (rc) return rc;
   }
   return mirror_overflow(h, scheme, stream);
 }

@@ -120,6 +120,18 @@ def ragged_plan(sizes, tile_h: int, tile_w: int, max_pass_pixels: int = 0) -> li
     return passes
 
 
+def ragged_train_calls(sizes, max_pass_pixels: int) -> list:
+    """How ``Engine.forward_train_ragged`` groups images of ``sizes`` [(h, w), ...] into training calls:
+    ``ragged_plan`` at ``max_pass_pixels`` slot pixels per pass with a tile as large as the largest image, so that
+    every image is one window and every pass one call of wn_forward_train_ragged (n x slot pixels <= the limit, at
+    most 65535 images, at most 25 % padding when a call holds more than one image).  Returns one list of image
+    indices per call, in call order."""
+    if not sizes:
+        return []
+    th, tw = max(h for h, _ in sizes), max(w for _, w in sizes)
+    return [[r["img"] for r in p["windows"]] for p in ragged_plan(sizes, th, tw, max_pass_pixels)]
+
+
 def _stream_ptr(device: torch.device) -> ctypes.c_void_p:
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -712,6 +724,124 @@ class Engine:
                                                ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
         _lib.check(rc, "wn_enhance_u8_ragged")
         return outs
+
+    # ---- ragged batches of fp32 tensors (wn_forward_ragged, wn_forward_train_ragged / wn_backward_ragged) ---------
+    def _ragged_items(self, items):
+        """items: [(x, wb, he, gc), ...], each four (N_i,3,H_i,W_i) tensors.  Returns the checked inputs, one
+        contiguous output per item and the flat list of its images as (item, index in the item, h, w), zero-pixel
+        images left out."""
+        ins, outs, images = [], [], []
+        for i, item in enumerate(items):
+            if len(item) != 4:
+                raise ValueError(f"item {i}: expected the four tensors (x, wb, he, gc), got {len(item)}")
+            t = self._check_inputs(item)
+            n, _, h, w = t[0].shape
+            ins.append(t)
+            outs.append(torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device))
+            if h * w > 0:
+                images += [(i, j, h, w) for j in range(n)]
+        return ins, outs, images
+
+    @staticmethod
+    def _ragged_tensors(ins, outs, images):
+        """wn_ragged_tensors descriptors of ``images`` (as ``_ragged_items`` lists them)."""
+        table = (_lib.RaggedTensors * len(images))()
+        for k, (i, j, h, w) in enumerate(images):
+            t = ins[i]
+            d = table[k]
+            d.x, d.wb, d.he, d.gc = (u[j].data_ptr() for u in t)
+            d.in_strides[:] = [s for u in t for s in u.stride()]
+            d.out = outs[i][j].data_ptr()
+            d.height, d.width = h, w
+        return table
+
+    def forward_ragged_workspace_bytes(self, sizes, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
+                                       max_pass_pixels: int = 0) -> int:
+        """Workspace of one ``forward_ragged`` call over images of ``sizes`` [(h, w), ...]
+        (wn_forward_ragged_workspace_bytes); 0 for rejected arguments."""
+        th, tw = self._tile_hw(tile)
+        n = len(sizes)
+        hs = (ctypes.c_int * max(1, n))(*[int(h) for h, _ in sizes])
+        ws = (ctypes.c_int * max(1, n))(*[int(w) for _, w in sizes])
+        return int(self.lib.wn_forward_ragged_workspace_bytes(hs, ws, n, th, tw, int(max_pass_pixels), mode))
+
+    def forward_ragged(self, items, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT, max_pass_pixels: int = 0) -> list:
+        """``forward`` of images of their own sizes in one call (wn_forward_ragged).  ``items``: a list of 4-tuples
+        (x, wb, he, gc) of (N_i,3,H_i,W_i) CUDA tensors of any strides; every image of every item is one entry of the
+        ragged batch.  Returns one contiguous (N_i,3,H_i,W_i) output per item, each image bit for bit what ``forward``
+        returns for it alone (while the e4m3 range guard stays down).  ``tile`` and ``max_pass_pixels`` as in
+        ``enhance_ragged``.  Tensor-core modes only."""
+        th, tw = self._tile_hw(tile)
+        ins, outs, images = self._ragged_items(items)
+        if not images:
+            return outs
+        nbytes = self.forward_ragged_workspace_bytes([(h, w) for _, _, h, w in images], (th, tw), mode,
+                                                     max_pass_pixels)
+        ws = self._workspace("forward", nbytes)
+        table = self._ragged_tensors(ins, outs, images)
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_forward_ragged(self.handle, table, len(images), th, tw, int(max_pass_pixels), mode,
+                                            ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
+        _lib.check(rc, "wn_forward_ragged")
+        return outs
+
+    def _train_ragged_workspace(self, nbytes: int) -> torch.Tensor:
+        """One training call's own workspace (it lives until backward)."""
+        return torch.empty(int(nbytes), dtype=torch.uint8, device=self.device)
+
+    def forward_train_ragged(self, items):
+        """``forward_train`` of images of their own sizes (wn_forward_train_ragged): ``items`` as ``forward_ragged``.
+        The images are grouped into training calls by ``ragged_train_calls``; each call runs its images as one pass
+        of equally sized slots and keeps the activations in its own workspace.  Returns (one output per item, saved
+        state for ``backward_ragged``).  Each image's output equals ``forward_train`` of that image alone bit for
+        bit.  One image over TRAIN_MAX_PIXELS is refused."""
+        ins, outs, images = self._ragged_items(items)
+        for i, j, h, w in images:
+            if h * w > self.TRAIN_MAX_PIXELS:
+                raise _lib.WaterNetLibraryError(
+                    f"item {i}: one {h}x{w} image exceeds the {self.TRAIN_MAX_PIXELS >> 20} Mi pixels of one training "
+                    "call; set WaterNet.grad_tile to train it in overlapping windows (wn_backward_tiled)")
+        calls = []
+        for idx in ragged_train_calls([(h, w) for _, _, h, w in images], self.TRAIN_MAX_PIXELS):
+            imgs = [images[k] for k in idx]
+            hs = (ctypes.c_int * len(imgs))(*[h for _, _, h, _ in imgs])
+            wss = (ctypes.c_int * len(imgs))(*[w for _, _, _, w in imgs])
+            ws = self._train_ragged_workspace(self.lib.wn_train_ragged_workspace_bytes(hs, wss, len(imgs)))
+            table = self._ragged_tensors(ins, outs, imgs)
+            with torch.cuda.device(self.device):
+                rc = self.lib.wn_forward_train_ragged(self.handle, table, len(imgs), ws.data_ptr(), ws.numel(),
+                                                      _stream_ptr(self.device))
+            _lib.check(rc, "wn_forward_train_ragged")
+            calls.append((imgs, hs, wss, ws))
+        return outs, calls
+
+    def backward_ragged(self, grad_outs, saved, shapes, want_inputs=None):
+        """d(loss)/d(out) of every item (a list of (N_i,3,H_i,W_i) tensors) + the state of ``forward_train_ragged``
+        -> the 34 parameter gradients (state-dict order), the gradients of all images summed call by call in call
+        order, and one list of four input gradients per item (None where ``want_inputs[i][t]`` is false, or
+        everywhere when ``want_inputs`` is None)."""
+        grads_out = [g.detach().to(self.device, torch.float32).contiguous() for g in grad_outs]
+        saved = saved or []
+        make = torch.empty if saved else torch.zeros  # no images: zero gradients
+        grads = [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
+        part = grads if len(saved) <= 1 else [torch.empty_like(t) for t in grads]
+        # every image with pixels is written whole by its call; zero-pixel items are never passed to the library
+        gin = [[torch.empty_like(g) if want_inputs is not None and want_inputs[i][t] else None for t in range(4)]
+               for i, g in enumerate(grads_out)]
+        for k, (imgs, hs, wss, ws) in enumerate(saved):
+            arr = (ctypes.c_void_p * _lib.NUM_PARAMS)(*[t.data_ptr() for t in (grads if k == 0 else part)])
+            gptr = (ctypes.c_void_p * len(imgs))(*[grads_out[i][j].data_ptr() for i, j, _, _ in imgs])
+            gin_arr = None
+            if any(t is not None for row in gin for t in row):
+                gin_arr = (ctypes.c_void_p * (4 * len(imgs)))(
+                    *[None if gin[i][t] is None else gin[i][t][j].data_ptr() for i, j, _, _ in imgs for t in range(4)])
+            with torch.cuda.device(self.device):
+                rc = self.lib.wn_backward_ragged(self.handle, hs, wss, gptr, arr, gin_arr, len(imgs), ws.data_ptr(),
+                                                 ws.numel(), _stream_ptr(self.device))
+            _lib.check(rc, "wn_backward_ragged")
+            if k > 0:
+                torch._foreach_add_(grads, part)
+        return grads, gin
 
     # ---- windowed recompute backward (wn_backward_tiled) -------------------------------------------
     def backward_tiled_workspace_bytes(self, n: int, h: int, w: int, tile=DEFAULT_TILE, max_pass_pixels: int = 0) -> int:

@@ -414,6 +414,34 @@ class _KernelForward(torch.autograd.Function):
         return (None, None, None, *gin, *gpar)
 
 
+class _RaggedKernelForward(torch.autograd.Function):
+    """``WaterNet.forward_many`` under autograd: the images of their own sizes through the ragged training step
+    (wn_forward_train_ragged / wn_backward_ragged, the bf16x3 arithmetic of training).  Receives the four inputs of
+    every item, flattened, then the 34 parameters; returns one output per item."""
+
+    @staticmethod
+    def forward(ctx, model, n_items, *tensors):
+        flat, params = tensors[:4 * n_items], tensors[4 * n_items:]
+        items = [flat[4 * i:4 * i + 4] for i in range(n_items)]
+        eng = model._engine_with_weights(items[0][0])
+        outs, ctx.saved_calls = eng.forward_train_ragged(items)
+        ctx.engine, ctx.weights_key, ctx.n_items = eng, eng._weights_key, n_items
+        ctx.shapes = [p.shape for p in params]
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *grad_outs):
+        eng = ctx.engine
+        if eng._weights_key != ctx.weights_key:  # parameters changed between forward and backward
+            raise RuntimeError("model parameters were modified between forward and backward")
+        need = ctx.needs_input_grad[2:]
+        want_in = [need[4 * i:4 * i + 4] for i in range(ctx.n_items)]
+        grads, gin = eng.backward_ragged(grad_outs, ctx.saved_calls, ctx.shapes, want_in)
+        ctx.saved_calls = None
+        gpar = [g if w else None for g, w in zip(grads, need[4 * ctx.n_items:])]
+        return (None, None, *[t for row in gin for t in row], *gpar)
+
+
 class WaterNet(_PackedWeightsMixin, nn.Module):
     """
     Gated fusion network (reference ``net.py:83-108``)::
@@ -531,3 +559,41 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
         if tile is not None:
             return self._engine_with_weights(x).forward_tiled(x, wb, ce, gc, tile, mode)
         return self._kernel_forward(x, wb, ce, gc, mode)
+
+    def forward_many(self, xs, wbs, ces, gcs) -> list:
+        """``forward`` of images of their own sizes: four equally long lists of (N_i,3,H_i,W_i) tensors -> the list of
+        the (N_i,3,H_i,W_i) outputs.  Without an autograd graph one ragged call runs them all (``wn_forward_ragged``,
+        windows of ``tile``, or ``Engine.DEFAULT_TILE`` when that is None); each output equals ``model(...)`` of that
+        item alone bit for bit.  With a graph the images go through the ragged training step in as few calls as fit
+        ``Engine.TRAIN_MAX_PIXELS`` slot pixels each (``wn_forward_train_ragged`` / ``wn_backward_ragged``); gradients
+        reach the parameters and the inputs that require grad, and the parameter gradients are the sum over the
+        images.  With ``grad_tile`` set such a call runs the windowed path of ``forward`` once per item instead.
+        Tensor-core precisions only.
+
+        Cost under autograd: every training call keeps its whole activation workspace (~5.6 KB per slot pixel, slots
+        padded up to 25 %) until backward, so the list holds the activations of all its images at once.  One ragged
+        step pays off for small images, which leave SMs idle one at a time: on one H100 (700 W) 32 images of 64-160
+        pixels per side took 0.84x the time of a per-image loop, while 32 of 64 x 64 to 512 x 384 took 1.12x and
+        about 10x the peak memory (17.3 GB against 1.8).  For larger images loop over the items instead."""
+        mode = self._mode()
+        if mode == _lib.MODE_FP32_SIMT:
+            raise ValueError("forward_many: ragged batches run on the tensor cores only, and precision='fp32' is the "
+                             "CUDA-core mode; use precision='default' or 'bf16x3', or call the model per image")
+        if not (len(xs) == len(wbs) == len(ces) == len(gcs)):
+            raise ValueError("forward_many: xs, wbs, ces and gcs must have the same length")
+        items = list(zip(xs, wbs, ces, gcs))
+        if not items:
+            return []
+        x0 = items[0][0]
+        if not x0.is_cuda:
+            self._engine_for(x0, None)  # raises: there is no CPU path
+        params = list(self.parameters())
+        needs_graph = torch.is_grad_enabled() and (
+            any(t.requires_grad for it in items for t in it) or any(p.requires_grad for p in params))
+        if needs_graph:
+            grad_tile = _checked_grad_tile(self.grad_tile, mode)
+            if grad_tile is not None:
+                return [_KernelForward.apply(self, mode, grad_tile, *it, *params) for it in items]
+            return list(_RaggedKernelForward.apply(self, len(items), *[t for it in items for t in it], *params))
+        tile = _checked_tile(self.tile, mode) or Engine.DEFAULT_TILE
+        return self._engine_with_weights(x0).forward_ragged(items, tile, mode)

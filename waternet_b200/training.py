@@ -67,28 +67,61 @@ def perceptual_loss(vgg, out, ref):
 
 
 def _to_device(batch, device):
-    return [batch[k].to(device, non_blocking=True) for k in ("raw", "wb", "he", "gc", "ref")]
+    """The five batch entries on ``device``: tensors, or lists of per-image tensors (a ragged batch)."""
+    def move(v):
+        return [t.to(device, non_blocking=True) for t in v] if isinstance(v, (list, tuple)) else \
+            v.to(device, non_blocking=True)
+    return [move(batch[k]) for k in ("raw", "wb", "he", "gc", "ref")]
+
+
+def _forward(model, raw, wb, he, gc):
+    """model(...) of a tensor batch; WaterNet.forward_many of a ragged batch (lists of images)."""
+    return model.forward_many(raw, wb, he, gc) if isinstance(raw, list) else model(raw, wb, he, gc)
+
+
+def batch_losses(vgg, out, ref):
+    """(loss, perceptual loss, mse) of a batch, train.py:110-125.  For lists of images (a ragged batch) each term is
+    the mean over the images of that image's term, so loss = mean_i(0.05 perc_i + mse_i): the reference's batch loss
+    when all images have one size."""
+    if not isinstance(out, list):
+        perc = perceptual_loss(vgg, out, ref)
+        mse = torch.mean(torch.square(255 * (out - ref)))
+        return 0.05 * perc + mse, perc, mse
+    perc = torch.stack([perceptual_loss(vgg, o, r) for o, r in zip(out, ref)])
+    mse = torch.stack([torch.mean(torch.square(255 * (o - r))) for o, r in zip(out, ref)])
+    return (0.05 * perc + mse).mean(), perc.mean(), mse.mean()
+
+
+def batch_quality(out, ref):
+    """(SSIM, PSNR) of a batch.  For lists of images: the mean of the per-image SSIMs, and the PSNR of the MSE
+    pooled over every pixel of every image."""
+    if not isinstance(out, list):
+        return ssim(out, ref), psnr(out, ref, 1.0)
+    s = torch.stack([ssim(o, r) for o, r in zip(out, ref)]).mean()
+    sq = sum(torch.sum((o - r) ** 2) for o, r in zip(out, ref))
+    mse = sq / sum(o.numel() for o in out)
+    return s, 10.0 * torch.log10(1.0 / mse)
 
 
 def train_one_epoch(model, loader, optimizer, scheduler, vgg, device, log=None) -> Dict[str, float]:
+    """One epoch; a batch is five tensors, or five lists of images of their own sizes (GpuBatchLoader(ragged=True))."""
     model.train()
     totals = {k: 0.0 for k in TRAIN_METRICS_NAMES}
     for idx, batch in enumerate(loader):
         raw, wb, he, gc, ref = _to_device(batch, device)
-        out = model(raw, wb, he, gc)
-        perc = perceptual_loss(vgg, out, ref)
-        mse = torch.mean(torch.square(255 * (out - ref)))
-        loss = 0.05 * perc + mse
+        out = _forward(model, raw, wb, he, gc)
+        loss, perc, mse = batch_losses(vgg, out, ref)
         optimizer.zero_grad()
         loss.backward()
         optimizer.step()
         scheduler.step()  # per minibatch, like the reference (train.py:133)
         with torch.no_grad():
+            s, p = batch_quality(out, ref)
             totals["loss"] += loss.item()
             totals["perceptual_loss"] += perc.item()
             totals["mse"] += mse.item()
-            totals["ssim"] += ssim(out, ref).item()
-            totals["psnr"] += psnr(out, ref, 1.0).item()
+            totals["ssim"] += s.item()
+            totals["psnr"] += p.item()
         if log is not None and idx and idx % 10 == 0:
             log(f"  batch {idx}/{len(loader)} loss {loss.item():.4g}")
     return {k: v / max(len(loader), 1) for k, v in totals.items()}
@@ -102,11 +135,13 @@ def eval_one_epoch(model, loader, vgg, device) -> Dict[str, float]:
     with torch.no_grad():
         for batch in loader:
             raw, wb, he, gc, ref = _to_device(batch, device)
-            out = model(raw, wb, he, gc)
-            totals["perceptual_loss"] += perceptual_loss(vgg, out, ref).item()
-            totals["mse"] += torch.mean(torch.square(255 * (out - ref))).item()
-            totals["ssim"] += ssim(out, ref).item()
-            totals["psnr"] += psnr(out, ref, 1.0).item()
+            out = _forward(model, raw, wb, he, gc)
+            _, perc, mse = batch_losses(vgg, out, ref)
+            s, p = batch_quality(out, ref)
+            totals["perceptual_loss"] += perc.item()
+            totals["mse"] += mse.item()
+            totals["ssim"] += s.item()
+            totals["psnr"] += p.item()
     model.train()
     return {k: v / max(len(loader), 1) for k, v in totals.items()}
 

@@ -113,19 +113,24 @@ class UIEBDataset(torch.utils.data.Dataset):
 
 
 class SyntheticUIEB(torch.utils.data.Dataset):
-    """UIEB-shaped synthetic pairs: a smooth scene (reference) and a blue-green degraded copy (raw)."""
+    """UIEB-shaped synthetic pairs: a smooth scene (reference) and a blue-green degraded copy (raw).  ``sizes``: a
+    list of (h, w); item idx then has size sizes[idx % len(sizes)] instead of im_height x im_width (a dataset whose
+    items keep their own sizes)."""
 
-    def __init__(self, length: int = 890, im_height: int = 112, im_width: int = 112, seed: int = 0, transform=None):
+    def __init__(self, length: int = 890, im_height: int = 112, im_width: int = 112, seed: int = 0, transform=None,
+                 sizes=None):
         self.length, self.h, self.w, self.seed = length, im_height, im_width, seed
         self.transform = transform
+        self.sizes = list(sizes) if sizes else None
 
     def __len__(self):
         return self.length
 
     def _scene(self, idx):
+        h, w = self.sizes[idx % len(self.sizes)] if self.sizes else (self.h, self.w)
         rng = np.random.default_rng(self.seed * 100003 + idx)
-        coarse = rng.random((self.h // 8 + 2, self.w // 8 + 2, 3))
-        ref = np.kron(coarse, np.ones((8, 8, 1)))[: self.h, : self.w]
+        coarse = rng.random((h // 8 + 2, w // 8 + 2, 3))
+        ref = np.kron(coarse, np.ones((8, 8, 1)))[:h, :w]
         ref = (ref * 255).astype(np.uint8)
         cast = np.array([0.35, 0.8, 0.9])
         raw = (ref.astype(np.float64) * cast * (0.6 + 0.4 * rng.random())).astype(np.uint8)
@@ -154,10 +159,16 @@ class GpuBatchLoader:
     ``wn_preprocess_u8`` produce the five fp32 tensors of the reference's item dictionary, already
     on the device.  ``dataset`` needs ``__len__`` and ``pair(idx) -> (raw_u8, ref_u8)`` (both
     datasets of this module have it); ``torch.utils.data.Subset`` views are accepted.
+
+    ``ragged``: a batch whose items have different sizes (a dataset without im_height / im_width, which keeps every
+    item at its own size) comes as five lists ``raw, wb, gc, he, ref`` of (1,3,H_i,W_i) tensors in batch order, for
+    ``WaterNet.forward_many``.  Each distinct size is resized, augmented and preprocessed as one batch (a quarter
+    turn is applied to a non-square item only in pairs, as in a tensor batch).  A batch of one size still comes as
+    tensors.  Without it (the default) such a batch raises.
     """
 
     def __init__(self, dataset, batch_size: int, device=None, augment: bool = True, seed: Optional[int] = None,
-                 drop_last: bool = False):
+                 drop_last: bool = False, ragged: bool = False):
         from .engine import get_engine
         self.engine = get_engine(device)
         self.indices = list(range(len(dataset)))
@@ -168,6 +179,7 @@ class GpuBatchLoader:
         self.batch_size = batch_size
         self.augment = augment
         self.drop_last = drop_last
+        self.ragged = ragged
         self.rng = np.random.default_rng(seed)
 
     def __len__(self):
@@ -201,22 +213,50 @@ class GpuBatchLoader:
                 break
             if hasattr(self.dataset, "decoded"):
                 # file-backed dataset: cv2.imread on the host, then ONE batched bilinear resize + BGR->RGB on the
-                # device (wn_resize_u8, bit-exact cv2.resize arithmetic) instead of 2 x batch cv2.resize calls
+                # device (wn_resize_u8, bit-exact cv2.resize arithmetic) per target size instead of 2 x batch
+                # cv2.resize calls
                 items = [self.dataset.decoded(i) for i in idx]
-                sizes = {it[2] for it in items}
-                if len(sizes) != 1:
-                    raise ValueError("a batch needs one target size: give the dataset im_height / im_width")
-                (dw, dh), = sizes
-                raw = self.engine.resize_batch([it[0] for it in items], dh, dw, swap_rb=True)
-                ref = self.engine.resize_batch([it[1] for it in items], dh, dw, swap_rb=True)
+                groups = self._groups([(it[2][1], it[2][0]) for it in items])
+                batches = []
+                for (dh, dw), pos in groups:
+                    raw = self.engine.resize_batch([items[p][0] for p in pos], dh, dw, swap_rb=True)
+                    ref = self.engine.resize_batch([items[p][1] for p in pos], dh, dw, swap_rb=True)
+                    batches.append((pos, raw, ref))
             else:
                 pairs = [self.dataset.pair(i) for i in idx]
-                raw = torch.from_numpy(np.stack([p[0] for p in pairs])).to(dev, non_blocking=True)
-                ref = torch.from_numpy(np.stack([p[1] for p in pairs])).to(dev, non_blocking=True)
-            if self.augment:
-                raw, ref = self._augment(raw, ref)
-            pre = self.engine.preprocess(raw, tensors=True, images=False)
-            # u/255 must be the true fp32 quotient (arr2ten): torch's CUDA "tensor / scalar" multiplies by a
-            # reciprocal, so the reference image goes through the library's exact table as well
-            ref_t = self.engine.preprocess(ref, tensors=True, images=False)["x"]
-            yield {"raw": pre["x"], "wb": pre["wb"], "gc": pre["gc"], "he": pre["he"], "ref": ref_t}
+                groups = self._groups([p[0].shape[:2] for p in pairs])
+                batches = []
+                for _, pos in groups:
+                    raw = torch.from_numpy(np.stack([pairs[p][0] for p in pos])).to(dev, non_blocking=True)
+                    ref = torch.from_numpy(np.stack([pairs[p][1] for p in pos])).to(dev, non_blocking=True)
+                    batches.append((pos, raw, ref))
+            done = [(pos, self._tensors(raw, ref)) for pos, raw, ref in batches]
+            if len(done) == 1:
+                yield done[0][1]
+                continue
+            out = {k: [None] * len(idx) for k in ("raw", "wb", "gc", "he", "ref")}
+            for pos, t in done:
+                for j, p in enumerate(pos):
+                    for k in out:
+                        out[k][p] = t[k][j:j + 1]
+            yield out
+
+    def _groups(self, sizes):
+        """[((h, w), [positions in the batch])] in order of first appearance; more than one size only if ragged."""
+        groups = {}
+        for p, s in enumerate(sizes):
+            groups.setdefault(tuple(int(v) for v in s), []).append(p)
+        if len(groups) > 1 and not self.ragged:
+            raise ValueError("a batch needs one target size: give the dataset im_height / im_width, or pass "
+                             "ragged=True for batches of lists")
+        return list(groups.items())
+
+    def _tensors(self, raw: torch.Tensor, ref: torch.Tensor):
+        """Augment and preprocess one batch of equally sized NHWC uint8 pairs -> the five fp32 tensors."""
+        if self.augment:
+            raw, ref = self._augment(raw, ref)
+        pre = self.engine.preprocess(raw, tensors=True, images=False)
+        # u/255 must be the true fp32 quotient (arr2ten): torch's CUDA "tensor / scalar" multiplies by a
+        # reciprocal, so the reference image goes through the library's exact table as well
+        ref_t = self.engine.preprocess(ref, tensors=True, images=False)["x"]
+        return {"raw": pre["x"], "wb": pre["wb"], "gc": pre["gc"], "he": pre["he"], "ref": ref_t}
