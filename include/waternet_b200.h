@@ -28,6 +28,8 @@
  *   wn_forward_train_ragged / wn_backward_ragged
  *                         the same for n images of n sizes in one call (a dataset without a fixed size)
  *   wn_backward_tiled     the same gradients from the inputs alone, recomputed in overlapping windows
+ *   wn_backward_ragged_tiled
+ *                         ... for n images of n sizes in one call
  *   wn_confidence_maps_train / _backward, wn_refine_train / _backward
  *                         the sub-modules under autograd (net.py:45-56, :75-80 with parameters that require grad)
  *   wn_confidence_maps_backward_tiled, wn_refine_backward_tiled
@@ -371,6 +373,34 @@ int wn_backward_tiled(wn_handle* h, const float* x, const float* wb, const float
                       const int64_t in_strides[4][4], const float* grad_out, float* const* grads,
                       float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
                       long long max_pass_pixels, void* workspace, size_t workspace_bytes, void* stream);
+
+/*
+ * The windowed recompute backward of a ragged batch: wn_backward_tiled for n images of their own sizes in one call.
+ * Every image is cut into the windows wn_backward_tiled cuts it into; the windows of all images are sorted by shape
+ * and packed into passes of equally sized slots, as wn_forward_ragged packs them.  For each pass the call recomputes
+ * the training forward (the WN_MODE_BF16X3 arithmetic; the exact-levels decision over every input pixel of the n
+ * images, as wn_forward_ragged takes it) and runs the backward pass with d(loss)/d(out) taken inside each window's kept
+ * rectangle and 0 elsewhere.
+ *   - images_host: HOST array of n wn_ragged_tensors (the inputs of the forward; `out` is not used and may be NULL).
+ *   - grad_out_host: HOST array of n device pointers to fp32 contiguous (1,3,H_i,W_i).  grads: as wn_backward,
+ *     OVERWRITTEN with the gradients of the sum of the n images' losses.  input_grads_host: NULL or a HOST array of
+ *     4n device pointers, image i's d/d(x), d/d(wb), d/d(he), d/d(gc) at 4i .. 4i+3, fp32 contiguous (1,3,H_i,W_i);
+ *     any entry may be NULL.
+ *   - max_pass_pixels: slot pixels per pass, 0 = 2 Mi; at most 8 Mi.  A pass of one window may exceed it, but no
+ *     window may exceed 8 Mi pixels.  At most 65535 windows per pass; n <= 65535.
+ *   - Image i's input gradients equal those of wn_backward_tiled on image i alone at the same tile, bit for bit, and
+ *     do not depend on max_pass_pixels or on the other images.  The parameter gradients equal the sum of the
+ *     per-image ones up to the order of the fp32 sums; for n images of one size they equal wn_backward_tiled of the
+ *     batch bit for bit.  Deterministic, no atomics.
+ *   - The call copies its plan to the device from pageable host memory once, so it cannot be captured in a CUDA
+ *     graph.  The workspace is one pass of training buffers, the scratch parameter gradients and the plan.
+ * wn_backward_ragged_tiled_workspace_bytes returns 0 for every argument set the call rejects.
+ */
+size_t wn_backward_ragged_tiled_workspace_bytes(const int* heights_host, const int* widths_host, int n, int tile_h,
+                                                int tile_w, long long max_pass_pixels);
+int wn_backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images_host, const float* const* grad_out_host,
+                             float* const* grads, float* const* input_grads_host, int n, int tile_h, int tile_w,
+                             long long max_pass_pixels, void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * The windowed recompute backward of one sub-module: the gradients wn_confidence_maps_backward / wn_refine_backward

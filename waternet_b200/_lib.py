@@ -131,6 +131,11 @@ _SIGNATURES = {
     "wn_forward_train_ragged": (c_int, [c_void_p, POINTER(RaggedTensors), c_int, c_void_p, c_size_t, c_void_p]),
     "wn_backward_ragged": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_void_p), POINTER(c_void_p),
                                    POINTER(c_void_p), c_int, c_void_p, c_size_t, c_void_p]),
+    "wn_backward_ragged_tiled_workspace_bytes": (c_size_t, [POINTER(c_int), POINTER(c_int), c_int, c_int, c_int,
+                                                            ctypes.c_longlong]),
+    "wn_backward_ragged_tiled": (c_int, [c_void_p, POINTER(RaggedTensors), POINTER(c_void_p), POINTER(c_void_p),
+                                         POINTER(c_void_p), c_int, c_int, c_int, ctypes.c_longlong, c_void_p, c_size_t,
+                                         c_void_p]),
     "wn_debug_forward_layer": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int,
                                        c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "wn_enable_timing": (c_int, [c_void_p, c_int]),

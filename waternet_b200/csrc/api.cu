@@ -989,6 +989,82 @@ int wn_backward_tiled(wn_handle* h, const float* x, const float* wb, const float
                         max_pass_pixels, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
+// ---- the windowed recompute backward of a ragged batch: the limits of wn_backward_tiled, for every image
+static int backward_ragged_tiled_check(const char* what, const int* hs, const int* ws, int n, int tile_h, int tile_w,
+                                       long long max_pass_pixels) {
+  if (n <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
+    set_error("%s: bad shape n=%d tile=%dx%d max_pass_pixels=%lld", what, n, tile_h, tile_w, max_pass_pixels);
+    return WN_E_INVALID;
+  }
+  if (n > 65535) {
+    set_error("%s: too many images: n=%d", what, n);
+    return WN_E_UNSUPPORTED;
+  }
+  if (max_pass_pixels > kTrainMaxPixels) {
+    set_error("%s: max_pass_pixels=%lld exceeds the %lld pixels of one training pass", what, max_pass_pixels,
+              kTrainMaxPixels);
+    return WN_E_UNSUPPORTED;
+  }
+  for (int i = 0; i < n; i++) {
+    int rc = ragged_check_size(what, i, hs[i], ws[i]);
+    if (rc) return rc;
+    const TileGeom g = tile_geom(hs[i], ws[i], tile_h, tile_w);
+    if ((long long)g.win_h * g.win_w > kTrainMaxPixels) {
+      set_error("%s: a %dx%d window of image %d exceeds the %lld pixels of one training pass; use a smaller tile",
+                what, g.win_h, g.win_w, i, kTrainMaxPixels);
+      return WN_E_UNSUPPORTED;
+    }
+  }
+  return WN_OK;
+}
+
+size_t wn_backward_ragged_tiled_workspace_bytes(const int* heights_host, const int* widths_host, int n, int tile_h,
+                                                int tile_w, long long max_pass_pixels) {
+  if (!heights_host || !widths_host ||
+      backward_ragged_tiled_check("wn_backward_ragged_tiled_workspace_bytes", heights_host, widths_host, n, tile_h,
+                                  tile_w, max_pass_pixels))
+    return 0;
+  return backward_ragged_tiled_workspace_bytes(heights_host, widths_host, n, tile_h, tile_w, max_pass_pixels);
+}
+
+int wn_backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images_host, const float* const* grad_out_host,
+                             float* const* grads, float* const* input_grads_host, int n, int tile_h, int tile_w,
+                             long long max_pass_pixels, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* what = "wn_backward_ragged_tiled";
+  if (!h || !images_host || !grad_out_host || !grads || !workspace) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  for (int i = 0; i < WN_NUM_PARAMS; i++)
+    if (!grads[i]) {
+      set_error("%s: grads[%d] is NULL", what, i);
+      return WN_E_INVALID;
+    }
+  if (n <= 0 || n > 65535) {
+    set_error("%s: 1..65535 images per call, got n=%d", what, n);
+    return n <= 0 ? WN_E_INVALID : WN_E_UNSUPPORTED;
+  }
+  std::vector<int> hs(n), ws(n);
+  for (int i = 0; i < n; i++) {
+    const wn_ragged_tensors& t = images_host[i];
+    if (!t.x || !t.wb || !t.he || !t.gc || !grad_out_host[i]) {
+      set_error("%s: null image pointer (image %d)", what, i);
+      return WN_E_INVALID;
+    }
+    hs[i] = t.height;
+    ws[i] = t.width;
+  }
+  int rc = backward_ragged_tiled_check(what, hs.data(), ws.data(), n, tile_h, tile_w, max_pass_pixels);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  return backward_ragged_tiled(h, images_host, grad_out_host, grads, input_grads_host, n, tile_h, tile_w,
+                               max_pass_pixels, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 // ---- the windowed recompute backward of one sub-module: the limits of wn_backward_tiled
 size_t wn_submodule_backward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w,
                                                    long long max_pass_pixels, int stack) {

@@ -315,5 +315,12 @@ int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, v
                          cudaStream_t stream);
 int backward_ragged(wn_handle* h, const int* hs, const int* ws, const float* const* grad_out, float* const* grads,
                     float* const* input_grads, int n, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+// the windowed recompute backward of a ragged batch (wn_backward_ragged_tiled): the windows and passes of ragged_plan;
+// arguments checked by the caller (api.cu: the limits of wn_backward_tiled for every image)
+size_t backward_ragged_tiled_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
+                                             long long max_pass_pixels);
+int backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images, const float* const* grad_out,
+                          float* const* grads, float* const* input_grads, int n, int tile_h, int tile_w,
+                          long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace wn

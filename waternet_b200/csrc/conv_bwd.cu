@@ -677,6 +677,85 @@ fold_submodule_input_grads_kernel(const uint4* __restrict__ g, SubInputGrads out
   }
 }
 
+// The ragged windowed forms (wn_backward_ragged_tiled): slot blockIdx.y of a pass holds window wins[blockIdx.y] of the
+// plan at its top-left.  The seed reads d(out) of the window's own image at image coordinates inside the kept
+// rectangle and is 0 everywhere else, slot pixels beyond the valid extent included.
+__global__ void __launch_bounds__(256)
+gate_bwd_ragged_tiled_kernel(const RaggedGrads* __restrict__ imgs, const RaggedWindow* __restrict__ wins,
+                             const float* __restrict__ cm, const float* __restrict__ refined, uint4* __restrict__ g8,
+                             uint4* __restrict__ gr3, int slot_h, int slot_w) {
+  const int hw = slot_h * slot_w;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const RaggedWindow& r = wins[blockIdx.y];
+  const int wy = pix / slot_w, wx = pix - wy * slot_w;
+  const int y = r.ys + wy, x = r.xs + wx;
+  const bool kept = wy < r.vh && wx < r.vw && y >= r.ky0 && y < r.ky1 && x >= r.kx0 && x < r.kx1;
+  const size_t ihw = (size_t)r.H * r.W;
+  const float* g = imgs[r.img].g_out;
+  float go[3];
+#pragma unroll
+  for (int k = 0; k < 3; k++) go[k] = kept ? g[k * ihw + (size_t)y * r.W + x] : 0.f;
+  gate_bwd_pixel(go, cm, refined, g8, gr3, blockIdx.y, pix, hw);
+}
+
+// The fold: slot blockIdx.y is plan window p0 + blockIdx.y, and the pass holds plan windows [p0, p0 + count).  An
+// image's windows are contiguous in the plan in ascending tile order (checked on the host), so tile k of the image of
+// plan window w is plan window w - wins[w].tile + k.  Of the windows of the pixel's own image that contain it
+// (tile_cover on that image's tile_geom) and sit in this pass, only the first does the work: it adds their
+// contributions one at a time in ascending tile order to what earlier passes left there, the order of
+// fold_input_grads_kernel for that image alone.  Only the valid extent of a slot is read: the first layer's data
+// gradient has no ReLU mask and is not zero beyond it.  No atomics.
+__global__ void __launch_bounds__(256)
+fold_input_grads_ragged_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb,
+                               const RaggedGrads* __restrict__ imgs, const RaggedWindow* __restrict__ wins,
+                               long long p0, int count, int slot_h, int slot_w, int tile_h, int tile_w) {
+  const int hw = slot_h * slot_w;
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const long long me = p0 + blockIdx.y;
+  const RaggedWindow& r = wins[me];
+  const int wy = pix / slot_w, wx = pix - wy * slot_w;
+  if (wy >= r.vh || wx >= r.vw) return;
+  const int y = r.ys + wy, x = r.xs + wx;
+  const TileGeom tiles = tile_geom(r.H, r.W, tile_h, tile_w);
+  const TileCover c = tile_cover(tiles, y, x);
+  const long long img0 = me - r.tile;
+  long long first = -1;
+  for (int i = c.i0; i <= c.i1 && first < 0; i++)
+    for (int j = c.j0; j <= c.j1; j++) {
+      const long long k = img0 + (long long)i * tiles.nx + j;
+      if (k >= p0 && k < p0 + count) {
+        first = k;
+        break;
+      }
+    }
+  if (first != me) return;
+  const RaggedGrads& d = imgs[r.img];
+  const size_t ihw = (size_t)r.H * r.W, o = (size_t)y * r.W + x;
+  float acc[12];
+#pragma unroll
+  for (int q = 0; q < 4; q++)
+#pragma unroll
+    for (int ch = 0; ch < 3; ch++) acc[q * 3 + ch] = d.in[q] ? d.in[q][o + ch * ihw] : 0.f;
+  for (int i = c.i0; i <= c.i1; i++)
+    for (int j = c.j0; j <= c.j1; j++) {
+      const long long k = img0 + (long long)i * tiles.nx + j;
+      if (k < p0 || k >= p0 + count) continue;
+      const RaggedWindow& u = wins[k];
+      float v[16];
+      input_grads_pixel(ga, gb, (int)(k - p0), (y - u.ys) * slot_w + (x - u.xs), hw, v);
+#pragma unroll
+      for (int q = 0; q < 12; q++) acc[q] += v[q];
+    }
+#pragma unroll
+  for (int q = 0; q < 4; q++) {
+    if (!d.in[q]) continue;
+#pragma unroll
+    for (int ch = 0; ch < 3; ch++) d.in[q][o + ch * ihw] = acc[q * 3 + ch];
+  }
+}
+
 // dst.p[k][i] += src.p[k][i] for the 34 parameter gradients; blockIdx.y = k
 struct ParamGrads {
   float* p[WN_NUM_PARAMS];
@@ -1418,6 +1497,153 @@ int backward_tiled(wn_handle* h, const float* const in[4], const int64_t st[4][4
     if (input_grads) {
       fold_input_grads_kernel<<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(t.gin_a, t.gin_b, ig,
                                                                                                 g, w0, cur);
+      WN_LAUNCH_CHECK(h);
+    }
+  }
+  return WN_OK;
+}
+
+// ---- windowed recompute backward of a ragged batch (wn_backward_ragged_tiled, DESIGN.md 4.11) ---------------------
+// The pass loop of backward_tiled over the plan of ragged_plan: n images of their own sizes, cut into the windows
+// wn_backward_tiled cuts each of them into, sorted by shape and packed into passes of equally sized slots.  Per pass:
+// the bf16x3 training forward of forward_train_ragged (every ReLU layer stores zeros beyond each window's valid
+// extent), the seed from d(out) inside each kept rectangle, the backward pass of the slots, and the fold of the input
+// gradients into their images.  The first pass writes the parameter gradients, every later one a scratch copy that
+// add_param_grads_kernel adds in.  Workspace: [flag | scratch parameter gradients | table: one PackInArgs and one
+// RaggedGrads per image, then the windows in plan order | the largest pass of training buffers].  The table is
+// copied from pageable host memory once per call.
+static size_t ragged_tiled_table_bytes(int n, size_t windows) {
+  return align256b((size_t)n * sizeof(PackInArgs)) + align256b((size_t)n * sizeof(RaggedGrads)) +
+         align256b(windows * sizeof(RaggedWindow));
+}
+
+static void ragged_tiled_plan(const int* hs, const int* ws, int n, int tile_h, int tile_w, long long max_pass_pixels,
+                              std::vector<RaggedWindow>* wins, std::vector<RaggedPass>* passes) {
+  ragged_plan(hs, ws, n, tile_h, tile_w, max_pass_pixels ? max_pass_pixels : kTiledTrainPassPixels, wins, passes);
+}
+
+static size_t ragged_tiled_workspace(int n, const std::vector<RaggedWindow>& wins,
+                                     const std::vector<RaggedPass>& passes) {
+  long long px = 0;
+  for (const RaggedPass& p : passes) px = std::max(px, (long long)p.count * p.slot_h * p.slot_w);
+  return 256 + param_grads_bytes() + ragged_tiled_table_bytes(n, wins.size()) +
+         train_workspace_bytes_padded(1, 1, (int)px) + 256;
+}
+
+size_t backward_ragged_tiled_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
+                                             long long max_pass_pixels) {
+  std::vector<RaggedWindow> wins;
+  std::vector<RaggedPass> passes;
+  ragged_tiled_plan(hs, ws, n, tile_h, tile_w, max_pass_pixels, &wins, &passes);
+  return ragged_tiled_workspace(n, wins, passes);
+}
+
+int backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images, const float* const* grad_out,
+                          float* const* grads, float* const* input_grads, int n, int tile_h, int tile_w,
+                          long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (!h->bwd || !h->umma) {
+    set_error("backward weights have not been packed");
+    return WN_E_STATE;
+  }
+  std::vector<int> hs(n), ws(n);
+  for (int i = 0; i < n; i++) {
+    hs[i] = images[i].height;
+    ws[i] = images[i].width;
+  }
+  std::vector<RaggedWindow> wins;
+  std::vector<RaggedPass> passes;
+  ragged_tiled_plan(hs.data(), ws.data(), n, tile_h, tile_w, max_pass_pixels, &wins, &passes);
+  const size_t need = ragged_tiled_workspace(n, wins, passes);
+  if (workspace_bytes < need) {
+    set_error("ragged tiled backward workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  // the fold's precondition: every image's windows are contiguous in the plan, in ascending tile order
+  std::vector<long long> first(n, -1);
+  for (size_t p = 0; p < wins.size(); p++) {
+    const int i = wins[p].img;
+    if (first[i] < 0) first[i] = (long long)p;
+    if (wins[p].tile != (long long)p - first[i]) {
+      set_error("ragged plan: the windows of image %d are not contiguous in tile order", i);
+      return WN_E_STATE;
+    }
+  }
+  int rc = get_encoder();
+  if (rc) return rc;
+  uint8_t* base = (uint8_t*)align256b((uintptr_t)workspace);
+  int* exact = (int*)base;
+  ParamGrads dst, part;
+  param_grad_sizes(dst.size);
+  uint8_t* p = base + 256;
+  for (int k = 0; k < WN_NUM_PARAMS; k++) {
+    dst.p[k] = grads[k];
+    part.p[k] = (float*)p;
+    part.size[k] = dst.size[k];
+    p += align256b((size_t)dst.size[k] * sizeof(float));
+  }
+  // the table, built on the host in its device layout
+  const size_t in_b = align256b((size_t)n * sizeof(PackInArgs)), g_b = align256b((size_t)n * sizeof(RaggedGrads));
+  std::vector<uint8_t> host(in_b + g_b + wins.size() * sizeof(RaggedWindow));
+  PackInArgs* imgs = reinterpret_cast<PackInArgs*>(host.data());
+  RaggedGrads* rg = reinterpret_cast<RaggedGrads*>(host.data() + in_b);
+  bool want_in = false;
+  for (int i = 0; i < n; i++) {
+    const wn_ragged_tensors& d = images[i];
+    const float* in[4] = {d.x, d.wb, d.he, d.gc};
+    for (int t = 0; t < 4; t++) {
+      imgs[i].p[t] = in[t];
+      for (int k = 0; k < 4; k++) imgs[i].s[t][k] = d.in_strides[t][k];
+    }
+    rg[i].g_out = grad_out[i];
+    for (int t = 0; t < 4; t++) {
+      rg[i].in[t] = input_grads ? input_grads[4 * i + t] : nullptr;
+      if (rg[i].in[t]) {
+        want_in = true;
+        WN_CUDA(cudaMemsetAsync(rg[i].in[t], 0, (size_t)3 * d.height * d.width * sizeof(float), stream));
+      }
+    }
+  }
+  memcpy(host.data() + in_b + g_b, wins.data(), wins.size() * sizeof(RaggedWindow));
+  uint8_t* table = p;
+  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
+  WN_CUDA(cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
+  const PackInArgs* d_imgs = reinterpret_cast<const PackInArgs*>(table);
+  const RaggedGrads* d_grads = reinterpret_cast<const RaggedGrads*>(table + in_b);
+  const RaggedWindow* d_wins = reinterpret_cast<const RaggedWindow*>(table + in_b + g_b);
+  void* pass_ws = table + ragged_tiled_table_bytes(n, wins.size());
+  const size_t pass_bytes = workspace_bytes - (size_t)((uint8_t*)pass_ws - (uint8_t*)workspace);
+  // the first layer drops its a_lo pass exactly when the forward that produced the output did (wn_forward_ragged)
+  WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
+  for (const RaggedPass& q : passes)
+    if ((rc = pack_input_ragged(h, d_imgs, d_wins + q.first, q.count, q.slot_h, q.slot_w, nullptr, exact, stream)))
+      return rc;
+  const int64_t none[4][4] = {};
+  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (size_t pi = 0; pi < passes.size(); pi++) {
+    const RaggedPass& q = passes[pi];
+    if ((rc = check_train_args(q.count, q.slot_h, q.slot_w, pass_bytes))) return rc;
+    TrainBuffers t;
+    carve(&t, pass_ws, (size_t)q.count * q.slot_h * q.slot_w);
+    t.f.exact_flag = exact;
+    if ((rc = pack_input_ragged(h, d_imgs, d_wins + q.first, q.count, q.slot_h, q.slot_w, t.f.act0, exact, stream)))
+      return rc;
+    FwdOpts o;  // the bf16x3 scheme; the backward needs cm and refined, not the output
+    o.packed = true;
+    o.rwin = d_wins + q.first;
+    if ((rc = umma_forward_layers(h, no_in, none, nullptr, q.count, q.slot_h, q.slot_w, t.f, stream, o))) return rc;
+    const dim3 grid((unsigned)(((size_t)q.slot_h * q.slot_w + 255) / 256), q.count);
+    gate_bwd_ragged_tiled_kernel<<<grid, 256, 0, stream>>>(d_grads, d_wins + q.first, t.f.cm, t.f.refined, t.g8,
+                                                           t.gr3, q.slot_h, q.slot_w);
+    WN_LAUNCH_CHECK(h);
+    if ((rc = backward_layers(h, t, pi == 0 ? grads : part.p, want_in, q.count, q.slot_h, q.slot_w, stream)))
+      return rc;
+    if (pi > 0) {
+      add_param_grads_kernel<<<dim3(64, WN_NUM_PARAMS), 256, 0, stream>>>(dst, part);
+      WN_LAUNCH_CHECK(h);
+    }
+    if (want_in) {
+      fold_input_grads_ragged_kernel<<<grid, 256, 0, stream>>>(t.gin_a, t.gin_b, d_grads, d_wins, q.first, q.count,
+                                                               q.slot_h, q.slot_w, tile_h, tile_w);
       WN_LAUNCH_CHECK(h);
     }
   }

@@ -109,7 +109,7 @@ struct RaggedWindow {
   int ys, xs;              // window origin in the image
   int vh, vw;              // valid extent: the window's size
   int ky0, ky1, kx0, kx1;  // kept rectangle, image coordinates
-  int pad_;
+  int tile;                // the window's index within its image (tile_window numbering)
 };
 static_assert(sizeof(RaggedWindow) == 72, "RaggedWindow: engine.RAGGED_WINDOW_BYTES restates this size");
 
@@ -120,7 +120,8 @@ struct RaggedPass {
 };
 
 // max_pass_pixels > 0; the caller has checked n, the sizes and the tile.  Windows go into *wins in pass order
-// (shape sorted: taller first, then wider, then image and window order) with their pointers left null.  A window
+// (shape sorted: taller first, then wider, then image and window order) with their pointers left null.  All windows
+// of one image have one shape, so the stable sort keeps them contiguous and in ascending tile order.  A window
 // joins the open pass unless that would break one of its limits: count x slot pixels <= max_pass_pixels, at most
 // 65535 windows (the grid limit of the apply kernel), and masked padding at most a quarter of the slot pixels.
 inline void ragged_plan(const int* hs, const int* ws, int n, int tile_h, int tile_w, long long max_pass_pixels,
@@ -143,6 +144,7 @@ inline void ragged_plan(const int* hs, const int* ws, int n, int tile_h, int til
       r.ky1 = t.ky1;
       r.kx0 = t.kx0;
       r.kx1 = t.kx1;
+      r.tile = (int)k;
       wins->push_back(r);
     }
   }

@@ -726,10 +726,10 @@ class Engine:
         return outs
 
     # ---- ragged batches of fp32 tensors (wn_forward_ragged, wn_forward_train_ragged / wn_backward_ragged) ---------
-    def _ragged_items(self, items):
+    def _ragged_items(self, items, outputs: bool = True):
         """items: [(x, wb, he, gc), ...], each four (N_i,3,H_i,W_i) tensors.  Returns the checked inputs, one
-        contiguous output per item and the flat list of its images as (item, index in the item, h, w), zero-pixel
-        images left out."""
+        contiguous output per item (None without ``outputs``) and the flat list of its images as (item, index in the
+        item, h, w), zero-pixel images left out."""
         ins, outs, images = [], [], []
         for i, item in enumerate(items):
             if len(item) != 4:
@@ -737,7 +737,7 @@ class Engine:
             t = self._check_inputs(item)
             n, _, h, w = t[0].shape
             ins.append(t)
-            outs.append(torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device))
+            outs.append(torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) if outputs else None)
             if h * w > 0:
                 images += [(i, j, h, w) for j in range(n)]
         return ins, outs, images
@@ -751,7 +751,7 @@ class Engine:
             d = table[k]
             d.x, d.wb, d.he, d.gc = (u[j].data_ptr() for u in t)
             d.in_strides[:] = [s for u in t for s in u.stride()]
-            d.out = outs[i][j].data_ptr()
+            d.out = outs[i][j].data_ptr() if outs[i] is not None else None
             d.height, d.width = h, w
         return table
 
@@ -786,7 +786,7 @@ class Engine:
         return outs
 
     def _train_ragged_workspace(self, nbytes: int) -> torch.Tensor:
-        """One training call's own workspace (it lives until backward)."""
+        """One training call's own workspace (it lives until backward), or that of one backward_ragged_tiled call."""
         return torch.empty(int(nbytes), dtype=torch.uint8, device=self.device)
 
     def forward_train_ragged(self, items):
@@ -883,6 +883,59 @@ class Engine:
                                             _stream_ptr(self.device))
         _lib.check(rc, "wn_backward_tiled")
         return (grads, gin) if want_input_grads else grads
+
+    # ---- windowed recompute backward of a ragged batch (wn_backward_ragged_tiled) -------------------------------
+    def backward_ragged_tiled_workspace_bytes(self, sizes, tile=DEFAULT_TILE, max_pass_pixels: int = 0) -> int:
+        """Workspace of one ``backward_ragged_tiled`` call over images of ``sizes`` [(h, w), ...]
+        (wn_backward_ragged_tiled_workspace_bytes); 0 for rejected arguments."""
+        th, tw = self._tile_hw(tile)
+        n = len(sizes)
+        hs = (ctypes.c_int * max(1, n))(*[int(h) for h, _ in sizes])
+        ws = (ctypes.c_int * max(1, n))(*[int(w) for _, w in sizes])
+        return int(self.lib.wn_backward_ragged_tiled_workspace_bytes(hs, ws, n, th, tw, int(max_pass_pixels)))
+
+    def backward_ragged_tiled(self, grad_outs, items, shapes, tile=DEFAULT_TILE, want_inputs=None,
+                              max_pass_pixels: int = 0):
+        """The gradients of ``backward_ragged`` from the input images alone (wn_backward_ragged_tiled): ``items`` as
+        ``forward_ragged`` takes them, ``grad_outs`` one (N_i,3,H_i,W_i) tensor per item.  The windows of ``tile`` of
+        every image are packed into passes of ``max_pass_pixels`` slot pixels (0 = 2 Mi), and the training forward
+        is recomputed one pass at a time, so no activation outlives the call.  Returns the 34 parameter gradients
+        (state-dict order, summed over the images) and one list of four input gradients per item (None where
+        ``want_inputs[i][t]`` is false, or everywhere when ``want_inputs`` is None).  Zero-pixel items get zero
+        gradients.  The workspace is allocated for this call only."""
+        th, tw = self._tile_hw(tile)
+        ins, _, images = self._ragged_items(items, outputs=False)
+        grads_out = [g.detach().to(self.device, torch.float32).contiguous() for g in grad_outs]
+        for i, (t, g) in enumerate(zip(ins, grads_out)):
+            if g.shape != t[0].shape:
+                raise ValueError(f"item {i}: the output gradient must be {tuple(t[0].shape)}, got {tuple(g.shape)}")
+        make = torch.empty if images else torch.zeros  # no images: zero gradients
+        grads = [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
+        # every image with pixels is written whole by the call; zero-pixel items have no elements
+        gin = [[torch.empty_like(g) if want_inputs is not None and want_inputs[i][t] else None for t in range(4)]
+               for i, g in enumerate(grads_out)]
+        if not images:
+            return grads, gin
+        sizes = [(h, w) for _, _, h, w in images]
+        nbytes = self.backward_ragged_tiled_workspace_bytes(sizes, (th, tw), max_pass_pixels)
+        if nbytes == 0:
+            raise _lib.WaterNetLibraryError(
+                f"wn_backward_ragged_tiled rejects {len(images)} images up to {max(h for h, _ in sizes)}x"
+                f"{max(w for _, w in sizes)} at tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
+        ws = self._train_ragged_workspace(nbytes)
+        table = self._ragged_tensors(ins, [None] * len(ins), images)
+        gptr = (ctypes.c_void_p * len(images))(*[grads_out[i][j].data_ptr() for i, j, _, _ in images])
+        arr = (ctypes.c_void_p * _lib.NUM_PARAMS)(*[t.data_ptr() for t in grads])
+        gin_arr = None
+        if any(t is not None for row in gin for t in row):
+            gin_arr = (ctypes.c_void_p * (4 * len(images)))(
+                *[None if gin[i][t] is None else gin[i][t][j].data_ptr() for i, j, _, _ in images for t in range(4)])
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_backward_ragged_tiled(self.handle, table, gptr, arr, gin_arr, len(images), th, tw,
+                                                   int(max_pass_pixels), ws.data_ptr(), ws.numel(),
+                                                   _stream_ptr(self.device))
+        _lib.check(rc, "wn_backward_ragged_tiled")
+        return grads, gin
 
     # ---- windowed recompute backward of one sub-module (wn_confidence_maps_backward_tiled, wn_refine_backward_tiled) --
     def submodule_backward_tiled_workspace_bytes(self, n: int, h: int, w: int, stack: int, tile=DEFAULT_TILE,

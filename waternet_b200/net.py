@@ -417,16 +417,28 @@ class _KernelForward(torch.autograd.Function):
 class _RaggedKernelForward(torch.autograd.Function):
     """``WaterNet.forward_many`` under autograd: the images of their own sizes through the ragged training step
     (wn_forward_train_ragged / wn_backward_ragged, the bf16x3 arithmetic of training).  Receives the four inputs of
-    every item, flattened, then the 34 parameters; returns one output per item."""
+    every item, flattened, then the 34 parameters; returns one output per item.  With ``grad_tile`` the forward keeps
+    nothing but the inputs (wn_forward_ragged in the bf16x3 arithmetic of training) and the backward recomputes the
+    activations window by window (wn_backward_ragged_tiled); both hold at most one pass of TRAIN_PASS_PIXELS slot
+    pixels."""
 
     @staticmethod
-    def forward(ctx, model, n_items, *tensors):
+    def forward(ctx, model, grad_tile, n_items, *tensors):
         flat, params = tensors[:4 * n_items], tensors[4 * n_items:]
         items = [flat[4 * i:4 * i + 4] for i in range(n_items)]
         eng = model._engine_with_weights(items[0][0])
-        outs, ctx.saved_calls = eng.forward_train_ragged(items)
-        ctx.engine, ctx.weights_key, ctx.n_items = eng, eng._weights_key, n_items
+        ctx.engine, ctx.weights_key, ctx.n_items, ctx.grad_tile = eng, eng._weights_key, n_items, grad_tile
         ctx.shapes = [p.shape for p in params]
+        if grad_tile is not None:
+            # refuse here what the backward would refuse (a window over the pixels of one training pass)
+            sizes = [tuple(x.shape[2:]) for x, *_ in items for _ in range(x.shape[0]) if x.shape[2] * x.shape[3]]
+            if sizes and eng.backward_ragged_tiled_workspace_bytes(sizes, grad_tile, TRAIN_PASS_PIXELS) == 0:
+                raise _lib.WaterNetLibraryError(
+                    f"forward_many: wn_backward_ragged_tiled rejects these images at grad_tile={grad_tile} (a window "
+                    f"may have at most {Engine.TRAIN_MAX_PIXELS >> 20} Mi pixels); use a smaller grad_tile")
+            ctx.save_for_backward(*flat)
+            return tuple(eng.forward_ragged(items, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS))
+        outs, ctx.saved_calls = eng.forward_train_ragged(items)
         return tuple(outs)
 
     @staticmethod
@@ -434,12 +446,18 @@ class _RaggedKernelForward(torch.autograd.Function):
         eng = ctx.engine
         if eng._weights_key != ctx.weights_key:  # parameters changed between forward and backward
             raise RuntimeError("model parameters were modified between forward and backward")
-        need = ctx.needs_input_grad[2:]
+        need = ctx.needs_input_grad[3:]
         want_in = [need[4 * i:4 * i + 4] for i in range(ctx.n_items)]
-        grads, gin = eng.backward_ragged(grad_outs, ctx.saved_calls, ctx.shapes, want_in)
-        ctx.saved_calls = None
+        if ctx.grad_tile is not None:
+            flat = ctx.saved_tensors
+            items = [flat[4 * i:4 * i + 4] for i in range(ctx.n_items)]
+            grads, gin = eng.backward_ragged_tiled(grad_outs, items, ctx.shapes, ctx.grad_tile, want_in,
+                                                   max_pass_pixels=TRAIN_PASS_PIXELS)
+        else:
+            grads, gin = eng.backward_ragged(grad_outs, ctx.saved_calls, ctx.shapes, want_in)
+            ctx.saved_calls = None
         gpar = [g if w else None for g, w in zip(grads, need[4 * ctx.n_items:])]
-        return (None, None, *[t for row in gin for t in row], *gpar)
+        return (None, None, None, *[t for row in gin for t in row], *gpar)
 
 
 class WaterNet(_PackedWeightsMixin, nn.Module):
@@ -567,14 +585,20 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
         item alone bit for bit.  With a graph the images go through the ragged training step in as few calls as fit
         ``Engine.TRAIN_MAX_PIXELS`` slot pixels each (``wn_forward_train_ragged`` / ``wn_backward_ragged``); gradients
         reach the parameters and the inputs that require grad, and the parameter gradients are the sum over the
-        images.  With ``grad_tile`` set such a call runs the windowed path of ``forward`` once per item instead.
-        Tensor-core precisions only.
+        images.  Tensor-core precisions only.
 
         Cost under autograd: every training call keeps its whole activation workspace (~5.6 KB per slot pixel, slots
         padded up to 25 %) until backward, so the list holds the activations of all its images at once.  One ragged
         step pays off for small images, which leave SMs idle one at a time: on one H100 (700 W) 32 images of 64-160
         pixels per side took 0.84x the time of a per-image loop, while 32 of 64 x 64 to 512 x 384 took 1.12x and
-        about 10x the peak memory (17.3 GB against 1.8).  For larger images loop over the items instead."""
+        about 10x the peak memory (17.3 GB against 1.8).
+
+        With ``grad_tile`` set such a call keeps only the inputs: the outputs are one ``wn_forward_ragged`` call in the
+        bf16x3 arithmetic of training, and backward is one ``wn_backward_ragged_tiled`` call that recomputes the
+        windows of all images, packed into passes of ``TRAIN_PASS_PIXELS`` slot pixels, in about 12 GB whatever the
+        list.  Outputs and input gradients equal those of ``model(...)`` of each item under the same ``grad_tile``
+        bit for bit; the parameter gradients are their sum up to the order of fp32 sums.  A list with a window over
+        ``Engine.TRAIN_MAX_PIXELS`` is refused here, not in backward."""
         mode = self._mode()
         if mode == _lib.MODE_FP32_SIMT:
             raise ValueError("forward_many: ragged batches run on the tensor cores only, and precision='fp32' is the "
@@ -592,8 +616,7 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
             any(t.requires_grad for it in items for t in it) or any(p.requires_grad for p in params))
         if needs_graph:
             grad_tile = _checked_grad_tile(self.grad_tile, mode)
-            if grad_tile is not None:
-                return [_KernelForward.apply(self, mode, grad_tile, *it, *params) for it in items]
-            return list(_RaggedKernelForward.apply(self, len(items), *[t for it in items for t in it], *params))
+            return list(_RaggedKernelForward.apply(self, grad_tile, len(items), *[t for it in items for t in it],
+                                                   *params))
         tile = _checked_tile(self.tile, mode) or Engine.DEFAULT_TILE
         return self._engine_with_weights(x0).forward_ragged(items, tile, mode)
