@@ -507,6 +507,50 @@ int wn_memcpy_async(void* dst, const void* src, size_t bytes, void* stream);
 int wn_stream_write_value32(void* stream, void* addr, uint32_t value);
 int wn_stream_wait_value32(void* stream, void* addr, uint32_t value);
 
+/*
+ * The VGG19 perceptual loss of training, and its gradient, in overlapping windows (DESIGN.md 4.12):
+ *
+ *   L = mean over (n, c < 512, i < floor(H/16), j < floor(W/16)) of (255 * (F(out) - F(ref)))^2
+ *
+ * F = VGG19 features[:-1] (conv5_4 + ReLU) of (v - mean) / std with the ImageNet mean and std.  Every convolution
+ * is bf16x3 with fp32 accumulation; a max-pool takes the first maximum in row-major order.  No VGG weight gradient
+ * is computed.
+ *
+ * wn_vgg_pack_weights: params = weight and bias of the 16 convolutions in `features` order (fp32, contiguous OIHW
+ *   and O), device pointers.  Packs the forward and the data-gradient stages; call again after the weights change.
+ * wn_perceptual_loss: out and ref are (n, 3, H, W) fp32 with element strides (sN, sC, sH, sW).  *loss_dev (device
+ *   fp32) receives L.  grad_out, when not NULL, receives dL/d(out) as a contiguous (n, 3, H, W) fp32 tensor; ref
+ *   is a constant.  A window owns a rectangle of features (tile_h x tile_w input pixels, rounded up to multiples of
+ *   16) and reads 128 pixels of context per side, clamped to the image; tile_h = tile_w = 0 makes one window per
+ *   image.  Windows of one extent run in passes of at most max_pass_pixels window pixels (0 = 2 Mi, at most 8 Mi,
+ *   at least one window per pass); memory is bounded by one pass, about 1.9 KB per window pixel.  Limits: n in
+ *   1..65535, H and W at least 16, no window over 8 Mi pixels.  The result is deterministic and independent of the
+ *   workspace contents and of max_pass_pixels.  The call copies nothing from the host.
+ * wn_perceptual_loss_workspace_bytes: the workspace of that call; 0 for every argument set it rejects.
+ * wn_debug_vgg_layer (test aid): layer 0..19 = the output of launch `layer` of the forward (the 16 convolutions and
+ *   4 pools in features order) of x, whole images, tile 0 x 0, all n in one pass, as fp32 (n, C, H >> level,
+ *   W >> level); layer 20 = the conv5_4 features of the windowed call with that tile, as (n, 512, H/16, W/16).
+ *   The backward of the loss of (out = x, ref), whole images, tile 0 x 0: layer 21 = the seed (the gradient with
+ *   respect to conv5_4 before its ReLU, (n, 512, H >> 4, W >> 4)); layer 22 + k = the output of the backward launch
+ *   of forward launch k, the gradient with respect to that launch's input (k = 0: the 16 normalised channels, 3
+ *   real).  ref and ref_strides may be NULL for layers 0..20.  The workspace is that of
+ *   wn_perceptual_loss_workspace_bytes(n, H, W, tile_h, tile_w, 0).
+ *
+ * WN_ABI_VERSION stays 11: these four entry points are additions and no existing signature or structure changed,
+ * so a library built before them still serves every client that does not call them (as with wn_backward_ragged_tiled).
+ */
+#define WN_VGG_NUM_PARAMS 32
+int wn_vgg_pack_weights(wn_handle* h, const float* const* params, void* stream);
+size_t wn_perceptual_loss_workspace_bytes(int n, int height, int width, int tile_h, int tile_w,
+                                          long long max_pass_pixels);
+int wn_perceptual_loss(wn_handle* h, const float* out, const int64_t out_strides[4], const float* ref,
+                       const int64_t ref_strides[4], int n, int height, int width, int tile_h, int tile_w,
+                       long long max_pass_pixels, float* loss_dev, float* grad_out, void* workspace,
+                       size_t workspace_bytes, void* stream);
+int wn_debug_vgg_layer(wn_handle* h, const float* x, const int64_t strides[4], const float* ref,
+                       const int64_t ref_strides[4], int n, int height, int width, int tile_h, int tile_w, int layer,
+                       float* dst, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -26,6 +26,7 @@ def main():
     ap.add_argument("--epochs", type=int, default=400, help="accepted for command-line compatibility with the reference's "
                                                             "score.py (:96); scoring runs one validation pass")
     ap.add_argument("--synthetic", action="store_true")
+    T.add_perceptual_args(ap)
     args = ap.parse_args()
     assert args.weights is not None, "No weights specified in --weights!"
     if args.seed is not None:
@@ -44,7 +45,7 @@ def main():
     model = WaterNet()
     model.load_state_dict(torch.load(args.weights, map_location="cpu"))
     model.to(device).eval()
-    vgg = T.PerceptualModel().to(device).eval()
+    vgg = T.perceptual_model(args).to(device).eval()
     metrics = T.eval_one_epoch(model, loader, vgg, device)
     print("    Val   ||", "   ".join(f"{k}: {v:.03g}" for k, v in metrics.items()))
     print(f"Total time: {timer() - start}s")

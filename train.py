@@ -43,6 +43,7 @@ def main():
                          "rounded down to a multiple of 32, as the reference does) and batches of differently sized "
                          "images through WaterNet.forward_many.  With --synthetic: a mix of sizes around "
                          "--height x --width")
+    T.add_perceptual_args(ap)
     args = ap.parse_args()
     if args.native_size and args.loader != "gpu":
         raise SystemExit("--native-size needs --loader gpu (ragged batches are assembled on the device)")
@@ -86,7 +87,7 @@ def main():
     model.to(device).train()
     optimizer = torch.optim.Adam(model.parameters(), lr=1e-3)
     scheduler = torch.optim.lr_scheduler.StepLR(optimizer, step_size=10000, gamma=0.1)
-    vgg = T.PerceptualModel().to(device).eval()
+    vgg = T.perceptual_model(args).to(device).eval()
 
     train_hist, val_hist = [], []
     for epoch in range(args.epochs):

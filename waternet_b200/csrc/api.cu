@@ -105,6 +105,7 @@ void wn_destroy(wn_handle* h) {
   simt_free(h);
   umma_free(h);
   bwd_free(h);
+  vgg_free(h);
   if (h->d_tables) cudaFree(h->d_tables);
   if (h->timing) {
     for (int i = 0; i < h->timing->created; i++) {
@@ -1159,6 +1160,50 @@ int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const 
                             (cudaStream_t)stream);
   return umma_debug_layer(h, in, in_strides, n, height, width, layer, dst, workspace, workspace_bytes,
                           (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0);
+}
+
+// ---- the VGG19 perceptual loss (vgg.cu)
+int wn_vgg_pack_weights(wn_handle* h, const float* const* params, void* stream) {
+  if (!h || !params) {
+    set_error("wn_vgg_pack_weights: null argument");
+    return WN_E_INVALID;
+  }
+  for (int i = 0; i < WN_VGG_NUM_PARAMS; i++)
+    if (!params[i]) {
+      set_error("wn_vgg_pack_weights: params[%d] is NULL", i);
+      return WN_E_INVALID;
+    }
+  DeviceGuard guard(h->device);
+  return vgg_pack_weights(h, params, (cudaStream_t)stream);
+}
+
+size_t wn_perceptual_loss_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels) {
+  return vgg_loss_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels);
+}
+
+int wn_perceptual_loss(wn_handle* h, const float* out, const int64_t out_strides[4], const float* ref,
+                       const int64_t ref_strides[4], int n, int height, int width, int tile_h, int tile_w,
+                       long long max_pass_pixels, float* loss_dev, float* grad_out, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+  if (!h || !out || !out_strides || !ref || !ref_strides || !loss_dev || !workspace) {
+    set_error("wn_perceptual_loss: null argument");
+    return WN_E_INVALID;
+  }
+  DeviceGuard guard(h->device);
+  return vgg_perceptual_loss(h, out, out_strides, ref, ref_strides, n, height, width, tile_h, tile_w, max_pass_pixels,
+                             loss_dev, grad_out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int wn_debug_vgg_layer(wn_handle* h, const float* x, const int64_t strides[4], const float* ref,
+                       const int64_t ref_strides[4], int n, int height, int width, int tile_h, int tile_w, int layer,
+                       float* dst, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!h || !x || !strides || !dst || !workspace) {
+    set_error("wn_debug_vgg_layer: null argument");
+    return WN_E_INVALID;
+  }
+  DeviceGuard guard(h->device);
+  return vgg_debug_layer(h, x, strides, ref, ref_strides, n, height, width, tile_h, tile_w, layer, dst, workspace,
+                         workspace_bytes, (cudaStream_t)stream);
 }
 
 int wn_enable_timing(wn_handle* h, int on) {

@@ -57,6 +57,7 @@ struct SimtLayer {
 
 struct UmmaWeights;  // conv_umma.cu
 struct UmmaBwd;      // conv_bwd.cu
+struct VggWeights;   // vgg.cu
 
 // Optional per-kernel timing with CUDA events on the launching stream (bench.py's roofline leg).
 enum TimingSlot {
@@ -92,6 +93,7 @@ struct wn_handle {
   wn::Timing* timing;
   wn::UmmaBwd* bwd;
   long long chunk_pixels;  // cap on pixels per pass of the tensor-core forward (0 = default, wn_set_chunk_pixels)
+  wn::VggWeights* vgg;     // the perceptual loss's VGG19 stages (wn_vgg_pack_weights)
 };
 
 namespace wn {
@@ -322,5 +324,18 @@ size_t backward_ragged_tiled_workspace_bytes(const int* hs, const int* ws, int n
 int backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images, const float* const* grad_out,
                           float* const* grads, float* const* input_grads, int n, int tile_h, int tile_w,
                           long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+
+// vgg.cu: the windowed VGG19 perceptual loss (wn_perceptual_loss).  The workspace function returns 0, and the calls
+// fail with the reason set, for every argument set the loss rejects.
+int vgg_pack_weights(wn_handle* h, const float* const* params, cudaStream_t stream);
+void vgg_free(wn_handle* h);
+size_t vgg_loss_workspace_bytes(int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels);
+int vgg_perceptual_loss(wn_handle* h, const float* out, const int64_t out_strides[4], const float* ref,
+                        const int64_t ref_strides[4], int n, int height, int width, int tile_h, int tile_w,
+                        long long max_pass_pixels, float* loss, float* grad_out, void* workspace,
+                        size_t workspace_bytes, cudaStream_t stream);
+int vgg_debug_layer(wn_handle* h, const float* x, const int64_t strides[4], const float* ref,
+                    const int64_t ref_strides[4], int n, int height, int width, int tile_h, int tile_w, int layer,
+                    float* dst, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace wn

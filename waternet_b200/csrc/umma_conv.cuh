@@ -138,7 +138,10 @@ struct UmmaCfg {
   static_assert((KS * KS) % TPS == 0, "taps per weight stage must divide the filter");
   static constexpr int NSTAGE_PER_CHUNK = KS * KS / TPS;
   static constexpr int STAGING = 2 * 64 * kStageLd * 4;
-  static constexpr int BUDGET = 227 * 1024 - 1024 - 2048 - STAGING;
+  // barriers (512 B) + the biases of every column group: 2048 B, more for layers over 384 channels (VGG's 512)
+  static constexpr int BIAS_BYTES = NG * NBLK * NPAD * 4;
+  static constexpr int TAIL = 512 + (BIAS_BYTES > 1536 ? BIAS_BYTES : 1536);
+  static constexpr int BUDGET = 227 * 1024 - 1024 - TAIL - STAGING;
   // halo ring: enough stages to prefetch the next chunk (or the next tile when there is one chunk)
   // (a 1x1 layer is HBM-bound and its stages are small: keep more loads in flight)
   static constexpr int NA_WANT = NCHUNK == 1 ? 2 : KS == 1 ? 6 : 3;
@@ -153,7 +156,7 @@ struct UmmaCfg {
   static constexpr int COLS = NBLK * BLK_COLS;             // accumulator columns of the tile
   static constexpr int ACC = COLS / 2;                     // fp32 accumulator registers per thread (M = 64 per warpgroup)
   static constexpr int ACC8 = F8IN ? ACC : 1;              // ... of the fp8 correction product
-  static constexpr int SMEM_BYTES = NA * A_STAGE + NB * B_STAGE + STAGING + 2048 + 1024;  // + barriers/bias + align slack
+  static constexpr int SMEM_BYTES = NA * A_STAGE + NB * B_STAGE + STAGING + TAIL + 1024;  // + barriers/bias + align slack
   static_assert(NA >= 1, "halo tile does not fit in shared memory");
   static_assert(NCHUNK % NBLK == 0, "chunks must split evenly over the diagonal blocks");
   static_assert(NPAD % 16 == 0 && (DUAL ? 2 : 1) * NPAD <= 256, "invalid wgmma N");
@@ -386,7 +389,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
   uint64_t* b_full = a_empty + C::NA;
   uint64_t* b_empty = b_full + C::NB;
   float* s_bias = reinterpret_cast<float*>(tail + 512);
-  static_assert((2 * 6 + 2 * 8) * 8 <= 512 && NG * NBLK * NPAD * 4 <= 2048 - 512, "barrier / bias area");
+  static_assert((2 * 6 + 2 * 8) * 8 <= 512 && C::BIAS_BYTES <= C::TAIL - 512, "barrier / bias area");
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int num_tiles = g.tiles_x * g.tiles_y * g.N * NG;

@@ -132,6 +132,81 @@ def ragged_train_calls(sizes, max_pass_pixels: int) -> list:
     return [[r["img"] for r in p["windows"]] for p in ragged_plan(sizes, th, tw, max_pass_pixels)]
 
 
+VGG_HALO = 128                  # input pixels a perceptual-loss window reads beyond its features, per side
+VGG_SUPPORT = (-118, 133)       # input rows (columns) conv5_4 feature i depends on: [16 i - 118, 16 i + 133]
+VGG_PASS_PIXELS = 2 << 20       # max_pass_pixels = 0 of wn_perceptual_loss
+VGG_MAX_PIXELS = 8 << 20        # cap on a window and on max_pass_pixels
+VGG_SEED_BLOCKS = 16            # float64 loss partials per window
+# (cin, cout) of VGG19's 16 convolutions in features order (csrc/vgg.cu kVggFwd), all 3 x 3
+VGG_CONVS = ((3, 64), (64, 64), (64, 128), (128, 128), (128, 256), (256, 256), (256, 256), (256, 256), (256, 512),
+             (512, 512), (512, 512), (512, 512), (512, 512), (512, 512), (512, 512), (512, 512))
+# the 20 launches of the VGG19 forward in features order: (convolution index or -1 for a max-pool, level, channels)
+VGG_STEPS = ((0, 0, 64), (1, 0, 64), (-1, 1, 64), (2, 1, 128), (3, 1, 128), (-1, 2, 128), (4, 2, 256), (5, 2, 256),
+             (6, 2, 256), (7, 2, 256), (-1, 3, 256), (8, 3, 512), (9, 3, 512), (10, 3, 512), (11, 3, 512),
+             (-1, 4, 512), (12, 4, 512), (13, 4, 512), (14, 4, 512), (15, 4, 512))
+
+
+def vgg_tile_hw(tile) -> Tuple[int, int]:
+    """``tile`` of the perceptual loss as (tile_h, tile_w): None -> (0, 0), one window per image."""
+    if tile is None:
+        return 0, 0
+    th, tw = (tile, tile) if isinstance(tile, int) else tile
+    if th <= 0 or tw <= 0:
+        raise ValueError(f"perceptual-loss tile must be positive, got {tile}")
+    return int(th), int(tw)
+
+
+def perceptual_windows(size: int, tile: int) -> list:
+    """The window rule of wn_perceptual_loss (csrc/vgg.cu) along one axis of ``size`` pixels: a list of (start, end,
+    f0, f1), the input pixels [start, end) a window reads and the features [f0, f1) it owns.  ``tile`` 0: one window."""
+    f = size // 16
+    q = min(f, -(-tile // 16)) if tile > 0 else f
+    count = -(-f // q)
+    return [(max(0, 16 * k * q - VGG_HALO), min(size, 16 * (k + 1) * q + VGG_HALO), k * q, min(f, (k + 1) * q))
+            for k in range(count)]
+
+
+def perceptual_passes(n: int, h: int, w: int, tile_h: int, tile_w: int, max_pass_pixels: int = 0) -> list:
+    """The passes of wn_perceptual_loss: classes of windows of one extent (runs of equal extent per axis), each split
+    into passes of at most ``max_pass_pixels`` window pixels.  Returns [(count, win_h, win_w), ...] in order."""
+    def runs(wins):
+        out = []
+        for s, e, _, _ in wins:
+            if out and out[-1][1] == e - s:
+                out[-1][0] += 1
+            else:
+                out.append([1, e - s])
+        return out
+    limit = max_pass_pixels or VGG_PASS_PIXELS
+    passes = []
+    for ny, wh in runs(perceptual_windows(h, tile_h)):
+        for nx, ww in runs(perceptual_windows(w, tile_w)):
+            total = n * ny * nx
+            per = min(65535, max(1, limit // (wh * ww)))
+            passes += [(min(per, total - w0), wh, ww) for w0 in range(0, total, per)]
+    return passes
+
+
+def perceptual_loss_workspace_bytes(n: int, h: int, w: int, tile_h: int, tile_w: int, max_pass_pixels: int = 0) -> int:
+    """wn_perceptual_loss_workspace_bytes restated: 0 for rejected arguments, else the float64 partials of every
+    window plus the largest pass (act0, two scratch buffers, ref's conv5_4 and the 20 saved launch outputs, each 1 KiB
+    aligned) plus 1 KiB."""
+    if (n <= 0 or n > 65535 or h < 16 or w < 16 or tile_h < 0 or tile_w < 0 or (tile_h == 0) != (tile_w == 0)
+            or max_pass_pixels < 0 or max_pass_pixels > VGG_MAX_PIXELS or h * w > 0x7fffffff // 3):
+        return 0
+    a1k = lambda v: -(-v // 1024) * 1024
+    passes = perceptual_passes(n, h, w, tile_h, tile_w, max_pass_pixels)
+    if any(wh * ww > VGG_MAX_PIXELS for _, wh, ww in passes):
+        return 0
+    windows = sum(c for c, _, _ in passes)
+
+    def pass_bytes(c, wh, ww):
+        steps = [(wh >> lv) * (ww >> lv) * ch * 4 for _, lv, ch in VGG_STEPS]
+        scratch = max([wh * ww * 64] + steps)
+        return sum(a1k(c * b) for b in [wh * ww * 64, scratch, scratch, steps[-1]] + steps)
+    return a1k(windows * VGG_SEED_BLOCKS * 8) + max(pass_bytes(*p) for p in passes) + 1024
+
+
 def _stream_ptr(device: torch.device) -> ctypes.c_void_p:
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -1007,3 +1082,91 @@ class Engine:
             lambda st, g, arr, gin, n, h, w, th, tw, ws: self.lib.wn_refine_backward_tiled(
                 self.handle, int(which), ins[0].data_ptr(), ins[1].data_ptr(), st, g, arr, gin, n, h, w, th, tw, mpp,
                 ws.data_ptr(), ws.numel(), stream), "wn_refine_backward_tiled")
+
+    # ---- the VGG19 perceptual loss (wn_perceptual_loss) ----------------------------------------
+    def pack_vgg_weights(self, params: Sequence[torch.Tensor], key=None) -> None:
+        """params: weight and bias of VGG19's 16 convolutions in ``features`` order (32 tensors).  Skipped when
+        ``key`` equals the key of the last pack."""
+        if len(params) != _lib.VGG_NUM_PARAMS:
+            raise ValueError(f"expected {_lib.VGG_NUM_PARAMS} VGG parameter tensors, got {len(params)}")
+        for i, (cin, cout) in enumerate(VGG_CONVS):  # the kernels read these shapes: anything else is refused
+            want = ((cout, cin, 3, 3), (cout,))
+            got = (tuple(params[2 * i].shape), tuple(params[2 * i + 1].shape))
+            if got != want:
+                raise ValueError(f"VGG convolution {i}: weight and bias of shapes {got}, expected {want} (VGG19)")
+        if key is not None and key == getattr(self, "_vgg_key", None):
+            return
+        staged = [p.detach().to(device=self.device, dtype=torch.float32).contiguous() for p in params]
+        arr = (ctypes.c_void_p * _lib.VGG_NUM_PARAMS)(*[t.data_ptr() for t in staged])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.wn_vgg_pack_weights(self.handle, arr, _stream_ptr(self.device)), "wn_vgg_pack_weights")
+        self._vgg_keepalive = staged  # until the async pack kernels have consumed them
+        self._vgg_key = key
+
+    def perceptual_loss_workspace_bytes(self, n: int, h: int, w: int, tile=None, max_pass_pixels: int = 0) -> int:
+        th, tw = vgg_tile_hw(tile)
+        return int(self.lib.wn_perceptual_loss_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels)))
+
+    def _vgg_workspace(self, n, h, w, th, tw, mpp, what):
+        nbytes = int(self.lib.wn_perceptual_loss_workspace_bytes(n, h, w, th, tw, mpp))
+        if nbytes == 0:
+            hint = " (pass a tile)" if th == 0 and h * w > VGG_MAX_PIXELS else ""
+            raise ValueError(f"{what}: unsupported arguments n={n} {h}x{w} tile={th}x{tw} max_pass_pixels={mpp}: images "
+                             f"must be at least 16 x 16 and a window at most {VGG_MAX_PIXELS} pixels{hint}")
+        return self._workspace("vgg", nbytes)
+
+    def perceptual_loss(self, out, ref, tile=None, want_grad: bool = False, max_pass_pixels: int = 0):
+        """mean((255 (F(out) - F(ref)))^2) with F = VGG19 features[:-1] of the normalised images, on the packed VGG
+        weights (wn_perceptual_loss), in windows that own ``tile`` input pixels of features (None: one window per
+        image).  Returns (0-d loss, d(loss)/d(out) as a contiguous (N,3,H,W) tensor, or None without ``want_grad``)."""
+        o, r = (t.detach() if t.dtype == torch.float32 else t.detach().float() for t in (out, ref))
+        for t in (o, r):
+            if t.device != self.device or t.dim() != 4 or t.shape[1] != 3:
+                raise ValueError(f"expected (N,3,H,W) inputs on {self.device}, got {tuple(t.shape)} on {t.device}")
+        if o.shape != r.shape:
+            raise ValueError(f"out and ref differ in shape: {tuple(o.shape)} vs {tuple(r.shape)}")
+        n, _, h, w = o.shape
+        th, tw = vgg_tile_hw(tile)
+        mpp = int(max_pass_pixels)
+        ws = self._vgg_workspace(n, h, w, th, tw, mpp, "perceptual_loss")
+        loss = torch.empty((), dtype=torch.float32, device=self.device)
+        grad = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) if want_grad else None
+        so = (ctypes.c_int64 * 4)(*o.stride())
+        sr = (ctypes.c_int64 * 4)(*r.stride())
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_perceptual_loss(self.handle, o.data_ptr(), so, r.data_ptr(), sr, n, h, w, th, tw, mpp,
+                                             loss.data_ptr(), grad.data_ptr() if grad is not None else None,
+                                             ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
+        _lib.check(rc, "wn_perceptual_loss")
+        return loss, grad
+
+    def debug_vgg_layer(self, x, layer: int, tile=None, ref=None) -> torch.Tensor:
+        """Test aid (wn_debug_vgg_layer), as fp32 (N, C, H >> level, W >> level): launch ``layer`` (0..19) of the VGG
+        forward of whole images; (20) the conv5_4 features of the windowed call with ``tile``; for the loss of
+        (out = x, ``ref``): (21) the seed, d(loss)/d(conv5_4 before its ReLU); (22 + k) the output of the backward
+        launch of forward launch k, d(loss)/d(input of launch k) (k = 0: 16 normalised channels, 3 real)."""
+        x = x.detach().float()
+        n, _, h, w = x.shape
+        th, tw = vgg_tile_hw(tile)
+        steps = len(VGG_STEPS)
+        if layer == steps:
+            shape = (n, 512, h // 16, w // 16)
+        elif layer == steps + 1:
+            shape = (n, 512, h >> 4, w >> 4)
+        elif layer > steps + 1:
+            k = layer - steps - 2
+            lv, ch = (VGG_STEPS[k - 1][1], VGG_STEPS[k - 1][2]) if k else (0, 16)
+            shape = (n, ch, h >> lv, w >> lv)
+        else:
+            _, lv, ch = VGG_STEPS[layer]
+            shape = (n, ch, h >> lv, w >> lv)
+        r = ref.detach().float() if ref is not None else None
+        dst = torch.empty(shape, dtype=torch.float32, device=self.device)
+        ws = self._vgg_workspace(n, h, w, th, tw, 0, "debug_vgg_layer")
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_debug_vgg_layer(
+                self.handle, x.data_ptr(), (ctypes.c_int64 * 4)(*x.stride()), r.data_ptr() if r is not None else None,
+                (ctypes.c_int64 * 4)(*r.stride()) if r is not None else None, n, h, w, th, tw, int(layer),
+                dst.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
+        _lib.check(rc, "wn_debug_vgg_layer")
+        return dst

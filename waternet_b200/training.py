@@ -3,8 +3,9 @@
 The model's forward values and all of its gradients come from the CUDA library
 (``wn_forward_train`` / ``wn_backward``: tensor-core forward that keeps its activations, data-gradient and
 weight-gradient kernels; only ``precision="fp32"`` re-evaluates the torch graph for its backward).  The
-VGG19 perceptual model, Adam and the metrics stay PyTorch: they are not on the
-north-star path.
+VGG19 perceptual loss is the torch expression by default; ``PerceptualModel(native=True)`` computes it and its
+gradient in overlapping windows on the library's kernels (``wn_perceptual_loss``).  Adam and the metrics stay
+PyTorch.
 """
 from __future__ import annotations
 
@@ -17,7 +18,9 @@ import numpy as np
 import torch
 import torch.nn as nn
 
+from .engine import new_engine
 from .metrics import psnr, ssim
+from .net import _model_engines, _model_engines_lock, _PackedWeightsMixin, _param_version
 
 TRAIN_METRICS_NAMES = ["mse", "ssim", "psnr", "perceptual_loss", "loss"]
 VAL_METRICS_NAMES = ["mse", "ssim", "psnr", "perceptual_loss"]
@@ -32,11 +35,20 @@ def next_run_dir(root: Path) -> Path:
     return root / str(max(taken) + 1 if taken else 0)
 
 
-class PerceptualModel(nn.Module):
-    """VGG19 ``features`` without the final max-pool (train.py:254-263)."""
+class PerceptualModel(_PackedWeightsMixin, nn.Module):
+    """VGG19 ``features`` without the final max-pool (train.py:254-263).
 
-    def __init__(self, pretrained: bool = True):
+    ``native=True``: on CUDA tensors ``perceptual_loss(vgg, out, ref)`` is one ``wn_perceptual_loss`` call -- the
+    loss and d(loss)/d(out) on the tensor cores (bf16x3), in windows that own ``tile`` input pixels of features
+    (None: one window per image; an image over 8 Mi pixels then needs a tile), so memory is bounded by one pass
+    whatever the image and batch size.  Autograd keeps only d(out), 12 bytes per pixel; no VGG weight gradient is
+    computed (the VGG parameters' ``.grad`` stays untouched) and ``ref`` is a constant.  ``native=False`` and CPU
+    tensors evaluate the torch expression."""
+
+    def __init__(self, pretrained: bool = True, native: bool = False, tile=None):
         super().__init__()
+        self.native = native
+        self.tile = tile
         import torchvision
         vgg = None
         if pretrained:
@@ -54,6 +66,68 @@ class PerceptualModel(nn.Module):
     def forward(self, x):
         return self.model(x)
 
+    def vgg_params(self):
+        """Weight and bias of the 16 convolutions in ``features`` order."""
+        return [t for m in self.model if isinstance(m, nn.Conv2d) for t in (m.weight, m.bias)]
+
+    def _vgg_engine(self, x):
+        """This module's engine on x's device with the VGG weights packed; re-packed when the cache key of
+        ``_PackedWeightsMixin`` (epoch, data_ptr and _version of every parameter) changes."""
+        params = self.vgg_params()
+        if params[0].device != x.device:
+            raise RuntimeError(f"VGG parameters on {params[0].device}, inputs on {x.device}")
+        with _model_engines_lock:
+            per_dev = _model_engines.setdefault(self, {})
+            eng = per_dev.get(x.device.index)
+            if eng is None:
+                eng = per_dev[x.device.index] = new_engine(x.device)
+        key = (getattr(self, "_pack_epoch", 0),) + tuple((p.data_ptr(), _param_version(p)) for p in params)
+        eng.pack_vgg_weights(params, key=key)
+        return eng
+
+    def native_loss(self, out, ref):
+        """The loss of ``perceptual_loss`` from one ``wn_perceptual_loss`` call (autograd: d(out) only)."""
+        want = torch.is_grad_enabled() and out.requires_grad
+        return _NativePerceptualLoss.apply(out, ref, self, want)
+
+
+class _NativePerceptualLoss(torch.autograd.Function):
+    """forward: one wn_perceptual_loss call; keeps d(loss)/d(out) when out needs a gradient, nothing else.
+    backward: grad_output * d(out)."""
+
+    @staticmethod
+    def forward(ctx, out, ref, vgg, want_grad):
+        loss, grad = vgg._vgg_engine(out).perceptual_loss(out, ref, tile=vgg.tile, want_grad=want_grad)
+        if grad is not None:
+            ctx.save_for_backward(grad)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        (grad,) = ctx.saved_tensors
+        return grad_output * grad, None, None, None
+
+
+def add_perceptual_args(ap) -> None:
+    """``--perceptual {torch,native}`` and ``--perceptual-tile N`` of train.py and score.py."""
+    ap.add_argument("--perceptual", default="torch", choices=["torch", "native"],
+                    help="(Optional) torch: the perceptual loss as the torch VGG19 expression (default); native: the "
+                         "loss and its gradient on the library's kernels in overlapping windows "
+                         "(PerceptualModel(native=True)), memory bounded by one pass")
+    ap.add_argument("--perceptual-tile", type=int, default=None, metavar="N",
+                    help="(Optional) needs --perceptual native: windows owning N x N input pixels of VGG features "
+                         "(rounded up to a multiple of 16).  Unset: one window per image")
+
+
+def perceptual_model(args) -> PerceptualModel:
+    """The PerceptualModel the command-line arguments of ``add_perceptual_args`` ask for; --perceptual-tile without
+    --perceptual native is refused (the torch expression has no windows)."""
+    if args.perceptual_tile is not None and args.perceptual != "native":
+        raise SystemExit("--perceptual-tile needs --perceptual native")
+    if args.perceptual_tile is not None and args.perceptual_tile <= 0:
+        raise SystemExit("--perceptual-tile must be positive")
+    return PerceptualModel(native=args.perceptual == "native", tile=args.perceptual_tile)
+
 
 def _normalize(x):
     mean = torch.tensor(_MEAN, device=x.device, dtype=x.dtype).view(1, 3, 1, 1)
@@ -62,7 +136,10 @@ def _normalize(x):
 
 
 def perceptual_loss(vgg, out, ref):
-    """mean((255 * (vgg(norm(out)) - vgg(norm(ref))))^2)  (train.py:110-122)."""
+    """mean((255 * (vgg(norm(out)) - vgg(norm(ref))))^2)  (train.py:110-122).  A ``PerceptualModel(native=True)``
+    takes CUDA tensors to ``wn_perceptual_loss`` instead."""
+    if getattr(vgg, "native", False) and out.is_cuda:
+        return vgg.native_loss(out, ref)
     return torch.mean(torch.square(255 * (vgg(_normalize(out)) - vgg(_normalize(ref)))))
 
 
