@@ -453,6 +453,35 @@ int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const 
                            int width, int mode, int layer, float* dst, void* workspace,
                            size_t workspace_bytes, void* stream);
 
+/*
+ * Test aid: one buffer of the training backward, decoded to contiguous fp32 NCHW (bf16 hi + lo planes as hi + lo in
+ * fp32).  `workspace` is a training workspace that the forward call of the same stack has just filled and nothing has
+ * touched since: stack -1 = the whole network (wn_forward_train), 0 = the confidence maps
+ * (wn_confidence_maps_train), 1 = refiner `which` (wn_refine_train of that `which`; ignored for the others).  The
+ * buffers, by number, with their channel counts:
+ *    0  act0      16  the packed input planes: the snapped v * 255 operands of x, wb, he, gc (12 real channels)
+ *    1..7 a1..a7  128, 128, 128, 64, 64, 64, 64  the saved cmg.conv1..conv7 activations (after ReLU)
+ *    8  cm         3  the confidence maps
+ *    9  r1        96  the refiners' conv1 activations, three refiners side by side
+ *   10  r2        96  their conv2 activations
+ *   11  refined    9  the three refined images
+ *   12  g8        16  the seed of cmg.conv8 (3 real channels): gate_bwd_kernel (stack -1) or maps_bwd_kernel (0)
+ *   13  gr3       16  the seed of the refiners' conv3 (9 real): gate_bwd_kernel (-1) or refine_bwd_kernel (1)
+ *   14 + k        the output of data-gradient launch k, the gradient with respect to that convolution's input (after
+ *                 the ReLU' mask of the saved activation, where there is one): k = 0..6 cmg.conv8 .. cmg.conv2
+ *                 (64, 64, 64, 64, 128, 128, 128), 7 and 8 the refiners' conv3 and conv2 (96, 96), 9 cmg.conv1
+ *                 and 10 the refiners' conv1 (32 each: the packed input's channels, 12 real)
+ * Buffers 0..11 only read the workspace.  12 and 13 run the seed from grad_out (d(loss)/d(out), d(maps) or refiner
+ * `which`'s d(out), fp32 contiguous (N,3,H,W)).  14 + k run the seed and the backward up to launch k, then stop; the
+ * parameter gradients of the layers before it are written into grads (the layout of wn_backward; the stack's own
+ * entries must be given).  A stack has only its own buffers (0 belongs to all).  The buffer number is checked before
+ * any other argument.  dst must hold n*C*h*w floats.  An addition: no existing call changed, WN_ABI_VERSION stays.
+ */
+#define WN_DEBUG_BACKWARD_BUFFERS 25
+int wn_debug_backward_layer(wn_handle* h, int stack, int which, int buffer, const float* grad_out,
+                            float* const* grads, int n, int height, int width, float* dst, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 /* Number of kernels the library has launched on this handle since creation. */
 uint64_t wn_launch_count(const wn_handle* h);
 

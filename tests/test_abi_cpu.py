@@ -83,6 +83,24 @@ def test_debug_layer_bound(lib):
         assert call(layer) != 0 and b"bad argument" in lib.wn_last_error()
 
 
+def test_debug_backward_layer_bound(lib):
+    """wn_debug_backward_layer numbers its buffers 0..24 (Engine.BACKWARD_BUFFER_CHANNELS, the header's table); the
+    number is checked before anything else, then the stack, so both bounds show without a device."""
+    from waternet_b200 import _lib
+    from waternet_b200.engine import Engine
+    assert len(Engine.BACKWARD_BUFFER_CHANNELS) == _lib.DEBUG_BACKWARD_BUFFERS == 25
+    text = open(os.path.join(ROOT, "include", "waternet_b200.h")).read()
+    assert int(re.search(r"#define\s+WN_DEBUG_BACKWARD_BUFFERS\s+(\d+)", text).group(1)) == 25
+    call = lambda stack, which, buffer: lib.wn_debug_backward_layer(None, stack, which, buffer, None, None, 1, 1, 1,
+                                                                    None, None, 0, None)
+    for buffer in (-1, 25):
+        assert call(-1, 0, buffer) != 0 and b"not in 0..24" in lib.wn_last_error()
+    for stack, which in ((-2, 0), (2, 0), (1, -1), (1, 3)):
+        assert call(stack, which, 0) != 0 and b"stack must be" in lib.wn_last_error()
+    for stack, which, buffer in ((-1, 0, 0), (0, 0, 24), (1, 2, 13)):
+        assert call(stack, which, buffer) != 0 and b"null argument" in lib.wn_last_error()
+
+
 def test_state_dict_is_reference_compatible():
     from waternet_b200.net import WaterNet
     m = WaterNet()

@@ -20,6 +20,7 @@ MODE_DEFAULT = -1
 NUM_PARAMS = 34
 VGG_NUM_PARAMS = 32     # WN_VGG_NUM_PARAMS: weight and bias of VGG19's 16 convolutions
 NUM_TIMING_SLOTS = 23
+DEBUG_BACKWARD_BUFFERS = 25  # WN_DEBUG_BACKWARD_BUFFERS
 ABI_VERSION = 11
 PEER_HANDLE_BYTES = 64  # WN_PEER_HANDLE_BYTES
 MAX_PEERS = 15          # WN_MAX_PEERS
@@ -139,6 +140,8 @@ _SIGNATURES = {
                                          c_void_p]),
     "wn_debug_forward_layer": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int,
                                        c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "wn_debug_backward_layer": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, POINTER(c_void_p), c_int, c_int,
+                                        c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "wn_vgg_pack_weights": (c_int, [c_void_p, POINTER(c_void_p), c_void_p]),
     "wn_perceptual_loss_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong]),
     "wn_perceptual_loss": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_void_p, POINTER(c_int64), c_int, c_int,

@@ -1162,6 +1162,42 @@ int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const 
                           (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0);
 }
 
+int wn_debug_backward_layer(wn_handle* h, int stack, int which, int buffer, const float* grad_out,
+                            float* const* grads, int n, int height, int width, float* dst, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  const char* what = "wn_debug_backward_layer";
+  if (buffer < 0 || buffer >= WN_DEBUG_BACKWARD_BUFFERS) {
+    set_error("%s: buffer %d is not in 0..%d", what, buffer, WN_DEBUG_BACKWARD_BUFFERS - 1);
+    return WN_E_INVALID;
+  }
+  if (stack < -1 || stack > 1 || (stack == 1 && (which < 0 || which > 2))) {
+    set_error("%s: stack must be -1, 0 or 1 (with which 0, 1 or 2), got stack %d which %d", what, stack, which);
+    return WN_E_INVALID;
+  }
+  if (!h || !dst || !workspace || (buffer >= 12 && !grad_out) || (buffer >= 14 && !grads)) {
+    set_error("%s: null argument", what);
+    return WN_E_INVALID;
+  }
+  // the parameter gradients the backward up to the launch writes: the stack's own entries
+  const int first = stack == 1 ? 16 + 6 * which : 0, count = stack == -1 ? WN_NUM_PARAMS : stack == 0 ? 16 : 6;
+  if (buffer >= 14)
+    for (int i = first; i < first + count; i++)
+      if (!grads[i]) {
+        set_error("%s: grads[%d] is NULL", what, i);
+        return WN_E_INVALID;
+      }
+  int rc = submodule_train_check(what, n, height, width);
+  if (rc) return rc;
+  if (!h->packed) {
+    set_error("%s: wn_pack_weights has not been called", what);
+    return WN_E_STATE;
+  }
+  DeviceGuard guard(h->device);
+  return debug_backward_layer(h, stack == -1 ? kStackAll : stack == 0 ? kStackCmg : kStackRefiners, which, buffer,
+                              grad_out, grads, n, height, width, dst, workspace, workspace_bytes,
+                              (cudaStream_t)stream);
+}
+
 // ---- the VGG19 perceptual loss (vgg.cu)
 int wn_vgg_pack_weights(wn_handle* h, const float* const* params, void* stream) {
   if (!h || !params) {

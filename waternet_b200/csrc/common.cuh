@@ -213,6 +213,8 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
 int umma_debug_layer(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], int n,
                      int height, int width, int layer, float* dst, void* workspace,
                      size_t workspace_bytes, cudaStream_t stream, int scheme = 0);
+// bf16 hi + lo planes (planes_half 8-channel planes per half) of n images -> fp32 NCHW, hi + lo (test aid)
+int decode_planes(wn_handle* h, const uint4* src, float* dst, int planes_half, int n, int hw, cudaStream_t stream);
 int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t stream);
 void umma_free(wn_handle* h);
 size_t umma_forward_workspace_bytes(int n, int h, int w);
@@ -296,6 +298,11 @@ int refine_train(wn_handle* h, int which, const float* const in[4], const int64_
                  int height, int width, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 int refine_backward(wn_handle* h, int which, const float* grad_out, float* const* grads, float* const* input_grads,
                     int n, int height, int width, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+// wn_debug_backward_layer (test aid); stack: kStackAll, kStackCmg or kStackRefiners (refiner `which`); the buffer
+// number, the pointers and the shape are checked by the caller (api.cu)
+int debug_backward_layer(wn_handle* h, int stack, int which, int buffer, const float* grad_out, float* const* grads,
+                         int n, int height, int width, float* dst, void* workspace, size_t workspace_bytes,
+                         cudaStream_t stream);
 // the windowed recompute backward; arguments checked by the caller (api.cu)
 size_t backward_tiled_workspace_bytes(int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels);
 int backward_tiled(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], const float* grad_out,

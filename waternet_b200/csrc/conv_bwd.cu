@@ -1035,12 +1035,27 @@ static int launch_dgrad(wn_handle* h, uint4* g_in, uint4* g_out, const uint4* sa
                                                                               h->bwd->zero_bias, g_in, a, stream);
 }
 
+// wn_debug_backward_layer: the backward pass stops after data-gradient launch `li` and decodes its output into dst
+// (the gradient buffers ping-pong, so it cannot be read afterwards).  li = -1: the normal path, never stops.
+struct BwdStop {
+  int li = -1;
+  float* dst = nullptr;
+};
+static constexpr int kBwdStopped = 1;  // returned up the call chain once the launch asked for has been decoded
+
+static int stop_after(wn_handle* h, const BwdStop& stop, int li, const uint4* g_out, int n, int hw,
+                      cudaStream_t stream) {
+  if (stop.li != li) return WN_OK;
+  const int rc = decode_planes(h, g_out, stop.dst, kDSpecs[li].npad * kDSpecs[li].nblk / 8, n, hw, stream);
+  return rc ? rc : kBwdStopped;
+}
+
 // Backward of one cmg convolution from g, the gradient with respect to its output: its weight and bias gradients,
 // then, when g_dst is given, the gradient with respect to its input into g_dst.  Its input is the saved activation
 // a[conv], whose zeros gate that gradient (ReLU'); conv 0 reads act0 instead, the images * 255 with no ReLU.
 template <int LI>
 static int cmg_conv_backward(wn_handle* h, const TrainBuffers& t, float* const* grads, uint4* g, uint4* g_dst, int n,
-                             int H, int W, cudaStream_t stream) {
+                             int H, int W, cudaStream_t stream, const BwdStop& stop) {
   constexpr DgradSpec s = kDSpecs[LI];
   static_assert(s.conv >= 0, "not a cmg convolution");
   const LayerDesc& d = kCmg[s.conv];
@@ -1052,7 +1067,9 @@ static int cmg_conv_backward(wn_handle* h, const TrainBuffers& t, float* const* 
     return rc;
   if ((rc = bias_grad(h, g, (d.cout + 15) / 16 * 2, d.cout, grads[2 * s.conv + 1], t.partial, n, H * W, stream)))
     return rc;
-  return g_dst ? launch_dgrad<LI>(h, g, g_dst, s.conv ? act : nullptr, n, H, W, stream) : WN_OK;
+  if (!g_dst) return WN_OK;
+  if ((rc = launch_dgrad<LI>(h, g, g_dst, s.conv ? act : nullptr, n, H, W, stream))) return rc;
+  return stop_after(h, stop, LI, g_dst, n, H * W, stream);
 }
 
 // The two halves of the backward pass of a batch whose forward activations are in t.  The confidence-map half starts
@@ -1060,24 +1077,25 @@ static int cmg_conv_backward(wn_handle* h, const TrainBuffers& t, float* const* 
 // overwrites its stack's parameter gradients in grads (state-dict order) and, when want_input_grads, writes the data
 // gradient of the packed 16-channel input into t.gin_a (cmg.conv1) or t.gin_b (the refiners' conv1).
 static int backward_cmg(wn_handle* h, const TrainBuffers& t, float* const* grads, bool want_input_grads, int n, int H,
-                        int W, cudaStream_t stream) {
+                        int W, cudaStream_t stream, const BwdStop& stop = BwdStop()) {
   int rc;
   // conv8 ... conv1, the gradient ping-ponging between ga and gb.  conv8's output gradient g8 has 16-channel planes,
   // 3 valid; conv1's input gradient only when asked for
-  if ((rc = cmg_conv_backward<kD8>(h, t, grads, t.g8, t.ga, n, H, W, stream))) return rc;
-  if ((rc = cmg_conv_backward<kD7>(h, t, grads, t.ga, t.gb, n, H, W, stream))) return rc;
-  if ((rc = cmg_conv_backward<kD6>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
-  if ((rc = cmg_conv_backward<kD5>(h, t, grads, t.ga, t.gb, n, H, W, stream))) return rc;
-  if ((rc = cmg_conv_backward<kD4>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
-  if ((rc = cmg_conv_backward<kD3>(h, t, grads, t.ga, t.gb, n, H, W, stream))) return rc;
-  if ((rc = cmg_conv_backward<kD2>(h, t, grads, t.gb, t.ga, n, H, W, stream))) return rc;
-  return cmg_conv_backward<kD1>(h, t, grads, t.ga, want_input_grads ? t.gin_a : nullptr, n, H, W, stream);
+  if ((rc = cmg_conv_backward<kD8>(h, t, grads, t.g8, t.ga, n, H, W, stream, stop))) return rc;
+  if ((rc = cmg_conv_backward<kD7>(h, t, grads, t.ga, t.gb, n, H, W, stream, stop))) return rc;
+  if ((rc = cmg_conv_backward<kD6>(h, t, grads, t.gb, t.ga, n, H, W, stream, stop))) return rc;
+  if ((rc = cmg_conv_backward<kD5>(h, t, grads, t.ga, t.gb, n, H, W, stream, stop))) return rc;
+  if ((rc = cmg_conv_backward<kD4>(h, t, grads, t.gb, t.ga, n, H, W, stream, stop))) return rc;
+  if ((rc = cmg_conv_backward<kD3>(h, t, grads, t.ga, t.gb, n, H, W, stream, stop))) return rc;
+  if ((rc = cmg_conv_backward<kD2>(h, t, grads, t.gb, t.ga, n, H, W, stream, stop))) return rc;
+  return cmg_conv_backward<kD1>(h, t, grads, t.ga, want_input_grads ? t.gin_a : nullptr, n, H, W, stream, stop);
 }
 
 // conv3, conv2, conv1 of the three refiners side by side.  which = -1: the gradients of all three; 0..2: of refiner
 // `which` alone (the launches are the same, only its weight and bias gradients are extracted)
 static int backward_refiners(wn_handle* h, const TrainBuffers& t, float* const* grads, int which,
-                             bool want_input_grads, int n, int H, int W, cudaStream_t stream) {
+                             bool want_input_grads, int n, int H, int W, cudaStream_t stream,
+                             const BwdStop& stop = BwdStop()) {
   int rc;
   const int hw = H * W;
   const int r0 = which < 0 ? 0 : which, r1 = which < 0 ? 3 : which + 1;
@@ -1095,6 +1113,7 @@ static int backward_refiners(wn_handle* h, const TrainBuffers& t, float* const* 
       WN_CUDA(cudaMemcpyAsync(gb(8 + 3 * r + 2), tmp + 3 * r, 3 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   }
   if ((rc = launch_dgrad<kDR3>(h, t.gr3, t.gra, t.f.r[2], n, H, W, stream))) return rc;
+  if ((rc = stop_after(h, stop, kDR3, t.gra, n, hw, stream))) return rc;
   if ((rc = launch_wgrad<kDR2>(h, t.gra, 96, t.f.r[1], t.dense, t.partial, n, H, W, stream))) return rc;
   {
     float* tmp = t.dense + (size_t)25 * 128 * 96;
@@ -1105,6 +1124,7 @@ static int backward_refiners(wn_handle* h, const TrainBuffers& t, float* const* 
     }
   }
   if ((rc = launch_dgrad<kDR2>(h, t.gra, t.grb, t.f.r[1], n, H, W, stream))) return rc;
+  if ((rc = stop_after(h, stop, kDR2, t.grb, n, hw, stream))) return rc;
   if ((rc = launch_wgrad<kDR1>(h, t.grb, 96, t.f.act0, t.dense, t.partial, n, H, W, stream))) return rc;
   {
     float* tmp = t.dense + (size_t)49 * 128 * 16;
@@ -1115,16 +1135,17 @@ static int backward_refiners(wn_handle* h, const TrainBuffers& t, float* const* 
       WN_CUDA(cudaMemcpyAsync(gb(8 + 3 * r), tmp + 32 * r, 32 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
     }
   }
-  if (want_input_grads) return launch_dgrad<kDR1>(h, t.grb, t.gin_b, nullptr, n, H, W, stream);
-  return WN_OK;
+  if (!want_input_grads) return WN_OK;
+  if ((rc = launch_dgrad<kDR1>(h, t.grb, t.gin_b, nullptr, n, H, W, stream))) return rc;
+  return stop_after(h, stop, kDR1, t.gin_b, n, hw, stream);
 }
 
 // The whole network: the 34 parameter gradients into grads (overwritten) and, when want_input_grads, t.gin_a and
 // t.gin_b
 static int backward_layers(wn_handle* h, const TrainBuffers& t, float* const* grads, bool want_input_grads, int n,
-                           int H, int W, cudaStream_t stream) {
-  int rc = backward_cmg(h, t, grads, want_input_grads, n, H, W, stream);
-  return rc ? rc : backward_refiners(h, t, grads, -1, want_input_grads, n, H, W, stream);
+                           int H, int W, cudaStream_t stream, const BwdStop& stop = BwdStop()) {
+  int rc = backward_cmg(h, t, grads, want_input_grads, n, H, W, stream, stop);
+  return rc ? rc : backward_refiners(h, t, grads, -1, want_input_grads, n, H, W, stream, stop);
 }
 
 int backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n, int H,
@@ -1394,6 +1415,65 @@ int refine_backward(wn_handle* h, int which, const float* grad_out, float* const
     WN_LAUNCH_CHECK(h);
   }
   return WN_OK;
+}
+
+// ---- wn_debug_backward_layer (test aid) ---------------------------------------------------------------------------
+// Buffer numbers (include/waternet_b200.h): 0 act0, 1..7 a1..a7, 8 cm, 9 r1, 10 r2, 11 refined, 12 g8, 13 gr3,
+// 14 + li the output of data-gradient launch li (DgradLayer).  Which of them a stack's training pass has:
+static bool debug_buffer_in_stack(int buffer, int stack) {
+  if (buffer == 0 || stack == kStackAll) return true;
+  const bool cmg_buffer = buffer <= 8 || buffer == 12 || (buffer >= 14 + kD8 && buffer <= 14 + kD2) ||
+                          buffer == 14 + kD1;
+  return cmg_buffer == (stack == kStackCmg);
+}
+
+int debug_backward_layer(wn_handle* h, int stack, int which, int buffer, const float* grad_out, float* const* grads,
+                         int n, int H, int W, float* dst, void* workspace, size_t workspace_bytes,
+                         cudaStream_t stream) {
+  if (!h->bwd) {
+    set_error("backward weights have not been packed");
+    return WN_E_STATE;
+  }
+  if (!debug_buffer_in_stack(buffer, stack)) {
+    set_error("wn_debug_backward_layer: the training pass of this stack has no buffer %d", buffer);
+    return WN_E_INVALID;
+  }
+  int rc = stack == kStackAll ? check_train_args(n, H, W, workspace_bytes)
+                              : check_submodule_args(n, H, W, stack, workspace_bytes);
+  if (rc) return rc;
+  if ((rc = get_encoder())) return rc;
+  TrainBuffers t;
+  carve(&t, workspace, (size_t)n * H * W, stack);
+  const int hw = H * W;
+  // the saved forward activations, as wn_forward_train or the sub-module's *_train call left them
+  if (buffer <= 11) {
+    static constexpr int kChannels[12] = {16, 128, 128, 128, 64, 64, 64, 64, 3, 96, 96, 9};
+    const int c = kChannels[buffer];
+    if (buffer == 8 || buffer == 11) {
+      WN_CUDA(cudaMemcpyAsync(dst, buffer == 8 ? t.f.cm : t.f.refined, (size_t)n * c * hw * sizeof(float),
+                              cudaMemcpyDeviceToDevice, stream));
+      return WN_OK;
+    }
+    const uint4* planes = buffer == 0 ? t.f.act0 : buffer <= 7 ? t.f.a[buffer] : t.f.r[buffer - 8];
+    return decode_planes(h, planes, dst, c / 8, n, hw, stream);
+  }
+  // the seed of the stack's backward, then the backward up to the launch asked for (input gradients included)
+  const dim3 grid((hw + 255) / 256, n);
+  if (stack == kStackAll)
+    gate_bwd_kernel<<<grid, 256, 0, stream>>>(grad_out, t.f.cm, t.f.refined, t.g8, t.gr3, hw);
+  else if (stack == kStackCmg)
+    maps_bwd_kernel<<<grid, 256, 0, stream>>>(grad_out, t.f.cm, t.g8, hw);
+  else
+    refine_bwd_kernel<<<grid, 256, 0, stream>>>(grad_out, t.f.refined, t.gr3, which, hw);
+  WN_LAUNCH_CHECK(h);
+  if (buffer == 12 || buffer == 13) return decode_planes(h, buffer == 12 ? t.g8 : t.gr3, dst, 2, n, hw, stream);
+  BwdStop stop;
+  stop.li = buffer - 14;
+  stop.dst = dst;
+  rc = stack == kStackAll ? backward_layers(h, t, grads, true, n, H, W, stream, stop)
+       : stack == kStackCmg ? backward_cmg(h, t, grads, true, n, H, W, stream, stop)
+                            : backward_refiners(h, t, grads, which, true, n, H, W, stream, stop);
+  return rc == kBwdStopped ? WN_OK : rc;
 }
 
 // ---- windowed recompute backward (wn_backward_tiled, DESIGN.md "Windowed backward") -------------------------------

@@ -379,6 +379,12 @@ __global__ void decode_planes_kernel(const uint4* __restrict__ src, float* __res
   }
 }
 
+int decode_planes(wn_handle* h, const uint4* src, float* dst, int planes_half, int n, int hw, cudaStream_t stream) {
+  decode_planes_kernel<<<dim3((hw + 255) / 256, planes_half, n), 256, 0, stream>>>(src, dst, planes_half, hw, 0);
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+
 static PackInArgs pack_args(const float* const in[4], const int64_t st[4][4]) {
   PackInArgs pa;
   for (int t = 0; t < 4; t++) {

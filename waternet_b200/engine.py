@@ -424,6 +424,32 @@ class Engine:
                 torch._foreach_add_(grads, part)
         return (grads, gin) if want_input_grads else grads
 
+    # wn_debug_backward_layer's buffers 0..24 (include/waternet_b200.h): act0, a1..a7, cm, r1, r2, refined, g8, gr3 and
+    # the outputs of the 11 data-gradient launches cmg.conv8 .. cmg.conv2, refiners conv3, conv2, cmg.conv1, refiners conv1
+    BACKWARD_BUFFER_CHANNELS = (16, 128, 128, 128, 64, 64, 64, 64, 3, 96, 96, 9, 16, 16,
+                                64, 64, 64, 64, 128, 128, 128, 96, 96, 32, 32)
+
+    def debug_backward_layer(self, workspace: torch.Tensor, shape, buffer: int, stack: int = -1, which: int = 0,
+                             grad: Optional[torch.Tensor] = None, grads=None) -> torch.Tensor:
+        """Test aid (wn_debug_backward_layer): buffer ``buffer`` of the training backward as fp32 (N,C,H,W).
+
+        ``workspace`` is the workspace of one slice that ``forward_train`` (stack -1), ``confidence_maps_train`` (0)
+        or ``refine_train(which)`` (1) has just filled, ``shape`` = (n, h, w) of that slice.  ``grad``: d(loss)/d(out)
+        (d(maps) for the cmg) for the seeds and launches, buffers 12 and up.  ``grads``: 34 fp32 tensors or None
+        (None where the stack writes nothing) that receive the parameter gradients of the layers before a
+        data-gradient launch, buffers 14 and up."""
+        n, h, w = shape
+        dst = torch.empty((n, self.BACKWARD_BUFFER_CHANNELS[buffer], h, w), dtype=torch.float32, device=self.device)
+        g = None if grad is None else grad.detach().to(self.device, torch.float32).contiguous()
+        arr = None if grads is None else (ctypes.c_void_p * _lib.NUM_PARAMS)(
+            *[None if t is None else t.data_ptr() for t in grads])
+        with torch.cuda.device(self.device):
+            rc = self.lib.wn_debug_backward_layer(self.handle, int(stack), int(which), int(buffer),
+                                                  None if g is None else g.data_ptr(), arr, n, h, w, dst.data_ptr(),
+                                                  workspace.data_ptr(), workspace.numel(), _stream_ptr(self.device))
+        _lib.check(rc, "wn_debug_backward_layer")
+        return dst
+
     # ---- the sub-modules under autograd (wn_confidence_maps_train / _backward, wn_refine_train / _backward) --------
     STACK_CMG, STACK_REFINER = 0, 1
 
