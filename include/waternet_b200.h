@@ -465,8 +465,8 @@ int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const 
  *    9  r1        96  the refiners' conv1 activations, three refiners side by side
  *   10  r2        96  their conv2 activations
  *   11  refined    9  the three refined images
- *   12  g8        16  the seed of cmg.conv8 (3 real channels): gate_bwd_kernel (stack -1) or maps_bwd_kernel (0)
- *   13  gr3       16  the seed of the refiners' conv3 (9 real): gate_bwd_kernel (-1) or refine_bwd_kernel (1)
+ *   12  g8        16  the seed of cmg.conv8 (3 real channels): the gate's (stack -1) or the maps' (0)
+ *   13  gr3       16  the seed of the refiners' conv3 (9 real): the gate's (-1) or refiner `which`'s (1)
  *   14 + k        the output of data-gradient launch k, the gradient with respect to that convolution's input (after
  *                 the ReLU' mask of the saved activation, where there is one): k = 0..6 cmg.conv8 .. cmg.conv2
  *                 (64, 64, 64, 64, 128, 128, 128), 7 and 8 the refiners' conv3 and conv2 (96, 96), 9 cmg.conv1

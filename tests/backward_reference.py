@@ -8,7 +8,7 @@ can be used), and no launch inherits the error of the launches before it.  Each 
 on the same terms, and the check is ``grad_reference.assert_grad_close(G, R, M, tau)``, |G - R| <= tau M element by
 element; where M is 0 (a masked pixel, a padding channel) G must be exactly 0.0.
 
-* Seeds (``seed_reference``): gate_bwd_kernel, maps_bwd_kernel and refine_bwd_kernel's formulas from grad_out and the
+* Seeds (``seed_reference``): seed_kernel's gate, maps and refine formulas from grad_out and the
   GPU's cm and refined; M is the same products in absolute values.
 * Data gradient of a launch (``dgrad_reference``): R = mask * conv_transpose(g, W), M = mask * conv_transpose(|g|, |W|),
   g the decoded buffer the launch read, mask = (the GPU's saved input activation > 0) (none for the two launches
@@ -18,8 +18,8 @@ element; where M is 0 (a masked pixel, a padding channel) G must be exactly 0.0.
   padding), db = sum g, M the same sums in absolute values, with g the gradient the weight-gradient GEMM consumed
   (the seed, or the next launch's masked output) and a the GPU's saved input (act0 / 255 for the first layers:
   ``extract`` scales by 1/255; refiner r's conv1 reads packed channels 0..2 and 3(r+1)..3(r+1)+2).
-* The input-gradient fold (``fold_reference``): input_grads_kernel adds the decoded outputs of the two first-layer
-  launches; submodule_input_grads_kernel copies one of them.
+* The input-gradient fold (``fold_reference``): extract_input_grads_kernel adds the decoded outputs of the two
+  first-layer launches of the whole network, and copies the one of a sub-module.
 
 The bars (``TAU``, ``wgrad_tau``; DESIGN section 4.3).  A data-gradient launch is the forward kernel in bf16x3 on
 decoded operands: g_hi w_hi + g_lo w_hi + g_hi w_lo with fp32 accumulation, stored as bf16 hi + lo.  A weight
@@ -132,9 +132,9 @@ def stack_params(stack, which=0):
 
 # ------------------------------------------------------------------ the bars
 # 4x the worst |G - R| / M measured on an H100 (80 GB HBM3, 700 W limit) over tests/test_backward_layers_gpu.py
-# (DESIGN section 4.3).  seed: gate_bwd / maps_bwd / refine_bwd (7.7e-6); dgrad: the 11 data-gradient launches
-# (1.90e-5, the refiners' conv3 launch); bias: the 34 bias-gradient reductions (2.9e-7); fold: input_grads_kernel's
-# fp32 sums of the decoded first-layer gradients (1.19e-7, one rounding).
+# (DESIGN section 4.3).  seed: seed_kernel's gate / maps / refine (7.7e-6); dgrad: the 11 data-gradient launches
+# (1.90e-5, the refiners' conv3 launch); bias: the 34 bias-gradient reductions (2.9e-7); fold:
+# extract_input_grads_kernel's fp32 sums of the decoded first-layer gradients (1.19e-7, one rounding).
 TAU = {"seed": 3.1e-5, "dgrad": 7.6e-5, "bias": 1.2e-6, "fold": 4.8e-7}
 # The weight gradients.  Up to a few thousand pixels per partial sum the error is that of the bf16x3 products and
 # the bf16 hi + lo operands (worst 1.45e-5, flat in P); WGRAD_TAU0 is 4x that.  Beyond, the fp32 accumulation shows:
@@ -292,7 +292,7 @@ def emulate_forward(sd, ins):
 
 
 def emulate_seeds(stack, grad, bufs, which=0, fault=None):
-    """gate_bwd / maps_bwd / refine_bwd in fp32, stored as 16-channel bf16 hi + lo buffers."""
+    """seed_kernel's gate / maps / refine in fp32, stored as 16-channel bf16 hi + lo buffers."""
     go = _f32(grad.double())
     n, _, h, w = go.shape
     out = {}

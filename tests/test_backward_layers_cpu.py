@@ -52,7 +52,7 @@ def _check_all(sd, stack, grad, bufs, params, which=0, label=""):
 
 
 def _fold(stack, vals, which=0):
-    """input_grads_kernel's fp32 sums ((hi_a + lo_a) + hi_b) + lo_b, or submodule_input_grads_kernel's copy."""
+    """extract_input_grads_kernel's fp32 sums ((hi_a + lo_a) + hi_b) + lo_b, or its copy of one buffer."""
     if stack == "all":
         a, b = vals["kD1"], vals["kDR1"]
         return [a[:, 3 * t:3 * t + 3] + b[:, 3 * t:3 * t + 3] for t in range(4)]

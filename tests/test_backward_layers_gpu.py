@@ -174,7 +174,7 @@ def _check_case(eng, sd, stack, ins, seed_kind, worst, label, which=0, fill=None
     for t, (g, ref) in enumerate(zip(gin, folds)):
         if stack == "all":
             record("fold", ref, g, br.TAU["fold"], f"input {t}")
-        else:  # submodule_input_grads_kernel adds hi + lo as the decode does
+        else:  # extract_input_grads_kernel adds hi + lo of the one buffer as the decode does
             assert torch.equal(g, ref.R.float()), f"{label} input {t}"
     if probes is not None:
         keep = {}
@@ -233,7 +233,7 @@ def test_probe_seeds_stay_in_their_support(shape):
 
 @pytest.mark.parametrize("stack,which", [("cmg", 0), ("refiner", 0), ("refiner", 1), ("refiner", 2)])
 def test_submodule_stacks(stack, which):
-    """The cmg alone (maps_bwd_kernel's seed) and each refiner alone (refine_bwd_kernel's: the other refiners'
+    """The cmg alone (seed_kernel's maps seed) and each refiner alone (its refine seed: the other refiners'
     columns exactly 0), with MSE and probe seeds, on the stress and default weights."""
     worst = {}
     for weights in ("stress", "default"):

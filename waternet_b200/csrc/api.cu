@@ -696,21 +696,31 @@ int wn_forward_train(wn_handle* h, const float* x, const float* wb, const float*
                        (cudaStream_t)stream);
 }
 
+// the backward calls: the parameter gradients [first, first + count) they write must be given
+static int check_param_grads(const char* what, float* const* grads, int first, int count) {
+  for (int i = first; i < first + count; i++)
+    if (!grads[i]) {
+      set_error("%s: grads[%d] is NULL", what, i);
+      return WN_E_INVALID;
+    }
+  return WN_OK;
+}
+
+static int check_packed(const char* what, const wn_handle* h) {
+  if (h->packed) return WN_OK;
+  set_error("%s: wn_pack_weights has not been called", what);
+  return WN_E_STATE;
+}
+
 int wn_backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n,
                 int height, int width, void* train_workspace, size_t workspace_bytes, void* stream) {
   if (!h || !grad_out || !grads || !train_workspace || n <= 0 || height <= 0 || width <= 0) {
     set_error("wn_backward: bad argument");
     return WN_E_INVALID;
   }
-  for (int i = 0; i < WN_NUM_PARAMS; i++)
-    if (!grads[i]) {
-      set_error("wn_backward: grads[%d] is NULL", i);
-      return WN_E_INVALID;
-    }
-  if (!h->packed) {
-    set_error("wn_backward: wn_pack_weights has not been called");
-    return WN_E_STATE;
-  }
+  int rc = check_param_grads("wn_backward", grads, 0, WN_NUM_PARAMS);
+  if (rc) return rc;
+  if ((rc = check_packed("wn_backward", h))) return rc;
   if (n > 65535) {
     set_error("wn_backward: at most 65535 images per call, got n=%d", n);
     return WN_E_UNSUPPORTED;
@@ -799,22 +809,15 @@ int wn_backward_ragged(wn_handle* h, const int* heights_host, const int* widths_
     set_error("%s: null argument", what);
     return WN_E_INVALID;
   }
-  for (int i = 0; i < WN_NUM_PARAMS; i++)
-    if (!grads[i]) {
-      set_error("%s: grads[%d] is NULL", what, i);
-      return WN_E_INVALID;
-    }
-  int rc = train_ragged_check(what, heights_host, widths_host, n);
+  int rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS);
   if (rc) return rc;
+  if ((rc = train_ragged_check(what, heights_host, widths_host, n))) return rc;
   for (int i = 0; i < n; i++)
     if (!grad_out_host[i]) {
       set_error("%s: grad_out_host[%d] is NULL", what, i);
       return WN_E_INVALID;
     }
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  if ((rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   return backward_ragged(h, heights_host, widths_host, grad_out_host, grads, input_grads_host, n, workspace,
                          workspace_bytes, (cudaStream_t)stream);
@@ -841,18 +844,10 @@ static int submodule_backward_check(const char* what, wn_handle* h, const float*
     set_error("%s: null argument", what);
     return WN_E_INVALID;
   }
-  for (int i = first; i < first + count; i++)
-    if (!grads[i]) {
-      set_error("%s: grads[%d] is NULL", what, i);
-      return WN_E_INVALID;
-    }
-  int rc = submodule_train_check(what, n, height, width);
+  int rc = check_param_grads(what, grads, first, count);
   if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
-  return WN_OK;
+  if ((rc = submodule_train_check(what, n, height, width))) return rc;
+  return check_packed(what, h);
 }
 
 size_t wn_submodule_train_workspace_bytes(int n, int h, int w, int stack) {
@@ -967,23 +962,16 @@ int wn_backward_tiled(wn_handle* h, const float* x, const float* wb, const float
     set_error("%s: null argument", what);
     return WN_E_INVALID;
   }
-  for (int i = 0; i < WN_NUM_PARAMS; i++)
-    if (!grads[i]) {
-      set_error("%s: grads[%d] is NULL", what, i);
-      return WN_E_INVALID;
-    }
+  int rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS);
+  if (rc) return rc;
   if (input_grads)
     for (int i = 0; i < 4; i++)
       if (!input_grads[i]) {
         set_error("%s: input_grads[%d] is NULL", what, i);
         return WN_E_INVALID;
       }
-  int rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels);
-  if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  if ((rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels))) return rc;
+  if ((rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
   return backward_tiled(h, in, in_strides, grad_out, grads, input_grads, n, height, width, tile_h, tile_w,
@@ -1036,11 +1024,8 @@ int wn_backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images_host,
     set_error("%s: null argument", what);
     return WN_E_INVALID;
   }
-  for (int i = 0; i < WN_NUM_PARAMS; i++)
-    if (!grads[i]) {
-      set_error("%s: grads[%d] is NULL", what, i);
-      return WN_E_INVALID;
-    }
+  int rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS);
+  if (rc) return rc;
   if (n <= 0 || n > 65535) {
     set_error("%s: 1..65535 images per call, got n=%d", what, n);
     return n <= 0 ? WN_E_INVALID : WN_E_UNSUPPORTED;
@@ -1055,12 +1040,8 @@ int wn_backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images_host,
     hs[i] = t.height;
     ws[i] = t.width;
   }
-  int rc = backward_ragged_tiled_check(what, hs.data(), ws.data(), n, tile_h, tile_w, max_pass_pixels);
-  if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  if ((rc = backward_ragged_tiled_check(what, hs.data(), ws.data(), n, tile_h, tile_w, max_pass_pixels))) return rc;
+  if ((rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   return backward_ragged_tiled(h, images_host, grad_out_host, grads, input_grads_host, n, tile_h, tile_w,
                                max_pass_pixels, workspace, workspace_bytes, (cudaStream_t)stream);
@@ -1086,17 +1067,10 @@ int wn_confidence_maps_backward_tiled(wn_handle* h, const float* x, const float*
     set_error("%s: null argument", what);
     return WN_E_INVALID;
   }
-  for (int i = 0; i < 16; i++)
-    if (!grads[i]) {
-      set_error("%s: grads[%d] is NULL", what, i);
-      return WN_E_INVALID;
-    }
-  int rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels);
+  int rc = check_param_grads(what, grads, 0, 16);
   if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  if ((rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels))) return rc;
+  if ((rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
   return submodule_backward_tiled(h, kStackCmg, 0, in, in_strides, grad_maps, grads, input_grads, n, height, width,
@@ -1116,17 +1090,10 @@ int wn_refine_backward_tiled(wn_handle* h, int which, const float* x, const floa
     set_error("%s: null argument", what);
     return WN_E_INVALID;
   }
-  for (int i = 16 + 6 * which; i < 22 + 6 * which; i++)
-    if (!grads[i]) {
-      set_error("%s: grads[%d] is NULL", what, i);
-      return WN_E_INVALID;
-    }
-  int rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels);
+  int rc = check_param_grads(what, grads, 16 + 6 * which, 6);
   if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  if ((rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels))) return rc;
+  if ((rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   // as wn_refine_train: refiner r sees cat[x, input r+1], so xbar goes to every slot
   const float* in[4] = {x, xbar, xbar, xbar};
@@ -1180,18 +1147,10 @@ int wn_debug_backward_layer(wn_handle* h, int stack, int which, int buffer, cons
   }
   // the parameter gradients the backward up to the launch writes: the stack's own entries
   const int first = stack == 1 ? 16 + 6 * which : 0, count = stack == -1 ? WN_NUM_PARAMS : stack == 0 ? 16 : 6;
-  if (buffer >= 14)
-    for (int i = first; i < first + count; i++)
-      if (!grads[i]) {
-        set_error("%s: grads[%d] is NULL", what, i);
-        return WN_E_INVALID;
-      }
-  int rc = submodule_train_check(what, n, height, width);
+  int rc = buffer >= 14 ? check_param_grads(what, grads, first, count) : WN_OK;
   if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  if ((rc = submodule_train_check(what, n, height, width))) return rc;
+  if ((rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   return debug_backward_layer(h, stack == -1 ? kStackAll : stack == 0 ? kStackCmg : kStackRefiners, which, buffer,
                               grad_out, grads, n, height, width, dst, workspace, workspace_bytes,

@@ -1,7 +1,7 @@
 // Backward pass of WaterNet on the tensor cores (SURVEY.md section 8f.1): the training hot loop
 // of the reference's train.py:100-133 (loss.backward() through waternet/net.py:99-108).
 //
-//   gate_bwd_kernel      d(out)/d(refined), d(out)/d(cm) and sigmoid'/ReLU' -> gradient planes
+//   seed_kernel          d(out)/d(refined), d(out)/d(cm) and sigmoid'/ReLU' -> gradient planes
 //   conv_umma_kernel     data gradient = the forward implicit-GEMM kernel run on flipped,
 //   <..., kEpiDgrad>     transposed weights; the epilogue applies ReLU' from the saved activation
 //   wgrad_umma_kernel    weight gradient: dW[co][ci][tap] = sum_px g[px][co] * a[px+tap][ci], a
@@ -282,140 +282,6 @@ __device__ __forceinline__ void gate_bwd_pixel(const float* go, const float* __r
   store_grad16(gr3, v9, n, pix, hw);
 }
 
-__global__ void __launch_bounds__(256)
-gate_bwd_kernel(const float* __restrict__ g_out, const float* __restrict__ cm, const float* __restrict__ refined,
-                uint4* __restrict__ g8, uint4* __restrict__ gr3, int hw) {
-  const int n = blockIdx.y;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  float go[3];
-#pragma unroll
-  for (int k = 0; k < 3; k++) go[k] = g_out[((size_t)n * 3 + k) * hw + pix];
-  gate_bwd_pixel(go, cm, refined, g8, gr3, n, pix, hw);
-}
-
-// The seeds of the sub-modules called on their own (wn_confidence_maps_backward, wn_refine_backward), as 16-channel
-// gradient planes like gate_bwd_kernel's.  maps = sigmoid(z_8):  g_z8[r] = d(map_r) * cm_r * (1 - cm_r).
-__global__ void __launch_bounds__(256)
-maps_bwd_kernel(const float* __restrict__ g_maps, const float* __restrict__ cm, uint4* __restrict__ g8, int hw) {
-  const int n = blockIdx.y;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  float v8[16];
-#pragma unroll
-  for (int j = 0; j < 16; j++) v8[j] = 0.f;
-#pragma unroll
-  for (int r = 0; r < 3; r++) {
-    const size_t o = ((size_t)n * 3 + r) * hw + pix;
-    const float c = cm[o];
-    v8[r] = g_maps[o] * c * (1.0f - c);
-  }
-  store_grad16(g8, v8, n, pix, hw);
-}
-
-// refiner `which` alone, out = relu(z_r3) of its three columns:  g_zr3[3 which + c] = d(out_c) where
-// refined[3 which + c] > 0; the other refiners' six columns are exactly 0, so nothing flows into their halves
-__global__ void __launch_bounds__(256)
-refine_bwd_kernel(const float* __restrict__ g_out, const float* __restrict__ refined, uint4* __restrict__ gr3,
-                  int which, int hw) {
-  const int n = blockIdx.y;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  float v9[16];
-#pragma unroll
-  for (int j = 0; j < 16; j++) v9[j] = 0.f;
-#pragma unroll
-  for (int r = 0; r < 3; r++) {
-    if (r != which) continue;
-#pragma unroll
-    for (int c = 0; c < 3; c++) {
-      const float rf = refined[((size_t)n * 9 + 3 * r + c) * hw + pix];
-      v9[3 * r + c] = rf > 0.f ? g_out[((size_t)n * 3 + c) * hw + pix] : 0.f;
-    }
-  }
-  store_grad16(gr3, v9, n, pix, hw);
-}
-
-// The windowed form (wn_backward_tiled): window blockIdx.y of the pass is window win0 + blockIdx.y of `tiles`.
-// d(loss)/d(out) is read from the full images (contiguous NCHW) at the window's kept pixels and is 0 elsewhere, so
-// every window back-propagates only the output pixels it owns.
-__global__ void __launch_bounds__(256)
-gate_bwd_tiled_kernel(const float* __restrict__ g_out, const float* __restrict__ cm, const float* __restrict__ refined,
-                      uint4* __restrict__ g8, uint4* __restrict__ gr3, TileGeom tiles, long long win0) {
-  const int hw = tiles.win_h * tiles.win_w;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
-  const int wy = pix / tiles.win_w;
-  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
-  const bool kept = y >= t.ky0 && y < t.ky1 && x >= t.kx0 && x < t.kx1;
-  const size_t ihw = (size_t)tiles.H * tiles.W;
-  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
-  float go[3];
-#pragma unroll
-  for (int k = 0; k < 3; k++) go[k] = kept ? g_out[o + k * ihw] : 0.f;
-  gate_bwd_pixel(go, cm, refined, g8, gr3, blockIdx.y, pix, hw);
-}
-
-// The windowed forms of maps_bwd_kernel / refine_bwd_kernel (wn_confidence_maps_backward_tiled,
-// wn_refine_backward_tiled), as gate_bwd_tiled_kernel is of gate_bwd_kernel: d(maps) or d(out) is read from the full
-// images (contiguous NCHW) at the window's kept pixels and is 0 elsewhere.
-__global__ void __launch_bounds__(256)
-maps_bwd_tiled_kernel(const float* __restrict__ g_maps, const float* __restrict__ cm, uint4* __restrict__ g8,
-                      TileGeom tiles, long long win0) {
-  const int hw = tiles.win_h * tiles.win_w;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
-  const int wy = pix / tiles.win_w;
-  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
-  const bool kept = y >= t.ky0 && y < t.ky1 && x >= t.kx0 && x < t.kx1;
-  const size_t ihw = (size_t)tiles.H * tiles.W;
-  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
-  float v8[16];
-#pragma unroll
-  for (int j = 0; j < 16; j++) v8[j] = 0.f;
-#pragma unroll
-  for (int r = 0; r < 3; r++) {
-    const float c = cm[((size_t)blockIdx.y * 3 + r) * hw + pix];
-    const float gm = kept ? g_maps[o + r * ihw] : 0.f;
-    v8[r] = gm * c * (1.0f - c);
-  }
-  store_grad16(g8, v8, blockIdx.y, pix, hw);
-}
-
-__global__ void __launch_bounds__(256)
-refine_bwd_tiled_kernel(const float* __restrict__ g_out, const float* __restrict__ refined, uint4* __restrict__ gr3,
-                        int which, TileGeom tiles, long long win0) {
-  const int hw = tiles.win_h * tiles.win_w;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
-  const int wy = pix / tiles.win_w;
-  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
-  const bool kept = y >= t.ky0 && y < t.ky1 && x >= t.kx0 && x < t.kx1;
-  const size_t ihw = (size_t)tiles.H * tiles.W;
-  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
-  float go[3], v9[16];
-#pragma unroll
-  for (int c = 0; c < 3; c++) go[c] = kept ? g_out[o + c * ihw] : 0.f;
-#pragma unroll
-  for (int j = 0; j < 16; j++) v9[j] = 0.f;
-#pragma unroll
-  for (int r = 0; r < 3; r++) {
-#pragma unroll
-    for (int c = 0; c < 3; c++) {
-      float v = 0.f;
-      if (r == which) {
-        const float rf = refined[((size_t)blockIdx.y * 9 + 3 * r + c) * hw + pix];
-        v = rf > 0.f ? go[c] : 0.f;
-      }
-      v9[3 * r + c] = v;
-    }
-  }
-  store_grad16(gr3, v9, blockIdx.y, pix, hw);
-}
-
 // data-gradient weights: dense_d[row_off + c][col(o)][kk-1-t] = W[o][c][t]   (transpose + spatial flip)
 // input channel c lands in row  row_off + c  (c < split)  or  row_off + c + shift  (c >= split)
 __global__ void scatter_weights_T_kernel(const float* __restrict__ src, float* __restrict__ dense, int co, int ci,
@@ -430,19 +296,174 @@ __global__ void scatter_weights_T_kernel(const float* __restrict__ src, float* _
   }
 }
 
-// d(loss)/d(input images) from the two 32-channel gradient buffers of the first layers (12 real channels:
-// x, wb, he, gc): sum them (hi + lo each) and write the four fp32 (N,3,H,W) tensors.
-struct InputGrads {
-  float* p[4];
+// ---- where a slot pixel of a backward pass sits in its image ------------------------------------------------------
+// A backward pass runs a batch of slots, each holding one window (or one whole image) at its top-left.  The per-pixel
+// kernels below (the seed, the input-gradient copy and the fold) are written once against one question: where does
+// pixel pix of slot s sit in its image?  Two geometries answer it: GridSlots (the windows of one tile_geom, or whole
+// images) and TableSlots (a device table of RaggedWindows).
+//
+// Per image: d(loss)/d(out) and the four input-gradient tensors (any may be null), fp32 contiguous (1,3,H,W).
+struct RaggedGrads {
+  const float* g_out;
+  float* in[4];
 };
-// v[3t + c] = d(loss)/d(input t, channel c) at pixel pix of image n of the batch
-__device__ __forceinline__ void input_grads_pixel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, int n,
-                                                  int pix, int hw, float* v) {
+
+// d_out(p): the image's d(out) or d(maps), 3 planes; d_in(p, t): its input gradient t, 3 planes (NULL: not wanted)
+struct SlotPixel {
+  int img;          // the image
+  int y, x;         // image coordinates
+  bool valid;       // inside the slot's valid extent (slot pixels beyond it hold no image pixel)
+  bool kept;        // valid and inside the window's kept rectangle: the only pixels seeded from d(out)
+  size_t ihw, o;    // the image's plane size, and y * W + x
+  TileGeom tiles;   // the windows it is cut into (the fold)
+  long long k0;     // its tile k is window k0 + k of the pass's numbering
+};
+
+// Grid slots: slot s is window w0 + s of `tiles` (tile_window); d(out) and the input gradients are contiguous
+// (N,3,H,W) tensors.  An untiled call is the case tile = image size and w0 = 0: slot s is image s, kept everywhere.
+struct GridSlots {
+  TileGeom tiles;
+  long long w0;
+  const float* g_out;
+  float* in[4];
+  __device__ int slot_width() const { return tiles.win_w; }
+  __device__ int slot_hw() const { return tiles.win_h * tiles.win_w; }
+  __device__ void check_plan() const {}
+  __device__ const float* d_out(const SlotPixel& p) const { return g_out + (size_t)p.img * 3 * p.ihw; }
+  __device__ float* d_in(const SlotPixel& p, int t) const {
+    return in[t] ? in[t] + (size_t)p.img * 3 * p.ihw : nullptr;
+  }
+  __device__ void origin(long long k, int* ys, int* xs) const {
+    const TileWindow t = tile_window(tiles, k);
+    *ys = t.ys;
+    *xs = t.xs;
+  }
+  __device__ SlotPixel at(int s, int pix) const {
+    const TileWindow t = tile_window(tiles, w0 + s);
+    const int wy = pix / tiles.win_w;
+    SlotPixel p;
+    p.y = t.ys + wy;
+    p.x = t.xs + (pix - wy * tiles.win_w);
+    p.valid = true;
+    p.kept = p.y >= t.ky0 && p.y < t.ky1 && p.x >= t.kx0 && p.x < t.kx1;
+    p.img = t.img;
+    p.ihw = (size_t)tiles.H * tiles.W;
+    p.o = (size_t)p.y * tiles.W + p.x;
+    p.tiles = tiles;
+    p.k0 = (long long)t.img * tiles.ny * tiles.nx;
+    return p;
+  }
+};
+
+// Table slots: slot s is window wins[w0 + s] of a ragged plan, at the top-left of a slot_h x slot_w slot; each image
+// is cut into the windows of tile_geom(H, W, tile_h, tile_w), contiguous in the plan in ascending tile order (checked
+// on the host), so tile k of the image of plan window w is plan window w - wins[w].tile + k.
+struct TableSlots {
+  const RaggedWindow* wins;
+  const RaggedGrads* imgs;
+  long long w0;
+  int slot_h, slot_w;
+  int tile_h, tile_w;
+  const int* plan;  // wn_backward_ragged: n, slot_h, slot_w as the forward call wrote them; NULL otherwise
+  __device__ int slot_width() const { return slot_w; }
+  __device__ int slot_hw() const { return slot_h * slot_w; }
+  // a backward with sizes other than the forward's stops instead of reading the wrong activations
+  __device__ void check_plan() const {
+    assert(!plan || (plan[0] == (int)gridDim.y && plan[1] == slot_h && plan[2] == slot_w));
+  }
+  __device__ const float* d_out(const SlotPixel& p) const { return imgs[p.img].g_out; }
+  __device__ float* d_in(const SlotPixel& p, int t) const { return imgs[p.img].in[t]; }
+  __device__ void origin(long long k, int* ys, int* xs) const {
+    *ys = wins[k].ys;
+    *xs = wins[k].xs;
+  }
+  __device__ SlotPixel at(int s, int pix) const {
+    const long long me = w0 + s;
+    const RaggedWindow& r = wins[me];
+    const int wy = pix / slot_w, wx = pix - wy * slot_w;
+    SlotPixel p;
+    p.y = r.ys + wy;
+    p.x = r.xs + wx;
+    p.valid = wy < r.vh && wx < r.vw;
+    p.kept = p.valid && p.y >= r.ky0 && p.y < r.ky1 && p.x >= r.kx0 && p.x < r.kx1;
+    p.img = r.img;
+    p.ihw = (size_t)r.H * r.W;
+    p.o = (size_t)p.y * r.W + p.x;
+    p.tiles = tile_geom(r.H, r.W, tile_h, tile_w);
+    p.k0 = me - r.tile;
+    return p;
+  }
+};
+
+// The seed of a backward pass, from go = d(out) at kept pixels and 0 everywhere else (so every window
+// back-propagates only the output pixels it owns):
+//   kStackAll       the gate (gate_bwd_pixel) -> g8 and gr3
+//   kStackCmg       maps = sigmoid(z_8):  g_z8[r] = d(map_r) * cm_r * (1 - cm_r) -> g8
+//   kStackRefiners  refiner `which` alone, out = relu(z_r3) of its three columns:  g_zr3[3 which + c] = d(out_c)
+//                   where refined[3 which + c] > 0; the other refiners' six columns are exactly 0 -> gr3
+template <class Geom>
+__global__ void __launch_bounds__(256)
+seed_kernel(Geom geo, int stack, int which, const float* __restrict__ cm, const float* __restrict__ refined,
+            uint4* __restrict__ g8, uint4* __restrict__ gr3) {
+  geo.check_plan();
+  const int hw = geo.slot_hw();
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= hw) return;
+  const int s = blockIdx.y;
+  const SlotPixel p = geo.at(s, pix);
+  const float* g = geo.d_out(p);
+  float go[3];
+#pragma unroll
+  for (int k = 0; k < 3; k++) go[k] = p.kept ? g[k * p.ihw + p.o] : 0.f;
+  if (stack == kStackAll) {
+    gate_bwd_pixel(go, cm, refined, g8, gr3, s, pix, hw);
+    return;
+  }
+  float v[16];
+#pragma unroll
+  for (int j = 0; j < 16; j++) v[j] = 0.f;
+  if (stack == kStackCmg) {
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+      const float c = cm[((size_t)s * 3 + r) * hw + pix];
+      v[r] = go[r] * c * (1.0f - c);
+    }
+  } else {
+    float gz[3];  // refiner `which`'s three columns
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      const float rf = refined[((size_t)s * 9 + 3 * which + c) * hw + pix];
+      gz[c] = rf > 0.f ? go[c] : 0.f;
+    }
+#pragma unroll
+    for (int r = 0; r < 3; r++)  // constant indices into v
+#pragma unroll
+      for (int c = 0; c < 3; c++) v[3 * r + c] = r == which ? gz[c] : 0.f;
+  }
+  store_grad16(stack == kStackCmg ? g8 : gr3, v, s, pix, hw);
+}
+
+// d(loss)/d(input images) from the 32-channel buffers of the first layers (12 real channels: packed input k is
+// channels 3k..3k+2 of cat[x, wb, he, gc]): a = gin_a (cmg.conv1), b = gin_b (the refiners' conv1), NULL: not part
+// of the call.  Input t of the call receives packed input slot[t]: {0, 1, 2, 3} for the whole network (a and b) and
+// the cmg (a); {0, which + 1} for refiner `which` (b), which reads cat[x, input which+1] (the forward handed xbar to
+// all three refiners; the other refiners' seeds are zero, so their rows of the data gradient add exact zeros).
+struct FirstLayerGrads {
+  const uint4* a;
+  const uint4* b;
+  int slot[4];
+};
+
+// v[3k + c] = d(loss)/d(packed input k, channel c) at pixel pix of slot n: the buffers given, hi + lo each, summed
+// in the order a_hi, a_lo, b_hi, b_lo.  A NULL buffer is skipped.
+__device__ __forceinline__ void first_layer_grads_pixel(const uint4* __restrict__ ga, const uint4* __restrict__ gb,
+                                                        int n, int pix, int hw, float* v) {
 #pragma unroll
   for (int j = 0; j < 16; j++) v[j] = 0.f;
   const uint4* bufs[2] = {ga, gb};
 #pragma unroll
   for (int b = 0; b < 2; b++) {
+    if (!bufs[b]) continue;
 #pragma unroll
     for (int plane = 0; plane < 2; plane++) {
 #pragma unroll
@@ -457,305 +478,82 @@ __device__ __forceinline__ void input_grads_pixel(const uint4* __restrict__ ga, 
   }
 }
 
-__global__ void __launch_bounds__(256)
-input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, InputGrads out, int hw) {
-  const int n = blockIdx.y;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  float v[16];
-  input_grads_pixel(ga, gb, n, pix, hw, v);
-#pragma unroll
-  for (int t = 0; t < 4; t++)
-#pragma unroll
-    for (int c = 0; c < 3; c++) out.p[t][((size_t)n * 3 + c) * hw + pix] = v[t * 3 + c];
+// channel c of packed input s in v (constant indices into v)
+__device__ __forceinline__ float packed_input(const float* v, int s, int c) {
+  return s == 0 ? v[c] : s == 1 ? v[3 + c] : s == 2 ? v[6 + c] : v[9 + c];
 }
 
-// ---- the ragged training step (wn_forward_train_ragged / wn_backward_ragged): slot n of the pass holds image
-// wins[n].img at its top-left, valid extent wins[n].vh x wins[n].vw (the whole image).  Per image: d(loss)/d(out) and
-// the four input-gradient tensors (any may be null), fp32 contiguous (1,3,H,W).
-struct RaggedGrads {
-  const float* g_out;
-  float* in[4];
-};
-
-// The ragged form of gate_bwd_kernel: d(out) read at image coordinates inside the valid extent, 0 beyond it.  plan:
-// n, slot_h, slot_w as the forward call wrote them; the grid must be the same pass (gridDim.y = n slots).
-__global__ void __launch_bounds__(256)
-gate_bwd_ragged_kernel(const int* __restrict__ plan, const RaggedGrads* __restrict__ imgs, const RaggedWindow* __restrict__ wins,
-                       const float* __restrict__ cm, const float* __restrict__ refined, uint4* __restrict__ g8,
-                       uint4* __restrict__ gr3, int slot_h, int slot_w) {
-  assert(plan[0] == (int)gridDim.y && plan[1] == slot_h && plan[2] == slot_w);
-  const int hw = slot_h * slot_w;
+// The untiled calls: each slot's valid extent is copied into its image.  Only the valid extent is read: the first
+// layer's data gradient has no ReLU mask and is not zero beyond it.
+template <class Geom>
+__global__ void __launch_bounds__(256) extract_input_grads_kernel(Geom geo, FirstLayerGrads f) {
+  const int hw = geo.slot_hw();
   const int pix = blockIdx.x * 256 + threadIdx.x;
   if (pix >= hw) return;
-  const RaggedWindow& r = wins[blockIdx.y];
-  const int wy = pix / slot_w, wx = pix - wy * slot_w;
-  const bool valid = wy < r.vh && wx < r.vw;
-  const size_t ihw = (size_t)r.H * r.W;
-  const float* g = imgs[r.img].g_out + (size_t)(r.ys + wy) * r.W + (r.xs + wx);
-  float go[3];
-#pragma unroll
-  for (int k = 0; k < 3; k++) go[k] = valid ? g[k * ihw] : 0.f;
-  gate_bwd_pixel(go, cm, refined, g8, gr3, blockIdx.y, pix, hw);
-}
-
-// The ragged form of input_grads_kernel: only the valid extent of each slot is read (the input-gradient launches
-// have no ReLU mask, so gin_a / gin_b are not zero beyond it) and stored into the slot's image.
-__global__ void __launch_bounds__(256)
-input_grads_ragged_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb,
-                          const RaggedGrads* __restrict__ imgs, const RaggedWindow* __restrict__ wins, int slot_h,
-                          int slot_w) {
-  const int hw = slot_h * slot_w;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  const RaggedWindow& r = wins[blockIdx.y];
-  const int wy = pix / slot_w, wx = pix - wy * slot_w;
-  if (wy >= r.vh || wx >= r.vw) return;
+  const SlotPixel p = geo.at(blockIdx.y, pix);
+  if (!p.valid) return;
   float v[16];
-  input_grads_pixel(ga, gb, blockIdx.y, pix, hw, v);
-  const size_t ihw = (size_t)r.H * r.W, o = (size_t)(r.ys + wy) * r.W + (r.xs + wx);
-  const RaggedGrads& d = imgs[r.img];
-#pragma unroll
-  for (int t = 0; t < 4; t++)
-    if (d.in[t])
-#pragma unroll
-      for (int c = 0; c < 3; c++) d.in[t][c * ihw + o] = v[t * 3 + c];
-}
-
-// The input gradients of a sub-module call, from the one 32-channel buffer its first layer wrote (the cmg: gin_a,
-// a refiner: gin_b): out.p[t] (NULL: skipped) receives packed channels 3 slot[t] .. 3 slot[t] + 2 (hi + lo).
-struct SubInputGrads {
-  float* p[4];
-  int slot[4];
-};
-__global__ void __launch_bounds__(256)
-submodule_input_grads_kernel(const uint4* __restrict__ g, SubInputGrads out, int hw) {
-  const int n = blockIdx.y;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  float v[16];
-#pragma unroll
-  for (int j = 0; j < 16; j++) v[j] = 0.f;
-#pragma unroll
-  for (int plane = 0; plane < 2; plane++)
-#pragma unroll
-    for (int half = 0; half < 2; half++) {
-      const uint4 q = g[((size_t)n * 8 + half * 4 + plane) * hw + pix];
-      const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-      for (int j = 0; j < 8; j++) v[plane * 8 + j] += __uint_as_float(((w[j >> 1] >> ((j & 1) * 16)) & 0xffffu) << 16);
-    }
+  first_layer_grads_pixel(f.a, f.b, blockIdx.y, pix, hw, v);
 #pragma unroll
   for (int t = 0; t < 4; t++) {
-    if (!out.p[t]) continue;
+    float* d = geo.d_in(p, t);
+    if (!d) continue;
 #pragma unroll
-    for (int s = 0; s < 4; s++) {  // a constant index into v
-      if (s != out.slot[t]) continue;
-#pragma unroll
-      for (int c = 0; c < 3; c++) out.p[t][((size_t)n * 3 + c) * hw + pix] = v[3 * s + c];
-    }
+    for (int c = 0; c < 3; c++) d[c * p.ihw + p.o] = packed_input(v, f.slot[t], c);
   }
 }
 
-// The windowed form (wn_backward_tiled): add the input gradients of the pass's windows (w0, w0 + 1, ...) into the
-// four full (N,3,H,W) images.  Thread (blockIdx.y, pix) is pixel pix of window w0 + blockIdx.y.  Of the windows of
-// this pass that contain its image pixel (tile_cover), only the first does the work: it adds their contributions
-// one at a time in ascending window index to what earlier passes left there.  No atomics, and the order of the
-// additions at a pixel is the window order whatever the pass size.
-__global__ void __launch_bounds__(256)
-fold_input_grads_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb, InputGrads out, TileGeom tiles,
-                        long long w0, int count) {
-  const int hw = tiles.win_h * tiles.win_w;
+// The windowed calls: the pass holds windows [w0, w0 + count).  Of the windows of the pass that contain a valid
+// pixel's image pixel (tile_cover), only the first does the work: it adds their contributions one at a time in
+// ascending window index to what earlier passes left there.  No atomics, and the order of the additions at a pixel
+// is the window order whatever the pass size.
+template <class Geom>
+__global__ void __launch_bounds__(256) fold_input_grads_kernel(Geom geo, FirstLayerGrads f, int count) {
+  const int hw = geo.slot_hw();
   const int pix = blockIdx.x * 256 + threadIdx.x;
   if (pix >= hw) return;
-  const long long me = w0 + blockIdx.y;
-  const TileWindow t = tile_window(tiles, me);
-  const int wy = pix / tiles.win_w;
-  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
-  const TileCover c = tile_cover(tiles, y, x);
-  const long long img0 = (long long)t.img * tiles.ny * tiles.nx;
+  const SlotPixel p = geo.at(blockIdx.y, pix);
+  if (!p.valid) return;
+  const long long w0 = geo.w0;
+  const TileCover c = tile_cover(p.tiles, p.y, p.x);
   long long first = -1;
   for (int i = c.i0; i <= c.i1 && first < 0; i++)
     for (int j = c.j0; j <= c.j1; j++) {
-      const long long k = img0 + (long long)i * tiles.nx + j;
+      const long long k = p.k0 + (long long)i * p.tiles.nx + j;
       if (k >= w0 && k < w0 + count) {
         first = k;
         break;
       }
     }
-  if (first != me) return;
-  const size_t ihw = (size_t)tiles.H * tiles.W;
-  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
+  if (first != w0 + blockIdx.y) return;
   float acc[12];
 #pragma unroll
-  for (int q = 0; q < 4; q++)
+  for (int q = 0; q < 4; q++) {
+    const float* d = geo.d_in(p, q);
 #pragma unroll
-    for (int ch = 0; ch < 3; ch++) acc[q * 3 + ch] = out.p[q][o + ch * ihw];
+    for (int ch = 0; ch < 3; ch++) acc[q * 3 + ch] = d ? d[p.o + ch * p.ihw] : 0.f;
+  }
   for (int i = c.i0; i <= c.i1; i++)
     for (int j = c.j0; j <= c.j1; j++) {
-      const long long k = img0 + (long long)i * tiles.nx + j;
+      const long long k = p.k0 + (long long)i * p.tiles.nx + j;
       if (k < w0 || k >= w0 + count) continue;
-      const TileWindow u = tile_window(tiles, k);
+      int ys, xs;
+      geo.origin(k, &ys, &xs);
       float v[16];
-      input_grads_pixel(ga, gb, (int)(k - w0), (y - u.ys) * tiles.win_w + (x - u.xs), hw, v);
+      first_layer_grads_pixel(f.a, f.b, (int)(k - w0), (p.y - ys) * geo.slot_width() + (p.x - xs), hw, v);
 #pragma unroll
-      for (int q = 0; q < 12; q++) acc[q] += v[q];
-    }
+      for (int q = 0; q < 4; q++)
 #pragma unroll
-  for (int q = 0; q < 4; q++)
-#pragma unroll
-    for (int ch = 0; ch < 3; ch++) out.p[q][o + ch * ihw] = acc[q * 3 + ch];
-}
-
-// The windowed form of submodule_input_grads_kernel (wn_confidence_maps_backward_tiled, wn_refine_backward_tiled):
-// the one 32-channel buffer g of the pass's windows, folded into the full images out.p[t] (NULL: skipped) in the
-// order of fold_input_grads_kernel: the first covering window of the pass adds the contributions of all of them, in
-// ascending window index, to what earlier passes left.  No atomics.
-__device__ __forceinline__ void sub_input_grads_pixel(const uint4* __restrict__ g, int n, int pix, int hw, float* v) {
-#pragma unroll
-  for (int j = 0; j < 16; j++) v[j] = 0.f;
-#pragma unroll
-  for (int plane = 0; plane < 2; plane++)
-#pragma unroll
-    for (int half = 0; half < 2; half++) {
-      const uint4 q = g[((size_t)n * 8 + half * 4 + plane) * hw + pix];
-      const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-      for (int j = 0; j < 8; j++) v[plane * 8 + j] += __uint_as_float(((w[j >> 1] >> ((j & 1) * 16)) & 0xffffu) << 16);
-    }
-}
-
-__global__ void __launch_bounds__(256)
-fold_submodule_input_grads_kernel(const uint4* __restrict__ g, SubInputGrads out, TileGeom tiles, long long w0,
-                                  int count) {
-  const int hw = tiles.win_h * tiles.win_w;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  const long long me = w0 + blockIdx.y;
-  const TileWindow t = tile_window(tiles, me);
-  const int wy = pix / tiles.win_w;
-  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
-  const TileCover c = tile_cover(tiles, y, x);
-  const long long img0 = (long long)t.img * tiles.ny * tiles.nx;
-  long long first = -1;
-  for (int i = c.i0; i <= c.i1 && first < 0; i++)
-    for (int j = c.j0; j <= c.j1; j++) {
-      const long long k = img0 + (long long)i * tiles.nx + j;
-      if (k >= w0 && k < w0 + count) {
-        first = k;
-        break;
-      }
-    }
-  if (first != me) return;
-  const size_t ihw = (size_t)tiles.H * tiles.W;
-  const size_t o = (size_t)t.img * 3 * ihw + (size_t)y * tiles.W + x;
-  float acc[12];
-#pragma unroll
-  for (int q = 0; q < 4; q++)
-#pragma unroll
-    for (int ch = 0; ch < 3; ch++) acc[q * 3 + ch] = out.p[q] ? out.p[q][o + ch * ihw] : 0.f;
-  for (int i = c.i0; i <= c.i1; i++)
-    for (int j = c.j0; j <= c.j1; j++) {
-      const long long k = img0 + (long long)i * tiles.nx + j;
-      if (k < w0 || k >= w0 + count) continue;
-      const TileWindow u = tile_window(tiles, k);
-      float v[16];
-      sub_input_grads_pixel(g, (int)(k - w0), (y - u.ys) * tiles.win_w + (x - u.xs), hw, v);
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        const int s = out.slot[q];
-#pragma unroll
-        for (int ch = 0; ch < 3; ch++)  // constant indices into v
-          acc[q * 3 + ch] += s == 0 ? v[ch] : s == 1 ? v[3 + ch] : s == 2 ? v[6 + ch] : v[9 + ch];
-      }
+        for (int ch = 0; ch < 3; ch++) acc[q * 3 + ch] += packed_input(v, f.slot[q], ch);
     }
 #pragma unroll
   for (int q = 0; q < 4; q++) {
-    if (!out.p[q]) continue;
+    float* d = geo.d_in(p, q);
+    if (!d) continue;
 #pragma unroll
-    for (int ch = 0; ch < 3; ch++) out.p[q][o + ch * ihw] = acc[q * 3 + ch];
+    for (int ch = 0; ch < 3; ch++) d[p.o + ch * p.ihw] = acc[q * 3 + ch];
   }
 }
-
-// The ragged windowed forms (wn_backward_ragged_tiled): slot blockIdx.y of a pass holds window wins[blockIdx.y] of the
-// plan at its top-left.  The seed reads d(out) of the window's own image at image coordinates inside the kept
-// rectangle and is 0 everywhere else, slot pixels beyond the valid extent included.
-__global__ void __launch_bounds__(256)
-gate_bwd_ragged_tiled_kernel(const RaggedGrads* __restrict__ imgs, const RaggedWindow* __restrict__ wins,
-                             const float* __restrict__ cm, const float* __restrict__ refined, uint4* __restrict__ g8,
-                             uint4* __restrict__ gr3, int slot_h, int slot_w) {
-  const int hw = slot_h * slot_w;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  const RaggedWindow& r = wins[blockIdx.y];
-  const int wy = pix / slot_w, wx = pix - wy * slot_w;
-  const int y = r.ys + wy, x = r.xs + wx;
-  const bool kept = wy < r.vh && wx < r.vw && y >= r.ky0 && y < r.ky1 && x >= r.kx0 && x < r.kx1;
-  const size_t ihw = (size_t)r.H * r.W;
-  const float* g = imgs[r.img].g_out;
-  float go[3];
-#pragma unroll
-  for (int k = 0; k < 3; k++) go[k] = kept ? g[k * ihw + (size_t)y * r.W + x] : 0.f;
-  gate_bwd_pixel(go, cm, refined, g8, gr3, blockIdx.y, pix, hw);
-}
-
-// The fold: slot blockIdx.y is plan window p0 + blockIdx.y, and the pass holds plan windows [p0, p0 + count).  An
-// image's windows are contiguous in the plan in ascending tile order (checked on the host), so tile k of the image of
-// plan window w is plan window w - wins[w].tile + k.  Of the windows of the pixel's own image that contain it
-// (tile_cover on that image's tile_geom) and sit in this pass, only the first does the work: it adds their
-// contributions one at a time in ascending tile order to what earlier passes left there, the order of
-// fold_input_grads_kernel for that image alone.  Only the valid extent of a slot is read: the first layer's data
-// gradient has no ReLU mask and is not zero beyond it.  No atomics.
-__global__ void __launch_bounds__(256)
-fold_input_grads_ragged_kernel(const uint4* __restrict__ ga, const uint4* __restrict__ gb,
-                               const RaggedGrads* __restrict__ imgs, const RaggedWindow* __restrict__ wins,
-                               long long p0, int count, int slot_h, int slot_w, int tile_h, int tile_w) {
-  const int hw = slot_h * slot_w;
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  if (pix >= hw) return;
-  const long long me = p0 + blockIdx.y;
-  const RaggedWindow& r = wins[me];
-  const int wy = pix / slot_w, wx = pix - wy * slot_w;
-  if (wy >= r.vh || wx >= r.vw) return;
-  const int y = r.ys + wy, x = r.xs + wx;
-  const TileGeom tiles = tile_geom(r.H, r.W, tile_h, tile_w);
-  const TileCover c = tile_cover(tiles, y, x);
-  const long long img0 = me - r.tile;
-  long long first = -1;
-  for (int i = c.i0; i <= c.i1 && first < 0; i++)
-    for (int j = c.j0; j <= c.j1; j++) {
-      const long long k = img0 + (long long)i * tiles.nx + j;
-      if (k >= p0 && k < p0 + count) {
-        first = k;
-        break;
-      }
-    }
-  if (first != me) return;
-  const RaggedGrads& d = imgs[r.img];
-  const size_t ihw = (size_t)r.H * r.W, o = (size_t)y * r.W + x;
-  float acc[12];
-#pragma unroll
-  for (int q = 0; q < 4; q++)
-#pragma unroll
-    for (int ch = 0; ch < 3; ch++) acc[q * 3 + ch] = d.in[q] ? d.in[q][o + ch * ihw] : 0.f;
-  for (int i = c.i0; i <= c.i1; i++)
-    for (int j = c.j0; j <= c.j1; j++) {
-      const long long k = img0 + (long long)i * tiles.nx + j;
-      if (k < p0 || k >= p0 + count) continue;
-      const RaggedWindow& u = wins[k];
-      float v[16];
-      input_grads_pixel(ga, gb, (int)(k - p0), (y - u.ys) * slot_w + (x - u.xs), hw, v);
-#pragma unroll
-      for (int q = 0; q < 12; q++) acc[q] += v[q];
-    }
-#pragma unroll
-  for (int q = 0; q < 4; q++) {
-    if (!d.in[q]) continue;
-#pragma unroll
-    for (int ch = 0; ch < 3; ch++) d.in[q][o + ch * ihw] = acc[q * 3 + ch];
-  }
-}
-
 // dst.p[k][i] += src.p[k][i] for the 34 parameter gradients; blockIdx.y = k
 struct ParamGrads {
   float* p[WN_NUM_PARAMS];
@@ -1035,17 +833,19 @@ static int launch_dgrad(wn_handle* h, uint4* g_in, uint4* g_out, const uint4* sa
                                                                               h->bwd->zero_bias, g_in, a, stream);
 }
 
-// wn_debug_backward_layer: the backward pass stops after data-gradient launch `li` and decodes its output into dst
-// (the gradient buffers ping-pong, so it cannot be read afterwards).  li = -1: the normal path, never stops.
+// wn_debug_backward_layer: the backward pass stops after the seed (buffer kDebugG8 or kDebugGr3) or after
+// data-gradient launch li (buffer kDebugDgrad + li) and decodes that buffer into dst (the gradient buffers ping-pong,
+// so it cannot be read afterwards).  buffer = -1: the normal path, never stops.
+static constexpr int kDebugG8 = 12, kDebugGr3 = 13, kDebugDgrad = 14;
 struct BwdStop {
-  int li = -1;
+  int buffer = -1;
   float* dst = nullptr;
 };
-static constexpr int kBwdStopped = 1;  // returned up the call chain once the launch asked for has been decoded
+static constexpr int kBwdStopped = 1;  // returned up the call chain once the buffer asked for has been decoded
 
 static int stop_after(wn_handle* h, const BwdStop& stop, int li, const uint4* g_out, int n, int hw,
                       cudaStream_t stream) {
-  if (stop.li != li) return WN_OK;
+  if (stop.buffer != kDebugDgrad + li) return WN_OK;
   const int rc = decode_planes(h, g_out, stop.dst, kDSpecs[li].npad * kDSpecs[li].nblk / 8, n, hw, stream);
   return rc ? rc : kBwdStopped;
 }
@@ -1073,7 +873,7 @@ static int cmg_conv_backward(wn_handle* h, const TrainBuffers& t, float* const* 
 }
 
 // The two halves of the backward pass of a batch whose forward activations are in t.  The confidence-map half starts
-// from the gradient planes t.g8, the refiner half from t.gr3 (gate_bwd_kernel, or a sub-module's own seed).  Each
+// from the gradient planes t.g8, the refiner half from t.gr3 (seed_kernel).  Each
 // overwrites its stack's parameter gradients in grads (state-dict order) and, when want_input_grads, writes the data
 // gradient of the packed 16-channel input into t.gin_a (cmg.conv1) or t.gin_b (the refiners' conv1).
 static int backward_cmg(wn_handle* h, const TrainBuffers& t, float* const* grads, bool want_input_grads, int n, int H,
@@ -1148,29 +948,85 @@ static int backward_layers(wn_handle* h, const TrainBuffers& t, float* const* gr
   return rc ? rc : backward_refiners(h, t, grads, -1, want_input_grads, n, H, W, stream, stop);
 }
 
-int backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n, int H,
-             int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (!h->bwd) {
-    set_error("backward weights have not been packed");
-    return WN_E_STATE;
+// One backward pass over n slots of H x W whose training forward is in t, at the slots of geo: the seed of `stack`
+// (seed_kernel), that stack's backward (its parameter gradients into grads, overwritten), then, when want_in, the
+// input gradients of the first layer, copied into the images (untiled calls) or folded into them (windowed calls).
+template <class Geom>
+static int backward_pass(wn_handle* h, const Geom& geo, int stack, int which, const TrainBuffers& t,
+                         float* const* grads, bool want_in, bool fold, int n, int H, int W, cudaStream_t stream,
+                         const BwdStop& stop = BwdStop()) {
+  const dim3 grid((unsigned)(((size_t)H * W + 255) / 256), n);
+  seed_kernel<<<grid, 256, 0, stream>>>(geo, stack, which, t.f.cm, t.f.refined, t.g8, t.gr3);
+  WN_LAUNCH_CHECK(h);
+  int rc;
+  if (stop.buffer == kDebugG8 || stop.buffer == kDebugGr3) {
+    rc = decode_planes(h, stop.buffer == kDebugG8 ? t.g8 : t.gr3, stop.dst, 2, n, H * W, stream);
+    return rc ? rc : kBwdStopped;
   }
-  int rc = check_train_args(n, H, W, workspace_bytes);
+  rc = stack == kStackAll   ? backward_layers(h, t, grads, want_in, n, H, W, stream, stop)
+       : stack == kStackCmg ? backward_cmg(h, t, grads, want_in, n, H, W, stream, stop)
+                            : backward_refiners(h, t, grads, which, want_in, n, H, W, stream, stop);
+  if (rc || !want_in) return rc;
+  // carve() leaves the other stack's buffer of a sub-module NULL
+  FirstLayerGrads f = {t.gin_a, t.gin_b, {0, 1, 2, 3}};
+  if (stack == kStackRefiners) f.slot[1] = which + 1;
+  if (fold)
+    fold_input_grads_kernel<<<grid, 256, 0, stream>>>(geo, f, n);
+  else
+    extract_input_grads_kernel<<<grid, 256, 0, stream>>>(geo, f);
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+
+static int check_bwd_packed(const wn_handle* h) {
+  if (h->bwd && h->umma) return WN_OK;
+  set_error("backward weights have not been packed");
+  return WN_E_STATE;
+}
+
+static int check_submodule_args(int n, int H, int W, int stack, size_t bytes);
+
+// The training buffers of an untiled call of `stack`, as its training forward left them in the workspace
+static int untiled_buffers(TrainBuffers* t, int stack, int n, int H, int W, void* workspace, size_t workspace_bytes) {
+  int rc = stack == kStackAll ? check_train_args(n, H, W, workspace_bytes)
+                              : check_submodule_args(n, H, W, stack, workspace_bytes);
   if (rc) return rc;
   if ((rc = get_encoder())) return rc;
-  TrainBuffers t;
-  carve(&t, workspace, (size_t)n * H * W);
-  const int hw = H * W;
-
-  gate_bwd_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(grad_out, t.f.cm, t.f.refined, t.g8, t.gr3, hw);
-  WN_LAUNCH_CHECK(h);
-  if ((rc = backward_layers(h, t, grads, input_grads != nullptr, n, H, W, stream))) return rc;
-  if (input_grads) {
-    InputGrads ig;
-    for (int i = 0; i < 4; i++) ig.p[i] = input_grads[i];
-    input_grads_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(t.gin_a, t.gin_b, ig, hw);
-    WN_LAUNCH_CHECK(h);
-  }
+  carve(t, workspace, (size_t)n * H * W, stack);
   return WN_OK;
+}
+
+// The slots of an untiled call: slot s is image s, whole; g: d(out) or d(maps); in: NULL or n_in input gradients
+static GridSlots whole_images(int H, int W, const float* g, float* const* in, int n_in) {
+  GridSlots s = {tile_geom(H, W, H, W), 0, g, {nullptr, nullptr, nullptr, nullptr}};
+  for (int i = 0; in && i < n_in; i++) s.in[i] = in[i];
+  return s;
+}
+
+static bool any_of4(float* const* p, int count) {
+  if (!p) return false;
+  for (int i = 0; i < count; i++)
+    if (p[i]) return true;
+  return false;
+}
+
+// wn_backward, wn_confidence_maps_backward, wn_refine_backward: the backward of what the stack's training forward
+// left in the workspace
+static int untiled_backward(wn_handle* h, int stack, int which, const float* grad, float* const* grads,
+                            float* const* input_grads, int n, int H, int W, void* workspace, size_t workspace_bytes,
+                            cudaStream_t stream) {
+  int rc = check_bwd_packed(h);
+  if (rc) return rc;
+  TrainBuffers t;
+  if ((rc = untiled_buffers(&t, stack, n, H, W, workspace, workspace_bytes))) return rc;
+  const int n_in = stack == kStackRefiners ? 2 : 4;
+  return backward_pass(h, whole_images(H, W, grad, input_grads, n_in), stack, which, t, grads,
+                       any_of4(input_grads, n_in), false, n, H, W, stream);
+}
+
+int backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n, int H,
+             int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  return untiled_backward(h, kStackAll, -1, grad_out, grads, input_grads, n, H, W, workspace, workspace_bytes, stream);
 }
 
 // ---- the ragged training step ------------------------------------------------------------------------------------
@@ -1178,8 +1034,8 @@ int backward(wn_handle* h, const float* grad_out, float* const* grads, float* co
 // The forward masks every ReLU activation beyond each image (the RAG layers), and the backward seeds 0 there, so
 // every gradient plane a weight-gradient GEMM reads is 0 at masked pixels and adds exact zeros (DESIGN.md 4.10).
 // Workspace: [plan: n, slot_h, slot_w | windows | PackInArgs | RaggedGrads, one each per image][the training carve-up
-// of n slots].  The backward derives its carve-up from the sizes it is given; gate_bwd_ragged_kernel asserts that
-// they give the plan the forward wrote, so a backward with other sizes stops instead of reading the wrong activations.
+// of n slots].  The backward derives its carve-up from the sizes it is given; its seed asserts that they give the
+// plan the forward wrote, so a backward with other sizes stops instead of reading the wrong activations.
 static void ragged_slot(const int* hs, const int* ws, int n, int* sh, int* sw) {
   *sh = *sw = 0;
   for (int i = 0; i < n; i++) {
@@ -1197,6 +1053,32 @@ size_t train_ragged_workspace_bytes(const int* hs, const int* ws, int n) {
   int sh, sw;
   ragged_slot(hs, ws, n, &sh, &sw);
   return 256 + 256 + ragged_train_table_bytes(n) + train_workspace_bytes_padded(n, sh, sw);
+}
+
+// The per-image host table of a ragged call: imgs[i] (the four inputs and their strides) when imgs is given, and
+// grads[i] (d(out) and the four input gradients, NULL: not wanted) when grads is given.  Returns whether any input
+// gradient is wanted.
+static bool ragged_table(const wn_ragged_tensors* images, const float* const* grad_out, float* const* input_grads,
+                         int n, PackInArgs* imgs, RaggedGrads* grads) {
+  bool want_in = false;
+  for (int i = 0; i < n; i++) {
+    if (imgs) {
+      const wn_ragged_tensors& d = images[i];
+      const float* p[4] = {d.x, d.wb, d.he, d.gc};
+      for (int t = 0; t < 4; t++) {
+        imgs[i].p[t] = p[t];
+        for (int k = 0; k < 4; k++) imgs[i].s[t][k] = d.in_strides[t][k];
+      }
+    }
+    if (grads) {
+      grads[i].g_out = grad_out[i];
+      for (int t = 0; t < 4; t++) {
+        grads[i].in[t] = input_grads ? input_grads[4 * i + t] : nullptr;
+        want_in = want_in || grads[i].in[t];
+      }
+    }
+  }
+  return want_in;
 }
 
 // the table's three parts and the training buffers of a workspace of any alignment
@@ -1243,21 +1125,15 @@ int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, v
   const int plan[3] = {n, sh, sw};
   memcpy(host.data(), plan, sizeof(plan));
   RaggedWindow* wins = reinterpret_cast<RaggedWindow*>(host.data() + 256);
-  PackInArgs* imgs = reinterpret_cast<PackInArgs*>(host.data() + 256 + win_b);
   for (int i = 0; i < n; i++) {
-    const wn_ragged_tensors& d = images[i];
     RaggedWindow r = {};
-    r.out_f32 = d.out;
+    r.out_f32 = images[i].out;
     r.img = i;
-    r.H = r.vh = r.ky1 = d.height;
-    r.W = r.vw = r.kx1 = d.width;
+    r.H = r.vh = r.ky1 = images[i].height;
+    r.W = r.vw = r.kx1 = images[i].width;
     wins[i] = r;
-    const float* p[4] = {d.x, d.wb, d.he, d.gc};
-    for (int t = 0; t < 4; t++) {
-      imgs[i].p[t] = p[t];
-      for (int k = 0; k < 4; k++) imgs[i].s[t][k] = d.in_strides[t][k];
-    }
   }
+  ragged_table(images, nullptr, nullptr, n, reinterpret_cast<PackInArgs*>(host.data() + 256 + win_b), nullptr);
   // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
   WN_CUDA(cudaMemcpyAsync(l.plan, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
   int rc;
@@ -1274,39 +1150,23 @@ int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, v
 
 int backward_ragged(wn_handle* h, const int* hs, const int* ws, const float* const* grad_out, float* const* grads,
                     float* const* input_grads, int n, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (!h->bwd) {
-    set_error("backward weights have not been packed");
-    return WN_E_STATE;
-  }
+  int rc = check_bwd_packed(h);
+  if (rc) return rc;
   const size_t need = train_ragged_workspace_bytes(hs, ws, n);
   if (workspace_bytes < need) {
     set_error("ragged training workspace too small: %zu < %zu", workspace_bytes, need);
     return WN_E_WORKSPACE;
   }
-  int rc;
   if ((rc = get_encoder())) return rc;
   int sh, sw;
   ragged_slot(hs, ws, n, &sh, &sw);
   RaggedTrainLayout l = ragged_train_layout(workspace, n, sh, sw);
-  bool want_in = false;
   std::vector<RaggedGrads> host(n);
-  for (int i = 0; i < n; i++) {
-    host[i].g_out = grad_out[i];
-    for (int t = 0; t < 4; t++) {
-      host[i].in[t] = input_grads ? input_grads[4 * i + t] : nullptr;
-      want_in = want_in || host[i].in[t];
-    }
-  }
+  const bool want_in = ragged_table(nullptr, grad_out, input_grads, n, nullptr, host.data());
   WN_CUDA(cudaMemcpyAsync(l.grads, host.data(), (size_t)n * sizeof(RaggedGrads), cudaMemcpyHostToDevice, stream));
-  const dim3 grid((unsigned)(((size_t)sh * sw + 255) / 256), n);
-  gate_bwd_ragged_kernel<<<grid, 256, 0, stream>>>(l.plan, l.grads, l.wins, l.t.f.cm, l.t.f.refined, l.t.g8, l.t.gr3, sh, sw);
-  WN_LAUNCH_CHECK(h);
-  if ((rc = backward_layers(h, l.t, grads, want_in, n, sh, sw, stream))) return rc;
-  if (want_in) {
-    input_grads_ragged_kernel<<<grid, 256, 0, stream>>>(l.t.gin_a, l.t.gin_b, l.grads, l.wins, sh, sw);
-    WN_LAUNCH_CHECK(h);
-  }
-  return WN_OK;
+  // every image is one window of its own size
+  const TableSlots geo = {l.wins, l.grads, 0, sh, sw, sh, sw, l.plan};
+  return backward_pass(h, geo, kStackAll, -1, l.t, grads, want_in, false, n, sh, sw, stream);
 }
 
 // ---- the sub-modules under autograd (wn_confidence_maps_train / _backward, wn_refine_train / _backward) -----------
@@ -1327,13 +1187,6 @@ static int check_submodule_args(int n, int H, int W, int stack, size_t bytes) {
   return WN_OK;
 }
 
-static bool any_of4(float* const* p, int count) {
-  if (!p) return false;
-  for (int i = 0; i < count; i++)
-    if (p[i]) return true;
-  return false;
-}
-
 int confidence_maps_train(wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out_maps, int n,
                           int H, int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   int rc = check_submodule_args(n, H, W, kStackCmg, workspace_bytes);
@@ -1349,30 +1202,8 @@ int confidence_maps_train(wn_handle* h, const float* const in[4], const int64_t 
 
 int confidence_maps_backward(wn_handle* h, const float* grad_maps, float* const* grads, float* const* input_grads,
                              int n, int H, int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (!h->bwd) {
-    set_error("backward weights have not been packed");
-    return WN_E_STATE;
-  }
-  int rc = check_submodule_args(n, H, W, kStackCmg, workspace_bytes);
-  if (rc) return rc;
-  if ((rc = get_encoder())) return rc;
-  TrainBuffers t;
-  carve(&t, workspace, (size_t)n * H * W, kStackCmg);
-  const int hw = H * W;
-  const bool want_in = any_of4(input_grads, 4);
-  maps_bwd_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(grad_maps, t.f.cm, t.g8, hw);
-  WN_LAUNCH_CHECK(h);
-  if ((rc = backward_cmg(h, t, grads, want_in, n, H, W, stream))) return rc;
-  if (want_in) {
-    SubInputGrads ig;
-    for (int i = 0; i < 4; i++) {  // cat[x, wb, he, gc]: image i is packed channels 3i..3i+2
-      ig.p[i] = input_grads[i];
-      ig.slot[i] = i;
-    }
-    submodule_input_grads_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(t.gin_a, ig, hw);
-    WN_LAUNCH_CHECK(h);
-  }
-  return WN_OK;
+  return untiled_backward(h, kStackCmg, 0, grad_maps, grads, input_grads, n, H, W, workspace, workspace_bytes,
+                          stream);
 }
 
 int refine_train(wn_handle* h, int which, const float* const in[4], const int64_t st[4][4], float* out, int n, int H,
@@ -1393,28 +1224,8 @@ int refine_train(wn_handle* h, int which, const float* const in[4], const int64_
 
 int refine_backward(wn_handle* h, int which, const float* grad_out, float* const* grads, float* const* input_grads,
                     int n, int H, int W, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (!h->bwd) {
-    set_error("backward weights have not been packed");
-    return WN_E_STATE;
-  }
-  int rc = check_submodule_args(n, H, W, kStackRefiners, workspace_bytes);
-  if (rc) return rc;
-  if ((rc = get_encoder())) return rc;
-  TrainBuffers t;
-  carve(&t, workspace, (size_t)n * H * W, kStackRefiners);
-  const int hw = H * W;
-  const bool want_in = any_of4(input_grads, 2);
-  refine_bwd_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(grad_out, t.f.refined, t.gr3, which, hw);
-  WN_LAUNCH_CHECK(h);
-  if ((rc = backward_refiners(h, t, grads, which, want_in, n, H, W, stream))) return rc;
-  if (want_in) {
-    // refiner `which` reads cat[x, input which+1] (the forward handed xbar to all three slots; the other refiners'
-    // seeds are zero, so their rows of the first layer's data gradient add exact zeros)
-    SubInputGrads ig = {{input_grads[0], input_grads[1], nullptr, nullptr}, {0, which + 1, 0, 0}};
-    submodule_input_grads_kernel<<<dim3((hw + 255) / 256, n), 256, 0, stream>>>(t.gin_b, ig, hw);
-    WN_LAUNCH_CHECK(h);
-  }
-  return WN_OK;
+  return untiled_backward(h, kStackRefiners, which, grad_out, grads, input_grads, n, H, W, workspace, workspace_bytes,
+                          stream);
 }
 
 // ---- wn_debug_backward_layer (test aid) ---------------------------------------------------------------------------
@@ -1422,31 +1233,25 @@ int refine_backward(wn_handle* h, int which, const float* grad_out, float* const
 // 14 + li the output of data-gradient launch li (DgradLayer).  Which of them a stack's training pass has:
 static bool debug_buffer_in_stack(int buffer, int stack) {
   if (buffer == 0 || stack == kStackAll) return true;
-  const bool cmg_buffer = buffer <= 8 || buffer == 12 || (buffer >= 14 + kD8 && buffer <= 14 + kD2) ||
-                          buffer == 14 + kD1;
+  const bool cmg_buffer = buffer <= 8 || buffer == kDebugG8 || (buffer >= kDebugDgrad + kD8 && buffer <= kDebugDgrad + kD2) ||
+                          buffer == kDebugDgrad + kD1;
   return cmg_buffer == (stack == kStackCmg);
 }
 
 int debug_backward_layer(wn_handle* h, int stack, int which, int buffer, const float* grad_out, float* const* grads,
                          int n, int H, int W, float* dst, void* workspace, size_t workspace_bytes,
                          cudaStream_t stream) {
-  if (!h->bwd) {
-    set_error("backward weights have not been packed");
-    return WN_E_STATE;
-  }
+  int rc = check_bwd_packed(h);
+  if (rc) return rc;
   if (!debug_buffer_in_stack(buffer, stack)) {
     set_error("wn_debug_backward_layer: the training pass of this stack has no buffer %d", buffer);
     return WN_E_INVALID;
   }
-  int rc = stack == kStackAll ? check_train_args(n, H, W, workspace_bytes)
-                              : check_submodule_args(n, H, W, stack, workspace_bytes);
-  if (rc) return rc;
-  if ((rc = get_encoder())) return rc;
   TrainBuffers t;
-  carve(&t, workspace, (size_t)n * H * W, stack);
+  if ((rc = untiled_buffers(&t, stack, n, H, W, workspace, workspace_bytes))) return rc;
   const int hw = H * W;
   // the saved forward activations, as wn_forward_train or the sub-module's *_train call left them
-  if (buffer <= 11) {
+  if (buffer < kDebugG8) {
     static constexpr int kChannels[12] = {16, 128, 128, 128, 64, 64, 64, 64, 3, 96, 96, 9};
     const int c = kChannels[buffer];
     if (buffer == 8 || buffer == 11) {
@@ -1458,32 +1263,22 @@ int debug_backward_layer(wn_handle* h, int stack, int which, int buffer, const f
     return decode_planes(h, planes, dst, c / 8, n, hw, stream);
   }
   // the seed of the stack's backward, then the backward up to the launch asked for (input gradients included)
-  const dim3 grid((hw + 255) / 256, n);
-  if (stack == kStackAll)
-    gate_bwd_kernel<<<grid, 256, 0, stream>>>(grad_out, t.f.cm, t.f.refined, t.g8, t.gr3, hw);
-  else if (stack == kStackCmg)
-    maps_bwd_kernel<<<grid, 256, 0, stream>>>(grad_out, t.f.cm, t.g8, hw);
-  else
-    refine_bwd_kernel<<<grid, 256, 0, stream>>>(grad_out, t.f.refined, t.gr3, which, hw);
-  WN_LAUNCH_CHECK(h);
-  if (buffer == 12 || buffer == 13) return decode_planes(h, buffer == 12 ? t.g8 : t.gr3, dst, 2, n, hw, stream);
   BwdStop stop;
-  stop.li = buffer - 14;
+  stop.buffer = buffer;
   stop.dst = dst;
-  rc = stack == kStackAll ? backward_layers(h, t, grads, true, n, H, W, stream, stop)
-       : stack == kStackCmg ? backward_cmg(h, t, grads, true, n, H, W, stream, stop)
-                            : backward_refiners(h, t, grads, which, true, n, H, W, stream, stop);
+  rc = backward_pass(h, whole_images(H, W, grad_out, nullptr, 0), stack, which, t, grads, true, false, n, H, W,
+                     stream, stop);
   return rc == kBwdStopped ? WN_OK : rc;
 }
 
-// ---- windowed recompute backward (wn_backward_tiled, DESIGN.md "Windowed backward") -------------------------------
+// ---- windowed recompute backward (wn_backward_tiled and the sub-modules' windowed calls, DESIGN.md 4.8, 4.9, 4.11) -
 // The windows of tiling.cuh, one pass of them at a time: recompute the training forward of the pass, then run the
 // backward pass above on its windows as a batch, each window's output gradient taken from grad_out inside its kept
 // rectangle and 0 elsewhere.  Because no pixel more than kTileHalo from a kept pixel gets a gradient, each window's
 // contribution equals that of its kept pixels in the untiled backward.  The first pass writes the parameter
-// gradients, every later pass writes them into a scratch copy and adds that in (pass order).  Input gradients are
-// zeroed, then folded in window order.  Workspace: [flag | scratch parameter gradients | one pass of training
-// buffers], independent of the image size.  Nothing is copied from the host.
+// gradients of the stack, every later pass writes them into a scratch copy that add_param_grads_kernel adds in (pass
+// order).  Input gradients are zeroed, then folded in window order.  Workspace: [flag | scratch parameter gradients |
+// (ragged: the table) | one pass of training buffers].
 static void param_grad_sizes(int* size) {
   for (int c = 0; c < 8; c++) {
     size[2 * c] = kCmg[c].cout * kCmg[c].cin * kCmg[c].ks * kCmg[c].ks;
@@ -1497,12 +1292,91 @@ static void param_grad_sizes(int* size) {
     }
 }
 
-static size_t param_grads_bytes() {
-  int size[WN_NUM_PARAMS];
+// the stack's own entries [first, first + count) of the 34 parameter gradients
+static void stack_params(int stack, int which, int* first, int* count) {
+  *first = stack == kStackRefiners ? 16 + 6 * which : 0;
+  *count = stack == kStackAll ? WN_NUM_PARAMS : stack == kStackCmg ? 16 : 6;
+}
+
+static size_t param_grads_bytes(int stack) {
+  int size[WN_NUM_PARAMS], first, count;
   param_grad_sizes(size);
+  stack_params(stack, 0, &first, &count);  // the three refiners have the same shapes
   size_t b = 0;
-  for (int k = 0; k < WN_NUM_PARAMS; k++) b += ((size_t)size[k] * sizeof(float) + 255) / 256 * 256;
+  for (int k = first; k < first + count; k++) b += align256b((size_t)size[k] * sizeof(float));
   return b;
+}
+
+// The scratch copy of the stack's parameter gradients, from p on: dst / part are the stack's own entries, compacted
+// (add_param_grads_kernel grid y = count); later is the 34-entry layout the backward writes from the second pass
+// on, the own entries pointing at the scratch copy.  Returns the end of the copy.
+struct ScratchGrads {
+  ParamGrads dst, part;
+  float* later[WN_NUM_PARAMS];
+  int count;
+};
+static uint8_t* scratch_grads(ScratchGrads* s, uint8_t* p, float* const* grads, int stack, int which) {
+  int size[WN_NUM_PARAMS], first;
+  param_grad_sizes(size);
+  stack_params(stack, which, &first, &s->count);
+  for (int k = 0; k < WN_NUM_PARAMS; k++) s->later[k] = nullptr;
+  for (int k = 0; k < s->count; k++) {
+    s->dst.p[k] = grads[first + k];
+    s->part.p[k] = s->later[first + k] = (float*)p;
+    s->dst.size[k] = s->part.size[k] = size[first + k];
+    p += align256b((size_t)size[first + k] * sizeof(float));
+  }
+  return p;
+}
+
+// Each pass's act0 planes (and, for a ragged pass, its window table for the masked forward)
+static int pack_pass(wn_handle* h, GridSlots* geo, const float* const in[4], const int64_t st[4][4],
+                     const PackInArgs*, const RaggedPass& q, uint4* act0, int*, FwdOpts*, cudaStream_t stream) {
+  geo->w0 = q.first;
+  return pack_input_windows(h, in, st, act0, geo->tiles.H, geo->tiles.W, geo->tiles, q.first, q.count, stream);
+}
+static int pack_pass(wn_handle* h, TableSlots* geo, const float* const*, const int64_t (*)[4],
+                     const PackInArgs* imgs, const RaggedPass& q, uint4* act0, int* exact, FwdOpts* o,
+                     cudaStream_t stream) {
+  geo->w0 = q.first;
+  geo->slot_h = q.slot_h;
+  geo->slot_w = q.slot_w;
+  o->rwin = geo->wins + q.first;
+  return pack_input_ragged(h, imgs, geo->wins + q.first, q.count, q.slot_h, q.slot_w, act0, exact, stream);
+}
+
+// The pass loop: per pass, the bf16x3 training forward of the stack (a refiner's first layer is kRL1, as in
+// refine_train; the backward needs cm and refined, not the output), then backward_pass with the fold.  in / st: the
+// four images of a grid call; imgs: the per-image table of a ragged one.  *exact already holds the exact-levels flag
+// of the forward that produced the output (the first layer drops its a_lo pass exactly when that forward did).
+template <class Geom>
+static int recompute_passes(wn_handle* h, Geom geo, const std::vector<RaggedPass>& passes, int stack, int which,
+                            const float* const in[4], const int64_t st[4][4], const PackInArgs* imgs, int* exact,
+                            ScratchGrads& s, float* const* grads, bool want_in, void* pass_ws, size_t pass_bytes,
+                            cudaStream_t stream) {
+  for (size_t pi = 0; pi < passes.size(); pi++) {
+    const RaggedPass& q = passes[pi];
+    int rc = stack == kStackAll ? check_train_args(q.count, q.slot_h, q.slot_w, pass_bytes)
+                                : check_submodule_args(q.count, q.slot_h, q.slot_w, stack, pass_bytes);
+    if (rc) return rc;
+    TrainBuffers t;
+    carve(&t, pass_ws, (size_t)q.count * q.slot_h * q.slot_w, stack);
+    t.f.exact_flag = exact;
+    FwdOpts o;
+    o.packed = true;
+    o.stack = stack;
+    o.refiner_l1 = stack == kStackRefiners;
+    if ((rc = pack_pass(h, &geo, in, st, imgs, q, t.f.act0, exact, &o, stream))) return rc;
+    if ((rc = umma_forward_layers(h, in, st, nullptr, q.count, q.slot_h, q.slot_w, t.f, stream, o))) return rc;
+    if ((rc = backward_pass(h, geo, stack, which, t, pi == 0 ? grads : s.later, want_in, true, q.count, q.slot_h,
+                            q.slot_w, stream)))
+      return rc;
+    if (pi > 0) {
+      add_param_grads_kernel<<<dim3(64, s.count), 256, 0, stream>>>(s.dst, s.part);
+      WN_LAUNCH_CHECK(h);
+    }
+  }
+  return WN_OK;
 }
 
 static long long tiled_train_pass(const TileGeom& g, int n, long long max_pass_pixels) {
@@ -1512,86 +1386,84 @@ static long long tiled_train_pass(const TileGeom& g, int n, long long max_pass_p
 size_t backward_tiled_workspace_bytes(int n, int H, int W, int tile_h, int tile_w, long long max_pass_pixels) {
   const TileGeom g = tile_geom(H, W, tile_h, tile_w);
   const long long p = tiled_train_pass(g, n, max_pass_pixels);
-  return 256 + param_grads_bytes() + train_workspace_bytes_padded((int)p, g.win_h, g.win_w) + 256;
+  return 256 + param_grads_bytes(kStackAll) + train_workspace_bytes_padded((int)p, g.win_h, g.win_w) + 256;
+}
+
+// The windows of one stack's call (kTileHalo = 13 for both sub-modules too; a refiner's receptive-field radius is 6)
+// once the workspace is checked.  in: the stack's four packed inputs; grad: d(out) or d(maps); input_grads: NULL or
+// 4 (kStackAll, kStackCmg) / 2 (kStackRefiners) entries.  Nothing is copied from the host.
+static int grid_recompute_backward(wn_handle* h, int stack, int which, const float* const in[4],
+                                   const int64_t st[4][4], const float* grad, float* const* grads,
+                                   float* const* input_grads, int n, int H, int W, int tile_h, int tile_w,
+                                   long long max_pass_pixels, void* workspace, size_t workspace_bytes,
+                                   cudaStream_t stream) {
+  int rc = get_encoder();
+  if (rc) return rc;
+  GridSlots geo = whole_images(H, W, grad, input_grads, stack == kStackRefiners ? 2 : 4);
+  geo.tiles = tile_geom(H, W, tile_h, tile_w);
+  const TileGeom& g = geo.tiles;
+  uint8_t* base = (uint8_t*)align256b((uintptr_t)workspace);
+  int* exact = (int*)base;
+  ScratchGrads s;
+  uint8_t* pass_ws = scratch_grads(&s, base + 256, grads, stack, which);
+  const size_t pass_bytes = workspace_bytes - (size_t)(pass_ws - (uint8_t*)workspace);
+  bool want_in = false;
+  for (int i = 0; i < 4; i++)
+    if (geo.in[i]) {
+      want_in = true;
+      WN_CUDA(cudaMemsetAsync(geo.in[i], 0, (size_t)n * 3 * H * W * sizeof(float), stream));
+    }
+  if ((rc = pack_exact_flag(h, in, st, exact, n, H, W, g, stream))) return rc;
+  std::vector<RaggedPass> passes;
+  const long long total = (long long)n * g.ny * g.nx, per_pass = tiled_train_pass(g, n, max_pass_pixels);
+  for (long long w0 = 0; w0 < total; w0 += per_pass)
+    passes.push_back({w0, (int)std::min(per_pass, total - w0), g.win_h, g.win_w});
+  return recompute_passes(h, geo, passes, stack, which, in, st, nullptr, exact, s, grads, want_in, pass_ws,
+                          pass_bytes, stream);
 }
 
 int backward_tiled(wn_handle* h, const float* const in[4], const int64_t st[4][4], const float* grad_out,
                    float* const* grads, float* const* input_grads, int n, int H, int W, int tile_h, int tile_w,
                    long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (!h->bwd || !h->umma) {
-    set_error("backward weights have not been packed");
-    return WN_E_STATE;
-  }
+  int rc = check_bwd_packed(h);
+  if (rc) return rc;
   const size_t need = backward_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels);
   if (workspace_bytes < need) {
     set_error("tiled backward workspace too small: %zu < %zu", workspace_bytes, need);
     return WN_E_WORKSPACE;
   }
-  int rc = get_encoder();
-  if (rc) return rc;
+  return grid_recompute_backward(h, kStackAll, -1, in, st, grad_out, grads, input_grads, n, H, W, tile_h, tile_w,
+                                 max_pass_pixels, workspace, workspace_bytes, stream);
+}
+
+size_t submodule_backward_tiled_workspace_bytes(int n, int H, int W, int tile_h, int tile_w, long long max_pass_pixels,
+                                                int stack) {
   const TileGeom g = tile_geom(H, W, tile_h, tile_w);
-  const long long total = (long long)n * g.ny * g.nx;
-  const long long per_pass = tiled_train_pass(g, n, max_pass_pixels);
-  const size_t win_px = (size_t)g.win_h * g.win_w;
-  uint8_t* base = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
-  int* exact = (int*)base;
-  ParamGrads dst, part;
-  param_grad_sizes(dst.size);
-  uint8_t* p = base + 256;
-  for (int k = 0; k < WN_NUM_PARAMS; k++) {
-    dst.p[k] = grads[k];
-    part.p[k] = (float*)p;
-    part.size[k] = dst.size[k];
-    p += ((size_t)dst.size[k] * sizeof(float) + 255) / 256 * 256;
+  const long long p = tiled_train_pass(g, n, max_pass_pixels);
+  return 256 + param_grads_bytes(stack) + submodule_train_workspace_bytes((int)p, g.win_h, g.win_w, stack) + 256;
+}
+
+int submodule_backward_tiled(wn_handle* h, int stack, int which, const float* const in[4], const int64_t st[4][4],
+                             const float* grad, float* const* grads, float* const* input_grads, int n, int H, int W,
+                             int tile_h, int tile_w, long long max_pass_pixels, void* workspace, size_t workspace_bytes,
+                             cudaStream_t stream) {
+  int rc = check_bwd_packed(h);
+  if (rc) return rc;
+  const size_t need = submodule_backward_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels, stack);
+  if (workspace_bytes < need) {
+    set_error("tiled sub-module backward workspace too small: %zu < %zu", workspace_bytes, need);
+    return WN_E_WORKSPACE;
   }
-  void* pass_ws = p;
-  const size_t pass_bytes = workspace_bytes - (size_t)(p - (uint8_t*)workspace);
-  InputGrads ig;
-  if (input_grads)
-    for (int i = 0; i < 4; i++) {
-      ig.p[i] = input_grads[i];
-      WN_CUDA(cudaMemsetAsync(ig.p[i], 0, (size_t)n * 3 * H * W * sizeof(float), stream));
-    }
-  // the first layer drops its a_lo pass exactly when the forward that produced the output did (wn_forward_tiled)
-  if ((rc = pack_exact_flag(h, in, st, exact, n, H, W, g, stream))) return rc;
-  for (long long w0 = 0; w0 < total; w0 += per_pass) {
-    const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
-    if ((rc = check_train_args(cur, g.win_h, g.win_w, pass_bytes))) return rc;
-    TrainBuffers t;
-    carve(&t, pass_ws, (size_t)cur * win_px);
-    t.f.exact_flag = exact;
-    if ((rc = pack_input_windows(h, in, st, t.f.act0, H, W, g, w0, cur, stream))) return rc;
-    FwdOpts o;  // the bf16x3 scheme; the backward needs cm and refined, not the output
-    o.packed = true;
-    if ((rc = umma_forward_layers(h, in, st, nullptr, cur, g.win_h, g.win_w, t.f, stream, o))) return rc;
-    gate_bwd_tiled_kernel<<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(
-        grad_out, t.f.cm, t.f.refined, t.g8, t.gr3, g, w0);
-    WN_LAUNCH_CHECK(h);
-    if ((rc = backward_layers(h, t, w0 == 0 ? grads : part.p, input_grads != nullptr, cur, g.win_h, g.win_w,
-                              stream)))
-      return rc;
-    if (w0 > 0) {
-      add_param_grads_kernel<<<dim3(64, WN_NUM_PARAMS), 256, 0, stream>>>(dst, part);
-      WN_LAUNCH_CHECK(h);
-    }
-    if (input_grads) {
-      fold_input_grads_kernel<<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(t.gin_a, t.gin_b, ig,
-                                                                                                g, w0, cur);
-      WN_LAUNCH_CHECK(h);
-    }
-  }
-  return WN_OK;
+  return grid_recompute_backward(h, stack, which, in, st, grad, grads, input_grads, n, H, W, tile_h, tile_w,
+                                 max_pass_pixels, workspace, workspace_bytes, stream);
 }
 
 // ---- windowed recompute backward of a ragged batch (wn_backward_ragged_tiled, DESIGN.md 4.11) ---------------------
-// The pass loop of backward_tiled over the plan of ragged_plan: n images of their own sizes, cut into the windows
-// wn_backward_tiled cuts each of them into, sorted by shape and packed into passes of equally sized slots.  Per pass:
-// the bf16x3 training forward of forward_train_ragged (every ReLU layer stores zeros beyond each window's valid
-// extent), the seed from d(out) inside each kept rectangle, the backward pass of the slots, and the fold of the input
-// gradients into their images.  The first pass writes the parameter gradients, every later one a scratch copy that
-// add_param_grads_kernel adds in.  Workspace: [flag | scratch parameter gradients | table: one PackInArgs and one
-// RaggedGrads per image, then the windows in plan order | the largest pass of training buffers].  The table is
-// copied from pageable host memory once per call.
+// The pass loop over the plan of ragged_plan: n images of their own sizes, cut into the windows wn_backward_tiled
+// cuts each of them into, sorted by shape and packed into passes of equally sized slots.  Each pass's forward is
+// that of forward_train_ragged (every ReLU layer stores zeros beyond each window's valid extent).  The table (one
+// PackInArgs and one RaggedGrads per image, then the windows in plan order) sits between the scratch parameter
+// gradients and the pass buffers and is copied from pageable host memory once per call.
 static size_t ragged_tiled_table_bytes(int n, size_t windows) {
   return align256b((size_t)n * sizeof(PackInArgs)) + align256b((size_t)n * sizeof(RaggedGrads)) +
          align256b(windows * sizeof(RaggedWindow));
@@ -1606,7 +1478,7 @@ static size_t ragged_tiled_workspace(int n, const std::vector<RaggedWindow>& win
                                      const std::vector<RaggedPass>& passes) {
   long long px = 0;
   for (const RaggedPass& p : passes) px = std::max(px, (long long)p.count * p.slot_h * p.slot_w);
-  return 256 + param_grads_bytes() + ragged_tiled_table_bytes(n, wins.size()) +
+  return 256 + param_grads_bytes(kStackAll) + ragged_tiled_table_bytes(n, wins.size()) +
          train_workspace_bytes_padded(1, 1, (int)px) + 256;
 }
 
@@ -1621,10 +1493,8 @@ size_t backward_ragged_tiled_workspace_bytes(const int* hs, const int* ws, int n
 int backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images, const float* const* grad_out,
                           float* const* grads, float* const* input_grads, int n, int tile_h, int tile_w,
                           long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (!h->bwd || !h->umma) {
-    set_error("backward weights have not been packed");
-    return WN_E_STATE;
-  }
+  int rc = check_bwd_packed(h);
+  if (rc) return rc;
   std::vector<int> hs(n), ws(n);
   for (int i = 0; i < n; i++) {
     hs[i] = images[i].height;
@@ -1648,200 +1518,38 @@ int backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images, const f
       return WN_E_STATE;
     }
   }
-  int rc = get_encoder();
-  if (rc) return rc;
+  if ((rc = get_encoder())) return rc;
   uint8_t* base = (uint8_t*)align256b((uintptr_t)workspace);
   int* exact = (int*)base;
-  ParamGrads dst, part;
-  param_grad_sizes(dst.size);
-  uint8_t* p = base + 256;
-  for (int k = 0; k < WN_NUM_PARAMS; k++) {
-    dst.p[k] = grads[k];
-    part.p[k] = (float*)p;
-    part.size[k] = dst.size[k];
-    p += align256b((size_t)dst.size[k] * sizeof(float));
-  }
+  ScratchGrads s;
+  uint8_t* table = scratch_grads(&s, base + 256, grads, kStackAll, -1);
   // the table, built on the host in its device layout
   const size_t in_b = align256b((size_t)n * sizeof(PackInArgs)), g_b = align256b((size_t)n * sizeof(RaggedGrads));
   std::vector<uint8_t> host(in_b + g_b + wins.size() * sizeof(RaggedWindow));
-  PackInArgs* imgs = reinterpret_cast<PackInArgs*>(host.data());
   RaggedGrads* rg = reinterpret_cast<RaggedGrads*>(host.data() + in_b);
-  bool want_in = false;
-  for (int i = 0; i < n; i++) {
-    const wn_ragged_tensors& d = images[i];
-    const float* in[4] = {d.x, d.wb, d.he, d.gc};
-    for (int t = 0; t < 4; t++) {
-      imgs[i].p[t] = in[t];
-      for (int k = 0; k < 4; k++) imgs[i].s[t][k] = d.in_strides[t][k];
-    }
-    rg[i].g_out = grad_out[i];
-    for (int t = 0; t < 4; t++) {
-      rg[i].in[t] = input_grads ? input_grads[4 * i + t] : nullptr;
-      if (rg[i].in[t]) {
-        want_in = true;
-        WN_CUDA(cudaMemsetAsync(rg[i].in[t], 0, (size_t)3 * d.height * d.width * sizeof(float), stream));
-      }
-    }
-  }
+  const bool want_in =
+      ragged_table(images, grad_out, input_grads, n, reinterpret_cast<PackInArgs*>(host.data()), rg);
+  for (int i = 0; i < n; i++)
+    for (int t = 0; t < 4; t++)
+      if (rg[i].in[t])
+        WN_CUDA(cudaMemsetAsync(rg[i].in[t], 0, (size_t)3 * hs[i] * ws[i] * sizeof(float), stream));
   memcpy(host.data() + in_b + g_b, wins.data(), wins.size() * sizeof(RaggedWindow));
-  uint8_t* table = p;
   // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
   WN_CUDA(cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
   const PackInArgs* d_imgs = reinterpret_cast<const PackInArgs*>(table);
-  const RaggedGrads* d_grads = reinterpret_cast<const RaggedGrads*>(table + in_b);
-  const RaggedWindow* d_wins = reinterpret_cast<const RaggedWindow*>(table + in_b + g_b);
-  void* pass_ws = table + ragged_tiled_table_bytes(n, wins.size());
-  const size_t pass_bytes = workspace_bytes - (size_t)((uint8_t*)pass_ws - (uint8_t*)workspace);
-  // the first layer drops its a_lo pass exactly when the forward that produced the output did (wn_forward_ragged)
+  const TableSlots geo = {reinterpret_cast<const RaggedWindow*>(table + in_b + g_b),
+                          reinterpret_cast<const RaggedGrads*>(table + in_b), 0, 0, 0, tile_h, tile_w, nullptr};
+  uint8_t* pass_ws = table + ragged_tiled_table_bytes(n, wins.size());
+  const size_t pass_bytes = workspace_bytes - (size_t)(pass_ws - (uint8_t*)workspace);
+  // the exact-levels flag over every pass, as wn_forward_ragged takes it
   WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
   for (const RaggedPass& q : passes)
-    if ((rc = pack_input_ragged(h, d_imgs, d_wins + q.first, q.count, q.slot_h, q.slot_w, nullptr, exact, stream)))
+    if ((rc = pack_input_ragged(h, d_imgs, geo.wins + q.first, q.count, q.slot_h, q.slot_w, nullptr, exact, stream)))
       return rc;
   const int64_t none[4][4] = {};
   const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
-  for (size_t pi = 0; pi < passes.size(); pi++) {
-    const RaggedPass& q = passes[pi];
-    if ((rc = check_train_args(q.count, q.slot_h, q.slot_w, pass_bytes))) return rc;
-    TrainBuffers t;
-    carve(&t, pass_ws, (size_t)q.count * q.slot_h * q.slot_w);
-    t.f.exact_flag = exact;
-    if ((rc = pack_input_ragged(h, d_imgs, d_wins + q.first, q.count, q.slot_h, q.slot_w, t.f.act0, exact, stream)))
-      return rc;
-    FwdOpts o;  // the bf16x3 scheme; the backward needs cm and refined, not the output
-    o.packed = true;
-    o.rwin = d_wins + q.first;
-    if ((rc = umma_forward_layers(h, no_in, none, nullptr, q.count, q.slot_h, q.slot_w, t.f, stream, o))) return rc;
-    const dim3 grid((unsigned)(((size_t)q.slot_h * q.slot_w + 255) / 256), q.count);
-    gate_bwd_ragged_tiled_kernel<<<grid, 256, 0, stream>>>(d_grads, d_wins + q.first, t.f.cm, t.f.refined, t.g8,
-                                                           t.gr3, q.slot_h, q.slot_w);
-    WN_LAUNCH_CHECK(h);
-    if ((rc = backward_layers(h, t, pi == 0 ? grads : part.p, want_in, q.count, q.slot_h, q.slot_w, stream)))
-      return rc;
-    if (pi > 0) {
-      add_param_grads_kernel<<<dim3(64, WN_NUM_PARAMS), 256, 0, stream>>>(dst, part);
-      WN_LAUNCH_CHECK(h);
-    }
-    if (want_in) {
-      fold_input_grads_ragged_kernel<<<grid, 256, 0, stream>>>(t.gin_a, t.gin_b, d_grads, d_wins, q.first, q.count,
-                                                               q.slot_h, q.slot_w, tile_h, tile_w);
-      WN_LAUNCH_CHECK(h);
-    }
-  }
-  return WN_OK;
-}
-
-// ---- windowed recompute backward of one sub-module (wn_confidence_maps_backward_tiled, wn_refine_backward_tiled) --
-// The pass loop of backward_tiled for one stack: the windows are those of the same rule (kTileHalo = 13 for both
-// stacks; a refiner's receptive-field radius is 6), each pass recomputes that stack's training forward (a refiner's
-// first layer is kRL1, as in refine_train), seeds it from d(maps) or d(out) inside the kept rectangles, runs that
-// stack's half of the backward and folds its input gradients.  Parameter gradients: the first pass writes the stack's
-// own entries of grads, every later pass writes a scratch copy of them that add_param_grads_kernel adds in.
-// Workspace: [flag | scratch copy of the stack's parameter gradients | one pass of carve(stack)].
-static void stack_params(int stack, int which, int* first, int* count) {
-  *first = stack == kStackCmg ? 0 : 16 + 6 * which;
-  *count = stack == kStackCmg ? 16 : 6;
-}
-
-static size_t stack_param_grads_bytes(int stack) {
-  int size[WN_NUM_PARAMS], first, count;
-  param_grad_sizes(size);
-  stack_params(stack, 0, &first, &count);  // the three refiners have the same shapes
-  size_t b = 0;
-  for (int k = first; k < first + count; k++) b += ((size_t)size[k] * sizeof(float) + 255) / 256 * 256;
-  return b;
-}
-
-size_t submodule_backward_tiled_workspace_bytes(int n, int H, int W, int tile_h, int tile_w, long long max_pass_pixels,
-                                                int stack) {
-  const TileGeom g = tile_geom(H, W, tile_h, tile_w);
-  const long long p = tiled_train_pass(g, n, max_pass_pixels);
-  return 256 + stack_param_grads_bytes(stack) + submodule_train_workspace_bytes((int)p, g.win_h, g.win_w, stack) + 256;
-}
-
-int submodule_backward_tiled(wn_handle* h, int stack, int which, const float* const in[4], const int64_t st[4][4],
-                             const float* grad, float* const* grads, float* const* input_grads, int n, int H, int W,
-                             int tile_h, int tile_w, long long max_pass_pixels, void* workspace, size_t workspace_bytes,
-                             cudaStream_t stream) {
-  if (!h->bwd || !h->umma) {
-    set_error("backward weights have not been packed");
-    return WN_E_STATE;
-  }
-  const size_t need = submodule_backward_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels, stack);
-  if (workspace_bytes < need) {
-    set_error("tiled sub-module backward workspace too small: %zu < %zu", workspace_bytes, need);
-    return WN_E_WORKSPACE;
-  }
-  int rc = get_encoder();
-  if (rc) return rc;
-  const bool cmg = stack == kStackCmg;
-  const TileGeom g = tile_geom(H, W, tile_h, tile_w);
-  const long long total = (long long)n * g.ny * g.nx;
-  const long long per_pass = tiled_train_pass(g, n, max_pass_pixels);
-  const size_t win_px = (size_t)g.win_h * g.win_w;
-  uint8_t* base = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
-  int* exact = (int*)base;
-  int size[WN_NUM_PARAMS], first, count;
-  param_grad_sizes(size);
-  stack_params(stack, which, &first, &count);
-  // dst / part: the stack's own entries, compacted (add_param_grads_kernel grid y = count); later: the 34-entry
-  // layout the backward halves write, the own entries pointing at the scratch copy
-  ParamGrads dst, part;
-  float* later[WN_NUM_PARAMS] = {};
-  uint8_t* p = base + 256;
-  for (int k = 0; k < count; k++) {
-    dst.p[k] = grads[first + k];
-    part.p[k] = later[first + k] = (float*)p;
-    dst.size[k] = part.size[k] = size[first + k];
-    p += ((size_t)size[first + k] * sizeof(float) + 255) / 256 * 256;
-  }
-  void* pass_ws = p;
-  const size_t pass_bytes = workspace_bytes - (size_t)(p - (uint8_t*)workspace);
-  const int n_in = cmg ? 4 : 2;
-  bool want_in = false;
-  SubInputGrads ig = {{nullptr, nullptr, nullptr, nullptr}, {0, 0, 0, 0}};
-  for (int i = 0; i < n_in; i++) {
-    ig.p[i] = input_grads ? input_grads[i] : nullptr;
-    // cat[x, wb, he, gc]: image i is packed channels 3i..3i+2; refiner `which` reads cat[x, input which+1]
-    ig.slot[i] = cmg ? i : (i == 0 ? 0 : which + 1);
-    if (ig.p[i]) {
-      want_in = true;
-      WN_CUDA(cudaMemsetAsync(ig.p[i], 0, (size_t)n * 3 * H * W * sizeof(float), stream));
-    }
-  }
-  if ((rc = pack_exact_flag(h, in, st, exact, n, H, W, g, stream))) return rc;
-  for (long long w0 = 0; w0 < total; w0 += per_pass) {
-    const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
-    if ((rc = check_submodule_args(cur, g.win_h, g.win_w, stack, pass_bytes))) return rc;
-    TrainBuffers t;
-    carve(&t, pass_ws, (size_t)cur * win_px, stack);
-    t.f.exact_flag = exact;
-    if ((rc = pack_input_windows(h, in, st, t.f.act0, H, W, g, w0, cur, stream))) return rc;
-    FwdOpts o;
-    o.packed = true;
-    o.stack = stack;
-    o.refiner_l1 = !cmg;
-    if ((rc = umma_forward_layers(h, in, st, nullptr, cur, g.win_h, g.win_w, t.f, stream, o))) return rc;
-    const dim3 grid((unsigned)((win_px + 255) / 256), cur);
-    if (cmg)
-      maps_bwd_tiled_kernel<<<grid, 256, 0, stream>>>(grad, t.f.cm, t.g8, g, w0);
-    else
-      refine_bwd_tiled_kernel<<<grid, 256, 0, stream>>>(grad, t.f.refined, t.gr3, which, g, w0);
-    WN_LAUNCH_CHECK(h);
-    float* const* out = w0 == 0 ? grads : later;
-    rc = cmg ? backward_cmg(h, t, out, want_in, cur, g.win_h, g.win_w, stream)
-             : backward_refiners(h, t, out, which, want_in, cur, g.win_h, g.win_w, stream);
-    if (rc) return rc;
-    if (w0 > 0) {
-      add_param_grads_kernel<<<dim3(64, count), 256, 0, stream>>>(dst, part);
-      WN_LAUNCH_CHECK(h);
-    }
-    if (want_in) {
-      fold_submodule_input_grads_kernel<<<grid, 256, 0, stream>>>(cmg ? t.gin_a : t.gin_b, ig, g, w0, cur);
-      WN_LAUNCH_CHECK(h);
-    }
-  }
-  return WN_OK;
+  return recompute_passes(h, geo, passes, kStackAll, -1, no_in, none, d_imgs, exact, s, grads, want_in, pass_ws,
+                          pass_bytes, stream);
 }
 
 }  // namespace wn
-
