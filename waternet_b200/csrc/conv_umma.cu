@@ -19,11 +19,12 @@
 // out-of-image pixels come back as zeros from the TMA (padding="same").
 //
 // One persistent CTA per SM, warp-specialised:
-//   warps 0-7  two consumer warpgroups: each issues the m64 wgmmas of half of the 8x16- or 16x16-pixel tile
-//              (accumulators in registers; kSpecs mw, ng) and then runs the epilogue of those pixels
+//   warps 0-7  two consumer warpgroups (kSpecs wgs 2; wgs 3: warps 0-11, three): each issues the m64 wgmmas of its
+//              8 rows of the 8x16-, 16x16- or 8x24-pixel tile (accumulators in registers; kSpecs mw, ng) and then
+//              runs the epilogue of those pixels
 //              (registers -> shared-memory transpose -> bias/act -> bf16 hi/lo planes or fp32)
-//   warp 8     A producer (TMA halo tiles, one 16-channel chunk per stage)
-//   warp 9     B producer (bulk copies of pre-packed weight stages, 1-9 taps of a chunk per stage)
+//   warp 8     A producer (TMA halo tiles, one 16-channel chunk per stage); wgs 3: warp 12
+//   warp 9     B producer (bulk copies of pre-packed weight stages, 1-9 taps of a chunk per stage); wgs 3: warp 13
 #include "umma_conv.cuh"
 
 namespace wn {
@@ -151,24 +152,32 @@ enum UmmaLayer {
 // has an fp8-correction form (UmmaCfg FMT bit 0, the tensor-bound layers), which uses CONCAT 0.  mw = m64 blocks per
 // warpgroup (2: 16 x 16-pixel tiles, which halve the weight bytes streamed per pixel) and ng = column groups of npad /
 // ng channels each (UmmaCfg MW, NG): at mw = 2 the accumulators of both blocks must fit in 128 registers per thread.
+// wgs = consumer warpgroups (UmmaCfg WGS): 3 gives 8 x 24-pixel tiles, which cut the weight bytes streamed per pixel
+// by a third at mw = 1; a layer takes it where its kernels stay free of spills at 160 registers and measure faster.
 struct UmmaLayerSpec {
   int ks, cinpad, npad, epi, concat, nblk, tps, slot;
   bool f8;
-  int mw, ng;
+  int mw, ng, wgs;
 };
 static constexpr UmmaLayerSpec kSpecs[kNumUmmaLayers] = {
-    // ks cinpad npad epi       concat nblk tps slot f8  mw ng
-    {7, 16, 224, kEpiAct, 0, 1, 1, 0, false, 1, 1},     // kL1
-    {5, 128, 128, kEpiAct, 0, 1, 5, 1, true, 1, 1},     // kC2
-    {3, 128, 128, kEpiAct, 0, 1, 3, 2, true, 1, 1},     // kC3
-    {1, 128, 64, kEpiAct, 1, 1, 1, 3, false, 1, 1},     // kC4
-    {7, 64, 64, kEpiAct, 1, 1, 7, 4, true, 2, 1},       // kC5
-    {5, 64, 64, kEpiAct, 1, 1, 5, 5, true, 2, 1},       // kC6
-    {3, 64, 64, kEpiAct, 1, 1, 9, 6, true, 2, 1},       // kC7
-    {3, 64, 16, kEpiSigmoid, 1, 1, 9, 7, false, 1, 1},  // kC8
-    {5, 96, 32, kEpiAct, 1, 3, 5, 9, true, 1, 1},       // kR2
-    {3, 96, 16, kEpiGate, 1, 1, 9, 10, false, 1, 1},    // kR3
-    {7, 16, 96, kEpiAct, 0, 1, 1, 8, false, 1, 1}};     // kRL1 (CONCAT 0 as kL1: the same sums per channel)
+    // ks cinpad npad epi       concat nblk tps slot f8  mw ng wgs
+    {7, 16, 224, kEpiAct, 0, 1, 1, 0, false, 1, 1, 2},     // kL1
+    {5, 128, 128, kEpiAct, 0, 1, 5, 1, true, 1, 1, 2},     // kC2
+    {3, 128, 128, kEpiAct, 0, 1, 3, 2, true, 1, 1, 3},     // kC3
+    {1, 128, 64, kEpiAct, 1, 1, 1, 3, false, 1, 1, 3},     // kC4
+    {7, 64, 64, kEpiAct, 1, 1, 7, 4, true, 2, 1, 2},       // kC5
+    {5, 64, 64, kEpiAct, 1, 1, 5, 5, true, 2, 1, 2},       // kC6
+    {3, 64, 64, kEpiAct, 1, 1, 9, 6, true, 2, 1, 2},       // kC7
+    {3, 64, 16, kEpiSigmoid, 1, 1, 9, 7, false, 1, 1, 3},  // kC8
+    {5, 96, 32, kEpiAct, 1, 3, 5, 9, true, 1, 1, 3},       // kR2
+    {3, 96, 16, kEpiGate, 1, 1, 9, 10, false, 1, 1, 3},    // kR3
+    {7, 16, 96, kEpiAct, 0, 1, 1, 8, false, 1, 1, 3}};     // kRL1 (CONCAT 0 as kL1: the same sums per channel)
+// WN_UMMA_WGS2 builds every layer with two consumer warpgroups (16-row tiles), for A/B runs against the table
+#ifdef WN_UMMA_WGS2
+static constexpr int layer_wgs(int) { return 2; }
+#else
+static constexpr int layer_wgs(int li) { return kSpecs[li].wgs; }
+#endif
 
 // In the fp8-correction scheme a layer writes the hi + fp8-planes format (FMT bit 1) when its consumers read it with
 // their fp8 form.  L1 feeds C2 and R2; every other layer feeds the next one, except the last layer of each stack.
@@ -335,10 +344,10 @@ static int launch_layer_as(wn_handle* h, bool f8, void* in_base, ConvArgs a, cud
     constexpr int FMT = (s.f8 ? kFmtIn8 : 0) | (writes_f8(LI) ? kFmtOut8 : 0);
     if constexpr ((FMT & kFmtOut8) != 0) a.f8_overflow = u->overflow_dev;
     if constexpr (s.f8) a.f8_scale = u->scale8[LI] + 1;
-    return launch_conv<s.ks, s.cinpad, GW, s.epi, (s.f8 ? 0 : s.concat), s.nblk, s.tps, FMT, R, s.mw, s.ng>(
-        h, s.slot, s.f8 ? u->stages8[LI] : u->stages[LI], u->bias[LI], in_base, a, stream);
+    return launch_conv<s.ks, s.cinpad, GW, s.epi, (s.f8 ? 0 : s.concat), s.nblk, s.tps, FMT, R, s.mw, s.ng,
+                       layer_wgs(LI)>(h, s.slot, s.f8 ? u->stages8[LI] : u->stages[LI], u->bias[LI], in_base, a, stream);
   }
-  return launch_conv<s.ks, s.cinpad, GW, s.epi, s.concat, s.nblk, s.tps, 0, R, s.mw, s.ng>(
+  return launch_conv<s.ks, s.cinpad, GW, s.epi, s.concat, s.nblk, s.tps, 0, R, s.mw, s.ng, layer_wgs(LI)>(
       h, s.slot, u->stages[LI], u->bias[LI], in_base, a, stream);
 }
 template <int LI>
@@ -453,7 +462,7 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   if (o.refiner_l1) {  // the refiners' conv1 alone, bf16x3 (the sums of kL1's refiner columns)
     constexpr UmmaLayerSpec s = kSpecs[kRL1];
     act(b.r[1], 96, nullptr, 0);
-    rc = launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps, 0, false, s.mw, s.ng>(
+    rc = launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps, 0, false, s.mw, s.ng, layer_wgs(kRL1)>(
         h, s.slot, h->umma->stages[kRL1], h->umma->bias[kRL1], b.act0, a, stream);
     if (rc) return rc;
   } else {

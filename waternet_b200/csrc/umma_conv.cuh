@@ -66,7 +66,7 @@ __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.alig
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int PENDING>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
-// barrier over the 128 threads of one warpgroup (ids 1, 2; 0 is __syncthreads)
+// barrier over the 128 threads of one warpgroup (id 1 + warpgroup; 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 // four floats -> four e4m3 bytes, f0 at the lowest address
 __device__ __forceinline__ uint32_t pack_e4m3x4(float f0, float f1, float f2, float f3) {
@@ -89,13 +89,10 @@ __device__ __forceinline__ uint16_t pack_e4m3x2(float f0, float f1) {
 // kEpiDgrad (backward): no bias; zero where the saved forward activation is zero (ReLU'), -> planes.
 enum Epilogue { kEpiAct = 0, kEpiSigmoid = 1, kEpiGate = 2, kEpiDgrad = 3 };
 
-// One CTA tile = (8 * MW) x 16 pixels: warpgroup w computes pixel rows 8w..8w+7 as MW m64 blocks (block b = tile
-// columns 8b..8b+7) with m64nNk16 wgmma, accumulators in registers, and then runs the epilogue of those rows itself.
-constexpr int kTileH = 16;
-// warps 0-7: two consumer warpgroups (wgmma + epilogue); 8: A producer (TMA halo tiles); 9: B producer (weights)
-constexpr int kThreads = 320;
-constexpr int kWarpA = 8, kWarpB = 9;
-constexpr int kConsumerWarps = 8;  // arrivals per "stage empty"
+// One CTA tile = (8 * MW) x (8 * WGS) pixels: consumer warpgroup w computes pixel rows 8w..8w+7 as MW m64 blocks
+// (block b = tile columns 8b..8b+7) with m64nNk16 wgmma, accumulators in registers, and then runs the epilogue of
+// those rows itself.  Warps 0 .. 4 WGS - 1 are the consumers; warp 4 WGS is the A producer (TMA halo tiles), warp
+// 4 WGS + 1 the B producer (weights).
 constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 channels + 4 against bank conflicts)
 
 // NPAD   output channels per diagonal block
@@ -120,14 +117,23 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 // NG     column groups: a CTA computes the NPAD output channels [g * NPAD, (g + 1) * NPAD) of column group g; the
 //        layer has NG * NPAD channels and each group's weight stages are packed contiguously.  Splitting the columns
 //        keeps MW = 2 within the registers of a wide layer, at the price of reading each halo tile once per group.
+// WGS    consumer warpgroups: 2 = 16-row tiles, 320 threads (warps 0-7 consumers, 8-9 producers); 3 = 24-row tiles,
+//        512 threads (warps 0-11 consumers, 12-13 producers, 14-15 only complete the producer warpgroup).  A third
+//        warpgroup serves every weight stage to 192 pixels instead of 128 without more accumulators per thread; at
+//        512 threads the register file allows 128 per thread, so the producer warpgroup gives its registers up
+//        (setmaxnreg) and the consumers run at kWgs3ConsumerRegs.
 constexpr int kFmtIn8 = 1, kFmtOut8 = 2;
+constexpr int kWgs3ProducerRegs = 24, kWgs3ConsumerRegs = 160;  // 128 x 24 + 384 x 160 <= 65,536
 template <int KS, int CIN_PAD, int NPAD, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0, int MW = 1,
-          int NG = 1>
+          int NG = 1, int WGS = 2>
 struct UmmaCfg {
   static constexpr bool F8IN = (FMT & kFmtIn8) != 0;
   static constexpr bool DUAL = CONCAT != 0;  // two accumulator halves per block: [a x w_hi | a_hi x w_lo]
-  static constexpr int TILE_W = 8 * MW;
-  static constexpr int HALO_W = TILE_W + KS - 1, HALO_H = kTileH + KS - 1;
+  static constexpr int TILE_W = 8 * MW, TILE_H = 8 * WGS;
+  static constexpr int CONSUMER_WARPS = 4 * WGS;                  // arrivals per "stage empty"
+  static constexpr int WARP_A = CONSUMER_WARPS, WARP_B = CONSUMER_WARPS + 1;
+  static constexpr int THREADS = WGS == 2 ? 320 : 512;
+  static constexpr int HALO_W = TILE_W + KS - 1, HALO_H = TILE_H + KS - 1;
   static constexpr int NCHUNK = CIN_PAD / 16;
   static constexpr int PLANE_BYTES = HALO_W * HALO_H * 16;
   static constexpr int A_STAGE = (4 * PLANE_BYTES + 1023) / 1024 * 1024;  // hi k0, hi k1, lo k0, lo k1
@@ -137,7 +143,7 @@ struct UmmaCfg {
   static constexpr int B_STAGE = TPS * B_TAP;
   static_assert((KS * KS) % TPS == 0, "taps per weight stage must divide the filter");
   static constexpr int NSTAGE_PER_CHUNK = KS * KS / TPS;
-  static constexpr int STAGING = 2 * 64 * kStageLd * 4;
+  static constexpr int STAGING = WGS * 64 * kStageLd * 4;
   // barriers (512 B) + the biases of every column group: 2048 B, more for layers over 384 channels (VGG's 512)
   static constexpr int BIAS_BYTES = NG * NBLK * NPAD * 4;
   static constexpr int TAIL = 512 + (BIAS_BYTES > 1536 ? BIAS_BYTES : 1536);
@@ -161,6 +167,7 @@ struct UmmaCfg {
   static_assert(NCHUNK % NBLK == 0, "chunks must split evenly over the diagonal blocks");
   static_assert(NPAD % 16 == 0 && (DUAL ? 2 : 1) * NPAD <= 256, "invalid wgmma N");
   static_assert(MW == 1 || MW == 2, "one or two m64 blocks per warpgroup");
+  static_assert(WGS == 2 || (WGS == 3 && MW == 1), "two consumer warpgroups, or three of one m64 block each");
   static_assert(NG == 1 || NBLK == 1, "column groups of a block-diagonal layer");
   static_assert(MW * (ACC + (F8IN ? ACC8 : 0)) <= 128, "accumulators do not fit in registers");
   // full weight image of one column group: every (chunk, stage)
@@ -370,10 +377,10 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
 // RAG: a pass of a ragged batch (ConvArgs::rwin).  Work item t is pixel tile t / NG, column group t % NG, so the
 // groups of one pixel tile run on neighbouring CTAs at the same time and share its halo loads in L2.
 template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT, int NBLK, int TPS, int FMT = 0, bool RAG = false,
-          int MW = 1, int NG = 1>
-__global__ void __launch_bounds__(kThreads, 1)
+          int MW = 1, int NG = 1, int WGS = 2>
+__global__ void __launch_bounds__(WGS == 2 ? 320 : 512, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) {
-  using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT, MW, NG>;
+  using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT, MW, NG, WGS>;
   constexpr bool F8IN = C::F8IN, DUAL = C::DUAL, OUT8 = (FMT & kFmtOut8) != 0;
   static_assert(!OUT8 || EPI == kEpiAct, "fp8 planes are written by the activation epilogue only");
   static_assert(!RAG || EPI == kEpiAct || EPI == kEpiGate, "ragged passes mask activations and store the gate");
@@ -394,14 +401,21 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int num_tiles = g.tiles_x * g.tiles_y * g.N * NG;
   if (tid == 0) {
-    for (int i = 0; i < C::NA; i++) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], kConsumerWarps); }
-    for (int i = 0; i < C::NB; i++) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], kConsumerWarps); }
+    for (int i = 0; i < C::NA; i++) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], C::CONSUMER_WARPS); }
+    for (int i = 0; i < C::NB; i++) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], C::CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  for (int i = tid; i < NG * NBLK * NPAD; i += kThreads) s_bias[i] = g.bias[i];
+  for (int i = tid; i < NG * NBLK * NPAD; i += C::THREADS) s_bias[i] = g.bias[i];
   __syncthreads();
-
-  if (warp == kWarpA) {
+  // WGS = 3: the producer warpgroup gives registers up, the consumer warpgroups take them; each setmaxnreg sits at
+  // one place that dominates the code of its role, so that ptxas compiles the consumers for kWgs3ConsumerRegs
+  if constexpr (WGS == 3) {
+    if (warp >= C::CONSUMER_WARPS) {
+      asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kWgs3ProducerRegs));
+      if (warp > C::WARP_B) return;  // warps 14-15 only complete the producer warpgroup
+    }
+  }
+  if (warp == C::WARP_A) {
     // ===================== A producer: halo tiles by TMA =====================
     if (lane == 0) {
       int stage = 0;
@@ -411,7 +425,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
         const int n = pt / (g.tiles_x * g.tiles_y);
         const int rem = pt - n * g.tiles_x * g.tiles_y;
         const int ty = rem / g.tiles_x, tx = rem - ty * g.tiles_x;
-        const int x0 = tx * C::TILE_W - KS / 2, y0 = ty * kTileH - KS / 2;
+        const int x0 = tx * C::TILE_W - KS / 2, y0 = ty * C::TILE_H - KS / 2;
         for (int c = 0; c < C::NCHUNK; c++) {
           mbar_wait(&a_empty[stage], phase ^ 1);
           uint8_t* dst = a_stages + stage * C::A_STAGE;
@@ -425,7 +439,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     }
     return;
   }
-  if (warp == kWarpB) {
+  if (warp == C::WARP_B) {
     // ===================== B producer: packed weight stages =====================
     if (lane == 0) {
       int stage = 0;
@@ -442,11 +456,13 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     }
     return;
   }
+  if constexpr (WGS == 3) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kWgs3ConsumerRegs));
 
   // ===================== consumers: wgmma, then the epilogue of the warpgroup's 64 rows =====================
   const int wg = warp >> 2, wtid = tid & 127;
   const bool skip_lo = (g.skip_lo != nullptr && *g.skip_lo != 0) || g.a_hi_only;
-  const float dscale = F8IN ? *g.f8_scale : 1.f;
+  // WGS = 3 reads the fp8 dequantisation factor in the epilogue: one register less across the main loop
+  const float dscale0 = F8IN && WGS == 2 ? *g.f8_scale : 1.f;
   // A operand: rows of the tile = pixels, 8 consecutive pixels of a halo row = one core matrix; this warpgroup's
   // rows start 8 halo rows further, its second m64 block 8 pixels (128 B) further along the same halo rows.  K halves
   // (channels 0-7 / 8-15 of the chunk) are one plane apart.
@@ -538,7 +554,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     const int frow = (warp & 3) * 16 + (lane >> 2), fcol = (lane & 3) * 2;
     const int r = wtid & 63, half = wtid >> 6;
     const int m = wg * 64 + r;
-    const int gy = ty * kTileH + (m >> 3);
+    const int gy = ty * C::TILE_H + (m >> 3);
+    const float dscale = F8IN && WGS == 3 ? *g.f8_scale : dscale0;
     constexpr int NCH = NBLK * NPAD;
 #pragma unroll
     for (int mb = 0; mb < MW; mb++) {
@@ -741,10 +758,10 @@ static int make_tmap(CUtensorMap* tm, void* base, int planes_total, int N, int H
 
 // Launch one convolution.  `slot` is the timing slot (common.cuh).  One persistent CTA per SM (shared-memory footprint).
 template <int KS, int CIN_PAD, int NPAD, int EPI, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0,
-          bool RAG = false, int MW = 1, int NG = 1>
+          bool RAG = false, int MW = 1, int NG = 1, int WGS = 2>
 static int launch_conv(wn_handle* h, int slot, const uint8_t* wpk, const float* bias, void* in_base, ConvArgs a,
                        cudaStream_t stream) {
-  using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT, MW, NG>;
+  using C = UmmaCfg<KS, CIN_PAD, NPAD, CONCAT, NBLK, TPS, FMT, MW, NG, WGS>;
   int rc = get_encoder();
   if (rc) return rc;
   CUtensorMap tm;
@@ -754,13 +771,13 @@ static int launch_conv(wn_handle* h, int slot, const uint8_t* wpk, const float* 
   a.bias = bias;
   a.in_planes_half = CIN_PAD / 8;
   a.tiles_x = (a.W + C::TILE_W - 1) / C::TILE_W;
-  a.tiles_y = (a.H + kTileH - 1) / kTileH;
+  a.tiles_y = (a.H + C::TILE_H - 1) / C::TILE_H;
   const long long tiles = (long long)a.tiles_x * a.tiles_y * a.N * NG;
-  auto kern = conv_umma_kernel<KS, CIN_PAD, NPAD, EPI, CONCAT, NBLK, TPS, FMT, RAG, MW, NG>;
+  auto kern = conv_umma_kernel<KS, CIN_PAD, NPAD, EPI, CONCAT, NBLK, TPS, FMT, RAG, MW, NG, WGS>;
   WN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
   TimedScope ts(h, slot, stream);
   const int grid = (int)(tiles < h->sm_count ? tiles : h->sm_count);
-  kern<<<grid, kThreads, C::SMEM_BYTES, stream>>>(tm, a);
+  kern<<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(tm, a);
   WN_LAUNCH_CHECK(h);
   return WN_OK;
 }
