@@ -240,7 +240,6 @@ int wn_resize_u8(wn_handle* h, const uint8_t* const* src_dev, const int* src_h, 
   return resize_u8(h, src_dev, src_h, src_w, n, dst_nhwc, dst_h, dst_w, swap_rb, (cudaStream_t)stream);
 }
 
-static size_t align256(size_t v) { return (v + 255) / 256 * 256; }
 
 // fp32 CUDA-core mode: the API tensors are materialised (preprocess -> 4 fp32 tensors -> forward -> fp32 -> ten2arr)
 static size_t enhance_simt_workspace_bytes(int n, int h, int w) {

@@ -12,6 +12,9 @@ namespace wn {
 
 void set_error(const char* fmt, ...);
 
+// workspace sub-buffers start at 256-byte boundaries
+inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
+
 #define WN_CUDA(call)                                                                   \
   do {                                                                                  \
     cudaError_t err__ = (call);                                                         \
@@ -249,25 +252,29 @@ int umma_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images, int n, i
                            int scheme);
 int umma_f8_overflowed(const wn_handle* h);
 
-// conv_umma.cu: the two packing steps of the tiled forward, shared with the windowed backward.  The exact-levels
-// flag over every input pixel of the n images (*flag is set to 1, then cleared unless all are 8-bit levels), and the
-// act0 planes of `count` windows (win0, win0 + 1, ...) of `tiles`, read at image coordinates.
-int pack_exact_flag(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], int* flag, int n,
-                    int height, int width, const TileGeom& tiles, cudaStream_t stream);
-int pack_input_windows(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], uint4* act0, int height,
-                       int width, const TileGeom& tiles, long long win0, int count, cudaStream_t stream);
-
-// The ragged forms of the two packing steps (wn_forward_ragged, wn_forward_train_ragged).  imgs: one entry per image
-// (its four inputs and element strides), device table; wins: the `count` windows of one pass, device table, window k
-// in slot k at the slot's top-left.  With act0 NULL the call only clears *flag unless every input pixel of the
-// windows' valid extents is an 8-bit level; otherwise it writes the pass's act0 planes, zeros beyond each valid
-// extent, and leaves the flag alone.
+// conv_umma.cu: the operand packing of fp32 inputs, shared with the training forward and the windowed backward.  The
+// four inputs of an image and their element strides; a grid geometry reads image n of one set at offset n * s[t][0].
 struct PackInArgs {
   const float* p[4];
   long long s[4][4];
 };
-int pack_input_ragged(wn_handle* h, const PackInArgs* imgs, const RaggedWindow* wins, int count, int slot_h,
-                      int slot_w, uint4* act0, int* flag, cudaStream_t stream);
+inline PackInArgs pack_args(const float* const in[4], const int64_t st[4][4]) {
+  PackInArgs pa;
+  for (int t = 0; t < 4; t++) {
+    pa.p[t] = in[t];
+    for (int k = 0; k < 4; k++) pa.s[t][k] = st[t][k];
+  }
+  return pa;
+}
+// `count` slots of geo, read at image coordinates: the slots' act0 planes when act0 is given (zeros beyond each valid
+// extent), and the exact-levels flag when flag is given (cleared unless every input pixel of the valid extents is an
+// 8-bit level).  The grid form reads one set of (N,3,H,W) tensors and sets the flag to 1 before it packs.  The table
+// form reads one PackInArgs per image, a device table; its flag spans several launches, so the caller sets it to 1
+// once, and with act0 given the table form leaves the flag alone.
+int pack_inputs(wn_handle* h, const GridGeom& geo, const PackInArgs& in, int count, uint4* act0, int* flag,
+                cudaStream_t stream);
+int pack_inputs(wn_handle* h, const TableGeom& geo, const PackInArgs* imgs, int count, uint4* act0, int* flag,
+                cudaStream_t stream);
 // wn_forward_ragged (arguments checked by the caller, api.cu): the windows and passes of ragged_plan
 size_t umma_forward_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
                                            long long max_pass_pixels);

@@ -298,9 +298,9 @@ __global__ void scatter_weights_T_kernel(const float* __restrict__ src, float* _
 
 // ---- where a slot pixel of a backward pass sits in its image ------------------------------------------------------
 // A backward pass runs a batch of slots, each holding one window (or one whole image) at its top-left.  The per-pixel
-// kernels below (the seed, the input-gradient copy and the fold) are written once against one question: where does
-// pixel pix of slot s sit in its image?  Two geometries answer it: GridSlots (the windows of one tile_geom, or whole
-// images) and TableSlots (a device table of RaggedWindows).
+// kernels below (the seed, the input-gradient copy and the fold) are written once against the slot geometry of
+// tiling.cuh (GridGeom, TableGeom: where does pixel pix of slot s sit in its image?), each paired here with the
+// images' d(out) and input-gradient tensors.  Only the kept pixels are seeded from d(out).
 //
 // Per image: d(loss)/d(out) and the four input-gradient tensors (any may be null), fp32 contiguous (1,3,H,W).
 struct RaggedGrads {
@@ -309,90 +309,27 @@ struct RaggedGrads {
 };
 
 // d_out(p): the image's d(out) or d(maps), 3 planes; d_in(p, t): its input gradient t, 3 planes (NULL: not wanted)
-struct SlotPixel {
-  int img;          // the image
-  int y, x;         // image coordinates
-  bool valid;       // inside the slot's valid extent (slot pixels beyond it hold no image pixel)
-  bool kept;        // valid and inside the window's kept rectangle: the only pixels seeded from d(out)
-  size_t ihw, o;    // the image's plane size, and y * W + x
-  TileGeom tiles;   // the windows it is cut into (the fold)
-  long long k0;     // its tile k is window k0 + k of the pass's numbering
-};
-
-// Grid slots: slot s is window w0 + s of `tiles` (tile_window); d(out) and the input gradients are contiguous
-// (N,3,H,W) tensors.  An untiled call is the case tile = image size and w0 = 0: slot s is image s, kept everywhere.
-struct GridSlots {
-  TileGeom tiles;
-  long long w0;
+// Grid slots: d(out) and the input gradients are contiguous (N,3,H,W) tensors.
+struct GridSlots : GridGeom {
   const float* g_out;
   float* in[4];
-  __device__ int slot_width() const { return tiles.win_w; }
-  __device__ int slot_hw() const { return tiles.win_h * tiles.win_w; }
   __device__ void check_plan() const {}
   __device__ const float* d_out(const SlotPixel& p) const { return g_out + (size_t)p.img * 3 * p.ihw; }
   __device__ float* d_in(const SlotPixel& p, int t) const {
     return in[t] ? in[t] + (size_t)p.img * 3 * p.ihw : nullptr;
   }
-  __device__ void origin(long long k, int* ys, int* xs) const {
-    const TileWindow t = tile_window(tiles, k);
-    *ys = t.ys;
-    *xs = t.xs;
-  }
-  __device__ SlotPixel at(int s, int pix) const {
-    const TileWindow t = tile_window(tiles, w0 + s);
-    const int wy = pix / tiles.win_w;
-    SlotPixel p;
-    p.y = t.ys + wy;
-    p.x = t.xs + (pix - wy * tiles.win_w);
-    p.valid = true;
-    p.kept = p.y >= t.ky0 && p.y < t.ky1 && p.x >= t.kx0 && p.x < t.kx1;
-    p.img = t.img;
-    p.ihw = (size_t)tiles.H * tiles.W;
-    p.o = (size_t)p.y * tiles.W + p.x;
-    p.tiles = tiles;
-    p.k0 = (long long)t.img * tiles.ny * tiles.nx;
-    return p;
-  }
 };
 
-// Table slots: slot s is window wins[w0 + s] of a ragged plan, at the top-left of a slot_h x slot_w slot; each image
-// is cut into the windows of tile_geom(H, W, tile_h, tile_w), contiguous in the plan in ascending tile order (checked
-// on the host), so tile k of the image of plan window w is plan window w - wins[w].tile + k.
-struct TableSlots {
-  const RaggedWindow* wins;
+// Table slots: per image, one RaggedGrads entry of a device table.
+struct TableSlots : TableGeom {
   const RaggedGrads* imgs;
-  long long w0;
-  int slot_h, slot_w;
-  int tile_h, tile_w;
   const int* plan;  // wn_backward_ragged: n, slot_h, slot_w as the forward call wrote them; NULL otherwise
-  __device__ int slot_width() const { return slot_w; }
-  __device__ int slot_hw() const { return slot_h * slot_w; }
   // a backward with sizes other than the forward's stops instead of reading the wrong activations
   __device__ void check_plan() const {
     assert(!plan || (plan[0] == (int)gridDim.y && plan[1] == slot_h && plan[2] == slot_w));
   }
   __device__ const float* d_out(const SlotPixel& p) const { return imgs[p.img].g_out; }
   __device__ float* d_in(const SlotPixel& p, int t) const { return imgs[p.img].in[t]; }
-  __device__ void origin(long long k, int* ys, int* xs) const {
-    *ys = wins[k].ys;
-    *xs = wins[k].xs;
-  }
-  __device__ SlotPixel at(int s, int pix) const {
-    const long long me = w0 + s;
-    const RaggedWindow& r = wins[me];
-    const int wy = pix / slot_w, wx = pix - wy * slot_w;
-    SlotPixel p;
-    p.y = r.ys + wy;
-    p.x = r.xs + wx;
-    p.valid = wy < r.vh && wx < r.vw;
-    p.kept = p.valid && p.y >= r.ky0 && p.y < r.ky1 && p.x >= r.kx0 && p.x < r.kx1;
-    p.img = r.img;
-    p.ihw = (size_t)r.H * r.W;
-    p.o = (size_t)p.y * r.W + p.x;
-    p.tiles = tile_geom(r.H, r.W, tile_h, tile_w);
-    p.k0 = me - r.tile;
-    return p;
-  }
 };
 
 // The seed of a backward pass, from go = d(out) at kept pixels and 0 everywhere else (so every window
@@ -996,9 +933,9 @@ static int untiled_buffers(TrainBuffers* t, int stack, int n, int H, int W, void
   return WN_OK;
 }
 
-// The slots of an untiled call: slot s is image s, whole; g: d(out) or d(maps); in: NULL or n_in input gradients
-static GridSlots whole_images(int H, int W, const float* g, float* const* in, int n_in) {
-  GridSlots s = {tile_geom(H, W, H, W), 0, g, {nullptr, nullptr, nullptr, nullptr}};
+// The slots of geo; g: d(out) or d(maps); in: NULL or n_in input gradients
+static GridSlots grid_slots(const GridGeom& geo, const float* g, float* const* in, int n_in) {
+  GridSlots s = {geo, g, {nullptr, nullptr, nullptr, nullptr}};
   for (int i = 0; in && i < n_in; i++) s.in[i] = in[i];
   return s;
 }
@@ -1020,7 +957,7 @@ static int untiled_backward(wn_handle* h, int stack, int which, const float* gra
   TrainBuffers t;
   if ((rc = untiled_buffers(&t, stack, n, H, W, workspace, workspace_bytes))) return rc;
   const int n_in = stack == kStackRefiners ? 2 : 4;
-  return backward_pass(h, whole_images(H, W, grad, input_grads, n_in), stack, which, t, grads,
+  return backward_pass(h, grid_slots(whole_images(H, W), grad, input_grads, n_in), stack, which, t, grads,
                        any_of4(input_grads, n_in), false, n, H, W, stream);
 }
 
@@ -1043,10 +980,9 @@ static void ragged_slot(const int* hs, const int* ws, int n, int* sh, int* sw) {
     *sw = ws[i] > *sw ? ws[i] : *sw;
   }
 }
-static size_t align256b(size_t v) { return (v + 255) / 256 * 256; }
 static size_t ragged_train_table_bytes(int n) {
-  return align256b((size_t)n * sizeof(RaggedWindow)) + align256b((size_t)n * sizeof(PackInArgs)) +
-         align256b((size_t)n * sizeof(RaggedGrads));
+  return align256((size_t)n * sizeof(RaggedWindow)) + align256((size_t)n * sizeof(PackInArgs)) +
+         align256((size_t)n * sizeof(RaggedGrads));
 }
 
 size_t train_ragged_workspace_bytes(const int* hs, const int* ws, int n) {
@@ -1065,10 +1001,7 @@ static bool ragged_table(const wn_ragged_tensors* images, const float* const* gr
     if (imgs) {
       const wn_ragged_tensors& d = images[i];
       const float* p[4] = {d.x, d.wb, d.he, d.gc};
-      for (int t = 0; t < 4; t++) {
-        imgs[i].p[t] = p[t];
-        for (int k = 0; k < 4; k++) imgs[i].s[t][k] = d.in_strides[t][k];
-      }
+      imgs[i] = pack_args(p, d.in_strides);
     }
     if (grads) {
       grads[i].g_out = grad_out[i];
@@ -1091,15 +1024,15 @@ struct RaggedTrainLayout {
 };
 static RaggedTrainLayout ragged_train_layout(void* workspace, int n, int sh, int sw) {
   RaggedTrainLayout l;
-  uint8_t* p = (uint8_t*)align256b((uintptr_t)workspace);
+  uint8_t* p = (uint8_t*)align256((uintptr_t)workspace);
   l.plan = (int*)p;
   p += 256;
   l.wins = (RaggedWindow*)p;
-  p += align256b((size_t)n * sizeof(RaggedWindow));
+  p += align256((size_t)n * sizeof(RaggedWindow));
   l.imgs = (PackInArgs*)p;
-  p += align256b((size_t)n * sizeof(PackInArgs));
+  p += align256((size_t)n * sizeof(PackInArgs));
   l.grads = (RaggedGrads*)p;
-  p += align256b((size_t)n * sizeof(RaggedGrads));
+  p += align256((size_t)n * sizeof(RaggedGrads));
   carve(&l.t, p, (size_t)n * sh * sw);
   return l;
 }
@@ -1120,7 +1053,7 @@ int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, v
   ragged_slot(hs.data(), ws.data(), n, &sh, &sw);
   RaggedTrainLayout l = ragged_train_layout(workspace, n, sh, sw);
   // host copy of the plan, the windows and the PackInArgs, contiguous as in the workspace
-  const size_t win_b = align256b((size_t)n * sizeof(RaggedWindow));
+  const size_t win_b = align256((size_t)n * sizeof(RaggedWindow));
   std::vector<uint8_t> host(256 + win_b + (size_t)n * sizeof(PackInArgs));
   const int plan[3] = {n, sh, sw};
   memcpy(host.data(), plan, sizeof(plan));
@@ -1138,8 +1071,9 @@ int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, v
   WN_CUDA(cudaMemcpyAsync(l.plan, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
   int rc;
   WN_CUDA(cudaMemsetAsync(l.t.f.exact_flag, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
-  if ((rc = pack_input_ragged(h, l.imgs, l.wins, n, sh, sw, nullptr, l.t.f.exact_flag, stream))) return rc;
-  if ((rc = pack_input_ragged(h, l.imgs, l.wins, n, sh, sw, l.t.f.act0, l.t.f.exact_flag, stream))) return rc;
+  const TableGeom geo = {l.wins, 0, sh, sw, sh, sw};  // every image is one window of its own size
+  if ((rc = pack_inputs(h, geo, l.imgs, n, nullptr, l.t.f.exact_flag, stream))) return rc;
+  if ((rc = pack_inputs(h, geo, l.imgs, n, l.t.f.act0, nullptr, stream))) return rc;
   FwdOpts o;
   o.packed = true;
   o.rwin = l.wins;
@@ -1165,7 +1099,7 @@ int backward_ragged(wn_handle* h, const int* hs, const int* ws, const float* con
   const bool want_in = ragged_table(nullptr, grad_out, input_grads, n, nullptr, host.data());
   WN_CUDA(cudaMemcpyAsync(l.grads, host.data(), (size_t)n * sizeof(RaggedGrads), cudaMemcpyHostToDevice, stream));
   // every image is one window of its own size
-  const TableSlots geo = {l.wins, l.grads, 0, sh, sw, sh, sw, l.plan};
+  const TableSlots geo = {{l.wins, 0, sh, sw, sh, sw}, l.grads, l.plan};
   return backward_pass(h, geo, kStackAll, -1, l.t, grads, want_in, false, n, sh, sw, stream);
 }
 
@@ -1266,8 +1200,8 @@ int debug_backward_layer(wn_handle* h, int stack, int which, int buffer, const f
   BwdStop stop;
   stop.buffer = buffer;
   stop.dst = dst;
-  rc = backward_pass(h, whole_images(H, W, grad_out, nullptr, 0), stack, which, t, grads, true, false, n, H, W,
-                     stream, stop);
+  rc = backward_pass(h, grid_slots(whole_images(H, W), grad_out, nullptr, 0), stack, which, t, grads, true, false, n,
+                     H, W, stream, stop);
   return rc == kBwdStopped ? WN_OK : rc;
 }
 
@@ -1303,7 +1237,7 @@ static size_t param_grads_bytes(int stack) {
   param_grad_sizes(size);
   stack_params(stack, 0, &first, &count);  // the three refiners have the same shapes
   size_t b = 0;
-  for (int k = first; k < first + count; k++) b += align256b((size_t)size[k] * sizeof(float));
+  for (int k = first; k < first + count; k++) b += align256((size_t)size[k] * sizeof(float));
   return b;
 }
 
@@ -1324,36 +1258,22 @@ static uint8_t* scratch_grads(ScratchGrads* s, uint8_t* p, float* const* grads, 
     s->dst.p[k] = grads[first + k];
     s->part.p[k] = s->later[first + k] = (float*)p;
     s->dst.size[k] = s->part.size[k] = size[first + k];
-    p += align256b((size_t)size[first + k] * sizeof(float));
+    p += align256((size_t)size[first + k] * sizeof(float));
   }
   return p;
 }
 
-// Each pass's act0 planes (and, for a ragged pass, its window table for the masked forward)
-static int pack_pass(wn_handle* h, GridSlots* geo, const float* const in[4], const int64_t st[4][4],
-                     const PackInArgs*, const RaggedPass& q, uint4* act0, int*, FwdOpts*, cudaStream_t stream) {
-  geo->w0 = q.first;
-  return pack_input_windows(h, in, st, act0, geo->tiles.H, geo->tiles.W, geo->tiles, q.first, q.count, stream);
-}
-static int pack_pass(wn_handle* h, TableSlots* geo, const float* const*, const int64_t (*)[4],
-                     const PackInArgs* imgs, const RaggedPass& q, uint4* act0, int* exact, FwdOpts* o,
-                     cudaStream_t stream) {
-  geo->w0 = q.first;
-  geo->slot_h = q.slot_h;
-  geo->slot_w = q.slot_w;
-  o->rwin = geo->wins + q.first;
-  return pack_input_ragged(h, imgs, geo->wins + q.first, q.count, q.slot_h, q.slot_w, act0, exact, stream);
-}
-
 // The pass loop: per pass, the bf16x3 training forward of the stack (a refiner's first layer is kRL1, as in
-// refine_train; the backward needs cm and refined, not the output), then backward_pass with the fold.  in / st: the
-// four images of a grid call; imgs: the per-image table of a ragged one.  *exact already holds the exact-levels flag
-// of the forward that produced the output (the first layer drops its a_lo pass exactly when that forward did).
-template <class Geom>
+// refine_train; the backward needs cm and refined, not the output), then backward_pass with the fold.  in: the
+// four images of a grid call, or the per-image table of a ragged one (pack_inputs).  *exact already holds the
+// exact-levels flag of the forward that produced the output (the first layer drops its a_lo pass exactly when that
+// forward did).
+template <class Geom, class In>
 static int recompute_passes(wn_handle* h, Geom geo, const std::vector<RaggedPass>& passes, int stack, int which,
-                            const float* const in[4], const int64_t st[4][4], const PackInArgs* imgs, int* exact,
-                            ScratchGrads& s, float* const* grads, bool want_in, void* pass_ws, size_t pass_bytes,
-                            cudaStream_t stream) {
+                            const In& in, int* exact, ScratchGrads& s, float* const* grads, bool want_in,
+                            void* pass_ws, size_t pass_bytes, cudaStream_t stream) {
+  const int64_t none[4][4] = {};
+  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
   for (size_t pi = 0; pi < passes.size(); pi++) {
     const RaggedPass& q = passes[pi];
     int rc = stack == kStackAll ? check_train_args(q.count, q.slot_h, q.slot_w, pass_bytes)
@@ -1366,8 +1286,10 @@ static int recompute_passes(wn_handle* h, Geom geo, const std::vector<RaggedPass
     o.packed = true;
     o.stack = stack;
     o.refiner_l1 = stack == kStackRefiners;
-    if ((rc = pack_pass(h, &geo, in, st, imgs, q, t.f.act0, exact, &o, stream))) return rc;
-    if ((rc = umma_forward_layers(h, in, st, nullptr, q.count, q.slot_h, q.slot_w, t.f, stream, o))) return rc;
+    geo.set_pass(q);
+    o.rwin = geo.rwin();
+    if ((rc = pack_inputs(h, geo, in, q.count, t.f.act0, nullptr, stream))) return rc;
+    if ((rc = umma_forward_layers(h, no_in, none, nullptr, q.count, q.slot_h, q.slot_w, t.f, stream, o))) return rc;
     if ((rc = backward_pass(h, geo, stack, which, t, pi == 0 ? grads : s.later, want_in, true, q.count, q.slot_h,
                             q.slot_w, stream)))
       return rc;
@@ -1399,10 +1321,10 @@ static int grid_recompute_backward(wn_handle* h, int stack, int which, const flo
                                    cudaStream_t stream) {
   int rc = get_encoder();
   if (rc) return rc;
-  GridSlots geo = whole_images(H, W, grad, input_grads, stack == kStackRefiners ? 2 : 4);
-  geo.tiles = tile_geom(H, W, tile_h, tile_w);
+  const GridSlots geo =
+      grid_slots({tile_geom(H, W, tile_h, tile_w), 0}, grad, input_grads, stack == kStackRefiners ? 2 : 4);
   const TileGeom& g = geo.tiles;
-  uint8_t* base = (uint8_t*)align256b((uintptr_t)workspace);
+  uint8_t* base = (uint8_t*)align256((uintptr_t)workspace);
   int* exact = (int*)base;
   ScratchGrads s;
   uint8_t* pass_ws = scratch_grads(&s, base + 256, grads, stack, which);
@@ -1413,13 +1335,13 @@ static int grid_recompute_backward(wn_handle* h, int stack, int which, const flo
       want_in = true;
       WN_CUDA(cudaMemsetAsync(geo.in[i], 0, (size_t)n * 3 * H * W * sizeof(float), stream));
     }
-  if ((rc = pack_exact_flag(h, in, st, exact, n, H, W, g, stream))) return rc;
+  const PackInArgs pa = pack_args(in, st);
+  if ((rc = pack_inputs(h, whole_images(H, W), pa, n, nullptr, exact, stream))) return rc;
   std::vector<RaggedPass> passes;
   const long long total = (long long)n * g.ny * g.nx, per_pass = tiled_train_pass(g, n, max_pass_pixels);
   for (long long w0 = 0; w0 < total; w0 += per_pass)
     passes.push_back({w0, (int)std::min(per_pass, total - w0), g.win_h, g.win_w});
-  return recompute_passes(h, geo, passes, stack, which, in, st, nullptr, exact, s, grads, want_in, pass_ws,
-                          pass_bytes, stream);
+  return recompute_passes(h, geo, passes, stack, which, pa, exact, s, grads, want_in, pass_ws, pass_bytes, stream);
 }
 
 int backward_tiled(wn_handle* h, const float* const in[4], const int64_t st[4][4], const float* grad_out,
@@ -1465,8 +1387,8 @@ int submodule_backward_tiled(wn_handle* h, int stack, int which, const float* co
 // PackInArgs and one RaggedGrads per image, then the windows in plan order) sits between the scratch parameter
 // gradients and the pass buffers and is copied from pageable host memory once per call.
 static size_t ragged_tiled_table_bytes(int n, size_t windows) {
-  return align256b((size_t)n * sizeof(PackInArgs)) + align256b((size_t)n * sizeof(RaggedGrads)) +
-         align256b(windows * sizeof(RaggedWindow));
+  return align256((size_t)n * sizeof(PackInArgs)) + align256((size_t)n * sizeof(RaggedGrads)) +
+         align256(windows * sizeof(RaggedWindow));
 }
 
 static void ragged_tiled_plan(const int* hs, const int* ws, int n, int tile_h, int tile_w, long long max_pass_pixels,
@@ -1476,10 +1398,8 @@ static void ragged_tiled_plan(const int* hs, const int* ws, int n, int tile_h, i
 
 static size_t ragged_tiled_workspace(int n, const std::vector<RaggedWindow>& wins,
                                      const std::vector<RaggedPass>& passes) {
-  long long px = 0;
-  for (const RaggedPass& p : passes) px = std::max(px, (long long)p.count * p.slot_h * p.slot_w);
   return 256 + param_grads_bytes(kStackAll) + ragged_tiled_table_bytes(n, wins.size()) +
-         train_workspace_bytes_padded(1, 1, (int)px) + 256;
+         train_workspace_bytes_padded(1, 1, (int)largest_pass_pixels(passes)) + 256;
 }
 
 size_t backward_ragged_tiled_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
@@ -1519,12 +1439,12 @@ int backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images, const f
     }
   }
   if ((rc = get_encoder())) return rc;
-  uint8_t* base = (uint8_t*)align256b((uintptr_t)workspace);
+  uint8_t* base = (uint8_t*)align256((uintptr_t)workspace);
   int* exact = (int*)base;
   ScratchGrads s;
   uint8_t* table = scratch_grads(&s, base + 256, grads, kStackAll, -1);
   // the table, built on the host in its device layout
-  const size_t in_b = align256b((size_t)n * sizeof(PackInArgs)), g_b = align256b((size_t)n * sizeof(RaggedGrads));
+  const size_t in_b = align256((size_t)n * sizeof(PackInArgs)), g_b = align256((size_t)n * sizeof(RaggedGrads));
   std::vector<uint8_t> host(in_b + g_b + wins.size() * sizeof(RaggedWindow));
   RaggedGrads* rg = reinterpret_cast<RaggedGrads*>(host.data() + in_b);
   const bool want_in =
@@ -1537,19 +1457,18 @@ int backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images, const f
   // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
   WN_CUDA(cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
   const PackInArgs* d_imgs = reinterpret_cast<const PackInArgs*>(table);
-  const TableSlots geo = {reinterpret_cast<const RaggedWindow*>(table + in_b + g_b),
-                          reinterpret_cast<const RaggedGrads*>(table + in_b), 0, 0, 0, tile_h, tile_w, nullptr};
+  TableSlots geo = {{reinterpret_cast<const RaggedWindow*>(table + in_b + g_b), 0, 0, 0, tile_h, tile_w},
+                    reinterpret_cast<const RaggedGrads*>(table + in_b), nullptr};
   uint8_t* pass_ws = table + ragged_tiled_table_bytes(n, wins.size());
   const size_t pass_bytes = workspace_bytes - (size_t)(pass_ws - (uint8_t*)workspace);
   // the exact-levels flag over every pass, as wn_forward_ragged takes it
   WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
-  for (const RaggedPass& q : passes)
-    if ((rc = pack_input_ragged(h, d_imgs, geo.wins + q.first, q.count, q.slot_h, q.slot_w, nullptr, exact, stream)))
-      return rc;
-  const int64_t none[4][4] = {};
-  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
-  return recompute_passes(h, geo, passes, kStackAll, -1, no_in, none, d_imgs, exact, s, grads, want_in, pass_ws,
-                          pass_bytes, stream);
+  for (const RaggedPass& q : passes) {
+    geo.set_pass(q);
+    if ((rc = pack_inputs(h, geo, d_imgs, q.count, nullptr, exact, stream))) return rc;
+  }
+  return recompute_passes(h, geo, passes, kStackAll, -1, d_imgs, exact, s, grads, want_in, pass_ws, pass_bytes,
+                          stream);
 }
 
 }  // namespace wn

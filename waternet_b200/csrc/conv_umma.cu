@@ -60,77 +60,74 @@ __device__ __forceinline__ void store_packed(uint4* o, int hw, float* v) {
   o[2 * (size_t)hw] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
   o[3 * (size_t)hw] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
 }
-// FORM kPackImages: pixel blockIdx.x * 256 + tid of image blockIdx.y -> act0 planes, and the flag.
-// kPackWindows (tiled forward): pixel of window win0 + blockIdx.y of `tiles`, read at image coordinates -> that
-// window's act0 planes (blockIdx.y of the pass); the flag is not touched.
-// kPackFlag: the flag alone, over every pixel of every image (same grid as kPackImages), nothing is written.
-enum PackForm { kPackImages = 0, kPackWindows = 1, kPackFlag = 2 };
-template <int FORM = kPackImages>
-__global__ void __launch_bounds__(256) pack_inputs_kernel(PackInArgs a, uint4* __restrict__ out, int H, int W,
-                                                          int* __restrict__ exact_flag, TileGeom tiles, long long win0) {
-  const int pix = blockIdx.x * 256 + threadIdx.x;
-  const int hw = FORM == kPackWindows ? tiles.win_h * tiles.win_w : H * W;
-  bool exact = true;
-  if (pix < hw) {
-    int n = blockIdx.y, y, x;
-    if constexpr (FORM == kPackWindows) {
-      const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
-      const int wy = pix / tiles.win_w;
-      n = t.img;
-      y = t.ys + wy;
-      x = t.xs + (pix - wy * tiles.win_w);
-    } else {
-      y = pix / W;
-      x = pix - y * W;
-    }
-    float v[16];
-    exact = pack_pixel(a, n, y, x, v);
-    if constexpr (FORM != kPackFlag) store_packed(out + (size_t)blockIdx.y * 4 * hw + pix, hw, v);
-  }
-  if constexpr (FORM != kPackWindows)
-    if (!__syncthreads_and(exact) && threadIdx.x == 0) atomicExch(exact_flag, 0);
+// The operands of one slot pixel: a grid geometry reads image p.img of one set of four tensors, a table geometry the
+// tensors of image p.img (one PackInArgs per image, read through its strides with 64-bit offsets)
+__device__ __forceinline__ bool pack_slot_pixel(const PackInArgs& a, const SlotPixel& p, float* v) {
+  return pack_pixel(a, p.img, p.y, p.x, v);
+}
+__device__ __forceinline__ bool pack_slot_pixel(const PackInArgs* __restrict__ imgs, const SlotPixel& p, float* v) {
+  return pack_pixel(imgs[p.img], 0, p.y, p.x, v);
 }
 
-// The ragged form (pack_input_ragged): slot pixel blockIdx.x * 256 + tid of slot blockIdx.y, which holds window
-// wins[blockIdx.y] at its top-left.  Inside the window's valid extent the pixel is read at image coordinates through
-// its image's strides (64-bit offsets) with the arithmetic above; beyond it the planes are zeros.  FLAG: only the
-// exact-levels flag, over the valid extents, nothing is written.
-template <bool FLAG>
+// Slot pixel blockIdx.x * 256 + tid of slot blockIdx.y of geo (tiling.cuh), read at image coordinates.  PLANES: the
+// slot's act0 planes (zeros beyond the valid extent).  FLAG: *exact_flag is cleared unless every valid pixel is an
+// 8-bit level.  Whole images (GridGeom tile = image size) take both in one launch; the windowed calls take the flag
+// once per call over whole images (or over every pass of a ragged plan) and then the planes per pass.
+template <class Geom, class In, bool PLANES, bool FLAG>
 __global__ void __launch_bounds__(256)
-pack_inputs_ragged_kernel(const PackInArgs* __restrict__ imgs, const RaggedWindow* __restrict__ wins,
-                          uint4* __restrict__ out, int slot_h, int slot_w, int* __restrict__ exact_flag) {
+pack_inputs_kernel(Geom geo, In in, uint4* __restrict__ out, int* __restrict__ exact_flag) {
   const int pix = blockIdx.x * 256 + threadIdx.x;
-  const int hw = slot_h * slot_w;
+  const int hw = geo.slot_hw();
   bool exact = true;
   if (pix < hw) {
-    const RaggedWindow& r = wins[blockIdx.y];
-    const int wy = pix / slot_w, wx = pix - wy * slot_w;
+    const SlotPixel p = geo.at(blockIdx.y, pix);
     float v[16];
 #pragma unroll
     for (int j = 0; j < 12; j++) v[j] = 0.f;
-    if (wy < r.vh && wx < r.vw) exact = pack_pixel(imgs[r.img], 0, r.ys + wy, r.xs + wx, v);
-    if constexpr (!FLAG) store_packed(out + (size_t)blockIdx.y * 4 * hw + pix, hw, v);
+    if (p.valid) exact = pack_slot_pixel(in, p, v);
+    if constexpr (PLANES) store_packed(out + (size_t)blockIdx.y * 4 * hw + pix, hw, v);
   }
   if constexpr (FLAG)
     if (!__syncthreads_and(exact) && threadIdx.x == 0) atomicExch(exact_flag, 0);
 }
 
-// Sub-modules of the tiled forward: window blockIdx.y of the pass (window win0 + blockIdx.y of `tiles`) holds `cs`
-// fp32 planes of win_h x win_w; channels [c0, c0 + c) of its kept rectangle are stored into dst, contiguous NCHW
-// (N, c, H, W), at image coordinates.
+// reset: *flag is set to 1 ("all inputs are 8-bit levels") first, inside the packing's timing slot
+template <bool PLANES, bool FLAG, class Geom, class In>
+static int launch_pack(wn_handle* h, const Geom& geo, const In& in, int count, uint4* act0, int* flag, bool reset,
+                       cudaStream_t stream) {
+  TimedScope ts(h, kSlotPack, stream);
+  if (reset) WN_CUDA(cudaMemsetAsync(flag, 1, sizeof(int), stream));
+  const dim3 grid((unsigned)(((size_t)geo.slot_hw() + 255) / 256), count);
+  pack_inputs_kernel<Geom, In, PLANES, FLAG><<<grid, 256, 0, stream>>>(geo, in, act0, flag);
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+int pack_inputs(wn_handle* h, const GridGeom& geo, const PackInArgs& in, int count, uint4* act0, int* flag,
+                cudaStream_t stream) {
+  if (!act0) return launch_pack<false, true>(h, geo, in, count, nullptr, flag, true, stream);
+  if (flag) return launch_pack<true, true>(h, geo, in, count, act0, flag, true, stream);
+  return launch_pack<true, false>(h, geo, in, count, act0, nullptr, false, stream);
+}
+// a ragged call takes its flag over every pass before the first, so it never asks for both in one launch, and the
+// caller sets the flag once before the first of those launches
+int pack_inputs(wn_handle* h, const TableGeom& geo, const PackInArgs* imgs, int count, uint4* act0, int* flag,
+                cudaStream_t stream) {
+  if (!act0) return launch_pack<false, true>(h, geo, imgs, count, nullptr, flag, false, stream);
+  return launch_pack<true, false>(h, geo, imgs, count, act0, nullptr, false, stream);
+}
+
+// Sub-modules of the tiled forward: slot blockIdx.y of geo holds `cs` fp32 planes; channels [c0, c0 + c) of its kept
+// rectangle are stored into dst, contiguous NCHW (N, c, H, W), at image coordinates.
 __global__ void __launch_bounds__(256) store_kept_kernel(const float* __restrict__ src, int cs, int c0, int c,
-                                                         float* __restrict__ dst, TileGeom tiles, long long win0) {
+                                                         float* __restrict__ dst, GridGeom geo) {
   const int pix = blockIdx.x * 256 + threadIdx.x;
-  const int hw = tiles.win_h * tiles.win_w;
+  const int hw = geo.slot_hw();
   if (pix >= hw) return;
-  const TileWindow t = tile_window(tiles, win0 + blockIdx.y);
-  const int wy = pix / tiles.win_w;
-  const int y = t.ys + wy, x = t.xs + (pix - wy * tiles.win_w);
-  if (y < t.ky0 || y >= t.ky1 || x < t.kx0 || x >= t.kx1) return;
-  const size_t ihw = (size_t)tiles.H * tiles.W;
+  const SlotPixel p = geo.at(blockIdx.y, pix);
+  if (!p.kept) return;
   const float* s = src + ((size_t)blockIdx.y * cs + c0) * hw + pix;
-  float* d = dst + (size_t)t.img * c * ihw + (size_t)y * tiles.W + x;
-  for (int k = 0; k < c; k++) d[k * ihw] = s[(size_t)k * hw];
+  float* d = dst + (size_t)p.img * c * p.ihw + p.o;
+  for (int k = 0; k < c; k++) d[k * p.ihw] = s[(size_t)k * hw];
 }
 
 // ------------------------------------------------------------------------------------------
@@ -394,15 +391,6 @@ int decode_planes(wn_handle* h, const uint4* src, float* dst, int planes_half, i
   return WN_OK;
 }
 
-static PackInArgs pack_args(const float* const in[4], const int64_t st[4][4]) {
-  PackInArgs pa;
-  for (int t = 0; t < 4; t++) {
-    pa.p[t] = in[t];
-    for (int k = 0; k < 4; k++) pa.s[t][k] = st[t][k];
-  }
-  return pa;
-}
-
 // Where every layer's output lives.  Inference ping-pongs two buffers per stack; the training
 // forward (conv_bwd.cu) gives every activation its own buffer because the backward pass needs them.
 int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out, int n, int H,
@@ -410,12 +398,8 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   const int dbg_layer = o.dbg_layer;
   float* const dbg_dst = o.dbg_dst;
   if (!o.packed) {
-    const PackInArgs pa = pack_args(in, st);
-    TimedScope ts(h, kSlotPack, stream);
-    WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
-    pack_inputs_kernel<kPackImages><<<dim3((H * W + 255) / 256, n), 256, 0, stream>>>(pa, b.act0, H, W, b.exact_flag,
-                                                                                       TileGeom(), 0);
-    WN_LAUNCH_CHECK(h);
+    const int rc = pack_inputs(h, whole_images(H, W), pack_args(in, st), n, b.act0, b.exact_flag, stream);
+    if (rc) return rc;
   }
   ConvArgs a;
   memset(&a, 0, sizeof(a));
@@ -530,7 +514,7 @@ static FwdBuffers carve(void* workspace, int n, int H, int W) {
   refAB[0] = (uint4*)ws;   ws += px * 384;
   refAB[1] = (uint4*)ws;   ws += px * 384;
   b.cm = (float*)ws;       ws += px * 12;
-  b.exact_flag = (int*)(((uintptr_t)ws + 255) / 256 * 256);
+  b.exact_flag = (int*)align256((uintptr_t)ws);
   for (int l = 1; l <= 7; l++) b.a[l] = cmgAB[(l - 1) & 1];
   b.r[1] = refAB[0];
   b.r[2] = refAB[1];
@@ -617,7 +601,7 @@ int umma_forward(wn_handle* h, const float* const in[4], const int64_t in_stride
 // planes only), the last launch's epilogue writes uint8 NHWC (hubconf.py:8-34, SURVEY 8f.2).
 size_t umma_enhance_workspace_bytes(int n, int h, int w) {
   const int nb = umma_chunk(0, n, h, w);
-  return umma_forward_workspace_bytes(n, h, w) + (preprocess_workspace_bytes(nb, h, w) + 255) / 256 * 256 + 1024;
+  return umma_forward_workspace_bytes(n, h, w) + align256(preprocess_workspace_bytes(nb, h, w)) + 1024;
 }
 
 int umma_enhance_u8(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* out_f32, int n, int H, int W,
@@ -634,8 +618,8 @@ int umma_enhance_u8(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* ou
   if (rc) return rc;
   scheme = effective_scheme(h, scheme);
   const int nb = umma_chunk(h->chunk_pixels, n, H, W);
-  uint8_t* pre_ws = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
-  const size_t pre_b = (preprocess_workspace_bytes(nb, H, W) + 255) / 256 * 256;
+  uint8_t* pre_ws = (uint8_t*)align256((uintptr_t)workspace);
+  const size_t pre_b = align256(preprocess_workspace_bytes(nb, H, W));
   void* fwd_ws = pre_ws + pre_b;
   const int64_t none[4][4] = {};
   const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -668,7 +652,7 @@ size_t umma_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int t
   if ((size_t)h * w > (size_t)0x7fffffff / 3 || n > 65535) return 0;
   const TileGeom g = tile_geom(h, w, tile_h, tile_w);
   const long long p = tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels);
-  return (size_t)p * g.win_h * g.win_w * kUmmaBytesPerPixel + 4096 + (preprocess_workspace_bytes(n, h, w) + 255) / 256 * 256 +
+  return (size_t)p * g.win_h * g.win_w * kUmmaBytesPerPixel + 4096 + align256(preprocess_workspace_bytes(n, h, w)) +
          1024;
 }
 
@@ -690,8 +674,8 @@ int umma_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, flo
   const TileGeom g = tile_geom(H, W, tile_h, tile_w);
   const long long total = (long long)n * g.ny * g.nx;
   const long long per_pass = tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels);
-  uint8_t* pre_ws = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
-  const size_t pre_b = (preprocess_workspace_bytes(n, H, W) + 255) / 256 * 256;
+  uint8_t* pre_ws = (uint8_t*)align256((uintptr_t)workspace);
+  const size_t pre_b = align256(preprocess_workspace_bytes(n, H, W));
   void* fwd_ws = pre_ws + pre_b;
   if ((rc = preprocess_u8_luts(h, rgb, n, H, W, pre_ws, pre_b, stream))) return rc;
   const int64_t none[4][4] = {};
@@ -720,7 +704,6 @@ int umma_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, flo
 // valid extent is masked and its kept rectangle stored into its own image.  The plan (per-image geometry and one
 // descriptor per window) is copied into the workspace once per call, so the call cannot be captured in a graph.
 // Workspace: the largest pass plus the per-image LUTs plus the table, independent of the image sizes.
-static size_t align256(size_t v) { return (v + 255) / 256 * 256; }
 static size_t ragged_table_bytes(int n, size_t windows) {
   return align256(align256((size_t)n * sizeof(RaggedImage)) + windows * sizeof(RaggedWindow));
 }
@@ -728,13 +711,8 @@ static long long ragged_pass_pixels(long long max_pass_pixels) {
   return max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels;
 }
 static size_t ragged_workspace(int n, const std::vector<RaggedWindow>& wins, const std::vector<RaggedPass>& passes) {
-  long long px = 0;
-  for (const RaggedPass& p : passes) {
-    const long long v = (long long)p.count * p.slot_h * p.slot_w;
-    px = v > px ? v : px;
-  }
-  return (size_t)px * kUmmaBytesPerPixel + 4096 + (preprocess_workspace_bytes(n, 1, 1) + 255) / 256 * 256 +
-         ragged_table_bytes(n, wins.size()) + 1024;
+  return (size_t)largest_pass_pixels(passes) * kUmmaBytesPerPixel + 4096 +
+         align256(preprocess_workspace_bytes(n, 1, 1)) + ragged_table_bytes(n, wins.size()) + 1024;
 }
 
 size_t umma_enhance_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
@@ -769,8 +747,8 @@ int umma_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images, int n, i
   if (rc) return rc;
   scheme = effective_scheme(h, scheme);
   // workspace: [LUTs of the n images][table: n RaggedImage | windows][one pass]
-  uint8_t* pre_ws = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
-  const size_t pre_b = (preprocess_workspace_bytes(n, 1, 1) + 255) / 256 * 256;
+  uint8_t* pre_ws = (uint8_t*)align256((uintptr_t)workspace);
+  const size_t pre_b = align256(preprocess_workspace_bytes(n, 1, 1));
   uint8_t* table = pre_ws + pre_b;
   const size_t img_b = align256((size_t)n * sizeof(RaggedImage));
   void* fwd_ws = table + ragged_table_bytes(n, wins.size());
@@ -814,33 +792,13 @@ int umma_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images, int n, i
 // The tiled form of umma_forward (fp32 tensors in): the windows of tiling.cuh, one pass of them at a time through
 // the same ten launches and range guard.  The windowed packing kernel reads each window's operands at image
 // coordinates through the caller's strides.  Whether the first layer drops its a_lo pass is decided once for the
-// whole call, over every input pixel of the n images (kPackFlag), so it takes the path wn_forward takes when that
+// whole call, over every input pixel of the n images (whole_images), so it takes the path wn_forward takes when that
 // runs the batch in one pass.  The flag sits at the start of the workspace, outside the per-pass carve-up (whose
 // layout moves with the window count), and stays valid for the bf16x3 re-run of every pass.  kStackAll: the gate
 // epilogue stores each kept rectangle into `out`.  The sub-modules keep their result (the maps, or the three refined
 // images) in window layout and store_kept_kernel copies the kept rectangle of the wanted planes into `out`.
 // Workspace: [flag | refined images of one pass (sub-modules) | one pass], independent of the image size.  Nothing
 // is copied from the host: the call can be captured in a graph.
-int pack_exact_flag(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], int* flag, int n, int H,
-                    int W, const TileGeom& tiles, cudaStream_t stream) {
-  TimedScope ts(h, kSlotPack, stream);
-  WN_CUDA(cudaMemsetAsync(flag, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
-  pack_inputs_kernel<kPackFlag><<<dim3((H * W + 255) / 256, n), 256, 0, stream>>>(pack_args(in, in_strides), nullptr,
-                                                                                  H, W, flag, tiles, 0);
-  WN_LAUNCH_CHECK(h);
-  return WN_OK;
-}
-
-int pack_input_windows(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], uint4* act0, int H,
-                       int W, const TileGeom& tiles, long long win0, int count, cudaStream_t stream) {
-  TimedScope ts(h, kSlotPack, stream);
-  const size_t win_px = (size_t)tiles.win_h * tiles.win_w;
-  pack_inputs_kernel<kPackWindows><<<dim3((unsigned)((win_px + 255) / 256), count), 256, 0, stream>>>(
-      pack_args(in, in_strides), act0, H, W, nullptr, tiles, win0);
-  WN_LAUNCH_CHECK(h);
-  return WN_OK;
-}
-
 size_t umma_forward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
                                           bool submodule) {
   const TileGeom g = tile_geom(h, w, tile_h, tile_w);
@@ -873,12 +831,14 @@ int umma_forward_tiled(wn_handle* h, const float* const in[4], const int64_t in_
   int* exact = (int*)base;
   float* refined = (float*)(base + 256);
   void* fwd_ws = base + 256 + (sub ? align256(per_pass * win_px * 9 * sizeof(float)) : 0);
-  if ((rc = pack_exact_flag(h, in, in_strides, exact, n, H, W, g, stream))) return rc;
+  const PackInArgs pa = pack_args(in, in_strides);
+  if ((rc = pack_inputs(h, whole_images(H, W), pa, n, nullptr, exact, stream))) return rc;
   for (long long w0 = 0; w0 < total; w0 += per_pass) {
     const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
+    const GridGeom geo = {g, w0};
     FwdBuffers b = carve(fwd_ws, cur, g.win_h, g.win_w);
     b.exact_flag = exact;
-    if ((rc = pack_input_windows(h, in, in_strides, b.act0, H, W, g, w0, cur, stream))) return rc;
+    if ((rc = pack_inputs(h, geo, pa, cur, b.act0, nullptr, stream))) return rc;
     FwdOpts o;
     o.scheme = scheme;
     o.packed = true;
@@ -894,27 +854,15 @@ int umma_forward_tiled(wn_handle* h, const float* const in[4], const int64_t in_
       TimedScope ts(h, kSlotGate, stream);
       const bool maps = stack == kStackCmg;
       store_kept_kernel<<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(
-          maps ? b.cm : refined, maps ? 3 : 9, maps ? 0 : 3 * which, 3, out, g, w0);
+          maps ? b.cm : refined, maps ? 3 : 9, maps ? 0 : 3 * which, 3, out, geo);
       WN_LAUNCH_CHECK(h);
     }
   }
   return mirror_overflow(h, scheme, stream);
 }
 
-int pack_input_ragged(wn_handle* h, const PackInArgs* imgs, const RaggedWindow* wins, int count, int slot_h,
-                      int slot_w, uint4* act0, int* flag, cudaStream_t stream) {
-  TimedScope ts(h, kSlotPack, stream);
-  const dim3 grid((unsigned)(((size_t)slot_h * slot_w + 255) / 256), count);
-  if (act0)
-    pack_inputs_ragged_kernel<false><<<grid, 256, 0, stream>>>(imgs, wins, act0, slot_h, slot_w, flag);
-  else
-    pack_inputs_ragged_kernel<true><<<grid, 256, 0, stream>>>(imgs, wins, nullptr, slot_h, slot_w, flag);
-  WN_LAUNCH_CHECK(h);
-  return WN_OK;
-}
-
 // The ragged form of umma_forward (fp32 tensors in, wn_forward_ragged): the windows and passes of ragged_plan, as
-// umma_enhance_u8_ragged runs them, with the operands read through each image's strides (pack_inputs_ragged_kernel)
+// umma_enhance_u8_ragged runs them, with the operands read through each image's strides (pack_inputs on the table)
 // instead of preprocessed from uint8.  The exact-levels flag is taken once over every input pixel of every image
 // before the first pass, as umma_forward_tiled takes it, and stays valid for the bf16x3 re-run of every pass.  The
 // gate epilogue stores each window's kept rectangle into its image's `out` (RaggedWindow::out_f32).  The plan (one
@@ -925,12 +873,8 @@ static size_t ragged_fp32_table_bytes(int n, size_t windows) {
 }
 static size_t ragged_fp32_workspace(int n, const std::vector<RaggedWindow>& wins,
                                     const std::vector<RaggedPass>& passes) {
-  long long px = 0;
-  for (const RaggedPass& p : passes) {
-    const long long v = (long long)p.count * p.slot_h * p.slot_w;
-    px = v > px ? v : px;
-  }
-  return (size_t)px * kUmmaBytesPerPixel + 4096 + 256 + ragged_fp32_table_bytes(n, wins.size()) + 1024;
+  return (size_t)largest_pass_pixels(passes) * kUmmaBytesPerPixel + 4096 + 256 +
+         ragged_fp32_table_bytes(n, wins.size()) + 1024;
 }
 
 size_t umma_forward_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
@@ -981,22 +925,23 @@ int umma_forward_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, in
   // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
   WN_CUDA(cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
   const PackInArgs* d_imgs = reinterpret_cast<const PackInArgs*>(table);
-  const RaggedWindow* d_wins = reinterpret_cast<const RaggedWindow*>(table + img_b);
+  TableGeom geo = {reinterpret_cast<const RaggedWindow*>(table + img_b), 0, 0, 0, tile_h, tile_w};
   WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
-  for (const RaggedPass& p : passes)
-    if ((rc = pack_input_ragged(h, d_imgs, d_wins + p.first, p.count, p.slot_h, p.slot_w, nullptr, exact, stream)))
-      return rc;
+  for (const RaggedPass& p : passes) {
+    geo.set_pass(p);
+    if ((rc = pack_inputs(h, geo, d_imgs, p.count, nullptr, exact, stream))) return rc;
+  }
   const int64_t none[4][4] = {};
   const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
   for (const RaggedPass& p : passes) {
     FwdBuffers b = carve(fwd_ws, p.count, p.slot_h, p.slot_w);
     b.exact_flag = exact;
-    if ((rc = pack_input_ragged(h, d_imgs, d_wins + p.first, p.count, p.slot_h, p.slot_w, b.act0, exact, stream)))
-      return rc;
+    geo.set_pass(p);
+    if ((rc = pack_inputs(h, geo, d_imgs, p.count, b.act0, nullptr, stream))) return rc;
     FwdOpts o;
     o.scheme = scheme;
     o.packed = true;
-    o.rwin = d_wins + p.first;
+    o.rwin = geo.rwin();
     rc = umma_pass(h, no_in, none, nullptr, p.count, p.slot_h, p.slot_w, b, stream, o);
     if (rc) return rc;
   }

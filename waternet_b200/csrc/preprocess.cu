@@ -559,15 +559,13 @@ static PreGeom geometry(int H, int W) {
   return g;
 }
 
-static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
 // workspace: [tile_hist N*64*256 u32][rgb_hist N*768 u32][clahe_lut N*64*256 u8][wb_lut N*768 u8]
 size_t preprocess_workspace_bytes(int n, int, int) {
   size_t b = 0;
-  b += align_up((size_t)n * 64 * 256 * 4, 256);
-  b += align_up((size_t)n * 768 * 4, 256);
-  b += align_up((size_t)n * 64 * 256, 256);
-  b += align_up((size_t)n * 768, 256);
+  b += align256((size_t)n * 64 * 256 * 4);
+  b += align256((size_t)n * 768 * 4);
+  b += align256((size_t)n * 64 * 256);
+  b += align256((size_t)n * 768);
   return b;
 }
 
@@ -587,7 +585,7 @@ __global__ void gray_extract_kernel(const uint8_t* __restrict__ rgb, uint8_t* __
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += (size_t)gridDim.x * blockDim.x) g[i] = rgb[3 * i];
 }
 size_t white_balance_gray_workspace_bytes(int n, int h, int w) {
-  return align_up(preprocess_workspace_bytes(n, h, w), 256) + 2 * align_up((size_t)n * h * w * 3, 256);
+  return align256(preprocess_workspace_bytes(n, h, w)) + 2 * align256((size_t)n * h * w * 3);
 }
 int white_balance_gray_u8(wn_handle* h, const uint8_t* gray, uint8_t* out, int n, int H, int W, void* workspace,
                           size_t workspace_bytes, cudaStream_t stream) {
@@ -596,7 +594,7 @@ int white_balance_gray_u8(wn_handle* h, const uint8_t* gray, uint8_t* out, int n
     return WN_E_WORKSPACE;
   }
   uint8_t* ws = (uint8_t*)workspace;
-  const size_t pre_b = align_up(preprocess_workspace_bytes(n, H, W), 256), img_b = align_up((size_t)n * H * W * 3, 256);
+  const size_t pre_b = align256(preprocess_workspace_bytes(n, H, W)), img_b = align256((size_t)n * H * W * 3);
   uint8_t* rgb = ws + pre_b;
   uint8_t* wb = rgb + img_b;
   const size_t npix = (size_t)n * H * W;
@@ -632,11 +630,11 @@ static PreBufs pre_carve(void* workspace, int n) {
   PreBufs b;
   uint8_t* ws = (uint8_t*)workspace;
   b.tile_hist = (uint32_t*)ws;
-  ws += align_up((size_t)n * 64 * 256 * 4, 256);
+  ws += align256((size_t)n * 64 * 256 * 4);
   b.rgb_hist = (uint32_t*)ws;
-  ws += align_up((size_t)n * 768 * 4, 256);
+  ws += align256((size_t)n * 768 * 4);
   b.clahe_lut = ws;
-  ws += align_up((size_t)n * 64 * 256, 256);
+  ws += align256((size_t)n * 64 * 256);
   b.wb_lut = ws;
   return b;
 }
@@ -659,7 +657,7 @@ static int preprocess_luts(wn_handle* h, const uint8_t* rgb, int n, int H, int W
                            cudaStream_t stream, int gray) {
   uint32_t* tile_hist = b.tile_hist;
   uint32_t* rgb_hist = b.rgb_hist;
-  size_t hist_bytes = align_up((size_t)n * 64 * 256 * 4, 256) + (size_t)n * 768 * 4;
+  size_t hist_bytes = align256((size_t)n * 64 * 256 * 4) + (size_t)n * 768 * 4;
   WN_CUDA(cudaMemsetAsync(tile_hist, 0, hist_bytes, stream));
   // ~4K pixels per CTA keeps the grid well above two CTAs per SM even for one 1080p image
   int slabs = (g.th * g.tw + 4095) / 4096;
@@ -767,7 +765,7 @@ RaggedImage ragged_image(const uint8_t* rgb, int H, int W) {
 int preprocess_u8_ragged_luts(wn_handle* h, int n, const RaggedImage* imgs, int max_slabs, void* workspace,
                               cudaStream_t stream) {
   const PreBufs b = pre_carve(workspace, n);
-  WN_CUDA(cudaMemsetAsync(b.tile_hist, 0, align_up((size_t)n * 64 * 256 * 4, 256) + (size_t)n * 768 * 4, stream));
+  WN_CUDA(cudaMemsetAsync(b.tile_hist, 0, align256((size_t)n * 64 * 256 * 4) + (size_t)n * 768 * 4, stream));
   {
   TimedScope ts(h, kSlotStats, stream);
   stats_kernel<true><<<dim3(64, max_slabs, n), kStatsThreads, 0, stream>>>(nullptr, 0, 0, 0, 0, 0, h->d_tables,

@@ -1,5 +1,6 @@
-// Window geometry of the tiled forward (wn_enhance_u8_tiled).  The apply kernel, the gate epilogue and the host
-// planner all call these functions: this is the only place that knows the rule.
+// Window geometry of the tiled forward (wn_enhance_u8_tiled).  The apply kernel, the gate epilogue, the per-pixel
+// kernels of a pass (slot geometry, below) and the host planner all call these functions: this is the only place
+// that knows the rule.
 //
 // Every output pixel of WaterNet depends on the input within kTileHalo pixels (the eight cmg convolutions have
 // radii 3+2+1+0+3+2+1+1; the refiners need 6, the gate is per pixel).  An image is cut into balanced output tiles
@@ -176,5 +177,99 @@ inline void ragged_plan(const int* hs, const int* ws, int n, int tile_h, int til
   }
   if (p.count > 0) passes->push_back(p);
 }
+
+// the pixels of a pass list's largest pass (its workspace is sized for that one)
+inline long long largest_pass_pixels(const std::vector<RaggedPass>& passes) {
+  long long px = 0;
+  for (const RaggedPass& p : passes) px = std::max(px, (long long)p.count * p.slot_h * p.slot_w);
+  return px;
+}
+
+// ---- slot geometry: where pixel pix of slot s of a pass sits in its image ----
+// A pass runs a batch of slots, each holding one window (or one whole image) at its top-left.  Every per-pixel kernel
+// of a pass that reads or writes image coordinates (the operand packing, the kept-rectangle store, the backward's
+// seed, input-gradient copy and fold) asks one of two geometries: GridGeom, window w0 + s of one tile_geom (an
+// untiled call is the case tile = image size and w0 = 0: slot s is image s, kept everywhere), and TableGeom, window
+// wins[w0 + s] of a ragged plan.  Each user pairs the geometry with its own per-image data.
+struct SlotPixel {
+  int img;          // the image
+  int y, x;         // image coordinates
+  bool valid;       // inside the slot's valid extent (slot pixels beyond it hold no image pixel)
+  bool kept;        // valid and inside the window's kept rectangle
+  size_t ihw, o;    // the image's plane size, and y * W + x
+  TileGeom tiles;   // the windows its image is cut into (the backward's fold)
+  long long k0;     // its image's tile k is window k0 + k of the pass's numbering
+};
+
+struct GridGeom {
+  TileGeom tiles;
+  long long w0;
+  __host__ __device__ int slot_width() const { return tiles.win_w; }
+  __host__ __device__ int slot_hw() const { return tiles.win_h * tiles.win_w; }
+  // host: the slots of pass q, and the window table of its masked forward (FwdOpts::rwin; none for a grid)
+  void set_pass(const RaggedPass& q) { w0 = q.first; }
+  const RaggedWindow* rwin() const { return nullptr; }
+  __device__ void origin(long long k, int* ys, int* xs) const {
+    const TileWindow t = tile_window(tiles, k);
+    *ys = t.ys;
+    *xs = t.xs;
+  }
+  __device__ SlotPixel at(int s, int pix) const {
+    const TileWindow t = tile_window(tiles, w0 + s);
+    const int wy = pix / tiles.win_w;
+    SlotPixel p;
+    p.y = t.ys + wy;
+    p.x = t.xs + (pix - wy * tiles.win_w);
+    p.valid = true;
+    p.kept = p.y >= t.ky0 && p.y < t.ky1 && p.x >= t.kx0 && p.x < t.kx1;
+    p.img = t.img;
+    p.ihw = (size_t)tiles.H * tiles.W;
+    p.o = (size_t)p.y * tiles.W + p.x;
+    p.tiles = tiles;
+    p.k0 = (long long)t.img * tiles.ny * tiles.nx;
+    return p;
+  }
+};
+
+// the slots of an untiled call of n images of H x W: slot s is image s, whole
+inline GridGeom whole_images(int H, int W) { return {tile_geom(H, W, H, W), 0}; }
+
+// Slot s is window wins[w0 + s] at the top-left of a slot_h x slot_w slot; each image is cut into the windows of
+// tile_geom(H, W, tile_h, tile_w), contiguous in the plan in ascending tile order (the callers of the fold check this
+// on the host), so tile k of the image of plan window w is plan window w - wins[w].tile + k.
+struct TableGeom {
+  const RaggedWindow* wins;
+  long long w0;
+  int slot_h, slot_w;
+  int tile_h, tile_w;
+  __host__ __device__ int slot_width() const { return slot_w; }
+  __host__ __device__ int slot_hw() const { return slot_h * slot_w; }
+  void set_pass(const RaggedPass& q) {
+    w0 = q.first;
+    slot_h = q.slot_h;
+    slot_w = q.slot_w;
+  }
+  const RaggedWindow* rwin() const { return wins + w0; }
+  __device__ void origin(long long k, int* ys, int* xs) const {
+    *ys = wins[k].ys;
+    *xs = wins[k].xs;
+  }
+  __device__ SlotPixel at(int s, int pix) const {
+    const long long me = w0 + s;
+    const RaggedWindow& r = wins[me];
+    const int wy = pix / slot_w, wx = pix - wy * slot_w;
+    SlotPixel p;
+    p.y = r.ys + wy;
+    p.x = r.xs + wx;
+    p.valid = wy < r.vh && wx < r.vw;
+    p.kept = p.valid && p.y >= r.ky0 && p.y < r.ky1 && p.x >= r.kx0 && p.x < r.kx1;
+    p.img = r.img;
+    p.ihw = (size_t)r.H * r.W;
+    p.o = (size_t)p.y * r.W + p.x;
+    p.tiles = tile_geom(r.H, r.W, tile_h, tile_w);
+    p.k0 = me - r.tile;
+    return p;
+  }
+};
 
 }  // namespace wn
