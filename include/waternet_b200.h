@@ -66,6 +66,8 @@ extern "C" {
 #define WN_MODE_BF16X3 1    /* wgmma tensor cores, 3-term bf16 split operands, fp32 accumulate */
 #define WN_MODE_BF16_FP8 2  /* same, the two correction terms of the tensor-bound layers as one fp8 MMA */
 #define WN_MODE_DEFAULT (-1) /* the library's fastest mode that meets the 1e-3 parity bar: WN_MODE_BF16_FP8 */
+/* Not a forward mode: the training arithmetic of wn_set_train_mode (3), one bf16 wgmma per product, fp32 accumulate */
+#define WN_MODE_BF16 (WN_MODE_BF16_FP8 + 1)
 
 #define WN_NUM_PARAMS 34
 
@@ -292,6 +294,20 @@ int wn_enhance_u8_peers(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, flo
  * (wn_train_workspace_bytes returns 0 beyond that).
  */
 size_t wn_train_workspace_bytes(int n, int h, int w);
+
+/*
+ * The arithmetic of the training calls of this handle: WN_MODE_BF16X3 (the default of a new handle: three bf16
+ * products per product, ~1e-5 of fp32) or WN_MODE_BF16 (one bf16 product, a_hi x w_hi, with fp32 accumulation: the
+ * operands rounded to bf16 once, as autocast trains convolutions).  Any other mode returns WN_E_INVALID.  A host-side
+ * setting: no device pointer, no launch.  It is read by wn_forward_train / wn_backward, wn_forward_train_ragged /
+ * wn_backward_ragged, wn_backward_tiled, wn_backward_ragged_tiled, wn_confidence_maps_train / _backward / _backward_tiled,
+ * wn_refine_train / _backward / _backward_tiled and wn_debug_backward_layer: their training forward, seeds, data
+ * gradients and weight gradients all run in it.  In WN_MODE_BF16 every stored activation and gradient plane holds
+ * bf16(v) with lo = 0; the workspace sizes do not change.  A backward must run under the mode of the forward that
+ * filled its workspace.  The inference calls ignore the setting (and reject WN_MODE_BF16 as their `mode`).
+ * WN_ABI_VERSION stays 11: an addition, no existing signature or structure changed (as with wn_backward_ragged_tiled).
+ */
+int wn_set_train_mode(wn_handle* h, int mode);
 int wn_forward_train(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
                      const int64_t in_strides[4][4], float* out, int n, int height, int width,
                      void* train_workspace, size_t workspace_bytes, void* stream);

@@ -31,6 +31,10 @@ def main():
     ap.add_argument("--seed", type=int, default=None, help="(Optional) Seed for torch, defaults to None")
     ap.add_argument("--synthetic", action="store_true", help="Use UIEB-shaped synthetic pairs (no dataset offline)")
     ap.add_argument("--precision", default="default", choices=["default", "fp32", "bf16x3", "bf16_fp8"])
+    ap.add_argument("--train-precision", default="bf16x3", choices=["bf16x3", "bf16"],
+                    help="(Optional) Arithmetic of the native training step (WaterNet.train_precision): bf16x3 "
+                         "(default, ~1e-5 of fp32) or bf16 (one bf16 tensor-core product, fp32 accumulation, as "
+                         "autocast trains convolutions)")
     ap.add_argument("--loader", default="gpu", choices=["gpu", "torch"],
                     help="gpu: batches augmented + preprocessed on the device in one call; torch: the reference's "
                          "per-item DataLoader path")
@@ -80,7 +84,7 @@ def main():
         train_loader = torch.utils.data.DataLoader(train_set, batch_size=args.batch_size)
         val_loader = torch.utils.data.DataLoader(val_set, batch_size=args.batch_size)
 
-    model = WaterNet(precision=args.precision)
+    model = WaterNet(precision=args.precision, train_precision=args.train_precision)
     model.grad_tile = args.grad_tile
     if args.weights is not None:
         model.load_state_dict(torch.load(args.weights, map_location="cpu"))
@@ -102,7 +106,8 @@ def main():
         torch.save(model.state_dict(), savedir / "last.pt")
     T.save_metrics(savedir, train_hist, val_hist, {
         "epochs": args.epochs, "batch_size": args.batch_size, "im_height": args.height, "im_width": args.width,
-        "weights": args.weights, "native_size": args.native_size})
+        "weights": args.weights, "native_size": args.native_size,
+        "train_precision": args.train_precision})
     print(f"Metrics and weights saved to {savedir}")
     print(f"Total time: {timer() - start}s")
 

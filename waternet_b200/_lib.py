@@ -17,6 +17,7 @@ MODE_FP32_SIMT = 0
 MODE_BF16X3 = 1
 MODE_BF16_FP8 = 2
 MODE_DEFAULT = -1
+MODE_BF16 = 3          # WN_MODE_BF16: single-pass bf16 training (wn_set_train_mode)
 NUM_PARAMS = 34
 VGG_NUM_PARAMS = 32     # WN_VGG_NUM_PARAMS: weight and bias of VGG19's 16 convolutions
 NUM_TIMING_SLOTS = 23
@@ -91,6 +92,7 @@ _SIGNATURES = {
                                 c_int, c_int, ctypes.c_longlong, c_int, c_void_p, c_size_t, c_void_p]),
     "wn_forward_chunk_images": (c_int, [c_void_p, c_int, c_int, c_int]),
     "wn_set_chunk_pixels": (c_int, [c_void_p, ctypes.c_longlong]),
+    "wn_set_train_mode": (c_int, [c_void_p, c_int]),
     "wn_f8_overflowed": (c_int, [c_void_p]),
     "wn_peer_alloc": (c_int, [c_size_t, POINTER(c_void_p), c_void_p]),
     "wn_peer_open": (c_int, [c_void_p, POINTER(c_void_p)]),

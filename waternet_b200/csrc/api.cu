@@ -659,6 +659,19 @@ int wn_set_chunk_pixels(wn_handle* h, long long max_pixels) {
   return WN_OK;
 }
 
+int wn_set_train_mode(wn_handle* h, int mode) {
+  if (!h) {
+    set_error("wn_set_train_mode: null handle");
+    return WN_E_INVALID;
+  }
+  if (mode != WN_MODE_BF16X3 && mode != WN_MODE_BF16) {
+    set_error("wn_set_train_mode: mode %d is not a training mode (WN_MODE_BF16X3 = 1 or WN_MODE_BF16 = 3)", mode);
+    return WN_E_INVALID;
+  }
+  h->train_bf16 = mode == WN_MODE_BF16;
+  return WN_OK;
+}
+
 int wn_forward_chunk_images(const wn_handle* h, int n, int height, int width) {
   if (!h || n <= 0 || height <= 0 || width <= 0) return 0;
   return umma_chunk_images(h, n, height, width);

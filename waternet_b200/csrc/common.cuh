@@ -97,6 +97,7 @@ struct wn_handle {
   wn::UmmaBwd* bwd;
   long long chunk_pixels;  // cap on pixels per pass of the tensor-core forward (0 = default, wn_set_chunk_pixels)
   wn::VggWeights* vgg;     // the perceptual loss's VGG19 stages (wn_vgg_pack_weights)
+  bool train_bf16;         // wn_set_train_mode(WN_MODE_BF16): the training calls run single-pass bf16 (kFmtHi)
 };
 
 namespace wn {
@@ -194,8 +195,11 @@ struct PeerOut {
   uint8_t* p[WN_MAX_PEERS];
   int n;
 };
+constexpr int kSchemeBf16 = 2;  // FwdOpts::scheme of the WN_MODE_BF16 training forward (UmmaCfg kFmtHi)
+// the scheme of a training forward: the handle's training arithmetic (wn_set_train_mode)
+inline int train_scheme(const wn_handle* h) { return h->train_bf16 ? kSchemeBf16 : 0; }
 struct FwdOpts {
-  int scheme = 0;              // 1 = fp8 correction passes (WN_MODE_BF16_FP8)
+  int scheme = 0;              // 1 = fp8 correction passes (WN_MODE_BF16_FP8); kSchemeBf16 = one bf16 pass (training)
   int dbg_layer = -1;          // wn_debug_forward_layer: stop after this layer and decode it into dbg_dst
   float* dbg_dst = nullptr;
   bool packed = false;         // act0 already holds the 16-channel operand planes of this batch
@@ -270,11 +274,12 @@ inline PackInArgs pack_args(const float* const in[4], const int64_t st[4][4]) {
 // extent), and the exact-levels flag when flag is given (cleared unless every input pixel of the valid extents is an
 // 8-bit level).  The grid form reads one set of (N,3,H,W) tensors and sets the flag to 1 before it packs.  The table
 // form reads one PackInArgs per image, a device table; its flag spans several launches, so the caller sets it to 1
-// once, and with act0 given the table form leaves the flag alone.
+// once, and with act0 given the table form leaves the flag alone.  hi: the act0 planes of the single-pass bf16
+// training forward (kSchemeBf16), lo planes stored as 0.
 int pack_inputs(wn_handle* h, const GridGeom& geo, const PackInArgs& in, int count, uint4* act0, int* flag,
-                cudaStream_t stream);
+                cudaStream_t stream, bool hi = false);
 int pack_inputs(wn_handle* h, const TableGeom& geo, const PackInArgs* imgs, int count, uint4* act0, int* flag,
-                cudaStream_t stream);
+                cudaStream_t stream, bool hi = false);
 // wn_forward_ragged (arguments checked by the caller, api.cu): the windows and passes of ragged_plan
 size_t umma_forward_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
                                            long long max_pass_pixels);

@@ -13,7 +13,9 @@
 //                        them in a fixed order (bit-reproducible gradients, no atomics).
 //   bias_grad_kernel     db[co] = sum_px g[px][co]
 //
-// All three GEMM-shaped pieces use the same bf16x3 split as the forward (gradient error ~1e-5).
+// All three GEMM-shaped pieces use the same bf16x3 split as the forward (gradient error ~1e-5), or, when the handle
+// trains in WN_MODE_BF16 (wn_set_train_mode), one bf16 product each: the kFmtHi data gradient, the HI weight gradient
+// (g_hi x a_hi) and seeds whose lo planes are 0.
 #include <assert.h>
 
 #include "umma_conv.cuh"
@@ -61,7 +63,8 @@ struct WgradArgs {
 
 constexpr int kWgradThreads = 288;  // warps 0-7: two consumer warpgroups (64 output channels each), 8: TMA producer
 
-template <int KS, int NCI, int TPG>
+// HI: single-pass bf16 (WN_MODE_BF16): only the hi halves are loaded and only g_hi x a_hi is issued
+template <int KS, int NCI, int TPG, bool HI = false>
 __global__ void __launch_bounds__(kWgradThreads, 1)
 wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_a,
                   const WgradArgs g) {
@@ -105,11 +108,11 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_const
         uint8_t* g_tile = smem + st * C::STAGE;
         uint8_t* a_tile = g_tile + C::G_BYTES;
         mbar_wait(&empty[st], phase ^ 1);
-        mbar_expect_tx(&full[st], (uint32_t)(2 * g.co_planes * C::G_PLANE + 2 * C::A_HALF));
+        mbar_expect_tx(&full[st], (uint32_t)((HI ? 1 : 2) * g.co_planes * C::G_PLANE + (HI ? 1 : 2) * C::A_HALF));
         tma_load_5d(g_tile, &tmap_g, &full[st], 0, x0, y0, 0, n);
-        tma_load_5d(g_tile + C::G_HALF, &tmap_g, &full[st], 0, x0, y0, g.planes_half, n);
+        if constexpr (!HI) tma_load_5d(g_tile + C::G_HALF, &tmap_g, &full[st], 0, x0, y0, g.planes_half, n);
         tma_load_5d(a_tile, &tmap_a, &full[st], 0, x0 - KS / 2, y0 - KS / 2, 0, n);
-        tma_load_5d(a_tile + C::A_HALF, &tmap_a, &full[st], 0, x0 - KS / 2, y0 - KS / 2, C::A_PLANES, n);
+        if constexpr (!HI) tma_load_5d(a_tile + C::A_HALF, &tmap_a, &full[st], 0, x0 - KS / 2, y0 - KS / 2, C::A_PLANES, n);
         if (++st == C::NSTAGE) { st = 0; phase ^= 1; }
       }
     }
@@ -141,8 +144,10 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_const
         const uint64_t gh = make_desc(g_row, 128, C::G_PLANE), gl = make_desc(g_row + C::G_HALF, 128, C::G_PLANE);
         const uint64_t ah = make_desc(a_row, 128, C::A_PLANE), al = make_desc(a_row + C::A_HALF, 128, C::A_PLANE);
         wgmma_bf16_mn<NCI>(d, gh, ah);  // g_hi x a_hi
-        wgmma_bf16_mn<NCI>(d, gl, ah);  // g_lo x a_hi
-        wgmma_bf16_mn<NCI>(d, gh, al);  // g_hi x a_lo
+        if constexpr (!HI) {
+          wgmma_bf16_mn<NCI>(d, gl, ah);  // g_lo x a_hi
+          wgmma_bf16_mn<NCI>(d, gh, al);  // g_hi x a_lo
+        }
       }
     }
     wg_commit();
@@ -244,12 +249,20 @@ __global__ void extract_wgrad_kernel(const float* __restrict__ dense, float* __r
 //   g_zr3[3r+c] = g_out[c] * cm[r]            where refined[3r+c] > 0
 //   g_z8[r]     = (sum_c g_out[c] * refined[3r+c]) * cm[r] * (1 - cm[r])
 // Both are written as 16-channel gradient planes (bf16 hi/lo), unused channels zero.
-// 16 gradient values of pixel pix of image n -> a 16-channel gradient buffer (planes hi0, hi1, lo0, lo1)
+// 16 gradient values of pixel pix of image n -> a 16-channel gradient buffer (planes hi0, hi1, lo0, lo1); HI: the
+// single-pass bf16 seed, bf16(v) and lo = 0
+template <bool HI>
 __device__ __forceinline__ void store_grad16(uint4* base, const float* v, int n, int pix, int hw) {
   uint32_t hi[8], lo[8];
 #pragma unroll
   for (int j = 0; j < 16; j += 2) {
-    split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
+    if constexpr (HI) {
+      const __nv_bfloat162 hb = __floats2bfloat162_rn(v[j], v[j + 1]);
+      hi[j >> 1] = *reinterpret_cast<const uint32_t*>(&hb);
+      lo[j >> 1] = 0u;
+    } else {
+      split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
+    }
   }
   uint4* o = base + (size_t)n * 4 * hw + pix;
   o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
@@ -259,6 +272,7 @@ __device__ __forceinline__ void store_grad16(uint4* base, const float* v, int n,
 }
 
 // go: d(loss)/d(out) at pixel pix of image n of the batch
+template <bool HI>
 __device__ __forceinline__ void gate_bwd_pixel(const float* go, const float* __restrict__ cm,
                                                const float* __restrict__ refined, uint4* __restrict__ g8,
                                                uint4* __restrict__ gr3, int n, int pix, int hw) {
@@ -278,8 +292,8 @@ __device__ __forceinline__ void gate_bwd_pixel(const float* go, const float* __r
     }
     v8[r] = dot * c[r] * (1.0f - c[r]);
   }
-  store_grad16(g8, v8, n, pix, hw);
-  store_grad16(gr3, v9, n, pix, hw);
+  store_grad16<HI>(g8, v8, n, pix, hw);
+  store_grad16<HI>(gr3, v9, n, pix, hw);
 }
 
 // data-gradient weights: dense_d[row_off + c][col(o)][kk-1-t] = W[o][c][t]   (transpose + spatial flip)
@@ -338,7 +352,8 @@ struct TableSlots : TableGeom {
 //   kStackCmg       maps = sigmoid(z_8):  g_z8[r] = d(map_r) * cm_r * (1 - cm_r) -> g8
 //   kStackRefiners  refiner `which` alone, out = relu(z_r3) of its three columns:  g_zr3[3 which + c] = d(out_c)
 //                   where refined[3 which + c] > 0; the other refiners' six columns are exactly 0 -> gr3
-template <class Geom>
+// HI: the planes of the single-pass bf16 backward (lo = 0)
+template <class Geom, bool HI = false>
 __global__ void __launch_bounds__(256)
 seed_kernel(Geom geo, int stack, int which, const float* __restrict__ cm, const float* __restrict__ refined,
             uint4* __restrict__ g8, uint4* __restrict__ gr3) {
@@ -353,7 +368,7 @@ seed_kernel(Geom geo, int stack, int which, const float* __restrict__ cm, const 
 #pragma unroll
   for (int k = 0; k < 3; k++) go[k] = p.kept ? g[k * p.ihw + p.o] : 0.f;
   if (stack == kStackAll) {
-    gate_bwd_pixel(go, cm, refined, g8, gr3, s, pix, hw);
+    gate_bwd_pixel<HI>(go, cm, refined, g8, gr3, s, pix, hw);
     return;
   }
   float v[16];
@@ -377,7 +392,7 @@ seed_kernel(Geom geo, int stack, int which, const float* __restrict__ cm, const 
 #pragma unroll
       for (int c = 0; c < 3; c++) v[3 * r + c] = r == which ? gz[c] : 0.f;
   }
-  store_grad16(stack == kStackCmg ? g8 : gr3, v, s, pix, hw);
+  store_grad16<HI>(stack == kStackCmg ? g8 : gr3, v, s, pix, hw);
 }
 
 // d(loss)/d(input images) from the 32-channel buffers of the first layers (12 real channels: packed input k is
@@ -678,7 +693,9 @@ int forward_train(wn_handle* h, const float* const in[4], const int64_t st[4][4]
   if (rc) return rc;
   TrainBuffers t;
   carve(&t, workspace, (size_t)n * H * W);
-  return umma_forward_layers(h, in, st, out, n, H, W, t.f, stream);
+  FwdOpts o;
+  o.scheme = train_scheme(h);
+  return umma_forward_layers(h, in, st, out, n, H, W, t.f, stream, o);
 }
 
 static int make_plane_tmap(CUtensorMap* tm, void* base, int planes_total, int N, int H, int W, int box_w, int box_h,
@@ -725,7 +742,7 @@ static int launch_wgrad(wn_handle* h, uint4* gplanes, int co_valid, uint4* aplan
   if (splits < 1) splits = 1;
   if (splits * C::NGROUPS > kPartialSlots) splits = kPartialSlots / C::NGROUPS;
   static_assert((size_t)s.tpg * 128 * s.nci * sizeof(float) <= kPartialSlotBytes, "partial-sum slot");
-  auto kern = wgrad_umma_kernel<s.ks, s.nci, s.tpg>;
+  auto kern = h->train_bf16 ? wgrad_umma_kernel<s.ks, s.nci, s.tpg, true> : wgrad_umma_kernel<s.ks, s.nci, s.tpg>;
   WN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
   kern<<<dim3(C::NGROUPS, (unsigned)splits), kWgradThreads, C::SMEM_BYTES, stream>>>(tg, ta, a);
   WN_LAUNCH_CHECK(h);
@@ -766,6 +783,9 @@ static int launch_dgrad(wn_handle* h, uint4* g_in, uint4* g_out, const uint4* sa
   a.cout = out_channels;
   a.mask_base = saved;  // nullptr: no ReLU in front (network input)
   a.mask_planes_half = out_channels / 8;
+  if (h->train_bf16)
+    return launch_conv<s.ks, s.kpad, s.npad, kEpiDgrad, s.concat, s.nblk, s.tps, kFmtHi>(
+        h, kSlotGate, h->bwd->stages[LI], h->bwd->zero_bias, g_in, a, stream);
   return launch_conv<s.ks, s.kpad, s.npad, kEpiDgrad, s.concat, s.nblk, s.tps>(h, kSlotGate, h->bwd->stages[LI],
                                                                               h->bwd->zero_bias, g_in, a, stream);
 }
@@ -893,7 +913,10 @@ static int backward_pass(wn_handle* h, const Geom& geo, int stack, int which, co
                          float* const* grads, bool want_in, bool fold, int n, int H, int W, cudaStream_t stream,
                          const BwdStop& stop = BwdStop()) {
   const dim3 grid((unsigned)(((size_t)H * W + 255) / 256), n);
-  seed_kernel<<<grid, 256, 0, stream>>>(geo, stack, which, t.f.cm, t.f.refined, t.g8, t.gr3);
+  if (h->train_bf16)
+    seed_kernel<Geom, true><<<grid, 256, 0, stream>>>(geo, stack, which, t.f.cm, t.f.refined, t.g8, t.gr3);
+  else
+    seed_kernel<<<grid, 256, 0, stream>>>(geo, stack, which, t.f.cm, t.f.refined, t.g8, t.gr3);
   WN_LAUNCH_CHECK(h);
   int rc;
   if (stop.buffer == kDebugG8 || stop.buffer == kDebugGr3) {
@@ -1073,8 +1096,9 @@ int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, v
   WN_CUDA(cudaMemsetAsync(l.t.f.exact_flag, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
   const TableGeom geo = {l.wins, 0, sh, sw, sh, sw};  // every image is one window of its own size
   if ((rc = pack_inputs(h, geo, l.imgs, n, nullptr, l.t.f.exact_flag, stream))) return rc;
-  if ((rc = pack_inputs(h, geo, l.imgs, n, l.t.f.act0, nullptr, stream))) return rc;
   FwdOpts o;
+  o.scheme = train_scheme(h);
+  if ((rc = pack_inputs(h, geo, l.imgs, n, l.t.f.act0, nullptr, stream, o.scheme == kSchemeBf16))) return rc;
   o.packed = true;
   o.rwin = l.wins;
   const int64_t none[4][4] = {};
@@ -1128,6 +1152,7 @@ int confidence_maps_train(wn_handle* h, const float* const in[4], const int64_t 
   TrainBuffers t;
   carve(&t, workspace, (size_t)n * H * W, kStackCmg);
   FwdOpts o;
+  o.scheme = train_scheme(h);
   o.stack = kStackCmg;
   if ((rc = umma_forward_layers(h, in, st, nullptr, n, H, W, t.f, stream, o))) return rc;
   WN_CUDA(cudaMemcpyAsync(out_maps, t.f.cm, (size_t)n * 3 * H * W * sizeof(float), cudaMemcpyDeviceToDevice, stream));
@@ -1147,6 +1172,7 @@ int refine_train(wn_handle* h, int which, const float* const in[4], const int64_
   TrainBuffers t;
   carve(&t, workspace, (size_t)n * H * W, kStackRefiners);
   FwdOpts o;
+  o.scheme = train_scheme(h);
   o.stack = kStackRefiners;
   o.refiner_l1 = true;
   if ((rc = umma_forward_layers(h, in, st, nullptr, n, H, W, t.f, stream, o))) return rc;
@@ -1263,7 +1289,7 @@ static uint8_t* scratch_grads(ScratchGrads* s, uint8_t* p, float* const* grads, 
   return p;
 }
 
-// The pass loop: per pass, the bf16x3 training forward of the stack (a refiner's first layer is kRL1, as in
+// The pass loop: per pass, the training forward of the stack in the handle's training arithmetic (a refiner's first layer is kRL1, as in
 // refine_train; the backward needs cm and refined, not the output), then backward_pass with the fold.  in: the
 // four images of a grid call, or the per-image table of a ragged one (pack_inputs).  *exact already holds the
 // exact-levels flag of the forward that produced the output (the first layer drops its a_lo pass exactly when that
@@ -1283,12 +1309,13 @@ static int recompute_passes(wn_handle* h, Geom geo, const std::vector<RaggedPass
     carve(&t, pass_ws, (size_t)q.count * q.slot_h * q.slot_w, stack);
     t.f.exact_flag = exact;
     FwdOpts o;
+    o.scheme = train_scheme(h);
     o.packed = true;
     o.stack = stack;
     o.refiner_l1 = stack == kStackRefiners;
     geo.set_pass(q);
     o.rwin = geo.rwin();
-    if ((rc = pack_inputs(h, geo, in, q.count, t.f.act0, nullptr, stream))) return rc;
+    if ((rc = pack_inputs(h, geo, in, q.count, t.f.act0, nullptr, stream, o.scheme == kSchemeBf16))) return rc;
     if ((rc = umma_forward_layers(h, no_in, none, nullptr, q.count, q.slot_h, q.slot_w, t.f, stream, o))) return rc;
     if ((rc = backward_pass(h, geo, stack, which, t, pi == 0 ? grads : s.later, want_in, true, q.count, q.slot_h,
                             q.slot_w, stream)))

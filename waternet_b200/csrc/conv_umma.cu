@@ -47,13 +47,20 @@ __device__ __forceinline__ bool pack_pixel(const PackInArgs& a, int n, int y, in
     }
   return exact;
 }
-// 16 channels -> the four operand planes hi0, hi1, lo0, lo1 of pixel o[0] (planes hw apart)
+// 16 channels -> the four operand planes hi0, hi1, lo0, lo1 of pixel o[0] (planes hw apart); HI: lo = 0
+template <bool HI>
 __device__ __forceinline__ void store_packed(uint4* o, int hw, float* v) {
   v[12] = v[13] = v[14] = v[15] = 0.f;
   uint32_t hi[8], lo[8];
 #pragma unroll
   for (int j = 0; j < 16; j += 2) {
-    split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
+    if constexpr (HI) {
+      const __nv_bfloat162 hb = __floats2bfloat162_rn(v[j], v[j + 1]);
+      hi[j >> 1] = *reinterpret_cast<const uint32_t*>(&hb);
+      lo[j >> 1] = 0u;
+    } else {
+      split_bf16x2(v[j], v[j + 1], hi[j >> 1], lo[j >> 1]);
+    }
   }
   o[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
   o[hw] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
@@ -72,8 +79,9 @@ __device__ __forceinline__ bool pack_slot_pixel(const PackInArgs* __restrict__ i
 // Slot pixel blockIdx.x * 256 + tid of slot blockIdx.y of geo (tiling.cuh), read at image coordinates.  PLANES: the
 // slot's act0 planes (zeros beyond the valid extent).  FLAG: *exact_flag is cleared unless every valid pixel is an
 // 8-bit level.  Whole images (GridGeom tile = image size) take both in one launch; the windowed calls take the flag
-// once per call over whole images (or over every pass of a ragged plan) and then the planes per pass.
-template <class Geom, class In, bool PLANES, bool FLAG>
+// once per call over whole images (or over every pass of a ragged plan) and then the planes per pass.  HI: the planes
+// of the single-pass bf16 training forward, lo = 0.
+template <class Geom, class In, bool PLANES, bool FLAG, bool HI = false>
 __global__ void __launch_bounds__(256)
 pack_inputs_kernel(Geom geo, In in, uint4* __restrict__ out, int* __restrict__ exact_flag) {
   const int pix = blockIdx.x * 256 + threadIdx.x;
@@ -85,7 +93,7 @@ pack_inputs_kernel(Geom geo, In in, uint4* __restrict__ out, int* __restrict__ e
 #pragma unroll
     for (int j = 0; j < 12; j++) v[j] = 0.f;
     if (p.valid) exact = pack_slot_pixel(in, p, v);
-    if constexpr (PLANES) store_packed(out + (size_t)blockIdx.y * 4 * hw + pix, hw, v);
+    if constexpr (PLANES) store_packed<HI>(out + (size_t)blockIdx.y * 4 * hw + pix, hw, v);
   }
   if constexpr (FLAG)
     if (!__syncthreads_and(exact) && threadIdx.x == 0) atomicExch(exact_flag, 0);
@@ -94,26 +102,29 @@ pack_inputs_kernel(Geom geo, In in, uint4* __restrict__ out, int* __restrict__ e
 // reset: *flag is set to 1 ("all inputs are 8-bit levels") first, inside the packing's timing slot
 template <bool PLANES, bool FLAG, class Geom, class In>
 static int launch_pack(wn_handle* h, const Geom& geo, const In& in, int count, uint4* act0, int* flag, bool reset,
-                       cudaStream_t stream) {
+                       cudaStream_t stream, bool hi = false) {
   TimedScope ts(h, kSlotPack, stream);
   if (reset) WN_CUDA(cudaMemsetAsync(flag, 1, sizeof(int), stream));
   const dim3 grid((unsigned)(((size_t)geo.slot_hw() + 255) / 256), count);
-  pack_inputs_kernel<Geom, In, PLANES, FLAG><<<grid, 256, 0, stream>>>(geo, in, act0, flag);
+  if (PLANES && hi)
+    pack_inputs_kernel<Geom, In, PLANES, FLAG, true><<<grid, 256, 0, stream>>>(geo, in, act0, flag);
+  else
+    pack_inputs_kernel<Geom, In, PLANES, FLAG><<<grid, 256, 0, stream>>>(geo, in, act0, flag);
   WN_LAUNCH_CHECK(h);
   return WN_OK;
 }
 int pack_inputs(wn_handle* h, const GridGeom& geo, const PackInArgs& in, int count, uint4* act0, int* flag,
-                cudaStream_t stream) {
+                cudaStream_t stream, bool hi) {
   if (!act0) return launch_pack<false, true>(h, geo, in, count, nullptr, flag, true, stream);
-  if (flag) return launch_pack<true, true>(h, geo, in, count, act0, flag, true, stream);
-  return launch_pack<true, false>(h, geo, in, count, act0, nullptr, false, stream);
+  if (flag) return launch_pack<true, true>(h, geo, in, count, act0, flag, true, stream, hi);
+  return launch_pack<true, false>(h, geo, in, count, act0, nullptr, false, stream, hi);
 }
 // a ragged call takes its flag over every pass before the first, so it never asks for both in one launch, and the
 // caller sets the flag once before the first of those launches
 int pack_inputs(wn_handle* h, const TableGeom& geo, const PackInArgs* imgs, int count, uint4* act0, int* flag,
-                cudaStream_t stream) {
+                cudaStream_t stream, bool hi) {
   if (!act0) return launch_pack<false, true>(h, geo, imgs, count, nullptr, flag, false, stream);
-  return launch_pack<true, false>(h, geo, imgs, count, act0, nullptr, false, stream);
+  return launch_pack<true, false>(h, geo, imgs, count, act0, nullptr, false, stream, hi);
 }
 
 // Sub-modules of the tiled forward: slot blockIdx.y of geo holds `cs` fp32 planes; channels [c0, c0 + c) of its kept
@@ -140,7 +151,7 @@ enum UmmaLayer {
   kC8,        // 64 -> 3 (pad 16), sigmoid
   kR2,        // three refiner conv2 as one block-diagonal 96 -> 96, 5x5
   kR3,        // three refiner conv3 as block-diagonal 96 -> 9 (pad 16), ReLU, gated sum
-  kRL1,       // the three refiner conv1 alone (16 -> 96, 7x7): the training forward of a refiner (bf16x3 only)
+  kRL1,       // the three refiner conv1 alone (16 -> 96, 7x7): the training forward of a refiner
   kNumUmmaLayers
 };
 // Everything a layer's launches and packed weights depend on (UmmaCfg in umma_conv.cuh).  npad = output columns
@@ -151,6 +162,9 @@ enum UmmaLayer {
 // ng channels each (UmmaCfg MW, NG): at mw = 2 the accumulators of both blocks must fit in 128 registers per thread.
 // wgs = consumer warpgroups (UmmaCfg WGS): 3 gives 8 x 24-pixel tiles, which cut the weight bytes streamed per pixel
 // by a third at mw = 1; a layer takes it where its kernels stay free of spills at 160 registers and measure faster.
+// Every layer also has a single-pass bf16 form (UmmaCfg FMT kFmtHi, the WN_MODE_BF16 training forward, kRL1 included):
+// the bf16x3 weight images, hi rows only, at the layer's own mw, ng and wgs.  It needs no more registers than the
+// bf16x3 form (a CONCAT layer's accumulators halve: N = npad instead of 2 * npad).
 struct UmmaLayerSpec {
   int ks, cinpad, npad, epi, concat, nblk, tps, slot;
   bool f8;
@@ -328,16 +342,20 @@ size_t umma_forward_workspace_bytes(int n, int h, int w) {
   return nb * h * w * kUmmaBytesPerPixel + nb * h * 64 + 4096;
 }
 
-// Launch layer LI in the fp8-correction scheme (f8) or in bf16x3.  A layer's fp8 form reads its own weight images,
-// in the [hi | fp8] layout.  A pass of a ragged batch (a.rwin) runs the RAG instantiations of the layers that mask
-// (kEpiAct) or store per window (kEpiGate); the confidence maps are per pixel and need neither.
+// Launch layer LI in `scheme` (FwdOpts): the fp8-correction scheme (1), single-pass bf16 (kSchemeBf16) or bf16x3 (0).
+// A layer's fp8 form reads its own weight images, in the [hi | fp8] layout; the single-pass form reads the hi rows of
+// the bf16x3 images.  A pass of a ragged batch (a.rwin) runs the RAG instantiations of the layers that mask (kEpiAct)
+// or store per window (kEpiGate); the confidence maps are per pixel and need neither.
 template <int LI, bool RAG>
-static int launch_layer_as(wn_handle* h, bool f8, void* in_base, ConvArgs a, cudaStream_t stream) {
+static int launch_layer_as(wn_handle* h, int scheme, void* in_base, ConvArgs a, cudaStream_t stream) {
   constexpr UmmaLayerSpec s = kSpecs[LI];
   constexpr bool R = RAG && s.epi != kEpiSigmoid;
   const UmmaWeights* u = h->umma;
   constexpr int GW = s.npad / s.ng;  // channels per column group
-  if (f8) {
+  if (scheme == kSchemeBf16)
+    return launch_conv<s.ks, s.cinpad, GW, s.epi, s.concat, s.nblk, s.tps, kFmtHi, R, s.mw, s.ng, layer_wgs(LI)>(
+        h, s.slot, u->stages[LI], u->bias[LI], in_base, a, stream);
+  if (scheme == 1) {
     constexpr int FMT = (s.f8 ? kFmtIn8 : 0) | (writes_f8(LI) ? kFmtOut8 : 0);
     if constexpr ((FMT & kFmtOut8) != 0) a.f8_overflow = u->overflow_dev;
     if constexpr (s.f8) a.f8_scale = u->scale8[LI] + 1;
@@ -348,9 +366,9 @@ static int launch_layer_as(wn_handle* h, bool f8, void* in_base, ConvArgs a, cud
       h, s.slot, u->stages[LI], u->bias[LI], in_base, a, stream);
 }
 template <int LI>
-static int launch_layer(wn_handle* h, bool f8, void* in_base, ConvArgs a, cudaStream_t stream) {
-  return a.rwin ? launch_layer_as<LI, true>(h, f8, in_base, a, stream)
-                : launch_layer_as<LI, false>(h, f8, in_base, a, stream);
+static int launch_layer(wn_handle* h, int scheme, void* in_base, ConvArgs a, cudaStream_t stream) {
+  return a.rwin ? launch_layer_as<LI, true>(h, scheme, in_base, a, stream)
+                : launch_layer_as<LI, false>(h, scheme, in_base, a, stream);
 }
 
 // bf16 hi/lo planes -> fp32 NCHW (test aid)
@@ -398,7 +416,8 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   const int dbg_layer = o.dbg_layer;
   float* const dbg_dst = o.dbg_dst;
   if (!o.packed) {
-    const int rc = pack_inputs(h, whole_images(H, W), pack_args(in, st), n, b.act0, b.exact_flag, stream);
+    const int rc = pack_inputs(h, whole_images(H, W), pack_args(in, st), n, b.act0, b.exact_flag, stream,
+                               o.scheme == kSchemeBf16);
     if (rc) return rc;
   }
   ConvArgs a;
@@ -410,6 +429,7 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   // fp8-correction scheme (inference): the tensor-bound layers replace the two bf16 correction passes by one
   // fp8 MMA (UmmaCfg FMT); a layer whose consumer is such a layer writes the hi + fp8-planes format
   const bool f8 = o.scheme == 1;
+  const int sc = o.scheme;
   // after layer li's launch: decode its output (a.dst0) when it is the one wn_debug_forward_layer asks for.  That
   // call numbers an output by its convolution in state-dict order, the layer's timing slot; L1's second output
   // (a.dst1) is the refiners' conv1, number 8.
@@ -443,48 +463,52 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   const bool want_cmg = o.stack != kStackRefiners, want_ref = o.stack != kStackCmg;
   a.skip_lo = b.exact_flag;
   a.a_hi_only = o.hi_only ? 1 : 0;
-  if (o.refiner_l1) {  // the refiners' conv1 alone, bf16x3 (the sums of kL1's refiner columns)
+  if (o.refiner_l1) {  // the refiners' conv1 alone, bf16x3 or single-pass bf16 (the sums of kL1's refiner columns)
     constexpr UmmaLayerSpec s = kSpecs[kRL1];
     act(b.r[1], 96, nullptr, 0);
-    rc = launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps, 0, false, s.mw, s.ng, layer_wgs(kRL1)>(
-        h, s.slot, h->umma->stages[kRL1], h->umma->bias[kRL1], b.act0, a, stream);
+    if (sc == kSchemeBf16)
+      rc = launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps, kFmtHi, false, s.mw, s.ng,
+                       layer_wgs(kRL1)>(h, s.slot, h->umma->stages[kRL1], h->umma->bias[kRL1], b.act0, a, stream);
+    else
+      rc = launch_conv<s.ks, s.cinpad, s.npad, s.epi, s.concat, s.nblk, s.tps, 0, false, s.mw, s.ng, layer_wgs(kRL1)>(
+          h, s.slot, h->umma->stages[kRL1], h->umma->bias[kRL1], b.act0, a, stream);
     if (rc) return rc;
   } else {
     // L1: 16 -> 128 (cmg) + 96 (refiners); the training forward of the cmg alone has no r[1] and stores 128
     act(b.a[1], 128, b.r[1], b.r[1] ? 96 : 0);
-    if ((rc = launch_layer<kL1>(h, f8, b.act0, a, stream))) return rc;
+    if ((rc = launch_layer<kL1>(h, sc, b.act0, a, stream))) return rc;
   }
   a.skip_lo = nullptr;
   a.a_hi_only = 0;
   if (dump(kL1)) return WN_OK;
   if (want_cmg) {
     act(b.a[2], 128, nullptr, 0);
-    if ((rc = launch_layer<kC2>(h, f8, b.a[1], a, stream))) return rc;
+    if ((rc = launch_layer<kC2>(h, sc, b.a[1], a, stream))) return rc;
     if (dump(kC2)) return WN_OK;
     act(b.a[3], 128, nullptr, 0);
-    if ((rc = launch_layer<kC3>(h, f8, b.a[2], a, stream))) return rc;
+    if ((rc = launch_layer<kC3>(h, sc, b.a[2], a, stream))) return rc;
     if (dump(kC3)) return WN_OK;
     act(b.a[4], 64, nullptr, 0);
-    if ((rc = launch_layer<kC4>(h, f8, b.a[3], a, stream))) return rc;
+    if ((rc = launch_layer<kC4>(h, sc, b.a[3], a, stream))) return rc;
     if (dump(kC4)) return WN_OK;
     act(b.a[5], 64, nullptr, 0);
-    if ((rc = launch_layer<kC5>(h, f8, b.a[4], a, stream))) return rc;
+    if ((rc = launch_layer<kC5>(h, sc, b.a[4], a, stream))) return rc;
     if (dump(kC5)) return WN_OK;
     act(b.a[6], 64, nullptr, 0);
-    if ((rc = launch_layer<kC6>(h, f8, b.a[5], a, stream))) return rc;
+    if ((rc = launch_layer<kC6>(h, sc, b.a[5], a, stream))) return rc;
     if (dump(kC6)) return WN_OK;
     act(b.a[7], 64, nullptr, 0);
-    if ((rc = launch_layer<kC7>(h, f8, b.a[6], a, stream))) return rc;
+    if ((rc = launch_layer<kC7>(h, sc, b.a[6], a, stream))) return rc;
     if (dump(kC7)) return WN_OK;
     // the confidence maps are fp32: a dump of them is written in place of b.cm
     const bool dump_maps = dbg_layer == kSpecs[kC8].slot;
     a.out_f32 = dump_maps ? dbg_dst : b.cm;
-    if ((rc = launch_layer<kC8>(h, f8, b.a[7], a, stream))) return rc;
+    if ((rc = launch_layer<kC8>(h, sc, b.a[7], a, stream))) return rc;
     if (dump_maps) return WN_OK;
   }
   if (!want_ref) return WN_OK;
   act(b.r[2], 96, nullptr, 0);
-  if ((rc = launch_layer<kR2>(h, f8, b.r[1], a, stream))) return rc;
+  if ((rc = launch_layer<kR2>(h, sc, b.r[1], a, stream))) return rc;
   if (dump(kR2)) return WN_OK;
   last();
   // a dump of the refined images (number 10): the same launch with no gate, storing them alone
@@ -495,7 +519,7 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
     a.cm = nullptr;
     a.refined_out = dbg_dst;
   }
-  if ((rc = launch_layer<kR3>(h, f8, b.r[2], a, stream))) return rc;
+  if ((rc = launch_layer<kR3>(h, sc, b.r[2], a, stream))) return rc;
   if (dump_refined) return WN_OK;
   return o.out_u8 ? mirror_u8(h, o.out_u8, o.peers, (size_t)n * H * W * 3, o.run_if, stream) : WN_OK;
 }

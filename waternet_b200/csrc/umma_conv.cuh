@@ -112,6 +112,10 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 //        The fp8 product accumulates in registers of its own: Hopper's fp8 wgmma adds with fewer mantissa bits
 //        than fp32, which is harmless for the small correction terms but not for the main product.
 //        bit 1 (kFmtOut8): the epilogue writes that hi + fp8-planes format (its consumer has bit 0 set).
+//        bit 2 (kFmtHi): single-pass bf16 (WN_MODE_BF16, training only): ONE wgmma per product, a_hi x w_hi of
+//        N = NPAD (a CONCAT layer takes the hi rows of its [hi | lo] stage rows), fp32 accumulation.  The a_lo and w_lo
+//        products are never issued and the halo loads fetch the two hi planes of a chunk only.  kEpiAct / kEpiDgrad
+//        store lo = 0, so every plane buffer of that mode holds exactly the bf16 operand its consumers multiply.
 // MW     m64 blocks per warpgroup: 1 = 8 x 16-pixel tile (M = 128), 2 = 16 x 16 (M = 256).  Every weight stage a
 //        CTA streams from L2 then serves twice the pixels.
 // NG     column groups: a CTA computes the NPAD output channels [g * NPAD, (g + 1) * NPAD) of column group g; the
@@ -122,13 +126,14 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 //        warpgroup serves every weight stage to 192 pixels instead of 128 without more accumulators per thread; at
 //        512 threads the register file allows 128 per thread, so the producer warpgroup gives its registers up
 //        (setmaxnreg) and the consumers run at kWgs3ConsumerRegs.
-constexpr int kFmtIn8 = 1, kFmtOut8 = 2;
+constexpr int kFmtIn8 = 1, kFmtOut8 = 2, kFmtHi = 4;
 constexpr int kWgs3ProducerRegs = 24, kWgs3ConsumerRegs = 160;  // 128 x 24 + 384 x 160 <= 65,536
 template <int KS, int CIN_PAD, int NPAD, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0, int MW = 1,
           int NG = 1, int WGS = 2>
 struct UmmaCfg {
   static constexpr bool F8IN = (FMT & kFmtIn8) != 0;
-  static constexpr bool DUAL = CONCAT != 0;  // two accumulator halves per block: [a x w_hi | a_hi x w_lo]
+  static constexpr bool HI = (FMT & kFmtHi) != 0;
+  static constexpr bool DUAL = CONCAT != 0 && !HI;  // two accumulator halves per block: [a x w_hi | a_hi x w_lo]
   static constexpr int TILE_W = 8 * MW, TILE_H = 8 * WGS;
   static constexpr int CONSUMER_WARPS = 4 * WGS;                  // arrivals per "stage empty"
   static constexpr int WARP_A = CONSUMER_WARPS, WARP_B = CONSUMER_WARPS + 1;
@@ -157,6 +162,7 @@ struct UmmaCfg {
   static constexpr int NA_FIT = (BUDGET - NB * B_STAGE) / A_STAGE;
   static constexpr int NA = NA_FIT > NA_WANT ? NA_WANT : NA_FIT;
   static_assert(!F8IN || !CONCAT, "fp8 corrections: the [hi | second part] weight layout");
+  static_assert(!HI || FMT == kFmtHi, "single-pass bf16 reads and writes bf16 planes only");
   static constexpr int CPB = NCHUNK / NBLK;                // chunks per diagonal block
   static constexpr int BLK_COLS = DUAL ? 2 * NPAD : NPAD;   // accumulator columns per block
   static constexpr int COLS = NBLK * BLK_COLS;             // accumulator columns of the tile
@@ -239,7 +245,8 @@ __device__ __forceinline__ void split_bf16x2(float f0, float f1, uint32_t& hi, u
 // Epilogue of 16 consecutive output channels [ch, ch + 16) of one pixel; f = the raw sums (scaled in the fp8 scheme).
 // RAG: `valid` is false at slot pixels outside the window's valid extent, where kEpiAct stores zeros (hi, lo and
 // fp8 planes alike; they cannot raise the e4m3 flag).
-template <int EPI, bool OUT8, bool RAG = false>
+// HI (kFmtHi): the planes hold bf16(v) and lo = 0.
+template <int EPI, bool OUT8, bool RAG = false, bool HI = false>
 __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bias, const float* f, int ch, int n,
                                            int gx, int gy, bool valid = true) {
   const size_t hw = (size_t)g.H * g.W;
@@ -309,7 +316,13 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
               f1 = valid ? f1 : 0.f;
             }
           }
-          split_bf16x2(f0, f1, hi[j >> 1], lo[j >> 1]);
+          if constexpr (HI) {
+            const __nv_bfloat162 hb = __floats2bfloat162_rn(f0, f1);
+            hi[j >> 1] = *reinterpret_cast<const uint32_t*>(&hb);
+            lo[j >> 1] = 0u;
+          } else {
+            split_bf16x2(f0, f1, hi[j >> 1], lo[j >> 1]);
+          }
         }
         const bool second = c >= g.split_c;
         const ActDst& d = second ? g.dst1 : g.dst0;
@@ -429,9 +442,10 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
         for (int c = 0; c < C::NCHUNK; c++) {
           mbar_wait(&a_empty[stage], phase ^ 1);
           uint8_t* dst = a_stages + stage * C::A_STAGE;
-          mbar_expect_tx(&a_full[stage], (g.a_hi_only ? 2 : 4) * C::PLANE_BYTES);
+          // kFmtHi never reads the lo planes
+          mbar_expect_tx(&a_full[stage], (C::HI || g.a_hi_only ? 2 : 4) * C::PLANE_BYTES);
           tma_load_5d(dst, &tmap_in, &a_full[stage], 0, x0, y0, 2 * c, n);
-          if (!g.a_hi_only)
+          if (!C::HI && !g.a_hi_only)
             tma_load_5d(dst + 2 * C::PLANE_BYTES, &tmap_in, &a_full[stage], 0, x0, y0, g.in_planes_half + 2 * c, n);
           if (++stage == C::NA) { stage = 0; phase ^= 1; }
         }
@@ -516,7 +530,9 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
             for (int b = 0; b < NBLK; b++) {
               if (NBLK > 1 && b != blk) continue;
               float* d = acc[mb] + b * C::BLK_COLS / 2;
-              if constexpr (F8IN) {
+              if constexpr (C::HI) {
+                wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));                // a_hi x w_hi
+              } else if constexpr (F8IN) {
                 // w_hi * ws * 2^9 (bf16, K = 16), then [e4m3(lo*2^9) | e4m3(v)] x [e4m3(w*ws) ; e4m3(w_lo*ws*2^9)] (K = 32)
                 wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, NPAD * 16, 128));
                 wgmma_e4m3<NPAD>(acc8[mb] + b * C::BLK_COLS / 2, a_lo, make_desc(b_tap + NPAD * 32, NPAD * 16, 128));
@@ -592,7 +608,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
             const float4 x = s[q];
             f[4 * q] = x.x; f[4 * q + 1] = x.y; f[4 * q + 2] = x.z; f[4 * q + 3] = x.w;
           }
-          epilogue16<EPI, OUT8, RAG>(g, s_bias, f, c0 + cb, n, gx, gy, valid);
+          epilogue16<EPI, OUT8, RAG, C::HI>(g, s_bias, f, c0 + cb, n, gx, gy, valid);
         }
         wg_bar(1 + wg);
       }

@@ -250,6 +250,12 @@ class Engine:
         """Lower the per-pass pixel cap (0 = default 8 Mi); tests force the multi-pass path with it."""
         _lib.check(self.lib.wn_set_chunk_pixels(self.handle, int(max_pixels)), "wn_set_chunk_pixels")
 
+    def set_train_mode(self, mode: int) -> None:
+        """The arithmetic of this handle's training calls (wn_set_train_mode): MODE_BF16X3 or MODE_BF16.  Every
+        training method below sets it from its ``train_mode`` argument first, so a backward runs under the mode its
+        caller passes (the mode of the matching forward), whatever another module did on this handle in between."""
+        _lib.check(self.lib.wn_set_train_mode(self.handle, int(mode)), "wn_set_train_mode")
+
     def f8_overflowed(self) -> bool:
         """True once the fp8-correction mode saw an activation beyond the e4m3 range.  The batch that did was
         recomputed by the bf16x3 kernels within the same call; from then on the handle uses those kernels
@@ -369,12 +375,13 @@ class Engine:
     TRAIN_MAX_PIXELS = 8 << 20
     TRAIN_MAX_IMAGES = 65535
 
-    def forward_train(self, x, wb, he, gc):
+    def forward_train(self, x, wb, he, gc, train_mode: int = _lib.MODE_BF16X3):
         """Tensor-core forward that keeps every activation.  Returns (out, saved workspaces).
 
         wn_forward_train takes at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES per call; a larger batch runs as several
         calls over slices of the batch, each with its own workspace (~5.6 KB per pixel in total, like the reference's autograd graph)."""
         ins = self._check_inputs((x, wb, he, gc))
+        self.set_train_mode(train_mode)
         n, _, h, w = ins[0].shape
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
         if out.numel() == 0:
@@ -399,10 +406,11 @@ class Engine:
             saved.append((a, b, ws))
         return out, saved
 
-    def backward(self, grad_out: torch.Tensor, saved, shapes, want_input_grads: bool = False):
+    def backward(self, grad_out: torch.Tensor, saved, shapes, want_input_grads: bool = False, train_mode: int = _lib.MODE_BF16X3):
         """d(loss)/d(out) + the workspaces of forward_train -> the 34 parameter gradients (state-dict order)
         and, on request, the gradients of the four input images.  Batch slices are processed in order and their
-        parameter gradients added in that order (deterministic)."""
+        parameter gradients added in that order (deterministic).  ``train_mode``: that of the forward."""
+        self.set_train_mode(train_mode)
         g = grad_out.detach().to(self.device, torch.float32).contiguous()
         n, _, h, w = g.shape
         saved = saved or []
@@ -430,14 +438,15 @@ class Engine:
                                 64, 64, 64, 64, 128, 128, 128, 96, 96, 32, 32)
 
     def debug_backward_layer(self, workspace: torch.Tensor, shape, buffer: int, stack: int = -1, which: int = 0,
-                             grad: Optional[torch.Tensor] = None, grads=None) -> torch.Tensor:
+                             grad: Optional[torch.Tensor] = None, grads=None, train_mode: int = _lib.MODE_BF16X3) -> torch.Tensor:
         """Test aid (wn_debug_backward_layer): buffer ``buffer`` of the training backward as fp32 (N,C,H,W).
 
         ``workspace`` is the workspace of one slice that ``forward_train`` (stack -1), ``confidence_maps_train`` (0)
         or ``refine_train(which)`` (1) has just filled, ``shape`` = (n, h, w) of that slice.  ``grad``: d(loss)/d(out)
         (d(maps) for the cmg) for the seeds and launches, buffers 12 and up.  ``grads``: 34 fp32 tensors or None
         (None where the stack writes nothing) that receive the parameter gradients of the layers before a
-        data-gradient launch, buffers 14 and up."""
+        data-gradient launch, buffers 14 and up.  ``train_mode``: that of the forward that filled the workspace."""
+        self.set_train_mode(train_mode)
         n, h, w = shape
         dst = torch.empty((n, self.BACKWARD_BUFFER_CHANNELS[buffer], h, w), dtype=torch.float32, device=self.device)
         g = None if grad is None else grad.detach().to(self.device, torch.float32).contiguous()
@@ -453,9 +462,10 @@ class Engine:
     # ---- the sub-modules under autograd (wn_confidence_maps_train / _backward, wn_refine_train / _backward) --------
     STACK_CMG, STACK_REFINER = 0, 1
 
-    def _submodule_train(self, stack: int, ins, call, what: str):
+    def _submodule_train(self, stack: int, ins, call, what: str, train_mode: int):
         """The batch in slices of at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES, one workspace per slice, as
         ``forward_train``.  call(slice inputs, strides, slice output, n, h, w, workspace) -> rc."""
+        self.set_train_mode(train_mode)
         n, _, h, w = ins[0].shape
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
         if out.numel() == 0:
@@ -477,10 +487,11 @@ class Engine:
             saved.append((a, b, ws))
         return out, saved
 
-    def _submodule_backward(self, grad, saved, shapes, first: int, want_inputs, call, what: str):
+    def _submodule_backward(self, grad, saved, shapes, first: int, want_inputs, call, what: str, train_mode: int):
         """The parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) added in slice order, and
         the input gradients asked for by ``want_inputs`` (None where not).  call(grad slice, grads array, input grads
         array or None, n, h, w, workspace) -> rc."""
+        self.set_train_mode(train_mode)
         g = grad.detach().to(self.device, torch.float32).contiguous()
         n, _, h, w = g.shape
         saved = saved or []
@@ -503,41 +514,41 @@ class Engine:
                 torch._foreach_add_(grads, part)
         return grads, gin
 
-    def confidence_maps_train(self, x, wb, he, gc):
-        """``confidence_maps`` in the bf16x3 arithmetic of training, keeping the activations of the cmg stack
+    def confidence_maps_train(self, x, wb, he, gc, train_mode: int = _lib.MODE_BF16X3):
+        """``confidence_maps`` in the arithmetic of training (``train_mode``), keeping the activations of the cmg stack
         (wn_confidence_maps_train).  Returns (maps, saved workspaces) for ``confidence_maps_backward``."""
         ins = self._check_inputs((x, wb, he, gc))
         stream = _stream_ptr(self.device)
         return self._submodule_train(self.STACK_CMG, ins, lambda p, st, o, n, h, w, ws: self.lib.wn_confidence_maps_train(
             self.handle, p[0].data_ptr(), p[1].data_ptr(), p[2].data_ptr(), p[3].data_ptr(), st, o.data_ptr(), n, h, w,
-            ws.data_ptr(), ws.numel(), stream), "wn_confidence_maps_train")
+            ws.data_ptr(), ws.numel(), stream), "wn_confidence_maps_train", train_mode)
 
-    def confidence_maps_backward(self, grad_maps, saved, shapes, want_inputs=(False,) * 4):
+    def confidence_maps_backward(self, grad_maps, saved, shapes, want_inputs=(False,) * 4, train_mode: int = _lib.MODE_BF16X3):
         """d(loss)/d(maps) + the workspaces of ``confidence_maps_train`` -> the 16 cmg parameter gradients
         (state-dict order) and the gradients of x, wb, he, gc where ``want_inputs`` asks for them (else None)."""
         stream = _stream_ptr(self.device)
         return self._submodule_backward(grad_maps, saved, shapes, 0, want_inputs, lambda g, arr, gin, n, h, w, ws:
                                         self.lib.wn_confidence_maps_backward(self.handle, g, arr, gin, n, h, w,
                                                                              ws.data_ptr(), ws.numel(), stream),
-                                        "wn_confidence_maps_backward")
+                                        "wn_confidence_maps_backward", train_mode)
 
-    def refine_train(self, which: int, x, xbar):
-        """``refine`` in the bf16x3 arithmetic of training, keeping the activations of the refiner stack
+    def refine_train(self, which: int, x, xbar, train_mode: int = _lib.MODE_BF16X3):
+        """``refine`` in the arithmetic of training (``train_mode``), keeping the activations of the refiner stack
         (wn_refine_train).  Returns (out, saved workspaces) for ``refine_backward``."""
         ins = self._check_inputs((x, xbar))
         stream = _stream_ptr(self.device)
         return self._submodule_train(self.STACK_REFINER, ins, lambda p, st, o, n, h, w, ws: self.lib.wn_refine_train(
             self.handle, int(which), p[0].data_ptr(), p[1].data_ptr(), st, o.data_ptr(), n, h, w, ws.data_ptr(),
-            ws.numel(), stream), "wn_refine_train")
+            ws.numel(), stream), "wn_refine_train", train_mode)
 
-    def refine_backward(self, which: int, grad_out, saved, shapes, want_inputs=(False, False)):
+    def refine_backward(self, which: int, grad_out, saved, shapes, want_inputs=(False, False), train_mode: int = _lib.MODE_BF16X3):
         """d(loss)/d(out) + the workspaces of ``refine_train`` -> the 6 parameter gradients of refiner ``which``
         (state-dict order) and the gradients of x, xbar where ``want_inputs`` asks for them (else None)."""
         stream = _stream_ptr(self.device)
         return self._submodule_backward(grad_out, saved, shapes, 16 + 6 * int(which), want_inputs,
                                         lambda g, arr, gin, n, h, w, ws: self.lib.wn_refine_backward(
                                             self.handle, int(which), g, arr, gin, n, h, w, ws.data_ptr(), ws.numel(),
-                                            stream), "wn_refine_backward")
+                                            stream), "wn_refine_backward", train_mode)
 
     # ---- preprocess / postprocess ----------------------------------------------
     def preprocess(self, rgb_u8: torch.Tensor, tensors: bool = True, images: bool = False):
@@ -890,13 +901,14 @@ class Engine:
         """One training call's own workspace (it lives until backward), or that of one backward_ragged_tiled call."""
         return torch.empty(int(nbytes), dtype=torch.uint8, device=self.device)
 
-    def forward_train_ragged(self, items):
+    def forward_train_ragged(self, items, train_mode: int = _lib.MODE_BF16X3):
         """``forward_train`` of images of their own sizes (wn_forward_train_ragged): ``items`` as ``forward_ragged``.
         The images are grouped into training calls by ``ragged_train_calls``; each call runs its images as one pass
         of equally sized slots and keeps the activations in its own workspace.  Returns (one output per item, saved
         state for ``backward_ragged``).  Each image's output equals ``forward_train`` of that image alone bit for
         bit.  One image over TRAIN_MAX_PIXELS is refused."""
         ins, outs, images = self._ragged_items(items)
+        self.set_train_mode(train_mode)
         for i, j, h, w in images:
             if h * w > self.TRAIN_MAX_PIXELS:
                 raise _lib.WaterNetLibraryError(
@@ -916,11 +928,12 @@ class Engine:
             calls.append((imgs, hs, wss, ws))
         return outs, calls
 
-    def backward_ragged(self, grad_outs, saved, shapes, want_inputs=None):
+    def backward_ragged(self, grad_outs, saved, shapes, want_inputs=None, train_mode: int = _lib.MODE_BF16X3):
         """d(loss)/d(out) of every item (a list of (N_i,3,H_i,W_i) tensors) + the state of ``forward_train_ragged``
         -> the 34 parameter gradients (state-dict order), the gradients of all images summed call by call in call
         order, and one list of four input gradients per item (None where ``want_inputs[i][t]`` is false, or
         everywhere when ``want_inputs`` is None)."""
+        self.set_train_mode(train_mode)
         grads_out = [g.detach().to(self.device, torch.float32).contiguous() for g in grad_outs]
         saved = saved or []
         make = torch.empty if saved else torch.zeros  # no images: zero gradients
@@ -951,11 +964,13 @@ class Engine:
         return int(self.lib.wn_backward_tiled_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels)))
 
     def backward_tiled(self, grad_out: torch.Tensor, inputs, shapes, tile=DEFAULT_TILE, want_input_grads: bool = False,
-                       max_pass_pixels: int = 0):
+                       max_pass_pixels: int = 0, train_mode: int = _lib.MODE_BF16X3):
         """The gradients of ``backward`` from the four input images alone (wn_backward_tiled): the training forward
         is recomputed in the overlapping windows of ``forward_tiled``, one pass of windows at a time, so no
         activation outlives the call and the workspace does not grow with the image size.  ``max_pass_pixels``:
-        window pixels per pass (0 = 2 Mi, ~11.8 GB).  The workspace is allocated for this call only."""
+        window pixels per pass (0 = 2 Mi, ~11.8 GB).  The workspace is allocated for this call only.  ``train_mode``:
+        the arithmetic of the recomputed forward and of the backward."""
+        self.set_train_mode(train_mode)
         th, tw = self._tile_hw(tile)
         ins = self._check_inputs(inputs)
         g = grad_out.detach().to(self.device, torch.float32).contiguous()
@@ -996,14 +1011,15 @@ class Engine:
         return int(self.lib.wn_backward_ragged_tiled_workspace_bytes(hs, ws, n, th, tw, int(max_pass_pixels)))
 
     def backward_ragged_tiled(self, grad_outs, items, shapes, tile=DEFAULT_TILE, want_inputs=None,
-                              max_pass_pixels: int = 0):
+                              max_pass_pixels: int = 0, train_mode: int = _lib.MODE_BF16X3):
         """The gradients of ``backward_ragged`` from the input images alone (wn_backward_ragged_tiled): ``items`` as
         ``forward_ragged`` takes them, ``grad_outs`` one (N_i,3,H_i,W_i) tensor per item.  The windows of ``tile`` of
         every image are packed into passes of ``max_pass_pixels`` slot pixels (0 = 2 Mi), and the training forward
         is recomputed one pass at a time, so no activation outlives the call.  Returns the 34 parameter gradients
         (state-dict order, summed over the images) and one list of four input gradients per item (None where
         ``want_inputs[i][t]`` is false, or everywhere when ``want_inputs`` is None).  Zero-pixel items get zero
-        gradients.  The workspace is allocated for this call only."""
+        gradients.  The workspace is allocated for this call only.  ``train_mode`` as ``backward_tiled``."""
+        self.set_train_mode(train_mode)
         th, tw = self._tile_hw(tile)
         ins, _, images = self._ragged_items(items, outputs=False)
         grads_out = [g.detach().to(self.device, torch.float32).contiguous() for g in grad_outs]
@@ -1048,10 +1064,11 @@ class Engine:
                                                                         int(stack)))
 
     def _submodule_backward_tiled(self, stack: int, first: int, grad, ins, shapes, tile, want_inputs,
-                                  max_pass_pixels: int, call, what: str):
+                                  max_pass_pixels: int, call, what: str, train_mode: int):
         """The parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) and the input gradients
         asked for by ``want_inputs`` (None where not), in one call with a workspace of its own.  call(strides, grad,
         grads array, input grads array or None, n, h, w, th, tw, workspace) -> rc."""
+        self.set_train_mode(train_mode)
         th, tw = self._tile_hw(tile)
         g = grad.detach().to(self.device, torch.float32).contiguous()
         n, _, h, w = ins[0].shape
@@ -1080,7 +1097,7 @@ class Engine:
         return grads, gin
 
     def confidence_maps_backward_tiled(self, grad_maps, inputs, shapes, tile=DEFAULT_TILE, want_inputs=(False,) * 4,
-                                       max_pass_pixels: int = 0):
+                                       max_pass_pixels: int = 0, train_mode: int = _lib.MODE_BF16X3):
         """The gradients of ``confidence_maps_backward`` from the four input images alone
         (wn_confidence_maps_backward_tiled): the cmg's training forward is recomputed in the overlapping windows of
         ``confidence_maps_tiled``, one pass at a time, so no activation outlives the call and the workspace does not
@@ -1094,10 +1111,11 @@ class Engine:
             self.STACK_CMG, 0, grad_maps, ins, shapes, tile, want_inputs, mpp,
             lambda st, g, arr, gin, n, h, w, th, tw, ws: self.lib.wn_confidence_maps_backward_tiled(
                 self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(), ins[3].data_ptr(), st, g, arr,
-                gin, n, h, w, th, tw, mpp, ws.data_ptr(), ws.numel(), stream), "wn_confidence_maps_backward_tiled")
+                gin, n, h, w, th, tw, mpp, ws.data_ptr(), ws.numel(), stream), "wn_confidence_maps_backward_tiled",
+            train_mode)
 
     def refine_backward_tiled(self, which: int, grad_out, inputs, shapes, tile=DEFAULT_TILE,
-                              want_inputs=(False, False), max_pass_pixels: int = 0):
+                              want_inputs=(False, False), max_pass_pixels: int = 0, train_mode: int = _lib.MODE_BF16X3):
         """The gradients of ``refine_backward`` from x and xbar alone (wn_refine_backward_tiled), as
         ``confidence_maps_backward_tiled`` (0 = 2 Mi window pixels per pass, ~3.8 GB)."""
         ins = self._check_inputs(inputs)
@@ -1107,7 +1125,7 @@ class Engine:
             self.STACK_REFINER, 16 + 6 * int(which), grad_out, ins, shapes, tile, want_inputs, mpp,
             lambda st, g, arr, gin, n, h, w, th, tw, ws: self.lib.wn_refine_backward_tiled(
                 self.handle, int(which), ins[0].data_ptr(), ins[1].data_ptr(), st, g, arr, gin, n, h, w, th, tw, mpp,
-                ws.data_ptr(), ws.numel(), stream), "wn_refine_backward_tiled")
+                ws.data_ptr(), ws.numel(), stream), "wn_refine_backward_tiled", train_mode)
 
     # ---- the VGG19 perceptual loss (wn_perceptual_loss) ----------------------------------------
     def pack_vgg_weights(self, params: Sequence[torch.Tensor], key=None) -> None:

@@ -33,6 +33,15 @@ from .engine import TRAIN_PASS_PIXELS, Engine, new_engine
 
 MODES = {"default": _lib.MODE_DEFAULT, "fp32": _lib.MODE_FP32_SIMT, "bf16x3": _lib.MODE_BF16X3,
          "bf16_fp8": _lib.MODE_BF16_FP8}
+# the arithmetic of the native training calls (wn_set_train_mode): three bf16 products per product (~1e-5 of fp32),
+# or one (operands rounded to bf16 once, fp32 accumulation, as autocast trains convolutions)
+TRAIN_PRECISIONS = {"bf16x3": _lib.MODE_BF16X3, "bf16": _lib.MODE_BF16}
+
+
+def _checked_train_mode(train_precision) -> int:
+    if train_precision not in TRAIN_PRECISIONS:
+        raise ValueError(f"unknown train_precision {train_precision!r}; choose from {sorted(TRAIN_PRECISIONS)}")
+    return TRAIN_PRECISIONS[train_precision]
 
 # model -> {device index: Engine}.  Every module that can be called on its own (WaterNet and, like in the
 # reference, its sub-modules) has a private engine per device = its own packed-weight slot in the library.
@@ -132,7 +141,8 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
     With autograd recording (a parameter or an input requires grad) a call on CUDA tensors in a tensor-core
     precision trains natively: the forward runs in the bf16x3 arithmetic of training and keeps the stack's
     activations (``wn_confidence_maps_train`` / ``wn_refine_train``), and backward gives the gradients of the stack's
-    own parameters and of its inputs (``wn_confidence_maps_backward`` / ``wn_refine_backward``).  Nothing reaches the
+    own parameters and of its inputs (``wn_confidence_maps_backward`` / ``wn_refine_backward``), in the arithmetic of
+    ``train_precision`` (as ``WaterNet.train_precision``; the default "bf16x3").  Nothing reaches the
     parent's other parameters.  Whole images per call (``tile`` does not apply), at most ``Engine.TRAIN_MAX_PIXELS``
     pixels per image; a batch over that runs in slices.  CPU tensors, ``precision="fp32"`` and a larger image
     evaluate the torch graph instead.
@@ -140,12 +150,13 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
     ``wn_confidence_maps_tiled`` / ``wn_refine_tiled`` in the bf16x3 arithmetic of training, and backward recomputes
     the stack's activations window by window (``wn_confidence_maps_backward_tiled`` / ``wn_refine_backward_tiled``),
     in about 8 GB for the cmg and 4 GB for a refiner whatever the image or batch size, with no limit on the image
-    size.  Bound to a ``WaterNet`` a stack follows the parent's ``precision``, ``tile`` and ``grad_tile``; a
-    free-standing one uses its own attributes.
+    size.  Bound to a ``WaterNet`` a stack follows the parent's ``precision``, ``train_precision``, ``tile`` and
+    ``grad_tile``; a free-standing one uses its own attributes.
     """
 
     spec: List[tuple] = []
     precision = "default"
+    train_precision = "bf16x3"
     tile = None
     grad_tile = None
 
@@ -225,12 +236,18 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
             raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(MODES)}")
         return _checked_grad_tile(self.grad_tile, MODES[self.precision])
 
+    def _train_mode(self) -> int:
+        """The training arithmetic (wn_set_train_mode) of a call that records an autograd graph: the parent's
+        ``train_precision`` for a bound stack, else its own."""
+        parent = self._parent_ref() if self._parent_ref is not None else None
+        return parent._train_mode() if parent is not None else _checked_train_mode(self.train_precision)
+
     def _train_call(self, x):
-        """(engine with the right state dict packed, slot, grad_tile or None) for a call that records an autograd
-        graph, or None where the torch graph runs instead.  With grad_tile any image size runs natively."""
+        """(engine with the right state dict packed, slot, grad_tile or None, training mode) for a call that records
+        an autograd graph, or None where the torch graph runs instead.  With grad_tile any image size runs natively."""
         grad_tile = self._grad_tile()
         native = self._train_engine(x, any_size=grad_tile is not None)
-        return None if native is None else (*native, grad_tile)
+        return None if native is None else (*native, grad_tile, self._train_mode())
 
     @staticmethod
     def _needs_graph(tensors, params):
@@ -245,12 +262,13 @@ class _SubmoduleForward(torch.autograd.Function):
     With ``grad_tile`` the forward keeps nothing but the inputs (wn_confidence_maps_tiled / wn_refine_tiled in the
     bf16x3 arithmetic of training) and the backward recomputes the stack's activations window by window
     (wn_confidence_maps_backward_tiled / wn_refine_backward_tiled); both hold at most one pass of TRAIN_PASS_PIXELS
-    window pixels."""
+    window pixels.  train_mode (wn_set_train_mode) is kept for the backward, so that it runs under the forward's mode
+    whatever another module trains on the same engine in between."""
 
     @staticmethod
-    def forward(ctx, eng, which, grad_tile, n_in, *tensors):
+    def forward(ctx, eng, which, grad_tile, train_mode, n_in, *tensors):
         ins, params = tensors[:n_in], tensors[n_in:]
-        ctx.engine, ctx.which, ctx.n_in, ctx.grad_tile = eng, which, n_in, grad_tile
+        ctx.engine, ctx.which, ctx.n_in, ctx.grad_tile, ctx.train_mode = eng, which, n_in, grad_tile, train_mode
         ctx.weights_key = eng._weights_key
         ctx.shapes = [p.shape for p in params]
         if grad_tile is not None:
@@ -258,7 +276,10 @@ class _SubmoduleForward(torch.autograd.Function):
             if which is None:
                 return eng.confidence_maps_tiled(*ins, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS)
             return eng.refine_tiled(which, *ins, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS)
-        out, ctx.saved_ws = eng.confidence_maps_train(*ins) if which is None else eng.refine_train(which, *ins)
+        if which is None:
+            out, ctx.saved_ws = eng.confidence_maps_train(*ins, train_mode=train_mode)
+        else:
+            out, ctx.saved_ws = eng.refine_train(which, *ins, train_mode=train_mode)
         return out
 
     @staticmethod
@@ -266,22 +287,23 @@ class _SubmoduleForward(torch.autograd.Function):
         eng = ctx.engine
         if eng._weights_key != ctx.weights_key:
             raise RuntimeError("sub-module parameters were modified between forward and backward")
-        need = ctx.needs_input_grad[4:]
+        need = ctx.needs_input_grad[5:]
         want_in, want_par = need[:ctx.n_in], need[ctx.n_in:]
+        tm = ctx.train_mode
         if ctx.grad_tile is not None:
             ins = ctx.saved_tensors
             if ctx.which is None:
                 grads, gin = eng.confidence_maps_backward_tiled(grad, ins, ctx.shapes, ctx.grad_tile, want_in,
-                                                                max_pass_pixels=TRAIN_PASS_PIXELS)
+                                                                max_pass_pixels=TRAIN_PASS_PIXELS, train_mode=tm)
             else:
                 grads, gin = eng.refine_backward_tiled(ctx.which, grad, ins, ctx.shapes, ctx.grad_tile, want_in,
-                                                       max_pass_pixels=TRAIN_PASS_PIXELS)
+                                                       max_pass_pixels=TRAIN_PASS_PIXELS, train_mode=tm)
         elif ctx.which is None:
-            grads, gin = eng.confidence_maps_backward(grad, ctx.saved_ws, ctx.shapes, want_in)
+            grads, gin = eng.confidence_maps_backward(grad, ctx.saved_ws, ctx.shapes, want_in, train_mode=tm)
         else:
-            grads, gin = eng.refine_backward(ctx.which, grad, ctx.saved_ws, ctx.shapes, want_in)
+            grads, gin = eng.refine_backward(ctx.which, grad, ctx.saved_ws, ctx.shapes, want_in, train_mode=tm)
         ctx.saved_ws = None
-        return (None, None, None, None, *gin, *[g if w else None for g, w in zip(grads, want_par)])
+        return (None, None, None, None, None, *gin, *[g if w else None for g, w in zip(grads, want_par)])
 
 
 def _zeros_like_spec(spec, ref):
@@ -315,8 +337,8 @@ class ConfidenceMapGenerator(_ConvStack):
             if native is None:
                 maps = self._graph(x, wb, ce, gc)
             else:
-                eng, _, grad_tile = native
-                maps = _SubmoduleForward.apply(eng, None, grad_tile, 4, x, wb, ce, gc, *self._own_params())
+                eng, _, grad_tile, train_mode = native
+                maps = _SubmoduleForward.apply(eng, None, grad_tile, train_mode, 4, x, wb, ce, gc, *self._own_params())
         else:
             mode, eng, _, tile = self._mode_and_engine(x, self._zero_layout)
             if tile is None:
@@ -346,8 +368,8 @@ class Refiner(_ConvStack):
             native = self._train_call(x)
             if native is None:
                 return self._graph(x, xbar)
-            eng, slot, grad_tile = native
-            return _SubmoduleForward.apply(eng, slot, grad_tile, 2, x, xbar, *self._own_params())
+            eng, slot, grad_tile, train_mode = native
+            return _SubmoduleForward.apply(eng, slot, grad_tile, train_mode, 2, x, xbar, *self._own_params())
         mode, eng, slot, tile = self._mode_and_engine(x, self._zero_layout)
         if tile is None:
             return eng.refine(slot, x, xbar, mode)
@@ -359,7 +381,8 @@ class _KernelForward(torch.autograd.Function):
     grad) from the CUDA library (wn_forward_train / wn_backward).  Only the fp32 CUDA-core mode obtains
     its gradients by re-evaluating the torch graph.  With ``grad_tile`` the forward keeps nothing but the four
     inputs (wn_forward_tiled in the bf16x3 arithmetic of training) and the backward recomputes the activations
-    window by window (wn_backward_tiled); both hold at most one pass of TRAIN_PASS_PIXELS window pixels.
+    window by window (wn_backward_tiled); both hold at most one pass of TRAIN_PASS_PIXELS window pixels.  The native
+    calls run in the model's ``train_precision``, kept in ctx for the backward.
     """
 
     @staticmethod
@@ -367,6 +390,7 @@ class _KernelForward(torch.autograd.Function):
         ctx.model = model
         ctx.native = mode != _lib.MODE_FP32_SIMT
         ctx.grad_tile = grad_tile
+        ctx.train_mode = model._train_mode() if ctx.native else None
         ctx.input_needs_grad = [t.requires_grad for t in (x, wb, ce, gc)]
         if grad_tile is not None:
             eng = model._engine_with_weights(x)
@@ -375,7 +399,7 @@ class _KernelForward(torch.autograd.Function):
             return eng.forward_tiled(x, wb, ce, gc, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS)
         if ctx.native:
             eng = model._engine_with_weights(x)
-            out, ws = eng.forward_train(x, wb, ce, gc)
+            out, ws = eng.forward_train(x, wb, ce, gc, train_mode=ctx.train_mode)
             ctx.engine, ctx.saved_ws = eng, ws
             ctx.weights_key = eng._weights_key
             return out
@@ -394,9 +418,9 @@ class _KernelForward(torch.autograd.Function):
             shapes = [p.shape for p in params]
             if ctx.grad_tile is not None:
                 res = eng.backward_tiled(grad_out, ctx.saved_tensors, shapes, ctx.grad_tile, want_input_grads=want_in,
-                                         max_pass_pixels=TRAIN_PASS_PIXELS)
+                                         max_pass_pixels=TRAIN_PASS_PIXELS, train_mode=ctx.train_mode)
             else:
-                res = eng.backward(grad_out, ctx.saved_ws, shapes, want_input_grads=want_in)
+                res = eng.backward(grad_out, ctx.saved_ws, shapes, want_input_grads=want_in, train_mode=ctx.train_mode)
                 ctx.saved_ws = None
             grads, gin = res if want_in else (res, [None] * 4)
             gpar = [g if p.requires_grad else None for g, p in zip(grads, params)]
@@ -428,6 +452,7 @@ class _RaggedKernelForward(torch.autograd.Function):
         items = [flat[4 * i:4 * i + 4] for i in range(n_items)]
         eng = model._engine_with_weights(items[0][0])
         ctx.engine, ctx.weights_key, ctx.n_items, ctx.grad_tile = eng, eng._weights_key, n_items, grad_tile
+        ctx.train_mode = model._train_mode()
         ctx.shapes = [p.shape for p in params]
         if grad_tile is not None:
             # refuse here what the backward would refuse (a window over the pixels of one training pass)
@@ -438,7 +463,7 @@ class _RaggedKernelForward(torch.autograd.Function):
                     f"may have at most {Engine.TRAIN_MAX_PIXELS >> 20} Mi pixels); use a smaller grad_tile")
             ctx.save_for_backward(*flat)
             return tuple(eng.forward_ragged(items, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS))
-        outs, ctx.saved_calls = eng.forward_train_ragged(items)
+        outs, ctx.saved_calls = eng.forward_train_ragged(items, train_mode=ctx.train_mode)
         return tuple(outs)
 
     @staticmethod
@@ -452,9 +477,9 @@ class _RaggedKernelForward(torch.autograd.Function):
             flat = ctx.saved_tensors
             items = [flat[4 * i:4 * i + 4] for i in range(ctx.n_items)]
             grads, gin = eng.backward_ragged_tiled(grad_outs, items, ctx.shapes, ctx.grad_tile, want_in,
-                                                   max_pass_pixels=TRAIN_PASS_PIXELS)
+                                                   max_pass_pixels=TRAIN_PASS_PIXELS, train_mode=ctx.train_mode)
         else:
-            grads, gin = eng.backward_ragged(grad_outs, ctx.saved_calls, ctx.shapes, want_in)
+            grads, gin = eng.backward_ragged(grad_outs, ctx.saved_calls, ctx.shapes, want_in, train_mode=ctx.train_mode)
             ctx.saved_calls = None
         gpar = [g if w else None for g, w in zip(grads, need[4 * ctx.n_items:])]
         return (None, None, None, *[t for row in gin for t in row], *gpar)
@@ -485,13 +510,21 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
     about 12 GB whatever the image or batch size.  The gradients equal the untiled ones up to the order of fp32 sums.
     It costs one more forward and the windows' overlap, so where the untiled path fits it is faster.  Tensor-core
     precisions only.  Calls of ``cmg`` and the refiners on their own follow it as well (``_ConvStack``).
+
+    ``train_precision``: the arithmetic of the native training calls (forward, data gradients and weight gradients of
+    every call that records an autograd graph, windowed and ragged ones included).  ``"bf16x3"`` (default, ~1e-5 of
+    fp32) or ``"bf16"``: one bf16 tensor-core product per product with fp32 accumulation, the operands rounded to bf16
+    once, as autocast trains convolutions (DESIGN.md 4.13).  The forward of a ``grad_tile`` call stays bf16x3 (it is
+    ``wn_forward_tiled``); ``precision`` and inference are unaffected.  ``cmg`` and the refiners follow it.
     """
 
     tile = None  # models pickled before the attribute existed
     grad_tile = None
+    train_precision = "bf16x3"
 
-    def __init__(self, precision: str = "default", tile=None, grad_tile=None):
+    def __init__(self, precision: str = "default", tile=None, grad_tile=None, train_precision: str = "bf16x3"):
         super().__init__()
+        _checked_train_mode(train_precision)
         self.cmg = ConfidenceMapGenerator()
         self.wb_refiner = Refiner()
         self.ce_refiner = Refiner()
@@ -499,6 +532,7 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
         self.precision = precision
         self.tile = tile
         self.grad_tile = grad_tile
+        self.train_precision = train_precision
         if tile is not None:
             _checked_tile(tile, self._mode())
         if grad_tile is not None:
@@ -524,6 +558,9 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
         if self.precision not in MODES:
             raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(MODES)}")
         return MODES[self.precision]
+
+    def _train_mode(self) -> int:
+        return _checked_train_mode(self.train_precision)
 
     def _ordered_params(self):
         """The 34 tensors in state-dict order (what wn_pack_weights expects)."""
