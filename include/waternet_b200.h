@@ -302,8 +302,9 @@ size_t wn_train_workspace_bytes(int n, int h, int w);
  * setting: no device pointer, no launch.  It is read by wn_forward_train / wn_backward, wn_forward_train_ragged /
  * wn_backward_ragged, wn_backward_tiled, wn_backward_ragged_tiled, wn_confidence_maps_train / _backward / _backward_tiled,
  * wn_refine_train / _backward / _backward_tiled and wn_debug_backward_layer: their training forward, seeds, data
- * gradients and weight gradients all run in it.  In WN_MODE_BF16 every stored activation and gradient plane holds
- * bf16(v) with lo = 0; the workspace sizes do not change.  A backward must run under the mode of the forward that
+ * gradients and weight gradients all run in it.  wn_perceptual_loss and wn_debug_vgg_layer read it too: their VGG
+ * convolutions, data gradients, packed image and seed run in it (DESIGN.md 4.14).  In WN_MODE_BF16 every stored
+ * activation and gradient plane holds bf16(v) with lo = 0; the workspace sizes do not change.  A backward must run under the mode of the forward that
  * filled its workspace.  The inference calls ignore the setting (and reject WN_MODE_BF16 as their `mode`).
  * WN_ABI_VERSION stays 11: an addition, no existing signature or structure changed (as with wn_backward_ragged_tiled).
  */
@@ -558,8 +559,11 @@ int wn_stream_wait_value32(void* stream, void* addr, uint32_t value);
  *   L = mean over (n, c < 512, i < floor(H/16), j < floor(W/16)) of (255 * (F(out) - F(ref)))^2
  *
  * F = VGG19 features[:-1] (conv5_4 + ReLU) of (v - mean) / std with the ImageNet mean and std.  Every convolution
- * is bf16x3 with fp32 accumulation; a max-pool takes the first maximum in row-major order.  No VGG weight gradient
- * is computed.
+ * and data gradient runs in the handle's training mode (wn_set_train_mode) with fp32 accumulation: WN_MODE_BF16X3,
+ * the default of a new handle, three bf16 products per product; WN_MODE_BF16 one, a_hi x w_hi, with the packed image,
+ * every activation and gradient plane and the seed stored as bf16 with lo = 0 (DESIGN.md 4.14).  The loss partials
+ * are float64 sums of the decoded features in both modes.  A max-pool takes the first maximum in row-major order.
+ * No VGG weight gradient is computed.
  *
  * wn_vgg_pack_weights: params = weight and bias of the 16 convolutions in `features` order (fp32, contiguous OIHW
  *   and O), device pointers.  Packs the forward and the data-gradient stages; call again after the weights change.
@@ -579,7 +583,7 @@ int wn_stream_wait_value32(void* stream, void* addr, uint32_t value);
  *   respect to conv5_4 before its ReLU, (n, 512, H >> 4, W >> 4)); layer 22 + k = the output of the backward launch
  *   of forward launch k, the gradient with respect to that launch's input (k = 0: the 16 normalised channels, 3
  *   real).  ref and ref_strides may be NULL for layers 0..20.  The workspace is that of
- *   wn_perceptual_loss_workspace_bytes(n, H, W, tile_h, tile_w, 0).
+ *   wn_perceptual_loss_workspace_bytes(n, H, W, tile_h, tile_w, 0).  Every layer runs in the handle's training mode.
  *
  * WN_ABI_VERSION stays 11: these four entry points are additions and no existing signature or structure changed,
  * so a library built before them still serves every client that does not call them (as with wn_backward_ragged_tiled).

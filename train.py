@@ -107,7 +107,7 @@ def main():
     T.save_metrics(savedir, train_hist, val_hist, {
         "epochs": args.epochs, "batch_size": args.batch_size, "im_height": args.height, "im_width": args.width,
         "weights": args.weights, "native_size": args.native_size,
-        "train_precision": args.train_precision})
+        "train_precision": args.train_precision, **T.perceptual_config(args)})
     print(f"Metrics and weights saved to {savedir}")
     print(f"Total time: {timer() - start}s")
 

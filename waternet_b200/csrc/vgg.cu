@@ -5,8 +5,8 @@
 //   F = VGG19 features[:-1] (conv5_4 + ReLU) of the ImageNet-normalised image.
 //
 //   vgg_pack_kernel        strided fp32 NCHW -> (v - mean) / std -> the 16-channel bf16 hi/lo planes of each window
-//   conv_umma_kernel       the 16 convolutions (kEpiAct, bf16x3) and their data gradients (kEpiDgrad, ReLU' from the
-//                          saved planes) -- the kernel of the WaterNet layers, from the spec tables below
+//   conv_umma_kernel       the 16 convolutions (kEpiAct) and their data gradients (kEpiDgrad, ReLU' from the saved
+//                          planes) -- the kernel of the WaterNet layers, from the spec tables below
 //   vgg_pool_kernel        2 x 2 max-pool on planes: the first maximum of hi + lo in row-major order, hi/lo copied
 //   vgg_pool_bwd_kernel    routes each pooled gradient to the element the forward chose
 //   vgg_seed_kernel        each window's owned features: loss partials (float64) and the seed of the backward
@@ -16,6 +16,10 @@
 // so that it holds the 252-pixel support of every owned feature and its pooling grid is the image's.  The windows of
 // one pass have one size (a "class": a run of windows of equal extent per axis), so every level of a pass is an exact
 // tensor of floor(extent / 2^level) pixels per axis: beyond it the convolutions read zeros, as torch pads.
+//
+// Arithmetic: the handle's training mode (wn_set_train_mode), DESIGN.md 4.14.  bf16x3 issues three bf16 products per
+// product.  WN_MODE_BF16 issues one, a_hi x w_hi (UmmaCfg kFmtHi, the same packed weight images), and the pack, the
+// convolutions and the seed store bf16(v) with lo = 0; the pools, the fold and the decoders read hi + lo either way.
 #include <stdlib.h>
 #include <string.h>
 
@@ -273,11 +277,12 @@ static __global__ void vgg_scatter_kernel(const float* __restrict__ src, float* 
 }
 
 // pixel blockIdx.x * 256 + tid of window blockIdx.y of the pass: (v - mean) / std of the 3 channels (as torch
-// evaluates it in fp32) -> hi/lo planes of 16 channels (13 zero)
+// evaluates it in fp32) -> hi/lo planes of 16 channels (13 zero).  HI: single-pass bf16, bf16(v) and lo = 0.
 struct ImgArgs {
   const float* p;
   long long s[4];
 };
+template <bool HI = false>
 static __global__ void __launch_bounds__(256) vgg_pack_kernel(ImgArgs a, VggPass p, uint4* __restrict__ act0) {
   const int hw = p.h * p.w;
   const int pix = blockIdx.x * 256 + threadIdx.x;
@@ -290,8 +295,17 @@ static __global__ void __launch_bounds__(256) vgg_pack_kernel(ImgArgs a, VggPass
 #pragma unroll
   for (int c = 0; c < 3; c++) f[c] = __fdiv_rn(__fsub_rn(src[c * a.s[1]], mean[c]), stdv[c]);
   uint32_t hi[2], lo[2];
-  split_bf16x2(f[0], f[1], hi[0], lo[0]);
-  split_bf16x2(f[2], f[3], hi[1], lo[1]);
+  if constexpr (HI) {
+#pragma unroll
+    for (int j = 0; j < 2; j++) {
+      const __nv_bfloat162 hb = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
+      hi[j] = *reinterpret_cast<const uint32_t*>(&hb);
+      lo[j] = 0u;
+    }
+  } else {
+    split_bf16x2(f[0], f[1], hi[0], lo[0]);
+    split_bf16x2(f[2], f[3], hi[1], lo[1]);
+  }
   uint4* o = act0 + (size_t)blockIdx.y * 4 * hw + pix;
   const uint4 z = make_uint4(0, 0, 0, 0);
   o[0] = make_uint4(hi[0], hi[1], 0, 0);
@@ -392,7 +406,9 @@ static __global__ void __launch_bounds__(256) vgg_pool_bwd_kernel(const uint4* _
 
 // Window blockIdx.y, block blockIdx.x of kSeedBlocks: over its owned features, partial = sum of (255 (Fo - Fr))^2 in
 // float64, stored at partials[(base + w0 + window) * kSeedBlocks + block]; with g, the seed of the backward: scale *
-// (Fo - Fr) where Fo > 0 (ReLU' of conv5_4) at owned features, 0 everywhere else in the window.
+// (Fo - Fr) where Fo > 0 (ReLU' of conv5_4) at owned features, 0 everywhere else in the window.  HI: the seed of the
+// single-pass bf16 backward, bf16 and lo = 0 (the loss partials are the same sums of the decoded features).
+template <bool HI = false>
 static __global__ void __launch_bounds__(256) vgg_seed_kernel(const uint4* __restrict__ fo, const uint4* __restrict__ fr,
                                                               uint4* __restrict__ g, double* __restrict__ partials,
                                                               VggPass p, float scale) {
@@ -420,7 +436,14 @@ static __global__ void __launch_bounds__(256) vgg_seed_kernel(const uint4* __res
         s[j] = a > 0.f ? scale * d : 0.f;
       }
 #pragma unroll
-      for (int j = 0; j < 8; j += 2) split_bf16x2(s[j], s[j + 1], sh[j >> 1], sl[j >> 1]);
+      for (int j = 0; j < 8; j += 2) {
+        if constexpr (HI) {
+          const __nv_bfloat162 hb = __floats2bfloat162_rn(s[j], s[j + 1]);
+          sh[j >> 1] = *reinterpret_cast<const uint32_t*>(&hb);
+        } else {
+          split_bf16x2(s[j], s[j + 1], sh[j >> 1], sl[j >> 1]);
+        }
+      }
     }
     if (g) {
       g[o] = make_uint4(sh[0], sh[1], sh[2], sh[3]);
@@ -589,6 +612,10 @@ static int conv_fwd(wn_handle* h, const uint4* in, uint4* out, int cnt, int H, i
   a.dst0.planes_half = s.cout / 8;
   a.split_c = s.cout;
   a.cout = s.cout;
+  // single-pass bf16: the hi rows of the same weight images, at the table's tile geometry
+  if (h->train_bf16)
+    return launch_conv<3, s.cinpad, s.gw, kEpiAct, s.concat, 1, s.tps, kFmtHi, false, s.mw, s.ng>(
+        h, kSlotPost, h->vgg->fwd[LI], h->vgg->bias[LI], (void*)in, a, stream);
   return launch_conv<3, s.cinpad, s.gw, kEpiAct, s.concat, 1, s.tps, 0, false, s.mw, s.ng>(
       h, kSlotPost, h->vgg->fwd[LI], h->vgg->bias[LI], (void*)in, a, stream);
 }
@@ -606,6 +633,9 @@ static int conv_dgrad(wn_handle* h, const uint4* in, uint4* out, const uint4* ma
   a.cout = cout;
   a.mask_base = mask;  // nullptr: the normalised image, no ReLU in front
   a.mask_planes_half = cout / 8;
+  if (h->train_bf16)
+    return launch_conv<3, s.kpad, s.npad, kEpiDgrad, s.concat, 1, s.tps, kFmtHi, false, 1, s.ng>(
+        h, kSlotPost, h->vgg->bwd[LI], h->vgg->zero_bias, (void*)in, a, stream);
   return launch_conv<3, s.kpad, s.npad, kEpiDgrad, s.concat, 1, s.tps, 0, false, 1, s.ng>(
       h, kSlotPost, h->vgg->bwd[LI], h->vgg->zero_bias, (void*)in, a, stream);
 }
@@ -676,7 +706,19 @@ static int pack_window(wn_handle* h, const float* img, const int64_t st[4], cons
   ImgArgs a;
   a.p = img;
   for (int k = 0; k < 4; k++) a.s[k] = st[k];
-  vgg_pack_kernel<<<dim3((p.h * p.w + 255) / 256, p.count), 256, 0, stream>>>(a, p, act0);
+  const dim3 grid((p.h * p.w + 255) / 256, p.count);
+  if (h->train_bf16) vgg_pack_kernel<true><<<grid, 256, 0, stream>>>(a, p, act0);
+  else vgg_pack_kernel<<<grid, 256, 0, stream>>>(a, p, act0);
+  WN_LAUNCH_CHECK(h);
+  return WN_OK;
+}
+
+// the loss partials of the pass's windows and, with g, the seed of the backward in the handle's training mode
+static int seed_window(wn_handle* h, const uint4* fo, const uint4* fr, uint4* g, double* partials, const VggPass& p,
+                       float scale, cudaStream_t stream) {
+  const dim3 grid(kSeedBlocks, p.count);
+  if (h->train_bf16) vgg_seed_kernel<true><<<grid, 256, 0, stream>>>(fo, fr, g, partials, p, scale);
+  else vgg_seed_kernel<<<grid, 256, 0, stream>>>(fo, fr, g, partials, p, scale);
   WN_LAUNCH_CHECK(h);
   return WN_OK;
 }
@@ -721,9 +763,7 @@ static int vgg_run(wn_handle* h, const float* out, const int64_t out_st[4], cons
     if ((rc = pack_window(h, out, out_st, p, b.act0, stream))) return rc;
     uint4* fo = grad ? b.saved[kVggSteps - 1] : b.saved[0];
     if ((rc = vgg_forward(h, b, grad != nullptr, fo, p.count, p.h, p.w, stream))) return rc;
-    vgg_seed_kernel<<<dim3(kSeedBlocks, p.count), 256, 0, stream>>>(fo, b.fref, grad ? b.ping : nullptr, partials, p,
-                                                                    scale);
-    WN_LAUNCH_CHECK(h);
+    if ((rc = seed_window(h, fo, b.fref, grad ? b.ping : nullptr, partials, p, scale, stream))) return rc;
     if (!grad) continue;
     uint4* gin = nullptr;
     if ((rc = vgg_backward(h, b, p.count, p.h, p.w, stream, &gin))) return rc;
@@ -811,9 +851,9 @@ int vgg_debug_layer(wn_handle* h, const float* x, const int64_t st[4], const flo
   if ((rc = vgg_forward(h, b, false, b.fref, p.count, p.h, p.w, stream))) return rc;
   if ((rc = pack_window(h, x, st, p, b.act0, stream))) return rc;
   if ((rc = vgg_forward(h, b, true, nullptr, p.count, p.h, p.w, stream))) return rc;
-  vgg_seed_kernel<<<dim3(kSeedBlocks, p.count), 256, 0, stream>>>(b.saved[kVggSteps - 1], b.fref, b.ping, partials, p,
-                                                                  (float)(2.0 * 255.0 * 255.0 / (double)count));
-  WN_LAUNCH_CHECK(h);
+  if ((rc = seed_window(h, b.saved[kVggSteps - 1], b.fref, b.ping, partials, p,
+                        (float)(2.0 * 255.0 * 255.0 / (double)count), stream)))
+    return rc;
   uint4* g = b.ping;
   int l = 4, c = 512;
   if (layer > kVggSteps + 1) {

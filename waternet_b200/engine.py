@@ -1159,10 +1159,13 @@ class Engine:
                              f"must be at least 16 x 16 and a window at most {VGG_MAX_PIXELS} pixels{hint}")
         return self._workspace("vgg", nbytes)
 
-    def perceptual_loss(self, out, ref, tile=None, want_grad: bool = False, max_pass_pixels: int = 0):
+    def perceptual_loss(self, out, ref, tile=None, want_grad: bool = False, max_pass_pixels: int = 0,
+                        train_mode: int = _lib.MODE_BF16X3):
         """mean((255 (F(out) - F(ref)))^2) with F = VGG19 features[:-1] of the normalised images, on the packed VGG
         weights (wn_perceptual_loss), in windows that own ``tile`` input pixels of features (None: one window per
-        image).  Returns (0-d loss, d(loss)/d(out) as a contiguous (N,3,H,W) tensor, or None without ``want_grad``)."""
+        image).  Returns (0-d loss, d(loss)/d(out) as a contiguous (N,3,H,W) tensor, or None without ``want_grad``).
+        ``train_mode``: the arithmetic of the VGG convolutions, MODE_BF16X3 or single-pass MODE_BF16."""
+        self.set_train_mode(train_mode)
         o, r = (t.detach() if t.dtype == torch.float32 else t.detach().float() for t in (out, ref))
         for t in (o, r):
             if t.device != self.device or t.dim() != 4 or t.shape[1] != 3:
@@ -1184,11 +1187,13 @@ class Engine:
         _lib.check(rc, "wn_perceptual_loss")
         return loss, grad
 
-    def debug_vgg_layer(self, x, layer: int, tile=None, ref=None) -> torch.Tensor:
+    def debug_vgg_layer(self, x, layer: int, tile=None, ref=None, train_mode: int = _lib.MODE_BF16X3) -> torch.Tensor:
         """Test aid (wn_debug_vgg_layer), as fp32 (N, C, H >> level, W >> level): launch ``layer`` (0..19) of the VGG
         forward of whole images; (20) the conv5_4 features of the windowed call with ``tile``; for the loss of
         (out = x, ``ref``): (21) the seed, d(loss)/d(conv5_4 before its ReLU); (22 + k) the output of the backward
-        launch of forward launch k, d(loss)/d(input of launch k) (k = 0: 16 normalised channels, 3 real)."""
+        launch of forward launch k, d(loss)/d(input of launch k) (k = 0: 16 normalised channels, 3 real).
+        ``train_mode`` as ``perceptual_loss``."""
+        self.set_train_mode(train_mode)
         x = x.detach().float()
         n, _, h, w = x.shape
         th, tw = vgg_tile_hw(tile)

@@ -20,7 +20,7 @@ import torch.nn as nn
 
 from .engine import new_engine
 from .metrics import psnr, ssim
-from .net import _model_engines, _model_engines_lock, _PackedWeightsMixin, _param_version
+from .net import TRAIN_PRECISIONS, _model_engines, _model_engines_lock, _PackedWeightsMixin, _param_version
 
 TRAIN_METRICS_NAMES = ["mse", "ssim", "psnr", "perceptual_loss", "loss"]
 VAL_METRICS_NAMES = ["mse", "ssim", "psnr", "perceptual_loss"]
@@ -39,16 +39,25 @@ class PerceptualModel(_PackedWeightsMixin, nn.Module):
     """VGG19 ``features`` without the final max-pool (train.py:254-263).
 
     ``native=True``: on CUDA tensors ``perceptual_loss(vgg, out, ref)`` is one ``wn_perceptual_loss`` call -- the
-    loss and d(loss)/d(out) on the tensor cores (bf16x3), in windows that own ``tile`` input pixels of features
+    loss and d(loss)/d(out) on the tensor cores (``precision``), in windows that own ``tile`` input pixels of features
     (None: one window per image; an image over 8 Mi pixels then needs a tile), so memory is bounded by one pass
     whatever the image and batch size.  Autograd keeps only d(out), 12 bytes per pixel; no VGG weight gradient is
     computed (the VGG parameters' ``.grad`` stays untouched) and ``ref`` is a constant.  ``native=False`` and CPU
-    tensors evaluate the torch expression."""
+    tensors evaluate the torch expression.
 
-    def __init__(self, pretrained: bool = True, native: bool = False, tile=None):
+    ``precision``: the arithmetic of the native calls' 32 VGG convolutions.  "bf16x3" (default) issues three bf16
+    tensor-core products per product; "bf16" issues one, a_hi x w_hi with fp32 accumulation, as autocast runs a frozen
+    VGG (DESIGN.md 4.14).  "bf16" needs ``native=True``: the torch expression has its own arithmetic.  Read at every
+    call, so a change takes effect at the next one."""
+
+    precision = "bf16x3"  # class default: a module pickled before the attribute existed loads as bf16x3
+
+    def __init__(self, pretrained: bool = True, native: bool = False, tile=None, precision: str = "bf16x3"):
         super().__init__()
         self.native = native
         self.tile = tile
+        self.precision = precision
+        self._train_mode()
         import torchvision
         vgg = None
         if pretrained:
@@ -65,6 +74,16 @@ class PerceptualModel(_PackedWeightsMixin, nn.Module):
 
     def forward(self, x):
         return self.model(x)
+
+    def _train_mode(self) -> int:
+        """The wn_set_train_mode of ``precision`` for the native calls; ValueError for an unknown value or for "bf16"
+        without ``native``."""
+        if self.precision not in TRAIN_PRECISIONS:
+            raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(TRAIN_PRECISIONS)}")
+        if self.precision != "bf16x3" and not self.native:
+            raise ValueError(f"precision={self.precision!r} needs native=True: the torch expression (native=False) "
+                             "has its own arithmetic")
+        return TRAIN_PRECISIONS[self.precision]
 
     def vgg_params(self):
         """Weight and bias of the 16 convolutions in ``features`` order."""
@@ -97,7 +116,8 @@ class _NativePerceptualLoss(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, out, ref, vgg, want_grad):
-        loss, grad = vgg._vgg_engine(out).perceptual_loss(out, ref, tile=vgg.tile, want_grad=want_grad)
+        loss, grad = vgg._vgg_engine(out).perceptual_loss(out, ref, tile=vgg.tile, want_grad=want_grad,
+                                                          train_mode=vgg._train_mode())
         if grad is not None:
             ctx.save_for_backward(grad)
         return loss
@@ -109,7 +129,8 @@ class _NativePerceptualLoss(torch.autograd.Function):
 
 
 def add_perceptual_args(ap) -> None:
-    """``--perceptual {torch,native}`` and ``--perceptual-tile N`` of train.py and score.py."""
+    """``--perceptual {torch,native}``, ``--perceptual-tile N`` and ``--perceptual-precision {bf16x3,bf16}`` of train.py
+    and score.py."""
     ap.add_argument("--perceptual", default="torch", choices=["torch", "native"],
                     help="(Optional) torch: the perceptual loss as the torch VGG19 expression (default); native: the "
                          "loss and its gradient on the library's kernels in overlapping windows "
@@ -117,16 +138,30 @@ def add_perceptual_args(ap) -> None:
     ap.add_argument("--perceptual-tile", type=int, default=None, metavar="N",
                     help="(Optional) needs --perceptual native: windows owning N x N input pixels of VGG features "
                          "(rounded up to a multiple of 16).  Unset: one window per image")
+    ap.add_argument("--perceptual-precision", default=None, choices=sorted(TRAIN_PRECISIONS),
+                    help="(Optional) needs --perceptual native: the arithmetic of the VGG convolutions "
+                         "(PerceptualModel.precision), bf16x3 (default, three bf16 tensor-core products per product) "
+                         "or bf16 (one, fp32 accumulation).  --train-precision does not set it")
 
 
 def perceptual_model(args) -> PerceptualModel:
-    """The PerceptualModel the command-line arguments of ``add_perceptual_args`` ask for; --perceptual-tile without
-    --perceptual native is refused (the torch expression has no windows)."""
+    """The PerceptualModel the command-line arguments of ``add_perceptual_args`` ask for; --perceptual-tile and
+    --perceptual-precision without --perceptual native are refused (the torch expression has no windows and its own
+    arithmetic)."""
     if args.perceptual_tile is not None and args.perceptual != "native":
         raise SystemExit("--perceptual-tile needs --perceptual native")
     if args.perceptual_tile is not None and args.perceptual_tile <= 0:
         raise SystemExit("--perceptual-tile must be positive")
-    return PerceptualModel(native=args.perceptual == "native", tile=args.perceptual_tile)
+    if args.perceptual_precision is not None and args.perceptual != "native":
+        raise SystemExit("--perceptual-precision needs --perceptual native")
+    return PerceptualModel(native=args.perceptual == "native", tile=args.perceptual_tile,
+                           precision=perceptual_config(args)["perceptual_precision"])
+
+
+def perceptual_config(args) -> dict:
+    """The perceptual-loss settings of ``add_perceptual_args`` as train.py records them in config.json."""
+    return {"perceptual": args.perceptual, "perceptual_tile": args.perceptual_tile,
+            "perceptual_precision": args.perceptual_precision or "bf16x3"}
 
 
 def _normalize(x):
