@@ -213,6 +213,7 @@ struct FwdOpts {
   long long win0 = 0;               // last launch stores its kept rectangle into out / out_u8 at image coordinates
   const RaggedWindow* rwin = nullptr;  // ragged pass (device table): image n of the batch is window rwin[n] in its
                                        // slot; every layer masks it, the last launch stores into its own image
+  const int* slot_levels = nullptr;    // ragged fp32 pass: slot n holds 8-bit levels only (ConvArgs::slot_levels)
 };
 int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out, int n,
                         int height, int width, const FwdBuffers& b, cudaStream_t stream,
@@ -279,7 +280,7 @@ inline PackInArgs pack_args(const float* const in[4], const int64_t st[4][4]) {
 int pack_inputs(wn_handle* h, const GridGeom& geo, const PackInArgs& in, int count, uint4* act0, int* flag,
                 cudaStream_t stream, bool hi = false);
 int pack_inputs(wn_handle* h, const TableGeom& geo, const PackInArgs* imgs, int count, uint4* act0, int* flag,
-                cudaStream_t stream, bool hi = false);
+                cudaStream_t stream, bool hi = false, int* slot_flags = nullptr);
 // wn_forward_ragged (arguments checked by the caller, api.cu): the windows and passes of ragged_plan
 size_t umma_forward_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
                                            long long max_pass_pixels);

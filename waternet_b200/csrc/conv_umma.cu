@@ -80,8 +80,8 @@ __device__ __forceinline__ bool pack_slot_pixel(const PackInArgs* __restrict__ i
 // slot's act0 planes (zeros beyond the valid extent).  FLAG: *exact_flag is cleared unless every valid pixel is an
 // 8-bit level.  Whole images (GridGeom tile = image size) take both in one launch; the windowed calls take the flag
 // once per call over whole images (or over every pass of a ragged plan) and then the planes per pass.  HI: the planes
-// of the single-pass bf16 training forward, lo = 0.
-template <class Geom, class In, bool PLANES, bool FLAG, bool HI = false>
+// of the single-pass bf16 training forward, lo = 0.  SLOT: the flag is one per slot, exact_flag[blockIdx.y].
+template <class Geom, class In, bool PLANES, bool FLAG, bool HI = false, bool SLOT = false>
 __global__ void __launch_bounds__(256)
 pack_inputs_kernel(Geom geo, In in, uint4* __restrict__ out, int* __restrict__ exact_flag) {
   const int pix = blockIdx.x * 256 + threadIdx.x;
@@ -96,7 +96,7 @@ pack_inputs_kernel(Geom geo, In in, uint4* __restrict__ out, int* __restrict__ e
     if constexpr (PLANES) store_packed<HI>(out + (size_t)blockIdx.y * 4 * hw + pix, hw, v);
   }
   if constexpr (FLAG)
-    if (!__syncthreads_and(exact) && threadIdx.x == 0) atomicExch(exact_flag, 0);
+    if (!__syncthreads_and(exact) && threadIdx.x == 0) atomicExch(exact_flag + (SLOT ? blockIdx.y : 0), 0);
 }
 
 // reset: *flag is set to 1 ("all inputs are 8-bit levels") first, inside the packing's timing slot
@@ -120,10 +120,20 @@ int pack_inputs(wn_handle* h, const GridGeom& geo, const PackInArgs& in, int cou
   return launch_pack<true, false>(h, geo, in, count, act0, nullptr, false, stream, hi);
 }
 // a ragged call takes its flag over every pass before the first, so it never asks for both in one launch, and the
-// caller sets the flag once before the first of those launches
+// caller sets the flag once before the first of those launches.  slot_flags (fp8-correction scheme): with the planes,
+// one flag per slot, set to 1 here and cleared unless the slot holds 8-bit levels only
 int pack_inputs(wn_handle* h, const TableGeom& geo, const PackInArgs* imgs, int count, uint4* act0, int* flag,
-                cudaStream_t stream, bool hi) {
+                cudaStream_t stream, bool hi, int* slot_flags) {
   if (!act0) return launch_pack<false, true>(h, geo, imgs, count, nullptr, flag, false, stream);
+  if (slot_flags) {
+    TimedScope ts(h, kSlotPack, stream);
+    WN_CUDA(cudaMemsetAsync(slot_flags, 1, (size_t)count * sizeof(int), stream));
+    const dim3 grid((unsigned)(((size_t)geo.slot_hw() + 255) / 256), count);
+    pack_inputs_kernel<TableGeom, const PackInArgs*, true, true, false, true><<<grid, 256, 0, stream>>>(geo, imgs, act0,
+                                                                                                      slot_flags);
+    WN_LAUNCH_CHECK(h);
+    return WN_OK;
+  }
   return launch_pack<true, false>(h, geo, imgs, count, act0, nullptr, false, stream, hi);
 }
 
@@ -190,6 +200,12 @@ static constexpr int layer_wgs(int) { return 2; }
 static constexpr int layer_wgs(int li) { return kSpecs[li].wgs; }
 #endif
 
+// The first layer's fp8-correction form is its tap-pair form (UmmaCfg kFmtPair8): one e4m3 wgmma for the w_lo
+// corrections of two taps, for 8-bit-level inputs; other inputs run its bf16x3 form in the same launch.
+static constexpr bool pairs_taps(int li) { return li == kL1; }
+static constexpr size_t kPairImageBytes = (size_t)((49 + 1) / 2 + 49) * 224 * 32;  // kL1's tap-pair weight image
+static constexpr size_t kPairScaleBytes = 2 * 224 * sizeof(float);                // s_c, then 2^-9 / s_c
+
 // In the fp8-correction scheme a layer writes the hi + fp8-planes format (FMT bit 1) when its consumers read it with
 // their fp8 form.  L1 feeds C2 and R2; every other layer feeds the next one, except the last layer of each stack.
 static_assert(kSpecs[kC2].f8 == kSpecs[kR2].f8, "L1 writes one format for both of its consumers");
@@ -219,8 +235,8 @@ int mirror_u8(wn_handle* h, const uint8_t* src, const PeerOut& peers, size_t byt
 }
 
 struct UmmaWeights {
-  uint8_t* stages8[kNumUmmaLayers];  // fp8-correction weight images (layers with an fp8 form)
-  float* scale8[kNumUmmaLayers];     // {ws, 2^-9 / ws, max|w|, -}
+  uint8_t* stages8[kNumUmmaLayers];  // fp8-correction weight images (layers with an fp8 form; kL1: tap pairs)
+  float* scale8[kNumUmmaLayers];     // {ws, 2^-9 / ws, max|w|, -}; kL1: per-column scales (pair_scale_kernel)
   int* overflow_dev;                 // sticky: an activation left the e4m3 range in the fp8-correction mode
   int* overflow_host;                // pinned mirror, refreshed at the end of every forward of that mode
   uint8_t* stages[kNumUmmaLayers];
@@ -236,9 +252,11 @@ int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t str
   for (int i = 0; i < kNumUmmaLayers; i++) {  // (re)allocate whatever an earlier, failed call left unallocated
     if (!h->umma->stages[i]) WN_CUDA(cudaMalloc(&h->umma->stages[i], stage_bytes_total(kSpecs[i])));
     if (!h->umma->bias[i]) WN_CUDA(cudaMalloc(&h->umma->bias[i], kSpecs[i].npad * kSpecs[i].nblk * sizeof(float)));
-    if (kSpecs[i].f8) {
-      if (!h->umma->stages8[i]) WN_CUDA(cudaMalloc(&h->umma->stages8[i], stage_bytes_total(kSpecs[i])));
-      if (!h->umma->scale8[i]) WN_CUDA(cudaMalloc(&h->umma->scale8[i], 4 * sizeof(float)));
+    if (kSpecs[i].f8 || pairs_taps(i)) {
+      const size_t img = pairs_taps(i) ? kPairImageBytes : stage_bytes_total(kSpecs[i]);
+      if (!h->umma->stages8[i]) WN_CUDA(cudaMalloc(&h->umma->stages8[i], img));
+      const size_t sc = pairs_taps(i) ? kPairScaleBytes : 4 * sizeof(float);
+      if (!h->umma->scale8[i]) WN_CUDA(cudaMalloc(&h->umma->scale8[i], sc));
     }
   }
   if (!h->umma->dense) WN_CUDA(cudaMalloc(&h->umma->dense, (size_t)224 * 128 * 49 * sizeof(float)));
@@ -287,6 +305,14 @@ int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t str
     for (int g = 0; g < s.ng; g++) {
       pack_stages_kernel<<<256, 256, 0, stream>>>(u->dense, (__nv_bfloat16*)(u->stages[li] + g * group_bytes), gw,
                                                   s.cinpad, kk, s.concat, s.nblk, g * gw);
+      WN_LAUNCH_CHECK(h);
+    }
+    if (pairs_taps(li)) {
+      static_assert(kSpecs[kL1].cinpad == 16 && kSpecs[kL1].ng == 1 && kSpecs[kL1].nblk == 1 && kSpecs[kL1].npad == 224 &&
+                    kSpecs[kL1].ks == 7, "kPairImageBytes");
+      pair_scale_kernel<<<s.npad, 256, 0, stream>>>(u->dense, u->scale8[li], s.npad, s.cinpad * kk);
+      WN_LAUNCH_CHECK(h);
+      pack_stages_pair_kernel<<<64, 256, 0, stream>>>(u->dense, u->stages8[li], u->scale8[li], s.npad, kk);
       WN_LAUNCH_CHECK(h);
     }
     if (s.f8) {
@@ -356,9 +382,13 @@ static int launch_layer_as(wn_handle* h, int scheme, void* in_base, ConvArgs a, 
     return launch_conv<s.ks, s.cinpad, GW, s.epi, s.concat, s.nblk, s.tps, kFmtHi, R, s.mw, s.ng, layer_wgs(LI)>(
         h, s.slot, u->stages[LI], u->bias[LI], in_base, a, stream);
   if (scheme == 1) {
-    constexpr int FMT = (s.f8 ? kFmtIn8 : 0) | (writes_f8(LI) ? kFmtOut8 : 0);
+    constexpr int FMT = (s.f8 ? kFmtIn8 : 0) | (writes_f8(LI) ? kFmtOut8 : 0) | (pairs_taps(LI) ? kFmtPair8 : 0);
     if constexpr ((FMT & kFmtOut8) != 0) a.f8_overflow = u->overflow_dev;
     if constexpr (s.f8) a.f8_scale = u->scale8[LI] + 1;
+    if constexpr (pairs_taps(LI)) {
+      a.f8_scale = u->scale8[LI] + s.npad;
+      a.wpk8 = u->stages8[LI];
+    }
     return launch_conv<s.ks, s.cinpad, GW, s.epi, (s.f8 ? 0 : s.concat), s.nblk, s.tps, FMT, R, s.mw, s.ng,
                        layer_wgs(LI)>(h, s.slot, s.f8 ? u->stages8[LI] : u->stages[LI], u->bias[LI], in_base, a, stream);
   }
@@ -463,6 +493,7 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   const bool want_cmg = o.stack != kStackRefiners, want_ref = o.stack != kStackCmg;
   a.skip_lo = b.exact_flag;
   a.a_hi_only = o.hi_only ? 1 : 0;
+  a.slot_levels = o.slot_levels;
   if (o.refiner_l1) {  // the refiners' conv1 alone, bf16x3 or single-pass bf16 (the sums of kL1's refiner columns)
     constexpr UmmaLayerSpec s = kSpecs[kRL1];
     act(b.r[1], 96, nullptr, 0);
@@ -480,6 +511,7 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   }
   a.skip_lo = nullptr;
   a.a_hi_only = 0;
+  a.slot_levels = nullptr;
   if (dump(kL1)) return WN_OK;
   if (want_cmg) {
     act(b.a[2], 128, nullptr, 0);
@@ -603,6 +635,11 @@ int umma_forward(wn_handle* h, const float* const in[4], const int64_t in_stride
   if (rc) return rc;
   scheme = effective_scheme(h, scheme);
   const int nb = umma_chunk(h->chunk_pixels, n, H, W);
+  // Several passes: whether the first layer runs its level form is decided once, over every input pixel of the n
+  // images, so that the result does not depend on how the batch is split (the tiled and ragged calls decide so too).
+  // The flag sits where a full pass puts it, beyond the buffers of any smaller pass.
+  int* flag = nb < n ? carve(workspace, nb, H, W).exact_flag : nullptr;
+  if (flag && (rc = pack_inputs(h, whole_images(H, W), pack_args(in, in_strides), n, nullptr, flag, stream))) return rc;
   for (int n0 = 0; n0 < n; n0 += nb) {
     const int cur = n - n0 < nb ? n - n0 : nb;
     const float* sub[4];
@@ -611,6 +648,13 @@ int umma_forward(wn_handle* h, const float* const in[4], const int64_t in_stride
     FwdOpts o;
     o.scheme = scheme;
     o.stack = stack;
+    if (flag) {
+      b.exact_flag = flag;
+      o.packed = true;
+      if ((rc = pack_inputs(h, whole_images(H, W), pack_args(sub, in_strides), cur, b.act0, nullptr, stream,
+                            scheme == kSchemeBf16)))
+        return rc;
+    }
       float* dst = out + (size_t)n0 * 3 * H * W;
     if (stack == kStackCmg) b.cm = dst;                                   // the maps are the result
     if (stack == kStackRefiners) { b.refined = refined + (size_t)n0 * 9 * H * W; dst = nullptr; }
@@ -961,11 +1005,15 @@ int umma_forward_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, in
     FwdBuffers b = carve(fwd_ws, p.count, p.slot_h, p.slot_w);
     b.exact_flag = exact;
     geo.set_pass(p);
-    if ((rc = pack_inputs(h, geo, d_imgs, p.count, b.act0, nullptr, stream))) return rc;
+    // the fp8-correction scheme decides the first layer's form per window (kFmtPair8): its flags sit in the buffer
+    // of cmg.conv2's output, which nothing reads or writes before the first layer has run
+    int* slot_flags = scheme == 1 ? reinterpret_cast<int*>(b.a[2]) : nullptr;
+    if ((rc = pack_inputs(h, geo, d_imgs, p.count, b.act0, nullptr, stream, false, slot_flags))) return rc;
     FwdOpts o;
     o.scheme = scheme;
     o.packed = true;
     o.rwin = geo.rwin();
+    o.slot_levels = slot_flags;
     rc = umma_pass(h, no_in, none, nullptr, p.count, p.slot_h, p.slot_w, b, stream, o);
     if (rc) return rc;
   }

@@ -116,6 +116,15 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 //        N = NPAD (a CONCAT layer takes the hi rows of its [hi | lo] stage rows), fp32 accumulation.  The a_lo and w_lo
 //        products are never issued and the halo loads fetch the two hi planes of a chunk only.  kEpiAct / kEpiDgrad
 //        store lo = 0, so every plane buffer of that mode holds exactly the bf16 operand its consumers multiply.
+//        bit 3 (kFmtPair8): the first layer's fp8 tap-pair form, for 8-bit-level inputs (*skip_lo set, or the tile's
+//        entry of slot_levels; otherwise the tile runs the bf16x3 form of FMT 0 from ConvArgs::wpk).  A level a is exact in bf16, so only a x w_lo has
+//        to be added to a x w_hi, and it is ONE e4m3 wgmma of K = 32 per PAIR of taps: the two 16-byte core matrices
+//        of a K = 32 row are the 16 channels of two taps of the same halo plane, one descriptor LBO apart (pair table
+//        in the consumer).  The consumers convert the halo tile's hi planes to e4m3 in shared memory themselves.
+//        Per tile and warpgroup: 25 e4m3 wgmmas (all of them first: the accumulator holds only correction sums while
+//        the fp8 MMA, which adds with fewer bits than fp32, adds into it), then 49 bf16 wgmmas a x w_hi; the weights
+//        (ConvArgs::wpk8) are scaled by s_c 2^9 per output column c (a power of two) and the epilogue multiplies
+//        column c by 2^-9 / s_c (ConvArgs::f8_scale[c]).  74 bf16-pass equivalents instead of 98.
 // MW     m64 blocks per warpgroup: 1 = 8 x 16-pixel tile (M = 128), 2 = 16 x 16 (M = 256).  Every weight stage a
 //        CTA streams from L2 then serves twice the pixels.
 // NG     column groups: a CTA computes the NPAD output channels [g * NPAD, (g + 1) * NPAD) of column group g; the
@@ -126,13 +135,14 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 //        warpgroup serves every weight stage to 192 pixels instead of 128 without more accumulators per thread; at
 //        512 threads the register file allows 128 per thread, so the producer warpgroup gives its registers up
 //        (setmaxnreg) and the consumers run at kWgs3ConsumerRegs.
-constexpr int kFmtIn8 = 1, kFmtOut8 = 2, kFmtHi = 4;
+constexpr int kFmtIn8 = 1, kFmtOut8 = 2, kFmtHi = 4, kFmtPair8 = 8;
 constexpr int kWgs3ProducerRegs = 24, kWgs3ConsumerRegs = 160;  // 128 x 24 + 384 x 160 <= 65,536
 template <int KS, int CIN_PAD, int NPAD, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0, int MW = 1,
           int NG = 1, int WGS = 2>
 struct UmmaCfg {
   static constexpr bool F8IN = (FMT & kFmtIn8) != 0;
   static constexpr bool HI = (FMT & kFmtHi) != 0;
+  static constexpr bool PAIR = (FMT & kFmtPair8) != 0;
   static constexpr bool DUAL = CONCAT != 0 && !HI;  // two accumulator halves per block: [a x w_hi | a_hi x w_lo]
   static constexpr int TILE_W = 8 * MW, TILE_H = 8 * WGS;
   static constexpr int CONSUMER_WARPS = 4 * WGS;                  // arrivals per "stage empty"
@@ -150,7 +160,8 @@ struct UmmaCfg {
   static constexpr int NSTAGE_PER_CHUNK = KS * KS / TPS;
   static constexpr int STAGING = WGS * 64 * kStageLd * 4;
   // barriers (512 B) + the biases of every column group: 2048 B, more for layers over 384 channels (VGG's 512)
-  static constexpr int BIAS_BYTES = NG * NBLK * NPAD * 4;
+  // (kFmtPair8: the per-column dequantisation factors follow the biases)
+  static constexpr int BIAS_BYTES = NG * NBLK * NPAD * 4 * (PAIR ? 2 : 1);
   static constexpr int TAIL = 512 + (BIAS_BYTES > 1536 ? BIAS_BYTES : 1536);
   static constexpr int BUDGET = 227 * 1024 - 1024 - TAIL - STAGING;
   // halo ring: enough stages to prefetch the next chunk (or the next tile when there is one chunk)
@@ -163,6 +174,13 @@ struct UmmaCfg {
   static constexpr int NA = NA_FIT > NA_WANT ? NA_WANT : NA_FIT;
   static_assert(!F8IN || !CONCAT, "fp8 corrections: the [hi | second part] weight layout");
   static_assert(!HI || FMT == kFmtHi, "single-pass bf16 reads and writes bf16 planes only");
+  // kFmtPair8: one chunk of 16 channels, one tap per bf16x3 stage; warpgroup w converts its halo rows into plane 2 + w
+  static_assert(!PAIR || (CIN_PAD == 16 && !CONCAT && NBLK == 1 && TPS == 1 && MW == 1 && NG == 1 && WGS == 2 &&
+                          !F8IN && !HI), "the tap-pair form is the first layer's");
+  static constexpr int PAIRS = (KS * KS + 1) / 2;           // e4m3 wgmmas per tile (the last tap pairs with a zero)
+  static constexpr int PAIR_UNITS = PAIRS + KS * KS;        // units of NPAD * 32 B: e4m3 pairs, then bf16 taps
+  static constexpr int PAIR_STAGES = PAIR_UNITS / 2;        // two units per weight stage of B_STAGE bytes
+  static_assert(!PAIR || PAIR_UNITS % 2 == 0, "whole weight stages");
   static constexpr int CPB = NCHUNK / NBLK;                // chunks per diagonal block
   static constexpr int BLK_COLS = DUAL ? 2 * NPAD : NPAD;   // accumulator columns per block
   static constexpr int COLS = NBLK * BLK_COLS;             // accumulator columns of the tile
@@ -210,8 +228,14 @@ struct ConvArgs {
   // kEpiDgrad: saved forward activation (planes) whose zeros gate the gradient
   const uint4* mask_base;
   int mask_planes_half;
-  // fp8 correction scheme (FMT bit 0): dequantisation factor 2^-9 / ws of the accumulator
+  // fp8 correction scheme (FMT bit 0): dequantisation factor 2^-9 / ws of the accumulator; kFmtPair8: one factor
+  // 2^-9 / s_c per output column
   const float* f8_scale;
+  // kFmtPair8: the tap-pair weight image (pack_stages_pair_kernel), streamed instead of wpk for level inputs
+  const uint8_t* wpk8;
+  // kFmtPair8, optional: per image of the launch, nonzero when it holds 8-bit levels only.  A ragged pass decides
+  // the form per window with it (its windows come from images of every kind); otherwise *skip_lo decides
+  const int* slot_levels;
   // FMT bit 1: sticky device flag raised when an activation leaves the e4m3 range (its correction terms would
   // saturate in the consumer's fp8 pass); the host side then re-runs the batch with the bf16x3 kernels
   int* f8_overflow;
@@ -419,7 +443,17 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int i = tid; i < NG * NBLK * NPAD; i += C::THREADS) s_bias[i] = g.bias[i];
+  if constexpr (C::PAIR)
+    for (int i = tid; i < NPAD; i += C::THREADS) s_bias[NPAD + i] = g.f8_scale[i];
   __syncthreads();
+  // kFmtPair8: the tap-pair form runs on tiles of 8-bit levels (decided per call on the device, like the a_lo pass,
+  // or per image with slot_levels); the B producer and the consumers take the same decision
+  const bool levels = (g.skip_lo != nullptr && *g.skip_lo != 0) || g.a_hi_only;
+  auto pair_tile = [&](int tile) {
+    if (!C::PAIR) return false;
+    if (g.a_hi_only || g.slot_levels == nullptr) return levels;
+    return g.slot_levels[tile / NG / (g.tiles_x * g.tiles_y)] != 0;
+  };
   // WGS = 3: the producer warpgroup gives registers up, the consumer warpgroups take them; each setmaxnreg sits at
   // one place that dominates the code of its role, so that ptxas compiles the consumers for kWgs3ConsumerRegs
   if constexpr (WGS == 3) {
@@ -459,8 +493,10 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const uint8_t* wpk = g.wpk + (size_t)(tile % NG) * C::GROUP_BYTES;
-        for (int it = 0; it < C::NCHUNK * C::NSTAGE_PER_CHUNK; it++) {
+        const bool pair = pair_tile(tile);
+        const uint8_t* wpk = pair ? g.wpk8 : g.wpk + (size_t)(tile % NG) * C::GROUP_BYTES;
+        const int nit = pair ? C::PAIR_STAGES : C::NCHUNK * C::NSTAGE_PER_CHUNK;
+        for (int it = 0; it < nit; it++) {
           mbar_wait(&b_empty[stage], phase ^ 1);
           mbar_expect_tx(&b_full[stage], C::B_STAGE);
           bulk_load(b_stages + stage * C::B_STAGE, wpk + (size_t)it * C::B_STAGE, C::B_STAGE, &b_full[stage]);
@@ -474,7 +510,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
 
   // ===================== consumers: wgmma, then the epilogue of the warpgroup's 64 rows =====================
   const int wg = warp >> 2, wtid = tid & 127;
-  const bool skip_lo = (g.skip_lo != nullptr && *g.skip_lo != 0) || g.a_hi_only;
+  const bool skip_lo = levels;
   // WGS = 3 reads the fp8 dequantisation factor in the epilogue: one register less across the main loop
   const float dscale0 = F8IN && WGS == 2 ? *g.f8_scale : 1.f;
   // A operand: rows of the tile = pixels, 8 consecutive pixels of a halo row = one core matrix; this warpgroup's
@@ -495,6 +531,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     pend_a = pend_b = -1;
   };
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const bool pair = pair_tile(tile);
 #pragma unroll
     for (int mb = 0; mb < MW; mb++) {
 #pragma unroll
@@ -508,51 +545,115 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
       mbar_wait(&a_full[astage], aphase);
       const uint32_t a_base = smem_u32(a_stages + astage * C::A_STAGE) + (uint32_t)(wg * 8 * C::HALO_W * 16);
       const int blk = NBLK > 1 ? c / C::CPB : 0;
-      for (int tg = 0; tg < C::NSTAGE_PER_CHUNK; tg++) {
+      if constexpr (C::PAIR) {
+        if (pair) {
+          // the e4m3 operand: warpgroup wg converts the two hi planes of its 14 halo rows (8 wg ..) into plane 2 + wg
+          // of the stage, at the same offsets (those planes hold lo planes or nothing, unused when the inputs are
+          // levels); then the async proxy may read them
+          uint8_t* st = a_stages + astage * C::A_STAGE;
+          for (int p = wtid; p < (8 + KS - 1) * C::HALO_W; p += 128) {
+            const size_t o = (size_t)(wg * 8 * C::HALO_W + p) * 16;
+            const uint4 h0 = *reinterpret_cast<const uint4*>(st + o);
+            const uint4 h1 = *reinterpret_cast<const uint4*>(st + C::PLANE_BYTES + o);
+            const uint32_t hw[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+            uint32_t q[4];
+#pragma unroll
+            for (int j = 0; j < 4; j++)
+              q[j] = pack_e4m3x4(__uint_as_float(hw[2 * j] << 16), __uint_as_float(hw[2 * j] & 0xffff0000u),
+                                 __uint_as_float(hw[2 * j + 1] << 16), __uint_as_float(hw[2 * j + 1] & 0xffff0000u));
+            *reinterpret_cast<uint4*>(st + (2 + wg) * C::PLANE_BYTES + o) = make_uint4(q[0], q[1], q[2], q[3]);
+          }
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          wg_bar(1 + wg);
+        }
+      }
+      // one weight stage: wait for it, issue its wgmmas (body), commit; its release waits for the next stage's group
+      auto stage = [&](bool last_of_chunk, auto&& body) {
         mbar_wait(&b_full[bstage], bphase);
         const uint32_t b_base = smem_u32(b_stages + bstage * C::B_STAGE);
         wg_fence();
-#pragma unroll
-        for (int t = 0; t < TPS; t++) {
-          const int tap = tg * TPS + t;
-          const int ky = tap / KS, kx = tap - ky * KS;
-          const uint32_t a_tap = a_base + (uint32_t)((ky * C::HALO_W + kx) * 16);
-          const uint32_t b_tap = b_base + (uint32_t)(t * C::B_TAP);
-          // MW = 2: block mb is the same descriptor 8 pixels further, as an add to the start-address field (that of a
-          // shared-memory address never carries into the next field); fewer live descriptors than building each anew
-          const uint64_t a_hi0 = make_desc(a_tap, C::PLANE_BYTES, kSboA);
-#pragma unroll
-          for (int mb = 0; mb < MW; mb++) {
-            const uint64_t a_hi = a_hi0 + mb * (128 >> 4);
-            const uint64_t a_lo = MW == 1 ? make_desc(a_tap + 2 * C::PLANE_BYTES, C::PLANE_BYTES, kSboA)
-                                          : a_hi + ((2 * C::PLANE_BYTES) >> 4);
-#pragma unroll
-            for (int b = 0; b < NBLK; b++) {
-              if (NBLK > 1 && b != blk) continue;
-              float* d = acc[mb] + b * C::BLK_COLS / 2;
-              if constexpr (C::HI) {
-                wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));                // a_hi x w_hi
-              } else if constexpr (F8IN) {
-                // w_hi * ws * 2^9 (bf16, K = 16), then [e4m3(lo*2^9) | e4m3(v)] x [e4m3(w*ws) ; e4m3(w_lo*ws*2^9)] (K = 32)
-                wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, NPAD * 16, 128));
-                wgmma_e4m3<NPAD>(acc8[mb] + b * C::BLK_COLS / 2, a_lo, make_desc(b_tap + NPAD * 32, NPAD * 16, 128));
-              } else if constexpr (CONCAT) {
-                wgmma_bf16<2 * NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));            // a_hi x [w_hi | w_lo]
-                if (!skip_lo) wgmma_bf16<NPAD>(d, a_lo, make_desc(b_tap, kLboB, 128));  // a_lo x w_hi
-              } else {
-                wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));                // a_hi x w_hi
-                if (!skip_lo) wgmma_bf16<NPAD>(d, a_lo, make_desc(b_tap, kLboB, 128));  // a_lo x w_hi
-                wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap + 2 * NPAD * 16, kLboB, 128));  // a_hi x w_lo
-              }
-            }
-          }
-        }
+        body(b_base);
         wg_commit();
         wg_wait<1>();
         release();
         pend_b = bstage;
-        if (tg == C::NSTAGE_PER_CHUNK - 1) pend_a = astage;
+        if (last_of_chunk) pend_a = astage;
         if (++bstage == C::NB) { bstage = 0; bphase ^= 1; }
+      };
+      bool issued = false;
+      if constexpr (C::PAIR) {
+        if (pair) {
+          // unrolled, so that each unit's wgmma is known at compile time (ptxas serialises wgmmas behind a branch
+          // on the unit index)
+#pragma unroll
+          for (int tg = 0; tg < C::PAIR_STAGES; tg++) {
+            stage(tg == C::PAIR_STAGES - 1, [&](uint32_t b_base) {
+              // units 2 tg, 2 tg + 1 of [25 e4m3 pairs | 49 bf16 taps].  Pair p: taps t0 = min(2p, 47) and t0 + 1, one
+              // descriptor from tap t0 with LBO = the distance to tap t0 + 1 (16 B along a kernel row, one halo row
+              // minus 6 pixels across rows); pair 24 is taps 47 (zero weights) and 48, so that no read leaves the rows
+              // of the warpgroup.  Every wgmma has N = NPAD, B = [K half][NPAD rows][16 B], LBO NPAD * 16.
+#pragma unroll
+              for (int j = 0; j < 2; j++) {
+                const int u = 2 * tg + j;
+                const uint32_t b_unit = b_base + (uint32_t)(j * NPAD * 32);
+                if (u < C::PAIRS) {
+                  const int t0 = 2 * u < KS * KS - 2 ? 2 * u : KS * KS - 2, t1 = t0 + 1;
+                  const uint32_t o0 = (uint32_t)(((t0 / KS) * C::HALO_W + t0 % KS) * 16);
+                  const uint32_t o1 = (uint32_t)(((t1 / KS) * C::HALO_W + t1 % KS) * 16);
+                  // (N = 32 where the form is compiled out: the e4m3 shapes other layers need are generated)
+                  const uint32_t a_pair = a_base + (2 + wg) * C::PLANE_BYTES + o0;
+                  wgmma_e4m3<C::PAIR ? NPAD : 32>(acc[0], make_desc(a_pair, o1 - o0, kSboA), make_desc(b_unit, NPAD * 16, 128));
+                } else {
+                  const int tap = u - C::PAIRS;
+                  const uint32_t a_tap = a_base + (uint32_t)(((tap / KS) * C::HALO_W + tap % KS) * 16);
+                  wgmma_bf16<NPAD>(acc[0], make_desc(a_tap, C::PLANE_BYTES, kSboA), make_desc(b_unit, NPAD * 16, 128));
+                }
+              }
+            });
+          }
+          issued = true;
+        }
+      }
+      if (!issued) {
+        for (int tg = 0; tg < C::NSTAGE_PER_CHUNK; tg++) {
+          stage(tg == C::NSTAGE_PER_CHUNK - 1, [&](uint32_t b_base) {
+#pragma unroll
+            for (int t = 0; t < TPS; t++) {
+              const int tap = tg * TPS + t;
+              const int ky = tap / KS, kx = tap - ky * KS;
+              const uint32_t a_tap = a_base + (uint32_t)((ky * C::HALO_W + kx) * 16);
+              const uint32_t b_tap = b_base + (uint32_t)(t * C::B_TAP);
+              // MW = 2: block mb is the same descriptor 8 pixels further, as an add to the start-address field (that of a
+              // shared-memory address never carries into the next field); fewer live descriptors than building each anew
+              const uint64_t a_hi0 = make_desc(a_tap, C::PLANE_BYTES, kSboA);
+#pragma unroll
+              for (int mb = 0; mb < MW; mb++) {
+                const uint64_t a_hi = a_hi0 + mb * (128 >> 4);
+                const uint64_t a_lo = MW == 1 ? make_desc(a_tap + 2 * C::PLANE_BYTES, C::PLANE_BYTES, kSboA)
+                                              : a_hi + ((2 * C::PLANE_BYTES) >> 4);
+#pragma unroll
+                for (int b = 0; b < NBLK; b++) {
+                  if (NBLK > 1 && b != blk) continue;
+                  float* d = acc[mb] + b * C::BLK_COLS / 2;
+                  if constexpr (C::HI) {
+                    wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));                // a_hi x w_hi
+                  } else if constexpr (F8IN) {
+                    // w_hi * ws * 2^9 (bf16, K = 16), then [e4m3(lo*2^9) | e4m3(v)] x [e4m3(w*ws) ; e4m3(w_lo*ws*2^9)] (K = 32)
+                    wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, NPAD * 16, 128));
+                    wgmma_e4m3<NPAD>(acc8[mb] + b * C::BLK_COLS / 2, a_lo, make_desc(b_tap + NPAD * 32, NPAD * 16, 128));
+                  } else if constexpr (CONCAT) {
+                    wgmma_bf16<2 * NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));            // a_hi x [w_hi | w_lo]
+                    if (!skip_lo) wgmma_bf16<NPAD>(d, a_lo, make_desc(b_tap, kLboB, 128));  // a_lo x w_hi
+                  } else {
+                    wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));                // a_hi x w_hi
+                    if (!skip_lo) wgmma_bf16<NPAD>(d, a_lo, make_desc(b_tap, kLboB, 128));  // a_lo x w_hi
+                    wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap + 2 * NPAD * 16, kLboB, 128));  // a_hi x w_lo
+                  }
+                }
+              }
+            }
+          });
+        }
       }
       if (++astage == C::NA) { astage = 0; aphase ^= 1; }
     }
@@ -592,6 +693,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
               v[k] = acc[mb][col / 2 + k];
               if constexpr (DUAL) v[k] += acc[mb][(col + NPAD) / 2 + k];
               if constexpr (F8IN) v[k] = (v[k] + acc8[mb][col / 2 + k]) * dscale;
+              if constexpr (C::PAIR) v[k] = pair ? v[k] * s_bias[NPAD + col + fcol + (k & 1)] : v[k];
             }
             float* s = stg + frow * kStageLd + 8 * j + fcol;
             *reinterpret_cast<float2*>(s) = make_float2(v[0], v[1]);
@@ -732,6 +834,64 @@ static __global__ void pack_stages_f8_kernel(const float* __restrict__ dense, ui
     *reinterpret_cast<uint16_t*>(p1 + ((size_t)0 * rows + row) * 16 + c) = pack_e4m3x2(w[0] * ws, w[1] * ws);
     *reinterpret_cast<uint16_t*>(p1 + ((size_t)1 * rows + row) * 16 + c) =
         pack_e4m3x2(wl[0] * ws * 512.f, wl[1] * ws * 512.f);
+  }
+}
+
+// kFmtPair8 (the first layer): per output column (dense row) c, scale[c] = s_c = 2^floor(log2(224 / max|w_c|)) and
+// scale[npad + c] = 2^-9 / s_c, what the epilogue multiplies column c with.  One block per column.
+static __global__ void pair_scale_kernel(const float* __restrict__ dense, float* __restrict__ scale, int npad, int n) {
+  __shared__ float smax[256];
+  float m = 0.f;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(dense[(size_t)blockIdx.x * n + i]));
+  smax[threadIdx.x] = m;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) smax[threadIdx.x] = fmaxf(smax[threadIdx.x], smax[threadIdx.x + o]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const float s = exp2f(floorf(log2f(224.f / fmaxf(smax[0], 1e-30f))));
+    scale[blockIdx.x] = s;
+    scale[npad + blockIdx.x] = 1.f / (512.f * s);
+  }
+}
+// The tap-pair weight image of a 16-channel layer (dense [npad][16][kk]): units of npad * 32 B,
+//   units 0 .. (kk + 1) / 2 - 1   pair p:  [K half 0|1][rows][16 e4m3]  e4m3(w_lo s_c 2^9) of taps t0, t0 + 1
+//                                 (t0 = min(2p, kk - 2); half 0 of the last pair is zero when kk is odd)
+//   then one unit per tap t:      [k8 0|1][rows][8 bf16]               bf16(w) s_c 2^9 (exact: a power of two)
+// One thread per (unit, row).
+static __global__ void pack_stages_pair_kernel(const float* __restrict__ dense, uint8_t* __restrict__ out,
+                                               const float* __restrict__ scale, int npad, int kk) {
+  const int pairs = (kk + 1) / 2, units = pairs + kk;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < units * npad; i += gridDim.x * blockDim.x) {
+    const int u = i / npad, row = i - u * npad;
+    const float s = scale[row] * 512.f;
+    uint8_t* unit = out + (size_t)u * npad * 32;
+    const float* w = dense + (size_t)row * 16 * kk;
+    if (u < pairs) {
+      const int t0 = 2 * u < kk - 2 ? 2 * u : kk - 2;
+      for (int h = 0; h < 2; h++) {
+        const int tap = t0 + h;
+        const bool zero = h == 0 && 2 * u >= kk - 1;
+        uint32_t q[4];
+        for (int j = 0; j < 4; j++) {
+          float f[4];
+          for (int e = 0; e < 4; e++) {
+            const float x = w[(4 * j + e) * kk + tap];
+            f[e] = zero ? 0.f : (x - __bfloat162float(__float2bfloat16_rn(x))) * s;
+          }
+          q[j] = pack_e4m3x4(f[0], f[1], f[2], f[3]);
+        }
+        *reinterpret_cast<uint4*>(unit + ((size_t)h * npad + row) * 16) = make_uint4(q[0], q[1], q[2], q[3]);
+      }
+    } else {
+      const int tap = u - pairs;
+      for (int c = 0; c < 16; c++) {
+        const float hi = __bfloat162float(__float2bfloat16_rn(w[c * kk + tap])) * s;
+        *reinterpret_cast<__nv_bfloat16*>(unit + ((size_t)(c / 8) * npad + row) * 16 + (c % 8) * 2) =
+            __float2bfloat16_rn(hi);
+      }
+    }
   }
 }
 
