@@ -793,16 +793,15 @@ int wn_forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images_host, 
     set_error("%s: 1..65535 images per call, got n=%d", what, n);
     return n <= 0 ? WN_E_INVALID : WN_E_UNSUPPORTED;
   }
-  std::vector<int> hs(n), ws(n);
   for (int i = 0; i < n; i++) {
     const wn_ragged_tensors& t = images_host[i];
     if (!t.x || !t.wb || !t.he || !t.gc || !t.out) {
       set_error("%s: null image pointer (image %d)", what, i);
       return WN_E_INVALID;
     }
-    hs[i] = t.height;
-    ws[i] = t.width;
   }
+  std::vector<int> hs, ws;
+  ragged_sizes(images_host, n, &hs, &ws);
   int rc = train_ragged_check(what, hs.data(), ws.data(), n);
   if (rc) return rc;
   if (!h->packed) {
@@ -1042,16 +1041,15 @@ int wn_backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images_host,
     set_error("%s: 1..65535 images per call, got n=%d", what, n);
     return n <= 0 ? WN_E_INVALID : WN_E_UNSUPPORTED;
   }
-  std::vector<int> hs(n), ws(n);
   for (int i = 0; i < n; i++) {
     const wn_ragged_tensors& t = images_host[i];
     if (!t.x || !t.wb || !t.he || !t.gc || !grad_out_host[i]) {
       set_error("%s: null image pointer (image %d)", what, i);
       return WN_E_INVALID;
     }
-    hs[i] = t.height;
-    ws[i] = t.width;
   }
+  std::vector<int> hs, ws;
+  ragged_sizes(images_host, n, &hs, &ws);
   if ((rc = backward_ragged_tiled_check(what, hs.data(), ws.data(), n, tile_h, tile_w, max_pass_pixels))) return rc;
   if ((rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);

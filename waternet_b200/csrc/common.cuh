@@ -5,6 +5,9 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <initializer_list>
+#include <vector>
+
 #include "../../include/waternet_b200.h"
 #include "tiling.cuh"
 
@@ -23,6 +26,52 @@ inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
       return WN_E_CUDA;                                                                 \
     }                                                                                   \
   } while (0)
+
+// The device table of a ragged call: its parts in device order, each at a 256-byte boundary.  The parts are filled
+// in one host staging buffer in that layout and copied with one cudaMemcpyAsync; bytes() is the workspace they take.
+class HostTable {
+ public:
+  HostTable(std::initializer_list<size_t> part_bytes) {
+    for (size_t b : part_bytes) {
+      len_[parts_] = b;
+      off_[parts_ + 1] = off_[parts_] + align256(b);
+      parts_++;
+    }
+  }
+  size_t bytes() const { return off_[parts_]; }
+  // part k of the staging buffer (zero-filled at first use) and of the device table at `table`
+  template <class T> T* part(int k) {
+    if (host_.empty()) host_.resize(bytes());
+    return reinterpret_cast<T*>(host_.data() + off_[k]);
+  }
+  template <class T> T* dev(void* table, int k) const { return reinterpret_cast<T*>((uint8_t*)table + off_[k]); }
+  // parts [first, end) -> the device table, from the start of part `first` to the last byte of part end - 1.
+  // Pageable source: the copy is staged before cudaMemcpyAsync returns, so the table may go out of scope.
+  int upload(void* table, cudaStream_t stream, int first = 0, int end = -1) {
+    if (end < 0) end = parts_;
+    if (host_.empty()) host_.resize(bytes());
+    WN_CUDA(cudaMemcpyAsync(dev<uint8_t>(table, first), host_.data() + off_[first],
+                            off_[end - 1] + len_[end - 1] - off_[first], cudaMemcpyHostToDevice, stream));
+    return WN_OK;
+  }
+
+ private:
+  static constexpr int kMaxParts = 4;
+  size_t off_[kMaxParts + 1] = {}, len_[kMaxParts] = {};
+  int parts_ = 0;
+  std::vector<uint8_t> host_;
+};
+
+// the heights and widths of a ragged array (wn_ragged_tensors, wn_ragged_image)
+template <class Img>
+void ragged_sizes(const Img* images, int n, std::vector<int>* hs, std::vector<int>* ws) {
+  hs->resize(n);
+  ws->resize(n);
+  for (int i = 0; i < n; i++) {
+    (*hs)[i] = images[i].height;
+    (*ws)[i] = images[i].width;
+  }
+}
 
 #define WN_LAUNCH_CHECK(h)   \
   do {                       \
@@ -147,12 +196,9 @@ int preprocess_u8_planes(wn_handle* h, const uint8_t* rgb, int n, int height, in
 // (workspace: that of preprocess_u8_luts, untouched in between)
 int preprocess_u8_luts(wn_handle* h, const uint8_t* rgb, int n, int height, int width, void* workspace,
                        size_t workspace_bytes, cudaStream_t stream);
-int preprocess_u8_window_planes(wn_handle* h, const uint8_t* rgb, int n, const TileGeom& tiles, long long win0,
-                                int count, uint4* planes, void* workspace, cudaStream_t stream);
 // ... and for a ragged batch, where every image has its own size: the preprocess geometry of one image (CLAHE tile,
-// clip limit, LUT scale, histogram slabs), the statistics and LUTs of all n images from their device table (one
-// stats and one LUT launch), then the operand planes of `count` windows in slots of slot_h x slot_w (zeros outside
-// each window's valid extent).  Workspace: that of preprocess_workspace_bytes(n, ...), untouched in between.
+// clip limit, LUT scale, histogram slabs), and the statistics and LUTs of all n images from their device table (one
+// stats and one LUT launch).  Workspace: that of preprocess_workspace_bytes(n, ...), untouched in between.
 struct RaggedImage {
   const uint8_t* rgb;
   int H, W;
@@ -164,8 +210,13 @@ static_assert(sizeof(RaggedImage) == 40, "RaggedImage: engine.RAGGED_IMAGE_BYTES
 RaggedImage ragged_image(const uint8_t* rgb, int height, int width);
 int preprocess_u8_ragged_luts(wn_handle* h, int n, const RaggedImage* imgs, int max_slabs, void* workspace,
                               cudaStream_t stream);
-int preprocess_u8_ragged_planes(wn_handle* h, int n, const RaggedImage* imgs, const RaggedWindow* wins, int count,
-                                int slot_h, int slot_w, uint4* planes, void* workspace, cudaStream_t stream);
+// The operand planes of `count` slots of geo (tiling.cuh; zeros beyond each valid extent) from the LUTs of the n
+// images above.  The image data of a slot: one record for a grid geometry (image i at rgb + i * H * W * 3), the
+// device table of n records for a table geometry.  Defined for (GridGeom, RaggedImage) and (TableGeom, const
+// RaggedImage*).
+template <class Geom, class Img>
+int preprocess_u8_slot_planes(wn_handle* h, const Geom& geo, const Img& imgs, int n, int count, uint4* planes,
+                              void* workspace, cudaStream_t stream);
 
 // conv_simt.cu
 int simt_pack_weights(wn_handle* h, const float* const* params, cudaStream_t stream);

@@ -1003,15 +1003,16 @@ static void ragged_slot(const int* hs, const int* ws, int n, int* sh, int* sw) {
     *sw = ws[i] > *sw ? ws[i] : *sw;
   }
 }
-static size_t ragged_train_table_bytes(int n) {
-  return align256((size_t)n * sizeof(RaggedWindow)) + align256((size_t)n * sizeof(PackInArgs)) +
-         align256((size_t)n * sizeof(RaggedGrads));
+// the table: [plan: n, slot_h, slot_w | windows | PackInArgs | RaggedGrads]
+static HostTable ragged_train_table(int n) {
+  return HostTable({256, (size_t)n * sizeof(RaggedWindow), (size_t)n * sizeof(PackInArgs),
+                    (size_t)n * sizeof(RaggedGrads)});
 }
 
 size_t train_ragged_workspace_bytes(const int* hs, const int* ws, int n) {
   int sh, sw;
   ragged_slot(hs, ws, n, &sh, &sw);
-  return 256 + 256 + ragged_train_table_bytes(n) + train_workspace_bytes_padded(n, sh, sw);
+  return 256 + ragged_train_table(n).bytes() + train_workspace_bytes_padded(n, sh, sw);
 }
 
 // The per-image host table of a ragged call: imgs[i] (the four inputs and their strides) when imgs is given, and
@@ -1037,36 +1038,30 @@ static bool ragged_table(const wn_ragged_tensors* images, const float* const* gr
   return want_in;
 }
 
-// the table's three parts and the training buffers of a workspace of any alignment
+// the table's parts and the training buffers of a workspace of any alignment
 struct RaggedTrainLayout {
-  int* plan;  // n, slot_h, slot_w of the forward call
+  HostTable table;
+  uint8_t* base;  // the device table
+  int* plan;      // n, slot_h, slot_w of the forward call
   RaggedWindow* wins;
   PackInArgs* imgs;
   RaggedGrads* grads;
   TrainBuffers t;
 };
 static RaggedTrainLayout ragged_train_layout(void* workspace, int n, int sh, int sw) {
-  RaggedTrainLayout l;
-  uint8_t* p = (uint8_t*)align256((uintptr_t)workspace);
-  l.plan = (int*)p;
-  p += 256;
-  l.wins = (RaggedWindow*)p;
-  p += align256((size_t)n * sizeof(RaggedWindow));
-  l.imgs = (PackInArgs*)p;
-  p += align256((size_t)n * sizeof(PackInArgs));
-  l.grads = (RaggedGrads*)p;
-  p += align256((size_t)n * sizeof(RaggedGrads));
-  carve(&l.t, p, (size_t)n * sh * sw);
+  RaggedTrainLayout l = {ragged_train_table(n), (uint8_t*)align256((uintptr_t)workspace)};
+  l.plan = l.table.dev<int>(l.base, 0);
+  l.wins = l.table.dev<RaggedWindow>(l.base, 1);
+  l.imgs = l.table.dev<PackInArgs>(l.base, 2);
+  l.grads = l.table.dev<RaggedGrads>(l.base, 3);
+  carve(&l.t, l.base + l.table.bytes(), (size_t)n * sh * sw);
   return l;
 }
 
 int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, void* workspace, size_t workspace_bytes,
                          cudaStream_t stream) {
-  std::vector<int> hs(n), ws(n);
-  for (int i = 0; i < n; i++) {
-    hs[i] = images[i].height;
-    ws[i] = images[i].width;
-  }
+  std::vector<int> hs, ws;
+  ragged_sizes(images, n, &hs, &ws);
   const size_t need = train_ragged_workspace_bytes(hs.data(), ws.data(), n);
   if (workspace_bytes < need) {
     set_error("ragged training workspace too small: %zu < %zu", workspace_bytes, need);
@@ -1075,12 +1070,12 @@ int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, v
   int sh, sw;
   ragged_slot(hs.data(), ws.data(), n, &sh, &sw);
   RaggedTrainLayout l = ragged_train_layout(workspace, n, sh, sw);
-  // host copy of the plan, the windows and the PackInArgs, contiguous as in the workspace
-  const size_t win_b = align256((size_t)n * sizeof(RaggedWindow));
-  std::vector<uint8_t> host(256 + win_b + (size_t)n * sizeof(PackInArgs));
-  const int plan[3] = {n, sh, sw};
-  memcpy(host.data(), plan, sizeof(plan));
-  RaggedWindow* wins = reinterpret_cast<RaggedWindow*>(host.data() + 256);
+  // the plan, the windows and the PackInArgs; the backward writes the RaggedGrads
+  int* plan = l.table.part<int>(0);
+  plan[0] = n;
+  plan[1] = sh;
+  plan[2] = sw;
+  RaggedWindow* wins = l.table.part<RaggedWindow>(1);
   for (int i = 0; i < n; i++) {
     RaggedWindow r = {};
     r.out_f32 = images[i].out;
@@ -1089,10 +1084,9 @@ int forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, v
     r.W = r.vw = r.kx1 = images[i].width;
     wins[i] = r;
   }
-  ragged_table(images, nullptr, nullptr, n, reinterpret_cast<PackInArgs*>(host.data() + 256 + win_b), nullptr);
-  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
-  WN_CUDA(cudaMemcpyAsync(l.plan, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
-  int rc;
+  ragged_table(images, nullptr, nullptr, n, l.table.part<PackInArgs>(2), nullptr);
+  int rc = l.table.upload(l.base, stream, 0, 3);
+  if (rc) return rc;
   WN_CUDA(cudaMemsetAsync(l.t.f.exact_flag, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
   const TableGeom geo = {l.wins, 0, sh, sw, sh, sw};  // every image is one window of its own size
   if ((rc = pack_inputs(h, geo, l.imgs, n, nullptr, l.t.f.exact_flag, stream))) return rc;
@@ -1119,9 +1113,8 @@ int backward_ragged(wn_handle* h, const int* hs, const int* ws, const float* con
   int sh, sw;
   ragged_slot(hs, ws, n, &sh, &sw);
   RaggedTrainLayout l = ragged_train_layout(workspace, n, sh, sw);
-  std::vector<RaggedGrads> host(n);
-  const bool want_in = ragged_table(nullptr, grad_out, input_grads, n, nullptr, host.data());
-  WN_CUDA(cudaMemcpyAsync(l.grads, host.data(), (size_t)n * sizeof(RaggedGrads), cudaMemcpyHostToDevice, stream));
+  const bool want_in = ragged_table(nullptr, grad_out, input_grads, n, nullptr, l.table.part<RaggedGrads>(3));
+  if ((rc = l.table.upload(l.base, stream, 3, 4))) return rc;
   // every image is one window of its own size
   const TableSlots geo = {{l.wins, 0, sh, sw, sh, sw}, l.grads, l.plan};
   return backward_pass(h, geo, kStackAll, -1, l.t, grads, want_in, false, n, sh, sw, stream);
@@ -1364,10 +1357,8 @@ static int grid_recompute_backward(wn_handle* h, int stack, int which, const flo
     }
   const PackInArgs pa = pack_args(in, st);
   if ((rc = pack_inputs(h, whole_images(H, W), pa, n, nullptr, exact, stream))) return rc;
-  std::vector<RaggedPass> passes;
-  const long long total = (long long)n * g.ny * g.nx, per_pass = tiled_train_pass(g, n, max_pass_pixels);
-  for (long long w0 = 0; w0 < total; w0 += per_pass)
-    passes.push_back({w0, (int)std::min(per_pass, total - w0), g.win_h, g.win_w});
+  const std::vector<RaggedPass> passes =
+      grid_passes((long long)n * g.ny * g.nx, tiled_train_pass(g, n, max_pass_pixels), g.win_h, g.win_w);
   return recompute_passes(h, geo, passes, stack, which, pa, exact, s, grads, want_in, pass_ws, pass_bytes, stream);
 }
 
@@ -1413,9 +1404,8 @@ int submodule_backward_tiled(wn_handle* h, int stack, int which, const float* co
 // that of forward_train_ragged (every ReLU layer stores zeros beyond each window's valid extent).  The table (one
 // PackInArgs and one RaggedGrads per image, then the windows in plan order) sits between the scratch parameter
 // gradients and the pass buffers and is copied from pageable host memory once per call.
-static size_t ragged_tiled_table_bytes(int n, size_t windows) {
-  return align256((size_t)n * sizeof(PackInArgs)) + align256((size_t)n * sizeof(RaggedGrads)) +
-         align256(windows * sizeof(RaggedWindow));
+static HostTable ragged_tiled_table(int n, size_t windows) {
+  return HostTable({(size_t)n * sizeof(PackInArgs), (size_t)n * sizeof(RaggedGrads), windows * sizeof(RaggedWindow)});
 }
 
 static void ragged_tiled_plan(const int* hs, const int* ws, int n, int tile_h, int tile_w, long long max_pass_pixels,
@@ -1425,7 +1415,7 @@ static void ragged_tiled_plan(const int* hs, const int* ws, int n, int tile_h, i
 
 static size_t ragged_tiled_workspace(int n, const std::vector<RaggedWindow>& wins,
                                      const std::vector<RaggedPass>& passes) {
-  return 256 + param_grads_bytes(kStackAll) + ragged_tiled_table_bytes(n, wins.size()) +
+  return 256 + param_grads_bytes(kStackAll) + ragged_tiled_table(n, wins.size()).bytes() +
          train_workspace_bytes_padded(1, 1, (int)largest_pass_pixels(passes)) + 256;
 }
 
@@ -1442,11 +1432,8 @@ int backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images, const f
                           long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   int rc = check_bwd_packed(h);
   if (rc) return rc;
-  std::vector<int> hs(n), ws(n);
-  for (int i = 0; i < n; i++) {
-    hs[i] = images[i].height;
-    ws[i] = images[i].width;
-  }
+  std::vector<int> hs, ws;
+  ragged_sizes(images, n, &hs, &ws);
   std::vector<RaggedWindow> wins;
   std::vector<RaggedPass> passes;
   ragged_tiled_plan(hs.data(), ws.data(), n, tile_h, tile_w, max_pass_pixels, &wins, &passes);
@@ -1470,23 +1457,18 @@ int backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images, const f
   int* exact = (int*)base;
   ScratchGrads s;
   uint8_t* table = scratch_grads(&s, base + 256, grads, kStackAll, -1);
-  // the table, built on the host in its device layout
-  const size_t in_b = align256((size_t)n * sizeof(PackInArgs)), g_b = align256((size_t)n * sizeof(RaggedGrads));
-  std::vector<uint8_t> host(in_b + g_b + wins.size() * sizeof(RaggedWindow));
-  RaggedGrads* rg = reinterpret_cast<RaggedGrads*>(host.data() + in_b);
-  const bool want_in =
-      ragged_table(images, grad_out, input_grads, n, reinterpret_cast<PackInArgs*>(host.data()), rg);
+  HostTable t = ragged_tiled_table(n, wins.size());
+  RaggedGrads* rg = t.part<RaggedGrads>(1);
+  const bool want_in = ragged_table(images, grad_out, input_grads, n, t.part<PackInArgs>(0), rg);
   for (int i = 0; i < n; i++)
     for (int t = 0; t < 4; t++)
       if (rg[i].in[t])
         WN_CUDA(cudaMemsetAsync(rg[i].in[t], 0, (size_t)3 * hs[i] * ws[i] * sizeof(float), stream));
-  memcpy(host.data() + in_b + g_b, wins.data(), wins.size() * sizeof(RaggedWindow));
-  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
-  WN_CUDA(cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
-  const PackInArgs* d_imgs = reinterpret_cast<const PackInArgs*>(table);
-  TableSlots geo = {{reinterpret_cast<const RaggedWindow*>(table + in_b + g_b), 0, 0, 0, tile_h, tile_w},
-                    reinterpret_cast<const RaggedGrads*>(table + in_b), nullptr};
-  uint8_t* pass_ws = table + ragged_tiled_table_bytes(n, wins.size());
+  memcpy(t.part<RaggedWindow>(2), wins.data(), wins.size() * sizeof(RaggedWindow));
+  if ((rc = t.upload(table, stream))) return rc;
+  const PackInArgs* d_imgs = t.dev<PackInArgs>(table, 0);
+  TableSlots geo = {{t.dev<RaggedWindow>(table, 2), 0, 0, 0, tile_h, tile_w}, t.dev<RaggedGrads>(table, 1), nullptr};
+  uint8_t* pass_ws = table + t.bytes();
   const size_t pass_bytes = workspace_bytes - (size_t)(pass_ws - (uint8_t*)workspace);
   // the exact-levels flag over every pass, as wn_forward_ragged takes it
   WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"

@@ -25,6 +25,8 @@
 //              (registers -> shared-memory transpose -> bias/act -> bf16 hi/lo planes or fp32)
 //   warp 8     A producer (TMA halo tiles, one 16-channel chunk per stage); wgs 3: warp 12
 //   warp 9     B producer (bulk copies of pre-packed weight stages, 1-9 taps of a chunk per stage); wgs 3: warp 13
+#include <type_traits>
+
 #include "umma_conv.cuh"
 
 namespace wn {
@@ -577,23 +579,6 @@ static FwdBuffers carve(void* workspace, int n, int H, int W) {
   return b;
 }
 
-// One pass in `scheme`; in the fp8-correction scheme the bf16x3 chain of the same batch is enqueued right behind
-// it, every launch conditional on the sticky e4m3 range flag (ConvArgs::run_if): a batch whose activations left
-// the e4m3 range is recomputed within the same call, nobody ever sees the degraded result.
-static int umma_pass(wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out, int n, int H, int W,
-                     const FwdBuffers& b, cudaStream_t stream, FwdOpts o) {
-  int rc = umma_forward_layers(h, in, st, out, n, H, W, b, stream, o);
-  if (rc || o.scheme != 1 || o.dbg_layer >= 0) return rc;
-  o.scheme = 0;
-  o.packed = true;  // act0 (and the exact-levels flag) of this batch are still in place
-  o.run_if = h->umma->overflow_dev;
-  Timing* timing = h->timing;  // the conditional launches are not part of the per-kernel timing record
-  h->timing = nullptr;
-  rc = umma_forward_layers(h, in, st, out, n, H, W, b, stream, o);
-  h->timing = timing;
-  return rc;
-}
-
 int umma_debug_layer(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], int n, int H, int W,
                      int layer, float* dst, void* workspace, size_t workspace_bytes, cudaStream_t stream, int scheme) {
   if (!h->umma || umma_chunk(0, n, H, W) != n || workspace_bytes < umma_forward_workspace_bytes(n, H, W)) {
@@ -609,59 +594,133 @@ int umma_debug_layer(wn_handle* h, const float* const in[4], const int64_t in_st
   return umma_forward_layers(h, in, in_strides, nullptr, n, H, W, carve(workspace, n, H, W), stream, o);
 }
 
-// fp8-correction mode: once an activation has left the e4m3 range (sticky flag, mirrored to the host at the end
-// of every call) this handle keeps to the bf16x3 kernels until new weights are packed.
-static int effective_scheme(wn_handle* h, int scheme) {
-  return (scheme == 1 && *h->umma->overflow_host) ? 0 : scheme;
-}
-static int mirror_overflow(wn_handle* h, int scheme, cudaStream_t stream) {
-  if (scheme == 1)
+// Where the passes of a forward call store their results beyond their own buffers (FwdBuffers).  Whole images (no
+// tiles, no window table) store at the offsets of the pass's first image; windows store their kept rectangles.
+struct FwdOut {
+  float* f32 = nullptr;        // kStackAll: the images, fp32 NCHW (may be null); kStackCmg: the maps; windowed
+                               // kStackRefiners: refiner `which`'s image
+  float* refined = nullptr;    // kStackRefiners: whole images [n][9][H][W]; windowed, one pass of windows
+  int which = 0;
+  uint8_t* u8 = nullptr;       // ten2arr'd uint8 NHWC images (the gate epilogue)
+  PeerOut peers = {};          // ... and their peer copies
+  const TileGeom* tiles = nullptr;  // the slots are windows of these tiles (grid geometry)
+};
+
+// One forward call (WN_MODE_BF16X3, WN_MODE_BF16_FP8): the weights, workspace and encoder checks, the scheme this
+// handle runs (once an activation has left the e4m3 range, sticky flag, the handle keeps to bf16x3 until new weights
+// are packed), then `start` (the call's LUTs, table and call-wide exact-levels flag), then per pass of geo: its
+// buffers, `act0` (the operand planes, the per-pass flag), the ten launches, in the fp8-correction scheme the
+// bf16x3 chain of the same pass right behind them, every launch conditional on the range flag (ConvArgs::run_if: a
+// pass whose activations left the e4m3 range is recomputed within the call, nobody sees the degraded result), and a
+// windowed sub-module's kept-rectangle store.  The range flag is mirrored to the host at the end.  flag: the
+// call-wide exact-levels flag, or null when act0 sets one per pass.
+template <class Geom, class Start, class Act0>
+static int forward_call(wn_handle* h, const char* what, size_t workspace_bytes, size_t need, FwdOpts o, Geom geo,
+                        const std::vector<RaggedPass>& passes, void* fwd_ws, int* flag, const FwdOut& f,
+                        cudaStream_t stream, Start start, Act0 act0) {
+  if (!h->umma) {
+    set_error("tensor-core weights have not been packed");
+    return WN_E_STATE;
+  }
+  if (workspace_bytes < need) {
+    set_error("%s workspace too small: %zu < %zu", what, workspace_bytes, need);
+    return WN_E_WORKSPACE;
+  }
+  int rc = get_encoder();
+  if (rc) return rc;
+  if (o.scheme == 1 && *h->umma->overflow_host) o.scheme = 0;
+  if ((rc = start())) return rc;
+  const int64_t none[4][4] = {};
+  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
+  o.packed = true;
+  for (const RaggedPass& p : passes) {
+    geo.set_pass(p);
+    FwdBuffers b = carve(fwd_ws, p.count, p.slot_h, p.slot_w);
+    if (flag) b.exact_flag = flag;
+    FwdOpts po = o;
+    po.rwin = geo.rwin();
+    if ((rc = act0(geo, p, b, po))) return rc;
+    float* out = f.f32;
+    if (!f.tiles && !po.rwin) {  // images p.first, p.first + 1, ...
+      const size_t n0 = (size_t)p.first, px = (size_t)p.slot_h * p.slot_w;
+      if (out) out += n0 * 3 * px;
+      if (f.u8) po.out_u8 = f.u8 + n0 * px * 3;
+      for (int k = 0; k < f.peers.n; k++) po.peers.p[k] = f.peers.p[k] + n0 * px * 3;
+      po.peers.n = f.peers.n;
+      if (o.stack == kStackCmg) b.cm = out;  // the maps are the result
+      if (o.stack == kStackRefiners) {
+        b.refined = f.refined + n0 * 9 * px;
+        out = nullptr;
+      }
+    } else if (o.stack == kStackAll) {
+      po.out_u8 = f.u8;
+      if (f.tiles) {
+        po.tiles = f.tiles;
+        po.win0 = p.first;
+      }
+    } else {  // the sub-modules keep their result in window layout: store_kept_kernel below
+      out = nullptr;
+      if (o.stack == kStackRefiners) b.refined = f.refined;
+    }
+    if ((rc = umma_forward_layers(h, no_in, none, out, p.count, p.slot_h, p.slot_w, b, stream, po))) return rc;
+    if (po.scheme == 1) {
+      po.scheme = 0;
+      po.run_if = h->umma->overflow_dev;
+      Timing* timing = h->timing;  // the conditional launches are not part of the per-kernel timing record
+      h->timing = nullptr;
+      rc = umma_forward_layers(h, no_in, none, out, p.count, p.slot_h, p.slot_w, b, stream, po);
+      h->timing = timing;
+      if (rc) return rc;
+    }
+    if constexpr (std::is_same<Geom, GridGeom>::value)
+      if (f.tiles && o.stack != kStackAll) {  // after the pass and its conditional bf16x3 re-run
+        TimedScope ts(h, kSlotGate, stream);
+        const bool maps = o.stack == kStackCmg;
+        store_kept_kernel<<<dim3((unsigned)(((size_t)geo.slot_hw() + 255) / 256), p.count), 256, 0, stream>>>(
+            maps ? b.cm : f.refined, maps ? 3 : 9, maps ? 0 : 3 * f.which, 3, f.f32, geo);
+        WN_LAUNCH_CHECK(h);
+      }
+  }
+  if (o.scheme == 1)
     WN_CUDA(cudaMemcpyAsync(h->umma->overflow_host, h->umma->overflow_dev, sizeof(int), cudaMemcpyDeviceToHost, stream));
   return WN_OK;
+}
+
+static int no_start() { return WN_OK; }
+
+// uint8 in: the preprocess writes act0 as exact 8-bit levels (hi planes only), so the flag of every pass is set
+static FwdOpts u8_opts(int scheme) {
+  FwdOpts o;
+  o.scheme = scheme;
+  o.hi_only = true;
+  return o;
 }
 
 int umma_forward(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], float* out, int n, int H,
                  int W, void* workspace, size_t workspace_bytes, cudaStream_t stream, int scheme, int stack,
                  float* refined) {
-  if (!h->umma) {
-    set_error("tensor-core weights have not been packed");
-    return WN_E_STATE;
-  }
-  if (workspace_bytes < umma_forward_workspace_bytes(n, H, W)) {
-    set_error("forward workspace too small: %zu < %zu", workspace_bytes, umma_forward_workspace_bytes(n, H, W));
-    return WN_E_WORKSPACE;
-  }
-  int rc = get_encoder();
-  if (rc) return rc;
-  scheme = effective_scheme(h, scheme);
   const int nb = umma_chunk(h->chunk_pixels, n, H, W);
   // Several passes: whether the first layer runs its level form is decided once, over every input pixel of the n
   // images, so that the result does not depend on how the batch is split (the tiled and ragged calls decide so too).
-  // The flag sits where a full pass puts it, beyond the buffers of any smaller pass.
+  // The flag sits where a full pass puts it, beyond the buffers of any smaller pass.  One pass takes it in the
+  // packing launch.
   int* flag = nb < n ? carve(workspace, nb, H, W).exact_flag : nullptr;
-  if (flag && (rc = pack_inputs(h, whole_images(H, W), pack_args(in, in_strides), n, nullptr, flag, stream))) return rc;
-  for (int n0 = 0; n0 < n; n0 += nb) {
-    const int cur = n - n0 < nb ? n - n0 : nb;
-    const float* sub[4];
-    for (int t = 0; t < 4; t++) sub[t] = in[t] + (long long)n0 * in_strides[t][0];
-    FwdBuffers b = carve(workspace, cur, H, W);
-    FwdOpts o;
-    o.scheme = scheme;
-    o.stack = stack;
-    if (flag) {
-      b.exact_flag = flag;
-      o.packed = true;
-      if ((rc = pack_inputs(h, whole_images(H, W), pack_args(sub, in_strides), cur, b.act0, nullptr, stream,
-                            scheme == kSchemeBf16)))
-        return rc;
-    }
-      float* dst = out + (size_t)n0 * 3 * H * W;
-    if (stack == kStackCmg) b.cm = dst;                                   // the maps are the result
-    if (stack == kStackRefiners) { b.refined = refined + (size_t)n0 * 9 * H * W; dst = nullptr; }
-    rc = umma_pass(h, sub, in_strides, dst, cur, H, W, b, stream, o);
-    if (rc) return rc;
-  }
-  return mirror_overflow(h, scheme, stream);
+  FwdOpts o;
+  o.scheme = scheme;
+  o.stack = stack;
+  FwdOut f;
+  f.f32 = out;
+  f.refined = refined;
+  return forward_call(
+      h, "forward", workspace_bytes, umma_forward_workspace_bytes(n, H, W), o, whole_images(H, W),
+      grid_passes(n, nb, H, W), workspace, flag, f, stream,
+      [&] { return flag ? pack_inputs(h, whole_images(H, W), pack_args(in, in_strides), n, nullptr, flag, stream) : WN_OK; },
+      [&](const GridGeom&, const RaggedPass& p, FwdBuffers& b, FwdOpts& po) {
+        const float* sub[4];
+        for (int t = 0; t < 4; t++) sub[t] = in[t] + p.first * in_strides[t][0];
+        return pack_inputs(h, whole_images(H, W), pack_args(sub, in_strides), p.count, b.act0,
+                           flag ? nullptr : b.exact_flag, stream, po.scheme == kSchemeBf16);
+      });
 }
 
 // preprocess -> forward -> ten2arr without materialising the four fp32 input tensors or the fp32 output:
@@ -674,40 +733,20 @@ size_t umma_enhance_workspace_bytes(int n, int h, int w) {
 
 int umma_enhance_u8(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* out_f32, int n, int H, int W,
                     void* workspace, size_t workspace_bytes, cudaStream_t stream, int scheme, const PeerOut& peers) {
-  if (!h->umma) {
-    set_error("tensor-core weights have not been packed");
-    return WN_E_STATE;
-  }
-  if (workspace_bytes < umma_enhance_workspace_bytes(n, H, W)) {
-    set_error("enhance workspace too small: %zu < %zu", workspace_bytes, umma_enhance_workspace_bytes(n, H, W));
-    return WN_E_WORKSPACE;
-  }
-  int rc = get_encoder();
-  if (rc) return rc;
-  scheme = effective_scheme(h, scheme);
   const int nb = umma_chunk(h->chunk_pixels, n, H, W);
   uint8_t* pre_ws = (uint8_t*)align256((uintptr_t)workspace);
   const size_t pre_b = align256(preprocess_workspace_bytes(nb, H, W));
-  void* fwd_ws = pre_ws + pre_b;
-  const int64_t none[4][4] = {};
-  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
-  for (int n0 = 0; n0 < n; n0 += nb) {
-    const int cur = n - n0 < nb ? n - n0 : nb;
-    FwdBuffers b = carve(fwd_ws, cur, H, W);
-    WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));
-    rc = preprocess_u8_planes(h, rgb + (size_t)n0 * H * W * 3, cur, H, W, b.act0, pre_ws, pre_b, stream);
-    if (rc) return rc;
-    FwdOpts o;
-    o.scheme = scheme;
-    o.packed = true;
-    o.hi_only = true;
-    o.out_u8 = out_u8 + (size_t)n0 * H * W * 3;
-    o.peers.n = peers.n;
-    for (int k = 0; k < peers.n; k++) o.peers.p[k] = peers.p[k] + (size_t)n0 * H * W * 3;
-    rc = umma_pass(h, no_in, none, out_f32 ? out_f32 + (size_t)n0 * 3 * H * W : nullptr, cur, H, W, b, stream, o);
-    if (rc) return rc;
-  }
-  return mirror_overflow(h, scheme, stream);
+  FwdOut f;
+  f.f32 = out_f32;
+  f.u8 = out_u8;
+  f.peers = peers;
+  return forward_call(h, "enhance", workspace_bytes, umma_enhance_workspace_bytes(n, H, W), u8_opts(scheme),
+                      whole_images(H, W), grid_passes(n, nb, H, W), pre_ws + pre_b, nullptr, f, stream, no_start,
+                      [&](const GridGeom&, const RaggedPass& p, FwdBuffers& b, FwdOpts&) {
+                        WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));
+                        return preprocess_u8_planes(h, rgb + (size_t)p.first * H * W * 3, p.count, H, W, b.act0,
+                                                    pre_ws, pre_b, stream);
+                      });
 }
 
 // The tiled form (tiling.cuh): the statistics and LUTs of all n images once, then per pass a batch of equally sized
@@ -724,47 +763,31 @@ size_t umma_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int t
          1024;
 }
 
+// the passes of the windows of n images of g, as many per pass as fit in max_pass_pixels (0: the default)
+static std::vector<RaggedPass> window_passes(const TileGeom& g, int n, long long max_pass_pixels) {
+  return grid_passes((long long)n * g.ny * g.nx,
+                     tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels), g.win_h, g.win_w);
+}
+
 int umma_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* out_f32, int n, int H, int W,
                           int tile_h, int tile_w, long long max_pass_pixels, void* workspace, size_t workspace_bytes,
                           cudaStream_t stream, int scheme) {
-  if (!h->umma) {
-    set_error("tensor-core weights have not been packed");
-    return WN_E_STATE;
-  }
-  const size_t need = umma_enhance_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels);
-  if (workspace_bytes < need) {
-    set_error("tiled enhance workspace too small: %zu < %zu", workspace_bytes, need);
-    return WN_E_WORKSPACE;
-  }
-  int rc = get_encoder();
-  if (rc) return rc;
-  scheme = effective_scheme(h, scheme);
   const TileGeom g = tile_geom(H, W, tile_h, tile_w);
-  const long long total = (long long)n * g.ny * g.nx;
-  const long long per_pass = tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels);
   uint8_t* pre_ws = (uint8_t*)align256((uintptr_t)workspace);
   const size_t pre_b = align256(preprocess_workspace_bytes(n, H, W));
-  void* fwd_ws = pre_ws + pre_b;
-  if ((rc = preprocess_u8_luts(h, rgb, n, H, W, pre_ws, pre_b, stream))) return rc;
-  const int64_t none[4][4] = {};
-  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
-  for (long long w0 = 0; w0 < total; w0 += per_pass) {
-    const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
-    FwdBuffers b = carve(fwd_ws, cur, g.win_h, g.win_w);
-    WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));
-    rc = preprocess_u8_window_planes(h, rgb, n, g, w0, cur, b.act0, pre_ws, stream);
-    if (rc) return rc;
-    FwdOpts o;
-    o.scheme = scheme;
-    o.packed = true;
-    o.hi_only = true;
-    o.out_u8 = out_u8;
-    o.tiles = &g;
-    o.win0 = w0;
-    rc = umma_pass(h, no_in, none, out_f32, cur, g.win_h, g.win_w, b, stream, o);
-    if (rc) return rc;
-  }
-  return mirror_overflow(h, scheme, stream);
+  const RaggedImage img = ragged_image(rgb, H, W);
+  FwdOut f;
+  f.f32 = out_f32;
+  f.u8 = out_u8;
+  f.tiles = &g;
+  return forward_call(
+      h, "tiled enhance", workspace_bytes, umma_enhance_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels),
+      u8_opts(scheme), GridGeom{g, 0}, window_passes(g, n, max_pass_pixels), pre_ws + pre_b, nullptr, f, stream,
+      [&] { return preprocess_u8_luts(h, rgb, n, H, W, pre_ws, pre_b, stream); },
+      [&](const GridGeom& geo, const RaggedPass& p, FwdBuffers& b, FwdOpts&) {
+        WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));
+        return preprocess_u8_slot_planes(h, geo, img, n, p.count, b.act0, pre_ws, stream);
+      });
 }
 
 // The ragged form (tiling.cuh ragged_plan): the statistics and LUTs of all n images in one launch each, then per
@@ -772,15 +795,15 @@ int umma_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, flo
 // valid extent is masked and its kept rectangle stored into its own image.  The plan (per-image geometry and one
 // descriptor per window) is copied into the workspace once per call, so the call cannot be captured in a graph.
 // Workspace: the largest pass plus the per-image LUTs plus the table, independent of the image sizes.
-static size_t ragged_table_bytes(int n, size_t windows) {
-  return align256(align256((size_t)n * sizeof(RaggedImage)) + windows * sizeof(RaggedWindow));
+static HostTable ragged_u8_table(int n, size_t windows) {
+  return HostTable({(size_t)n * sizeof(RaggedImage), windows * sizeof(RaggedWindow)});
 }
 static long long ragged_pass_pixels(long long max_pass_pixels) {
   return max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels;
 }
 static size_t ragged_workspace(int n, const std::vector<RaggedWindow>& wins, const std::vector<RaggedPass>& passes) {
   return (size_t)largest_pass_pixels(passes) * kUmmaBytesPerPixel + 4096 +
-         align256(preprocess_workspace_bytes(n, 1, 1)) + ragged_table_bytes(n, wins.size()) + 1024;
+         align256(preprocess_workspace_bytes(n, 1, 1)) + ragged_u8_table(n, wins.size()).bytes() + 1024;
 }
 
 size_t umma_enhance_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
@@ -794,67 +817,41 @@ size_t umma_enhance_ragged_workspace_bytes(const int* hs, const int* ws, int n, 
 int umma_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images, int n, int tile_h, int tile_w,
                            long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream,
                            int scheme) {
-  if (!h->umma) {
-    set_error("tensor-core weights have not been packed");
-    return WN_E_STATE;
-  }
-  std::vector<int> hs(n), ws(n);
-  for (int i = 0; i < n; i++) {
-    hs[i] = images[i].height;
-    ws[i] = images[i].width;
-  }
+  std::vector<int> hs, ws;
+  ragged_sizes(images, n, &hs, &ws);
   std::vector<RaggedWindow> wins;
   std::vector<RaggedPass> passes;
   ragged_plan(hs.data(), ws.data(), n, tile_h, tile_w, ragged_pass_pixels(max_pass_pixels), &wins, &passes);
-  const size_t need = ragged_workspace(n, wins, passes);
-  if (workspace_bytes < need) {
-    set_error("ragged enhance workspace too small: %zu < %zu", workspace_bytes, need);
-    return WN_E_WORKSPACE;
-  }
-  int rc = get_encoder();
-  if (rc) return rc;
-  scheme = effective_scheme(h, scheme);
   // workspace: [LUTs of the n images][table: n RaggedImage | windows][one pass]
   uint8_t* pre_ws = (uint8_t*)align256((uintptr_t)workspace);
   const size_t pre_b = align256(preprocess_workspace_bytes(n, 1, 1));
   uint8_t* table = pre_ws + pre_b;
-  const size_t img_b = align256((size_t)n * sizeof(RaggedImage));
-  void* fwd_ws = table + ragged_table_bytes(n, wins.size());
-  std::vector<uint8_t> host(img_b + wins.size() * sizeof(RaggedWindow));
-  RaggedImage* imgs = reinterpret_cast<RaggedImage*>(host.data());
-  int max_slabs = 1;
-  for (int i = 0; i < n; i++) {
-    imgs[i] = ragged_image(images[i].rgb, images[i].height, images[i].width);
-    max_slabs = imgs[i].slabs > max_slabs ? imgs[i].slabs : max_slabs;
-  }
-  for (RaggedWindow& w : wins) {
-    w.rgb = images[w.img].rgb;
-    w.out_u8 = images[w.img].out_u8;
-    w.out_f32 = images[w.img].out_f32;
-  }
-  memcpy(host.data() + img_b, wins.data(), wins.size() * sizeof(RaggedWindow));
-  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
-  WN_CUDA(cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
-  const RaggedImage* d_imgs = reinterpret_cast<const RaggedImage*>(table);
-  const RaggedWindow* d_wins = reinterpret_cast<const RaggedWindow*>(table + img_b);
-  if ((rc = preprocess_u8_ragged_luts(h, n, d_imgs, max_slabs, pre_ws, stream))) return rc;
-  const int64_t none[4][4] = {};
-  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
-  for (const RaggedPass& p : passes) {
-    FwdBuffers b = carve(fwd_ws, p.count, p.slot_h, p.slot_w);
-    WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));
-    rc = preprocess_u8_ragged_planes(h, n, d_imgs, d_wins + p.first, p.count, p.slot_h, p.slot_w, b.act0, pre_ws,
-                                     stream);
-    if (rc) return rc;
-    FwdOpts o;
-    o.scheme = scheme;
-    o.packed = true;
-    o.hi_only = true;
-    o.rwin = d_wins + p.first;
-    rc = umma_pass(h, no_in, none, nullptr, p.count, p.slot_h, p.slot_w, b, stream, o);
-    if (rc) return rc;
-  }
-  return mirror_overflow(h, scheme, stream);
+  HostTable t = ragged_u8_table(n, wins.size());
+  const RaggedImage* d_imgs = t.dev<RaggedImage>(table, 0);
+  const TableGeom geo = {t.dev<RaggedWindow>(table, 1), 0, 0, 0, tile_h, tile_w};
+  auto start = [&]() {
+    RaggedImage* imgs = t.part<RaggedImage>(0);
+    int max_slabs = 1;
+    for (int i = 0; i < n; i++) {
+      imgs[i] = ragged_image(images[i].rgb, images[i].height, images[i].width);
+      max_slabs = imgs[i].slabs > max_slabs ? imgs[i].slabs : max_slabs;
+    }
+    RaggedWindow* rw = t.part<RaggedWindow>(1);
+    for (size_t k = 0; k < wins.size(); k++) {
+      rw[k] = wins[k];
+      rw[k].rgb = images[wins[k].img].rgb;
+      rw[k].out_u8 = images[wins[k].img].out_u8;
+      rw[k].out_f32 = images[wins[k].img].out_f32;
+    }
+    const int rc = t.upload(table, stream);
+    return rc ? rc : preprocess_u8_ragged_luts(h, n, d_imgs, max_slabs, pre_ws, stream);
+  };
+  return forward_call(h, "ragged enhance", workspace_bytes, ragged_workspace(n, wins, passes), u8_opts(scheme), geo,
+                      passes, table + t.bytes(), nullptr, FwdOut(), stream, start,
+                      [&](const TableGeom& pg, const RaggedPass& p, FwdBuffers& b, FwdOpts&) {
+                        WN_CUDA(cudaMemsetAsync(b.exact_flag, 1, sizeof(int), stream));
+                        return preprocess_u8_slot_planes(h, pg, d_imgs, n, p.count, b.act0, pre_ws, stream);
+                      });
 }
 
 // The tiled form of umma_forward (fp32 tensors in): the windows of tiling.cuh, one pass of them at a time through
@@ -878,55 +875,28 @@ size_t umma_forward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int t
 int umma_forward_tiled(wn_handle* h, const float* const in[4], const int64_t in_strides[4][4], float* out, int n,
                        int H, int W, int tile_h, int tile_w, long long max_pass_pixels, void* workspace,
                        size_t workspace_bytes, cudaStream_t stream, int scheme, int stack, int which) {
-  if (!h->umma) {
-    set_error("tensor-core weights have not been packed");
-    return WN_E_STATE;
-  }
   const bool sub = stack != kStackAll;
-  const size_t need = umma_forward_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels, sub);
-  if (workspace_bytes < need) {
-    set_error("tiled forward workspace too small: %zu < %zu", workspace_bytes, need);
-    return WN_E_WORKSPACE;
-  }
-  int rc = get_encoder();
-  if (rc) return rc;
-  scheme = effective_scheme(h, scheme);
   const TileGeom g = tile_geom(H, W, tile_h, tile_w);
-  const long long total = (long long)n * g.ny * g.nx;
-  const long long per_pass = tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels);
-  const size_t win_px = (size_t)g.win_h * g.win_w;
+  const std::vector<RaggedPass> passes = window_passes(g, n, max_pass_pixels);
   uint8_t* base = (uint8_t*)align256((uintptr_t)workspace);
   int* exact = (int*)base;
-  float* refined = (float*)(base + 256);
-  void* fwd_ws = base + 256 + (sub ? align256(per_pass * win_px * 9 * sizeof(float)) : 0);
+  FwdOut f;
+  f.f32 = out;
+  f.refined = (float*)(base + 256);
+  f.which = which;
+  f.tiles = &g;
+  void* fwd_ws = base + 256 + (sub ? align256(largest_pass_pixels(passes) * 9 * sizeof(float)) : 0);
   const PackInArgs pa = pack_args(in, in_strides);
-  if ((rc = pack_inputs(h, whole_images(H, W), pa, n, nullptr, exact, stream))) return rc;
-  for (long long w0 = 0; w0 < total; w0 += per_pass) {
-    const int cur = (int)(total - w0 < per_pass ? total - w0 : per_pass);
-    const GridGeom geo = {g, w0};
-    FwdBuffers b = carve(fwd_ws, cur, g.win_h, g.win_w);
-    b.exact_flag = exact;
-    if ((rc = pack_inputs(h, geo, pa, cur, b.act0, nullptr, stream))) return rc;
-    FwdOpts o;
-    o.scheme = scheme;
-    o.packed = true;
-    o.stack = stack;
-    if (stack == kStackRefiners) b.refined = refined;
-    if (!sub) {
-      o.tiles = &g;
-      o.win0 = w0;
-    }
-    rc = umma_pass(h, in, in_strides, sub ? nullptr : out, cur, g.win_h, g.win_w, b, stream, o);
-    if (rc) return rc;
-    if (sub) {  // after the pass and its conditional bf16x3 re-run
-      TimedScope ts(h, kSlotGate, stream);
-      const bool maps = stack == kStackCmg;
-      store_kept_kernel<<<dim3((unsigned)((win_px + 255) / 256), cur), 256, 0, stream>>>(
-          maps ? b.cm : refined, maps ? 3 : 9, maps ? 0 : 3 * which, 3, out, geo);
-      WN_LAUNCH_CHECK(h);
-    }
-  }
-  return mirror_overflow(h, scheme, stream);
+  FwdOpts o;
+  o.scheme = scheme;
+  o.stack = stack;
+  return forward_call(
+      h, "tiled forward", workspace_bytes,
+      umma_forward_tiled_workspace_bytes(n, H, W, tile_h, tile_w, max_pass_pixels, sub), o, GridGeom{g, 0}, passes,
+      fwd_ws, exact, f, stream, [&] { return pack_inputs(h, whole_images(H, W), pa, n, nullptr, exact, stream); },
+      [&](const GridGeom& geo, const RaggedPass& p, FwdBuffers& b, FwdOpts&) {
+        return pack_inputs(h, geo, pa, p.count, b.act0, nullptr, stream);
+      });
 }
 
 // The ragged form of umma_forward (fp32 tensors in, wn_forward_ragged): the windows and passes of ragged_plan, as
@@ -936,13 +906,13 @@ int umma_forward_tiled(wn_handle* h, const float* const in[4], const int64_t in_
 // gate epilogue stores each window's kept rectangle into its image's `out` (RaggedWindow::out_f32).  The plan (one
 // PackInArgs per image, one descriptor per window) is copied into the workspace once per call, so the call cannot be
 // captured in a graph.  Workspace: [flag | table | the largest pass].
-static size_t ragged_fp32_table_bytes(int n, size_t windows) {
-  return align256(align256((size_t)n * sizeof(PackInArgs)) + windows * sizeof(RaggedWindow));
+static HostTable ragged_fp32_table(int n, size_t windows) {
+  return HostTable({(size_t)n * sizeof(PackInArgs), windows * sizeof(RaggedWindow)});
 }
 static size_t ragged_fp32_workspace(int n, const std::vector<RaggedWindow>& wins,
                                     const std::vector<RaggedPass>& passes) {
   return (size_t)largest_pass_pixels(passes) * kUmmaBytesPerPixel + 4096 + 256 +
-         ragged_fp32_table_bytes(n, wins.size()) + 1024;
+         ragged_fp32_table(n, wins.size()).bytes() + 1024;
 }
 
 size_t umma_forward_ragged_workspace_bytes(const int* hs, const int* ws, int n, int tile_h, int tile_w,
@@ -956,68 +926,51 @@ size_t umma_forward_ragged_workspace_bytes(const int* hs, const int* ws, int n, 
 int umma_forward_ragged(wn_handle* h, const wn_ragged_tensors* images, int n, int tile_h, int tile_w,
                         long long max_pass_pixels, void* workspace, size_t workspace_bytes, cudaStream_t stream,
                         int scheme) {
-  if (!h->umma) {
-    set_error("tensor-core weights have not been packed");
-    return WN_E_STATE;
-  }
-  std::vector<int> hs(n), ws(n);
-  for (int i = 0; i < n; i++) {
-    hs[i] = images[i].height;
-    ws[i] = images[i].width;
-  }
+  std::vector<int> hs, ws;
+  ragged_sizes(images, n, &hs, &ws);
   std::vector<RaggedWindow> wins;
   std::vector<RaggedPass> passes;
   ragged_plan(hs.data(), ws.data(), n, tile_h, tile_w, ragged_pass_pixels(max_pass_pixels), &wins, &passes);
-  const size_t need = ragged_fp32_workspace(n, wins, passes);
-  if (workspace_bytes < need) {
-    set_error("ragged forward workspace too small: %zu < %zu", workspace_bytes, need);
-    return WN_E_WORKSPACE;
-  }
-  int rc = get_encoder();
-  if (rc) return rc;
-  scheme = effective_scheme(h, scheme);
   uint8_t* base = (uint8_t*)align256((uintptr_t)workspace);
   int* exact = (int*)base;
   uint8_t* table = base + 256;
-  const size_t img_b = align256((size_t)n * sizeof(PackInArgs));
-  void* fwd_ws = table + ragged_fp32_table_bytes(n, wins.size());
-  std::vector<uint8_t> host(img_b + wins.size() * sizeof(RaggedWindow));
-  PackInArgs* imgs = reinterpret_cast<PackInArgs*>(host.data());
-  for (int i = 0; i < n; i++) {
-    const wn_ragged_tensors& t = images[i];
-    const float* in[4] = {t.x, t.wb, t.he, t.gc};
-    imgs[i] = pack_args(in, t.in_strides);
-  }
-  for (RaggedWindow& w : wins) w.out_f32 = images[w.img].out;
-  memcpy(host.data() + img_b, wins.data(), wins.size() * sizeof(RaggedWindow));
-  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `host` may go out of scope
-  WN_CUDA(cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, stream));
-  const PackInArgs* d_imgs = reinterpret_cast<const PackInArgs*>(table);
-  TableGeom geo = {reinterpret_cast<const RaggedWindow*>(table + img_b), 0, 0, 0, tile_h, tile_w};
-  WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
-  for (const RaggedPass& p : passes) {
-    geo.set_pass(p);
-    if ((rc = pack_inputs(h, geo, d_imgs, p.count, nullptr, exact, stream))) return rc;
-  }
-  const int64_t none[4][4] = {};
-  const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
-  for (const RaggedPass& p : passes) {
-    FwdBuffers b = carve(fwd_ws, p.count, p.slot_h, p.slot_w);
-    b.exact_flag = exact;
-    geo.set_pass(p);
-    // the fp8-correction scheme decides the first layer's form per window (kFmtPair8): its flags sit in the buffer
-    // of cmg.conv2's output, which nothing reads or writes before the first layer has run
-    int* slot_flags = scheme == 1 ? reinterpret_cast<int*>(b.a[2]) : nullptr;
-    if ((rc = pack_inputs(h, geo, d_imgs, p.count, b.act0, nullptr, stream, false, slot_flags))) return rc;
-    FwdOpts o;
-    o.scheme = scheme;
-    o.packed = true;
-    o.rwin = geo.rwin();
-    o.slot_levels = slot_flags;
-    rc = umma_pass(h, no_in, none, nullptr, p.count, p.slot_h, p.slot_w, b, stream, o);
+  HostTable t = ragged_fp32_table(n, wins.size());
+  const PackInArgs* d_imgs = t.dev<PackInArgs>(table, 0);
+  const TableGeom geo = {t.dev<RaggedWindow>(table, 1), 0, 0, 0, tile_h, tile_w};
+  auto start = [&]() {
+    PackInArgs* imgs = t.part<PackInArgs>(0);
+    for (int i = 0; i < n; i++) {
+      const wn_ragged_tensors& d = images[i];
+      const float* in[4] = {d.x, d.wb, d.he, d.gc};
+      imgs[i] = pack_args(in, d.in_strides);
+    }
+    RaggedWindow* rw = t.part<RaggedWindow>(1);
+    for (size_t k = 0; k < wins.size(); k++) {
+      rw[k] = wins[k];
+      rw[k].out_f32 = images[wins[k].img].out;
+    }
+    int rc = t.upload(table, stream);
     if (rc) return rc;
-  }
-  return mirror_overflow(h, scheme, stream);
+    WN_CUDA(cudaMemsetAsync(exact, 1, sizeof(int), stream));  // nonzero = "all inputs are 8-bit levels"
+    TableGeom fg = geo;
+    for (const RaggedPass& p : passes) {
+      fg.set_pass(p);
+      if ((rc = pack_inputs(h, fg, d_imgs, p.count, nullptr, exact, stream))) return rc;
+    }
+    return WN_OK;
+  };
+  FwdOpts o;
+  o.scheme = scheme;
+  return forward_call(h, "ragged forward", workspace_bytes, ragged_fp32_workspace(n, wins, passes), o, geo, passes,
+                      table + t.bytes(), exact, FwdOut(), stream, start,
+                      [&](const TableGeom& pg, const RaggedPass& p, FwdBuffers& b, FwdOpts& po) {
+                        // the fp8-correction scheme decides the first layer's form per window (kFmtPair8): its flags
+                        // sit in the buffer of cmg.conv2's output, which nothing reads or writes before the first
+                        // layer has run
+                        int* slot_flags = po.scheme == 1 ? reinterpret_cast<int*>(b.a[2]) : nullptr;
+                        po.slot_levels = slot_flags;
+                        return pack_inputs(h, pg, d_imgs, p.count, b.act0, nullptr, stream, false, slot_flags);
+                      });
 }
 
 int umma_f8_overflowed(const wn_handle* h) { return h->umma && h->umma->overflow_host ? *h->umma->overflow_host : 0; }

@@ -19,6 +19,8 @@
 #include <math.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace wn {
@@ -343,17 +345,28 @@ __device__ __forceinline__ void store_level_planes(uint4* planes, size_t n, size
   p[plane] = make_uint4(bf16_levels2(lv[8], lv[9]), bf16_levels2(lv[10], lv[11]), 0u, 0u);
 }
 
-// WIN (the tiled forward): blockIdx.y is window win0 + blockIdx.y of `tiles`; the kernel writes that window's operand
-// planes (out.planes only), reading the full image and interpolating its CLAHE tiles at image coordinates.
-// RAG (ragged batches): blockIdx.y is window wins[blockIdx.y], in a slot of tiles.win_h x tiles.win_w; the image and
-// its geometry come from the descriptors, and slot pixels outside the window's valid extent get zero planes.
-template <bool VEC4, bool WIN = false, bool RAG = false>
+// The image data of slot image `img`: one record for every image of a grid call (image i at rgb + i * H * W * 3), or
+// the ragged call's device table
+__device__ __forceinline__ RaggedImage slot_image(const RaggedImage& one, int img) {
+  RaggedImage r = one;
+  r.rgb += (size_t)img * one.H * one.W * 3;
+  return r;
+}
+__device__ __forceinline__ RaggedImage slot_image(const RaggedImage* imgs, int img) { return imgs[img]; }
+
+// Whole images (Geom = WholeImages): blockIdx.y is image blockIdx.y of rgb, H x W; the kernel writes any of `out`.
+// The slot form (Geom = GridGeom or TableGeom, tiling.cuh): blockIdx.y is slot blockIdx.y of geo, whose pixels take
+// their image and coordinates from geo.at and their image data from slot_image(imgs, ...); the kernel writes that
+// slot's operand planes (out.planes only), zeros beyond its valid extent, interpolating the CLAHE tiles at image
+// coordinates.
+struct WholeImages {};
+template <bool VEC4, class Geom = WholeImages, class Img = WholeImages>
 __global__ void __launch_bounds__(256)
 apply_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw,
              const Tables* __restrict__ tables, const uint8_t* __restrict__ clahe_lut,
-             const uint8_t* __restrict__ wb_lut, ApplyOut out, int iters, TileGeom tiles, long long win0,
-             const RaggedImage* __restrict__ imgs, const RaggedWindow* __restrict__ wins) {
-  static_assert(!(VEC4 && WIN) && !(VEC4 && RAG) && !(WIN && RAG), "one windowed form, without a vector path");
+             const uint8_t* __restrict__ wb_lut, ApplyOut out, int iters, Geom geo, Img imgs) {
+  constexpr bool SLOT = !std::is_same<Geom, WholeImages>::value;
+  static_assert(!(VEC4 && SLOT), "the slot form has no vector path");
   __shared__ __align__(16) uint8_t s_clahe[64 * 256];
   __shared__ __align__(16) uint8_t s_wb[768];
   __shared__ __align__(16) uint8_t s_gamma[256];
@@ -363,24 +376,24 @@ apply_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw,
   __shared__ int16_t s_ytab[256];
   __shared__ int16_t s_fytab[256];
   __shared__ float s_div[256];
-  TileWindow win = {};
-  if constexpr (WIN) win = tile_window(tiles, win0 + blockIdx.y);
-  RaggedWindow rw = {};
-  if constexpr (RAG) {
-    rw = wins[blockIdx.y];
-    const RaggedImage im = imgs[rw.img];
+  int n = blockIdx.y;
+  if constexpr (SLOT) {
+    n = geo.at(blockIdx.y, 0).img;
+    const RaggedImage im = slot_image(imgs, n);
     rgb = im.rgb;
     H = im.H;
     W = im.W;
     th = im.th;
     tw = im.tw;
   }
-  const int tid = threadIdx.x, n = WIN ? win.img : RAG ? rw.img : blockIdx.y;
+  const int tid = threadIdx.x;
+  // a slot's image index comes from memory: as unsigned, its LUT offset needs no sign extension (which ptxas spills)
+  const size_t lut = SLOT ? (size_t)(unsigned)n : (size_t)n;
   {
-    const uint4* src = reinterpret_cast<const uint4*>(clahe_lut + (size_t)n * 64 * 256);
+    const uint4* src = reinterpret_cast<const uint4*>(clahe_lut + lut * 64 * 256);
     uint4* dst = reinterpret_cast<uint4*>(s_clahe);
     for (int i = tid; i < 1024; i += 256) dst[i] = src[i];
-    const uint32_t* wsrc = reinterpret_cast<const uint32_t*>(wb_lut + (size_t)n * 768);
+    const uint32_t* wsrc = reinterpret_cast<const uint32_t*>(wb_lut + lut * 768);
     for (int i = tid; i < 192; i += 256) reinterpret_cast<uint32_t*>(s_wb)[i] = wsrc[i];
     const uint4* isrc = reinterpret_cast<const uint4*>(tables->igtab);
     for (int i = tid; i < 256; i += 256) reinterpret_cast<uint4*>(s_igtab)[i] = isrc[i];
@@ -462,31 +475,17 @@ apply_kernel(const uint8_t* __restrict__ rgb, int H, int W, int th, int tw,
         q[2] = (uint32_t)a2[2] | ((uint32_t)a3[0] << 8) | ((uint32_t)a3[1] << 16) | ((uint32_t)a3[2] << 24);
       }
     }
-  } else if constexpr (WIN) {
-    // pixel pix of the window is image pixel (ys + y, xs + x); planes [window of the pass][2][win_h * win_w]
-    const int wplane = tiles.win_h * tiles.win_w;
+  } else if constexpr (SLOT) {
+    // planes [slot][2][slot pixels]
+    const int wplane = geo.slot_hw();
     for (int it = 0; it < iters; it++) {
       const int pix = (blockIdx.x * iters + it) * 256 + tid;
       if (pix >= wplane) break;
-      const int wy = pix / tiles.win_w;
-      const int ipix = (win.ys + wy) * W + win.xs + (pix - wy * tiles.win_w);
-      const uint8_t* p = rgb + ((size_t)n * plane + ipix) * 3;
-      int lv[12];
-      one_pixel(ipix, p[0], p[1], p[2], lv);
-      store_level_planes(out.planes, blockIdx.y, wplane, pix, lv);
-    }
-  } else if constexpr (RAG) {
-    // slot pixel (sy, sx) is image pixel (ys + sy, xs + sx) inside the valid extent; planes [slot][2][slot pixels]
-    const int wplane = tiles.win_h * tiles.win_w;
-    for (int it = 0; it < iters; it++) {
-      const int pix = (blockIdx.x * iters + it) * 256 + tid;
-      if (pix >= wplane) break;
-      const int sy = pix / tiles.win_w, sx = pix - sy * tiles.win_w;
-      int lv[12] = {};  // zero operands outside the window: what the tiled call's TMA reads beyond its window
-      if (sy < rw.vh && sx < rw.vw) {
-        const int ipix = (rw.ys + sy) * W + rw.xs + sx;
-        const uint8_t* p = rgb + (size_t)ipix * 3;
-        one_pixel(ipix, p[0], p[1], p[2], lv);
+      const SlotPixel p = geo.at(blockIdx.y, pix);
+      int lv[12] = {};  // zero operands beyond the valid extent: what the tiled call's TMA reads beyond its window
+      if (p.valid) {
+        const uint8_t* q = rgb + p.o * 3;
+        one_pixel((int)p.o, q[0], q[1], q[2], lv);
       }
       store_level_planes(out.planes, blockIdx.y, wplane, pix, lv);
     }
@@ -692,7 +691,6 @@ static int preprocess_run(wn_handle* h, const uint8_t* rgb, int n, int H, int W,
   if (rc) return rc;
   const uint8_t* clahe_lut = b.clahe_lut;
   const uint8_t* wb_lut = b.wb_lut;
-  const TileGeom untiled = {};
   ApplyOut ao;
   ao.f32[0] = x; ao.f32[1] = wb; ao.f32[2] = he; ao.f32[3] = gc;
   ao.u8[0] = wb_u8; ao.u8[1] = he_u8; ao.u8[2] = gc_u8;
@@ -707,13 +705,13 @@ static int preprocess_run(wn_handle* h, const uint8_t* rgb, int n, int H, int W,
     const int per_cta = 256 * iters * 4;
     apply_kernel<true><<<dim3((H * W + per_cta - 1) / per_cta, n), 256, 0, stream>>>(rgb, H, W, g.th, g.tw, h->d_tables,
                                                                                    clahe_lut, wb_lut, ao, iters,
-                                                                                   untiled, 0, nullptr, nullptr);
+                                                                                   WholeImages(), WholeImages());
   } else {
     const int iters = apply_iters((long long)n * H * W, h->sm_count);
     const int per_cta = 256 * iters;
     apply_kernel<false><<<dim3((H * W + per_cta - 1) / per_cta, n), 256, 0, stream>>>(rgb, H, W, g.th, g.tw, h->d_tables,
                                                                                     clahe_lut, wb_lut, ao, iters,
-                                                                                    untiled, 0, nullptr, nullptr);
+                                                                                    WholeImages(), WholeImages());
   }
   WN_LAUNCH_CHECK(h);
   return WN_OK;
@@ -724,23 +722,6 @@ int preprocess_u8_luts(wn_handle* h, const uint8_t* rgb, int n, int H, int W, vo
   const int rc = preprocess_check(n, H, W, workspace_bytes);
   if (rc) return rc;
   return preprocess_luts(h, rgb, n, H, W, geometry(H, W), pre_carve(workspace, n), stream, 0);
-}
-
-int preprocess_u8_window_planes(wn_handle* h, const uint8_t* rgb, int n, const TileGeom& tiles, long long win0,
-                                int count, uint4* planes, void* workspace, cudaStream_t stream) {
-  const PreGeom g = geometry(tiles.H, tiles.W);
-  const PreBufs b = pre_carve(workspace, n);
-  ApplyOut ao;
-  memset(&ao, 0, sizeof(ao));
-  ao.planes = planes;
-  TimedScope ts(h, kSlotApply, stream);
-  const int wplane = tiles.win_h * tiles.win_w;
-  const int iters = apply_iters((long long)count * wplane, h->sm_count);
-  const int per_cta = 256 * iters;
-  apply_kernel<false, true><<<dim3((wplane + per_cta - 1) / per_cta, count), 256, 0, stream>>>(
-      rgb, tiles.H, tiles.W, g.th, g.tw, h->d_tables, b.clahe_lut, b.wb_lut, ao, iters, tiles, win0, nullptr, nullptr);
-  WN_LAUNCH_CHECK(h);
-  return WN_OK;
 }
 
 // the stats grid of one image, as preprocess_luts sizes it
@@ -779,24 +760,26 @@ int preprocess_u8_ragged_luts(wn_handle* h, int n, const RaggedImage* imgs, int 
   return WN_OK;
 }
 
-int preprocess_u8_ragged_planes(wn_handle* h, int n, const RaggedImage* imgs, const RaggedWindow* wins, int count,
-                                int slot_h, int slot_w, uint4* planes, void* workspace, cudaStream_t stream) {
+template <class Geom, class Img>
+int preprocess_u8_slot_planes(wn_handle* h, const Geom& geo, const Img& imgs, int n, int count, uint4* planes,
+                              void* workspace, cudaStream_t stream) {
   const PreBufs b = pre_carve(workspace, n);
   ApplyOut ao;
   memset(&ao, 0, sizeof(ao));
   ao.planes = planes;
-  TileGeom slot = {};
-  slot.win_h = slot_h;
-  slot.win_w = slot_w;
   TimedScope ts(h, kSlotApply, stream);
-  const int wplane = slot_h * slot_w;
+  const int wplane = geo.slot_hw();
   const int iters = apply_iters((long long)count * wplane, h->sm_count);
   const int per_cta = 256 * iters;
-  apply_kernel<false, false, true><<<dim3((wplane + per_cta - 1) / per_cta, count), 256, 0, stream>>>(
-      nullptr, 0, 0, 0, 0, h->d_tables, b.clahe_lut, b.wb_lut, ao, iters, slot, 0, imgs, wins);
+  apply_kernel<false><<<dim3((wplane + per_cta - 1) / per_cta, count), 256, 0, stream>>>(
+      nullptr, 0, 0, 0, 0, h->d_tables, b.clahe_lut, b.wb_lut, ao, iters, geo, imgs);
   WN_LAUNCH_CHECK(h);
   return WN_OK;
 }
+template int preprocess_u8_slot_planes(wn_handle*, const GridGeom&, const RaggedImage&, int, int, uint4*, void*,
+                                       cudaStream_t);
+template int preprocess_u8_slot_planes(wn_handle*, const TableGeom&, const RaggedImage* const&, int, int, uint4*,
+                                       void*, cudaStream_t);
 
 // ---------------------------------------------------------------------------
 // cv2.resize(img, (w, h)) of 8-bit images, default INTER_LINEAR (training_utils.py:94-103), batched: every source

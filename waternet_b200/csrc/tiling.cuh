@@ -185,6 +185,14 @@ inline long long largest_pass_pixels(const std::vector<RaggedPass>& passes) {
   return px;
 }
 
+// the passes of `total` slots of one grid geometry, slots [first, first + per_pass) each
+inline std::vector<RaggedPass> grid_passes(long long total, long long per_pass, int slot_h, int slot_w) {
+  std::vector<RaggedPass> passes;
+  for (long long first = 0; first < total; first += per_pass)
+    passes.push_back({first, (int)std::min(per_pass, total - first), slot_h, slot_w});
+  return passes;
+}
+
 // ---- slot geometry: where pixel pix of slot s of a pass sits in its image ----
 // A pass runs a batch of slots, each holding one window (or one whole image) at its top-left.  Every per-pixel kernel
 // of a pass that reads or writes image coordinates (the operand packing, the kept-rectangle store, the backward's
