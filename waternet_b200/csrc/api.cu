@@ -21,6 +21,9 @@ static int resolve_mode(int mode) {
   return mode;
 }
 
+// the tensor-core scheme of a mode: 1 = fp8 corrections, 0 = bf16x3
+static int scheme_of(int mode) { return resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0; }
+
 struct DeviceGuard {
   int prev = -1;
   bool ok = true;
@@ -30,6 +33,178 @@ struct DeviceGuard {
   }
   ~DeviceGuard() {
     if (prev >= 0) cudaSetDevice(prev);
+  }
+};
+
+// ---- the argument checks of the entry points, one helper per kind.  Each returns WN_OK or the error code with
+// wn_last_error() set; `what` names the entry point in the message.
+static bool all_set(std::initializer_list<const void*> ptrs) {
+  for (const void* p : ptrs)
+    if (!p) return false;
+  return true;
+}
+
+static int invalid(const char* what, const char* msg) {
+  set_error("%s: %s", what, msg);
+  return WN_E_INVALID;
+}
+
+static int check_ptrs(const char* what, std::initializer_list<const void*> ptrs, const char* msg = "null argument") {
+  return all_set(ptrs) ? WN_OK : invalid(what, msg);
+}
+
+// the calls that fold their pointers, their shape and `ok` into one "bad argument"
+static int check_args(const char* what, std::initializer_list<const void*> ptrs, int n, int height, int width,
+                      bool ok = true) {
+  return all_set(ptrs) && n > 0 && height > 0 && width > 0 && ok ? WN_OK : invalid(what, "bad argument");
+}
+
+static int check_shape(const char* what, int n, int height, int width) {
+  if (n > 0 && height > 0 && width > 0) return WN_OK;
+  set_error("%s: bad shape n=%d h=%d w=%d", what, n, height, width);
+  return WN_E_INVALID;
+}
+
+static int check_tiled_shape(const char* what, int n, int height, int width, int tile_h, int tile_w,
+                             long long max_pass_pixels) {
+  if (n > 0 && height > 0 && width > 0 && tile_h > 0 && tile_w > 0 && max_pass_pixels >= 0) return WN_OK;
+  set_error("%s: bad shape n=%d h=%d w=%d tile=%dx%d max_pass_pixels=%lld", what, n, height, width, tile_h, tile_w,
+            max_pass_pixels);
+  return WN_E_INVALID;
+}
+
+// the image count and tiling of a ragged call
+static int check_ragged_shape(const char* what, int n, int tile_h, int tile_w, long long max_pass_pixels) {
+  if (n <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
+    set_error("%s: bad shape n=%d tile=%dx%d max_pass_pixels=%lld", what, n, tile_h, tile_w, max_pass_pixels);
+    return WN_E_INVALID;
+  }
+  if (n > 65535) {
+    set_error("%s: too many images: n=%d", what, n);
+    return WN_E_UNSUPPORTED;
+  }
+  return WN_OK;
+}
+
+// one image per grid row of the per-pixel kernels
+static int check_images_per_call(const char* what, int n) {
+  if (n <= 65535) return WN_OK;
+  set_error("%s: at most 65535 images per call, got n=%d", what, n);
+  return WN_E_UNSUPPORTED;
+}
+
+static int check_ragged_count(const char* what, int n) {
+  if (n > 0 && n <= 65535) return WN_OK;
+  set_error("%s: 1..65535 images per call, got n=%d", what, n);
+  return n <= 0 ? WN_E_INVALID : WN_E_UNSUPPORTED;
+}
+
+// the image-size limit: a plane's element index fits an int
+static bool too_large(int height, int width) { return (size_t)height * width > (size_t)0x7fffffff / 3; }
+
+static int check_size(int n, int height, int width) {
+  if (!too_large(height, width) && n <= 65535) return WN_OK;
+  set_error("image too large: n=%d h=%d w=%d", n, height, width);
+  return WN_E_UNSUPPORTED;
+}
+
+// the size of image i of a ragged batch
+static int check_ragged_size(const char* what, int i, int height, int width) {
+  if (height <= 0 || width <= 0) {
+    set_error("%s: bad size of image %d: h=%d w=%d", what, i, height, width);
+    return WN_E_INVALID;
+  }
+  if (too_large(height, width)) {
+    set_error("image too large: image %d h=%d w=%d", i, height, width);
+    return WN_E_UNSUPPORTED;
+  }
+  return WN_OK;
+}
+
+static int check_packed(const char* what, const wn_handle* h) {
+  if (h->packed) return WN_OK;
+  set_error("%s: wn_pack_weights has not been called", what);
+  return WN_E_STATE;
+}
+
+static int check_workspace(const char* what, size_t have, size_t need) {
+  if (have >= need) return WN_OK;
+  set_error("%s: workspace too small", what);
+  return WN_E_WORKSPACE;
+}
+
+// The scheme of a mode (scheme_of), kSchemeSimt for WN_MODE_FP32_SIMT when `simt_refusal` is NULL, or the error:
+// WN_E_UNSUPPORTED with "<what>: <simt_refusal>" for WN_MODE_FP32_SIMT, WN_E_INVALID for an unknown mode.
+// Errors are negative.
+constexpr int kSchemeSimt = 2;
+static int check_mode(const char* what, int mode, const char* simt_refusal) {
+  const int m = resolve_mode(mode);
+  if (m == WN_MODE_FP32_SIMT) {
+    if (!simt_refusal) return kSchemeSimt;
+    set_error("%s: %s", what, simt_refusal);
+    return WN_E_UNSUPPORTED;
+  }
+  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) {
+    set_error("%s: unknown mode %d", what, mode);
+    return WN_E_INVALID;
+  }
+  return scheme_of(mode);
+}
+constexpr const char* kTiledRefusal = "the tiled forward runs in the tensor-core modes only, not WN_MODE_FP32_SIMT";
+constexpr const char* kRaggedRefusal = "ragged batches run in the tensor-core modes only, not WN_MODE_FP32_SIMT";
+
+// entries [first, first + count) of a host array of device pointers (params, grads, input_grads, grad_out_host)
+template <class P>
+static int check_entries(const char* what, const char* name, P const* a, int first, int count) {
+  for (int i = first; i < first + count; i++)
+    if (!a[i]) {
+      set_error("%s: %s[%d] is NULL", what, name, i);
+      return WN_E_INVALID;
+    }
+  return WN_OK;
+}
+
+// the backward calls: the parameter gradients [first, first + count) they write must be given
+static int check_param_grads(const char* what, float* const* grads, int first, int count) {
+  return check_entries(what, "grads", grads, first, count);
+}
+
+// the optional input gradients of the backward calls of WaterNet: all four or none
+static int check_input_grads(const char* what, float* const* input_grads) {
+  return input_grads ? check_entries(what, "input_grads", input_grads, 0, 4) : WN_OK;
+}
+
+// The images of a ragged table in order: `given(image, i)` says whether image i's device pointers are given; with
+// `sizes` its size is checked after them.
+template <class Image, class Given>
+static int check_images(const char* what, const Image* images, int n, bool sizes, Given given) {
+  for (int i = 0; i < n; i++) {
+    if (!given(images[i], i)) {
+      set_error("%s: null image pointer (image %d)", what, i);
+      return WN_E_INVALID;
+    }
+    int rc = sizes ? check_ragged_size(what, i, images[i].height, images[i].width) : WN_OK;
+    if (rc) return rc;
+  }
+  return WN_OK;
+}
+static bool inputs_given(const wn_ragged_tensors& t) { return t.x && t.wb && t.he && t.gc; }
+
+static int check_which(const char* what, int which) {
+  if (which >= 0 && which <= 2) return WN_OK;
+  set_error("%s: which must be 0, 1 or 2, got %d", what, which);
+  return WN_E_INVALID;
+}
+static bool submodule_stack(int stack) { return stack == 0 || stack == 1; }
+
+// Refiner r sees cat[x, input r+1] (net.py:101-103): the refiner stack gets xbar in every slot after x, with the
+// strides {x, xbar} of in_strides[2][4] spread to the [4][4] the stack takes.
+struct RefinerInputs {
+  const float* in[4];
+  int64_t st[4][4];
+  RefinerInputs(const float* x, const float* xbar, const int64_t in_strides[2][4]) : in{x, xbar, xbar, xbar} {
+    for (int t = 0; t < 4; t++)
+      for (int k = 0; k < 4; k++) st[t][k] = in_strides[t == 0 ? 0 : 1][k];
   }
 };
 
@@ -45,10 +220,8 @@ const char* wn_last_error(void) { return g_err; }
 
 int wn_build_tables_host(uint16_t* gtab, uint16_t* ctab, int16_t* ytab, int16_t* fytab,
                          uint8_t* igtab, uint8_t* gamma, float* div255) {
-  if (!gtab || !ctab || !ytab || !fytab || !igtab || !gamma || !div255) {
-    set_error("wn_build_tables_host: null output");
-    return WN_E_INVALID;
-  }
+  int rc = check_ptrs("wn_build_tables_host", {gtab, ctab, ytab, fytab, igtab, gamma, div255}, "null output");
+  if (rc) return rc;
   Tables* t = (Tables*)malloc(sizeof(Tables));
   build_tables_host(t);
   memcpy(gtab, t->gtab, sizeof(t->gtab));
@@ -118,17 +291,11 @@ void wn_destroy(wn_handle* h) {
 }
 
 int wn_pack_weights(wn_handle* h, const float* const* params, void* stream) {
-  if (!h || !params) {
-    set_error("wn_pack_weights: null argument");
-    return WN_E_INVALID;
-  }
-  for (int i = 0; i < WN_NUM_PARAMS; i++)
-    if (!params[i]) {
-      set_error("wn_pack_weights: params[%d] is NULL", i);
-      return WN_E_INVALID;
-    }
+  const char* what = "wn_pack_weights";
+  int rc = check_ptrs(what, {h, params});
+  if (rc || (rc = check_entries(what, "params", params, 0, WN_NUM_PARAMS))) return rc;
   DeviceGuard guard(h->device);
-  int rc = simt_pack_weights(h, params, (cudaStream_t)stream);
+  rc = simt_pack_weights(h, params, (cudaStream_t)stream);
   if (rc) return rc;
   rc = umma_pack_weights(h, params, (cudaStream_t)stream);
   if (rc) return rc;
@@ -151,33 +318,16 @@ size_t wn_forward_workspace_bytes(int n, int h, int w, int mode) {
 int wn_forward(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
                const int64_t in_strides[4][4], float* out, int n, int height, int width, int mode,
                void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !x || !wb || !he || !gc || !in_strides || !out || !workspace) {
-    set_error("wn_forward: null argument");
-    return WN_E_INVALID;
-  }
-  if (n <= 0 || height <= 0 || width <= 0) {
-    set_error("wn_forward: bad shape n=%d h=%d w=%d", n, height, width);
-    return WN_E_INVALID;
-  }
-  if (!h->packed) {
-    set_error("wn_forward: wn_pack_weights has not been called");
-    return WN_E_STATE;
-  }
+  const char* what = "wn_forward";
+  int rc = check_ptrs(what, {h, x, wb, he, gc, in_strides, out, workspace});
+  if (rc || (rc = check_shape(what, n, height, width)) || (rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
-  switch (resolve_mode(mode)) {
-    case WN_MODE_FP32_SIMT:
-      return simt_forward(h, in, in_strides, out, n, height, width, workspace, workspace_bytes,
-                          (cudaStream_t)stream);
-    case WN_MODE_BF16X3:
-      return umma_forward(h, in, in_strides, out, n, height, width, workspace, workspace_bytes,
-                          (cudaStream_t)stream, 0);
-    case WN_MODE_BF16_FP8:
-      return umma_forward(h, in, in_strides, out, n, height, width, workspace, workspace_bytes,
-                          (cudaStream_t)stream, 1);
-  }
-  set_error("wn_forward: unknown mode %d", mode);
-  return WN_E_INVALID;
+  const int s = check_mode(what, mode, nullptr);
+  if (s < 0) return s;
+  if (s == kSchemeSimt)
+    return simt_forward(h, in, in_strides, out, n, height, width, workspace, workspace_bytes, (cudaStream_t)stream);
+  return umma_forward(h, in, in_strides, out, n, height, width, workspace, workspace_bytes, (cudaStream_t)stream, s);
 }
 
 size_t wn_preprocess_workspace_bytes(int n, int h, int w) {
@@ -188,14 +338,9 @@ size_t wn_preprocess_workspace_bytes(int n, int h, int w) {
 int wn_preprocess_u8(wn_handle* h, const uint8_t* rgb, int n, int height, int width, float* x,
                      float* wb, float* he, float* gc, uint8_t* wb_u8, uint8_t* he_u8,
                      uint8_t* gc_u8, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !rgb || !workspace) {
-    set_error("wn_preprocess_u8: null argument");
-    return WN_E_INVALID;
-  }
-  if (n <= 0 || height <= 0 || width <= 0) {
-    set_error("wn_preprocess_u8: bad shape n=%d h=%d w=%d", n, height, width);
-    return WN_E_INVALID;
-  }
+  const char* what = "wn_preprocess_u8";
+  int rc = check_ptrs(what, {h, rgb, workspace});
+  if (rc || (rc = check_shape(what, n, height, width))) return rc;
   DeviceGuard guard(h->device);
   return preprocess_u8(h, rgb, n, height, width, x, wb, he, gc, wb_u8, he_u8, gc_u8, workspace,
                        workspace_bytes, (cudaStream_t)stream);
@@ -203,10 +348,8 @@ int wn_preprocess_u8(wn_handle* h, const uint8_t* rgb, int n, int height, int wi
 
 int wn_postprocess_u8(wn_handle* h, const float* out_nchw, uint8_t* out_nhwc, int n, int height,
                       int width, void* stream) {
-  if (!h || !out_nchw || !out_nhwc || n <= 0 || height <= 0 || width <= 0) {
-    set_error("wn_postprocess_u8: bad argument");
-    return WN_E_INVALID;
-  }
+  int rc = check_args("wn_postprocess_u8", {h, out_nchw, out_nhwc}, n, height, width);
+  if (rc) return rc;
   DeviceGuard guard(h->device);
   return postprocess_u8(h, out_nchw, out_nhwc, n, height, width, (cudaStream_t)stream);
 }
@@ -218,24 +361,16 @@ size_t wn_white_balance_gray_workspace_bytes(int n, int h, int w) {
 
 int wn_white_balance_gray_u8(wn_handle* h, const uint8_t* gray, uint8_t* out, int n, int height, int width,
                              void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !gray || !out || !workspace || n <= 0 || height <= 0 || width <= 0) {
-    set_error("wn_white_balance_gray_u8: bad argument");
-    return WN_E_INVALID;
-  }
-  if ((size_t)height * width > (size_t)0x7fffffff / 3 || n > 65535) {
-    set_error("image too large: n=%d h=%d w=%d", n, height, width);
-    return WN_E_UNSUPPORTED;
-  }
+  int rc = check_args("wn_white_balance_gray_u8", {h, gray, out, workspace}, n, height, width);
+  if (rc || (rc = check_size(n, height, width))) return rc;
   DeviceGuard guard(h->device);
   return white_balance_gray_u8(h, gray, out, n, height, width, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int wn_resize_u8(wn_handle* h, const uint8_t* const* src_dev, const int* src_h, const int* src_w, int n,
                  uint8_t* dst_nhwc, int dst_h, int dst_w, int swap_rb, void* stream) {
-  if (!h || !src_dev || !src_h || !src_w || !dst_nhwc || n <= 0 || dst_h <= 0 || dst_w <= 0) {
-    set_error("wn_resize_u8: bad argument");
-    return WN_E_INVALID;
-  }
+  int rc = check_args("wn_resize_u8", {h, src_dev, src_h, src_w, dst_nhwc}, n, dst_h, dst_w);
+  if (rc) return rc;
   DeviceGuard guard(h->device);
   return resize_u8(h, src_dev, src_h, src_w, n, dst_nhwc, dst_h, dst_w, swap_rb, (cudaStream_t)stream);
 }
@@ -277,30 +412,16 @@ int wn_enhance_u8_peers(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, flo
     peers.p[k] = peer_out[k];
   }
   peers.n = n_peers;
-  if (!h || !rgb || !out_nhwc || !workspace) {
-    set_error("wn_enhance_u8: null argument");
-    return WN_E_INVALID;
-  }
-  if (n <= 0 || height <= 0 || width <= 0) {
-    set_error("wn_enhance_u8: bad shape n=%d h=%d w=%d", n, height, width);
-    return WN_E_INVALID;
-  }
-  if (!h->packed) {
-    set_error("wn_enhance_u8: wn_pack_weights has not been called");
-    return WN_E_STATE;
-  }
-  if (workspace_bytes < wn_enhance_workspace_bytes(n, height, width, mode)) {
-    set_error("wn_enhance_u8: workspace too small");
-    return WN_E_WORKSPACE;
-  }
-  if ((size_t)height * width > (size_t)0x7fffffff / 3 || n > 65535) {
-    set_error("image too large: n=%d h=%d w=%d", n, height, width);
-    return WN_E_UNSUPPORTED;
-  }
+  const char* what = "wn_enhance_u8";
+  int rc = check_ptrs(what, {h, rgb, out_nhwc, workspace});
+  if (rc || (rc = check_shape(what, n, height, width)) || (rc = check_packed(what, h)) ||
+      (rc = check_workspace(what, workspace_bytes, wn_enhance_workspace_bytes(n, height, width, mode))) ||
+      (rc = check_size(n, height, width)))
+    return rc;
   DeviceGuard guard(h->device);
   if (resolve_mode(mode) != WN_MODE_FP32_SIMT)  // tensor-core modes: folded path, nothing fp32 is materialised
     return umma_enhance_u8(h, rgb, out_nhwc, out_f32_or_null, n, height, width, workspace, workspace_bytes,
-                           (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0, peers);
+                           (cudaStream_t)stream, scheme_of(mode), peers);
   uint8_t* ws = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
   const size_t tens = align256((size_t)n * 3 * height * width * sizeof(float));
   float* t[5];
@@ -313,8 +434,8 @@ int wn_enhance_u8_peers(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, flo
   ws += pre_b;
   void* fwd_ws = ws;
   size_t fwd_b = align256(simt_forward_workspace_bytes(n, height, width));
-  int rc = wn_preprocess_u8(h, rgb, n, height, width, t[0], t[1], t[2], t[3], nullptr, nullptr,
-                            nullptr, pre_ws, pre_b, stream);
+  rc = wn_preprocess_u8(h, rgb, n, height, width, t[0], t[1], t[2], t[3], nullptr, nullptr,
+                        nullptr, pre_ws, pre_b, stream);
   if (rc) return rc;
   const int64_t hw = (int64_t)height * width;
   const int64_t st[4][4] = {{3 * hw, hw, width, 1}, {3 * hw, hw, width, 1}, {3 * hw, hw, width, 1},
@@ -327,149 +448,104 @@ int wn_enhance_u8_peers(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, flo
   return mirror_u8(h, out_nhwc, peers, (size_t)n * height * width * 3, nullptr, (cudaStream_t)stream);
 }
 
+// ---- the tiled forward (wn_enhance_u8_tiled, and WaterNet.forward and its sub-modules in windows)
+// the argument checks the tiled forward calls and the three tiled workspace functions share (pointers aside):
+// the scheme, or the (negative) error
+static int forward_tiled_check(const char* what, int n, int height, int width, int tile_h, int tile_w,
+                               long long max_pass_pixels, int mode) {
+  int rc = check_tiled_shape(what, n, height, width, tile_h, tile_w, max_pass_pixels);
+  if (rc) return rc;
+  const int s = check_mode(what, mode, kTiledRefusal);
+  if (s < 0) return s;
+  return (rc = check_size(n, height, width)) ? rc : s;
+}
+
 size_t wn_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
                                         int mode) {
-  const int m = resolve_mode(mode);
-  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) return 0;
+  if (forward_tiled_check("wn_enhance_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels, mode) < 0)
+    return 0;
   return umma_enhance_tiled_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels);
 }
 
 int wn_enhance_u8_tiled(wn_handle* h, const uint8_t* rgb, uint8_t* out_nhwc, float* out_f32_or_null, int n,
                         int height, int width, int tile_h, int tile_w, long long max_pass_pixels, int mode,
                         void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !rgb || !out_nhwc || !workspace) {
-    set_error("wn_enhance_u8_tiled: null argument");
-    return WN_E_INVALID;
-  }
-  if (n <= 0 || height <= 0 || width <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
-    set_error("wn_enhance_u8_tiled: bad shape n=%d h=%d w=%d tile=%dx%d max_pass_pixels=%lld", n, height, width,
-              tile_h, tile_w, max_pass_pixels);
-    return WN_E_INVALID;
-  }
-  const int m = resolve_mode(mode);
-  if (m == WN_MODE_FP32_SIMT) {
-    set_error("wn_enhance_u8_tiled: the tiled forward runs in the tensor-core modes only, not WN_MODE_FP32_SIMT");
-    return WN_E_UNSUPPORTED;
-  }
-  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) {
-    set_error("wn_enhance_u8_tiled: unknown mode %d", mode);
-    return WN_E_INVALID;
-  }
-  if (!h->packed) {
-    set_error("wn_enhance_u8_tiled: wn_pack_weights has not been called");
-    return WN_E_STATE;
-  }
-  if ((size_t)height * width > (size_t)0x7fffffff / 3 || n > 65535) {
-    set_error("image too large: n=%d h=%d w=%d", n, height, width);
-    return WN_E_UNSUPPORTED;
-  }
+  const char* what = "wn_enhance_u8_tiled";
+  int rc = check_ptrs(what, {h, rgb, out_nhwc, workspace});
+  if (rc || (rc = check_tiled_shape(what, n, height, width, tile_h, tile_w, max_pass_pixels))) return rc;
+  const int s = check_mode(what, mode, kTiledRefusal);
+  if (s < 0) return s;
+  if ((rc = check_packed(what, h)) || (rc = check_size(n, height, width))) return rc;
   DeviceGuard guard(h->device);
   return umma_enhance_u8_tiled(h, rgb, out_nhwc, out_f32_or_null, n, height, width, tile_h, tile_w, max_pass_pixels,
-                               workspace, workspace_bytes, (cudaStream_t)stream, m == WN_MODE_BF16_FP8 ? 1 : 0);
+                               workspace, workspace_bytes, (cudaStream_t)stream, s);
 }
 
-// the argument checks the ragged call and its workspace function share (the image pointers aside)
+// ---- ragged batches (wn_enhance_u8_ragged, wn_forward_ragged)
+// the argument checks the ragged calls and their workspace functions share (the images aside): the scheme, or the
+// (negative) error
 static int ragged_check(const char* what, int n, int tile_h, int tile_w, long long max_pass_pixels, int mode) {
-  if (n <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
-    set_error("%s: bad shape n=%d tile=%dx%d max_pass_pixels=%lld", what, n, tile_h, tile_w, max_pass_pixels);
-    return WN_E_INVALID;
-  }
-  if (n > 65535) {
-    set_error("%s: too many images: n=%d", what, n);
-    return WN_E_UNSUPPORTED;
-  }
-  const int m = resolve_mode(mode);
-  if (m == WN_MODE_FP32_SIMT) {
-    set_error("%s: ragged batches run in the tensor-core modes only, not WN_MODE_FP32_SIMT", what);
-    return WN_E_UNSUPPORTED;
-  }
-  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) {
-    set_error("%s: unknown mode %d", what, mode);
-    return WN_E_INVALID;
-  }
-  return WN_OK;
+  int rc = check_ragged_shape(what, n, tile_h, tile_w, max_pass_pixels);
+  return rc ? rc : check_mode(what, mode, kRaggedRefusal);
 }
-static int ragged_check_size(const char* what, int i, int height, int width) {
-  if (height <= 0 || width <= 0) {
-    set_error("%s: bad size of image %d: h=%d w=%d", what, i, height, width);
-    return WN_E_INVALID;
-  }
-  if ((size_t)height * width > (size_t)0x7fffffff / 3) {
-    set_error("image too large: image %d h=%d w=%d", i, height, width);
-    return WN_E_UNSUPPORTED;
-  }
-  return WN_OK;
+
+// the checks of a ragged workspace function: those of its call, with the sizes for the images
+static bool ragged_sizes_ok(const char* what, const int* hs, const int* ws, int n, int tile_h, int tile_w,
+                            long long max_pass_pixels, int mode) {
+  if (!hs || !ws || ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode) < 0) return false;
+  for (int i = 0; i < n; i++)
+    if (check_ragged_size(what, i, hs[i], ws[i])) return false;
+  return true;
 }
 
 size_t wn_enhance_ragged_workspace_bytes(const int* heights_host, const int* widths_host, int n, int tile_h,
                                          int tile_w, long long max_pass_pixels, int mode) {
-  const char* what = "wn_enhance_ragged_workspace_bytes";
-  if (!heights_host || !widths_host || ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode)) return 0;
-  for (int i = 0; i < n; i++)
-    if (ragged_check_size(what, i, heights_host[i], widths_host[i])) return 0;
+  if (!ragged_sizes_ok("wn_enhance_ragged_workspace_bytes", heights_host, widths_host, n, tile_h, tile_w,
+                       max_pass_pixels, mode))
+    return 0;
   return umma_enhance_ragged_workspace_bytes(heights_host, widths_host, n, tile_h, tile_w, max_pass_pixels);
 }
 
 int wn_enhance_u8_ragged(wn_handle* h, const wn_ragged_image* images_host, int n, int tile_h, int tile_w,
                          long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream) {
   const char* what = "wn_enhance_u8_ragged";
-  if (!h || !images_host || !workspace) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode);
+  int rc = check_ptrs(what, {h, images_host, workspace});
   if (rc) return rc;
-  for (int i = 0; i < n; i++) {
-    if (!images_host[i].rgb || !images_host[i].out_u8) {
-      set_error("%s: null image pointer (image %d)", what, i);
-      return WN_E_INVALID;
-    }
-    if ((rc = ragged_check_size(what, i, images_host[i].height, images_host[i].width))) return rc;
-  }
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  const int s = ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode);
+  if (s < 0) return s;
+  if ((rc = check_images(what, images_host, n, true,
+                         [](const wn_ragged_image& im, int) { return im.rgb && im.out_u8; })) ||
+      (rc = check_packed(what, h)))
+    return rc;
   DeviceGuard guard(h->device);
   return umma_enhance_u8_ragged(h, images_host, n, tile_h, tile_w, max_pass_pixels, workspace, workspace_bytes,
-                                (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0);
+                                (cudaStream_t)stream, s);
 }
 
 static_assert(sizeof(wn_ragged_tensors) == 176, "wn_ragged_tensors: _lib.RAGGED_TENSORS_BYTES restates this size");
 
 size_t wn_forward_ragged_workspace_bytes(const int* heights_host, const int* widths_host, int n, int tile_h,
                                          int tile_w, long long max_pass_pixels, int mode) {
-  const char* what = "wn_forward_ragged_workspace_bytes";
-  if (!heights_host || !widths_host || ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode)) return 0;
-  for (int i = 0; i < n; i++)
-    if (ragged_check_size(what, i, heights_host[i], widths_host[i])) return 0;
+  if (!ragged_sizes_ok("wn_forward_ragged_workspace_bytes", heights_host, widths_host, n, tile_h, tile_w,
+                       max_pass_pixels, mode))
+    return 0;
   return umma_forward_ragged_workspace_bytes(heights_host, widths_host, n, tile_h, tile_w, max_pass_pixels);
 }
 
 int wn_forward_ragged(wn_handle* h, const wn_ragged_tensors* images_host, int n, int tile_h, int tile_w,
                       long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream) {
   const char* what = "wn_forward_ragged";
-  if (!h || !images_host || !workspace) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode);
+  int rc = check_ptrs(what, {h, images_host, workspace});
   if (rc) return rc;
-  for (int i = 0; i < n; i++) {
-    const wn_ragged_tensors& t = images_host[i];
-    if (!t.x || !t.wb || !t.he || !t.gc || !t.out) {
-      set_error("%s: null image pointer (image %d)", what, i);
-      return WN_E_INVALID;
-    }
-    if ((rc = ragged_check_size(what, i, t.height, t.width))) return rc;
-  }
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  const int s = ragged_check(what, n, tile_h, tile_w, max_pass_pixels, mode);
+  if (s < 0) return s;
+  if ((rc = check_images(what, images_host, n, true,
+                         [](const wn_ragged_tensors& t, int) { return inputs_given(t) && t.out; })) ||
+      (rc = check_packed(what, h)))
+    return rc;
   DeviceGuard guard(h->device);
   return umma_forward_ragged(h, images_host, n, tile_h, tile_w, max_pass_pixels, workspace, workspace_bytes,
-                             (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0);
+                             (cudaStream_t)stream, s);
 }
 
 // ---- the reference's callable sub-modules (net.py:45-56 ConfidenceMapGenerator.forward, :75-80 Refiner.forward)
@@ -483,67 +559,42 @@ size_t wn_submodule_workspace_bytes(int n, int h, int w, int mode) {
 int wn_confidence_maps(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
                        const int64_t in_strides[4][4], float* out_maps, int n, int height, int width, int mode,
                        void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !x || !wb || !he || !gc || !in_strides || !out_maps || !workspace || n <= 0 || height <= 0 || width <= 0) {
-    set_error("wn_confidence_maps: bad argument");
-    return WN_E_INVALID;
-  }
-  if (!h->packed) {
-    set_error("wn_confidence_maps: wn_pack_weights has not been called");
-    return WN_E_STATE;
-  }
-  if (workspace_bytes < wn_submodule_workspace_bytes(n, height, width, mode)) {
-    set_error("wn_confidence_maps: workspace too small");
-    return WN_E_WORKSPACE;
-  }
+  const char* what = "wn_confidence_maps";
+  int rc = check_args(what, {h, x, wb, he, gc, in_strides, out_maps, workspace}, n, height, width);
+  if (rc || (rc = check_packed(what, h)) ||
+      (rc = check_workspace(what, workspace_bytes, wn_submodule_workspace_bytes(n, height, width, mode))))
+    return rc;
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
-  const int m = resolve_mode(mode);
-  if (m == WN_MODE_FP32_SIMT)
+  const int s = check_mode(what, mode, nullptr);
+  if (s == kSchemeSimt)
     return simt_forward(h, in, in_strides, out_maps, n, height, width, workspace, workspace_bytes,
                         (cudaStream_t)stream, kStackCmg, 0);
-  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) {
-    set_error("wn_confidence_maps: unknown mode %d", mode);
-    return WN_E_INVALID;
-  }
+  if (s < 0) return s;
   return umma_forward(h, in, in_strides, out_maps, n, height, width, workspace, workspace_bytes,
-                      (cudaStream_t)stream, m == WN_MODE_BF16_FP8 ? 1 : 0, kStackCmg, nullptr);
+                      (cudaStream_t)stream, s, kStackCmg, nullptr);
 }
 
 int wn_refine(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
               float* out, int n, int height, int width, int mode, void* workspace, size_t workspace_bytes,
               void* stream) {
-  if (!h || !x || !xbar || !in_strides || !out || !workspace || n <= 0 || height <= 0 || width <= 0 || which < 0 ||
-      which > 2) {
-    set_error("wn_refine: bad argument");
-    return WN_E_INVALID;
-  }
-  if (!h->packed) {
-    set_error("wn_refine: wn_pack_weights has not been called");
-    return WN_E_STATE;
-  }
-  if (workspace_bytes < wn_submodule_workspace_bytes(n, height, width, mode)) {
-    set_error("wn_refine: workspace too small");
-    return WN_E_WORKSPACE;
-  }
+  const char* what = "wn_refine";
+  int rc = check_args(what, {h, x, xbar, in_strides, out, workspace}, n, height, width, which >= 0 && which <= 2);
+  if (rc || (rc = check_packed(what, h)) ||
+      (rc = check_workspace(what, workspace_bytes, wn_submodule_workspace_bytes(n, height, width, mode))))
+    return rc;
   DeviceGuard guard(h->device);
-  // refiner r sees cat[x, input r+1] (net.py:101-103): hand xbar to every slot, keep refiner `which`
-  const float* in[4] = {x, xbar, xbar, xbar};
-  int64_t st[4][4];
-  for (int t = 0; t < 4; t++)
-    for (int k = 0; k < 4; k++) st[t][k] = in_strides[t == 0 ? 0 : 1][k];
-  const int m = resolve_mode(mode);
-  if (m == WN_MODE_FP32_SIMT)
-    return simt_forward(h, in, st, out, n, height, width, workspace, workspace_bytes, (cudaStream_t)stream,
+  const RefinerInputs r(x, xbar, in_strides);
+  const int s = check_mode(what, mode, nullptr);
+  if (s == kSchemeSimt)
+    return simt_forward(h, r.in, r.st, out, n, height, width, workspace, workspace_bytes, (cudaStream_t)stream,
                         kStackRefiners, which);
-  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) {
-    set_error("wn_refine: unknown mode %d", mode);
-    return WN_E_INVALID;
-  }
+  if (s < 0) return s;
   uint8_t* ws = (uint8_t*)(((uintptr_t)workspace + 255) / 256 * 256);
   const size_t fwd_b = align256(umma_forward_workspace_bytes(n, height, width));
   float* refined = (float*)(ws + fwd_b);
-  int rc = umma_forward(h, in, st, nullptr, n, height, width, ws, fwd_b, (cudaStream_t)stream,
-                        m == WN_MODE_BF16_FP8 ? 1 : 0, kStackRefiners, refined);
+  rc = umma_forward(h, r.in, r.st, nullptr, n, height, width, ws, fwd_b, (cudaStream_t)stream, s, kStackRefiners,
+                    refined);
   if (rc) return rc;
   const size_t img = (size_t)3 * height * width * sizeof(float);
   WN_CUDA(cudaMemcpy2DAsync(out, img, refined + (size_t)which * 3 * height * width, 3 * img, img, n,
@@ -552,102 +603,65 @@ int wn_refine(wn_handle* h, int which, const float* x, const float* xbar, const 
 }
 
 // ---- the tiled forward of fp32 tensors (WaterNet.forward and its sub-modules, in windows)
-// the argument checks the tiled forward calls and their workspace functions share (pointers aside)
-static int forward_tiled_check(const char* what, int n, int height, int width, int tile_h, int tile_w,
-                               long long max_pass_pixels, int mode) {
-  if (n <= 0 || height <= 0 || width <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
-    set_error("%s: bad shape n=%d h=%d w=%d tile=%dx%d max_pass_pixels=%lld", what, n, height, width, tile_h, tile_w,
-              max_pass_pixels);
-    return WN_E_INVALID;
-  }
-  const int m = resolve_mode(mode);
-  if (m == WN_MODE_FP32_SIMT) {
-    set_error("%s: the tiled forward runs in the tensor-core modes only, not WN_MODE_FP32_SIMT", what);
-    return WN_E_UNSUPPORTED;
-  }
-  if (m != WN_MODE_BF16X3 && m != WN_MODE_BF16_FP8) {
-    set_error("%s: unknown mode %d", what, mode);
-    return WN_E_INVALID;
-  }
-  if ((size_t)height * width > (size_t)0x7fffffff / 3 || n > 65535) {
-    set_error("image too large: n=%d h=%d w=%d", n, height, width);
-    return WN_E_UNSUPPORTED;
-  }
-  return WN_OK;
-}
-
 size_t wn_forward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
                                         int mode) {
-  if (forward_tiled_check("wn_forward_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels, mode)) return 0;
+  if (forward_tiled_check("wn_forward_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels, mode) < 0)
+    return 0;
   return umma_forward_tiled_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels, false);
 }
 
 size_t wn_submodule_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels,
                                           int mode) {
-  if (forward_tiled_check("wn_submodule_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels, mode))
+  if (forward_tiled_check("wn_submodule_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels, mode) < 0)
     return 0;
   return umma_forward_tiled_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels, true);
 }
 
-// the checks and the call shared by the three entry points; `what` names the entry point
+// the checks and the call shared by the three fp32 entry points; `what` names the entry point
 static int forward_tiled(const char* what, wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out,
                          int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels, int mode,
                          void* workspace, size_t workspace_bytes, void* stream, int stack, int which) {
-  int rc = forward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels, mode);
+  const int s = forward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels, mode);
+  if (s < 0) return s;
+  int rc = check_packed(what, h);
   if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
   DeviceGuard guard(h->device);
   return umma_forward_tiled(h, in, st, out, n, height, width, tile_h, tile_w, max_pass_pixels, workspace,
-                            workspace_bytes, (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0,
-                            stack, which);
+                            workspace_bytes, (cudaStream_t)stream, s, stack, which);
 }
 
 int wn_forward_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
                      const int64_t in_strides[4][4], float* out, int n, int height, int width, int tile_h, int tile_w,
                      long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !x || !wb || !he || !gc || !in_strides || !out || !workspace) {
-    set_error("wn_forward_tiled: null argument");
-    return WN_E_INVALID;
-  }
+  const char* what = "wn_forward_tiled";
+  int rc = check_ptrs(what, {h, x, wb, he, gc, in_strides, out, workspace});
+  if (rc) return rc;
   const float* in[4] = {x, wb, he, gc};
-  return forward_tiled("wn_forward_tiled", h, in, in_strides, out, n, height, width, tile_h, tile_w, max_pass_pixels,
-                       mode, workspace, workspace_bytes, stream, kStackAll, 0);
+  return forward_tiled(what, h, in, in_strides, out, n, height, width, tile_h, tile_w, max_pass_pixels, mode,
+                       workspace, workspace_bytes, stream, kStackAll, 0);
 }
 
 int wn_confidence_maps_tiled(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
                              const int64_t in_strides[4][4], float* out_maps, int n, int height, int width, int tile_h,
                              int tile_w, long long max_pass_pixels, int mode, void* workspace, size_t workspace_bytes,
                              void* stream) {
-  if (!h || !x || !wb || !he || !gc || !in_strides || !out_maps || !workspace) {
-    set_error("wn_confidence_maps_tiled: null argument");
-    return WN_E_INVALID;
-  }
+  const char* what = "wn_confidence_maps_tiled";
+  int rc = check_ptrs(what, {h, x, wb, he, gc, in_strides, out_maps, workspace});
+  if (rc) return rc;
   const float* in[4] = {x, wb, he, gc};
-  return forward_tiled("wn_confidence_maps_tiled", h, in, in_strides, out_maps, n, height, width, tile_h, tile_w,
-                       max_pass_pixels, mode, workspace, workspace_bytes, stream, kStackCmg, 0);
+  return forward_tiled(what, h, in, in_strides, out_maps, n, height, width, tile_h, tile_w, max_pass_pixels, mode,
+                       workspace, workspace_bytes, stream, kStackCmg, 0);
 }
 
 int wn_refine_tiled(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
                     float* out, int n, int height, int width, int tile_h, int tile_w, long long max_pass_pixels,
                     int mode, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !x || !xbar || !in_strides || !out || !workspace) {
-    set_error("wn_refine_tiled: null argument");
-    return WN_E_INVALID;
-  }
-  if (which < 0 || which > 2) {
-    set_error("wn_refine_tiled: which must be 0, 1 or 2, got %d", which);
-    return WN_E_INVALID;
-  }
-  // as wn_refine: refiner r sees cat[x, input r+1], so xbar goes to every slot
-  const float* in[4] = {x, xbar, xbar, xbar};
-  int64_t st[4][4];
-  for (int t = 0; t < 4; t++)
-    for (int k = 0; k < 4; k++) st[t][k] = in_strides[t == 0 ? 0 : 1][k];
-  return forward_tiled("wn_refine_tiled", h, in, st, out, n, height, width, tile_h, tile_w, max_pass_pixels, mode,
-                       workspace, workspace_bytes, stream, kStackRefiners, which);
+  const char* what = "wn_refine_tiled";
+  int rc = check_ptrs(what, {h, x, xbar, in_strides, out, workspace});
+  if (rc || (rc = check_which(what, which))) return rc;
+  const RefinerInputs r(x, xbar, in_strides);
+  return forward_tiled(what, h, r.in, r.st, out, n, height, width, tile_h, tile_w, max_pass_pixels, mode, workspace,
+                       workspace_bytes, stream, kStackRefiners, which);
 }
 
 int wn_set_chunk_pixels(wn_handle* h, long long max_pixels) {
@@ -660,10 +674,8 @@ int wn_set_chunk_pixels(wn_handle* h, long long max_pixels) {
 }
 
 int wn_set_train_mode(wn_handle* h, int mode) {
-  if (!h) {
-    set_error("wn_set_train_mode: null handle");
-    return WN_E_INVALID;
-  }
+  int rc = check_ptrs("wn_set_train_mode", {h}, "null handle");
+  if (rc) return rc;
   if (mode != WN_MODE_BF16X3 && mode != WN_MODE_BF16) {
     set_error("wn_set_train_mode: mode %d is not a training mode (WN_MODE_BF16X3 = 1 or WN_MODE_BF16 = 3)", mode);
     return WN_E_INVALID;
@@ -681,6 +693,7 @@ int wn_f8_overflowed(const wn_handle* h) { return h ? umma_f8_overflowed(h) : 0;
 
 uint64_t wn_launch_count(const wn_handle* h) { return h ? h->launches : 0; }
 
+// ---- the training step (wn_forward_train / wn_backward)
 size_t wn_train_workspace_bytes(int n, int h, int w) {
   if (n <= 0 || h <= 0 || w <= 0 || n > 65535) return 0;
   return train_workspace_bytes_padded(n, h, w);
@@ -689,60 +702,22 @@ size_t wn_train_workspace_bytes(int n, int h, int w) {
 int wn_forward_train(wn_handle* h, const float* x, const float* wb, const float* he, const float* gc,
                      const int64_t in_strides[4][4], float* out, int n, int height, int width,
                      void* train_workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !x || !wb || !he || !gc || !in_strides || !out || !train_workspace || n <= 0 || height <= 0 ||
-      width <= 0) {
-    set_error("wn_forward_train: bad argument");
-    return WN_E_INVALID;
-  }
-  if (!h->packed) {
-    set_error("wn_forward_train: wn_pack_weights has not been called");
-    return WN_E_STATE;
-  }
-  if (n > 65535) {  // one image per grid row of the per-pixel kernels
-    set_error("wn_forward_train: at most 65535 images per call, got n=%d", n);
-    return WN_E_UNSUPPORTED;
-  }
+  const char* what = "wn_forward_train";
+  int rc = check_args(what, {h, x, wb, he, gc, in_strides, out, train_workspace}, n, height, width);
+  if (rc || (rc = check_packed(what, h)) || (rc = check_images_per_call(what, n))) return rc;
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
   return forward_train(h, in, in_strides, out, n, height, width, train_workspace, workspace_bytes,
                        (cudaStream_t)stream);
 }
 
-// the backward calls: the parameter gradients [first, first + count) they write must be given
-static int check_param_grads(const char* what, float* const* grads, int first, int count) {
-  for (int i = first; i < first + count; i++)
-    if (!grads[i]) {
-      set_error("%s: grads[%d] is NULL", what, i);
-      return WN_E_INVALID;
-    }
-  return WN_OK;
-}
-
-static int check_packed(const char* what, const wn_handle* h) {
-  if (h->packed) return WN_OK;
-  set_error("%s: wn_pack_weights has not been called", what);
-  return WN_E_STATE;
-}
-
 int wn_backward(wn_handle* h, const float* grad_out, float* const* grads, float* const* input_grads, int n,
                 int height, int width, void* train_workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !grad_out || !grads || !train_workspace || n <= 0 || height <= 0 || width <= 0) {
-    set_error("wn_backward: bad argument");
-    return WN_E_INVALID;
-  }
-  int rc = check_param_grads("wn_backward", grads, 0, WN_NUM_PARAMS);
-  if (rc) return rc;
-  if ((rc = check_packed("wn_backward", h))) return rc;
-  if (n > 65535) {
-    set_error("wn_backward: at most 65535 images per call, got n=%d", n);
-    return WN_E_UNSUPPORTED;
-  }
-  if (input_grads)
-    for (int i = 0; i < 4; i++)
-      if (!input_grads[i]) {
-        set_error("wn_backward: input_grads[%d] is NULL", i);
-        return WN_E_INVALID;
-      }
+  const char* what = "wn_backward";
+  int rc = check_args(what, {h, grad_out, grads, train_workspace}, n, height, width);
+  if (rc || (rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS)) || (rc = check_packed(what, h)) ||
+      (rc = check_images_per_call(what, n)) || (rc = check_input_grads(what, input_grads)))
+    return rc;
   DeviceGuard guard(h->device);
   return backward(h, grad_out, grads, input_grads, n, height, width, train_workspace, workspace_bytes,
                   (cudaStream_t)stream);
@@ -755,10 +730,8 @@ static int train_ragged_check(const char* what, const int* hs, const int* ws, in
     set_error("%s: bad image count n=%d", what, n);
     return WN_E_INVALID;
   }
-  if (n > 65535) {
-    set_error("%s: at most 65535 images per call, got n=%d", what, n);
-    return WN_E_UNSUPPORTED;
-  }
+  int rc = check_images_per_call(what, n);
+  if (rc) return rc;
   int sh = 0, sw = 0;
   for (int i = 0; i < n; i++) {
     if (hs[i] <= 0 || ws[i] <= 0) {
@@ -785,29 +758,14 @@ size_t wn_train_ragged_workspace_bytes(const int* heights_host, const int* width
 int wn_forward_train_ragged(wn_handle* h, const wn_ragged_tensors* images_host, int n, void* workspace,
                             size_t workspace_bytes, void* stream) {
   const char* what = "wn_forward_train_ragged";
-  if (!h || !images_host || !workspace) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  if (n <= 0 || n > 65535) {
-    set_error("%s: 1..65535 images per call, got n=%d", what, n);
-    return n <= 0 ? WN_E_INVALID : WN_E_UNSUPPORTED;
-  }
-  for (int i = 0; i < n; i++) {
-    const wn_ragged_tensors& t = images_host[i];
-    if (!t.x || !t.wb || !t.he || !t.gc || !t.out) {
-      set_error("%s: null image pointer (image %d)", what, i);
-      return WN_E_INVALID;
-    }
-  }
+  int rc = check_ptrs(what, {h, images_host, workspace});
+  if (rc || (rc = check_ragged_count(what, n)) ||
+      (rc = check_images(what, images_host, n, false,
+                         [](const wn_ragged_tensors& t, int) { return inputs_given(t) && t.out; })))
+    return rc;
   std::vector<int> hs, ws;
   ragged_sizes(images_host, n, &hs, &ws);
-  int rc = train_ragged_check(what, hs.data(), ws.data(), n);
-  if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  if ((rc = train_ragged_check(what, hs.data(), ws.data(), n)) || (rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   return forward_train_ragged(h, images_host, n, workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -816,19 +774,11 @@ int wn_backward_ragged(wn_handle* h, const int* heights_host, const int* widths_
                        float* const* grads, float* const* input_grads_host, int n, void* workspace,
                        size_t workspace_bytes, void* stream) {
   const char* what = "wn_backward_ragged";
-  if (!h || !heights_host || !widths_host || !grad_out_host || !grads || !workspace) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS);
-  if (rc) return rc;
-  if ((rc = train_ragged_check(what, heights_host, widths_host, n))) return rc;
-  for (int i = 0; i < n; i++)
-    if (!grad_out_host[i]) {
-      set_error("%s: grad_out_host[%d] is NULL", what, i);
-      return WN_E_INVALID;
-    }
-  if ((rc = check_packed(what, h))) return rc;
+  int rc = check_ptrs(what, {h, heights_host, widths_host, grad_out_host, grads, workspace});
+  if (rc || (rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS)) ||
+      (rc = train_ragged_check(what, heights_host, widths_host, n)) ||
+      (rc = check_entries(what, "grad_out_host", grad_out_host, 0, n)) || (rc = check_packed(what, h)))
+    return rc;
   DeviceGuard guard(h->device);
   return backward_ragged(h, heights_host, widths_host, grad_out_host, grads, input_grads_host, n, workspace,
                          workspace_bytes, (cudaStream_t)stream);
@@ -837,10 +787,8 @@ int wn_backward_ragged(wn_handle* h, const int* heights_host, const int* widths_
 // ---- the sub-modules under autograd
 // the shape checks the four calls and the workspace function share; 0 = accepted
 static int submodule_train_check(const char* what, int n, int height, int width) {
-  if (n <= 0 || height <= 0 || width <= 0) {
-    set_error("%s: bad shape n=%d h=%d w=%d", what, n, height, width);
-    return WN_E_INVALID;
-  }
+  int rc = check_shape(what, n, height, width);
+  if (rc) return rc;
   if (n > 65535 || (long long)n * height * width > kTrainMaxPixels) {
     set_error("%s: at most 65535 images and %lld pixels per call, got n=%d h=%d w=%d", what, kTrainMaxPixels, n,
               height, width);
@@ -851,18 +799,15 @@ static int submodule_train_check(const char* what, int n, int height, int width)
 // the backward calls: the sub-module's own parameter gradients [first, first + count) must be given
 static int submodule_backward_check(const char* what, wn_handle* h, const float* grad, float* const* grads, int first,
                                     int count, int n, int height, int width, void* ws) {
-  if (!h || !grad || !grads || !ws) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = check_param_grads(what, grads, first, count);
-  if (rc) return rc;
-  if ((rc = submodule_train_check(what, n, height, width))) return rc;
+  int rc = check_ptrs(what, {h, grad, grads, ws});
+  if (rc || (rc = check_param_grads(what, grads, first, count)) ||
+      (rc = submodule_train_check(what, n, height, width)))
+    return rc;
   return check_packed(what, h);
 }
 
 size_t wn_submodule_train_workspace_bytes(int n, int h, int w, int stack) {
-  if ((stack != 0 && stack != 1) || submodule_train_check("wn_submodule_train_workspace_bytes", n, h, w)) return 0;
+  if (!submodule_stack(stack) || submodule_train_check("wn_submodule_train_workspace_bytes", n, h, w)) return 0;
   return submodule_train_workspace_bytes(n, h, w, stack == 0 ? kStackCmg : kStackRefiners);
 }
 
@@ -870,16 +815,8 @@ int wn_confidence_maps_train(wn_handle* h, const float* x, const float* wb, cons
                              const int64_t in_strides[4][4], float* out_maps, int n, int height, int width, void* ws,
                              size_t ws_bytes, void* stream) {
   const char* what = "wn_confidence_maps_train";
-  if (!h || !x || !wb || !he || !gc || !in_strides || !out_maps || !ws) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = submodule_train_check(what, n, height, width);
-  if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  int rc = check_ptrs(what, {h, x, wb, he, gc, in_strides, out_maps, ws});
+  if (rc || (rc = submodule_train_check(what, n, height, width)) || (rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
   return confidence_maps_train(h, in, in_strides, out_maps, n, height, width, ws, ws_bytes, (cudaStream_t)stream);
@@ -897,59 +834,38 @@ int wn_confidence_maps_backward(wn_handle* h, const float* grad_maps, float* con
 int wn_refine_train(wn_handle* h, int which, const float* x, const float* xbar, const int64_t in_strides[2][4],
                     float* out, int n, int height, int width, void* ws, size_t ws_bytes, void* stream) {
   const char* what = "wn_refine_train";
-  if (which < 0 || which > 2) {
-    set_error("%s: which must be 0, 1 or 2, got %d", what, which);
-    return WN_E_INVALID;
-  }
-  if (!h || !x || !xbar || !in_strides || !out || !ws) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = submodule_train_check(what, n, height, width);
-  if (rc) return rc;
-  if (!h->packed) {
-    set_error("%s: wn_pack_weights has not been called", what);
-    return WN_E_STATE;
-  }
+  int rc = check_which(what, which);
+  if (rc || (rc = check_ptrs(what, {h, x, xbar, in_strides, out, ws})) ||
+      (rc = submodule_train_check(what, n, height, width)) || (rc = check_packed(what, h)))
+    return rc;
   DeviceGuard guard(h->device);
-  // as wn_refine: refiner r sees cat[x, input r+1], so xbar goes to every slot
-  const float* in[4] = {x, xbar, xbar, xbar};
-  int64_t st[4][4];
-  for (int t = 0; t < 4; t++)
-    for (int k = 0; k < 4; k++) st[t][k] = in_strides[t == 0 ? 0 : 1][k];
-  return refine_train(h, which, in, st, out, n, height, width, ws, ws_bytes, (cudaStream_t)stream);
+  const RefinerInputs r(x, xbar, in_strides);
+  return refine_train(h, which, r.in, r.st, out, n, height, width, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 int wn_refine_backward(wn_handle* h, int which, const float* grad_out, float* const* grads, float* const* input_grads,
                        int n, int height, int width, void* ws, size_t ws_bytes, void* stream) {
   const char* what = "wn_refine_backward";
-  if (which < 0 || which > 2) {
-    set_error("%s: which must be 0, 1 or 2, got %d", what, which);
-    return WN_E_INVALID;
-  }
-  int rc = submodule_backward_check(what, h, grad_out, grads, 16 + 6 * which, 6, n, height, width, ws);
-  if (rc) return rc;
+  int rc = check_which(what, which);
+  if (rc || (rc = submodule_backward_check(what, h, grad_out, grads, 16 + 6 * which, 6, n, height, width, ws)))
+    return rc;
   DeviceGuard guard(h->device);
   return refine_backward(h, which, grad_out, grads, input_grads, n, height, width, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+// ---- the windowed recompute backward (wn_backward_tiled and the sub-modules' and ragged forms)
+static int check_train_pass(const char* what, long long max_pass_pixels) {
+  if (max_pass_pixels <= kTrainMaxPixels) return WN_OK;
+  set_error("%s: max_pass_pixels=%lld exceeds the %lld pixels of one training pass", what, max_pass_pixels,
+            kTrainMaxPixels);
+  return WN_E_UNSUPPORTED;
 }
 
 // the argument checks wn_backward_tiled and its workspace function share (pointers aside)
 static int backward_tiled_check(const char* what, int n, int height, int width, int tile_h, int tile_w,
                                 long long max_pass_pixels) {
-  if (n <= 0 || height <= 0 || width <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
-    set_error("%s: bad shape n=%d h=%d w=%d tile=%dx%d max_pass_pixels=%lld", what, n, height, width, tile_h, tile_w,
-              max_pass_pixels);
-    return WN_E_INVALID;
-  }
-  if ((size_t)height * width > (size_t)0x7fffffff / 3 || n > 65535) {
-    set_error("image too large: n=%d h=%d w=%d", n, height, width);
-    return WN_E_UNSUPPORTED;
-  }
-  if (max_pass_pixels > kTrainMaxPixels) {
-    set_error("%s: max_pass_pixels=%lld exceeds the %lld pixels of one training pass", what, max_pass_pixels,
-              kTrainMaxPixels);
-    return WN_E_UNSUPPORTED;
-  }
+  int rc = check_tiled_shape(what, n, height, width, tile_h, tile_w, max_pass_pixels);
+  if (rc || (rc = check_size(n, height, width)) || (rc = check_train_pass(what, max_pass_pixels))) return rc;
   const TileGeom g = tile_geom(height, width, tile_h, tile_w);
   if ((long long)g.win_h * g.win_w > kTrainMaxPixels) {
     set_error("%s: a %dx%d window exceeds the %lld pixels of one training pass; use a smaller tile", what, g.win_h,
@@ -969,20 +885,11 @@ int wn_backward_tiled(wn_handle* h, const float* x, const float* wb, const float
                       float* const* input_grads, int n, int height, int width, int tile_h, int tile_w,
                       long long max_pass_pixels, void* workspace, size_t workspace_bytes, void* stream) {
   const char* what = "wn_backward_tiled";
-  if (!h || !x || !wb || !he || !gc || !in_strides || !grad_out || !grads || !workspace) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS);
-  if (rc) return rc;
-  if (input_grads)
-    for (int i = 0; i < 4; i++)
-      if (!input_grads[i]) {
-        set_error("%s: input_grads[%d] is NULL", what, i);
-        return WN_E_INVALID;
-      }
-  if ((rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels))) return rc;
-  if ((rc = check_packed(what, h))) return rc;
+  int rc = check_ptrs(what, {h, x, wb, he, gc, in_strides, grad_out, grads, workspace});
+  if (rc || (rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS)) || (rc = check_input_grads(what, input_grads)) ||
+      (rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels)) ||
+      (rc = check_packed(what, h)))
+    return rc;
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
   return backward_tiled(h, in, in_strides, grad_out, grads, input_grads, n, height, width, tile_h, tile_w,
@@ -992,22 +899,10 @@ int wn_backward_tiled(wn_handle* h, const float* x, const float* wb, const float
 // ---- the windowed recompute backward of a ragged batch: the limits of wn_backward_tiled, for every image
 static int backward_ragged_tiled_check(const char* what, const int* hs, const int* ws, int n, int tile_h, int tile_w,
                                        long long max_pass_pixels) {
-  if (n <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) {
-    set_error("%s: bad shape n=%d tile=%dx%d max_pass_pixels=%lld", what, n, tile_h, tile_w, max_pass_pixels);
-    return WN_E_INVALID;
-  }
-  if (n > 65535) {
-    set_error("%s: too many images: n=%d", what, n);
-    return WN_E_UNSUPPORTED;
-  }
-  if (max_pass_pixels > kTrainMaxPixels) {
-    set_error("%s: max_pass_pixels=%lld exceeds the %lld pixels of one training pass", what, max_pass_pixels,
-              kTrainMaxPixels);
-    return WN_E_UNSUPPORTED;
-  }
+  int rc = check_ragged_shape(what, n, tile_h, tile_w, max_pass_pixels);
+  if (rc || (rc = check_train_pass(what, max_pass_pixels))) return rc;
   for (int i = 0; i < n; i++) {
-    int rc = ragged_check_size(what, i, hs[i], ws[i]);
-    if (rc) return rc;
+    if ((rc = check_ragged_size(what, i, hs[i], ws[i]))) return rc;
     const TileGeom g = tile_geom(hs[i], ws[i], tile_h, tile_w);
     if ((long long)g.win_h * g.win_w > kTrainMaxPixels) {
       set_error("%s: a %dx%d window of image %d exceeds the %lld pixels of one training pass; use a smaller tile",
@@ -1031,27 +926,16 @@ int wn_backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images_host,
                              float* const* grads, float* const* input_grads_host, int n, int tile_h, int tile_w,
                              long long max_pass_pixels, void* workspace, size_t workspace_bytes, void* stream) {
   const char* what = "wn_backward_ragged_tiled";
-  if (!h || !images_host || !grad_out_host || !grads || !workspace) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS);
-  if (rc) return rc;
-  if (n <= 0 || n > 65535) {
-    set_error("%s: 1..65535 images per call, got n=%d", what, n);
-    return n <= 0 ? WN_E_INVALID : WN_E_UNSUPPORTED;
-  }
-  for (int i = 0; i < n; i++) {
-    const wn_ragged_tensors& t = images_host[i];
-    if (!t.x || !t.wb || !t.he || !t.gc || !grad_out_host[i]) {
-      set_error("%s: null image pointer (image %d)", what, i);
-      return WN_E_INVALID;
-    }
-  }
+  int rc = check_ptrs(what, {h, images_host, grad_out_host, grads, workspace});
+  if (rc || (rc = check_param_grads(what, grads, 0, WN_NUM_PARAMS)) || (rc = check_ragged_count(what, n)) ||
+      (rc = check_images(what, images_host, n, false,
+                         [&](const wn_ragged_tensors& t, int i) { return inputs_given(t) && grad_out_host[i]; })))
+    return rc;
   std::vector<int> hs, ws;
   ragged_sizes(images_host, n, &hs, &ws);
-  if ((rc = backward_ragged_tiled_check(what, hs.data(), ws.data(), n, tile_h, tile_w, max_pass_pixels))) return rc;
-  if ((rc = check_packed(what, h))) return rc;
+  if ((rc = backward_ragged_tiled_check(what, hs.data(), ws.data(), n, tile_h, tile_w, max_pass_pixels)) ||
+      (rc = check_packed(what, h)))
+    return rc;
   DeviceGuard guard(h->device);
   return backward_ragged_tiled(h, images_host, grad_out_host, grads, input_grads_host, n, tile_h, tile_w,
                                max_pass_pixels, workspace, workspace_bytes, (cudaStream_t)stream);
@@ -1060,7 +944,7 @@ int wn_backward_ragged_tiled(wn_handle* h, const wn_ragged_tensors* images_host,
 // ---- the windowed recompute backward of one sub-module: the limits of wn_backward_tiled
 size_t wn_submodule_backward_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w,
                                                    long long max_pass_pixels, int stack) {
-  if ((stack != 0 && stack != 1) ||
+  if (!submodule_stack(stack) ||
       backward_tiled_check("wn_submodule_backward_tiled_workspace_bytes", n, h, w, tile_h, tile_w, max_pass_pixels))
     return 0;
   return submodule_backward_tiled_workspace_bytes(n, h, w, tile_h, tile_w, max_pass_pixels,
@@ -1073,14 +957,11 @@ int wn_confidence_maps_backward_tiled(wn_handle* h, const float* x, const float*
                                       long long max_pass_pixels, void* workspace, size_t workspace_bytes,
                                       void* stream) {
   const char* what = "wn_confidence_maps_backward_tiled";
-  if (!h || !x || !wb || !he || !gc || !in_strides || !grad_maps || !grads || !workspace) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = check_param_grads(what, grads, 0, 16);
-  if (rc) return rc;
-  if ((rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels))) return rc;
-  if ((rc = check_packed(what, h))) return rc;
+  int rc = check_ptrs(what, {h, x, wb, he, gc, in_strides, grad_maps, grads, workspace});
+  if (rc || (rc = check_param_grads(what, grads, 0, 16)) ||
+      (rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels)) ||
+      (rc = check_packed(what, h)))
+    return rc;
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
   return submodule_backward_tiled(h, kStackCmg, 0, in, in_strides, grad_maps, grads, input_grads, n, height, width,
@@ -1092,25 +973,15 @@ int wn_refine_backward_tiled(wn_handle* h, int which, const float* x, const floa
                              int width, int tile_h, int tile_w, long long max_pass_pixels, void* workspace,
                              size_t workspace_bytes, void* stream) {
   const char* what = "wn_refine_backward_tiled";
-  if (which < 0 || which > 2) {
-    set_error("%s: which must be 0, 1 or 2, got %d", what, which);
-    return WN_E_INVALID;
-  }
-  if (!h || !x || !xbar || !in_strides || !grad_out || !grads || !workspace) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
-  int rc = check_param_grads(what, grads, 16 + 6 * which, 6);
-  if (rc) return rc;
-  if ((rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels))) return rc;
-  if ((rc = check_packed(what, h))) return rc;
+  int rc = check_which(what, which);
+  if (rc || (rc = check_ptrs(what, {h, x, xbar, in_strides, grad_out, grads, workspace})) ||
+      (rc = check_param_grads(what, grads, 16 + 6 * which, 6)) ||
+      (rc = backward_tiled_check(what, n, height, width, tile_h, tile_w, max_pass_pixels)) ||
+      (rc = check_packed(what, h)))
+    return rc;
   DeviceGuard guard(h->device);
-  // as wn_refine_train: refiner r sees cat[x, input r+1], so xbar goes to every slot
-  const float* in[4] = {x, xbar, xbar, xbar};
-  int64_t st[4][4];
-  for (int t = 0; t < 4; t++)
-    for (int k = 0; k < 4; k++) st[t][k] = in_strides[t == 0 ? 0 : 1][k];
-  return submodule_backward_tiled(h, kStackRefiners, which, in, st, grad_out, grads, input_grads, n, height, width,
+  const RefinerInputs r(x, xbar, in_strides);
+  return submodule_backward_tiled(h, kStackRefiners, which, r.in, r.st, grad_out, grads, input_grads, n, height, width,
                                   tile_h, tile_w, max_pass_pixels, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
@@ -1118,25 +989,20 @@ int wn_debug_forward_layer(wn_handle* h, const float* x, const float* wb, const 
                            const float* gc, const int64_t in_strides[4][4], int n, int height,
                            int width, int mode, int layer, float* dst, void* workspace,
                            size_t workspace_bytes, void* stream) {
+  const char* what = "wn_debug_forward_layer";
   if (layer < 0 || layer > 10) {
-    set_error("wn_debug_forward_layer: layer %d is not in 0..10", layer);
+    set_error("%s: layer %d is not in 0..10", what, layer);
     return WN_E_INVALID;
   }
-  if (!h || !x || !wb || !he || !gc || !in_strides || !dst || !workspace) {
-    set_error("wn_debug_forward_layer: bad argument");
-    return WN_E_INVALID;
-  }
-  if (!h->packed) {
-    set_error("wn_debug_forward_layer: wn_pack_weights has not been called");
-    return WN_E_STATE;
-  }
+  int rc = check_ptrs(what, {h, x, wb, he, gc, in_strides, dst, workspace}, "bad argument");
+  if (rc || (rc = check_packed(what, h))) return rc;
   DeviceGuard guard(h->device);
   const float* in[4] = {x, wb, he, gc};
   if (resolve_mode(mode) == WN_MODE_FP32_SIMT)
     return simt_debug_layer(h, in, in_strides, n, height, width, layer, dst, workspace, workspace_bytes,
                             (cudaStream_t)stream);
   return umma_debug_layer(h, in, in_strides, n, height, width, layer, dst, workspace, workspace_bytes,
-                          (cudaStream_t)stream, resolve_mode(mode) == WN_MODE_BF16_FP8 ? 1 : 0);
+                          (cudaStream_t)stream, scheme_of(mode));
 }
 
 int wn_debug_backward_layer(wn_handle* h, int stack, int which, int buffer, const float* grad_out,
@@ -1151,16 +1017,15 @@ int wn_debug_backward_layer(wn_handle* h, int stack, int which, int buffer, cons
     set_error("%s: stack must be -1, 0 or 1 (with which 0, 1 or 2), got stack %d which %d", what, stack, which);
     return WN_E_INVALID;
   }
-  if (!h || !dst || !workspace || (buffer >= 12 && !grad_out) || (buffer >= 14 && !grads)) {
-    set_error("%s: null argument", what);
-    return WN_E_INVALID;
-  }
+  // grad_out from the seeds on, the parameter gradients from the first data-gradient launch on
+  if (!all_set({h, dst, workspace}) || (buffer >= 12 && !grad_out) || (buffer >= 14 && !grads))
+    return invalid(what, "null argument");
+  int rc;
   // the parameter gradients the backward up to the launch writes: the stack's own entries
   const int first = stack == 1 ? 16 + 6 * which : 0, count = stack == -1 ? WN_NUM_PARAMS : stack == 0 ? 16 : 6;
-  int rc = buffer >= 14 ? check_param_grads(what, grads, first, count) : WN_OK;
-  if (rc) return rc;
-  if ((rc = submodule_train_check(what, n, height, width))) return rc;
-  if ((rc = check_packed(what, h))) return rc;
+  if ((buffer >= 14 && (rc = check_param_grads(what, grads, first, count))) ||
+      (rc = submodule_train_check(what, n, height, width)) || (rc = check_packed(what, h)))
+    return rc;
   DeviceGuard guard(h->device);
   return debug_backward_layer(h, stack == -1 ? kStackAll : stack == 0 ? kStackCmg : kStackRefiners, which, buffer,
                               grad_out, grads, n, height, width, dst, workspace, workspace_bytes,
@@ -1169,15 +1034,9 @@ int wn_debug_backward_layer(wn_handle* h, int stack, int which, int buffer, cons
 
 // ---- the VGG19 perceptual loss (vgg.cu)
 int wn_vgg_pack_weights(wn_handle* h, const float* const* params, void* stream) {
-  if (!h || !params) {
-    set_error("wn_vgg_pack_weights: null argument");
-    return WN_E_INVALID;
-  }
-  for (int i = 0; i < WN_VGG_NUM_PARAMS; i++)
-    if (!params[i]) {
-      set_error("wn_vgg_pack_weights: params[%d] is NULL", i);
-      return WN_E_INVALID;
-    }
+  const char* what = "wn_vgg_pack_weights";
+  int rc = check_ptrs(what, {h, params});
+  if (rc || (rc = check_entries(what, "params", params, 0, WN_VGG_NUM_PARAMS))) return rc;
   DeviceGuard guard(h->device);
   return vgg_pack_weights(h, params, (cudaStream_t)stream);
 }
@@ -1190,10 +1049,8 @@ int wn_perceptual_loss(wn_handle* h, const float* out, const int64_t out_strides
                        const int64_t ref_strides[4], int n, int height, int width, int tile_h, int tile_w,
                        long long max_pass_pixels, float* loss_dev, float* grad_out, void* workspace,
                        size_t workspace_bytes, void* stream) {
-  if (!h || !out || !out_strides || !ref || !ref_strides || !loss_dev || !workspace) {
-    set_error("wn_perceptual_loss: null argument");
-    return WN_E_INVALID;
-  }
+  int rc = check_ptrs("wn_perceptual_loss", {h, out, out_strides, ref, ref_strides, loss_dev, workspace});
+  if (rc) return rc;
   DeviceGuard guard(h->device);
   return vgg_perceptual_loss(h, out, out_strides, ref, ref_strides, n, height, width, tile_h, tile_w, max_pass_pixels,
                              loss_dev, grad_out, workspace, workspace_bytes, (cudaStream_t)stream);
@@ -1202,20 +1059,16 @@ int wn_perceptual_loss(wn_handle* h, const float* out, const int64_t out_strides
 int wn_debug_vgg_layer(wn_handle* h, const float* x, const int64_t strides[4], const float* ref,
                        const int64_t ref_strides[4], int n, int height, int width, int tile_h, int tile_w, int layer,
                        float* dst, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !x || !strides || !dst || !workspace) {
-    set_error("wn_debug_vgg_layer: null argument");
-    return WN_E_INVALID;
-  }
+  int rc = check_ptrs("wn_debug_vgg_layer", {h, x, strides, dst, workspace});
+  if (rc) return rc;
   DeviceGuard guard(h->device);
   return vgg_debug_layer(h, x, strides, ref, ref_strides, n, height, width, tile_h, tile_w, layer, dst, workspace,
                          workspace_bytes, (cudaStream_t)stream);
 }
 
 int wn_enable_timing(wn_handle* h, int on) {
-  if (!h) {
-    set_error("wn_enable_timing: null handle");
-    return WN_E_INVALID;
-  }
+  int rc = check_ptrs("wn_enable_timing", {h}, "null handle");
+  if (rc) return rc;
   if (!h->timing) h->timing = (Timing*)calloc(1, sizeof(Timing));
   h->timing->on = on != 0;
   h->timing->used = 0;
@@ -1223,10 +1076,8 @@ int wn_enable_timing(wn_handle* h, int on) {
 }
 
 int wn_read_timings(wn_handle* h, float* ms, int* count) {
-  if (!h || !ms || !count) {
-    set_error("wn_read_timings: null argument");
-    return WN_E_INVALID;
-  }
+  int rc = check_ptrs("wn_read_timings", {h, ms, count});
+  if (rc) return rc;
   if (!h->timing) return WN_OK;
   DeviceGuard guard(h->device);
   Timing* t = h->timing;

@@ -753,10 +753,9 @@ int umma_enhance_u8(wn_handle* h, const uint8_t* rgb, uint8_t* out_u8, float* ou
 // windows runs through the same ten launches (and range guard) as a batch of images, and the last launch stores
 // each window's kept rectangle into the full-image outputs.  Workspace: one pass of windows plus the per-image
 // LUTs, independent of the image size.  The geometry is arithmetic on the window index: nothing is copied from the
-// host, so the call stays stream-ordered and can be captured in a graph.
+// host, so the call stays stream-ordered and can be captured in a graph.  Its callers have applied the shape and
+// image-size checks of wn_enhance_u8_tiled (api.cu).
 size_t umma_enhance_tiled_workspace_bytes(int n, int h, int w, int tile_h, int tile_w, long long max_pass_pixels) {
-  if (n <= 0 || h <= 0 || w <= 0 || tile_h <= 0 || tile_w <= 0 || max_pass_pixels < 0) return 0;
-  if ((size_t)h * w > (size_t)0x7fffffff / 3 || n > 65535) return 0;
   const TileGeom g = tile_geom(h, w, tile_h, tile_w);
   const long long p = tile_pass_windows(g, n, max_pass_pixels ? max_pass_pixels : kDefaultChunkPixels);
   return (size_t)p * g.win_h * g.win_w * kUmmaBytesPerPixel + 4096 + align256(preprocess_workspace_bytes(n, h, w)) +

@@ -211,6 +211,38 @@ def _stream_ptr(device: torch.device) -> ctypes.c_void_p:
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+# ---- the ctypes arrays the C ABI takes
+def _strides(tensors) -> ctypes.Array:
+    """The element strides of ``tensors``, flattened ({sN, sC, sH, sW} each): in_strides of the C ABI."""
+    return (ctypes.c_int64 * (4 * len(tensors)))(*[s for t in tensors for s in t.stride()])
+
+
+def _sizes(sizes) -> Tuple[ctypes.Array, ctypes.Array]:
+    """[(h, w), ...] -> the height and width arrays of the ragged calls (one entry at least)."""
+    n = max(1, len(sizes))
+    return (ctypes.c_int * n)(*[int(h) for h, _ in sizes]), (ctypes.c_int * n)(*[int(w) for _, w in sizes])
+
+
+def _ptrs(tensors) -> ctypes.Array:
+    """The device addresses of ``tensors`` (NULL for None) as an array of pointers."""
+    return (ctypes.c_void_p * len(tensors))(*[None if t is None else t.data_ptr() for t in tensors])
+
+
+def _grads_array(grads, first: int = 0) -> ctypes.Array:
+    """The NUM_PARAMS parameter-gradient pointers with ``grads`` (tensors or None) at entries first, first + 1, ...
+    and NULL elsewhere: the entries of a sub-module start at its first state-dict entry."""
+    arr = (ctypes.c_void_p * _lib.NUM_PARAMS)()
+    arr[first:first + len(grads)] = [None if t is None else t.data_ptr() for t in grads]
+    return arr
+
+
+def _require_workspace(nbytes: int, message: str) -> int:
+    """``nbytes`` from a workspace function, which returns 0 for the arguments its call rejects: then raise."""
+    if nbytes == 0:
+        raise _lib.WaterNetLibraryError(message)
+    return nbytes
+
+
 class Engine:
     def __init__(self, device: torch.device):
         self.lib = _lib.load()
@@ -231,6 +263,15 @@ class Engine:
             pass
 
     # ---- plumbing ----------------------------------------------------------
+    def _call(self, name: str, *args, stream: bool = True) -> None:
+        """``self.lib.<name>(handle, *args, current stream)`` on the engine's device (no stream argument without
+        ``stream``); raises WaterNetLibraryError when it returns an error code."""
+        with torch.cuda.device(self.device):
+            if stream:
+                args += (_stream_ptr(self.device),)
+            rc = getattr(self.lib, name)(self.handle, *args)
+        _lib.check(rc, name)
+
     def _workspace(self, tag: str, nbytes: int) -> torch.Tensor:
         buf = self._ws.get(tag)
         if buf is None or buf.numel() < nbytes:
@@ -248,13 +289,13 @@ class Engine:
 
     def set_chunk_pixels(self, max_pixels: int) -> None:
         """Lower the per-pass pixel cap (0 = default 8 Mi); tests force the multi-pass path with it."""
-        _lib.check(self.lib.wn_set_chunk_pixels(self.handle, int(max_pixels)), "wn_set_chunk_pixels")
+        self._call("wn_set_chunk_pixels", int(max_pixels), stream=False)
 
     def set_train_mode(self, mode: int) -> None:
         """The arithmetic of this handle's training calls (wn_set_train_mode): MODE_BF16X3 or MODE_BF16.  Every
         training method below sets it from its ``train_mode`` argument first, so a backward runs under the mode its
         caller passes (the mode of the matching forward), whatever another module did on this handle in between."""
-        _lib.check(self.lib.wn_set_train_mode(self.handle, int(mode)), "wn_set_train_mode")
+        self._call("wn_set_train_mode", int(mode), stream=False)
 
     def f8_overflowed(self) -> bool:
         """True once the fp8-correction mode saw an activation beyond the e4m3 range.  The batch that did was
@@ -267,14 +308,14 @@ class Engine:
         return int(self.lib.wn_launch_count(self.handle))
 
     def enable_timing(self, on: bool = True) -> None:
-        _lib.check(self.lib.wn_enable_timing(self.handle, 1 if on else 0), "wn_enable_timing")
+        self._call("wn_enable_timing", 1 if on else 0, stream=False)
 
     def read_timings(self):
         """(ms[slot], count[slot]) accumulated since the last read; synchronises the device first."""
         torch.cuda.synchronize(self.device)
         ms = (ctypes.c_float * _lib.NUM_TIMING_SLOTS)()
         cnt = (ctypes.c_int * _lib.NUM_TIMING_SLOTS)()
-        _lib.check(self.lib.wn_read_timings(self.handle, ms, cnt), "wn_read_timings")
+        self._call("wn_read_timings", ms, cnt, stream=False)
         return list(ms), list(cnt)
 
     # ---- weights -------------------------------------------------------------
@@ -285,9 +326,7 @@ class Engine:
         if key is not None and key == self._weights_key:
             return
         staged = [p.detach().to(device=self.device, dtype=torch.float32).contiguous() for p in params]
-        arr = (ctypes.c_void_p * _lib.NUM_PARAMS)(*[t.data_ptr() for t in staged])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.wn_pack_weights(self.handle, arr, _stream_ptr(self.device)), "wn_pack_weights")
+        self._call("wn_pack_weights", _ptrs(staged))
         self._weights_keepalive = staged  # until the async pack kernels have consumed them
         self._weights_key = key
 
@@ -300,14 +339,9 @@ class Engine:
             out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
         if n == 0 or h == 0 or w == 0:  # empty batch: nothing to launch (torch's convs return empty too)
             return out
-        strides = (ctypes.c_int64 * 16)(*[s for t in ins for s in t.stride()])
-        nbytes = self.lib.wn_forward_workspace_bytes(n, h, w, mode)
-        ws = self._workspace("forward", nbytes)
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_forward(self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(),
-                                     ins[3].data_ptr(), strides, out.data_ptr(), n, h, w, mode,
-                                     ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_forward")
+        ws = self._workspace("forward", self.lib.wn_forward_workspace_bytes(n, h, w, mode))
+        self._call("wn_forward", *(t.data_ptr() for t in ins), _strides(ins), out.data_ptr(), n, h, w, mode,
+                   ws.data_ptr(), ws.numel())
         return out
 
     def _check_inputs(self, tensors):
@@ -330,13 +364,9 @@ class Engine:
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
         if out.numel() == 0:
             return out
-        strides = (ctypes.c_int64 * 16)(*[s for t in ins for s in t.stride()])
         ws = self._workspace("forward", self.lib.wn_submodule_workspace_bytes(n, h, w, mode))
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_confidence_maps(self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(),
-                                             ins[3].data_ptr(), strides, out.data_ptr(), n, h, w, mode,
-                                             ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_confidence_maps")
+        self._call("wn_confidence_maps", *(t.data_ptr() for t in ins), _strides(ins), out.data_ptr(), n, h, w, mode,
+                   ws.data_ptr(), ws.numel())
         return out
 
     def refine(self, which: int, x, xbar, mode: int = _lib.MODE_DEFAULT) -> torch.Tensor:
@@ -346,13 +376,9 @@ class Engine:
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
         if out.numel() == 0:
             return out
-        strides = (ctypes.c_int64 * 8)(*[s for t in ins for s in t.stride()])
         ws = self._workspace("forward", self.lib.wn_submodule_workspace_bytes(n, h, w, mode))
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_refine(self.handle, int(which), ins[0].data_ptr(), ins[1].data_ptr(), strides,
-                                    out.data_ptr(), n, h, w, mode, ws.data_ptr(), ws.numel(),
-                                    _stream_ptr(self.device))
-        _lib.check(rc, "wn_refine")
+        self._call("wn_refine", int(which), *(t.data_ptr() for t in ins), _strides(ins), out.data_ptr(), n, h, w,
+                   mode, ws.data_ptr(), ws.numel())
         return out
 
     LAYER_CHANNELS = (128, 128, 128, 64, 64, 64, 64, 3, 96, 96, 9)
@@ -362,13 +388,9 @@ class Engine:
         ins = [t.detach().float() for t in (x, wb, he, gc)]
         n, _, h, w = ins[0].shape
         dst = torch.empty((n, self.LAYER_CHANNELS[layer], h, w), dtype=torch.float32, device=self.device)
-        strides = (ctypes.c_int64 * 16)(*[s for t in ins for s in t.stride()])
         ws = self._workspace("forward", self.lib.wn_forward_workspace_bytes(n, h, w, mode))
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_debug_forward_layer(self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(),
-                                                 ins[3].data_ptr(), strides, n, h, w, mode, layer, dst.data_ptr(),
-                                                 ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_debug_forward_layer")
+        self._call("wn_debug_forward_layer", *(t.data_ptr() for t in ins), _strides(ins), n, h, w, mode, layer,
+                   dst.data_ptr(), ws.data_ptr(), ws.numel())
         return dst
 
     # ---- training step (wn_forward_train / wn_backward) ---------------------------------------
@@ -396,13 +418,9 @@ class Engine:
         for a in range(0, n, per):
             b = min(n, a + per)
             part = [t[a:b] for t in ins]
-            strides = (ctypes.c_int64 * 16)(*[s for t in part for s in t.stride()])
             ws = torch.empty(self.lib.wn_train_workspace_bytes(b - a, h, w), dtype=torch.uint8, device=self.device)
-            with torch.cuda.device(self.device):
-                rc = self.lib.wn_forward_train(self.handle, part[0].data_ptr(), part[1].data_ptr(), part[2].data_ptr(),
-                                               part[3].data_ptr(), strides, out[a:b].data_ptr(), b - a, h, w,
-                                               ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-            _lib.check(rc, "wn_forward_train")
+            self._call("wn_forward_train", *(t.data_ptr() for t in part), _strides(part), out[a:b].data_ptr(), b - a,
+                       h, w, ws.data_ptr(), ws.numel())
             saved.append((a, b, ws))
         return out, saved
 
@@ -421,13 +439,9 @@ class Engine:
         if want_input_grads:
             gin = [torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) for _ in range(4)]
         for i, (a, b, ws) in enumerate(saved):
-            dst = grads if i == 0 else part
-            arr = (ctypes.c_void_p * _lib.NUM_PARAMS)(*[t.data_ptr() for t in dst])
-            gin_arr = (ctypes.c_void_p * 4)(*[t[a:b].data_ptr() for t in gin]) if want_input_grads else None
-            with torch.cuda.device(self.device):
-                rc = self.lib.wn_backward(self.handle, g[a:b].data_ptr(), arr, gin_arr, b - a, h, w, ws.data_ptr(),
-                                          ws.numel(), _stream_ptr(self.device))
-            _lib.check(rc, "wn_backward")
+            gin_arr = _ptrs([t[a:b] for t in gin]) if want_input_grads else None
+            self._call("wn_backward", g[a:b].data_ptr(), _grads_array(grads if i == 0 else part), gin_arr, b - a, h, w,
+                       ws.data_ptr(), ws.numel())
             if i > 0:
                 torch._foreach_add_(grads, part)
         return (grads, gin) if want_input_grads else grads
@@ -450,21 +464,17 @@ class Engine:
         n, h, w = shape
         dst = torch.empty((n, self.BACKWARD_BUFFER_CHANNELS[buffer], h, w), dtype=torch.float32, device=self.device)
         g = None if grad is None else grad.detach().to(self.device, torch.float32).contiguous()
-        arr = None if grads is None else (ctypes.c_void_p * _lib.NUM_PARAMS)(
-            *[None if t is None else t.data_ptr() for t in grads])
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_debug_backward_layer(self.handle, int(stack), int(which), int(buffer),
-                                                  None if g is None else g.data_ptr(), arr, n, h, w, dst.data_ptr(),
-                                                  workspace.data_ptr(), workspace.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_debug_backward_layer")
+        self._call("wn_debug_backward_layer", int(stack), int(which), int(buffer), None if g is None else g.data_ptr(),
+                   None if grads is None else _grads_array(grads), n, h, w, dst.data_ptr(), workspace.data_ptr(),
+                   workspace.numel())
         return dst
 
     # ---- the sub-modules under autograd (wn_confidence_maps_train / _backward, wn_refine_train / _backward) --------
     STACK_CMG, STACK_REFINER = 0, 1
 
-    def _submodule_train(self, stack: int, ins, call, what: str, train_mode: int):
+    def _submodule_train(self, stack: int, ins, lead, what: str, train_mode: int):
         """The batch in slices of at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES, one workspace per slice, as
-        ``forward_train``.  call(slice inputs, strides, slice output, n, h, w, workspace) -> rc."""
+        ``forward_train``.  Each slice is one call of ``what`` with the arguments ``lead`` (which) before the inputs."""
         self.set_train_mode(train_mode)
         n, _, h, w = ins[0].shape
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
@@ -478,19 +488,17 @@ class Engine:
         for a in range(0, n, per):
             b = min(n, a + per)
             part = [t[a:b] for t in ins]
-            strides = (ctypes.c_int64 * (4 * len(part)))(*[s for t in part for s in t.stride()])
             nbytes = self.lib.wn_submodule_train_workspace_bytes(b - a, h, w, stack)
             ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            with torch.cuda.device(self.device):
-                rc = call(part, strides, out[a:b], b - a, h, w, ws)
-            _lib.check(rc, what)
+            self._call(what, *lead, *(t.data_ptr() for t in part), _strides(part), out[a:b].data_ptr(), b - a, h, w,
+                       ws.data_ptr(), ws.numel())
             saved.append((a, b, ws))
         return out, saved
 
-    def _submodule_backward(self, grad, saved, shapes, first: int, want_inputs, call, what: str, train_mode: int):
+    def _submodule_backward(self, grad, saved, shapes, first: int, want_inputs, lead, what: str, train_mode: int):
         """The parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) added in slice order, and
-        the input gradients asked for by ``want_inputs`` (None where not).  call(grad slice, grads array, input grads
-        array or None, n, h, w, workspace) -> rc."""
+        the input gradients asked for by ``want_inputs`` (None where not).  Each slice is one call of ``what`` with the
+        arguments ``lead`` (which) before the gradient."""
         self.set_train_mode(train_mode)
         g = grad.detach().to(self.device, torch.float32).contiguous()
         n, _, h, w = g.shape
@@ -501,15 +509,9 @@ class Engine:
         gin = [torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) if want else None
                for want in want_inputs]
         for i, (a, b, ws) in enumerate(saved):
-            arr = (ctypes.c_void_p * _lib.NUM_PARAMS)()
-            for k, t in enumerate(grads if i == 0 else part):
-                arr[first + k] = t.data_ptr()
-            gin_arr = None
-            if any(want_inputs):
-                gin_arr = (ctypes.c_void_p * len(gin))(*[None if t is None else t[a:b].data_ptr() for t in gin])
-            with torch.cuda.device(self.device):
-                rc = call(g[a:b].data_ptr(), arr, gin_arr, b - a, h, w, ws)
-            _lib.check(rc, what)
+            gin_arr = _ptrs([None if t is None else t[a:b] for t in gin]) if any(want_inputs) else None
+            self._call(what, *lead, g[a:b].data_ptr(), _grads_array(grads if i == 0 else part, first), gin_arr, b - a,
+                       h, w, ws.data_ptr(), ws.numel())
             if i > 0:
                 torch._foreach_add_(grads, part)
         return grads, gin
@@ -518,37 +520,25 @@ class Engine:
         """``confidence_maps`` in the arithmetic of training (``train_mode``), keeping the activations of the cmg stack
         (wn_confidence_maps_train).  Returns (maps, saved workspaces) for ``confidence_maps_backward``."""
         ins = self._check_inputs((x, wb, he, gc))
-        stream = _stream_ptr(self.device)
-        return self._submodule_train(self.STACK_CMG, ins, lambda p, st, o, n, h, w, ws: self.lib.wn_confidence_maps_train(
-            self.handle, p[0].data_ptr(), p[1].data_ptr(), p[2].data_ptr(), p[3].data_ptr(), st, o.data_ptr(), n, h, w,
-            ws.data_ptr(), ws.numel(), stream), "wn_confidence_maps_train", train_mode)
+        return self._submodule_train(self.STACK_CMG, ins, (), "wn_confidence_maps_train", train_mode)
 
     def confidence_maps_backward(self, grad_maps, saved, shapes, want_inputs=(False,) * 4, train_mode: int = _lib.MODE_BF16X3):
         """d(loss)/d(maps) + the workspaces of ``confidence_maps_train`` -> the 16 cmg parameter gradients
         (state-dict order) and the gradients of x, wb, he, gc where ``want_inputs`` asks for them (else None)."""
-        stream = _stream_ptr(self.device)
-        return self._submodule_backward(grad_maps, saved, shapes, 0, want_inputs, lambda g, arr, gin, n, h, w, ws:
-                                        self.lib.wn_confidence_maps_backward(self.handle, g, arr, gin, n, h, w,
-                                                                             ws.data_ptr(), ws.numel(), stream),
-                                        "wn_confidence_maps_backward", train_mode)
+        return self._submodule_backward(grad_maps, saved, shapes, 0, want_inputs, (), "wn_confidence_maps_backward",
+                                        train_mode)
 
     def refine_train(self, which: int, x, xbar, train_mode: int = _lib.MODE_BF16X3):
         """``refine`` in the arithmetic of training (``train_mode``), keeping the activations of the refiner stack
         (wn_refine_train).  Returns (out, saved workspaces) for ``refine_backward``."""
         ins = self._check_inputs((x, xbar))
-        stream = _stream_ptr(self.device)
-        return self._submodule_train(self.STACK_REFINER, ins, lambda p, st, o, n, h, w, ws: self.lib.wn_refine_train(
-            self.handle, int(which), p[0].data_ptr(), p[1].data_ptr(), st, o.data_ptr(), n, h, w, ws.data_ptr(),
-            ws.numel(), stream), "wn_refine_train", train_mode)
+        return self._submodule_train(self.STACK_REFINER, ins, (int(which),), "wn_refine_train", train_mode)
 
     def refine_backward(self, which: int, grad_out, saved, shapes, want_inputs=(False, False), train_mode: int = _lib.MODE_BF16X3):
         """d(loss)/d(out) + the workspaces of ``refine_train`` -> the 6 parameter gradients of refiner ``which``
         (state-dict order) and the gradients of x, xbar where ``want_inputs`` asks for them (else None)."""
-        stream = _stream_ptr(self.device)
-        return self._submodule_backward(grad_out, saved, shapes, 16 + 6 * int(which), want_inputs,
-                                        lambda g, arr, gin, n, h, w, ws: self.lib.wn_refine_backward(
-                                            self.handle, int(which), g, arr, gin, n, h, w, ws.data_ptr(), ws.numel(),
-                                            stream), "wn_refine_backward", train_mode)
+        return self._submodule_backward(grad_out, saved, shapes, 16 + 6 * int(which), want_inputs, (int(which),),
+                                        "wn_refine_backward", train_mode)
 
     # ---- preprocess / postprocess ----------------------------------------------
     def preprocess(self, rgb_u8: torch.Tensor, tensors: bool = True, images: bool = False):
@@ -578,11 +568,8 @@ class Engine:
                 res[k] = torch.empty((n, h, w, 3), dtype=torch.uint8, device=self.device)
                 ptr[k] = res[k].data_ptr()
         ws = self._workspace("preprocess", self.lib.wn_preprocess_workspace_bytes(n, h, w))
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_preprocess_u8(self.handle, rgb_u8.data_ptr(), n, h, w, ptr["x"], ptr["wb"], ptr["he"],
-                                           ptr["gc"], ptr["wb_u8"], ptr["he_u8"], ptr["gc_u8"],
-                                           ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_preprocess_u8")
+        self._call("wn_preprocess_u8", rgb_u8.data_ptr(), n, h, w, ptr["x"], ptr["wb"], ptr["he"], ptr["gc"],
+                   ptr["wb_u8"], ptr["he_u8"], ptr["gc_u8"], ws.data_ptr(), ws.numel())
         return res
 
     def white_balance_gray(self, gray_u8: torch.Tensor) -> torch.Tensor:
@@ -595,10 +582,7 @@ class Engine:
             return out
         n, h, w = g.shape
         ws = self._workspace("preprocess", self.lib.wn_white_balance_gray_workspace_bytes(n, h, w))
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_white_balance_gray_u8(self.handle, g.data_ptr(), out.data_ptr(), n, h, w, ws.data_ptr(),
-                                                   ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_white_balance_gray_u8")
+        self._call("wn_white_balance_gray_u8", g.data_ptr(), out.data_ptr(), n, h, w, ws.data_ptr(), ws.numel())
         return out
 
     def resize_batch(self, images, dst_h: int, dst_w: int, swap_rb: bool = False) -> torch.Tensor:
@@ -615,13 +599,8 @@ class Engine:
         out = torch.empty((n, dst_h, dst_w, 3), dtype=torch.uint8, device=self.device)
         if n == 0 or out.numel() == 0:
             return out
-        ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in devs])
-        hs = (ctypes.c_int * n)(*[t.shape[0] for t in devs])
-        ws = (ctypes.c_int * n)(*[t.shape[1] for t in devs])
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_resize_u8(self.handle, ptrs, hs, ws, n, out.data_ptr(), dst_h, dst_w, 1 if swap_rb else 0,
-                                       _stream_ptr(self.device))
-        _lib.check(rc, "wn_resize_u8")
+        hs, ws = _sizes([t.shape[:2] for t in devs])
+        self._call("wn_resize_u8", _ptrs(devs), hs, ws, n, out.data_ptr(), dst_h, dst_w, 1 if swap_rb else 0)
         for t in devs:  # the kernel reads them on the current stream after this call returns
             t.record_stream(torch.cuda.current_stream(self.device))
         return out
@@ -635,10 +614,7 @@ class Engine:
         res = torch.empty((n, h, w, 3), dtype=torch.uint8, device=self.device)
         if res.numel() == 0:
             return res
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_postprocess_u8(self.handle, out.data_ptr(), res.data_ptr(), n, h, w,
-                                            _stream_ptr(self.device))
-        _lib.check(rc, "wn_postprocess_u8")
+        self._call("wn_postprocess_u8", out.data_ptr(), res.data_ptr(), n, h, w)
         return res
 
     def _enhance_args(self, rgb_u8, out_u8, out_f32):
@@ -668,12 +644,10 @@ class Engine:
         if out_u8.numel() == 0:
             return out_u8
         ws = self._workspace("enhance", self.lib.wn_enhance_workspace_bytes(n, h, w, mode))
-        peers = (ctypes.c_void_p * max(1, len(peer_out)))(*peer_out)
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_enhance_u8_peers(self.handle, rgb_u8.data_ptr(), out_u8.data_ptr(),
-                                              None if out_f32 is None else out_f32.data_ptr(), peers, len(peer_out),
-                                              n, h, w, mode, ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_enhance_u8_peers")
+        peers = (ctypes.c_void_p * max(1, len(peer_out)))(*peer_out)  # addresses, not tensors
+        self._call("wn_enhance_u8_peers", rgb_u8.data_ptr(), out_u8.data_ptr(),
+                   None if out_f32 is None else out_f32.data_ptr(), peers, len(peer_out), n, h, w, mode, ws.data_ptr(),
+                   ws.numel())
         return out_u8
 
     DEFAULT_TILE = (998, 998)  # a window (tile + 13 pixels of context per side) of at most 1024 x 1024
@@ -704,12 +678,9 @@ class Engine:
             return out_u8
         nbytes = self.lib.wn_enhance_tiled_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels), mode)
         ws = self._workspace("enhance", nbytes)
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_enhance_u8_tiled(self.handle, rgb_u8.data_ptr(), out_u8.data_ptr(),
-                                              None if out_f32 is None else out_f32.data_ptr(), n, h, w, th, tw,
-                                              int(max_pass_pixels), mode, ws.data_ptr(), ws.numel(),
-                                              _stream_ptr(self.device))
-        _lib.check(rc, "wn_enhance_u8_tiled")
+        self._call("wn_enhance_u8_tiled", rgb_u8.data_ptr(), out_u8.data_ptr(),
+                   None if out_f32 is None else out_f32.data_ptr(), n, h, w, th, tw, int(max_pass_pixels), mode,
+                   ws.data_ptr(), ws.numel())
         return out_u8
 
     # ---- the tiled forward of fp32 tensors (wn_forward_tiled, wn_confidence_maps_tiled, wn_refine_tiled) ----------
@@ -741,14 +712,9 @@ class Engine:
             raise ValueError(f"out must be a contiguous float32 {(n, 3, h, w)} tensor on {self.device}")
         if out.numel() == 0:
             return out
-        strides = (ctypes.c_int64 * 16)(*[s for t in ins for s in t.stride()])
         ws = self._workspace("forward", self.forward_tiled_workspace_bytes(n, h, w, (th, tw), mode, max_pass_pixels))
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_forward_tiled(self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(),
-                                           ins[3].data_ptr(), strides, out.data_ptr(), n, h, w, th, tw,
-                                           int(max_pass_pixels), mode, ws.data_ptr(), ws.numel(),
-                                           _stream_ptr(self.device))
-        _lib.check(rc, "wn_forward_tiled")
+        self._call("wn_forward_tiled", *(t.data_ptr() for t in ins), _strides(ins), out.data_ptr(), n, h, w, th, tw,
+                   int(max_pass_pixels), mode, ws.data_ptr(), ws.numel())
         return out
 
     def confidence_maps_tiled(self, x, wb, he, gc, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
@@ -760,14 +726,9 @@ class Engine:
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
         if out.numel() == 0:
             return out
-        strides = (ctypes.c_int64 * 16)(*[s for t in ins for s in t.stride()])
         ws = self._workspace("forward", self.submodule_tiled_workspace_bytes(n, h, w, (th, tw), mode, max_pass_pixels))
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_confidence_maps_tiled(self.handle, ins[0].data_ptr(), ins[1].data_ptr(),
-                                                   ins[2].data_ptr(), ins[3].data_ptr(), strides, out.data_ptr(), n,
-                                                   h, w, th, tw, int(max_pass_pixels), mode, ws.data_ptr(),
-                                                   ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_confidence_maps_tiled")
+        self._call("wn_confidence_maps_tiled", *(t.data_ptr() for t in ins), _strides(ins), out.data_ptr(), n, h, w,
+                   th, tw, int(max_pass_pixels), mode, ws.data_ptr(), ws.numel())
         return out
 
     def refine_tiled(self, which: int, x, xbar, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
@@ -779,13 +740,9 @@ class Engine:
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
         if out.numel() == 0:
             return out
-        strides = (ctypes.c_int64 * 8)(*[s for t in ins for s in t.stride()])
         ws = self._workspace("forward", self.submodule_tiled_workspace_bytes(n, h, w, (th, tw), mode, max_pass_pixels))
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_refine_tiled(self.handle, int(which), ins[0].data_ptr(), ins[1].data_ptr(), strides,
-                                          out.data_ptr(), n, h, w, th, tw, int(max_pass_pixels), mode, ws.data_ptr(),
-                                          ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_refine_tiled")
+        self._call("wn_refine_tiled", int(which), *(t.data_ptr() for t in ins), _strides(ins), out.data_ptr(), n, h,
+                   w, th, tw, int(max_pass_pixels), mode, ws.data_ptr(), ws.numel())
         return out
 
     def ragged_workspace_bytes(self, sizes, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
@@ -793,10 +750,8 @@ class Engine:
         """Workspace of one ``enhance_ragged`` call over images of ``sizes`` [(h, w), ...]
         (wn_enhance_ragged_workspace_bytes); 0 for rejected arguments."""
         th, tw = self._tile_hw(tile)
-        n = len(sizes)
-        hs = (ctypes.c_int * max(1, n))(*[int(h) for h, _ in sizes])
-        ws = (ctypes.c_int * max(1, n))(*[int(w) for _, w in sizes])
-        return int(self.lib.wn_enhance_ragged_workspace_bytes(hs, ws, n, th, tw, int(max_pass_pixels), mode))
+        return int(self.lib.wn_enhance_ragged_workspace_bytes(*_sizes(sizes), len(sizes), th, tw, int(max_pass_pixels),
+                                                              mode))
 
     def enhance_ragged(self, images: Sequence[torch.Tensor], tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
                        out_u8: Optional[Sequence[torch.Tensor]] = None,
@@ -831,10 +786,8 @@ class Engine:
         nbytes = self.ragged_workspace_bytes([(e.height, e.width) for e in entries], (th, tw), mode, max_pass_pixels)
         ws = self._workspace("enhance", nbytes)
         table = (_lib.RaggedImage * len(entries))(*entries)
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_enhance_u8_ragged(self.handle, table, len(entries), th, tw, int(max_pass_pixels), mode,
-                                               ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_enhance_u8_ragged")
+        self._call("wn_enhance_u8_ragged", table, len(entries), th, tw, int(max_pass_pixels), mode, ws.data_ptr(),
+                   ws.numel())
         return outs
 
     # ---- ragged batches of fp32 tensors (wn_forward_ragged, wn_forward_train_ragged / wn_backward_ragged) ---------
@@ -867,15 +820,21 @@ class Engine:
             d.height, d.width = h, w
         return table
 
+    @staticmethod
+    def _ragged_input_grads(gin, images):
+        """input_grads_host of the ragged backward calls: the four input gradients of each of ``images`` (as
+        ``_ragged_items`` lists them) from ``gin`` (per item, four tensors or None), or None when none is asked for."""
+        if all(t is None for row in gin for t in row):
+            return None
+        return _ptrs([None if gin[i][t] is None else gin[i][t][j] for i, j, _, _ in images for t in range(4)])
+
     def forward_ragged_workspace_bytes(self, sizes, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT,
                                        max_pass_pixels: int = 0) -> int:
         """Workspace of one ``forward_ragged`` call over images of ``sizes`` [(h, w), ...]
         (wn_forward_ragged_workspace_bytes); 0 for rejected arguments."""
         th, tw = self._tile_hw(tile)
-        n = len(sizes)
-        hs = (ctypes.c_int * max(1, n))(*[int(h) for h, _ in sizes])
-        ws = (ctypes.c_int * max(1, n))(*[int(w) for _, w in sizes])
-        return int(self.lib.wn_forward_ragged_workspace_bytes(hs, ws, n, th, tw, int(max_pass_pixels), mode))
+        return int(self.lib.wn_forward_ragged_workspace_bytes(*_sizes(sizes), len(sizes), th, tw, int(max_pass_pixels),
+                                                              mode))
 
     def forward_ragged(self, items, tile=DEFAULT_TILE, mode: int = _lib.MODE_DEFAULT, max_pass_pixels: int = 0) -> list:
         """``forward`` of images of their own sizes in one call (wn_forward_ragged).  ``items``: a list of 4-tuples
@@ -890,11 +849,8 @@ class Engine:
         nbytes = self.forward_ragged_workspace_bytes([(h, w) for _, _, h, w in images], (th, tw), mode,
                                                      max_pass_pixels)
         ws = self._workspace("forward", nbytes)
-        table = self._ragged_tensors(ins, outs, images)
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_forward_ragged(self.handle, table, len(images), th, tw, int(max_pass_pixels), mode,
-                                            ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_forward_ragged")
+        self._call("wn_forward_ragged", self._ragged_tensors(ins, outs, images), len(images), th, tw,
+                   int(max_pass_pixels), mode, ws.data_ptr(), ws.numel())
         return outs
 
     def _train_ragged_workspace(self, nbytes: int) -> torch.Tensor:
@@ -917,14 +873,10 @@ class Engine:
         calls = []
         for idx in ragged_train_calls([(h, w) for _, _, h, w in images], self.TRAIN_MAX_PIXELS):
             imgs = [images[k] for k in idx]
-            hs = (ctypes.c_int * len(imgs))(*[h for _, _, h, _ in imgs])
-            wss = (ctypes.c_int * len(imgs))(*[w for _, _, _, w in imgs])
+            hs, wss = _sizes([(h, w) for _, _, h, w in imgs])
             ws = self._train_ragged_workspace(self.lib.wn_train_ragged_workspace_bytes(hs, wss, len(imgs)))
-            table = self._ragged_tensors(ins, outs, imgs)
-            with torch.cuda.device(self.device):
-                rc = self.lib.wn_forward_train_ragged(self.handle, table, len(imgs), ws.data_ptr(), ws.numel(),
-                                                      _stream_ptr(self.device))
-            _lib.check(rc, "wn_forward_train_ragged")
+            self._call("wn_forward_train_ragged", self._ragged_tensors(ins, outs, imgs), len(imgs), ws.data_ptr(),
+                       ws.numel())
             calls.append((imgs, hs, wss, ws))
         return outs, calls
 
@@ -943,16 +895,9 @@ class Engine:
         gin = [[torch.empty_like(g) if want_inputs is not None and want_inputs[i][t] else None for t in range(4)]
                for i, g in enumerate(grads_out)]
         for k, (imgs, hs, wss, ws) in enumerate(saved):
-            arr = (ctypes.c_void_p * _lib.NUM_PARAMS)(*[t.data_ptr() for t in (grads if k == 0 else part)])
-            gptr = (ctypes.c_void_p * len(imgs))(*[grads_out[i][j].data_ptr() for i, j, _, _ in imgs])
-            gin_arr = None
-            if any(t is not None for row in gin for t in row):
-                gin_arr = (ctypes.c_void_p * (4 * len(imgs)))(
-                    *[None if gin[i][t] is None else gin[i][t][j].data_ptr() for i, j, _, _ in imgs for t in range(4)])
-            with torch.cuda.device(self.device):
-                rc = self.lib.wn_backward_ragged(self.handle, hs, wss, gptr, arr, gin_arr, len(imgs), ws.data_ptr(),
-                                                 ws.numel(), _stream_ptr(self.device))
-            _lib.check(rc, "wn_backward_ragged")
+            gptr = _ptrs([grads_out[i][j] for i, j, _, _ in imgs])
+            self._call("wn_backward_ragged", hs, wss, gptr, _grads_array(grads if k == 0 else part),
+                       self._ragged_input_grads(gin, imgs), len(imgs), ws.data_ptr(), ws.numel())
             if k > 0:
                 torch._foreach_add_(grads, part)
         return grads, gin
@@ -984,20 +929,13 @@ class Engine:
         grads = [torch.empty(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
         gin = [torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) for _ in range(4)] \
             if want_input_grads else None
-        nbytes = self.backward_tiled_workspace_bytes(n, h, w, (th, tw), max_pass_pixels)
-        if nbytes == 0:
-            raise _lib.WaterNetLibraryError(
-                f"wn_backward_tiled rejects n={n} h={h} w={w} tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
+        nbytes = _require_workspace(
+            self.backward_tiled_workspace_bytes(n, h, w, (th, tw), max_pass_pixels),
+            f"wn_backward_tiled rejects n={n} h={h} w={w} tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
         ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        strides = (ctypes.c_int64 * 16)(*[s for t in ins for s in t.stride()])
-        arr = (ctypes.c_void_p * _lib.NUM_PARAMS)(*[t.data_ptr() for t in grads])
-        gin_arr = (ctypes.c_void_p * 4)(*[t.data_ptr() for t in gin]) if want_input_grads else None
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_backward_tiled(self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(),
-                                            ins[3].data_ptr(), strides, g.data_ptr(), arr, gin_arr, n, h, w, th, tw,
-                                            int(max_pass_pixels), ws.data_ptr(), ws.numel(),
-                                            _stream_ptr(self.device))
-        _lib.check(rc, "wn_backward_tiled")
+        self._call("wn_backward_tiled", *(t.data_ptr() for t in ins), _strides(ins), g.data_ptr(), _grads_array(grads),
+                   _ptrs(gin) if want_input_grads else None, n, h, w, th, tw, int(max_pass_pixels), ws.data_ptr(),
+                   ws.numel())
         return (grads, gin) if want_input_grads else grads
 
     # ---- windowed recompute backward of a ragged batch (wn_backward_ragged_tiled) -------------------------------
@@ -1005,10 +943,8 @@ class Engine:
         """Workspace of one ``backward_ragged_tiled`` call over images of ``sizes`` [(h, w), ...]
         (wn_backward_ragged_tiled_workspace_bytes); 0 for rejected arguments."""
         th, tw = self._tile_hw(tile)
-        n = len(sizes)
-        hs = (ctypes.c_int * max(1, n))(*[int(h) for h, _ in sizes])
-        ws = (ctypes.c_int * max(1, n))(*[int(w) for _, w in sizes])
-        return int(self.lib.wn_backward_ragged_tiled_workspace_bytes(hs, ws, n, th, tw, int(max_pass_pixels)))
+        return int(self.lib.wn_backward_ragged_tiled_workspace_bytes(*_sizes(sizes), len(sizes), th, tw,
+                                                                     int(max_pass_pixels)))
 
     def backward_ragged_tiled(self, grad_outs, items, shapes, tile=DEFAULT_TILE, want_inputs=None,
                               max_pass_pixels: int = 0, train_mode: int = _lib.MODE_BF16X3):
@@ -1034,24 +970,15 @@ class Engine:
         if not images:
             return grads, gin
         sizes = [(h, w) for _, _, h, w in images]
-        nbytes = self.backward_ragged_tiled_workspace_bytes(sizes, (th, tw), max_pass_pixels)
-        if nbytes == 0:
-            raise _lib.WaterNetLibraryError(
-                f"wn_backward_ragged_tiled rejects {len(images)} images up to {max(h for h, _ in sizes)}x"
-                f"{max(w for _, w in sizes)} at tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
+        nbytes = _require_workspace(
+            self.backward_ragged_tiled_workspace_bytes(sizes, (th, tw), max_pass_pixels),
+            f"wn_backward_ragged_tiled rejects {len(images)} images up to {max(h for h, _ in sizes)}x"
+            f"{max(w for _, w in sizes)} at tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
         ws = self._train_ragged_workspace(nbytes)
-        table = self._ragged_tensors(ins, [None] * len(ins), images)
-        gptr = (ctypes.c_void_p * len(images))(*[grads_out[i][j].data_ptr() for i, j, _, _ in images])
-        arr = (ctypes.c_void_p * _lib.NUM_PARAMS)(*[t.data_ptr() for t in grads])
-        gin_arr = None
-        if any(t is not None for row in gin for t in row):
-            gin_arr = (ctypes.c_void_p * (4 * len(images)))(
-                *[None if gin[i][t] is None else gin[i][t][j].data_ptr() for i, j, _, _ in images for t in range(4)])
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_backward_ragged_tiled(self.handle, table, gptr, arr, gin_arr, len(images), th, tw,
-                                                   int(max_pass_pixels), ws.data_ptr(), ws.numel(),
-                                                   _stream_ptr(self.device))
-        _lib.check(rc, "wn_backward_ragged_tiled")
+        self._call("wn_backward_ragged_tiled", self._ragged_tensors(ins, [None] * len(ins), images),
+                   _ptrs([grads_out[i][j] for i, j, _, _ in images]), _grads_array(grads),
+                   self._ragged_input_grads(gin, images), len(images), th, tw, int(max_pass_pixels), ws.data_ptr(),
+                   ws.numel())
         return grads, gin
 
     # ---- windowed recompute backward of one sub-module (wn_confidence_maps_backward_tiled, wn_refine_backward_tiled) --
@@ -1064,10 +991,10 @@ class Engine:
                                                                         int(stack)))
 
     def _submodule_backward_tiled(self, stack: int, first: int, grad, ins, shapes, tile, want_inputs,
-                                  max_pass_pixels: int, call, what: str, train_mode: int):
+                                  max_pass_pixels: int, lead, what: str, train_mode: int):
         """The parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) and the input gradients
-        asked for by ``want_inputs`` (None where not), in one call with a workspace of its own.  call(strides, grad,
-        grads array, input grads array or None, n, h, w, th, tw, workspace) -> rc."""
+        asked for by ``want_inputs`` (None where not), in one call of ``what`` with a workspace of its own and the
+        arguments ``lead`` (which) before the inputs."""
         self.set_train_mode(train_mode)
         th, tw = self._tile_hw(tile)
         g = grad.detach().to(self.device, torch.float32).contiguous()
@@ -1079,21 +1006,13 @@ class Engine:
         gin = [make((n, 3, h, w), dtype=torch.float32, device=self.device) if want else None for want in want_inputs]
         if g.numel() == 0:
             return grads, gin
-        nbytes = self.submodule_backward_tiled_workspace_bytes(n, h, w, stack, (th, tw), max_pass_pixels)
-        if nbytes == 0:
-            raise _lib.WaterNetLibraryError(
-                f"{what} rejects n={n} h={h} w={w} tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
+        nbytes = _require_workspace(
+            self.submodule_backward_tiled_workspace_bytes(n, h, w, stack, (th, tw), max_pass_pixels),
+            f"{what} rejects n={n} h={h} w={w} tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
         ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        strides = (ctypes.c_int64 * (4 * len(ins)))(*[s for t in ins for s in t.stride()])
-        arr = (ctypes.c_void_p * _lib.NUM_PARAMS)()
-        for k, t in enumerate(grads):
-            arr[first + k] = t.data_ptr()
-        gin_arr = None
-        if any(want_inputs):
-            gin_arr = (ctypes.c_void_p * len(gin))(*[None if t is None else t.data_ptr() for t in gin])
-        with torch.cuda.device(self.device):
-            rc = call(strides, g.data_ptr(), arr, gin_arr, n, h, w, th, tw, ws)
-        _lib.check(rc, what)
+        self._call(what, *lead, *(t.data_ptr() for t in ins), _strides(ins), g.data_ptr(), _grads_array(grads, first),
+                   _ptrs(gin) if any(want_inputs) else None, n, h, w, th, tw, max_pass_pixels, ws.data_ptr(),
+                   ws.numel())
         return grads, gin
 
     def confidence_maps_backward_tiled(self, grad_maps, inputs, shapes, tile=DEFAULT_TILE, want_inputs=(False,) * 4,
@@ -1105,27 +1024,17 @@ class Engine:
         parameter gradients and the input gradients ``want_inputs`` asks for (else None).  The workspace is allocated
         for this call only."""
         ins = self._check_inputs(inputs)
-        stream = _stream_ptr(self.device)
-        mpp = int(max_pass_pixels)
-        return self._submodule_backward_tiled(
-            self.STACK_CMG, 0, grad_maps, ins, shapes, tile, want_inputs, mpp,
-            lambda st, g, arr, gin, n, h, w, th, tw, ws: self.lib.wn_confidence_maps_backward_tiled(
-                self.handle, ins[0].data_ptr(), ins[1].data_ptr(), ins[2].data_ptr(), ins[3].data_ptr(), st, g, arr,
-                gin, n, h, w, th, tw, mpp, ws.data_ptr(), ws.numel(), stream), "wn_confidence_maps_backward_tiled",
-            train_mode)
+        return self._submodule_backward_tiled(self.STACK_CMG, 0, grad_maps, ins, shapes, tile, want_inputs,
+                                              int(max_pass_pixels), (), "wn_confidence_maps_backward_tiled", train_mode)
 
     def refine_backward_tiled(self, which: int, grad_out, inputs, shapes, tile=DEFAULT_TILE,
                               want_inputs=(False, False), max_pass_pixels: int = 0, train_mode: int = _lib.MODE_BF16X3):
         """The gradients of ``refine_backward`` from x and xbar alone (wn_refine_backward_tiled), as
         ``confidence_maps_backward_tiled`` (0 = 2 Mi window pixels per pass, ~3.8 GB)."""
         ins = self._check_inputs(inputs)
-        stream = _stream_ptr(self.device)
-        mpp = int(max_pass_pixels)
-        return self._submodule_backward_tiled(
-            self.STACK_REFINER, 16 + 6 * int(which), grad_out, ins, shapes, tile, want_inputs, mpp,
-            lambda st, g, arr, gin, n, h, w, th, tw, ws: self.lib.wn_refine_backward_tiled(
-                self.handle, int(which), ins[0].data_ptr(), ins[1].data_ptr(), st, g, arr, gin, n, h, w, th, tw, mpp,
-                ws.data_ptr(), ws.numel(), stream), "wn_refine_backward_tiled", train_mode)
+        return self._submodule_backward_tiled(self.STACK_REFINER, 16 + 6 * int(which), grad_out, ins, shapes, tile,
+                                              want_inputs, int(max_pass_pixels), (int(which),),
+                                              "wn_refine_backward_tiled", train_mode)
 
     # ---- the VGG19 perceptual loss (wn_perceptual_loss) ----------------------------------------
     def pack_vgg_weights(self, params: Sequence[torch.Tensor], key=None) -> None:
@@ -1141,9 +1050,7 @@ class Engine:
         if key is not None and key == getattr(self, "_vgg_key", None):
             return
         staged = [p.detach().to(device=self.device, dtype=torch.float32).contiguous() for p in params]
-        arr = (ctypes.c_void_p * _lib.VGG_NUM_PARAMS)(*[t.data_ptr() for t in staged])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.wn_vgg_pack_weights(self.handle, arr, _stream_ptr(self.device)), "wn_vgg_pack_weights")
+        self._call("wn_vgg_pack_weights", _ptrs(staged))
         self._vgg_keepalive = staged  # until the async pack kernels have consumed them
         self._vgg_key = key
 
@@ -1178,13 +1085,8 @@ class Engine:
         ws = self._vgg_workspace(n, h, w, th, tw, mpp, "perceptual_loss")
         loss = torch.empty((), dtype=torch.float32, device=self.device)
         grad = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) if want_grad else None
-        so = (ctypes.c_int64 * 4)(*o.stride())
-        sr = (ctypes.c_int64 * 4)(*r.stride())
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_perceptual_loss(self.handle, o.data_ptr(), so, r.data_ptr(), sr, n, h, w, th, tw, mpp,
-                                             loss.data_ptr(), grad.data_ptr() if grad is not None else None,
-                                             ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_perceptual_loss")
+        self._call("wn_perceptual_loss", o.data_ptr(), _strides((o,)), r.data_ptr(), _strides((r,)), n, h, w, th, tw,
+                   mpp, loss.data_ptr(), grad.data_ptr() if grad is not None else None, ws.data_ptr(), ws.numel())
         return loss, grad
 
     def debug_vgg_layer(self, x, layer: int, tile=None, ref=None, train_mode: int = _lib.MODE_BF16X3) -> torch.Tensor:
@@ -1212,10 +1114,7 @@ class Engine:
         r = ref.detach().float() if ref is not None else None
         dst = torch.empty(shape, dtype=torch.float32, device=self.device)
         ws = self._vgg_workspace(n, h, w, th, tw, 0, "debug_vgg_layer")
-        with torch.cuda.device(self.device):
-            rc = self.lib.wn_debug_vgg_layer(
-                self.handle, x.data_ptr(), (ctypes.c_int64 * 4)(*x.stride()), r.data_ptr() if r is not None else None,
-                (ctypes.c_int64 * 4)(*r.stride()) if r is not None else None, n, h, w, th, tw, int(layer),
-                dst.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr(self.device))
-        _lib.check(rc, "wn_debug_vgg_layer")
+        self._call("wn_debug_vgg_layer", x.data_ptr(), _strides((x,)), r.data_ptr() if r is not None else None,
+                   _strides((r,)) if r is not None else None, n, h, w, th, tw, int(layer), dst.data_ptr(),
+                   ws.data_ptr(), ws.numel())
         return dst
