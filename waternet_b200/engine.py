@@ -397,53 +397,82 @@ class Engine:
     TRAIN_MAX_PIXELS = 8 << 20
     TRAIN_MAX_IMAGES = 65535
 
-    def forward_train(self, x, wb, he, gc, train_mode: int = _lib.MODE_BF16X3):
-        """Tensor-core forward that keeps every activation.  Returns (out, saved workspaces).
+    def _param_grads(self, shapes, written: bool):
+        """fp32 tensors of ``shapes`` for parameter gradients: uninitialised when a library call writes them, else
+        zeros (nothing to run has zero gradients)."""
+        make = torch.empty if written else torch.zeros
+        return [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
 
-        wn_forward_train takes at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES per call; a larger batch runs as several
-        calls over slices of the batch, each with its own workspace (~5.6 KB per pixel in total, like the reference's autograd graph)."""
-        ins = self._check_inputs((x, wb, he, gc))
+    def _sum_in_order(self, shapes, calls, run):
+        """The parameter gradients of ``shapes`` summed over ``calls`` in order: ``run(call, dst)`` makes one library
+        call that writes its gradients into ``dst``; the first call writes the result, each later one a scratch set
+        that is added to it in call order (deterministic)."""
+        grads = self._param_grads(shapes, bool(calls))
+        part = grads if len(calls) <= 1 else [torch.empty_like(t) for t in grads]
+        for k, call in enumerate(calls):
+            run(call, grads if k == 0 else part)
+            if k > 0:
+                torch._foreach_add_(grads, part)
+        return grads
+
+    def _train_slices(self, what: str, lead, ins, workspace_bytes, too_large: str, train_mode: int):
+        """``ins`` in slices of at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES, each one call of ``what`` (``lead``
+        before the inputs) with a workspace of its own of ``workspace_bytes(n, h, w)`` bytes.  Returns (out, [(a, b,
+        workspace), ...]), or (out, None) for an empty batch.  One image over TRAIN_MAX_PIXELS raises ``too_large``
+        with ``{h}`` and ``{w}`` filled in."""
         self.set_train_mode(train_mode)
         n, _, h, w = ins[0].shape
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
         if out.numel() == 0:
             return out, None
         if h * w > self.TRAIN_MAX_PIXELS:
-            raise _lib.WaterNetLibraryError(
-                f"a forward pass that keeps its activations for autograd holds ~5.6 KB per pixel: one {h}x{w} image "
-                f"exceeds the {self.TRAIN_MAX_PIXELS >> 20} Mi-pixel limit of wn_forward_train.  For inference wrap the "
-                "call in torch.no_grad()")
+            raise _lib.WaterNetLibraryError(too_large.format(h=h, w=w))
         per = min(self.TRAIN_MAX_IMAGES, max(1, self.TRAIN_MAX_PIXELS // (h * w)))
         saved = []
         for a in range(0, n, per):
             b = min(n, a + per)
             part = [t[a:b] for t in ins]
-            ws = torch.empty(self.lib.wn_train_workspace_bytes(b - a, h, w), dtype=torch.uint8, device=self.device)
-            self._call("wn_forward_train", *(t.data_ptr() for t in part), _strides(part), out[a:b].data_ptr(), b - a,
-                       h, w, ws.data_ptr(), ws.numel())
+            ws = torch.empty(workspace_bytes(b - a, h, w), dtype=torch.uint8, device=self.device)
+            self._call(what, *lead, *(t.data_ptr() for t in part), _strides(part), out[a:b].data_ptr(), b - a, h, w,
+                       ws.data_ptr(), ws.numel())
             saved.append((a, b, ws))
         return out, saved
+
+    def _slices_backward(self, what: str, lead, first: int, grad, saved, shapes, want_inputs, train_mode: int):
+        """The backward of the slices of ``_train_slices``: one call of ``what`` per slice (``lead`` before the
+        gradient), the parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) summed in slice
+        order, and the input gradients asked for by ``want_inputs`` (None where not)."""
+        self.set_train_mode(train_mode)
+        g = grad.detach().to(self.device, torch.float32).contiguous()
+        n, _, h, w = g.shape
+        gin = [torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) if want else None
+               for want in want_inputs]
+
+        def run(call, dst):
+            a, b, ws = call
+            gin_arr = _ptrs([None if t is None else t[a:b] for t in gin]) if any(want_inputs) else None
+            self._call(what, *lead, g[a:b].data_ptr(), _grads_array(dst, first), gin_arr, b - a, h, w, ws.data_ptr(),
+                       ws.numel())
+        return self._sum_in_order(shapes, saved or [], run), gin
+
+    def forward_train(self, x, wb, he, gc, train_mode: int = _lib.MODE_BF16X3):
+        """Tensor-core forward that keeps every activation.  Returns (out, saved workspaces).
+
+        wn_forward_train takes at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES per call; a larger batch runs as several
+        calls over slices of the batch, each with its own workspace (~5.6 KB per pixel in total, like the reference's autograd graph)."""
+        ins = self._check_inputs((x, wb, he, gc))
+        return self._train_slices(
+            "wn_forward_train", (), ins, self.lib.wn_train_workspace_bytes,
+            "a forward pass that keeps its activations for autograd holds ~5.6 KB per pixel: one {h}x{w} image exceeds "
+            f"the {self.TRAIN_MAX_PIXELS >> 20} Mi-pixel limit of wn_forward_train.  For inference wrap the call in "
+            "torch.no_grad()", train_mode)
 
     def backward(self, grad_out: torch.Tensor, saved, shapes, want_input_grads: bool = False, train_mode: int = _lib.MODE_BF16X3):
         """d(loss)/d(out) + the workspaces of forward_train -> the 34 parameter gradients (state-dict order)
         and, on request, the gradients of the four input images.  Batch slices are processed in order and their
         parameter gradients added in that order (deterministic).  ``train_mode``: that of the forward."""
-        self.set_train_mode(train_mode)
-        g = grad_out.detach().to(self.device, torch.float32).contiguous()
-        n, _, h, w = g.shape
-        saved = saved or []
-        make = torch.empty if saved else torch.zeros  # an empty batch has zero gradients
-        grads = [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
-        part = grads if len(saved) <= 1 else [torch.empty_like(t) for t in grads]
-        gin = None
-        if want_input_grads:
-            gin = [torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) for _ in range(4)]
-        for i, (a, b, ws) in enumerate(saved):
-            gin_arr = _ptrs([t[a:b] for t in gin]) if want_input_grads else None
-            self._call("wn_backward", g[a:b].data_ptr(), _grads_array(grads if i == 0 else part), gin_arr, b - a, h, w,
-                       ws.data_ptr(), ws.numel())
-            if i > 0:
-                torch._foreach_add_(grads, part)
+        grads, gin = self._slices_backward("wn_backward", (), 0, grad_out, saved, shapes, (want_input_grads,) * 4,
+                                           train_mode)
         return (grads, gin) if want_input_grads else grads
 
     # wn_debug_backward_layer's buffers 0..24 (include/waternet_b200.h): act0, a1..a7, cm, r1, r2, refined, g8, gr3 and
@@ -472,73 +501,35 @@ class Engine:
     # ---- the sub-modules under autograd (wn_confidence_maps_train / _backward, wn_refine_train / _backward) --------
     STACK_CMG, STACK_REFINER = 0, 1
 
-    def _submodule_train(self, stack: int, ins, lead, what: str, train_mode: int):
-        """The batch in slices of at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES, one workspace per slice, as
-        ``forward_train``.  Each slice is one call of ``what`` with the arguments ``lead`` (which) before the inputs."""
-        self.set_train_mode(train_mode)
-        n, _, h, w = ins[0].shape
-        out = torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device)
-        if out.numel() == 0:
-            return out, None
-        if h * w > self.TRAIN_MAX_PIXELS:
-            raise _lib.WaterNetLibraryError(
-                f"{what}: one {h}x{w} image exceeds the {self.TRAIN_MAX_PIXELS} pixels of one training call")
-        per = min(self.TRAIN_MAX_IMAGES, max(1, self.TRAIN_MAX_PIXELS // (h * w)))
-        saved = []
-        for a in range(0, n, per):
-            b = min(n, a + per)
-            part = [t[a:b] for t in ins]
-            nbytes = self.lib.wn_submodule_train_workspace_bytes(b - a, h, w, stack)
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            self._call(what, *lead, *(t.data_ptr() for t in part), _strides(part), out[a:b].data_ptr(), b - a, h, w,
-                       ws.data_ptr(), ws.numel())
-            saved.append((a, b, ws))
-        return out, saved
-
-    def _submodule_backward(self, grad, saved, shapes, first: int, want_inputs, lead, what: str, train_mode: int):
-        """The parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) added in slice order, and
-        the input gradients asked for by ``want_inputs`` (None where not).  Each slice is one call of ``what`` with the
-        arguments ``lead`` (which) before the gradient."""
-        self.set_train_mode(train_mode)
-        g = grad.detach().to(self.device, torch.float32).contiguous()
-        n, _, h, w = g.shape
-        saved = saved or []
-        make = torch.empty if saved else torch.zeros  # an empty batch has zero gradients
-        grads = [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
-        part = grads if len(saved) <= 1 else [torch.empty_like(t) for t in grads]
-        gin = [torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) if want else None
-               for want in want_inputs]
-        for i, (a, b, ws) in enumerate(saved):
-            gin_arr = _ptrs([None if t is None else t[a:b] for t in gin]) if any(want_inputs) else None
-            self._call(what, *lead, g[a:b].data_ptr(), _grads_array(grads if i == 0 else part, first), gin_arr, b - a,
-                       h, w, ws.data_ptr(), ws.numel())
-            if i > 0:
-                torch._foreach_add_(grads, part)
-        return grads, gin
+    def _submodule_train_slices(self, what: str, lead, stack: int, ins, train_mode: int):
+        """``_train_slices`` of one stack (wn_submodule_train_workspace_bytes of ``stack`` per slice)."""
+        return self._train_slices(
+            what, lead, ins, lambda n, h, w: self.lib.wn_submodule_train_workspace_bytes(n, h, w, stack),
+            f"{what}: one {{h}}x{{w}} image exceeds the {self.TRAIN_MAX_PIXELS} pixels of one training call", train_mode)
 
     def confidence_maps_train(self, x, wb, he, gc, train_mode: int = _lib.MODE_BF16X3):
         """``confidence_maps`` in the arithmetic of training (``train_mode``), keeping the activations of the cmg stack
         (wn_confidence_maps_train).  Returns (maps, saved workspaces) for ``confidence_maps_backward``."""
         ins = self._check_inputs((x, wb, he, gc))
-        return self._submodule_train(self.STACK_CMG, ins, (), "wn_confidence_maps_train", train_mode)
+        return self._submodule_train_slices("wn_confidence_maps_train", (), self.STACK_CMG, ins, train_mode)
 
     def confidence_maps_backward(self, grad_maps, saved, shapes, want_inputs=(False,) * 4, train_mode: int = _lib.MODE_BF16X3):
         """d(loss)/d(maps) + the workspaces of ``confidence_maps_train`` -> the 16 cmg parameter gradients
         (state-dict order) and the gradients of x, wb, he, gc where ``want_inputs`` asks for them (else None)."""
-        return self._submodule_backward(grad_maps, saved, shapes, 0, want_inputs, (), "wn_confidence_maps_backward",
-                                        train_mode)
+        return self._slices_backward("wn_confidence_maps_backward", (), 0, grad_maps, saved, shapes, want_inputs,
+                                     train_mode)
 
     def refine_train(self, which: int, x, xbar, train_mode: int = _lib.MODE_BF16X3):
         """``refine`` in the arithmetic of training (``train_mode``), keeping the activations of the refiner stack
         (wn_refine_train).  Returns (out, saved workspaces) for ``refine_backward``."""
         ins = self._check_inputs((x, xbar))
-        return self._submodule_train(self.STACK_REFINER, ins, (int(which),), "wn_refine_train", train_mode)
+        return self._submodule_train_slices("wn_refine_train", (int(which),), self.STACK_REFINER, ins, train_mode)
 
     def refine_backward(self, which: int, grad_out, saved, shapes, want_inputs=(False, False), train_mode: int = _lib.MODE_BF16X3):
         """d(loss)/d(out) + the workspaces of ``refine_train`` -> the 6 parameter gradients of refiner ``which``
         (state-dict order) and the gradients of x, xbar where ``want_inputs`` asks for them (else None)."""
-        return self._submodule_backward(grad_out, saved, shapes, 16 + 6 * int(which), want_inputs, (int(which),),
-                                        "wn_refine_backward", train_mode)
+        return self._slices_backward("wn_refine_backward", (int(which),), 16 + 6 * int(which), grad_out, saved, shapes,
+                                     want_inputs, train_mode)
 
     # ---- preprocess / postprocess ----------------------------------------------
     def preprocess(self, rgb_u8: torch.Tensor, tensors: bool = True, images: bool = False):
@@ -887,20 +878,21 @@ class Engine:
         everywhere when ``want_inputs`` is None)."""
         self.set_train_mode(train_mode)
         grads_out = [g.detach().to(self.device, torch.float32).contiguous() for g in grad_outs]
-        saved = saved or []
-        make = torch.empty if saved else torch.zeros  # no images: zero gradients
-        grads = [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
-        part = grads if len(saved) <= 1 else [torch.empty_like(t) for t in grads]
-        # every image with pixels is written whole by its call; zero-pixel items are never passed to the library
-        gin = [[torch.empty_like(g) if want_inputs is not None and want_inputs[i][t] else None for t in range(4)]
-               for i, g in enumerate(grads_out)]
-        for k, (imgs, hs, wss, ws) in enumerate(saved):
-            gptr = _ptrs([grads_out[i][j] for i, j, _, _ in imgs])
-            self._call("wn_backward_ragged", hs, wss, gptr, _grads_array(grads if k == 0 else part),
-                       self._ragged_input_grads(gin, imgs), len(imgs), ws.data_ptr(), ws.numel())
-            if k > 0:
-                torch._foreach_add_(grads, part)
-        return grads, gin
+        gin = self._ragged_gin(grads_out, want_inputs)
+
+        def run(call, dst):
+            imgs, hs, wss, ws = call
+            self._call("wn_backward_ragged", hs, wss, _ptrs([grads_out[i][j] for i, j, _, _ in imgs]),
+                       _grads_array(dst), self._ragged_input_grads(gin, imgs), len(imgs), ws.data_ptr(), ws.numel())
+        return self._sum_in_order(shapes, saved or [], run), gin
+
+    @staticmethod
+    def _ragged_gin(grads_out, want_inputs):
+        """The input gradients of the ragged backward calls: per item, four tensors like its output gradient, None
+        where ``want_inputs[i][t]`` is false or everywhere when ``want_inputs`` is None.  Every image with pixels is
+        written whole by the library; zero-pixel items have no elements."""
+        return [[torch.empty_like(g) if want_inputs is not None and want_inputs[i][t] else None for t in range(4)]
+                for i, g in enumerate(grads_out)]
 
     # ---- windowed recompute backward (wn_backward_tiled) -------------------------------------------
     def backward_tiled_workspace_bytes(self, n: int, h: int, w: int, tile=DEFAULT_TILE, max_pass_pixels: int = 0) -> int:
@@ -915,28 +907,37 @@ class Engine:
         activation outlives the call and the workspace does not grow with the image size.  ``max_pass_pixels``:
         window pixels per pass (0 = 2 Mi, ~11.8 GB).  The workspace is allocated for this call only.  ``train_mode``:
         the arithmetic of the recomputed forward and of the backward."""
+        grads, gin = self._windowed_backward("wn_backward_tiled", (), None, 0, "grad_out", grad_out, inputs, shapes,
+                                             tile, (want_input_grads,) * 4, max_pass_pixels, train_mode)
+        return (grads, gin) if want_input_grads else grads
+
+    def _windowed_backward(self, what: str, lead, stack, first: int, grad_name: str, grad, inputs, shapes, tile,
+                           want_inputs, max_pass_pixels, train_mode: int):
+        """One call of ``what`` (``lead`` before the inputs) that recomputes the training forward of ``inputs`` in
+        windows, with a workspace of its own (of the whole network for ``stack`` None, else of that stack): the
+        parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) and the input gradients asked for
+        by ``want_inputs`` (None where not).  An empty batch has zero gradients and makes no call."""
         self.set_train_mode(train_mode)
         th, tw = self._tile_hw(tile)
         ins = self._check_inputs(inputs)
-        g = grad_out.detach().to(self.device, torch.float32).contiguous()
+        g = grad.detach().to(self.device, torch.float32).contiguous()
         n, _, h, w = ins[0].shape
         if tuple(g.shape) != (n, 3, h, w):
-            raise ValueError(f"grad_out must be {(n, 3, h, w)}, got {tuple(g.shape)}")
+            raise ValueError(f"{grad_name} must be {(n, 3, h, w)}, got {tuple(g.shape)}")
+        grads = self._param_grads(shapes, g.numel() > 0)
+        make = torch.empty if g.numel() else torch.zeros
+        gin = [make((n, 3, h, w), dtype=torch.float32, device=self.device) if want else None for want in want_inputs]
         if g.numel() == 0:
-            grads = [torch.zeros(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
-            gin = [torch.zeros((n, 3, h, w), dtype=torch.float32, device=self.device) for _ in range(4)]
-            return (grads, gin) if want_input_grads else grads
-        grads = [torch.empty(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
-        gin = [torch.empty((n, 3, h, w), dtype=torch.float32, device=self.device) for _ in range(4)] \
-            if want_input_grads else None
+            return grads, gin
         nbytes = _require_workspace(
-            self.backward_tiled_workspace_bytes(n, h, w, (th, tw), max_pass_pixels),
-            f"wn_backward_tiled rejects n={n} h={h} w={w} tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
+            self.backward_tiled_workspace_bytes(n, h, w, (th, tw), max_pass_pixels) if stack is None else
+            self.submodule_backward_tiled_workspace_bytes(n, h, w, stack, (th, tw), max_pass_pixels),
+            f"{what} rejects n={n} h={h} w={w} tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
         ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        self._call("wn_backward_tiled", *(t.data_ptr() for t in ins), _strides(ins), g.data_ptr(), _grads_array(grads),
-                   _ptrs(gin) if want_input_grads else None, n, h, w, th, tw, int(max_pass_pixels), ws.data_ptr(),
+        self._call(what, *lead, *(t.data_ptr() for t in ins), _strides(ins), g.data_ptr(), _grads_array(grads, first),
+                   _ptrs(gin) if any(want_inputs) else None, n, h, w, th, tw, int(max_pass_pixels), ws.data_ptr(),
                    ws.numel())
-        return (grads, gin) if want_input_grads else grads
+        return grads, gin
 
     # ---- windowed recompute backward of a ragged batch (wn_backward_ragged_tiled) -------------------------------
     def backward_ragged_tiled_workspace_bytes(self, sizes, tile=DEFAULT_TILE, max_pass_pixels: int = 0) -> int:
@@ -962,11 +963,8 @@ class Engine:
         for i, (t, g) in enumerate(zip(ins, grads_out)):
             if g.shape != t[0].shape:
                 raise ValueError(f"item {i}: the output gradient must be {tuple(t[0].shape)}, got {tuple(g.shape)}")
-        make = torch.empty if images else torch.zeros  # no images: zero gradients
-        grads = [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
-        # every image with pixels is written whole by the call; zero-pixel items have no elements
-        gin = [[torch.empty_like(g) if want_inputs is not None and want_inputs[i][t] else None for t in range(4)]
-               for i, g in enumerate(grads_out)]
+        grads = self._param_grads(shapes, bool(images))
+        gin = self._ragged_gin(grads_out, want_inputs)
         if not images:
             return grads, gin
         sizes = [(h, w) for _, _, h, w in images]
@@ -990,31 +988,6 @@ class Engine:
         return int(self.lib.wn_submodule_backward_tiled_workspace_bytes(n, h, w, th, tw, int(max_pass_pixels),
                                                                         int(stack)))
 
-    def _submodule_backward_tiled(self, stack: int, first: int, grad, ins, shapes, tile, want_inputs,
-                                  max_pass_pixels: int, lead, what: str, train_mode: int):
-        """The parameter gradients of ``shapes`` (state-dict entries first, first + 1, ...) and the input gradients
-        asked for by ``want_inputs`` (None where not), in one call of ``what`` with a workspace of its own and the
-        arguments ``lead`` (which) before the inputs."""
-        self.set_train_mode(train_mode)
-        th, tw = self._tile_hw(tile)
-        g = grad.detach().to(self.device, torch.float32).contiguous()
-        n, _, h, w = ins[0].shape
-        if tuple(g.shape) != (n, 3, h, w):
-            raise ValueError(f"the output gradient must be {(n, 3, h, w)}, got {tuple(g.shape)}")
-        make = torch.zeros if g.numel() == 0 else torch.empty  # an empty batch has zero gradients
-        grads = [make(tuple(s), dtype=torch.float32, device=self.device) for s in shapes]
-        gin = [make((n, 3, h, w), dtype=torch.float32, device=self.device) if want else None for want in want_inputs]
-        if g.numel() == 0:
-            return grads, gin
-        nbytes = _require_workspace(
-            self.submodule_backward_tiled_workspace_bytes(n, h, w, stack, (th, tw), max_pass_pixels),
-            f"{what} rejects n={n} h={h} w={w} tile={th}x{tw} max_pass_pixels={max_pass_pixels}")
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        self._call(what, *lead, *(t.data_ptr() for t in ins), _strides(ins), g.data_ptr(), _grads_array(grads, first),
-                   _ptrs(gin) if any(want_inputs) else None, n, h, w, th, tw, max_pass_pixels, ws.data_ptr(),
-                   ws.numel())
-        return grads, gin
-
     def confidence_maps_backward_tiled(self, grad_maps, inputs, shapes, tile=DEFAULT_TILE, want_inputs=(False,) * 4,
                                        max_pass_pixels: int = 0, train_mode: int = _lib.MODE_BF16X3):
         """The gradients of ``confidence_maps_backward`` from the four input images alone
@@ -1023,18 +996,19 @@ class Engine:
         grow with the image size.  ``max_pass_pixels``: window pixels per pass (0 = 2 Mi, ~8.1 GB).  Returns the 16
         parameter gradients and the input gradients ``want_inputs`` asks for (else None).  The workspace is allocated
         for this call only."""
-        ins = self._check_inputs(inputs)
-        return self._submodule_backward_tiled(self.STACK_CMG, 0, grad_maps, ins, shapes, tile, want_inputs,
-                                              int(max_pass_pixels), (), "wn_confidence_maps_backward_tiled", train_mode)
+        ins = self._check_inputs(inputs)  # a sub-module call reports bad inputs before a bad tile or mode
+        return self._windowed_backward("wn_confidence_maps_backward_tiled", (), self.STACK_CMG, 0,
+                                       "the output gradient", grad_maps, ins, shapes, tile, want_inputs,
+                                       int(max_pass_pixels), train_mode)
 
     def refine_backward_tiled(self, which: int, grad_out, inputs, shapes, tile=DEFAULT_TILE,
                               want_inputs=(False, False), max_pass_pixels: int = 0, train_mode: int = _lib.MODE_BF16X3):
         """The gradients of ``refine_backward`` from x and xbar alone (wn_refine_backward_tiled), as
         ``confidence_maps_backward_tiled`` (0 = 2 Mi window pixels per pass, ~3.8 GB)."""
         ins = self._check_inputs(inputs)
-        return self._submodule_backward_tiled(self.STACK_REFINER, 16 + 6 * int(which), grad_out, ins, shapes, tile,
-                                              want_inputs, int(max_pass_pixels), (int(which),),
-                                              "wn_refine_backward_tiled", train_mode)
+        return self._windowed_backward("wn_refine_backward_tiled", (int(which),), self.STACK_REFINER,
+                                       16 + 6 * int(which), "the output gradient", grad_out, ins, shapes, tile,
+                                       want_inputs, int(max_pass_pixels), train_mode)
 
     # ---- the VGG19 perceptual loss (wn_perceptual_loss) ----------------------------------------
     def pack_vgg_weights(self, params: Sequence[torch.Tensor], key=None) -> None:

@@ -22,7 +22,7 @@ from __future__ import annotations
 
 import threading
 import weakref
-from typing import List
+from typing import List, NamedTuple
 
 import torch
 import torch.nn as nn
@@ -38,11 +38,6 @@ MODES = {"default": _lib.MODE_DEFAULT, "fp32": _lib.MODE_FP32_SIMT, "bf16x3": _l
 TRAIN_PRECISIONS = {"bf16x3": _lib.MODE_BF16X3, "bf16": _lib.MODE_BF16}
 
 
-def _checked_train_mode(train_precision) -> int:
-    if train_precision not in TRAIN_PRECISIONS:
-        raise ValueError(f"unknown train_precision {train_precision!r}; choose from {sorted(TRAIN_PRECISIONS)}")
-    return TRAIN_PRECISIONS[train_precision]
-
 # model -> {device index: Engine}.  Every module that can be called on its own (WaterNet and, like in the
 # reference, its sub-modules) has a private engine per device = its own packed-weight slot in the library.
 # Kept outside the module so that copy.deepcopy / pickling of a model never touches a C handle.
@@ -50,24 +45,15 @@ _model_engines = weakref.WeakKeyDictionary()
 _model_engines_lock = threading.Lock()
 
 
-def _checked_tile(tile, mode: int):
-    """``tile`` as (h, w), or None for whole images per pass.  The tiled forward runs on the tensor cores only."""
+def _checked_tile(name: str, runs: str, tile, mode: int):
+    """``tile`` (the attribute ``name``) as (h, w), or None.  ``runs`` (the tiled forward, the windowed backward) runs
+    on the tensor cores only."""
     if tile is None:
         return None
     if mode == _lib.MODE_FP32_SIMT:
-        raise ValueError("tile: the tiled forward runs on the tensor cores only, and precision='fp32' is the CUDA-core "
-                         "mode; use precision='default' or 'bf16x3', or tile=None")
+        raise ValueError(f"{name}: {runs} runs on the tensor cores only, and precision='fp32' is the CUDA-core mode; "
+                         f"use precision='default' or 'bf16x3', or {name}=None")
     return Engine._tile_hw(tile)
-
-
-def _checked_grad_tile(grad_tile, mode: int):
-    """``grad_tile`` as (h, w), or None for the untiled training path.  The windowed backward is tensor-core only."""
-    if grad_tile is None:
-        return None
-    if mode == _lib.MODE_FP32_SIMT:
-        raise ValueError("grad_tile: the windowed backward runs on the tensor cores only, and precision='fp32' is the "
-                         "CUDA-core mode; use precision='default' or 'bf16x3', or grad_tile=None")
-    return Engine._tile_hw(grad_tile)
 
 
 def _param_version(p) -> int:
@@ -75,6 +61,11 @@ def _param_version(p) -> int:
         return p._version
     except RuntimeError:  # tensors created under torch.inference_mode() do not track versions
         return -1
+
+
+def _needs_graph(tensors, params) -> bool:
+    """Whether a call records an autograd graph: grad mode is on and an input or a parameter requires grad."""
+    return torch.is_grad_enabled() and (any(t.requires_grad for t in tensors) or any(p.requires_grad for p in params))
 
 
 class _PackedWeightsMixin:
@@ -103,25 +94,142 @@ class _PackedWeightsMixin:
         self.invalidate_packed_weights()
         return out
 
-    def _engine_for(self, x, params, key_params=None):
-        """This module's private engine on x's device with ``params`` (34 tensors, state-dict order) packed.  The
-        cache key is taken over ``key_params`` when given (a free-standing stack: its own parameters, not the zeros
-        that fill the other slots)."""
-        if not x.is_cuda:
+    def _device_engine(self, device) -> Engine:
+        """This module's private engine on the CUDA ``device``, created on first use."""
+        with _model_engines_lock:
+            per_dev = _model_engines.setdefault(self, {})
+            eng = per_dev.get(device.index)
+            if eng is None:
+                eng = per_dev[device.index] = new_engine(device)
+        return eng
+
+    def _pack_key(self, params) -> tuple:
+        """The packed-weight cache key of ``params``: the epoch, then data_ptr and _version of every tensor."""
+        return (getattr(self, "_pack_epoch", 0),) + tuple((p.data_ptr(), _param_version(p)) for p in params)
+
+    def _engine_for(self, device, params, key_params=None):
+        """This module's private engine on ``device`` (that of the inputs) with ``params`` (34 tensors, state-dict
+        order) packed.  The cache key is taken over ``key_params`` when given (a free-standing stack: its own
+        parameters, not the zeros that fill the other slots)."""
+        if device.type != "cuda":
             raise _lib.WaterNetLibraryError(
                 f"{type(self).__name__}.forward got CPU tensors: waternet_b200 has no CPU path; move the model and "
                 "inputs to a CUDA device (H100)")
-        if params[0].device != x.device:
-            raise RuntimeError(f"model parameters on {params[0].device}, inputs on {x.device}")
-        with _model_engines_lock:
-            per_dev = _model_engines.setdefault(self, {})
-            eng = per_dev.get(x.device.index)
-            if eng is None:
-                eng = per_dev[x.device.index] = new_engine(x.device)
-        key = (getattr(self, "_pack_epoch", 0),) + tuple((p.data_ptr(), _param_version(p))
-                                                         for p in (params if key_params is None else key_params))
-        eng.pack_weights(params, key=key)
+        if params[0].device != device:
+            raise RuntimeError(f"model parameters on {params[0].device}, inputs on {device}")
+        eng = self._device_engine(device)
+        eng.pack_weights(params, key=self._pack_key(params if key_params is None else key_params))
         return eng
+
+
+class _NetModule(_PackedWeightsMixin, nn.Module):
+    """What ``WaterNet`` and its stacks share: the settings of a call, each validated where it is read, from the
+    module's owner (``_owner``: a stack bound to a ``WaterNet`` follows the parent's settings)."""
+
+    def _owner(self):
+        return self
+
+    def _mode(self) -> int:
+        precision = self._owner().precision
+        if precision not in MODES:
+            raise ValueError(f"unknown precision {precision!r}; choose from {sorted(MODES)}")
+        return MODES[precision]
+
+    def _train_mode(self) -> int:
+        """The training arithmetic (wn_set_train_mode) of a call that records an autograd graph."""
+        train_precision = self._owner().train_precision
+        if train_precision not in TRAIN_PRECISIONS:
+            raise ValueError(f"unknown train_precision {train_precision!r}; choose from {sorted(TRAIN_PRECISIONS)}")
+        return TRAIN_PRECISIONS[train_precision]
+
+    def _tile(self):
+        """The window tile of a call without an autograd graph, as (h, w), or None.  Refused with precision "fp32"."""
+        return _checked_tile("tile", "the tiled forward", self._owner().tile, self._mode())
+
+    def _grad_tile(self):
+        """The windowed-backward tile of a call that records an autograd graph, as (h, w), or None.  Refused with
+        precision "fp32"."""
+        return _checked_tile("grad_tile", "the windowed backward", self._owner().grad_tile, self._mode())
+
+
+class _Training(NamedTuple):
+    """How one kind of call trains on the library: the ``Engine`` methods of its training forward, backward, windowed
+    forward and windowed backward; the arguments before the tensors (a refiner's ``which``); and how its flat inputs
+    map onto those methods."""
+    train: str
+    backward: str
+    tiled: str
+    backward_tiled: str
+    lead: tuple = ()
+    items: bool = False    # the inputs are items of four tensors, one output per item (forward_many)
+    ask_all: bool = False  # the library is asked for all input gradients when any is needed (wn_backward*)
+    owner: str = "model"   # whose parameters a changed weights key reports
+
+    def group(self, flat):
+        """The inputs (or their needs) of a call as its methods take them: a list of items of four, or a tuple."""
+        return [flat[i:i + 4] for i in range(0, len(flat), 4)] if self.items else tuple(flat)
+
+
+_NET_TRAINING = _Training("forward_train", "backward", "forward_tiled", "backward_tiled", ask_all=True)
+_CMG_TRAINING = _Training("confidence_maps_train", "confidence_maps_backward", "confidence_maps_tiled",
+                          "confidence_maps_backward_tiled", owner="sub-module")
+_REFINER_TRAINING = tuple(_Training("refine_train", "refine_backward", "refine_tiled", "refine_backward_tiled",
+                                    lead=(which,), owner="sub-module") for which in range(3))
+_RAGGED_TRAINING = _Training("forward_train_ragged", "backward_ragged", "forward_ragged", "backward_ragged_tiled",
+                             items=True)
+
+
+class _NativeTraining(torch.autograd.Function):
+    """A call that records an autograd graph, on the library's training calls of ``kind`` (a ``_Training``).  It
+    receives the call's inputs, then the parameters it trains, so autograd routes gradients to them and to nothing
+    else.  Without ``grad_tile`` the forward keeps its activations until backward (wn_forward_train,
+    wn_confidence_maps_train, ...).  With ``grad_tile`` it keeps nothing but the inputs: the forward is the windowed
+    forward in the bf16x3 arithmetic of training, and the backward recomputes the activations window by window; both
+    hold at most one pass of TRAIN_PASS_PIXELS window pixels.  train_mode (wn_set_train_mode) is kept for the backward,
+    so that it runs under the forward's mode whatever another module trains on the same engine in between."""
+
+    @staticmethod
+    def forward(ctx, kind, eng, grad_tile, train_mode, n_in, *tensors):
+        ins, params = tensors[:n_in], tensors[n_in:]
+        ctx.kind, ctx.engine, ctx.grad_tile, ctx.train_mode, ctx.n_in = kind, eng, grad_tile, train_mode, n_in
+        ctx.weights_key = eng._weights_key
+        ctx.shapes = [p.shape for p in params]
+        args = (kind.group(ins),) if kind.items else ins
+        if grad_tile is not None:
+            ctx.save_for_backward(*ins)
+            out = getattr(eng, kind.tiled)(*kind.lead, *args, grad_tile, _lib.MODE_BF16X3,
+                                           max_pass_pixels=TRAIN_PASS_PIXELS)
+        else:
+            out, ctx.saved_ws = getattr(eng, kind.train)(*kind.lead, *args, train_mode=train_mode)
+        return tuple(out) if kind.items else out
+
+    @staticmethod
+    def backward(ctx, *grad_outs):
+        kind, eng = ctx.kind, ctx.engine
+        if eng._weights_key != ctx.weights_key:
+            raise RuntimeError(f"{kind.owner} parameters were modified between forward and backward")
+        need_in, need_par = ctx.needs_input_grad[5:5 + ctx.n_in], ctx.needs_input_grad[5 + ctx.n_in:]
+        grad = grad_outs if kind.items else grad_outs[0]
+        want = any(need_in) if kind.ask_all else kind.group(need_in)
+        if ctx.grad_tile is not None:
+            res = getattr(eng, kind.backward_tiled)(*kind.lead, grad, kind.group(ctx.saved_tensors), ctx.shapes,
+                                                    ctx.grad_tile, want, max_pass_pixels=TRAIN_PASS_PIXELS,
+                                                    train_mode=ctx.train_mode)
+        else:
+            res = getattr(eng, kind.backward)(*kind.lead, grad, ctx.saved_ws, ctx.shapes, want,
+                                              train_mode=ctx.train_mode)
+            ctx.saved_ws = None
+        grads, gin = (res, [None] * ctx.n_in) if kind.ask_all and not want else res
+        if kind.items:
+            gin = [t for row in gin for t in row]
+        return (None,) * 5 + tuple(g if need else None for g, need in zip(gin, need_in)) + \
+            tuple(g if need else None for g, need in zip(grads, need_par))
+
+
+class _SubmoduleForward(_NativeTraining):
+    """``_NativeTraining`` of a sub-module called on its own, under a name of its own in the autograd graph
+    (``grad_fn``), so that a sub-module's native node can be told from the whole network's."""
+
 
 # (in, out, kernel) of the confidence-map stack (reference net.py:12-42) and of a refiner (net.py:62-70)
 CMG_SPEC = [(12, 128, 7), (128, 128, 5), (128, 128, 3), (128, 64, 1), (64, 64, 7), (64, 64, 5), (64, 64, 3), (64, 3, 3)]
@@ -132,7 +240,7 @@ def _same_conv(cin: int, cout: int, k: int) -> nn.Conv2d:
     return nn.Conv2d(cin, cout, kernel_size=k, stride=1, dilation=1, padding=k // 2)
 
 
-class _ConvStack(_PackedWeightsMixin, nn.Module):
+class _ConvStack(_NetModule):
     """conv1..convK attributes (the names the reference's state dict uses).
 
     Like the reference's sub-modules (``net.py:45-56``, ``:75-80``) a stack can be called on its own.  Inside a
@@ -194,116 +302,39 @@ class _ConvStack(_PackedWeightsMixin, nn.Module):
         finally:
             self.__dict__["_parent_ref"] = ref
 
-    def _mode_and_engine(self, x, zero_layout):
-        """(mode, engine with the right state dict packed, slot, tile or None).  zero_layout(own) -> the 34-tensor
-        list of a free-standing stack."""
+    def _owner(self):
+        """The parent WaterNet of a bound stack, whose settings it follows, else the stack itself."""
         parent = self._parent_ref() if self._parent_ref is not None else None
-        if parent is not None:
-            mode = parent._mode()
-            return mode, parent._engine_with_weights(x), self._slot, _checked_tile(parent.tile, mode)
-        if self.precision not in MODES:
-            raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(MODES)}")
-        mode = MODES[self.precision]
-        tile = _checked_tile(self.tile, mode)
+        return self if parent is None else parent
+
+    def _engine_and_slot(self, x):
+        """(engine with the right state dict packed, slot) for a call on x: the parent's engine and this stack's slot
+        for a bound stack, else its own engine with its parameters in slot 0 of its kind and zeros elsewhere."""
+        owner = self._owner()
+        if owner is not self:
+            return owner._engine_with_weights(x), self._slot
         own = self._own_params()
-        return mode, self._engine_for(x, zero_layout(own), key_params=own), 0, tile
+        return self._engine_for(x.device, self._zero_layout(own), key_params=own), 0
 
     def _train_engine(self, x, any_size=False):
-        """(engine with the right state dict packed, slot) for a call that records an autograd graph, or None where
-        the torch graph runs instead: CPU tensors, precision "fp32", or one image over Engine.TRAIN_MAX_PIXELS (unless
-        ``any_size``: the windowed path)."""
-        if not x.is_cuda or (not any_size and x.shape[2] * x.shape[3] > Engine.TRAIN_MAX_PIXELS):
+        """(engine with the right state dict packed, slot) for a call on x that records an autograd graph, or None
+        where the torch graph runs instead: CPU tensors, precision "fp32", or one image over Engine.TRAIN_MAX_PIXELS
+        (unless ``any_size``: the windowed path of ``grad_tile``)."""
+        if (not x.is_cuda or (not any_size and x.shape[2] * x.shape[3] > Engine.TRAIN_MAX_PIXELS)
+                or self._mode() == _lib.MODE_FP32_SIMT):
             return None
-        parent = self._parent_ref() if self._parent_ref is not None else None
-        if parent is not None:
-            if parent._mode() == _lib.MODE_FP32_SIMT:
-                return None
-            return parent._engine_with_weights(x), self._slot
-        if self.precision not in MODES:
-            raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(MODES)}")
-        if MODES[self.precision] == _lib.MODE_FP32_SIMT:
-            return None
-        own = self._own_params()
-        return self._engine_for(x, self._zero_layout(own), key_params=own), 0
+        return self._engine_and_slot(x)
 
-    def _grad_tile(self):
-        """The windowed-backward tile of a call that records an autograd graph, as (h, w), or None: the parent's
-        ``grad_tile`` for a bound stack, else its own.  Refused with precision "fp32"."""
-        parent = self._parent_ref() if self._parent_ref is not None else None
-        if parent is not None:
-            return _checked_grad_tile(parent.grad_tile, parent._mode())
-        if self.precision not in MODES:
-            raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(MODES)}")
-        return _checked_grad_tile(self.grad_tile, MODES[self.precision])
-
-    def _train_mode(self) -> int:
-        """The training arithmetic (wn_set_train_mode) of a call that records an autograd graph: the parent's
-        ``train_precision`` for a bound stack, else its own."""
-        parent = self._parent_ref() if self._parent_ref is not None else None
-        return parent._train_mode() if parent is not None else _checked_train_mode(self.train_precision)
-
-    def _train_call(self, x):
-        """(engine with the right state dict packed, slot, grad_tile or None, training mode) for a call that records
-        an autograd graph, or None where the torch graph runs instead.  With grad_tile any image size runs natively."""
+    def _trained(self, ins):
+        """The stack on ``ins`` recording an autograd graph: natively where ``_train_engine`` allows, else the torch
+        graph."""
         grad_tile = self._grad_tile()
-        native = self._train_engine(x, any_size=grad_tile is not None)
-        return None if native is None else (*native, grad_tile, self._train_mode())
-
-    @staticmethod
-    def _needs_graph(tensors, params):
-        return torch.is_grad_enabled() and (any(t.requires_grad for t in tensors) or any(p.requires_grad for p in params))
-
-
-class _SubmoduleForward(torch.autograd.Function):
-    """A sub-module called on its own under autograd: forward values and gradients from the CUDA library
-    (wn_confidence_maps_train / _backward for the cmg, wn_refine_train / _backward for a refiner), in the bf16x3
-    arithmetic of training.  It receives the stack's own 16 or 6 parameters, so autograd routes gradients to them and
-    to nothing else.  which: None for the cmg, else the refiner slot (0 wb, 1 ce, 2 gc) of the packed state dict.
-    With ``grad_tile`` the forward keeps nothing but the inputs (wn_confidence_maps_tiled / wn_refine_tiled in the
-    bf16x3 arithmetic of training) and the backward recomputes the stack's activations window by window
-    (wn_confidence_maps_backward_tiled / wn_refine_backward_tiled); both hold at most one pass of TRAIN_PASS_PIXELS
-    window pixels.  train_mode (wn_set_train_mode) is kept for the backward, so that it runs under the forward's mode
-    whatever another module trains on the same engine in between."""
-
-    @staticmethod
-    def forward(ctx, eng, which, grad_tile, train_mode, n_in, *tensors):
-        ins, params = tensors[:n_in], tensors[n_in:]
-        ctx.engine, ctx.which, ctx.n_in, ctx.grad_tile, ctx.train_mode = eng, which, n_in, grad_tile, train_mode
-        ctx.weights_key = eng._weights_key
-        ctx.shapes = [p.shape for p in params]
-        if grad_tile is not None:
-            ctx.save_for_backward(*ins)
-            if which is None:
-                return eng.confidence_maps_tiled(*ins, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS)
-            return eng.refine_tiled(which, *ins, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS)
-        if which is None:
-            out, ctx.saved_ws = eng.confidence_maps_train(*ins, train_mode=train_mode)
-        else:
-            out, ctx.saved_ws = eng.refine_train(which, *ins, train_mode=train_mode)
-        return out
-
-    @staticmethod
-    def backward(ctx, grad):
-        eng = ctx.engine
-        if eng._weights_key != ctx.weights_key:
-            raise RuntimeError("sub-module parameters were modified between forward and backward")
-        need = ctx.needs_input_grad[5:]
-        want_in, want_par = need[:ctx.n_in], need[ctx.n_in:]
-        tm = ctx.train_mode
-        if ctx.grad_tile is not None:
-            ins = ctx.saved_tensors
-            if ctx.which is None:
-                grads, gin = eng.confidence_maps_backward_tiled(grad, ins, ctx.shapes, ctx.grad_tile, want_in,
-                                                                max_pass_pixels=TRAIN_PASS_PIXELS, train_mode=tm)
-            else:
-                grads, gin = eng.refine_backward_tiled(ctx.which, grad, ins, ctx.shapes, ctx.grad_tile, want_in,
-                                                       max_pass_pixels=TRAIN_PASS_PIXELS, train_mode=tm)
-        elif ctx.which is None:
-            grads, gin = eng.confidence_maps_backward(grad, ctx.saved_ws, ctx.shapes, want_in, train_mode=tm)
-        else:
-            grads, gin = eng.refine_backward(ctx.which, grad, ctx.saved_ws, ctx.shapes, want_in, train_mode=tm)
-        ctx.saved_ws = None
-        return (None, None, None, None, None, *gin, *[g if w else None for g, w in zip(grads, want_par)])
+        native = self._train_engine(ins[0], any_size=grad_tile is not None)
+        if native is None:
+            return self._graph(*ins)
+        eng, slot = native
+        return _SubmoduleForward.apply(self._training[slot], eng, grad_tile, self._train_mode(), len(ins), *ins,
+                                       *self._own_params())
 
 
 def _zeros_like_spec(spec, ref):
@@ -318,6 +349,7 @@ class ConfidenceMapGenerator(_ConvStack):
     """Eight convs, ReLU after the first seven, sigmoid after the last (net.py:7-56)."""
 
     spec = CMG_SPEC
+    _training = (_CMG_TRAINING,)
 
     def _graph(self, x, wb, ce, gc):
         out = torch.cat([x, wb, ce, gc], dim=1)
@@ -332,19 +364,13 @@ class ConfidenceMapGenerator(_ConvStack):
 
     def forward(self, x, wb, ce, gc):
         """Returns the three (N,1,H,W) maps ``out1, out2, out3`` like ``net.py:55-56``."""
-        if self._needs_graph((x, wb, ce, gc), self._own_params()):
-            native = self._train_call(x)
-            if native is None:
-                maps = self._graph(x, wb, ce, gc)
-            else:
-                eng, _, grad_tile, train_mode = native
-                maps = _SubmoduleForward.apply(eng, None, grad_tile, train_mode, 4, x, wb, ce, gc, *self._own_params())
+        ins = (x, wb, ce, gc)
+        if _needs_graph(ins, self._own_params()):
+            maps = self._trained(ins)
         else:
-            mode, eng, _, tile = self._mode_and_engine(x, self._zero_layout)
-            if tile is None:
-                maps = eng.confidence_maps(x, wb, ce, gc, mode)
-            else:
-                maps = eng.confidence_maps_tiled(x, wb, ce, gc, tile, mode)
+            mode, tile = self._mode(), self._tile()
+            eng, _ = self._engine_and_slot(x)
+            maps = eng.confidence_maps(*ins, mode) if tile is None else eng.confidence_maps_tiled(*ins, tile, mode)
         return torch.split(maps, [1, 1, 1], dim=1)
 
 
@@ -352,6 +378,7 @@ class Refiner(_ConvStack):
     """Three conv+ReLU on cat[x, x_bar] (net.py:59-80); the last ReLU is part of it."""
 
     spec = REFINER_SPEC
+    _training = _REFINER_TRAINING  # by slot (0 wb, 1 ce, 2 gc)
 
     def _graph(self, x, xbar):
         out = torch.cat([x, xbar], dim=1)
@@ -364,128 +391,38 @@ class Refiner(_ConvStack):
         return _zeros_like_spec(CMG_SPEC, own[0]) + own + 2 * _zeros_like_spec(REFINER_SPEC, own[0])
 
     def forward(self, x, xbar):
-        if self._needs_graph((x, xbar), self._own_params()):
-            native = self._train_call(x)
-            if native is None:
-                return self._graph(x, xbar)
-            eng, slot, grad_tile, train_mode = native
-            return _SubmoduleForward.apply(eng, slot, grad_tile, train_mode, 2, x, xbar, *self._own_params())
-        mode, eng, slot, tile = self._mode_and_engine(x, self._zero_layout)
-        if tile is None:
-            return eng.refine(slot, x, xbar, mode)
-        return eng.refine_tiled(slot, x, xbar, tile, mode)
+        if _needs_graph((x, xbar), self._own_params()):
+            return self._trained((x, xbar))
+        mode, tile = self._mode(), self._tile()
+        eng, slot = self._engine_and_slot(x)
+        return eng.refine(slot, x, xbar, mode) if tile is None else eng.refine_tiled(slot, x, xbar, tile, mode)
 
 
-class _KernelForward(torch.autograd.Function):
-    """Forward values and all gradients (34 parameters, and the four input images when they require
-    grad) from the CUDA library (wn_forward_train / wn_backward).  Only the fp32 CUDA-core mode obtains
-    its gradients by re-evaluating the torch graph.  With ``grad_tile`` the forward keeps nothing but the four
-    inputs (wn_forward_tiled in the bf16x3 arithmetic of training) and the backward recomputes the activations
-    window by window (wn_backward_tiled); both hold at most one pass of TRAIN_PASS_PIXELS window pixels.  The native
-    calls run in the model's ``train_precision``, kept in ctx for the backward.
-    """
+class _GraphBackward(torch.autograd.Function):
+    """``WaterNet`` in precision "fp32" under autograd: the forward on the fp32 CUDA-core kernels, the gradients (34
+    parameters and the inputs that require grad) by re-evaluating the torch graph (``model._graph``)."""
 
     @staticmethod
-    def forward(ctx, model, mode, grad_tile, x, wb, ce, gc, *params):
+    def forward(ctx, model, x, wb, ce, gc, *params):
         ctx.model = model
-        ctx.native = mode != _lib.MODE_FP32_SIMT
-        ctx.grad_tile = grad_tile
-        ctx.train_mode = model._train_mode() if ctx.native else None
-        ctx.input_needs_grad = [t.requires_grad for t in (x, wb, ce, gc)]
-        if grad_tile is not None:
-            eng = model._engine_with_weights(x)
-            ctx.engine, ctx.weights_key = eng, eng._weights_key
-            ctx.save_for_backward(x, wb, ce, gc)
-            return eng.forward_tiled(x, wb, ce, gc, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS)
-        if ctx.native:
-            eng = model._engine_with_weights(x)
-            out, ws = eng.forward_train(x, wb, ce, gc, train_mode=ctx.train_mode)
-            ctx.engine, ctx.saved_ws = eng, ws
-            ctx.weights_key = eng._weights_key
-            return out
         ctx.save_for_backward(x, wb, ce, gc)
-        return model._kernel_forward(x, wb, ce, gc, mode)
+        return model._engine_with_weights(x).forward(x, wb, ce, gc, _lib.MODE_FP32_SIMT)
 
     @staticmethod
     def backward(ctx, grad_out):
-        model = ctx.model
-        params = list(model.parameters())
-        if ctx.native:
-            eng = ctx.engine
-            if eng._weights_key != ctx.weights_key:  # parameters changed between forward and backward
-                raise RuntimeError("model parameters were modified between forward and backward")
-            want_in = any(ctx.input_needs_grad)
-            shapes = [p.shape for p in params]
-            if ctx.grad_tile is not None:
-                res = eng.backward_tiled(grad_out, ctx.saved_tensors, shapes, ctx.grad_tile, want_input_grads=want_in,
-                                         max_pass_pixels=TRAIN_PASS_PIXELS, train_mode=ctx.train_mode)
-            else:
-                res = eng.backward(grad_out, ctx.saved_ws, shapes, want_input_grads=want_in, train_mode=ctx.train_mode)
-                ctx.saved_ws = None
-            grads, gin = res if want_in else (res, [None] * 4)
-            gpar = [g if p.requires_grad else None for g, p in zip(grads, params)]
-            gin = [g if need else None for g, need in zip(gin, ctx.input_needs_grad)]
-            return (None, None, None, *gin, *gpar)
-        x, wb, ce, gc = ctx.saved_tensors
+        params = list(ctx.model.parameters())
         with torch.enable_grad():
-            ins = [t.detach().requires_grad_(t.requires_grad) for t in (x, wb, ce, gc)]
-            out = model._graph(*ins)
+            ins = [t.detach().requires_grad_(t.requires_grad) for t in ctx.saved_tensors]
+            out = ctx.model._graph(*ins)
             wanted = [t for t in ins if t.requires_grad] + [p for p in params if p.requires_grad]
             grads = torch.autograd.grad(out, wanted, grad_out, allow_unused=True)
         it = iter(grads)
         gin = [next(it) if t.requires_grad else None for t in ins]
         gpar = [next(it) if p.requires_grad else None for p in params]
-        return (None, None, None, *gin, *gpar)
+        return (None, *gin, *gpar)
 
 
-class _RaggedKernelForward(torch.autograd.Function):
-    """``WaterNet.forward_many`` under autograd: the images of their own sizes through the ragged training step
-    (wn_forward_train_ragged / wn_backward_ragged, the bf16x3 arithmetic of training).  Receives the four inputs of
-    every item, flattened, then the 34 parameters; returns one output per item.  With ``grad_tile`` the forward keeps
-    nothing but the inputs (wn_forward_ragged in the bf16x3 arithmetic of training) and the backward recomputes the
-    activations window by window (wn_backward_ragged_tiled); both hold at most one pass of TRAIN_PASS_PIXELS slot
-    pixels."""
-
-    @staticmethod
-    def forward(ctx, model, grad_tile, n_items, *tensors):
-        flat, params = tensors[:4 * n_items], tensors[4 * n_items:]
-        items = [flat[4 * i:4 * i + 4] for i in range(n_items)]
-        eng = model._engine_with_weights(items[0][0])
-        ctx.engine, ctx.weights_key, ctx.n_items, ctx.grad_tile = eng, eng._weights_key, n_items, grad_tile
-        ctx.train_mode = model._train_mode()
-        ctx.shapes = [p.shape for p in params]
-        if grad_tile is not None:
-            # refuse here what the backward would refuse (a window over the pixels of one training pass)
-            sizes = [tuple(x.shape[2:]) for x, *_ in items for _ in range(x.shape[0]) if x.shape[2] * x.shape[3]]
-            if sizes and eng.backward_ragged_tiled_workspace_bytes(sizes, grad_tile, TRAIN_PASS_PIXELS) == 0:
-                raise _lib.WaterNetLibraryError(
-                    f"forward_many: wn_backward_ragged_tiled rejects these images at grad_tile={grad_tile} (a window "
-                    f"may have at most {Engine.TRAIN_MAX_PIXELS >> 20} Mi pixels); use a smaller grad_tile")
-            ctx.save_for_backward(*flat)
-            return tuple(eng.forward_ragged(items, grad_tile, _lib.MODE_BF16X3, max_pass_pixels=TRAIN_PASS_PIXELS))
-        outs, ctx.saved_calls = eng.forward_train_ragged(items, train_mode=ctx.train_mode)
-        return tuple(outs)
-
-    @staticmethod
-    def backward(ctx, *grad_outs):
-        eng = ctx.engine
-        if eng._weights_key != ctx.weights_key:  # parameters changed between forward and backward
-            raise RuntimeError("model parameters were modified between forward and backward")
-        need = ctx.needs_input_grad[3:]
-        want_in = [need[4 * i:4 * i + 4] for i in range(ctx.n_items)]
-        if ctx.grad_tile is not None:
-            flat = ctx.saved_tensors
-            items = [flat[4 * i:4 * i + 4] for i in range(ctx.n_items)]
-            grads, gin = eng.backward_ragged_tiled(grad_outs, items, ctx.shapes, ctx.grad_tile, want_in,
-                                                   max_pass_pixels=TRAIN_PASS_PIXELS, train_mode=ctx.train_mode)
-        else:
-            grads, gin = eng.backward_ragged(grad_outs, ctx.saved_calls, ctx.shapes, want_in, train_mode=ctx.train_mode)
-            ctx.saved_calls = None
-        gpar = [g if w else None for g, w in zip(grads, need[4 * ctx.n_items:])]
-        return (None, None, None, *[t for row in gin for t in row], *gpar)
-
-
-class WaterNet(_PackedWeightsMixin, nn.Module):
+class WaterNet(_NetModule):
     """
     Gated fusion network (reference ``net.py:83-108``)::
 
@@ -524,19 +461,19 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
 
     def __init__(self, precision: str = "default", tile=None, grad_tile=None, train_precision: str = "bf16x3"):
         super().__init__()
-        _checked_train_mode(train_precision)
-        self.cmg = ConfidenceMapGenerator()
-        self.wb_refiner = Refiner()
-        self.ce_refiner = Refiner()
-        self.gc_refiner = Refiner()
         self.precision = precision
         self.tile = tile
         self.grad_tile = grad_tile
         self.train_precision = train_precision
+        self._train_mode()
         if tile is not None:
-            _checked_tile(tile, self._mode())
+            self._tile()
         if grad_tile is not None:
-            _checked_grad_tile(grad_tile, self._mode())
+            self._grad_tile()
+        self.cmg = ConfidenceMapGenerator()
+        self.wb_refiner = Refiner()
+        self.ce_refiner = Refiner()
+        self.gc_refiner = Refiner()
         self._bind_children()
 
     def _bind_children(self) -> None:
@@ -554,14 +491,6 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
         return new
 
     # -- plumbing -----------------------------------------------------------------
-    def _mode(self) -> int:
-        if self.precision not in MODES:
-            raise ValueError(f"unknown precision {self.precision!r}; choose from {sorted(MODES)}")
-        return MODES[self.precision]
-
-    def _train_mode(self) -> int:
-        return _checked_train_mode(self.train_precision)
-
     def _ordered_params(self):
         """The 34 tensors in state-dict order (what wn_pack_weights expects)."""
         out = []
@@ -572,25 +501,15 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
 
     def _engine_with_weights(self, x):
         """This model's private engine on x's device, its current parameters packed (no-op when unchanged)."""
-        return self._engine_for(x, self._ordered_params())
+        return self._engine_for(x.device, self._ordered_params())
 
     def engine(self):
         """The private engine on the device the parameters live on, current parameters packed."""
-        class _On:  # what _engine_for looks at
-            pass
-        on = _On()
-        on.device = self.cmg.conv1.weight.device
-        on.is_cuda = on.device.type == "cuda"
-        if on.is_cuda and on.device.index is None:
-            on.device = torch.device("cuda", torch.cuda.current_device())
-        return self._engine_for(on, self._ordered_params())
+        return self._engine_for(self.cmg.conv1.weight.device, self._ordered_params())
 
     def __setstate__(self, state):
         super().__setstate__(state)
         self._bind_children()
-
-    def _kernel_forward(self, x, wb, ce, gc, mode):
-        return self._engine_with_weights(x).forward(x, wb, ce, gc, mode)
 
     def _graph(self, x, wb, ce, gc):
         """Differentiable torch-op evaluation, used only to obtain gradients."""
@@ -603,17 +522,20 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
     # -- reference signature: forward(x, wb, ce, gc), ce == histogram-equalised image ---
     def forward(self, x, wb, ce, gc):
         mode = self._mode()
+        ins = (x, wb, ce, gc)
         if x.numel() == 0 and x.is_cuda:  # empty batch: nothing to launch (torch's convs return empty too)
-            return self._engine_with_weights(x).forward(x, wb, ce, gc, mode)
-        needs_graph = torch.is_grad_enabled() and (
-            any(t.requires_grad for t in (x, wb, ce, gc)) or any(p.requires_grad for p in self.parameters()))
-        if needs_graph:  # tile does not apply: training keeps every activation of whole images, unless grad_tile
-            grad_tile = _checked_grad_tile(self.grad_tile, mode)
-            return _KernelForward.apply(self, mode, grad_tile, x, wb, ce, gc, *self.parameters())
-        tile = _checked_tile(self.tile, mode)
-        if tile is not None:
-            return self._engine_with_weights(x).forward_tiled(x, wb, ce, gc, tile, mode)
-        return self._kernel_forward(x, wb, ce, gc, mode)
+            return self._engine_with_weights(x).forward(*ins, mode)
+        # tile does not apply to training: it keeps every activation of whole images, unless grad_tile
+        if _needs_graph(ins, self.parameters()):
+            grad_tile = self._grad_tile()
+            if mode == _lib.MODE_FP32_SIMT:
+                return _GraphBackward.apply(self, *ins, *self.parameters())
+            train_mode = self._train_mode()
+            return _NativeTraining.apply(_NET_TRAINING, self._engine_with_weights(x), grad_tile, train_mode, 4, *ins,
+                                         *self.parameters())
+        tile = self._tile()
+        eng = self._engine_with_weights(x)
+        return eng.forward(*ins, mode) if tile is None else eng.forward_tiled(*ins, tile, mode)
 
     def forward_many(self, xs, wbs, ces, gcs) -> list:
         """``forward`` of images of their own sizes: four equally long lists of (N_i,3,H_i,W_i) tensors -> the list of
@@ -647,13 +569,19 @@ class WaterNet(_PackedWeightsMixin, nn.Module):
             return []
         x0 = items[0][0]
         if not x0.is_cuda:
-            self._engine_for(x0, None)  # raises: there is no CPU path
-        params = list(self.parameters())
-        needs_graph = torch.is_grad_enabled() and (
-            any(t.requires_grad for it in items for t in it) or any(p.requires_grad for p in params))
-        if needs_graph:
-            grad_tile = _checked_grad_tile(self.grad_tile, mode)
-            return list(_RaggedKernelForward.apply(self, grad_tile, len(items), *[t for it in items for t in it],
-                                                   *params))
-        tile = _checked_tile(self.tile, mode) or Engine.DEFAULT_TILE
+            self._engine_for(x0.device, None)  # raises: there is no CPU path
+        flat = [t for it in items for t in it]
+        if _needs_graph(flat, self.parameters()):
+            grad_tile = self._grad_tile()
+            eng = self._engine_with_weights(x0)
+            train_mode = self._train_mode()
+            if grad_tile is not None:  # refuse here what the backward would refuse (a window over one training pass)
+                sizes = [tuple(x.shape[2:]) for x, *_ in items for _ in range(x.shape[0]) if x.shape[2] * x.shape[3]]
+                if sizes and eng.backward_ragged_tiled_workspace_bytes(sizes, grad_tile, TRAIN_PASS_PIXELS) == 0:
+                    raise _lib.WaterNetLibraryError(
+                        f"forward_many: wn_backward_ragged_tiled rejects these images at grad_tile={grad_tile} (a "
+                        f"window may have at most {Engine.TRAIN_MAX_PIXELS >> 20} Mi pixels); use a smaller grad_tile")
+            return list(_NativeTraining.apply(_RAGGED_TRAINING, eng, grad_tile, train_mode, len(flat), *flat,
+                                              *self.parameters()))
+        tile = self._tile() or Engine.DEFAULT_TILE
         return self._engine_with_weights(x0).forward_ragged(items, tile, mode)

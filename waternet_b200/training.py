@@ -18,9 +18,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from .engine import new_engine
 from .metrics import psnr, ssim
-from .net import TRAIN_PRECISIONS, _model_engines, _model_engines_lock, _PackedWeightsMixin, _param_version
+from .net import TRAIN_PRECISIONS, _PackedWeightsMixin
 
 TRAIN_METRICS_NAMES = ["mse", "ssim", "psnr", "perceptual_loss", "loss"]
 VAL_METRICS_NAMES = ["mse", "ssim", "psnr", "perceptual_loss"]
@@ -95,13 +94,8 @@ class PerceptualModel(_PackedWeightsMixin, nn.Module):
         params = self.vgg_params()
         if params[0].device != x.device:
             raise RuntimeError(f"VGG parameters on {params[0].device}, inputs on {x.device}")
-        with _model_engines_lock:
-            per_dev = _model_engines.setdefault(self, {})
-            eng = per_dev.get(x.device.index)
-            if eng is None:
-                eng = per_dev[x.device.index] = new_engine(x.device)
-        key = (getattr(self, "_pack_epoch", 0),) + tuple((p.data_ptr(), _param_version(p)) for p in params)
-        eng.pack_vgg_weights(params, key=key)
+        eng = self._device_engine(x.device)
+        eng.pack_vgg_weights(params, key=self._pack_key(params))
         return eng
 
     def native_loss(self, out, ref):
