@@ -114,9 +114,11 @@ def main():
         "slowest_new_beats_fastest_baseline": min(vals[new]) > max(vals[base]),
         "all_outputs_within_tolerance": all(x["outputs_within_tolerance"] for x in info["runs"]),
         "gpu_launches": sorted({x["gpu_launches"] for x in info["runs"]}),
+        # per arm, the slots its runs timed (a launch one build fuses away has no slot there)
         "kernel_ms_per_step_median": {a: {k: statistics.median(x["kernel_ms_per_step"][k] for x in info["runs"]
-                                                               if x["arm"] == a)
-                                          for k in info["runs"][0]["kernel_ms_per_step"]} for a in arms},
+                                                               if x["arm"] == a and k in x["kernel_ms_per_step"])
+                                          for k in dict.fromkeys(k for x in info["runs"] if x["arm"] == a
+                                                                 for k in x["kernel_ms_per_step"])} for a in arms},
     }
     line = json.dumps(info)
     with open(os.path.join(args.out, "ab_wgs.json"), "w") as f:

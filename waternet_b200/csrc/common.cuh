@@ -265,6 +265,8 @@ struct FwdOpts {
   const RaggedWindow* rwin = nullptr;  // ragged pass (device table): image n of the batch is window rwin[n] in its
                                        // slot; every layer masks it, the last launch stores into its own image
   const int* slot_levels = nullptr;    // ragged fp32 pass: slot n holds 8-bit levels only (ConvArgs::slot_levels)
+  bool fuse_c4 = false;        // inference: cmg.conv4 runs in cmg.conv3's epilogue (kFmtFuse1x1); the outputs of
+                               // cmg.conv4 to cmg.conv7 take the buffers a[3] .. a[6]
 };
 int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st[4][4], float* out, int n,
                         int height, int width, const FwdBuffers& b, cudaStream_t stream,

@@ -374,17 +374,33 @@ size_t umma_forward_workspace_bytes(int n, int h, int w) {
 // A layer's fp8 form reads its own weight images, in the [hi | fp8] layout; the single-pass form reads the hi rows of
 // the bf16x3 images.  A pass of a ragged batch (a.rwin) runs the RAG instantiations of the layers that mask (kEpiAct)
 // or store per window (kEpiGate); the confidence maps are per pixel and need neither.
-template <int LI, bool RAG>
+// FUSE (inference, fp8-correction and bf16x3 schemes): layer LI + 1, a 1x1 layer, runs in LI's epilogue (UmmaCfg
+// kFmtFuse1x1) from its bf16x3 weight image; the launch writes LI + 1's output in LI + 1's format, in LI's timing slot.
+template <int LI, bool RAG, bool FUSE = false>
 static int launch_layer_as(wn_handle* h, int scheme, void* in_base, ConvArgs a, cudaStream_t stream) {
   constexpr UmmaLayerSpec s = kSpecs[LI];
   constexpr bool R = RAG && s.epi != kEpiSigmoid;
   const UmmaWeights* u = h->umma;
   constexpr int GW = s.npad / s.ng;  // channels per column group
-  if (scheme == kSchemeBf16)
+  constexpr int FZ = FUSE ? kFmtFuse1x1 : 0;
+  constexpr int OUT_LI = FUSE ? LI + 1 : LI;  // the layer whose output the launch stores
+  if constexpr (FUSE) {
+    constexpr UmmaLayerSpec f = kSpecs[LI + 1];
+    static_assert(f.ks == 1 && f.cinpad == s.npad && f.npad == kFuseNpad && f.concat && f.nblk == 1 && !f.f8 &&
+                  f.epi == kEpiAct && s.epi == kEpiAct, "the fused layer: 1x1, CONCAT, bf16x3 weights, activation");
+    a.wpk1x1 = u->stages[LI + 1];
+    a.bias1x1 = u->bias[LI + 1];
+    if (scheme == kSchemeBf16) {
+      set_error("the fused 1x1 layer runs in the inference schemes only");
+      return WN_E_STATE;
+    }
+  } else if (scheme == kSchemeBf16) {
     return launch_conv<s.ks, s.cinpad, GW, s.epi, s.concat, s.nblk, s.tps, kFmtHi, R, s.mw, s.ng, layer_wgs(LI)>(
         h, s.slot, u->stages[LI], u->bias[LI], in_base, a, stream);
+  }
   if (scheme == 1) {
-    constexpr int FMT = (s.f8 ? kFmtIn8 : 0) | (writes_f8(LI) ? kFmtOut8 : 0) | (pairs_taps(LI) ? kFmtPair8 : 0);
+    constexpr int FMT =
+        (s.f8 ? kFmtIn8 : 0) | (writes_f8(OUT_LI) ? kFmtOut8 : 0) | (pairs_taps(LI) ? kFmtPair8 : 0) | FZ;
     if constexpr ((FMT & kFmtOut8) != 0) a.f8_overflow = u->overflow_dev;
     if constexpr (s.f8) a.f8_scale = u->scale8[LI] + 1;
     if constexpr (pairs_taps(LI)) {
@@ -394,14 +410,20 @@ static int launch_layer_as(wn_handle* h, int scheme, void* in_base, ConvArgs a, 
     return launch_conv<s.ks, s.cinpad, GW, s.epi, (s.f8 ? 0 : s.concat), s.nblk, s.tps, FMT, R, s.mw, s.ng,
                        layer_wgs(LI)>(h, s.slot, s.f8 ? u->stages8[LI] : u->stages[LI], u->bias[LI], in_base, a, stream);
   }
-  return launch_conv<s.ks, s.cinpad, GW, s.epi, s.concat, s.nblk, s.tps, 0, R, s.mw, s.ng, layer_wgs(LI)>(
+  return launch_conv<s.ks, s.cinpad, GW, s.epi, s.concat, s.nblk, s.tps, FZ, R, s.mw, s.ng, layer_wgs(LI)>(
       h, s.slot, u->stages[LI], u->bias[LI], in_base, a, stream);
 }
-template <int LI>
+template <int LI, bool FUSE = false>
 static int launch_layer(wn_handle* h, int scheme, void* in_base, ConvArgs a, cudaStream_t stream) {
-  return a.rwin ? launch_layer_as<LI, true>(h, scheme, in_base, a, stream)
-                : launch_layer_as<LI, false>(h, scheme, in_base, a, stream);
+  return a.rwin ? launch_layer_as<LI, true, FUSE>(h, scheme, in_base, a, stream)
+                : launch_layer_as<LI, false, FUSE>(h, scheme, in_base, a, stream);
 }
+// WN_UMMA_UNFUSED_C4 runs cmg.conv4 as a launch of its own in every forward, for A/B runs against the fused form
+#ifdef WN_UMMA_UNFUSED_C4
+static constexpr bool kFuseC4 = false;
+#else
+static constexpr bool kFuseC4 = true;
+#endif
 
 // bf16 hi/lo planes -> fp32 NCHW (test aid)
 __global__ void decode_planes_kernel(const uint4* __restrict__ src, float* __restrict__ dst, int planes_half, int hw,
@@ -519,25 +541,34 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
     act(b.a[2], 128, nullptr, 0);
     if ((rc = launch_layer<kC2>(h, sc, b.a[1], a, stream))) return rc;
     if (dump(kC2)) return WN_OK;
-    act(b.a[3], 128, nullptr, 0);
-    if ((rc = launch_layer<kC3>(h, sc, b.a[2], a, stream))) return rc;
-    if (dump(kC3)) return WN_OK;
-    act(b.a[4], 64, nullptr, 0);
-    if ((rc = launch_layer<kC4>(h, sc, b.a[3], a, stream))) return rc;
-    if (dump(kC4)) return WN_OK;
-    act(b.a[5], 64, nullptr, 0);
-    if ((rc = launch_layer<kC5>(h, sc, b.a[4], a, stream))) return rc;
+    // cmg.conv4 fused into cmg.conv3's launch: its output must not land in b.a[4], the ping-pong buffer of b.a[2]
+    // that the same launch's halo loads read, so from cmg.conv4 on every output moves one buffer back (b.a[l - 1])
+    const bool fuse = kFuseC4 && o.fuse_c4;
+    auto cmg_out = [&](int l) { return b.a[fuse ? l - 1 : l]; };
+    if (fuse) {  // one launch: cmg.conv3, and cmg.conv4 in its epilogue
+      act(cmg_out(4), 64, nullptr, 0);
+      if ((rc = launch_layer<kC3, true>(h, sc, b.a[2], a, stream))) return rc;
+    } else {
+      act(b.a[3], 128, nullptr, 0);
+      if ((rc = launch_layer<kC3>(h, sc, b.a[2], a, stream))) return rc;
+      if (dump(kC3)) return WN_OK;
+      act(b.a[4], 64, nullptr, 0);
+      if ((rc = launch_layer<kC4>(h, sc, b.a[3], a, stream))) return rc;
+      if (dump(kC4)) return WN_OK;
+    }
+    act(cmg_out(5), 64, nullptr, 0);
+    if ((rc = launch_layer<kC5>(h, sc, cmg_out(4), a, stream))) return rc;
     if (dump(kC5)) return WN_OK;
-    act(b.a[6], 64, nullptr, 0);
-    if ((rc = launch_layer<kC6>(h, sc, b.a[5], a, stream))) return rc;
+    act(cmg_out(6), 64, nullptr, 0);
+    if ((rc = launch_layer<kC6>(h, sc, cmg_out(5), a, stream))) return rc;
     if (dump(kC6)) return WN_OK;
-    act(b.a[7], 64, nullptr, 0);
-    if ((rc = launch_layer<kC7>(h, sc, b.a[6], a, stream))) return rc;
+    act(cmg_out(7), 64, nullptr, 0);
+    if ((rc = launch_layer<kC7>(h, sc, cmg_out(6), a, stream))) return rc;
     if (dump(kC7)) return WN_OK;
     // the confidence maps are fp32: a dump of them is written in place of b.cm
     const bool dump_maps = dbg_layer == kSpecs[kC8].slot;
     a.out_f32 = dump_maps ? dbg_dst : b.cm;
-    if ((rc = launch_layer<kC8>(h, sc, b.a[7], a, stream))) return rc;
+    if ((rc = launch_layer<kC8>(h, sc, cmg_out(7), a, stream))) return rc;
     if (dump_maps) return WN_OK;
   }
   if (!want_ref) return WN_OK;
@@ -633,6 +664,7 @@ static int forward_call(wn_handle* h, const char* what, size_t workspace_bytes, 
   const int64_t none[4][4] = {};
   const float* no_in[4] = {nullptr, nullptr, nullptr, nullptr};
   o.packed = true;
+  o.fuse_c4 = o.scheme != kSchemeBf16;  // nothing reads cmg.conv3's output but cmg.conv4
   for (const RaggedPass& p : passes) {
     geo.set_pass(p);
     FwdBuffers b = carve(fwd_ws, p.count, p.slot_h, p.slot_w);

@@ -125,6 +125,14 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 //        the fp8 MMA, which adds with fewer bits than fp32, adds into it), then 49 bf16 wgmmas a x w_hi; the weights
 //        (ConvArgs::wpk8) are scaled by s_c 2^9 per output column c (a power of two) and the epilogue multiplies
 //        column c by 2^-9 / s_c (ConvArgs::f8_scale[c]).  74 bf16-pass equivalents instead of 98.
+//        bit 4 (kFmtFuse1x1): a 1x1 layer NPAD -> kFuseNpad (cmg.conv4 behind cmg.conv3) runs in the epilogue.  Each
+//        warpgroup computes the layer's activation in the accumulator layout with the fp32 operations of the kEpiAct
+//        epilogue, splits it into bf16 hi / lo and packs the pairs into the A registers of RS wgmmas (an m64nNk16
+//        accumulator fragment's columns [16k, 16k + 16) are the A fragment of K step k); then, per 16-channel chunk,
+//        a_hi x [w_hi | w_lo] and a_lo x w_hi as the 1x1 layer's own CONCAT launch issues them, from its bf16x3 image
+//        (ConvArgs::wpk1x1), which the B producer sends as kFuseStages more weight stages behind each tile's.  The
+//        1x1 layer's output (ConvArgs::bias1x1, dst0, cout, kFmtOut8, f8_overflow) is what the epilogue stores; the
+//        layer's own activation never leaves registers.
 // MW     m64 blocks per warpgroup: 1 = 8 x 16-pixel tile (M = 128), 2 = 16 x 16 (M = 256).  Every weight stage a
 //        CTA streams from L2 then serves twice the pixels.
 // NG     column groups: a CTA computes the NPAD output channels [g * NPAD, (g + 1) * NPAD) of column group g; the
@@ -135,7 +143,10 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 //        warpgroup serves every weight stage to 192 pixels instead of 128 without more accumulators per thread; at
 //        512 threads the register file allows 128 per thread, so the producer warpgroup gives its registers up
 //        (setmaxnreg) and the consumers run at kWgs3ConsumerRegs.
-constexpr int kFmtIn8 = 1, kFmtOut8 = 2, kFmtHi = 4, kFmtPair8 = 8;
+constexpr int kFmtIn8 = 1, kFmtOut8 = 2, kFmtHi = 4, kFmtPair8 = 8, kFmtFuse1x1 = 16;
+// kFmtFuse1x1: output channels of the fused 1x1 layer, and its weight stages per tile (its 16-channel chunks, 4 KB
+// each in the CONCAT layout, UmmaCfg::FUSE_CHUNKS to a stage)
+constexpr int kFuseNpad = 64, kFuseStages = 2;
 constexpr int kWgs3ProducerRegs = 24, kWgs3ConsumerRegs = 160;  // 128 x 24 + 384 x 160 <= 65,536
 template <int KS, int CIN_PAD, int NPAD, int CONCAT = 0, int NBLK = 1, int TPS = 1, int FMT = 0, int MW = 1,
           int NG = 1, int WGS = 2>
@@ -143,6 +154,7 @@ struct UmmaCfg {
   static constexpr bool F8IN = (FMT & kFmtIn8) != 0;
   static constexpr bool HI = (FMT & kFmtHi) != 0;
   static constexpr bool PAIR = (FMT & kFmtPair8) != 0;
+  static constexpr bool FUSE = (FMT & kFmtFuse1x1) != 0;
   static constexpr bool DUAL = CONCAT != 0 && !HI;  // two accumulator halves per block: [a x w_hi | a_hi x w_lo]
   static constexpr int TILE_W = 8 * MW, TILE_H = 8 * WGS;
   static constexpr int CONSUMER_WARPS = 4 * WGS;                  // arrivals per "stage empty"
@@ -161,7 +173,8 @@ struct UmmaCfg {
   static constexpr int STAGING = WGS * 64 * kStageLd * 4;
   // barriers (512 B) + the biases of every column group: 2048 B, more for layers over 384 channels (VGG's 512)
   // (kFmtPair8: the per-column dequantisation factors follow the biases)
-  static constexpr int BIAS_BYTES = NG * NBLK * NPAD * 4 * (PAIR ? 2 : 1);
+  // (kFmtFuse1x1: the fused layer's biases follow)
+  static constexpr int BIAS_BYTES = NG * NBLK * NPAD * 4 * (PAIR ? 2 : 1) + (FUSE ? kFuseNpad * 4 : 0);
   static constexpr int TAIL = 512 + (BIAS_BYTES > 1536 ? BIAS_BYTES : 1536);
   static constexpr int BUDGET = 227 * 1024 - 1024 - TAIL - STAGING;
   // halo ring: enough stages to prefetch the next chunk (or the next tile when there is one chunk)
@@ -181,6 +194,12 @@ struct UmmaCfg {
   static constexpr int PAIR_UNITS = PAIRS + KS * KS;        // units of NPAD * 32 B: e4m3 pairs, then bf16 taps
   static constexpr int PAIR_STAGES = PAIR_UNITS / 2;        // two units per weight stage of B_STAGE bytes
   static_assert(!PAIR || PAIR_UNITS % 2 == 0, "whole weight stages");
+  // kFmtFuse1x1: the layer's NPAD outputs are the 1x1 layer's 16-channel chunks; its weight stages are those of a
+  // CONCAT launch (64 B per output channel and chunk for [w_hi | w_lo])
+  static constexpr int FUSE_CHUNKS = NPAD / 16 / kFuseStages;  // chunks of the 1x1 layer per weight stage
+  static constexpr int FUSE_STAGE = FUSE_CHUNKS * kFuseNpad * 64;
+  static_assert(!FUSE || (!CONCAT && NBLK == 1 && MW == 1 && NG == 1 && !HI && !PAIR && FUSE_STAGE <= B_STAGE &&
+                          NPAD % (16 * kFuseStages) == 0), "the fused 1x1 layer follows a plain layer of one block");
   static constexpr int CPB = NCHUNK / NBLK;                // chunks per diagonal block
   static constexpr int BLK_COLS = DUAL ? 2 * NPAD : NPAD;   // accumulator columns per block
   static constexpr int COLS = NBLK * BLK_COLS;             // accumulator columns of the tile
@@ -209,6 +228,7 @@ struct ConvArgs {
   int N, H, W;
   int in_planes_half;   // C_in_pad / 8
   int tiles_x, tiles_y;
+  int num_tiles;        // work items: tiles_x * tiles_y * N * NG (one parameter load, never a register kept live)
   // kEpiAct
   ActDst dst0, dst1;
   int split_c;          // channels [0, split_c) -> dst0, [split_c, cout) -> dst1
@@ -251,6 +271,9 @@ struct ConvArgs {
   // stores zeros at slot pixels outside its valid extent; kEpiGate stores its kept rectangle into that window's
   // image (its own out_f32 / out_u8 and width)
   const RaggedWindow* rwin;
+  // kFmtFuse1x1: the fused 1x1 layer's bf16x3 CONCAT weight image and its biases
+  const uint8_t* wpk1x1;
+  const float* bias1x1;
 };
 
 __device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b) {
@@ -436,7 +459,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
   static_assert((2 * 6 + 2 * 8) * 8 <= 512 && C::BIAS_BYTES <= C::TAIL - 512, "barrier / bias area");
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int num_tiles = g.tiles_x * g.tiles_y * g.N * NG;
+  const int num_tiles = g.num_tiles;
   if (tid == 0) {
     for (int i = 0; i < C::NA; i++) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], C::CONSUMER_WARPS); }
     for (int i = 0; i < C::NB; i++) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], C::CONSUMER_WARPS); }
@@ -445,6 +468,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
   for (int i = tid; i < NG * NBLK * NPAD; i += C::THREADS) s_bias[i] = g.bias[i];
   if constexpr (C::PAIR)
     for (int i = tid; i < NPAD; i += C::THREADS) s_bias[NPAD + i] = g.f8_scale[i];
+  if constexpr (C::FUSE)
+    for (int i = tid; i < kFuseNpad; i += C::THREADS) s_bias[NPAD + i] = g.bias1x1[i];
   __syncthreads();
   // kFmtPair8: the tap-pair form runs on tiles of 8-bit levels (decided per call on the device, like the a_lo pass,
   // or per image with slot_levels); the B producer and the consumers take the same decision
@@ -492,16 +517,19 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
+      auto send = [&](const uint8_t* src, uint32_t bytes) {
+        mbar_wait(&b_empty[stage], phase ^ 1);
+        mbar_expect_tx(&b_full[stage], bytes);
+        bulk_load(b_stages + stage * C::B_STAGE, src, bytes, &b_full[stage]);
+        if (++stage == C::NB) { stage = 0; phase ^= 1; }
+      };
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const bool pair = pair_tile(tile);
         const uint8_t* wpk = pair ? g.wpk8 : g.wpk + (size_t)(tile % NG) * C::GROUP_BYTES;
         const int nit = pair ? C::PAIR_STAGES : C::NCHUNK * C::NSTAGE_PER_CHUNK;
-        for (int it = 0; it < nit; it++) {
-          mbar_wait(&b_empty[stage], phase ^ 1);
-          mbar_expect_tx(&b_full[stage], C::B_STAGE);
-          bulk_load(b_stages + stage * C::B_STAGE, wpk + (size_t)it * C::B_STAGE, C::B_STAGE, &b_full[stage]);
-          if (++stage == C::NB) { stage = 0; phase ^= 1; }
-        }
+        for (int it = 0; it < nit; it++) send(wpk + (size_t)it * C::B_STAGE, C::B_STAGE);
+        if constexpr (C::FUSE)  // then the fused 1x1 layer's whole image, kFuseStages more stages through the same ring
+          for (int it = 0; it < kFuseStages; it++) send(g.wpk1x1 + (size_t)it * C::FUSE_STAGE, C::FUSE_STAGE);
       }
     }
     return;
@@ -673,7 +701,51 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     const int m = wg * 64 + r;
     const int gy = ty * C::TILE_H + (m >> 3);
     const float dscale = F8IN && WGS == 3 ? *g.f8_scale : dscale0;
-    constexpr int NCH = NBLK * NPAD;
+    // kFmtFuse1x1: the fused layer's A operands (hi / lo, 4 registers per K step) and the ring stages of its weights
+    static_assert(!C::FUSE || kFuseNpad <= C::ACC, "the fused layer's accumulators take the place of this layer's");
+    uint32_t a_hi[C::FUSE ? NPAD / 4 : 1], a_lo[C::FUSE ? NPAD / 4 : 1];
+    int fuse_stage[kFuseStages];
+    if constexpr (C::FUSE) {
+      // This layer's activation in the accumulator layout, with the fp32 operations of its kEpiAct epilogue (max((acc
+      // + acc8) dscale + b, 0), or max(acc + b, 0); __fmul_rn / __fadd_rn so that nothing contracts into an fma),
+      // masked as a ragged slot masks it, and split into the bf16 hi / lo the 1x1 layer's own launch reads.  Register
+      // 2j + h holds columns 8j + fcol, +1 of row frow + 8h: registers 4k .. 4k + 3 are the A fragment of K step k.
+      bool row_valid[2] = {true, true};
+      if constexpr (RAG) {
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          const int mh = wg * 64 + frow + 8 * h;
+          row_valid[h] = tx * C::TILE_W + (mh & 7) < g.rwin[n].vw && ty * C::TILE_H + (mh >> 3) < g.rwin[n].vh;
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < NPAD / 8; j++) {
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          float x[2];
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            float s = acc[0][4 * j + 2 * h + e];
+            if constexpr (F8IN) s = __fmul_rn(__fadd_rn(s, acc8[0][4 * j + 2 * h + e]), dscale);
+            x[e] = fmaxf(__fadd_rn(s, s_bias[8 * j + fcol + e]), 0.f);
+            if constexpr (RAG) x[e] = row_valid[h] ? x[e] : 0.f;
+          }
+          split_bf16x2(x[0], x[1], a_hi[2 * j + h], a_lo[2 * j + h]);
+        }
+      }
+      // its weight stages (the B producer sends them behind this tile's): released once the epilogue is done
+#pragma unroll
+      for (int s = 0; s < kFuseStages; s++) {
+        mbar_wait(&b_full[bstage], bphase);
+        fuse_stage[s] = bstage;
+        if (++bstage == C::NB) { bstage = 0; bphase ^= 1; }
+      }
+    }
+    // the epilogue stores this layer's output, or the fused 1x1 layer's (its biases follow this layer's)
+    constexpr bool EDUAL = DUAL || C::FUSE, EF8 = F8IN && !C::FUSE;
+    constexpr int ENPAD = C::FUSE ? kFuseNpad : NPAD;
+    constexpr int NCH = C::FUSE ? kFuseNpad : NBLK * NPAD;
+    const float* e_bias = C::FUSE ? s_bias + NPAD : s_bias;
 #pragma unroll
     for (int mb = 0; mb < MW; mb++) {
       const int gx = tx * C::TILE_W + mb * 8 + (m & 7);
@@ -682,6 +754,28 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
       if constexpr (RAG) valid = gx < g.rwin[n].vw && gy < g.rwin[n].vh;
 #pragma unroll
       for (int ch0 = 0; ch0 < NCH; ch0 += 32) {
+        if constexpr (C::FUSE) {
+          // the fused layer's output channels [ch0, ch0 + 32), into the registers of its columns in a CONCAT launch's
+          // accumulators (w_hi products at ch0, w_lo products at kFuseNpad + ch0): per chunk the N = 32 column blocks
+          // a_hi x w_hi, a_hi x w_lo, a_lo x w_hi -- per column the products and the order of that launch's
+          // a_hi x [w_hi | w_lo], a_lo x w_hi.  32 accumulators at a time beside the 64 A registers.
+          float* d_hi = acc[0] + ch0 / 2;
+          float* d_lo = acc[0] + (kFuseNpad + ch0) / 2;
+#pragma unroll
+          for (int i = 0; i < 16; i++) d_hi[i] = d_lo[i] = 0.f;
+          wg_fence();
+#pragma unroll
+          for (int k = 0; k < NPAD / 16; k++) {
+            const uint32_t b_hi = smem_u32(b_stages + fuse_stage[k / C::FUSE_CHUNKS] * C::B_STAGE) +
+                                  (uint32_t)((k % C::FUSE_CHUNKS) * kFuseNpad * 64 + ch0 * 16);
+            const uint32_t b_lo = b_hi + kFuseNpad * 16;
+            wgmma_bf16_rs<32>(d_hi, a_hi + 4 * k, make_desc(b_hi, 2 * kFuseNpad * 16, 128));  // a_hi x w_hi
+            wgmma_bf16_rs<32>(d_lo, a_hi + 4 * k, make_desc(b_lo, 2 * kFuseNpad * 16, 128));  // a_hi x w_lo
+            wgmma_bf16_rs<32>(d_hi, a_lo + 4 * k, make_desc(b_hi, 2 * kFuseNpad * 16, 128));  // a_lo x w_hi
+          }
+          wg_commit();
+          wg_wait<0>();
+        }
 #pragma unroll
         for (int j = 0; j < 4; j++) {
           const int ch = ch0 + 8 * j;
@@ -691,8 +785,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
 #pragma unroll
             for (int k = 0; k < 4; k++) {
               v[k] = acc[mb][col / 2 + k];
-              if constexpr (DUAL) v[k] += acc[mb][(col + NPAD) / 2 + k];
-              if constexpr (F8IN) v[k] = (v[k] + acc8[mb][col / 2 + k]) * dscale;
+              if constexpr (EDUAL) v[k] += acc[mb][(col + ENPAD) / 2 + k];
+              if constexpr (EF8) v[k] = (v[k] + acc8[mb][col / 2 + k]) * dscale;
               if constexpr (C::PAIR) v[k] = pair ? v[k] * s_bias[NPAD + col + fcol + (k & 1)] : v[k];
             }
             float* s = stg + frow * kStageLd + 8 * j + fcol;
@@ -710,11 +804,15 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
             const float4 x = s[q];
             f[4 * q] = x.x; f[4 * q + 1] = x.y; f[4 * q + 2] = x.z; f[4 * q + 3] = x.w;
           }
-          epilogue16<EPI, OUT8, RAG, C::HI>(g, s_bias, f, c0 + cb, n, gx, gy, valid);
+          epilogue16<EPI, OUT8, RAG, C::HI>(g, e_bias, f, c0 + cb, n, gx, gy, valid);
         }
         wg_bar(1 + wg);
       }
     }
+    if constexpr (C::FUSE)
+      if (lane == 0)
+#pragma unroll
+        for (int s = 0; s < kFuseStages; s++) mbar_arrive(&b_empty[fuse_stage[s]]);
   }
 }
 
@@ -949,6 +1047,7 @@ static int launch_conv(wn_handle* h, int slot, const uint8_t* wpk, const float* 
   a.tiles_x = (a.W + C::TILE_W - 1) / C::TILE_W;
   a.tiles_y = (a.H + C::TILE_H - 1) / C::TILE_H;
   const long long tiles = (long long)a.tiles_x * a.tiles_y * a.N * NG;
+  a.num_tiles = (int)tiles;
   auto kern = conv_umma_kernel<KS, CIN_PAD, NPAD, EPI, CONCAT, NBLK, TPS, FMT, RAG, MW, NG, WGS>;
   WN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
   TimedScope ts(h, slot, stream);
