@@ -1,7 +1,7 @@
 """Enhance images / videos (same CLI and output layout as the reference's inference.py).
 
     python inference.py --source <image|video|directory> [--weights W] [--name NAME] [--show-split]
-                        [--tile N] [--batch N]
+                        [--tile N|auto] [--batch N]
 
 Every frame goes uint8 -> GPU (preprocess, gated-fusion forward, uint8 postprocess) -> uint8
 through ``waternet_b200.api.Enhancer``; video frames are processed in small batches.  File and
@@ -17,7 +17,7 @@ import torch
 from waternet.net import WaterNet
 from waternet_b200.api import Enhancer
 from waternet_b200.hub import DEFAULT_CKPT_URL
-from waternet_b200.training import next_run_dir
+from waternet_b200.training import next_run_dir, tile_arg
 
 ROOT = Path(__file__).parent.resolve()
 DEFAULT_CKPT = "waternet_exported_state_dict-daa0ee.pt"
@@ -118,9 +118,10 @@ def main():
     ap.add_argument("--name", type=str, help="(Optional) Subfolder name to save under `./output`.")
     ap.add_argument("--show-split", action="store_true", default=False,
                     help="(Optional) Left/right of output is original/processed, with a before/after watermark.")
-    ap.add_argument("--tile", type=int, default=None,
+    ap.add_argument("--tile", type=tile_arg, default=None, metavar="N|auto",
                     help="(Optional) Compute each image in overlapping tiles of at most N x N output pixels: the same "
-                         "result with GPU memory that does not grow with the image size (e.g. 998 for large photos).")
+                         "result with GPU memory that does not grow with the image size (e.g. 998 for large photos).  "
+                         "auto: whole images where they fit half the card's memory, else tiles of 998, per call.")
     ap.add_argument("--batch", type=int, default=1,
                     help="(Optional) Enhance the still images of a directory N at a time, each at its own size, in "
                          "one GPU call per group (the same result; --tile sets the tile of that call).")

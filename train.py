@@ -38,10 +38,11 @@ def main():
     ap.add_argument("--loader", default="gpu", choices=["gpu", "torch"],
                     help="gpu: batches augmented + preprocessed on the device in one call; torch: the reference's "
                          "per-item DataLoader path")
-    ap.add_argument("--grad-tile", type=int, default=None, metavar="N",
+    ap.add_argument("--grad-tile", type=T.tile_arg, default=None, metavar="N|auto",
                     help="(Optional) Compute the gradients in overlapping windows of N x N output pixels "
                          "(WaterNet.grad_tile): about 12 GB of activations whatever the image and batch size, for "
-                         "about 1.5x the arithmetic.  Unset: whole images, ~5.6 KB per pixel")
+                         "about 1.5x the arithmetic.  auto: whole images where their activations fit half the card's "
+                         "memory, else windows of 998, per batch.  Unset: whole images, ~5.6 KB per pixel")
     ap.add_argument("--native-size", action="store_true",
                     help="(Optional) Train every image at its own size: the dataset without --height/--width (UIEB: "
                          "rounded down to a multiple of 32, as the reference does) and batches of differently sized "
@@ -106,7 +107,7 @@ def main():
         torch.save(model.state_dict(), savedir / "last.pt")
     T.save_metrics(savedir, train_hist, val_hist, {
         "epochs": args.epochs, "batch_size": args.batch_size, "im_height": args.height, "im_width": args.width,
-        "weights": args.weights, "native_size": args.native_size,
+        "weights": args.weights, "native_size": args.native_size, "grad_tile": args.grad_tile,
         "train_precision": args.train_precision, **T.perceptual_config(args)})
     print(f"Metrics and weights saved to {savedir}")
     print(f"Total time: {timer() - start}s")

@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .engine import Engine
+from .engine import AUTO_TILE, Engine, is_auto
 from .net import MODES
 
 
@@ -47,7 +47,9 @@ class Enhancer:
     ``tile``: ``None`` runs whole images per pass (``Engine.enhance``).  An int or (h, w) runs the tiled forward
     (``Engine.enhance_tiled``: the same bits, with a workspace that does not grow with the image size -- for photos
     and frames too large for one pass) one image per pipelined pass, so that image i+1's copy-in runs under image
-    i's kernels; it never captures a graph.  Tensor-core precisions only.
+    i's kernels; it never captures a graph.  Tensor-core precisions only.  ``"auto"`` chooses per call shape
+    (``Engine.auto_tile``): whole images where their workspace fits ``Engine.AUTO_WORKSPACE_BYTES`` (None: half the
+    card's memory), else the tiled forward with ``Engine.DEFAULT_TILE``; whole images always with precision "fp32".
     """
 
     GRAPH_MAX_PIXELS = 1 << 20
@@ -59,8 +61,8 @@ class Enhancer:
         self.model = model
         self.engine: Engine = model.engine()  # raises without CUDA: there is no CPU path
         self.mode = model._mode() if precision is None else MODES[precision]
-        self.tile = None if tile is None else Engine._tile_hw(tile)
-        if self.tile is not None and self.mode == _lib.MODE_FP32_SIMT:
+        self.tile = tile if tile is None or is_auto(tile) else Engine._tile_hw(tile)
+        if self.tile not in (None, AUTO_TILE) and self.mode == _lib.MODE_FP32_SIMT:
             raise ValueError("tile: the tiled forward runs in the tensor-core precisions only, not fp32")
         self.cuda_graph = cuda_graph
         self._slots: List[_Slot] = [_Slot() for _ in range(max(1, depth))]
@@ -91,9 +93,9 @@ class Enhancer:
 
     def enhance_many(self, images) -> list:
         """A list of uint8 HWC images, each of its own size (a directory of photos), enhanced in one ragged call
-        (``Engine.enhance_ragged`` with ``tile``, or ``Engine.DEFAULT_TILE`` when that is None): one copy in through
-        a pinned staging buffer of the total size, one call, one copy out.  Returns the list of enhanced images; each
-        equals what ``self(image)`` returns.  Tensor-core precisions only."""
+        (``Engine.enhance_ragged`` with ``tile``, or ``Engine.DEFAULT_TILE`` when that is None or "auto"): one copy
+        in through a pinned staging buffer of the total size, one call, one copy out.  Returns the list of enhanced
+        images; each equals what ``self(image)`` returns.  Tensor-core precisions only."""
         if self.mode == _lib.MODE_FP32_SIMT:
             raise ValueError("enhance_many: ragged batches run in the tensor-core precisions only, not fp32")
         arrs = [np.asarray(a) for a in images]
@@ -118,7 +120,8 @@ class Enhancer:
             dev_in.copy_(pin_in[:total], non_blocking=True)
             views = [(dev_in[o:o + a.size].view(a.shape), dev_out[o:o + a.size].view(a.shape))
                      for a, o in zip(arrs, offs)]
-            eng.enhance_ragged([v for v, _ in views], tile=self.tile or Engine.DEFAULT_TILE, mode=self.mode,
+            tile = Engine.DEFAULT_TILE if self.tile in (None, AUTO_TILE) else self.tile
+            eng.enhance_ragged([v for v, _ in views], tile=tile, mode=self.mode,
                                out_u8=[v for _, v in views])
             pin_out[:total].copy_(dev_out, non_blocking=True)
             torch.cuda.current_stream(dev).synchronize()
@@ -126,12 +129,19 @@ class Enhancer:
         return [out[o:o + a.size].reshape(a.shape).copy() for a, o in zip(arrs, offs)]
 
     # ---- kernels of one pass --------------------------------------------------------------------
-    def _run_kernels(self, eng: Engine, slot: _Slot, a: int, b: int, whole: bool, peer_out=()) -> None:
-        """preprocess -> forward -> ten2arr of images [a, b) of the slot (graph replay when small)."""
+    def _call_tile(self, n: int, h: int, w: int):
+        """The tile of a call on n images of h x w: ``tile``, with "auto" resolved for that shape."""
+        if self.tile != AUTO_TILE:
+            return self.tile
+        return Engine.auto_tile("enhance", (n, h, w), self.mode, device=self.engine.device)
+
+    def _run_kernels(self, eng: Engine, slot: _Slot, a: int, b: int, whole: bool, tile=None, peer_out=()) -> None:
+        """preprocess -> forward -> ten2arr of images [a, b) of the slot (graph replay when small), in windows of
+        ``tile`` when it is not None."""
         src, dst = slot.dev_in[a:b], slot.dev_out[a:b]
         shape = tuple(slot.dev_in.shape)
-        if self.tile is not None:
-            eng.enhance_tiled(src, tile=self.tile, mode=self.mode, out_u8=dst)
+        if tile is not None:
+            eng.enhance_tiled(src, tile=tile, mode=self.mode, out_u8=dst)
             return
         if peer_out or not (self.cuda_graph and whole and shape[0] * shape[1] * shape[2] <= self.GRAPH_MAX_PIXELS):
             eng.enhance(src, mode=self.mode, out_u8=dst, peer_out=peer_out)
@@ -165,11 +175,12 @@ class Enhancer:
         ``exchange``: a :class:`waternet_b200.dist.PeerGather` -- the multi-GPU all-gather of the output fused into the
         kernels: every pass's last launch stores its output into all ranks' buffers as well (``exchange.addresses``),
         ``exchange.signal()`` follows the last pass on the compute stream and ``exchange.wait()`` the last D2H copy
-        on the copy-out stream.
+        on the copy-out stream.  With ``tile`` "auto" a batch that would run in windows refuses ``exchange``.
         """
         if pin_in.dtype != torch.uint8 or pin_in.dim() != 4 or pin_in.shape[3] != 3 or pin_in.shape != pin_out.shape:
             raise ValueError(f"expected uint8 (N,H,W,3) pinned tensors of one shape, got {tuple(pin_in.shape)}")
-        if exchange is not None and self.tile is not None:
+        tile = self._call_tile(*pin_in.shape[:3])
+        if exchange is not None and tile is not None:
             raise ValueError("exchange: the fused multi-GPU exchange is not available with tile")
         eng = self.model.engine()  # re-packs if the parameters changed since the last call (no-op otherwise)
         dev = eng.device
@@ -191,7 +202,7 @@ class Enhancer:
             slot.done = torch.cuda.Event()
             slot.done.record(cur)
             return slot
-        nb = 1 if self.tile is not None else eng.chunk_images(n, h, w)
+        nb = 1 if tile is not None else eng.chunk_images(n, h, w)
         self._s_in.wait_stream(cur)   # whatever the caller enqueued before (e.g. filling pin_in on the device side)
         self._s_out.wait_stream(cur)
         for a in range(0, n, nb):
@@ -201,7 +212,7 @@ class Enhancer:
                 ev_in = torch.cuda.Event()
                 ev_in.record(self._s_in)
             cur.wait_event(ev_in)
-            self._run_kernels(eng, slot, a, b, whole=(a == 0 and b == n),
+            self._run_kernels(eng, slot, a, b, whole=(a == 0 and b == n), tile=tile,
                               peer_out=exchange.addresses(a) if exchange is not None else ())
             if exchange is not None and b == n:
                 exchange.signal()

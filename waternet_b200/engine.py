@@ -207,6 +207,18 @@ def perceptual_loss_workspace_bytes(n: int, h: int, w: int, tile_h: int, tile_w:
     return a1k(windows * VGG_SEED_BLOCKS * 8) + max(pass_bytes(*p) for p in passes) + 1024
 
 
+AUTO_TILE = "auto"  # the value of tile / grad_tile that leaves the choice to Engine.auto_tile, call by call
+
+
+def is_auto(tile, name: str = "tile") -> bool:
+    """Whether the setting ``tile`` (named ``name`` in errors) is "auto"; any other string raises ValueError."""
+    if isinstance(tile, str):
+        if tile != AUTO_TILE:
+            raise ValueError(f"{name} must be None, {AUTO_TILE!r}, an int or (h, w); got {tile!r}")
+        return True
+    return False
+
+
 def _stream_ptr(device: torch.device) -> ctypes.c_void_p:
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -415,6 +427,12 @@ class Engine:
                 torch._foreach_add_(grads, part)
         return grads
 
+    @classmethod
+    def _train_slice_bounds(cls, n: int, h: int, w: int) -> list:
+        """The slices [(a, b), ...] of ``_train_slices`` for n images of h x w (at most TRAIN_MAX_PIXELS)."""
+        per = min(cls.TRAIN_MAX_IMAGES, max(1, cls.TRAIN_MAX_PIXELS // (h * w)))
+        return [(a, min(n, a + per)) for a in range(0, n, per)]
+
     def _train_slices(self, what: str, lead, ins, workspace_bytes, too_large: str, train_mode: int):
         """``ins`` in slices of at most TRAIN_MAX_PIXELS and TRAIN_MAX_IMAGES, each one call of ``what`` (``lead``
         before the inputs) with a workspace of its own of ``workspace_bytes(n, h, w)`` bytes.  Returns (out, [(a, b,
@@ -427,10 +445,8 @@ class Engine:
             return out, None
         if h * w > self.TRAIN_MAX_PIXELS:
             raise _lib.WaterNetLibraryError(too_large.format(h=h, w=w))
-        per = min(self.TRAIN_MAX_IMAGES, max(1, self.TRAIN_MAX_PIXELS // (h * w)))
         saved = []
-        for a in range(0, n, per):
-            b = min(n, a + per)
+        for a, b in self._train_slice_bounds(n, h, w):
             part = [t[a:b] for t in ins]
             ws = torch.empty(workspace_bytes(b - a, h, w), dtype=torch.uint8, device=self.device)
             self._call(what, *lead, *(t.data_ptr() for t in part), _strides(part), out[a:b].data_ptr(), b - a, h, w,
@@ -642,6 +658,63 @@ class Engine:
         return out_u8
 
     DEFAULT_TILE = (998, 998)  # a window (tile + 13 pixels of context per side) of at most 1024 x 1024
+
+    # ---- tile "auto": whole images where their workspace fits a budget, else windows of DEFAULT_TILE ----------------
+    # The budget of auto_tile in bytes; None: half the device's total memory (42.5 GB on an H100 80GB).  It comes from
+    # the card, not from its free memory, so that other work on a shared card never decides which path a call takes
+    # (in training the two paths differ in the last bits of the gradients).
+    AUTO_WORKSPACE_BYTES: Optional[int] = None
+
+    @classmethod
+    def whole_image_bytes(cls, kind: str, shapes, mode: int, train_mode: Optional[int] = None) -> int:
+        """The device memory the whole-image path of one call of ``kind`` takes, from the library's workspace
+        queries, or 0 where that path refuses the call.  ``shapes``: (n, h, w), or [(h, w), ...] for "ragged".
+
+        Kinds: "net" (``WaterNet``), "cmg", "refiner" -- with ``train_mode`` None the inference workspace
+        (wn_forward_workspace_bytes, wn_submodule_workspace_bytes: the largest pass), else the sum of the training
+        workspaces of the slices ``_train_slices`` makes, all of which are kept until backward; "ragged"
+        (``forward_many`` under autograd: the training calls of ``ragged_train_calls``); "enhance" (uint8,
+        wn_enhance_workspace_bytes) and "vgg" (the perceptual loss with one window per image)."""
+        lib = _lib.load()
+        if kind == "ragged":
+            sizes = [(h, w) for h, w in shapes if h * w > 0]
+            if any(h * w > cls.TRAIN_MAX_PIXELS for h, w in sizes):
+                return 0
+            parts = [lib.wn_train_ragged_workspace_bytes(*_sizes([sizes[k] for k in idx]), len(idx))
+                     for idx in ragged_train_calls(sizes, cls.TRAIN_MAX_PIXELS)]
+            return 0 if 0 in parts else int(sum(parts))
+        n, h, w = (int(v) for v in shapes)
+        if kind == "enhance":
+            return int(lib.wn_enhance_workspace_bytes(n, h, w, mode))
+        if kind == "vgg":
+            return int(lib.wn_perceptual_loss_workspace_bytes(n, h, w, 0, 0, 0))
+        if kind not in ("net", "cmg", "refiner"):
+            raise ValueError(f"unknown kind {kind!r}")
+        if train_mode is None:
+            query = lib.wn_forward_workspace_bytes if kind == "net" else lib.wn_submodule_workspace_bytes
+            return int(query(n, h, w, mode))
+        if n <= 0 or h * w > cls.TRAIN_MAX_PIXELS:
+            return 0
+        stack = cls.STACK_CMG if kind == "cmg" else cls.STACK_REFINER
+        parts = [lib.wn_train_workspace_bytes(b - a, h, w) if kind == "net" else
+                 lib.wn_submodule_train_workspace_bytes(b - a, h, w, stack)
+                 for a, b in cls._train_slice_bounds(n, h, w)]
+        return 0 if 0 in parts else int(sum(parts))
+
+    @classmethod
+    def auto_tile(cls, kind: str, shapes, mode: int, train_mode: Optional[int] = None, device=None):
+        """What tile (or grad_tile) "auto" means for one call: None (whole images) when ``whole_image_bytes`` of the
+        call is at most the budget (``AUTO_WORKSPACE_BYTES``, or half of ``device``'s memory), else DEFAULT_TILE.  A
+        call the whole-image path refuses takes windows; a call without pixels and any call in ``mode``
+        MODE_FP32_SIMT (which has no windowed path) take whole images."""
+        sizes = shapes if kind == "ragged" else [tuple(shapes[1:])] if shapes[0] > 0 else []
+        if mode == _lib.MODE_FP32_SIMT or not any(h * w for h, w in sizes):
+            return None
+        need = cls.whole_image_bytes(kind, shapes, mode, train_mode)
+        budget = cls.AUTO_WORKSPACE_BYTES
+        if budget is None:
+            budget = torch.cuda.get_device_properties(_require_cuda(device)).total_memory // 2
+        return None if 0 < need <= budget else cls.DEFAULT_TILE
 
     @staticmethod
     def _tile_hw(tile) -> Tuple[int, int]:

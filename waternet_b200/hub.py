@@ -43,7 +43,8 @@ def waternet(pretrained: bool = True, device=None, tile=None):
     ``preprocess(rgb_arr)``: HWC (or NHWC) uint8 array -> ``(rgb, wb, he, gc)`` fp32
     (N,3,H,W) tensors on the device (``hubconf.py:85-91``).  ``postprocess(out)``:
     model output -> uint8 NHWC array (``hubconf.py:93-94``).  ``tile`` sets ``model.tile``
-    (e.g. 998): the model then runs in overlapping windows, so that images of any size fit.
+    (e.g. 998): the model then runs in overlapping windows, so that images of any size fit; ``"auto"`` runs whole
+    images where they fit half the card's memory and windows otherwise, chosen per call (``Engine.auto_tile``).
     """
     eng = get_engine(device)
     model = WaterNet(tile=tile)

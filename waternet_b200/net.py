@@ -29,7 +29,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib
-from .engine import TRAIN_PASS_PIXELS, Engine, new_engine
+from .engine import AUTO_TILE, TRAIN_PASS_PIXELS, Engine, is_auto, new_engine
 
 MODES = {"default": _lib.MODE_DEFAULT, "fp32": _lib.MODE_FP32_SIMT, "bf16x3": _lib.MODE_BF16X3,
          "bf16_fp8": _lib.MODE_BF16_FP8}
@@ -45,11 +45,14 @@ _model_engines = weakref.WeakKeyDictionary()
 _model_engines_lock = threading.Lock()
 
 
-def _checked_tile(name: str, runs: str, tile, mode: int):
+def _checked_tile(name: str, runs: str, tile, mode: int, auto=None):
     """``tile`` (the attribute ``name``) as (h, w), or None.  ``runs`` (the tiled forward, the windowed backward) runs
-    on the tensor cores only."""
+    on the tensor cores only.  "auto" gives ``auto()``, the choice of ``Engine.auto_tile`` for one call, or "auto"
+    itself without ``auto`` (the setting checked outside a call)."""
     if tile is None:
         return None
+    if is_auto(tile, name):
+        return tile if auto is None else auto()
     if mode == _lib.MODE_FP32_SIMT:
         raise ValueError(f"{name}: {runs} runs on the tensor cores only, and precision='fp32' is the CUDA-core mode; "
                          f"use precision='default' or 'bf16x3', or {name}=None")
@@ -142,14 +145,34 @@ class _NetModule(_PackedWeightsMixin, nn.Module):
             raise ValueError(f"unknown train_precision {train_precision!r}; choose from {sorted(TRAIN_PRECISIONS)}")
         return TRAIN_PRECISIONS[train_precision]
 
-    def _tile(self):
-        """The window tile of a call without an autograd graph, as (h, w), or None.  Refused with precision "fp32"."""
-        return _checked_tile("tile", "the tiled forward", self._owner().tile, self._mode())
+    _auto_kind = "net"  # the kind of Engine.auto_tile for this module's calls
 
-    def _grad_tile(self):
-        """The windowed-backward tile of a call that records an autograd graph, as (h, w), or None.  Refused with
-        precision "fp32"."""
-        return _checked_tile("grad_tile", "the windowed backward", self._owner().grad_tile, self._mode())
+    def _auto(self, x, train: bool, sizes=None):
+        """The resolver of "auto" for a call on ``x`` (its first input; None: no call) that records an autograd graph
+        when ``train``: Engine.auto_tile of this module's kind on x's (n, h, w), or of forward_many's training calls on
+        the images of ``sizes``.  None (whole images) for CPU tensors, which have no windowed path."""
+        if x is None:
+            return None
+        mode = self._mode()
+
+        def resolve():
+            if not x.is_cuda or x.dim() != 4:
+                return None
+            train_mode = self._train_mode() if train else None
+            kind, shapes = ("ragged", sizes) if sizes is not None else (self._auto_kind, (x.shape[0],) + x.shape[2:])
+            return Engine.auto_tile(kind, shapes, mode, train_mode, device=x.device)
+        return resolve
+
+    def _tile(self, x=None):
+        """The window tile of a call without an autograd graph on ``x`` (its first input), as (h, w), or None; "auto"
+        is resolved from x's shape (and left as "auto" without x).  Refused with precision "fp32", except "auto"."""
+        return _checked_tile("tile", "the tiled forward", self._owner().tile, self._mode(), self._auto(x, False))
+
+    def _grad_tile(self, x=None, sizes=None):
+        """The windowed-backward tile of a call that records an autograd graph, as ``_tile``; ``sizes``: the images of
+        a forward_many call, [(h, w), ...].  Refused with precision "fp32", except "auto"."""
+        return _checked_tile("grad_tile", "the windowed backward", self._owner().grad_tile, self._mode(),
+                             self._auto(x, True, sizes))
 
 
 class _Training(NamedTuple):
@@ -259,7 +282,8 @@ class _ConvStack(_NetModule):
     the stack's activations window by window (``wn_confidence_maps_backward_tiled`` / ``wn_refine_backward_tiled``),
     in about 8 GB for the cmg and 4 GB for a refiner whatever the image or batch size, with no limit on the image
     size.  Bound to a ``WaterNet`` a stack follows the parent's ``precision``, ``train_precision``, ``tile`` and
-    ``grad_tile``; a free-standing one uses its own attributes.
+    ``grad_tile``; a free-standing one uses its own attributes.  "auto" chooses per call as ``WaterNet`` describes,
+    from this stack's own workspace.
     """
 
     spec: List[tuple] = []
@@ -328,7 +352,7 @@ class _ConvStack(_NetModule):
     def _trained(self, ins):
         """The stack on ``ins`` recording an autograd graph: natively where ``_train_engine`` allows, else the torch
         graph."""
-        grad_tile = self._grad_tile()
+        grad_tile = self._grad_tile(ins[0])
         native = self._train_engine(ins[0], any_size=grad_tile is not None)
         if native is None:
             return self._graph(*ins)
@@ -350,6 +374,7 @@ class ConfidenceMapGenerator(_ConvStack):
 
     spec = CMG_SPEC
     _training = (_CMG_TRAINING,)
+    _auto_kind = "cmg"
 
     def _graph(self, x, wb, ce, gc):
         out = torch.cat([x, wb, ce, gc], dim=1)
@@ -368,7 +393,7 @@ class ConfidenceMapGenerator(_ConvStack):
         if _needs_graph(ins, self._own_params()):
             maps = self._trained(ins)
         else:
-            mode, tile = self._mode(), self._tile()
+            mode, tile = self._mode(), self._tile(x)
             eng, _ = self._engine_and_slot(x)
             maps = eng.confidence_maps(*ins, mode) if tile is None else eng.confidence_maps_tiled(*ins, tile, mode)
         return torch.split(maps, [1, 1, 1], dim=1)
@@ -379,6 +404,7 @@ class Refiner(_ConvStack):
 
     spec = REFINER_SPEC
     _training = _REFINER_TRAINING  # by slot (0 wb, 1 ce, 2 gc)
+    _auto_kind = "refiner"
 
     def _graph(self, x, xbar):
         out = torch.cat([x, xbar], dim=1)
@@ -393,7 +419,7 @@ class Refiner(_ConvStack):
     def forward(self, x, xbar):
         if _needs_graph((x, xbar), self._own_params()):
             return self._trained((x, xbar))
-        mode, tile = self._mode(), self._tile()
+        mode, tile = self._mode(), self._tile(x)
         eng, slot = self._engine_and_slot(x)
         return eng.refine(slot, x, xbar, mode) if tile is None else eng.refine_tiled(slot, x, xbar, tile, mode)
 
@@ -447,6 +473,12 @@ class WaterNet(_NetModule):
     about 12 GB whatever the image or batch size.  The gradients equal the untiled ones up to the order of fp32 sums.
     It costs one more forward and the windows' overlap, so where the untiled path fits it is faster.  Tensor-core
     precisions only.  Calls of ``cmg`` and the refiners on their own follow it as well (``_ConvStack``).
+
+    ``tile="auto"`` / ``grad_tile="auto"`` choose per call, from the input's shape (``Engine.auto_tile``): whole images
+    where the whole-image path's workspace for the call (for training: every activation it keeps) is at most
+    ``Engine.AUTO_WORKSPACE_BYTES`` (None: half the card's memory), else windows of ``Engine.DEFAULT_TILE``; a call the
+    whole-image path refuses (an image over 8 Mi pixels under autograd) takes windows.  With ``precision="fp32"``
+    "auto" always means whole images.  ``forward_many`` decides ``grad_tile`` once for its whole list.
 
     ``train_precision``: the arithmetic of the native training calls (forward, data gradients and weight gradients of
     every call that records an autograd graph, windowed and ragged ones included).  ``"bf16x3"`` (default, ~1e-5 of
@@ -527,13 +559,13 @@ class WaterNet(_NetModule):
             return self._engine_with_weights(x).forward(*ins, mode)
         # tile does not apply to training: it keeps every activation of whole images, unless grad_tile
         if _needs_graph(ins, self.parameters()):
-            grad_tile = self._grad_tile()
+            grad_tile = self._grad_tile(x)
             if mode == _lib.MODE_FP32_SIMT:
                 return _GraphBackward.apply(self, *ins, *self.parameters())
             train_mode = self._train_mode()
             return _NativeTraining.apply(_NET_TRAINING, self._engine_with_weights(x), grad_tile, train_mode, 4, *ins,
                                          *self.parameters())
-        tile = self._tile()
+        tile = self._tile(x)
         eng = self._engine_with_weights(x)
         return eng.forward(*ins, mode) if tile is None else eng.forward_tiled(*ins, tile, mode)
 
@@ -572,16 +604,18 @@ class WaterNet(_NetModule):
             self._engine_for(x0.device, None)  # raises: there is no CPU path
         flat = [t for it in items for t in it]
         if _needs_graph(flat, self.parameters()):
-            grad_tile = self._grad_tile()
+            sizes = [] if self.grad_tile is None else \
+                [tuple(x.shape[2:]) for x, *_ in items for _ in range(x.shape[0]) if x.shape[2] * x.shape[3]]
+            grad_tile = self._grad_tile(x0, sizes)  # "auto": once for the whole list, kept in ctx for backward
             eng = self._engine_with_weights(x0)
             train_mode = self._train_mode()
             if grad_tile is not None:  # refuse here what the backward would refuse (a window over one training pass)
-                sizes = [tuple(x.shape[2:]) for x, *_ in items for _ in range(x.shape[0]) if x.shape[2] * x.shape[3]]
                 if sizes and eng.backward_ragged_tiled_workspace_bytes(sizes, grad_tile, TRAIN_PASS_PIXELS) == 0:
                     raise _lib.WaterNetLibraryError(
                         f"forward_many: wn_backward_ragged_tiled rejects these images at grad_tile={grad_tile} (a "
                         f"window may have at most {Engine.TRAIN_MAX_PIXELS >> 20} Mi pixels); use a smaller grad_tile")
             return list(_NativeTraining.apply(_RAGGED_TRAINING, eng, grad_tile, train_mode, len(flat), *flat,
                                               *self.parameters()))
-        tile = self._tile() or Engine.DEFAULT_TILE
+        tile = self._tile()
+        tile = Engine.DEFAULT_TILE if tile is None or tile == AUTO_TILE else tile
         return self._engine_with_weights(x0).forward_ragged(items, tile, mode)

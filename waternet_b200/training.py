@@ -9,6 +9,7 @@ PyTorch.
 """
 from __future__ import annotations
 
+import argparse
 import json
 import warnings
 from pathlib import Path
@@ -18,6 +19,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
+from .engine import AUTO_TILE, Engine, is_auto
 from .metrics import psnr, ssim
 from .net import TRAIN_PRECISIONS, _PackedWeightsMixin
 
@@ -42,7 +44,9 @@ class PerceptualModel(_PackedWeightsMixin, nn.Module):
     (None: one window per image; an image over 8 Mi pixels then needs a tile), so memory is bounded by one pass
     whatever the image and batch size.  Autograd keeps only d(out), 12 bytes per pixel; no VGG weight gradient is
     computed (the VGG parameters' ``.grad`` stays untouched) and ``ref`` is a constant.  ``native=False`` and CPU
-    tensors evaluate the torch expression.
+    tensors evaluate the torch expression.  ``tile="auto"`` chooses per call (``Engine.auto_tile``): one window per
+    image where that workspace fits ``Engine.AUTO_WORKSPACE_BYTES`` (None: half the card's memory) and the call is
+    allowed, else windows of ``Engine.DEFAULT_TILE``.
 
     ``precision``: the arithmetic of the native calls' 32 VGG convolutions.  "bf16x3" (default) issues three bf16
     tensor-core products per product; "bf16" issues one, a_hi x w_hi with fp32 accumulation, as autocast runs a frozen
@@ -57,6 +61,7 @@ class PerceptualModel(_PackedWeightsMixin, nn.Module):
         self.tile = tile
         self.precision = precision
         self._train_mode()
+        is_auto(tile)  # a string other than "auto" is refused here
         import torchvision
         vgg = None
         if pretrained:
@@ -98,6 +103,13 @@ class PerceptualModel(_PackedWeightsMixin, nn.Module):
         eng.pack_vgg_weights(params, key=self._pack_key(params))
         return eng
 
+    def _loss_tile(self, out):
+        """``tile`` of a native call on ``out``, with "auto" resolved for its shape."""
+        if not is_auto(self.tile):
+            return self.tile
+        n, _, h, w = out.shape
+        return Engine.auto_tile("vgg", (n, h, w), self._train_mode(), device=out.device)
+
     def native_loss(self, out, ref):
         """The loss of ``perceptual_loss`` from one ``wn_perceptual_loss`` call (autograd: d(out) only)."""
         want = torch.is_grad_enabled() and out.requires_grad
@@ -110,7 +122,7 @@ class _NativePerceptualLoss(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, out, ref, vgg, want_grad):
-        loss, grad = vgg._vgg_engine(out).perceptual_loss(out, ref, tile=vgg.tile, want_grad=want_grad,
+        loss, grad = vgg._vgg_engine(out).perceptual_loss(out, ref, tile=vgg._loss_tile(out), want_grad=want_grad,
                                                           train_mode=vgg._train_mode())
         if grad is not None:
             ctx.save_for_backward(grad)
@@ -122,6 +134,16 @@ class _NativePerceptualLoss(torch.autograd.Function):
         return grad_output * grad, None, None, None
 
 
+def tile_arg(text: str):
+    """The argparse type of --tile, --grad-tile and --perceptual-tile: "auto", or an int (checked where it is used)."""
+    if text == AUTO_TILE:
+        return text
+    try:
+        return int(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"expected {AUTO_TILE!r} or an integer, got {text!r}") from None
+
+
 def add_perceptual_args(ap) -> None:
     """``--perceptual {torch,native}``, ``--perceptual-tile N`` and ``--perceptual-precision {bf16x3,bf16}`` of train.py
     and score.py."""
@@ -129,9 +151,10 @@ def add_perceptual_args(ap) -> None:
                     help="(Optional) torch: the perceptual loss as the torch VGG19 expression (default); native: the "
                          "loss and its gradient on the library's kernels in overlapping windows "
                          "(PerceptualModel(native=True)), memory bounded by one pass")
-    ap.add_argument("--perceptual-tile", type=int, default=None, metavar="N",
+    ap.add_argument("--perceptual-tile", type=tile_arg, default=None, metavar="N|auto",
                     help="(Optional) needs --perceptual native: windows owning N x N input pixels of VGG features "
-                         "(rounded up to a multiple of 16).  Unset: one window per image")
+                         "(rounded up to a multiple of 16).  auto: one window per image where that fits half the "
+                         "card's memory, else N = 998, chosen per call.  Unset: one window per image")
     ap.add_argument("--perceptual-precision", default=None, choices=sorted(TRAIN_PRECISIONS),
                     help="(Optional) needs --perceptual native: the arithmetic of the VGG convolutions "
                          "(PerceptualModel.precision), bf16x3 (default, three bf16 tensor-core products per product) "
@@ -144,7 +167,7 @@ def perceptual_model(args) -> PerceptualModel:
     arithmetic)."""
     if args.perceptual_tile is not None and args.perceptual != "native":
         raise SystemExit("--perceptual-tile needs --perceptual native")
-    if args.perceptual_tile is not None and args.perceptual_tile <= 0:
+    if args.perceptual_tile not in (None, AUTO_TILE) and args.perceptual_tile <= 0:
         raise SystemExit("--perceptual-tile must be positive")
     if args.perceptual_precision is not None and args.perceptual != "native":
         raise SystemExit("--perceptual-precision needs --perceptual native")
