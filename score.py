@@ -27,6 +27,7 @@ def main():
                                                             "score.py (:96); scoring runs one validation pass")
     ap.add_argument("--synthetic", action="store_true")
     T.add_perceptual_args(ap)
+    T.add_metrics_arg(ap)
     args = ap.parse_args()
     assert args.weights is not None, "No weights specified in --weights!"
     if args.seed is not None:
@@ -46,7 +47,7 @@ def main():
     model.load_state_dict(torch.load(args.weights, map_location="cpu"))
     model.to(device).eval()
     vgg = T.perceptual_model(args).to(device).eval()
-    metrics = T.eval_one_epoch(model, loader, vgg, device)
+    metrics = T.eval_one_epoch(model, loader, vgg, device, native_metrics=args.metrics == "native")
     print("    Val   ||", "   ".join(f"{k}: {v:.03g}" for k, v in metrics.items()))
     print(f"Total time: {timer() - start}s")
 

@@ -49,6 +49,7 @@ def main():
                          "images through WaterNet.forward_many.  With --synthetic: a mix of sizes around "
                          "--height x --width")
     T.add_perceptual_args(ap)
+    T.add_metrics_arg(ap)
     args = ap.parse_args()
     if args.native_size and args.loader != "gpu":
         raise SystemExit("--native-size needs --loader gpu (ragged batches are assembled on the device)")
@@ -94,11 +95,13 @@ def main():
     scheduler = torch.optim.lr_scheduler.StepLR(optimizer, step_size=10000, gamma=0.1)
     vgg = T.perceptual_model(args).to(device).eval()
 
+    native_metrics = args.metrics == "native"
     train_hist, val_hist = [], []
     for epoch in range(args.epochs):
         print(f"Epoch {epoch + 1}/{args.epochs}")
-        tm = T.train_one_epoch(model, train_loader, optimizer, scheduler, vgg, device, log=print)
-        vm = T.eval_one_epoch(model, val_loader, vgg, device)
+        tm = T.train_one_epoch(model, train_loader, optimizer, scheduler, vgg, device, log=print,
+                               native_metrics=native_metrics)
+        vm = T.eval_one_epoch(model, val_loader, vgg, device, native_metrics=native_metrics)
         print("    Train ||", "   ".join(f"{k}: {v:.03g}" for k, v in tm.items()))
         print("    Val   ||", "   ".join(f"{k}: {v:.03g}" for k, v in vm.items()))
         train_hist.append(tm)
@@ -108,7 +111,7 @@ def main():
     T.save_metrics(savedir, train_hist, val_hist, {
         "epochs": args.epochs, "batch_size": args.batch_size, "im_height": args.height, "im_width": args.width,
         "weights": args.weights, "native_size": args.native_size, "grad_tile": args.grad_tile,
-        "train_precision": args.train_precision, **T.perceptual_config(args)})
+        "train_precision": args.train_precision, **T.perceptual_config(args), **T.metrics_config(args)})
     print(f"Metrics and weights saved to {savedir}")
     print(f"Total time: {timer() - start}s")
 

@@ -42,6 +42,15 @@ class RaggedTensors(ctypes.Structure):
 RAGGED_TENSORS_BYTES = 176  # sizeof(wn_ragged_tensors), asserted in csrc/api.cu
 
 
+class QualityImage(ctypes.Structure):
+    """wn_quality_image: one (out, ref) pair of a wn_quality call, fp32 contiguous (3,H,W) device pointers, its size
+    and its group (the images sharing SSIM's data range)."""
+    _fields_ = [("out", c_void_p), ("ref", c_void_p), ("height", c_int), ("width", c_int), ("group", c_int)]
+
+
+QUALITY_STATS = 7  # WN_QUALITY_STATS: float64 statistics per image of wn_quality
+
+
 # name -> (restype, argtypes); mirrors include/waternet_b200.h one to one
 _SIGNATURES = {
     "wn_abi_version": (c_int, []),
@@ -155,7 +164,14 @@ _SIGNATURES = {
     "wn_read_timings": (c_int, [c_void_p, POINTER(c_float), POINTER(c_int)]),
 }
 
-EXPORTED_SYMBOLS = tuple(_SIGNATURES)
+# ... and include/waternet_b200_metrics.h, the SSIM / PSNR statistics (csrc/metrics.cu)
+_METRICS_SIGNATURES = {
+    "wn_quality_workspace_bytes": (c_size_t, [POINTER(c_int), POINTER(c_int), c_int]),
+    "wn_quality": (c_int, [c_void_p, POINTER(QualityImage), c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+}
+
+EXPORTED_SYMBOLS = tuple(_SIGNATURES)                # the entry points of include/waternet_b200.h
+METRICS_SYMBOLS = tuple(_METRICS_SIGNATURES)         # ... of include/waternet_b200_metrics.h
 
 _lib = None
 
@@ -176,7 +192,7 @@ def load() -> ctypes.CDLL:
             "Run `python -m waternet_b200.build` (needs nvcc 12.9); there is no CPU fallback."
         )
     lib = ctypes.CDLL(path)
-    for name, (res, args) in _SIGNATURES.items():
+    for name, (res, args) in {**_SIGNATURES, **_METRICS_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args

@@ -50,7 +50,8 @@ def build(force: bool = False, verbose: bool = False, defines=(), lib_name: str 
     lib_path = os.path.join(PKG_DIR, lib_name)
     os.makedirs(obj_dir, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    headers.append(os.path.join(os.path.dirname(PKG_DIR), "include", "waternet_b200.h"))
+    include = os.path.join(os.path.dirname(PKG_DIR), "include")
+    headers += [os.path.join(include, f) for f in os.listdir(include) if f.endswith(".h")]
     objs = []
     for src in _sources():
         src_path = os.path.join(CSRC, src)

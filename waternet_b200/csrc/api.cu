@@ -1066,6 +1066,37 @@ int wn_debug_vgg_layer(wn_handle* h, const float* x, const int64_t strides[4], c
                          workspace_bytes, (cudaStream_t)stream);
 }
 
+// ---- SSIM / PSNR statistics (metrics.cu)
+static_assert(sizeof(wn_quality_image) == 32, "wn_quality_image: _lib.QualityImage restates this layout");
+
+size_t wn_quality_workspace_bytes(const int* heights_host, const int* widths_host, int n) {
+  const char* what = "wn_quality_workspace_bytes";
+  if (check_ptrs(what, {heights_host, widths_host}) || check_ragged_count(what, n)) return 0;
+  return quality_workspace_bytes(heights_host, widths_host, n);
+}
+
+int wn_quality(wn_handle* h, const wn_quality_image* images_host, int n, double* stats, void* workspace,
+               size_t workspace_bytes, void* stream) {
+  const char* what = "wn_quality";
+  int rc = check_ptrs(what, {h, images_host, stats, workspace});
+  if (rc || (rc = check_ragged_count(what, n)) ||
+      (rc = check_images(what, images_host, n, true, [](const wn_quality_image& im, int) { return im.out && im.ref; })))
+    return rc;
+  for (int i = 0; i < n; i++)
+    if (images_host[i].group < 0 || images_host[i].group >= n) {
+      set_error("%s: image %d: group %d outside 0..%d", what, i, images_host[i].group, n - 1);
+      return WN_E_INVALID;
+    }
+  if ((uintptr_t)stats % alignof(double)) return invalid(what, "stats is not 8-byte aligned");
+  std::vector<int> hs, ws;
+  ragged_sizes(images_host, n, &hs, &ws);
+  if ((rc = quality_plan_check(hs.data(), ws.data(), n, what)) ||
+      (rc = check_workspace(what, workspace_bytes, quality_workspace_bytes(hs.data(), ws.data(), n))))
+    return rc;
+  DeviceGuard guard(h->device);
+  return quality(h, images_host, n, stats, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 int wn_enable_timing(wn_handle* h, int on) {
   int rc = check_ptrs("wn_enable_timing", {h}, "null handle");
   if (rc) return rc;

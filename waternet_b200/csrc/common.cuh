@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "../../include/waternet_b200.h"
+#include "../../include/waternet_b200_metrics.h"
 #include "tiling.cuh"
 
 namespace wn {
@@ -410,5 +411,12 @@ int vgg_perceptual_loss(wn_handle* h, const float* out, const int64_t out_stride
 int vgg_debug_layer(wn_handle* h, const float* x, const int64_t strides[4], const float* ref,
                     const int64_t ref_strides[4], int n, int height, int width, int tile_h, int tile_w, int layer,
                     float* dst, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+
+// metrics.cu: SSIM / PSNR statistics (wn_quality).  quality_plan_check refuses sides below 6 and calls too large;
+// quality runs on arguments the caller has checked (api.cu).  The workspace function returns 0 where the check fails.
+int quality_plan_check(const int* hs, const int* ws, int n, const char* what);
+size_t quality_workspace_bytes(const int* hs, const int* ws, int n);
+int quality(wn_handle* h, const wn_quality_image* images, int n, double* stats, void* workspace,
+            size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace wn

@@ -1165,3 +1165,36 @@ class Engine:
                    _strides((r,)) if r is not None else None, n, h, w, th, tw, int(layer), dst.data_ptr(),
                    ws.data_ptr(), ws.numel())
         return dst
+
+    # ---- SSIM / PSNR statistics (wn_quality) ------------------------------------------------------------------
+    def quality_workspace_bytes(self, sizes) -> int:
+        """Workspace of one ``quality`` call over images of ``sizes`` [(h, w), ...]; 0 for rejected sizes."""
+        return int(self.lib.wn_quality_workspace_bytes(*_sizes(sizes), len(sizes)))
+
+    def quality(self, outs, refs, groups) -> torch.Tensor:
+        """The SSIM / PSNR statistics of the pairs (outs[i], refs[i]) in one wn_quality call: (3,H_i,W_i) fp32
+        contiguous CUDA tensors, image i in group ``groups[i]`` (images of one group share SSIM's data range).
+        Returns a (n, 7) float64 tensor, per image: the SSIM sum over its counted pixels, their count, the sum of
+        squared differences, min and max of out, min and max of ref."""
+        n = len(outs)
+        if n == 0 or len(refs) != n or len(groups) != n:
+            raise ValueError(f"expected as many refs and groups as outs (at least one), got {n}, {len(refs)}, "
+                             f"{len(groups)}")
+        for o, r in zip(outs, refs):
+            for t in (o, r):
+                if t.device != self.device or t.dtype != torch.float32 or t.dim() != 3 or t.shape[0] != 3 or \
+                        not t.is_contiguous():
+                    raise ValueError(f"expected fp32 contiguous (3,H,W) tensors on {self.device}, got "
+                                     f"{t.dtype} {tuple(t.shape)} on {t.device}")
+            if o.shape != r.shape:
+                raise ValueError(f"out and ref differ in shape: {tuple(o.shape)} vs {tuple(r.shape)}")
+        table = (_lib.QualityImage * n)()
+        for d, o, r, g in zip(table, outs, refs, groups):
+            d.out, d.ref, d.height, d.width, d.group = o.data_ptr(), r.data_ptr(), o.shape[1], o.shape[2], int(g)
+        sizes = [tuple(o.shape[1:]) for o in outs]
+        ws = self._workspace("quality", _require_workspace(
+            self.quality_workspace_bytes(sizes), f"quality: unsupported sizes {sizes}: 1..65535 images, each side at "
+                                                 "least 6 and at most 0x7fffffff / 3 pixels per plane"))
+        stats = torch.empty((n, _lib.QUALITY_STATS), dtype=torch.float64, device=self.device)
+        self._call("wn_quality", table, n, stats.data_ptr(), ws.data_ptr(), ws.numel())
+        return stats

@@ -4,6 +4,8 @@
 sigma 1.5, k1 0.01, k2 0.03, data range inferred as max(preds.max()-preds.min(),
 target.max()-target.min()), reflect padding cropped away, mean over the batch.
 ``peak_signal_noise_ratio(preds, target, data_range=1)``: 10*log10(1/mse) over all elements.
+
+``native_quality`` computes the same two numbers on the library's kernels (``wn_quality``, DESIGN.md 4.16).
 """
 from __future__ import annotations
 
@@ -41,3 +43,56 @@ def ssim(preds: torch.Tensor, target: torch.Tensor, kernel_size: int = 11, sigma
 def psnr(preds: torch.Tensor, target: torch.Tensor, data_range: float = 1.0) -> torch.Tensor:
     mse = torch.mean((preds - target) ** 2)
     return 10.0 * torch.log10(data_range ** 2 / mse)
+
+
+def _check_pair(o, r, what: str) -> None:
+    """ValueError unless ``o`` and ``r`` are (N,3,H,W) of one shape with both sides above 5 (the reflect padding of
+    ``ssim`` refuses a side of 5 or less)."""
+    if o.dim() != 4 or o.shape[1] != 3 or o.shape != r.shape:
+        raise ValueError(f"{what}: expected out and ref of one (N,3,H,W) shape, got {tuple(o.shape)} and "
+                         f"{tuple(r.shape)}")
+    if o.shape[0] == 0:
+        raise ValueError(f"{what}: empty batch")
+    if min(o.shape[2:]) <= 5:
+        raise ValueError(f"{what}: padding size should be less than the corresponding input dimension, but got "
+                         f"padding (5, 5) for input {list(o.shape)}: both sides must be at least 6")
+
+
+def native_quality(out, ref):
+    """(SSIM, PSNR) as ``training.batch_quality`` computes them, from one ``wn_quality`` call (two launches, no
+    per-pixel scratch), as 0-d float64 CUDA tensors.
+
+    ``out``, ``ref``: (N,3,H,W) tensors, one group sharing SSIM's data range: ``ssim`` and ``psnr``.  Or two lists
+    of (N_i,3,H_i,W_i) tensors, each item its own group: the mean of the items' SSIMs, and the PSNR of the squared
+    error pooled over every element.  Shapes are checked first (ValueError, as ``ssim`` refuses them); CPU tensors
+    raise WaterNetLibraryError: there is no CPU path.  SSIM's separable window rounds differently from the 121-tap
+    convolution of ``ssim`` (DESIGN.md 4.16 states the bar against float64); the statistics of an item do not depend
+    on the other items of the call, bit for bit."""
+    from .engine import get_engine
+
+    if isinstance(out, (list, tuple)):
+        if not isinstance(ref, (list, tuple)) or len(out) != len(ref) or not out:
+            raise ValueError("native_quality: expected two equally long, non-empty lists of (N_i,3,H_i,W_i) tensors")
+        items = list(zip(out, ref))
+    else:
+        items = [(out, ref)]
+    for k, (o, r) in enumerate(items):
+        _check_pair(o, r, f"native_quality (item {k})" if len(items) > 1 else "native_quality")
+    eng = get_engine(items[0][0].device)
+    outs, refs, groups, counts = [], [], [], []
+    for k, (o, r) in enumerate(items):
+        if o.device != eng.device or r.device != eng.device:
+            raise ValueError(f"native_quality: every tensor must be on {eng.device}, item {k} is on {o.device} and "
+                             f"{r.device}")
+        o, r = (t.detach().to(torch.float32).contiguous() for t in (o, r))
+        outs += list(o)
+        refs += list(r)
+        groups += [k] * o.shape[0]
+        counts.append(o.shape[0])
+    stats = eng.quality(outs, refs, groups)
+    per_image = stats[:, 0] / stats[:, 1]
+    item = torch.tensor(groups, device=eng.device)
+    per_item = torch.zeros(len(items), dtype=torch.float64, device=eng.device).index_add_(0, item, per_image)
+    s = (per_item / torch.tensor(counts, dtype=torch.float64, device=eng.device)).mean()
+    elements = sum(o.numel() for o in outs)
+    return s, 10.0 * torch.log10(elements / stats[:, 2].sum())

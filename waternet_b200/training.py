@@ -4,8 +4,9 @@ The model's forward values and all of its gradients come from the CUDA library
 (``wn_forward_train`` / ``wn_backward``: tensor-core forward that keeps its activations, data-gradient and
 weight-gradient kernels; only ``precision="fp32"`` re-evaluates the torch graph for its backward).  The
 VGG19 perceptual loss is the torch expression by default; ``PerceptualModel(native=True)`` computes it and its
-gradient in overlapping windows on the library's kernels (``wn_perceptual_loss``).  Adam and the metrics stay
-PyTorch.
+gradient in overlapping windows on the library's kernels (``wn_perceptual_loss``).  SSIM and PSNR are the torch
+expressions of ``metrics`` by default; ``native=True`` (``--metrics native``) computes them with ``wn_quality``.
+Adam stays PyTorch.
 """
 from __future__ import annotations
 
@@ -20,7 +21,7 @@ import torch
 import torch.nn as nn
 
 from .engine import AUTO_TILE, Engine, is_auto
-from .metrics import psnr, ssim
+from .metrics import native_quality, psnr, ssim
 from .net import TRAIN_PRECISIONS, _PackedWeightsMixin
 
 TRAIN_METRICS_NAMES = ["mse", "ssim", "psnr", "perceptual_loss", "loss"]
@@ -175,6 +176,18 @@ def perceptual_model(args) -> PerceptualModel:
                            precision=perceptual_config(args)["perceptual_precision"])
 
 
+def add_metrics_arg(ap) -> None:
+    """``--metrics {torch,native}`` of train.py and score.py."""
+    ap.add_argument("--metrics", default="torch", choices=["torch", "native"],
+                    help="(Optional) torch: SSIM and PSNR as the torch expressions (default); native: one wn_quality "
+                         "call per batch on the library's kernels, no per-pixel temporaries")
+
+
+def metrics_config(args) -> dict:
+    """The metric setting of ``add_metrics_arg`` as train.py records it in config.json."""
+    return {"metrics": args.metrics}
+
+
 def perceptual_config(args) -> dict:
     """The perceptual-loss settings of ``add_perceptual_args`` as train.py records them in config.json."""
     return {"perceptual": args.perceptual, "perceptual_tile": args.perceptual_tile,
@@ -221,9 +234,12 @@ def batch_losses(vgg, out, ref):
     return (0.05 * perc + mse).mean(), perc.mean(), mse.mean()
 
 
-def batch_quality(out, ref):
+def batch_quality(out, ref, native: bool = False):
     """(SSIM, PSNR) of a batch.  For lists of images: the mean of the per-image SSIMs, and the PSNR of the MSE
-    pooled over every pixel of every image."""
+    pooled over every pixel of every image.  ``native``: both from one ``metrics.native_quality`` call (CUDA tensors
+    only; float64 results)."""
+    if native:
+        return native_quality(out, ref)
     if not isinstance(out, list):
         return ssim(out, ref), psnr(out, ref, 1.0)
     s = torch.stack([ssim(o, r) for o, r in zip(out, ref)]).mean()
@@ -232,8 +248,10 @@ def batch_quality(out, ref):
     return s, 10.0 * torch.log10(1.0 / mse)
 
 
-def train_one_epoch(model, loader, optimizer, scheduler, vgg, device, log=None) -> Dict[str, float]:
-    """One epoch; a batch is five tensors, or five lists of images of their own sizes (GpuBatchLoader(ragged=True))."""
+def train_one_epoch(model, loader, optimizer, scheduler, vgg, device, log=None,
+                    native_metrics: bool = False) -> Dict[str, float]:
+    """One epoch; a batch is five tensors, or five lists of images of their own sizes (GpuBatchLoader(ragged=True)).
+    ``native_metrics``: SSIM and PSNR from ``batch_quality(native=True)``."""
     model.train()
     totals = {k: 0.0 for k in TRAIN_METRICS_NAMES}
     for idx, batch in enumerate(loader):
@@ -245,7 +263,7 @@ def train_one_epoch(model, loader, optimizer, scheduler, vgg, device, log=None) 
         optimizer.step()
         scheduler.step()  # per minibatch, like the reference (train.py:133)
         with torch.no_grad():
-            s, p = batch_quality(out, ref)
+            s, p = batch_quality(out, ref, native_metrics)
             totals["loss"] += loss.item()
             totals["perceptual_loss"] += perc.item()
             totals["mse"] += mse.item()
@@ -256,9 +274,9 @@ def train_one_epoch(model, loader, optimizer, scheduler, vgg, device, log=None) 
     return {k: v / max(len(loader), 1) for k, v in totals.items()}
 
 
-def eval_one_epoch(model, loader, vgg, device) -> Dict[str, float]:
+def eval_one_epoch(model, loader, vgg, device, native_metrics: bool = False) -> Dict[str, float]:
     """Validation pass; the perceptual loss is averaged over batches (the reference logs only the
-    last batch divided by the batch count, train.py:71-74)."""
+    last batch divided by the batch count, train.py:71-74).  ``native_metrics`` as ``train_one_epoch``."""
     model.eval()
     totals = {k: 0.0 for k in VAL_METRICS_NAMES}
     with torch.no_grad():
@@ -266,7 +284,7 @@ def eval_one_epoch(model, loader, vgg, device) -> Dict[str, float]:
             raw, wb, he, gc, ref = _to_device(batch, device)
             out = _forward(model, raw, wb, he, gc)
             _, perc, mse = batch_losses(vgg, out, ref)
-            s, p = batch_quality(out, ref)
+            s, p = batch_quality(out, ref, native_metrics)
             totals["perceptual_loss"] += perc.item()
             totals["mse"] += mse.item()
             totals["ssim"] += s.item()
