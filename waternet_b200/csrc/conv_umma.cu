@@ -6,8 +6,8 @@
 // (SURVEY.md section 0).  Each fp32 operand is split into bf16 hi + lo and
 // hi*hi + lo*w + hi*w_lo accumulates in fp32 registers: as three bf16 MMAs ("bf16x3",
 // ~2^-16 relative operand error), or -- the default for the tensor-bound layers -- as
-// one bf16 MMA plus ONE fp8 (e4m3) MMA of K = 32 for both correction terms
-// (UmmaCfg FMT in umma_conv.cuh; DESIGN.md 4.2).
+// one bf16 MMA plus ONE fp8 (e4m3) MMA of K = 32 for both correction terms, all of a tile's e4m3 MMAs first, into
+// the one accumulator (UmmaCfg FMT in umma_conv.cuh; DESIGN.md 4.2).
 //
 // Data layout in HBM: activations are bf16 planes of 8 channels,
 //     act[n][plane][y][x][8]   planes [0, C/8) = hi parts, [C/8, 2C/8) = lo parts,
@@ -20,7 +20,7 @@
 //
 // One persistent CTA per SM, warp-specialised:
 //   warps 0-7  two consumer warpgroups (kSpecs wgs 2; wgs 3: warps 0-11, three): each issues the m64 wgmmas of its
-//              8 rows of the 8x16-, 16x16- or 8x24-pixel tile (accumulators in registers; kSpecs mw, ng) and then
+//              8 rows of the 8x16-, 16x16-, 8x24- or 16x24-pixel tile (accumulators in registers; kSpecs mw, ng) and then
 //              runs the epilogue of those pixels
 //              (registers -> shared-memory transpose -> bias/act -> bf16 hi/lo planes or fp32)
 //   warp 8     A producer (TMA halo tiles, one 16-channel chunk per stage); wgs 3: warp 12
@@ -170,10 +170,11 @@ enum UmmaLayer {
 // per diagonal block; concat = CONCAT of the bf16x3 form, set where the a_hi x [w_hi | w_lo] product fits one wgmma
 // (N = 2 * NPAD <= 256); slot = timing slot, the state-dict index of the layer's (first) convolution; f8 = the layer
 // has an fp8-correction form (UmmaCfg FMT bit 0, the tensor-bound layers), which uses CONCAT 0.  mw = m64 blocks per
-// warpgroup (2: 16 x 16-pixel tiles, which halve the weight bytes streamed per pixel) and ng = column groups of npad /
-// ng channels each (UmmaCfg MW, NG): at mw = 2 the accumulators of both blocks must fit in 128 registers per thread.
-// wgs = consumer warpgroups (UmmaCfg WGS): 3 gives 8 x 24-pixel tiles, which cut the weight bytes streamed per pixel
-// by a third at mw = 1; a layer takes it where its kernels stay free of spills at 160 registers and measure faster.
+// warpgroup (2: 16-pixel-wide tiles, which halve the weight bytes streamed per pixel) and ng = column groups of npad /
+// ng channels each (UmmaCfg MW, NG): at mw = 2 the accumulators of both blocks must fit in 128 registers per thread
+// in every form (R2's bf16x3 form, CONCAT over three blocks, holds 96 per block).
+// wgs = consumer warpgroups (UmmaCfg WGS): 3 gives 24-row tiles, which cut the weight bytes streamed per pixel by a
+// third; a layer takes it where its kernels stay free of spills at 160 registers and measure faster.
 // Every layer also has a single-pass bf16 form (UmmaCfg FMT kFmtHi, the WN_MODE_BF16 training forward, kRL1 included):
 // the bf16x3 weight images, hi rows only, at the layer's own mw, ng and wgs.  It needs no more registers than the
 // bf16x3 form (a CONCAT layer's accumulators halve: N = npad instead of 2 * npad).
@@ -185,12 +186,12 @@ struct UmmaLayerSpec {
 static constexpr UmmaLayerSpec kSpecs[kNumUmmaLayers] = {
     // ks cinpad npad epi       concat nblk tps slot f8  mw ng wgs
     {7, 16, 224, kEpiAct, 0, 1, 1, 0, false, 1, 1, 2},     // kL1
-    {5, 128, 128, kEpiAct, 0, 1, 5, 1, true, 1, 1, 2},     // kC2
+    {5, 128, 128, kEpiAct, 0, 1, 5, 1, true, 1, 1, 3},     // kC2
     {3, 128, 128, kEpiAct, 0, 1, 3, 2, true, 1, 1, 3},     // kC3
     {1, 128, 64, kEpiAct, 1, 1, 1, 3, false, 1, 1, 3},     // kC4
     {7, 64, 64, kEpiAct, 1, 1, 7, 4, true, 2, 1, 2},       // kC5
-    {5, 64, 64, kEpiAct, 1, 1, 5, 5, true, 2, 1, 2},       // kC6
-    {3, 64, 64, kEpiAct, 1, 1, 9, 6, true, 2, 1, 2},       // kC7
+    {5, 64, 64, kEpiAct, 1, 1, 5, 5, true, 2, 1, 3},       // kC6
+    {3, 64, 64, kEpiAct, 1, 1, 9, 6, true, 2, 1, 3},       // kC7
     {3, 64, 16, kEpiSigmoid, 1, 1, 9, 7, false, 1, 1, 3},  // kC8
     {5, 96, 32, kEpiAct, 1, 3, 5, 9, true, 1, 1, 3},       // kR2
     {3, 96, 16, kEpiGate, 1, 1, 9, 10, false, 1, 1, 3},    // kR3
@@ -325,7 +326,7 @@ int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t str
       WN_LAUNCH_CHECK(h);
       for (int g = 0; g < s.ng; g++) {
         pack_stages_f8_kernel<<<256, 256, 0, stream>>>(u->dense, u->stages8[li] + g * group_bytes, u->scale8[li], gw,
-                                                       s.cinpad, kk, s.nblk, g * gw);
+                                                       s.cinpad, kk, s.tps, s.nblk, g * gw);
         WN_LAUNCH_CHECK(h);
       }
     }

@@ -109,8 +109,12 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 //        used to be) by [e4m3(w * ws) ; e4m3(w_lo * ws * 2^9)]: 2 pass-equivalents instead of 3 at half the
 //        operand bytes.  The bf16 weights of such a layer are packed pre-scaled by the power of two ws * 2^9
 //        (exact), so the two products carry the same scale and the epilogue multiplies their sum by 2^-9 / ws once.
-//        The fp8 product accumulates in registers of its own: Hopper's fp8 wgmma adds with fewer mantissa bits
-//        than fp32, which is harmless for the small correction terms but not for the main product.
+//        Both products go into ONE accumulator, in two phases per tile: the correction phase issues every chunk's
+//        e4m3 wgmmas, then the main phase every chunk's bf16 a_hi x w_hi.  Hopper's fp8 wgmma adds with fewer mantissa
+//        bits than fp32; in this order it only ever adds into correction sums (about 2^-8 of the result), never into
+//        the main product.  Each phase walks the chunks in pairs: a halo stage holds the two planes of each chunk of
+//        a pair that the phase reads, a weight stage the phase's 32-byte-per-channel units of TPS taps of both chunks
+//        (pack_stages_f8_kernel), so stages keep the bytes and the wgmma count of the other forms.
 //        bit 1 (kFmtOut8): the epilogue writes that hi + fp8-planes format (its consumer has bit 0 set).
 //        bit 2 (kFmtHi): single-pass bf16 (WN_MODE_BF16, training only): ONE wgmma per product, a_hi x w_hi of
 //        N = NPAD (a CONCAT layer takes the hi rows of its [hi | lo] stage rows), fp32 accumulation.  The a_lo and w_lo
@@ -163,11 +167,17 @@ struct UmmaCfg {
   static constexpr int HALO_W = TILE_W + KS - 1, HALO_H = TILE_H + KS - 1;
   static constexpr int NCHUNK = CIN_PAD / 16;
   static constexpr int PLANE_BYTES = HALO_W * HALO_H * 16;
-  static constexpr int A_STAGE = (4 * PLANE_BYTES + 1023) / 1024 * 1024;  // hi k0, hi k1, lo k0, lo k1
-  // one tap of weights: [hi|lo][k8 0|1][NPAD][16 B] (CONCAT: [k8][hi rows | lo rows]; fp8 scheme: bf16 part
-  // [k8][NPAD][16 B] then fp8 part [k16 half][NPAD][16 B]) -- 64 B per output channel in every form
-  static constexpr int B_TAP = NPAD * 64;
-  static constexpr int B_STAGE = TPS * B_TAP;
+  // hi k0, hi k1, lo k0, lo k1; F8IN: the two planes its phase reads of each chunk of a pair (fp8 or hi planes)
+  static constexpr int A_STAGE = (4 * PLANE_BYTES + 1023) / 1024 * 1024;
+  // one tap of weights: [hi|lo][k8 0|1][NPAD][16 B] (CONCAT: [k8][hi rows | lo rows]) -- 64 B per output channel;
+  // fp8 scheme: one phase's unit of a tap, [k16 half][NPAD][16 B] e4m3 or [k8][NPAD][16 B] bf16 -- 32 B, and a
+  // stage holds TPS taps of both chunks of a pair
+  static constexpr int B_TAP = NPAD * (F8IN ? 32 : 64);
+  static constexpr int B_STAGE = (F8IN ? 2 : 1) * TPS * B_TAP;
+  // kFmtFuse1x1: the layer's NPAD outputs are the 1x1 layer's 16-channel chunks; its weight stages are those of a
+  // CONCAT launch (64 B per output channel and chunk for [w_hi | w_lo])
+  static constexpr int FUSE_CHUNKS = NPAD / 16 / kFuseStages;  // chunks of the 1x1 layer per weight stage
+  static constexpr int FUSE_STAGE = FUSE_CHUNKS * kFuseNpad * 64;
   static_assert((KS * KS) % TPS == 0, "taps per weight stage must divide the filter");
   static constexpr int NSTAGE_PER_CHUNK = KS * KS / TPS;
   static constexpr int STAGING = WGS * 64 * kStageLd * 4;
@@ -194,26 +204,22 @@ struct UmmaCfg {
   static constexpr int PAIR_UNITS = PAIRS + KS * KS;        // units of NPAD * 32 B: e4m3 pairs, then bf16 taps
   static constexpr int PAIR_STAGES = PAIR_UNITS / 2;        // two units per weight stage of B_STAGE bytes
   static_assert(!PAIR || PAIR_UNITS % 2 == 0, "whole weight stages");
-  // kFmtFuse1x1: the layer's NPAD outputs are the 1x1 layer's 16-channel chunks; its weight stages are those of a
-  // CONCAT launch (64 B per output channel and chunk for [w_hi | w_lo])
-  static constexpr int FUSE_CHUNKS = NPAD / 16 / kFuseStages;  // chunks of the 1x1 layer per weight stage
-  static constexpr int FUSE_STAGE = FUSE_CHUNKS * kFuseNpad * 64;
   static_assert(!FUSE || (!CONCAT && NBLK == 1 && MW == 1 && NG == 1 && !HI && !PAIR && FUSE_STAGE <= B_STAGE &&
                           NPAD % (16 * kFuseStages) == 0), "the fused 1x1 layer follows a plain layer of one block");
   static constexpr int CPB = NCHUNK / NBLK;                // chunks per diagonal block
   static constexpr int BLK_COLS = DUAL ? 2 * NPAD : NPAD;   // accumulator columns per block
   static constexpr int COLS = NBLK * BLK_COLS;             // accumulator columns of the tile
   static constexpr int ACC = COLS / 2;                     // fp32 accumulator registers per thread (M = 64 per warpgroup)
-  static constexpr int ACC8 = F8IN ? ACC : 1;              // ... of the fp8 correction product
   static constexpr int SMEM_BYTES = NA * A_STAGE + NB * B_STAGE + STAGING + TAIL + 1024;  // + barriers/bias + align slack
   static_assert(NA >= 1, "halo tile does not fit in shared memory");
   static_assert(NCHUNK % NBLK == 0, "chunks must split evenly over the diagonal blocks");
   static_assert(NPAD % 16 == 0 && (DUAL ? 2 : 1) * NPAD <= 256, "invalid wgmma N");
   static_assert(MW == 1 || MW == 2, "one or two m64 blocks per warpgroup");
-  static_assert(WGS == 2 || (WGS == 3 && MW == 1), "two consumer warpgroups, or three of one m64 block each");
+  static_assert(WGS == 2 || WGS == 3, "two or three consumer warpgroups");
   static_assert(NG == 1 || NBLK == 1, "column groups of a block-diagonal layer");
-  static_assert(MW * (ACC + (F8IN ? ACC8 : 0)) <= 128, "accumulators do not fit in registers");
-  // full weight image of one column group: every (chunk, stage)
+  static_assert(MW * ACC <= 128, "accumulators do not fit in registers");
+  static_assert(!F8IN || CPB % 2 == 0, "fp8 corrections: chunk pairs of one diagonal block");
+  // full weight image of one column group: every (chunk, stage); F8IN: every (phase, chunk pair, stage)
   static constexpr size_t GROUP_BYTES = (size_t)NCHUNK * NSTAGE_PER_CHUNK * B_STAGE;
 };
 
@@ -501,11 +507,18 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
         for (int c = 0; c < C::NCHUNK; c++) {
           mbar_wait(&a_empty[stage], phase ^ 1);
           uint8_t* dst = a_stages + stage * C::A_STAGE;
-          // kFmtHi never reads the lo planes
-          mbar_expect_tx(&a_full[stage], (C::HI || g.a_hi_only ? 2 : 4) * C::PLANE_BYTES);
-          tma_load_5d(dst, &tmap_in, &a_full[stage], 0, x0, y0, 2 * c, n);
-          if (!C::HI && !g.a_hi_only)
-            tma_load_5d(dst + 2 * C::PLANE_BYTES, &tmap_in, &a_full[stage], 0, x0, y0, g.in_planes_half + 2 * c, n);
+          if constexpr (F8IN) {  // step c < NCHUNK / 2: the fp8 planes of chunks 2c, 2c + 1; then their hi planes
+            mbar_expect_tx(&a_full[stage], 4 * C::PLANE_BYTES);
+            const int plane = c < C::NCHUNK / 2 ? g.in_planes_half + 4 * c : 4 * (c - C::NCHUNK / 2);
+            tma_load_5d(dst, &tmap_in, &a_full[stage], 0, x0, y0, plane, n);
+            tma_load_5d(dst + 2 * C::PLANE_BYTES, &tmap_in, &a_full[stage], 0, x0, y0, plane + 2, n);
+          } else {
+            // kFmtHi never reads the lo planes
+            mbar_expect_tx(&a_full[stage], (C::HI || g.a_hi_only ? 2 : 4) * C::PLANE_BYTES);
+            tma_load_5d(dst, &tmap_in, &a_full[stage], 0, x0, y0, 2 * c, n);
+            if (!C::HI && !g.a_hi_only)
+              tma_load_5d(dst + 2 * C::PLANE_BYTES, &tmap_in, &a_full[stage], 0, x0, y0, g.in_planes_half + 2 * c, n);
+          }
           if (++stage == C::NA) { stage = 0; phase ^= 1; }
         }
       }
@@ -539,14 +552,12 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
   // ===================== consumers: wgmma, then the epilogue of the warpgroup's 64 rows =====================
   const int wg = warp >> 2, wtid = tid & 127;
   const bool skip_lo = levels;
-  // WGS = 3 reads the fp8 dequantisation factor in the epilogue: one register less across the main loop
-  const float dscale0 = F8IN && WGS == 2 ? *g.f8_scale : 1.f;
   // A operand: rows of the tile = pixels, 8 consecutive pixels of a halo row = one core matrix; this warpgroup's
   // rows start 8 halo rows further, its second m64 block 8 pixels (128 B) further along the same halo rows.  K halves
   // (channels 0-7 / 8-15 of the chunk) are one plane apart.
   constexpr uint32_t kSboA = C::HALO_W * 16;
   constexpr uint32_t kLboB = (CONCAT ? 2 * NPAD : NPAD) * 16;
-  float acc[MW][C::ACC], acc8[MW][C::ACC8];
+  float acc[MW][C::ACC];
   int astage = 0, bstage = 0, pend_a = -1, pend_b = -1;
   uint32_t aphase = 0, bphase = 0;
   // a stage may be refilled once the wgmma groups reading it have completed: the release of a stage waits for
@@ -564,15 +575,17 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     for (int mb = 0; mb < MW; mb++) {
 #pragma unroll
       for (int i = 0; i < C::ACC; i++) acc[mb][i] = 0.f;
-#pragma unroll
-      for (int i = 0; i < C::ACC8; i++) acc8[mb][i] = 0.f;
     }
-    // unrolled: the diagonal block a chunk feeds (which accumulator registers its wgmmas write) is a constant
+    // unrolled: the diagonal block a chunk feeds (which accumulator registers its wgmmas write) is a constant.
+    // F8IN: step c is chunk pair c % (NCHUNK / 2) of the correction phase (c < NCHUNK / 2), then of the main phase:
+    // every e4m3 wgmma of the tile comes first, so that while the fp8 MMA, which adds with fewer bits than fp32, adds
+    // into the accumulator, it holds only correction sums (about 2^-8 of the result)
 #pragma unroll
     for (int c = 0; c < C::NCHUNK; c++) {
+      const bool corr = F8IN && c < C::NCHUNK / 2;
       mbar_wait(&a_full[astage], aphase);
       const uint32_t a_base = smem_u32(a_stages + astage * C::A_STAGE) + (uint32_t)(wg * 8 * C::HALO_W * 16);
-      const int blk = NBLK > 1 ? c / C::CPB : 0;
+      const int blk = NBLK > 1 ? (F8IN ? 2 * (c % (C::NCHUNK / 2)) : c) / C::CPB : 0;
       if constexpr (C::PAIR) {
         if (pair) {
           // the e4m3 operand: warpgroup wg converts the two hi planes of its 14 halo rows (8 wg ..) into plane 2 + wg
@@ -666,9 +679,17 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
                   if constexpr (C::HI) {
                     wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));                // a_hi x w_hi
                   } else if constexpr (F8IN) {
-                    // w_hi * ws * 2^9 (bf16, K = 16), then [e4m3(lo*2^9) | e4m3(v)] x [e4m3(w*ws) ; e4m3(w_lo*ws*2^9)] (K = 32)
-                    wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, NPAD * 16, 128));
-                    wgmma_e4m3<NPAD>(acc8[mb] + b * C::BLK_COLS / 2, a_lo, make_desc(b_tap + NPAD * 32, NPAD * 16, 128));
+                    // chunk 2p (planes 0-1, a_hi) and chunk 2p + 1 (planes 2-3, a_lo) of the pair, each one of the
+                    // phase's units: [e4m3(lo*2^9) | e4m3(v)] x [e4m3(w*ws) ; e4m3(w_lo*ws*2^9)] (K = 32), then
+                    // a_hi x w_hi * ws * 2^9 (bf16, K = 16)
+                    const uint32_t b_odd = b_tap + TPS * C::B_TAP;
+                    if (corr) {
+                      wgmma_e4m3<NPAD>(d, a_hi, make_desc(b_tap, NPAD * 16, 128));
+                      wgmma_e4m3<NPAD>(d, a_lo, make_desc(b_odd, NPAD * 16, 128));
+                    } else {
+                      wgmma_bf16<NPAD>(d, a_hi, make_desc(b_tap, NPAD * 16, 128));
+                      wgmma_bf16<NPAD>(d, a_lo, make_desc(b_odd, NPAD * 16, 128));
+                    }
                   } else if constexpr (CONCAT) {
                     wgmma_bf16<2 * NPAD>(d, a_hi, make_desc(b_tap, kLboB, 128));            // a_hi x [w_hi | w_lo]
                     if (!skip_lo) wgmma_bf16<NPAD>(d, a_lo, make_desc(b_tap, kLboB, 128));  // a_lo x w_hi
@@ -700,14 +721,14 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     const int r = wtid & 63, half = wtid >> 6;
     const int m = wg * 64 + r;
     const int gy = ty * C::TILE_H + (m >> 3);
-    const float dscale = F8IN && WGS == 3 ? *g.f8_scale : dscale0;
+    const float dscale = F8IN ? *g.f8_scale : 1.f;
     // kFmtFuse1x1: the fused layer's A operands (hi / lo, 4 registers per K step) and the ring stages of its weights
     static_assert(!C::FUSE || kFuseNpad <= C::ACC, "the fused layer's accumulators take the place of this layer's");
     uint32_t a_hi[C::FUSE ? NPAD / 4 : 1], a_lo[C::FUSE ? NPAD / 4 : 1];
     int fuse_stage[kFuseStages];
     if constexpr (C::FUSE) {
-      // This layer's activation in the accumulator layout, with the fp32 operations of its kEpiAct epilogue (max((acc
-      // + acc8) dscale + b, 0), or max(acc + b, 0); __fmul_rn / __fadd_rn so that nothing contracts into an fma),
+      // This layer's activation in the accumulator layout, with the fp32 operations of its kEpiAct epilogue (max(acc
+      // dscale + b, 0), or max(acc + b, 0); __fmul_rn / __fadd_rn so that nothing contracts into an fma),
       // masked as a ragged slot masks it, and split into the bf16 hi / lo the 1x1 layer's own launch reads.  Register
       // 2j + h holds columns 8j + fcol, +1 of row frow + 8h: registers 4k .. 4k + 3 are the A fragment of K step k.
       bool row_valid[2] = {true, true};
@@ -726,7 +747,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
 #pragma unroll
           for (int e = 0; e < 2; e++) {
             float s = acc[0][4 * j + 2 * h + e];
-            if constexpr (F8IN) s = __fmul_rn(__fadd_rn(s, acc8[0][4 * j + 2 * h + e]), dscale);
+            if constexpr (F8IN) s = __fmul_rn(s, dscale);
             x[e] = fmaxf(__fadd_rn(s, s_bias[8 * j + fcol + e]), 0.f);
             if constexpr (RAG) x[e] = row_valid[h] ? x[e] : 0.f;
           }
@@ -786,7 +807,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
             for (int k = 0; k < 4; k++) {
               v[k] = acc[mb][col / 2 + k];
               if constexpr (EDUAL) v[k] += acc[mb][(col + ENPAD) / 2 + k];
-              if constexpr (EF8) v[k] = (v[k] + acc8[mb][col / 2 + k]) * dscale;
+              if constexpr (EF8) v[k] = v[k] * dscale;
               if constexpr (C::PAIR) v[k] = pair ? v[k] * s_bias[NPAD + col + fcol + (k & 1)] : v[k];
             }
             float* s = stg + frow * kStageLd + 8 * j + fcol;
@@ -867,12 +888,14 @@ static __global__ void pack_stages_kernel(const float* __restrict__ dense, __nv_
 }
 
 
-// fp8 correction scheme (UmmaCfg FMT bit 0): per (chunk, tap):
-//   part 0  [k8 0|1][rows][8 bf16]            w_hi * ws * 2^9              (K = 16 bf16 MMA)
-//   part 1  [k16 0|1][rows][16 fp8 (e4m3)]    w * ws  |  w_lo * ws * 2^9   (K = 32 fp8 MMA)
+// fp8 correction scheme (UmmaCfg FMT bit 0): units of rows * 32 B in the order the two phases of a tile read them,
+//   first one per (chunk, tap):  [k16 0|1][rows][16 fp8 (e4m3)]    w * ws  |  w_lo * ws * 2^9   (K = 32 fp8 MMA)
+//   then one per (chunk, tap):   [k8 0|1][rows][8 bf16]            w_hi * ws * 2^9              (K = 16 bf16 MMA)
+// Within a phase, unit (chunk, tap) is at ((pair * kk / tps + tap / tps) * 2 + chunk % 2) * tps + tap % tps, pair =
+// chunk / 2: a weight stage is tps taps of chunk 2 pair, then the same taps of chunk 2 pair + 1.
 // with rows = npad (dense rows from row_off on: one column group).  scale[0] = ws (a power of two placing max|w| in
 // [112, 224] over the whole layer),
-// scale[1] = 2^-9 / ws (what the epilogue multiplies the second accumulator with); scale[2] = max|w|.
+// scale[1] = 2^-9 / ws (what the epilogue multiplies the accumulator with); scale[2] = max|w|.
 // scale[2] (as unsigned bits) accumulates max|w| over the grid (bit patterns of non-negative floats are
 // ordered like the floats); f8_scale_finish_kernel turns it into scale[0], scale[1].
 static __global__ void f8_absmax_kernel(const float* __restrict__ dense, size_t n, float* __restrict__ scale) {
@@ -895,10 +918,10 @@ static __global__ void f8_scale_finish_kernel(float* __restrict__ scale) {
   scale[1] = 1.f / (512.f * ws);
 }
 static __global__ void pack_stages_f8_kernel(const float* __restrict__ dense, uint8_t* __restrict__ out,
-                                             const float* __restrict__ scale, int npad, int cinpad, int kk, int nblk,
-                                             int row_off) {
+                                             const float* __restrict__ scale, int npad, int cinpad, int kk, int tps,
+                                             int nblk, int row_off) {
   const int nchunk = cinpad / 16, cpb = nchunk / nblk, rows = npad;
-  const size_t tap_bytes = (size_t)rows * 64;
+  const size_t unit_bytes = (size_t)rows * 32;
   const float ws = scale[0];
   // one thread per (chunk, tap, row, channel pair of the chunk)
   const size_t total = (size_t)nchunk * kk * rows * 8;
@@ -918,8 +941,9 @@ static __global__ void pack_stages_f8_kernel(const float* __restrict__ dense, ui
       hb[t] = __bfloat16_as_ushort(h);
       wl[t] = w[t] - __bfloat162float(h);
     }
-    uint8_t* base = out + ((size_t)chunk * kk + tap) * tap_bytes;
-    // part 0: channel c = 2cp+t -> k8 = c / 8, element c % 8.  bf16(w) * (ws * 2^9): an exact power-of-two scaling
+    const size_t unit = ((size_t)(chunk / 2) * (kk / tps) + tap / tps) * 2 * tps + (chunk % 2) * tps + tap % tps;
+    uint8_t* base = out + ((size_t)nchunk * kk + unit) * unit_bytes;
+    // bf16 unit: channel c = 2cp+t -> k8 = c / 8, element c % 8.  bf16(w) * (ws * 2^9): an exact power-of-two scaling
     // that puts the bf16 product on the scale of the fp8 correction product (one shared accumulator)
     const int c = 2 * cp;
 #pragma unroll
@@ -927,8 +951,8 @@ static __global__ void pack_stages_f8_kernel(const float* __restrict__ dense, ui
       hb[t] = __bfloat16_as_ushort(__float2bfloat16_rn(__bfloat162float(__ushort_as_bfloat16(hb[t])) * ws * 512.f));
     *reinterpret_cast<uint32_t*>(base + ((size_t)(c / 8) * rows + row) * 16 + (c % 8) * 2) =
         (uint32_t)hb[0] | ((uint32_t)hb[1] << 16);
-    // part 1: K half 0 = e4m3(w * ws), K half 1 = e4m3(w_lo * ws * 512), 16 channels per row
-    uint8_t* p1 = base + (size_t)rows * 32;
+    // e4m3 unit: K half 0 = e4m3(w * ws), K half 1 = e4m3(w_lo * ws * 512), 16 channels per row
+    uint8_t* p1 = out + unit * unit_bytes;
     *reinterpret_cast<uint16_t*>(p1 + ((size_t)0 * rows + row) * 16 + c) = pack_e4m3x2(w[0] * ws, w[1] * ws);
     *reinterpret_cast<uint16_t*>(p1 + ((size_t)1 * rows + row) * 16 + c) =
         pack_e4m3x2(wl[0] * ws * 512.f, wl[1] * ws * 512.f);
