@@ -2,6 +2,7 @@
 
     python train.py [--epochs 400] [--batch-size 16] [--height 112] [--width 112] [--weights W] [--seed S]
     python train.py --native-size ...   every image at its own size (ragged batches, WaterNet.forward_many)
+    python train.py --ssim-weight 0.5 ...   add 0.5 * (1 - SSIM) to the loss (metrics.ssim_loss)
 
 Writes ``training/<n>/{last.pt, metrics-train.csv, metrics-val.csv, config.json}``.  Without the
 UIEB folders (``data/raw-890``, ``data/reference-890``) pass ``--synthetic`` for UIEB-shaped
@@ -50,6 +51,7 @@ def main():
                          "--height x --width")
     T.add_perceptual_args(ap)
     T.add_metrics_arg(ap)
+    T.add_loss_arg(ap)
     args = ap.parse_args()
     if args.native_size and args.loader != "gpu":
         raise SystemExit("--native-size needs --loader gpu (ragged batches are assembled on the device)")
@@ -100,7 +102,7 @@ def main():
     for epoch in range(args.epochs):
         print(f"Epoch {epoch + 1}/{args.epochs}")
         tm = T.train_one_epoch(model, train_loader, optimizer, scheduler, vgg, device, log=print,
-                               native_metrics=native_metrics)
+                               native_metrics=native_metrics, ssim_weight=args.ssim_weight)
         vm = T.eval_one_epoch(model, val_loader, vgg, device, native_metrics=native_metrics)
         print("    Train ||", "   ".join(f"{k}: {v:.03g}" for k, v in tm.items()))
         print("    Val   ||", "   ".join(f"{k}: {v:.03g}" for k, v in vm.items()))
@@ -111,7 +113,8 @@ def main():
     T.save_metrics(savedir, train_hist, val_hist, {
         "epochs": args.epochs, "batch_size": args.batch_size, "im_height": args.height, "im_width": args.width,
         "weights": args.weights, "native_size": args.native_size, "grad_tile": args.grad_tile,
-        "train_precision": args.train_precision, **T.perceptual_config(args), **T.metrics_config(args)})
+        "train_precision": args.train_precision, **T.perceptual_config(args), **T.metrics_config(args),
+        **T.loss_config(args)})
     print(f"Metrics and weights saved to {savedir}")
     print(f"Total time: {timer() - start}s")
 

@@ -51,6 +51,13 @@ class QualityImage(ctypes.Structure):
 QUALITY_STATS = 7  # WN_QUALITY_STATS: float64 statistics per image of wn_quality
 
 
+class SSIMGradImage(ctypes.Structure):
+    """wn_ssim_grad_image: one (out, ref) pair of a wn_ssim_grad call and the gradient it receives, fp32 contiguous
+    (3,H,W) device pointers, its size, its group and the weight of its SSIM in the differentiated sum."""
+    _fields_ = [("out", c_void_p), ("ref", c_void_p), ("grad", c_void_p), ("height", c_int), ("width", c_int),
+                ("group", c_int), ("scale", ctypes.c_double)]
+
+
 # name -> (restype, argtypes); mirrors include/waternet_b200.h one to one
 _SIGNATURES = {
     "wn_abi_version": (c_int, []),
@@ -170,8 +177,15 @@ _METRICS_SIGNATURES = {
     "wn_quality": (c_int, [c_void_p, POINTER(QualityImage), c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
 
+# ... and include/waternet_b200_ssim.h, SSIM's gradient (csrc/metrics.cu)
+_SSIM_SIGNATURES = {
+    "wn_ssim_grad_workspace_bytes": (c_size_t, [POINTER(c_int), POINTER(c_int), c_int]),
+    "wn_ssim_grad": (c_int, [c_void_p, POINTER(SSIMGradImage), c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+}
+
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)                # the entry points of include/waternet_b200.h
 METRICS_SYMBOLS = tuple(_METRICS_SIGNATURES)         # ... of include/waternet_b200_metrics.h
+SSIM_SYMBOLS = tuple(_SSIM_SIGNATURES)               # ... of include/waternet_b200_ssim.h
 
 _lib = None
 
@@ -192,7 +206,7 @@ def load() -> ctypes.CDLL:
             "Run `python -m waternet_b200.build` (needs nvcc 12.9); there is no CPU fallback."
         )
     lib = ctypes.CDLL(path)
-    for name, (res, args) in {**_SIGNATURES, **_METRICS_SIGNATURES}.items():
+    for name, (res, args) in {**_SIGNATURES, **_METRICS_SIGNATURES, **_SSIM_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args

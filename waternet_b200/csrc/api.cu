@@ -3,6 +3,9 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+#include <cmath>
+
 #include "common.cuh"
 
 namespace wn {
@@ -1095,6 +1098,72 @@ int wn_quality(wn_handle* h, const wn_quality_image* images_host, int n, double*
     return rc;
   DeviceGuard guard(h->device);
   return quality(h, images_host, n, stats, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// ---- SSIM's gradient (metrics.cu)
+static_assert(sizeof(wn_ssim_grad_image) == 48, "wn_ssim_grad_image: _lib.SSIMGradImage restates this layout");
+
+size_t wn_ssim_grad_workspace_bytes(const int* heights_host, const int* widths_host, int n) {
+  const char* what = "wn_ssim_grad_workspace_bytes";
+  if (check_ptrs(what, {heights_host, widths_host}) || check_ragged_count(what, n)) return 0;
+  return ssim_grad_workspace_bytes(heights_host, widths_host, n);
+}
+
+// no grad overlaps any out, ref or other grad: the intervals in order of their start, each writer checked against
+// the furthest end of everything before it and each reader against the furthest end of the writers before it
+static int check_grad_overlap(const char* what, const wn_ssim_grad_image* images, int n) {
+  struct Span {
+    uintptr_t begin, end;
+    bool writes;
+    int image;
+  };
+  std::vector<Span> spans;
+  spans.reserve(3 * (size_t)n);
+  for (int i = 0; i < n; i++) {
+    const size_t bytes = (size_t)3 * images[i].height * images[i].width * sizeof(float);
+    for (const void* p : {(const void*)images[i].out, (const void*)images[i].ref, (const void*)images[i].grad})
+      spans.push_back({(uintptr_t)p, (uintptr_t)p + bytes, p == images[i].grad, i});
+  }
+  std::sort(spans.begin(), spans.end(), [](const Span& a, const Span& b) { return a.begin < b.begin; });
+  uintptr_t reach = 0, reach_w = 0;
+  for (const Span& s : spans) {
+    if (s.begin < (s.writes ? reach : reach_w)) {
+      set_error("%s: grad of image %d overlaps an out, ref or grad of the call", what, s.image);
+      return WN_E_INVALID;
+    }
+    reach = std::max(reach, s.end);
+    if (s.writes) reach_w = std::max(reach_w, s.end);
+  }
+  return WN_OK;
+}
+
+int wn_ssim_grad(wn_handle* h, const wn_ssim_grad_image* images_host, int n, double* stats, void* workspace,
+                 size_t workspace_bytes, void* stream) {
+  const char* what = "wn_ssim_grad";
+  int rc = check_ptrs(what, {h, images_host, stats, workspace});
+  if (rc || (rc = check_ragged_count(what, n)) ||
+      (rc = check_images(what, images_host, n, true,
+                         [](const wn_ssim_grad_image& im, int) { return im.out && im.ref && im.grad; })))
+    return rc;
+  for (int i = 0; i < n; i++) {
+    if (images_host[i].group < 0 || images_host[i].group >= n) {
+      set_error("%s: image %d: group %d outside 0..%d", what, i, images_host[i].group, n - 1);
+      return WN_E_INVALID;
+    }
+    if (!std::isfinite(images_host[i].scale)) {
+      set_error("%s: image %d: scale %g is not finite", what, i, images_host[i].scale);
+      return WN_E_INVALID;
+    }
+  }
+  if ((uintptr_t)stats % alignof(double)) return invalid(what, "stats is not 8-byte aligned");
+  if ((rc = check_grad_overlap(what, images_host, n))) return rc;
+  std::vector<int> hs, ws;
+  ragged_sizes(images_host, n, &hs, &ws);
+  if ((rc = ssim_grad_plan_check(hs.data(), ws.data(), n, what)) ||
+      (rc = check_workspace(what, workspace_bytes, ssim_grad_workspace_bytes(hs.data(), ws.data(), n))))
+    return rc;
+  DeviceGuard guard(h->device);
+  return ssim_grad(h, images_host, n, stats, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int wn_enable_timing(wn_handle* h, int on) {

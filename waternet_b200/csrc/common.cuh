@@ -10,6 +10,7 @@
 
 #include "../../include/waternet_b200.h"
 #include "../../include/waternet_b200_metrics.h"
+#include "../../include/waternet_b200_ssim.h"
 #include "tiling.cuh"
 
 namespace wn {
@@ -418,5 +419,10 @@ int quality_plan_check(const int* hs, const int* ws, int n, const char* what);
 size_t quality_workspace_bytes(const int* hs, const int* ws, int n);
 int quality(wn_handle* h, const wn_quality_image* images, int n, double* stats, void* workspace,
             size_t workspace_bytes, cudaStream_t stream);
+// ... and SSIM's gradient (wn_ssim_grad): the same checks, plus the gradient grid's size
+int ssim_grad_plan_check(const int* hs, const int* ws, int n, const char* what);
+size_t ssim_grad_workspace_bytes(const int* hs, const int* ws, int n);
+int ssim_grad(wn_handle* h, const wn_ssim_grad_image* images, int n, double* stats, void* workspace,
+              size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace wn

@@ -1167,15 +1167,9 @@ class Engine:
         return dst
 
     # ---- SSIM / PSNR statistics (wn_quality) ------------------------------------------------------------------
-    def quality_workspace_bytes(self, sizes) -> int:
-        """Workspace of one ``quality`` call over images of ``sizes`` [(h, w), ...]; 0 for rejected sizes."""
-        return int(self.lib.wn_quality_workspace_bytes(*_sizes(sizes), len(sizes)))
-
-    def quality(self, outs, refs, groups) -> torch.Tensor:
-        """The SSIM / PSNR statistics of the pairs (outs[i], refs[i]) in one wn_quality call: (3,H_i,W_i) fp32
-        contiguous CUDA tensors, image i in group ``groups[i]`` (images of one group share SSIM's data range).
-        Returns a (n, 7) float64 tensor, per image: the SSIM sum over its counted pixels, their count, the sum of
-        squared differences, min and max of out, min and max of ref."""
+    def _check_pairs(self, outs, refs, groups) -> None:
+        """ValueError unless outs and refs are as many (at least one) fp32 contiguous (3,H,W) tensors on this
+        engine's device, pairwise of one shape, with one group each."""
         n = len(outs)
         if n == 0 or len(refs) != n or len(groups) != n:
             raise ValueError(f"expected as many refs and groups as outs (at least one), got {n}, {len(refs)}, "
@@ -1188,6 +1182,18 @@ class Engine:
                                      f"{t.dtype} {tuple(t.shape)} on {t.device}")
             if o.shape != r.shape:
                 raise ValueError(f"out and ref differ in shape: {tuple(o.shape)} vs {tuple(r.shape)}")
+
+    def quality_workspace_bytes(self, sizes) -> int:
+        """Workspace of one ``quality`` call over images of ``sizes`` [(h, w), ...]; 0 for rejected sizes."""
+        return int(self.lib.wn_quality_workspace_bytes(*_sizes(sizes), len(sizes)))
+
+    def quality(self, outs, refs, groups) -> torch.Tensor:
+        """The SSIM / PSNR statistics of the pairs (outs[i], refs[i]) in one wn_quality call: (3,H_i,W_i) fp32
+        contiguous CUDA tensors, image i in group ``groups[i]`` (images of one group share SSIM's data range).
+        Returns a (n, 7) float64 tensor, per image: the SSIM sum over its counted pixels, their count, the sum of
+        squared differences, min and max of out, min and max of ref."""
+        self._check_pairs(outs, refs, groups)
+        n = len(outs)
         table = (_lib.QualityImage * n)()
         for d, o, r, g in zip(table, outs, refs, groups):
             d.out, d.ref, d.height, d.width, d.group = o.data_ptr(), r.data_ptr(), o.shape[1], o.shape[2], int(g)
@@ -1198,3 +1204,37 @@ class Engine:
         stats = torch.empty((n, _lib.QUALITY_STATS), dtype=torch.float64, device=self.device)
         self._call("wn_quality", table, n, stats.data_ptr(), ws.data_ptr(), ws.numel())
         return stats
+
+    # ---- SSIM's gradient (wn_ssim_grad) -------------------------------------------------------------------------
+    def ssim_grad_workspace_bytes(self, sizes) -> int:
+        """Workspace of one ``ssim_grad`` call over images of ``sizes`` [(h, w), ...]; 0 for rejected sizes."""
+        return int(self.lib.wn_ssim_grad_workspace_bytes(*_sizes(sizes), len(sizes)))
+
+    def ssim_grad(self, outs, refs, groups, scales, grads=None):
+        """``quality``'s statistics of the pairs (outs[i], refs[i]) and, per image, d/d(outs[i]) of
+        sum_j scales[j] * SSIM_j (SSIM_j: image j's SSIM, its data-range term included) in one wn_ssim_grad call.
+        ``grads``: the (3,H_i,W_i) fp32 contiguous tensors that receive the gradients, None to allocate them; none
+        may overlap an out, a ref or another grad.  Returns (stats, grads)."""
+        self._check_pairs(outs, refs, groups)
+        n = len(outs)
+        if len(scales) != n:
+            raise ValueError(f"expected one scale per image, got {len(scales)} for {n}")
+        if grads is None:
+            grads = [torch.empty_like(o) for o in outs]
+        if len(grads) != n:
+            raise ValueError(f"expected one grad per image, got {len(grads)} for {n}")
+        for o, g in zip(outs, grads):
+            if g.device != self.device or g.dtype != torch.float32 or g.shape != o.shape or not g.is_contiguous():
+                raise ValueError(f"expected fp32 contiguous {tuple(o.shape)} grads on {self.device}, got {g.dtype} "
+                                 f"{tuple(g.shape)} on {g.device}")
+        table = (_lib.SSIMGradImage * n)()
+        for d, o, r, g, grp, sc in zip(table, outs, refs, grads, groups, scales):
+            d.out, d.ref, d.grad, d.height, d.width = o.data_ptr(), r.data_ptr(), g.data_ptr(), o.shape[1], o.shape[2]
+            d.group, d.scale = int(grp), float(sc)
+        sizes = [tuple(o.shape[1:]) for o in outs]
+        ws = self._workspace("ssim_grad", _require_workspace(
+            self.ssim_grad_workspace_bytes(sizes), f"ssim_grad: unsupported sizes {sizes}: 1..65535 images, each "
+                                                   "side at least 6 and at most 0x7fffffff / 3 pixels per plane"))
+        stats = torch.empty((n, _lib.QUALITY_STATS), dtype=torch.float64, device=self.device)
+        self._call("wn_ssim_grad", table, n, stats.data_ptr(), ws.data_ptr(), ws.numel())
+        return stats, grads

@@ -6,7 +6,8 @@ weight-gradient kernels; only ``precision="fp32"`` re-evaluates the torch graph 
 VGG19 perceptual loss is the torch expression by default; ``PerceptualModel(native=True)`` computes it and its
 gradient in overlapping windows on the library's kernels (``wn_perceptual_loss``).  SSIM and PSNR are the torch
 expressions of ``metrics`` by default; ``native=True`` (``--metrics native``) computes them with ``wn_quality``.
-Adam stays PyTorch.
+``ssim_weight`` (``--ssim-weight``) adds ``ssim_weight * metrics.ssim_loss(out, ref)`` to the loss, 1 - SSIM and its
+gradient from ``wn_ssim_grad``.  Adam stays PyTorch.
 """
 from __future__ import annotations
 
@@ -21,7 +22,7 @@ import torch
 import torch.nn as nn
 
 from .engine import AUTO_TILE, Engine, is_auto
-from .metrics import native_quality, psnr, ssim
+from .metrics import native_quality, psnr, ssim, ssim_loss
 from .net import TRAIN_PRECISIONS, _PackedWeightsMixin
 
 TRAIN_METRICS_NAMES = ["mse", "ssim", "psnr", "perceptual_loss", "loss"]
@@ -188,6 +189,29 @@ def metrics_config(args) -> dict:
     return {"metrics": args.metrics}
 
 
+def _nonnegative(text: str) -> float:
+    try:
+        v = float(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"expected a number, got {text!r}") from None
+    if not v >= 0 or v == float("inf"):
+        raise argparse.ArgumentTypeError(f"must be finite and at least 0, got {text!r}")
+    return v
+
+
+def add_loss_arg(ap) -> None:
+    """``--ssim-weight W`` of train.py."""
+    ap.add_argument("--ssim-weight", type=_nonnegative, default=0.0, metavar="W",
+                    help="(Optional) Add W * (1 - SSIM) to the loss, SSIM and its gradient on the library's kernels "
+                         "(metrics.ssim_loss), no per-pixel temporaries besides d(out).  Default 0: the reference's "
+                         "0.05 * perceptual + mse, nothing extra computed")
+
+
+def loss_config(args) -> dict:
+    """The loss setting of ``add_loss_arg`` as train.py records it in config.json."""
+    return {"ssim_weight": args.ssim_weight}
+
+
 def perceptual_config(args) -> dict:
     """The perceptual-loss settings of ``add_perceptual_args`` as train.py records them in config.json."""
     return {"perceptual": args.perceptual, "perceptual_tile": args.perceptual_tile,
@@ -249,15 +273,19 @@ def batch_quality(out, ref, native: bool = False):
 
 
 def train_one_epoch(model, loader, optimizer, scheduler, vgg, device, log=None,
-                    native_metrics: bool = False) -> Dict[str, float]:
+                    native_metrics: bool = False, ssim_weight: float = 0.0) -> Dict[str, float]:
     """One epoch; a batch is five tensors, or five lists of images of their own sizes (GpuBatchLoader(ragged=True)).
-    ``native_metrics``: SSIM and PSNR from ``batch_quality(native=True)``."""
+    ``native_metrics``: SSIM and PSNR from ``batch_quality(native=True)``.  ``ssim_weight``: the loss is
+    ``0.05 * perc + mse + ssim_weight * metrics.ssim_loss(out, ref)`` (1 - SSIM of ``batch_quality``'s semantics);
+    at 0 nothing extra is computed."""
     model.train()
     totals = {k: 0.0 for k in TRAIN_METRICS_NAMES}
     for idx, batch in enumerate(loader):
         raw, wb, he, gc, ref = _to_device(batch, device)
         out = _forward(model, raw, wb, he, gc)
         loss, perc, mse = batch_losses(vgg, out, ref)
+        if ssim_weight:
+            loss = loss + ssim_weight * ssim_loss(out, ref)
         optimizer.zero_grad()
         loss.backward()
         optimizer.step()
