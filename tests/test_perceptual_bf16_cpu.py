@@ -22,21 +22,12 @@ import torch
 import torch.nn.functional as F
 
 import bf16_replay as rp
+import vgg_reference as V
 from bf16_replay import _bf16, acc_tau
+from vgg_reference import CONVS, MEAN, STD, STEPS
 
-MEAN = (0.485, 0.456, 0.406)
-STD = (0.229, 0.224, 0.225)
 ROUND = 2.0 ** -8
 PACK_TAU = 2.0 ** -22  # (v - mean) / std: two fp32 operations, then the bf16 store (F)
-
-# (conv index or -1 for a pool, level, channels) of the 20 forward launches, and (cin, cout) of the 16 convolutions:
-# waternet_b200.engine.VGG_STEPS / VGG_CONVS, restated so that this module imports without the library
-STEPS = ((0, 0, 64), (1, 0, 64), (-1, 1, 64), (2, 1, 128), (3, 1, 128), (-1, 2, 128), (4, 2, 256), (5, 2, 256),
-         (6, 2, 256), (7, 2, 256), (-1, 3, 256), (8, 3, 512), (9, 3, 512), (10, 3, 512), (11, 3, 512),
-         (-1, 4, 512), (12, 4, 512), (13, 4, 512), (14, 4, 512), (15, 4, 512))
-CONVS = ((3, 64), (64, 64), (64, 128), (128, 128), (128, 256), (256, 256), (256, 256), (256, 256), (256, 512),
-         (512, 512), (512, 512), (512, 512), (512, 512), (512, 512), (512, 512), (512, 512))
-
 
 def fwd_k(conv):
     """Products per output element of forward convolution ``conv``: cinpad x 9 (the first one reads 16 channels)."""
@@ -117,6 +108,15 @@ def pool_bwd_replay(g, saved):
     return F.max_unpool2d(g.double(), idx, 2, 2, output_size=saved.shape[-2:])
 
 
+def pool_bwd_last(g, saved):
+    """A pool backward that routes a tie to the LAST maximum of its window: the first one of the window turned
+    around (both axes flipped on the even part, the floored edge 0)."""
+    h, w = saved.shape[-2] // 2 * 2, saved.shape[-1] // 2 * 2
+    _, idx = F.max_pool2d(saved[..., :h, :w].double().flip(-2, -1), 2, 2, return_indices=True)
+    r = F.max_unpool2d(g.double().flip(-2, -1), idx, 2, 2, output_size=(h, w)).flip(-2, -1)
+    return F.pad(r, (0, saved.shape[-1] - w, 0, saved.shape[-2] - h))
+
+
 def loss_from_features(fo, fr):
     return (torch.square(255.0 * (fo.double() - fr.double()))).sum().item() / fo.numel()
 
@@ -137,6 +137,17 @@ def image(n, h, w, seed):
     return torch.rand(n, 3, h, w, generator=torch.Generator().manual_seed(seed))
 
 
+def _bias(ws, conv, fault):
+    """The biases forward convolution ``conv`` adds: its own, or those of a fault -- "bias_group0" (every column group
+    of 128 channels reads group 0's), "bias_next" (the next convolution's), "no_bias"."""
+    b = ws[conv][1].double()
+    if fault == "bias_group0":
+        return b[torch.arange(b.numel()) % 128]
+    if fault == "bias_next":
+        return ws[conv + 1][1].double()
+    return torch.zeros_like(b) if fault == "no_bias" else b
+
+
 def emulate_forward(x, ws, fault=None, at=None):
     """(act0, the decoded outputs of the 20 forward launches).  ``at``: "pack" or a launch index."""
     v = _norm_f32(x)
@@ -154,7 +165,8 @@ def emulate_forward(x, ws, fault=None, at=None):
         z = F.conv2d(a, w_hi, padding=1)
         if (fault, at) == ("w_lo_pass", k):
             z = z + F.conv2d(a, _bf16(w - w_hi), padding=1)
-        val = F.relu(_f32(_f32(z) + b.double().view(1, -1, 1, 1)))
+        b = _bias(ws, conv, fault if at == k else None)
+        val = F.relu(_f32(_f32(z) + b.view(1, -1, 1, 1)))
         # an a_lo pass reads the lo plane its producer did not zero
         keep_lo = (fault, at) in (("lo_not_zeroed", k), ("a_lo_pass", k + 1))
         outs.append(_hilo(val) if keep_lo else _bf16(val))
@@ -184,7 +196,7 @@ def emulate_backward(fwd, seed, ws, fault=None, at=None):
     for k in range(len(STEPS) - 1, -1, -1):
         conv = STEPS[k][0]
         if conv < 0:
-            bwd[k] = pool_bwd_replay(g, fwd[k - 1])
+            bwd[k] = (pool_bwd_last if (fault, at) == ("ties_last", k) else pool_bwd_replay)(g, fwd[k - 1])
             g = bwd[k]
             continue
         w = ws[conv][0].double()
@@ -261,8 +273,11 @@ def ws():
     return vgg_weights(5)
 
 
-def _run(ws, shape, fault=None, at=None):
-    out, ref = image(*shape, seed=sum(shape)), image(*shape, seed=sum(shape) + 1)
+def _run(ws, shape, fault=None, at=None, kind=None):
+    if kind is None:
+        out, ref = image(*shape, seed=sum(shape)), image(*shape, seed=sum(shape) + 1)
+    else:
+        out, ref = V.pair(kind, *shape, seed=sum(shape))
     act0, fwd = emulate_forward(out, ws, fault, at)
     _, fref = emulate_forward(ref, ws)
     seed, loss = emulate_seed(fwd[-1], fref[-1], fault if at == "seed" else None)
@@ -324,6 +339,41 @@ def test_each_fault_fails_its_launch(ws, fault, at, kind):
             check_forward_launch(at, e.act0, e.fwd, ws)
         else:
             check_backward_launch(at, e.fwd, e.seed, e.bwd, ws)
+
+
+# the weights and images of vgg_reference: nonzero biases at each layer's spread, flat patches whose pools meet ties;
+# (fault, launch, which bar must fail).  Launch 6 is conv3_1 (2 column groups), 11 conv4_1 (4), 12 conv4_2.
+BIAS_FAULT_CASES = [
+    ("bias_group0", 6, "forward"), ("bias_group0", 11, "forward"), ("bias_next", 12, "forward"),
+    ("no_bias", 1, "forward"), ("no_bias", 17, "forward"),
+    ("ties_last", 2, "backward"), ("ties_last", 5, "backward"),
+]
+
+
+@pytest.fixture(scope="module")
+def biased():
+    return V.weights("biased")
+
+
+def test_emulation_on_biased_weights_and_flat_images_passes_the_replay_bars(biased):
+    e = _run(biased, SHAPES[0], kind="flat")
+    for k in range(len(STEPS)):
+        check_forward_launch(k, e.act0, e.fwd, biased)
+        check_backward_launch(k, e.fwd, e.seed, e.bwd, biased)
+    # the tie fault below has something to route: tied positive maxima that receive a gradient, at both pools
+    for k in (2, 5):
+        saved, g = e.fwd[k - 1], e.bwd[k + 1]
+        assert not torch.equal(pool_bwd_replay(g, saved), pool_bwd_last(g, saved)), k
+
+
+@pytest.mark.parametrize("fault,at,kind", BIAS_FAULT_CASES)
+def test_each_bias_or_tie_fault_fails_its_launch(biased, fault, at, kind):
+    e = _run(biased, SHAPES[0], fault, at, kind="flat")
+    with pytest.raises(AssertionError):
+        if kind == "forward":
+            check_forward_launch(at, e.act0, e.fwd, biased)
+        else:
+            check_backward_launch(at, e.fwd, e.seed, e.bwd, biased)
 
 
 # ------------------------------------------------------------------ the Python surface

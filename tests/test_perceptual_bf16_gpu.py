@@ -19,6 +19,7 @@ import torch
 
 import buffer_bounds as bb
 import test_perceptual_bf16_cpu as vr
+import vgg_reference as V
 from test_buffer_bounds_gpu import _ok, _outputs, _run
 
 pytestmark = pytest.mark.gpu
@@ -71,12 +72,15 @@ def _weights(vgg):
 
 # ---- every launch on its own input ---------------------------------------------------------------------------------
 @pytest.mark.parametrize("shape", SHAPES)
-def test_every_launch_against_its_float64_replay(vgg, shape):
+@pytest.mark.parametrize("wset", V.WEIGHT_SETS)
+def test_every_launch_against_its_float64_replay(wset, shape):
     """The 20 forward launches, the seed and the 20 backward launches of one (out, ref) pair, each replayed in float64
     from the GPU's own decoded input (ReLU' from the GPU's saved planes, pools routed by them), and the fold of
-    d(out); the loss is the float64 sum over the GPU's own conv5_4 features of out and ref."""
+    d(out); the loss is the float64 sum over the GPU's own conv5_4 features of out and ref.  Both weight sets of
+    vgg_reference: the default init's biases are all 0."""
     bf16, _ = _modes()
     out, ref = _pair(*shape, seed=sum(shape))
+    vgg = V.perceptual_model(wset, precision="bf16")
     eng = vgg._vgg_engine(out)
     ws = _weights(vgg)
     dbg = lambda x, k, r=None: eng.debug_vgg_layer(x, k, ref=r, train_mode=bf16).double()
@@ -93,7 +97,7 @@ def test_every_launch_against_its_float64_replay(vgg, shape):
         worst["backward"] = max(worst["backward"], vr.check_backward_launch(k, fwd, seed, bwd, ws))
     worst["seed"] = vr.check_seed(seed, fwd[19], fref)
     for kind, v in worst.items():
-        _report(f"{kind}{shape}", v)
+        _report(f"{kind} {wset} {shape}", v)
     loss, g = eng.perceptual_loss(out, ref, want_grad=True, train_mode=bf16)
     want = vr.loss_from_features(fwd[19], fref)
     assert abs(loss.item() - want) <= 2.0 ** -22 * want, (loss.item(), want)

@@ -8,7 +8,9 @@ import pytest
 import torch
 import torch.nn as nn
 
+import vgg_reference as V
 from conftest import ROOT
+from grad_reference import assert_grad_close, grad_error
 
 NEW = ["wn_vgg_pack_weights", "wn_perceptual_loss_workspace_bytes", "wn_perceptual_loss", "wn_debug_vgg_layer"]
 MEAN = (0.485, 0.456, 0.406)
@@ -140,8 +142,10 @@ def _whole(vgg, out, ref):
     return loss.detach(), o.grad
 
 
-def _windowed(vgg, out, ref, th, tw):
-    """The window rule of wn_perceptual_loss: every window's owned features, seeded alone, folded in window order."""
+def _windowed(vgg, out, ref, th, tw, fault=None):
+    """The window rule of wn_perceptual_loss: every window's owned features, seeded alone, folded in window order.
+    ``fault``: "last_row" (the fold misses each window's last read row), "shift" (it adds a window one row low) or
+    "seed_row" (each window also seeds the feature row after its owned ones)."""
     from waternet_b200.engine import perceptual_windows
     n, _, h, w = out.shape
     count = n * vgg[-2].out_channels * (h // 16) * (w // 16)
@@ -152,11 +156,17 @@ def _windowed(vgg, out, ref, th, tw):
             with torch.no_grad():
                 fr = vgg(_norm(ref[:, :, ys:ye, xs:xe]))
             fo = vgg(_norm(o))
-            sy, sx = slice(fy0 - ys // 16, fy1 - ys // 16), slice(fx0 - xs // 16, fx1 - xs // 16)
+            sy = slice(fy0 - ys // 16, fy1 - ys // 16 + (fault == "seed_row"))
+            sx = slice(fx0 - xs // 16, fx1 - xs // 16)
             part = torch.sum(torch.square(255 * (fo[:, :, sy, sx] - fr[:, :, sy, sx]))) / count
             part.backward()
             loss += part.detach()
-            grad[:, :, ys:ye, xs:xe] += o.grad
+            if fault == "last_row":
+                grad[:, :, ys:ye - 1, xs:xe] += o.grad[:, :, :-1]
+            elif fault == "shift":
+                grad[:, :, ys + 1:ye, xs:xe] += o.grad[:, :, :-1]
+            else:
+                grad[:, :, ys:ye, xs:xe] += o.grad
     return loss, grad
 
 
@@ -177,3 +187,60 @@ def test_windows_reproduce_the_whole_image_loss_and_gradient(shape, tile):
     assert abs(lt - lw) <= 1e-12 * abs(lw)
     assert torch.linalg.vector_norm(gt - gw) <= 1e-12 * torch.linalg.vector_norm(gw)
     assert torch.max(torch.abs(gt - gw)) <= 1e-11 * torch.max(torch.abs(gw))
+
+
+# ---- the element-wise bar of d(out) ----------------------------------------------------------------------------------
+def _conv_pairs(vgg):
+    return [(m.weight.detach(), m.bias.detach()) for m in vgg if isinstance(m, nn.Conv2d)]
+
+
+@pytest.fixture(scope="module")
+def chain_case():
+    """A narrow VGG19 with nonzero biases on 1 x 250 x 333: the windowed decomposition at tile 48 and the whole-image
+    chain R and magnitude M of vgg_reference (the GPU tests' reference, here from a float64 forward)."""
+    vgg = _vgg((4, 8, 8, 8, 8), seed=3)
+    g = torch.Generator().manual_seed(9)
+    out = torch.rand((1, 3, 250, 333), generator=g, dtype=torch.float64)
+    ref = (out + 0.2 * torch.rand(out.shape, generator=g, dtype=torch.float64)).clamp(0, 1)
+    ws = _conv_pairs(vgg)
+    fwd, fref = V.forward_outputs(out, ws), V.forward_outputs(ref, ws)
+    seed = V.seed_of(fwd[-1], fref[-1])
+    R, M = V.chain(fwd, seed, ws), V.chain(fwd, seed, ws, absolute=True)
+    return vgg, out, ref, R, M
+
+
+def test_the_chain_is_the_whole_image_gradient(chain_case):
+    vgg, out, ref, R, M = chain_case
+    _, gw = _whole(vgg, out, ref)
+    assert_grad_close(gw, R, M, 1e-12, "autograd against the chain")
+
+
+def test_the_clean_window_fold_passes_the_chain_bar(chain_case):
+    vgg, out, ref, R, M = chain_case
+    _, gt = _windowed(vgg, out, ref, 48, 48)
+    assert_grad_close(gt, R, M, V.TAU_CHAIN["bf16x3"], "windowed d(out)")
+
+
+@pytest.mark.parametrize("fault", ["last_row", "shift", "seed_row"])
+def test_each_fold_fault_fails_the_chain_bar(chain_case, fault):
+    """Each fault fails the bar of both arithmetics."""
+    vgg, out, ref, R, M = chain_case
+    _, gt = _windowed(vgg, out, ref, 48, 48, fault)
+    assert grad_error(gt, R, M).max().item() > max(V.TAU_CHAIN.values()), fault
+
+
+def test_max_pool_picks_the_first_maximum_on_the_cpu():
+    V.assert_first_maximum_routing("cpu")
+
+
+def test_support_mask_is_the_support_of_the_flagged_features():
+    from waternet_b200.engine import VGG_SUPPORT
+    assert V.SUPPORT == VGG_SUPPORT
+    nz = torch.zeros((2, 20, 19), dtype=torch.bool)
+    nz[0, 3, 17] = True
+    nz[1, 0, 0] = nz[1, 19, 5] = True
+    m = V.support_mask(328, 312, nz)[:, 0]
+    want = torch.zeros_like(m)
+    for n, i, j in nz.nonzero().tolist():
+        want[n, max(0, 16 * i - 118):16 * i + 134, max(0, 16 * j - 118):16 * j + 134] = True
+    assert torch.equal(m, want)

@@ -2,7 +2,9 @@
 against float64 on its own input, the loss and d(loss)/d(out) against float64 torch, seams, odd sizes, determinism,
 memory, autograd and training."""
 import copy
+import functools
 import os
+import types
 
 import numpy as np
 import pytest
@@ -10,29 +12,34 @@ import torch
 import torch.nn.functional as F
 
 from grad_reference import assert_grad_close
+import test_perceptual_bf16_gpu as bg
+import vgg_reference as V
+from vgg_reference import TAU_LAYER
 
 pytestmark = pytest.mark.gpu
 
 MEAN = (0.485, 0.456, 0.406)
 STD = (0.229, 0.224, 0.225)
-# Bars, measured on an H100 80GB HBM3 (700 W limit); DESIGN.md 4.12.
-# TAU_LAYER: 4x the worst |G - R| / M of a launch against float64 on its own input: forward 9.9e-6 (conv1_1), data
-#   gradients 5.4e-6 (the backward of conv1_2); pools and pool backwards are exact.
+# Bars, measured on an H100 80GB HBM3 (700 W limit); DESIGN.md 4.12.  TAU_LAYER: vgg_reference.
 # LOSS_REL: 4x the worst relative error of the loss, 2.43e-4 (1 x 300 x 500), and under 1e-3.
 # CHAIN_REL, CHAIN_TAU: d(out) against the float64 backward of the GPU's own seed, ReLU masks and pool choices at
 #   1 x 64 x 80: norm-wise the 1e-3 the loss's gradient is held to (measured 1.2e-4), element-wise 4x the worst
-#   |G - R| / max |R| (1.14e-4).
+#   |G - R| / max |R| (1.14e-4).  Against a per-element magnitude at every call: test_perceptual_chain_gpu.
 # GRAD_REL: d(out) against the float64 reference with its own forward, on seeded default-init weights and noise
 #   images: 4x the worst, 3.23e-2 (3 x 64 x 80).  That error is not arithmetic: at 1 x 64 x 80 three ReLU decisions
 #   and two pool choices of the bf16x3 forward differ from float64's, and the float64 chain with the GPU's decisions
 #   is as far from the reference (1.6e-2) as the GPU's d(out) is.  Torch in fp32 flips too (8.6e-3 at 1 x 300 x 500).
 # SEAM_GRAD_REL: 4x the windowed d(out) against the one-window d(out), 2.7e-5.
-TAU_LAYER = 4e-5
 LOSS_REL = 1e-3
 CHAIN_REL = 1e-3
 CHAIN_TAU = 5e-4
 GRAD_REL = 0.13
 SEAM_GRAD_REL = 1.2e-4
+# per-launch cases: the shapes of the bf16 replay, plus shapes whose levels have odd or 8 (mod 16) extents (level 3 of
+# 1 x 24 x 40 is 3 x 5, of 2 x 136 x 200 17 x 25), on both weight sets, noise and flat-patch images
+LAUNCH_SHAPES = list(bg.SHAPES) + [(1, 24, 40), (2, 136, 200)]
+CASES = [(ws, kind, shape) for ws in V.WEIGHT_SETS for kind in ("noise", "flat") for shape in LAUNCH_SHAPES]
+CASE_IDS = [f"{ws}-{kind}-{'x'.join(map(str, shape))}" for ws, kind, shape in CASES]
 
 
 def _vgg(seed=1234, device="cuda"):
@@ -42,16 +49,16 @@ def _vgg(seed=1234, device="cuda"):
 
 
 def _pair(n, h, w, seed=0, device="cuda"):
-    g = torch.Generator().manual_seed(seed)
-    out = torch.rand((n, 3, h, w), generator=g)
-    ref = (out + 0.3 * (torch.rand((n, 3, h, w), generator=g) - 0.5)).clamp(0, 1)
+    out, ref = V.noise_pair(n, h, w, seed)
     return out.to(device), ref.to(device)
 
 
 def _norm64(x):
-    mean = torch.tensor(MEAN, dtype=torch.float32).double().view(1, 3, 1, 1).to(x.device)
-    std = torch.tensor(STD, dtype=torch.float32).double().view(1, 3, 1, 1).to(x.device)
-    return (x.double() - mean) / std
+    return V.normalise(x)
+
+
+def _ws(vgg):
+    return [(m.weight.detach(), m.bias.detach()) for m in vgg.model if isinstance(m, torch.nn.Conv2d)]
 
 
 def _reference(vgg, out, ref):
@@ -86,85 +93,90 @@ def _eng(vgg, x):
     return vgg._vgg_engine(x)
 
 
-# ---- per launch ----------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("layer", range(20))
-def test_every_launch_against_float64_on_its_own_input(vgg, layer):
-    from waternet_b200.engine import VGG_STEPS
-    x, _ = _pair(2, 64, 96, seed=layer)
-    eng = _eng(vgg, x)
-    G = eng.debug_vgg_layer(x, layer).double()
-    conv, _, _ = VGG_STEPS[layer]
-    a = _norm64(x) if layer == 0 else eng.debug_vgg_layer(x, layer - 1).double()
-    if conv < 0:  # a pool copies the chosen element: exact
-        R = F.max_pool2d(a, 2, 2)
-        assert torch.equal(G, R)
-        return
-    mod = [m for m in vgg.model if isinstance(m, torch.nn.Conv2d)][conv]
-    w, b = mod.weight.detach().double(), mod.bias.detach().double()
-    R = torch.relu(F.conv2d(a, w, b, padding=1))
-    M = F.conv2d(a.abs(), w.abs(), b.abs(), padding=1)
-    worst = assert_grad_close(G, R, M, TAU_LAYER, f"conv {conv}")
-    _report(f"layer{layer}", worst)
-
-
-# ---- backward, per launch -------------------------------------------------------------------------------------------
-def _conv_weights(vgg, conv):
-    mod = [m for m in vgg.model if isinstance(m, torch.nn.Conv2d)][conv]
-    return mod.weight.detach().double(), mod.bias.detach().double()
-
-
-def _backward_launch_reference(vgg, fwd, gin, k):
-    """float64 backward of forward launch k from its own input gradient ``gin`` and the GPU's saved forward outputs
-    ``fwd`` (launch k - 1's output is launch k's input): (R, M), M = None for a pool (exact)."""
-    from waternet_b200.engine import VGG_STEPS
-    conv = VGG_STEPS[k][0]
-    if conv < 0:  # route to the first maximum of the 2 x 2 window of the saved input
-        saved = fwd[k - 1]
-        _, idx = F.max_pool2d(saved, 2, 2, return_indices=True)
-        return F.max_unpool2d(gin, idx, 2, 2, output_size=saved.shape[-2:]), None
-    w, _ = _conv_weights(vgg, conv)
-    R = F.conv_transpose2d(gin, w, padding=1)
-    M = F.conv_transpose2d(gin.abs(), w.abs(), padding=1)
-    if k:  # ReLU' of the launch's input
-        live = (fwd[k - 1] > 0).double()
-        R, M = R * live, M * live
-    return R, M
-
-
-@pytest.fixture(scope="module")
-def backward_launches(vgg):
-    """The GPU's forward outputs, seed and the outputs of the 20 backward launches of one (out, ref) pair."""
-    out, ref = _pair(2, 64, 96, seed=21)
+@functools.lru_cache(maxsize=1)
+def _launches(case):
+    """The GPU's forward outputs of out, conv5_4 of ref, the seed and the outputs of the 20 backward launches of one
+    case's (out, ref) pair, in float64 (the tests of one case run one after another)."""
+    wset, kind, shape = case
+    vgg = _models(wset)
+    out, ref = (t.cuda() for t in V.pair(kind, *shape, seed=sum(shape)))
     eng = _eng(vgg, out)
     fwd = [eng.debug_vgg_layer(out, k).double() for k in range(20)]
     fr = eng.debug_vgg_layer(ref, 19).double()
     seed = eng.debug_vgg_layer(out, 21, ref=ref).double()
     bwd = [eng.debug_vgg_layer(out, 22 + k, ref=ref).double() for k in range(20)]
-    return fwd, fr, seed, bwd
+    return types.SimpleNamespace(out=out, fwd=fwd, fr=fr, seed=seed, bwd=bwd, ws=V.weights(wset))
 
 
-def test_seed_against_float64(backward_launches):
-    fwd, fr, seed, _ = backward_launches
-    count = fr.numel()
-    R = 2 * 255.0 ** 2 * (fwd[19] - fr) / count * (fwd[19] > 0)
-    _report("seed", assert_grad_close(seed, R, R.abs(), 1e-5, "seed"))
+@functools.lru_cache(maxsize=None)
+def _models(wset):
+    return V.perceptual_model(wset)
+
+
+def _positive_ties(a, g=None):
+    """2 x 2 pool windows of ``a`` whose positive maximum is taken by two or more elements (and, with the pooled
+    gradient ``g``, that receive a nonzero gradient)."""
+    n, c, h, w = a.shape
+    t = a[..., :h // 2 * 2, :w // 2 * 2].reshape(n, c, h // 2, 2, w // 2, 2)
+    m = t.amax((3, 5))
+    tied = ((t == m[:, :, :, None, :, None]).sum((3, 5)) >= 2) & (m > 0)
+    if g is not None:
+        tied &= g != 0
+    return int(tied.sum())
+
+
+def test_max_pool_picks_the_first_maximum_on_the_device():
+    V.assert_first_maximum_routing("cuda")
+
+
+# ---- per launch ----------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("layer", range(20))
+@pytest.mark.parametrize("case", CASES, ids=CASE_IDS)
+def test_every_launch_against_float64_on_its_own_input(case, layer):
+    L = _launches(case)
+    G = L.fwd[layer]
+    conv = V.STEPS[layer][0]
+    a = _norm64(L.out) if layer == 0 else L.fwd[layer - 1]
+    if conv < 0:  # a pool copies the chosen element: exact
+        R = F.max_pool2d(a, 2, 2)
+        assert torch.equal(G, R)
+        if case[1] == "flat" and layer == 2:
+            assert _positive_ties(a) > 0, "no tied positive maximum: the flat patches do not reach the pool"
+        return
+    w, b = (t.to(a.device, torch.float64) for t in L.ws[conv])
+    R = torch.relu(F.conv2d(a, w, b, padding=1))
+    M = F.conv2d(a.abs(), w.abs(), b.abs(), padding=1)
+    worst = assert_grad_close(G, R, M, TAU_LAYER, f"conv {conv}")
+    _report(f"layer{layer} {case[0]}", worst)
+
+
+# ---- backward, per launch -------------------------------------------------------------------------------------------
+def test_seed_against_float64():
+    """The seed of every per-launch case within 1e-5 of |R| element by element (exactly 0 where R is)."""
+    for case, name in zip(CASES, CASE_IDS):
+        L = _launches(case)
+        R = V.seed_of(L.fwd[19], L.fr)
+        _report(f"seed {case[0]}", assert_grad_close(L.seed, R, R.abs(), 1e-5, f"seed of {name}"))
 
 
 @pytest.mark.parametrize("k", range(20))
-def test_every_backward_launch_against_float64_on_its_own_input(vgg, backward_launches, k):
+@pytest.mark.parametrize("case", CASES, ids=CASE_IDS)
+def test_every_backward_launch_against_float64_on_its_own_input(case, k):
     """Each data-gradient launch within TAU_LAYER of M = conv_transpose(|g|, |W|) on its own input gradient and ReLU'
-    mask; each pool backward exact, routed by the saved input."""
-    fwd, _, seed, bwd = backward_launches
-    gin = seed if k == 19 else bwd[k + 1]
-    R, M = _backward_launch_reference(vgg, fwd, gin, k)
-    G = bwd[k]
+    mask; each pool backward exact, routed by the saved input to the first maximum, ties included."""
+    L = _launches(case)
+    gin = L.seed if k == 19 else L.bwd[k + 1]
+    R, M = V.backward_launch_reference(L.ws, L.fwd, gin, k)
+    G = L.bwd[k]
     if k == 0:  # the 16 normalised channels: 3 real, 13 zero
         assert torch.count_nonzero(G[:, 3:]) == 0
         G = G[:, :3]
     if M is None:
         assert torch.equal(G, R)
+        if case[1] == "flat" and k == 2:
+            assert _positive_ties(L.fwd[1], gin) > 0, "no tied positive maximum receives a gradient"
         return
-    _report(f"bwd{k}", assert_grad_close(G, R, M, TAU_LAYER, f"backward of launch {k}"))
+    _report(f"bwd{k} {case[0]}", assert_grad_close(G, R, M, TAU_LAYER, f"backward of launch {k}"))
 
 
 def test_gradient_breakdown_in_float64(vgg):
@@ -180,11 +192,7 @@ def test_gradient_breakdown_in_float64(vgg):
     _, g = eng.perceptual_loss(out, ref, want_grad=True)
     fwd = [eng.debug_vgg_layer(out, k).double() for k in range(20)]
     seed = eng.debug_vgg_layer(out, 21, ref=ref).double()
-    gin = seed
-    for k in range(19, -1, -1):
-        gin, _ = _backward_launch_reference(vgg, fwd, gin, k)
-    std = torch.tensor(STD, dtype=torch.float32).double().view(1, 3, 1, 1).cuda()
-    chain = gin / std
+    chain = V.chain(fwd, seed, _ws(vgg))
     worst = assert_grad_close(g, chain, torch.full_like(chain, chain.abs().max().item()), CHAIN_TAU,
                               "d(out) against the float64 chain of the GPU's decisions")
     e_chain = _rel(g, chain)
@@ -332,6 +340,11 @@ def test_weights_are_repacked_when_they_change(vgg):
     b = perceptual_loss(v, out, ref).item()
     lr, _ = _reference(v, out, ref)
     assert a != b and abs(b - lr.item()) <= 1e-3 * lr.item()
+    with torch.no_grad():  # a bias alone: conv5_4's, which the loss reads directly
+        v.model[-2].bias.add_(0.5)
+    c = perceptual_loss(v, out, ref).item()
+    lr, _ = _reference(v, out, ref)
+    assert c != b and abs(c - lr.item()) <= 1e-3 * lr.item()
 
 
 # ---- training ------------------------------------------------------------------------------------------------------
