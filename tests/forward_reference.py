@@ -180,6 +180,87 @@ def graded_state_dict(sd):
     return sd
 
 
+# ------------------------------------------------------------------ producer / consumer pairs of the e4m3 range guard
+# P -> Q: the layer whose output Q reads.  FP8_PRODUCERS write hi + fp8 planes in the default mode (WRITES_F8), so
+# the range guard of their epilogue decides whether Q's fp8 pass may run; cmg.conv4 is computed in cmg.conv3's
+# epilogue (kFmtFuse1x1).  PLAIN_PRODUCERS write hi / lo planes (or registers): nothing of their output is converted
+# to e4m3, so they must never raise the flag.
+FP8_PRODUCERS = ("cmg.conv1",) + tuple(f"{r}.conv1" for r in ofw.REFINERS) + ("cmg.conv2", "cmg.conv4", "cmg.conv5",
+                                                                              "cmg.conv6")
+PLAIN_PRODUCERS = ("cmg.conv3", "cmg.conv7") + tuple(f"{r}.conv2" for r in ofw.REFINERS)
+E4M3_MAX = 448.0
+
+
+def _chain(producer):
+    stack, name = producer.split(".")
+    names = [n for n, _, _, _ in (ofw.CMG_LAYERS if stack == "cmg" else ofw.REFINER_LAYERS)]
+    return stack, names, names.index(name)
+
+
+def consumer(producer):
+    """The state-dict prefix of the layer that reads ``producer``'s output."""
+    stack, names, i = _chain(producer)
+    return f"{stack}.{names[i + 1]}"
+
+
+def producer_layer(producer):
+    """(debug-layer number, output channel slice) of ``producer``'s activation in ``Engine.debug_layer``'s dump."""
+    stack, _, i = _chain(producer)
+    if stack == "cmg":
+        return i, slice(None)
+    r = ofw.REFINERS.index(stack)
+    return 8 + i, slice(32 * r, 32 * r + 32)
+
+
+def pushed_state_dict(sd, producer, g):
+    """P's weights and bias times g, its consumer Q's weights times 1 / g: the same function, since ReLU commutes with
+    a positive scale.  With g a power of two, and nothing leaving fp32's normal range, the bf16 splits, every fp32
+    product and sum, the bias add, ReLU and the power-of-two fp8 weight scales (ws, s_c) commute with it as well, so
+    only P's own activations change, by exactly g.  ``producer``: a state-dict prefix (``cmg.conv4``,
+    ``gc_refiner.conv1``) or a tuple of them."""
+    sd = {k: v.clone() for k, v in sd.items()}
+    for p in (producer,) if isinstance(producer, str) else producer:
+        q = consumer(p)
+        sd[p + ".weight"] *= g
+        sd[p + ".bias"] *= g
+        sd[q + ".weight"] *= 1.0 / g
+    return sd
+
+
+def boundary_state_dict(sd, producer, channel, value):
+    """Every weight and bias upstream of P and P's own weights zeroed, and P's bias of output ``channel`` set to
+    ``value``: on any input that channel of P's activation is exactly relu(value) at every pixel."""
+    sd = {k: v.clone() for k, v in sd.items()}
+    stack, names, i = _chain(producer)
+    for n in names[:i]:
+        sd[f"{stack}.{n}.weight"].zero_()
+        sd[f"{stack}.{n}.bias"].zero_()
+    sd[producer + ".weight"].zero_()
+    sd[producer + ".bias"][channel] = value
+    return sd
+
+
+# a block of fp8 planes whose largest value is below this is recomputed in bf16x3 (kF8LowMax, DESIGN 4.2)
+F8_LOW_MAX = 2.0 ** -6
+
+
+def trip_gains(m, threshold=E4M3_MAX):
+    """(g_below, g_above) for a producer whose largest activation is m > 0: g_above the smallest power of two with
+    g_above m > threshold, g_below = g_above / 2, so that g_below m lies in (threshold / 2, threshold].  At 448 they
+    are g_safe and g_trip; at F8_LOW_MAX, g_above keeps P in range and g_below trips the low end."""
+    k = int(np.floor(np.log2(threshold / m))) + 1
+    while 2.0 ** k * m <= threshold:
+        k += 1
+    while 2.0 ** (k - 1) * m > threshold:
+        k -= 1
+    return 2.0 ** (k - 1), 2.0 ** k
+
+
+def guard_margin(x, threshold=E4M3_MAX):
+    """|x - threshold| / threshold: how far a pushed maximum is from one of the guard's thresholds."""
+    return abs(x - threshold) / threshold
+
+
 def weight_set(name, seed=0):
     return {"stress": lambda: ofw.synthetic_state_dict(seed, 3.0),
             "default": lambda: ofw.synthetic_state_dict(seed, 1.0),

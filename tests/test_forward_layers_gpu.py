@@ -27,8 +27,9 @@ def _model(sd, precision):
     return m.cuda().eval()
 
 
-def _check_case(m, sd, mode, ins, worst, label):
-    """Every launch of one forward and the gated output; worst[(layer)] keeps the largest excess (|G - R| - F) / M."""
+def _check_case(m, sd, mode, ins, worst, label, forward=True):
+    """Every launch of one forward and the gated output; worst[(layer)] keeps the largest excess (|G - R| - F) / M.
+    forward=False: the launches alone, for weights on which the forward is expected to raise the range flag."""
     eng = m.engine()
     tau = fr.TAU[mode]
     cu = [t.cuda() for t in ins]
@@ -42,6 +43,8 @@ def _check_case(m, sd, mode, ins, worst, label):
         fr.check(G, ref, tau, f"{label} {mode} {fr.LAYER_NAMES[layer]}")
         worst[layer] = max(worst.get(layer, 0.0), fr.excess(G, ref))
         outs[layer] = G
+    if not forward:
+        return
     with torch.no_grad():
         out = m(*cu)
     torch.cuda.synchronize()

@@ -242,6 +242,7 @@ struct UmmaWeights {
   float* scale8[kNumUmmaLayers];     // {ws, 2^-9 / ws, max|w|, -}; kL1: per-column scales (pair_scale_kernel)
   int* overflow_dev;                 // sticky: an activation left the e4m3 range in the fp8-correction mode
   int* overflow_host;                // pinned mirror, refreshed at the end of every forward of that mode
+  unsigned* live_dev;                // per launch: the low-end record of its fp8 planes (ConvArgs::f8_live)
   uint8_t* stages[kNumUmmaLayers];
   float* bias[kNumUmmaLayers];
   float* dense;  // scratch for packing
@@ -265,9 +266,11 @@ int umma_pack_weights(wn_handle* h, const float* const* params, cudaStream_t str
   if (!h->umma->dense) WN_CUDA(cudaMalloc(&h->umma->dense, (size_t)224 * 128 * 49 * sizeof(float)));
   if (!h->umma->overflow_dev) WN_CUDA(cudaMalloc(&h->umma->overflow_dev, sizeof(int)));
   if (!h->umma->overflow_host) WN_CUDA(cudaHostAlloc(&h->umma->overflow_host, sizeof(int), cudaHostAllocDefault));
+  if (!h->umma->live_dev) WN_CUDA(cudaMalloc(&h->umma->live_dev, kNumUmmaLayers * sizeof(unsigned)));
   UmmaWeights* u = h->umma;
   *u->overflow_host = 0;  // new weights: the fp8-correction mode gets a fresh chance
   WN_CUDA(cudaMemsetAsync(u->overflow_dev, 0, sizeof(int), stream));
+  WN_CUDA(cudaMemsetAsync(u->live_dev, 0, kNumUmmaLayers * sizeof(unsigned), stream));
   auto W = [&](int conv) { return params[2 * conv]; };
   auto B = [&](int conv) { return params[2 * conv + 1]; };
   for (int li = 0; li < kNumUmmaLayers; li++) {
@@ -345,6 +348,7 @@ void umma_free(wn_handle* h) {
   if (h->umma->dense) cudaFree(h->umma->dense);
   if (h->umma->overflow_dev) cudaFree(h->umma->overflow_dev);
   if (h->umma->overflow_host) cudaFreeHost(h->umma->overflow_host);
+  if (h->umma->live_dev) cudaFree(h->umma->live_dev);
   free(h->umma);
   h->umma = nullptr;
 }
@@ -402,8 +406,18 @@ static int launch_layer_as(wn_handle* h, int scheme, void* in_base, ConvArgs a, 
   if (scheme == 1) {
     constexpr int FMT =
         (s.f8 ? kFmtIn8 : 0) | (writes_f8(OUT_LI) ? kFmtOut8 : 0) | (pairs_taps(LI) ? kFmtPair8 : 0) | FZ;
-    if constexpr ((FMT & kFmtOut8) != 0) a.f8_overflow = u->overflow_dev;
-    if constexpr (s.f8) a.f8_scale = u->scale8[LI] + 1;
+    if constexpr ((FMT & kFmtOut8) != 0) {
+      a.f8_overflow = u->overflow_dev;
+      a.f8_live = u->live_dev + OUT_LI;
+    }
+    if constexpr (s.f8) {
+      a.f8_scale = u->scale8[LI] + 1;
+      // the planes it reads: L1's refiner blocks for R2, its cmg block for C2, else the launch before (C4: also
+      // when it runs in C3's epilogue)
+      a.f8_overflow = u->overflow_dev;
+      a.f8_live_in = u->live_dev + (LI == kR2 ? kL1 : LI - 1);
+      a.f8_live_need = LI == kR2 ? 0x54u : 0x1u;
+    }
     if constexpr (pairs_taps(LI)) {
       a.f8_scale = u->scale8[LI] + s.npad;
       a.wpk8 = u->stages8[LI];
@@ -480,6 +494,7 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   a.N = n; a.H = H; a.W = W;
   a.run_if = o.run_if;
   a.rwin = o.rwin;
+  a.f8_live_clear = ~0u;
   int rc;
   // fp8-correction scheme (inference): the tensor-bound layers replace the two bf16 correction passes by one
   // fp8 MMA (UmmaCfg FMT); a layer whose consumer is such a layer writes the hi + fp8-planes format
@@ -540,7 +555,9 @@ int umma_forward_layers(wn_handle* h, const float* const in[4], const int64_t st
   if (dump(kL1)) return WN_OK;
   if (want_cmg) {
     act(b.a[2], 128, nullptr, 0);
+    a.f8_live_clear = want_ref ? 0x3u : ~0u;  // L1's refiner blocks are R2's to check and clear
     if ((rc = launch_layer<kC2>(h, sc, b.a[1], a, stream))) return rc;
+    a.f8_live_clear = ~0u;
     if (dump(kC2)) return WN_OK;
     // cmg.conv4 fused into cmg.conv3's launch: its output must not land in b.a[4], the ping-pong buffer of b.a[2]
     // that the same launch's halo loads read, so from cmg.conv4 on every output moves one buffer back (b.a[l - 1])
@@ -619,6 +636,8 @@ int umma_debug_layer(wn_handle* h, const float* const in[4], const int64_t in_st
   }
   int rc = get_encoder();
   if (rc) return rc;
+  // a dump stops the chain before the consumers that check and clear the low-end records
+  WN_CUDA(cudaMemsetAsync(h->umma->live_dev, 0, kNumUmmaLayers * sizeof(unsigned), stream));
   FwdOpts o;
   o.scheme = scheme;
   o.dbg_layer = layer;

@@ -148,6 +148,8 @@ constexpr int kStageLd = 36;       // epilogue staging: floats per row (32 chann
 //        512 threads the register file allows 128 per thread, so the producer warpgroup gives its registers up
 //        (setmaxnreg) and the consumers run at kWgs3ConsumerRegs.
 constexpr int kFmtIn8 = 1, kFmtOut8 = 2, kFmtHi = 4, kFmtPair8 = 8, kFmtFuse1x1 = 16;
+// The low end of e4m3 (DESIGN 4.2): a block of fp8 planes whose largest value is below this is recomputed in bf16x3
+constexpr float kF8LowMax = 0.015625f;  // 2^-6, e4m3's smallest normal
 // kFmtFuse1x1: output channels of the fused 1x1 layer, and its weight stages per tile (its 16-channel chunks, 4 KB
 // each in the CONCAT layout, UmmaCfg::FUSE_CHUNKS to a stage)
 constexpr int kFuseNpad = 64, kFuseStages = 2;
@@ -263,8 +265,18 @@ struct ConvArgs {
   // the form per window with it (its windows come from images of every kind); otherwise *skip_lo decides
   const int* slot_levels;
   // FMT bit 1: sticky device flag raised when an activation leaves the e4m3 range (its correction terms would
-  // saturate in the consumer's fp8 pass); the host side then re-runs the batch with the bf16x3 kernels
+  // saturate in the consumer's fp8 pass); the host side then re-runs the batch with the bf16x3 kernels.  FMT bit 0
+  // raises it too, for operands at e4m3's low end (f8_live_in)
   int* f8_overflow;
+  // FMT bit 1: the low end of the launch's output, per block b of its columns (L1: block 0 the cmg's 128, blocks 1-3
+  // the refiners' 32 each; one block elsewhere): bit 2b once a value of the block is nonzero, bit 2b + 1 once one is
+  // at least kF8LowMax.  Each consumer warp ORs what it stored into it when it is done
+  unsigned* f8_live;
+  // FMT bit 0: the f8_live word of the launch whose fp8 planes this one reads.  Before anything else one thread checks
+  // the blocks of f8_live_need (their bits 2b): a block that is nonzero with no value of kF8LowMax or more raises
+  // f8_overflow; then it clears the bits of f8_live_clear for the next pass
+  unsigned* f8_live_in;
+  unsigned f8_live_need, f8_live_clear;
   // conditional launch: when non-null and *run_if == 0 the kernel returns at once (the bf16x3 re-run of a
   // batch is enqueued unconditionally behind the fp8-correction pass and only does work if the flag is up)
   const int* run_if;
@@ -299,13 +311,14 @@ __device__ __forceinline__ void split_bf16x2(float f0, float f1, uint32_t& hi, u
 // RAG: `valid` is false at slot pixels outside the window's valid extent, where kEpiAct stores zeros (hi, lo and
 // fp8 planes alike; they cannot raise the e4m3 flag).
 // HI (kFmtHi): the planes hold bf16(v) and lo = 0.
+// Returns OUT8's ConvArgs::f8_live bits of the 16 values (0 otherwise).
 template <int EPI, bool OUT8, bool RAG = false, bool HI = false>
-__device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bias, const float* f, int ch, int n,
+__device__ __forceinline__ unsigned epilogue16(const ConvArgs& g, const float* s_bias, const float* f, int ch, int n,
                                            int gx, int gy, bool valid = true) {
   const size_t hw = (size_t)g.H * g.W;
   const size_t pix = (size_t)gy * g.W + gx;
   if constexpr (EPI == kEpiAct || EPI == kEpiDgrad) {
-    if (ch >= g.cout) return;
+    if (ch >= g.cout) return 0u;
     if constexpr (OUT8) {
       // hi planes as usual; where the bf16 lo planes would be: per 16 channels one plane of
       // e4m3((v - hi) * 2^9) and one of e4m3(v) -- the K = 32 operand of the consumer's fp8 pass
@@ -331,17 +344,19 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
         l8[j >> 2] = pack_e4m3x4(r[0], r[1], r[2], r[3]);
         h8[j >> 2] = pack_e4m3x4(v[0], v[1], v[2], v[3]);
       }
-      // e4m3 range guard (|v| <= 448); written as !(<=) so that a NaN raises the flag too
+      // e4m3 range guard (|v| <= 448).  v is past the ReLU, whose fmaxf has already turned a NaN into 0; +inf raises it
       if (!(vmax <= 448.f) && g.f8_overflow) atomicOr(g.f8_overflow, 1);
       const bool second = ch >= g.split_c;
       const ActDst& d = second ? g.dst1 : g.dst0;
       const int chl = second ? ch - g.split_c : ch;
+      const unsigned live = vmax > 0.f ? (vmax >= kF8LowMax ? 3u : 1u) << (second ? 2 + 2 * (chl >> 5) : 0) : 0u;
       uint4* p_hi = d.base + ((size_t)n * 2 * d.planes_half + (chl >> 3)) * hw + pix;
       uint4* p_f8 = d.base + ((size_t)n * 2 * d.planes_half + d.planes_half + 2 * (chl >> 4)) * hw + pix;
       p_hi[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
       p_hi[hw] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
       p_f8[0] = make_uint4(l8[0], l8[1], l8[2], l8[3]);
       p_f8[hw] = make_uint4(h8[0], h8[1], h8[2], h8[3]);
+      return live;
     } else {
 #pragma unroll
       for (int q = 0; q < 16; q += 8) {  // one 8-channel plane at a time
@@ -386,7 +401,7 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
       }
     }
   } else {
-    if (ch != 0) return;
+    if (ch != 0) return 0u;
     const size_t o = (size_t)n * 3 * hw + pix;
     if constexpr (EPI == kEpiSigmoid) {
 #pragma unroll
@@ -411,7 +426,7 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
         if constexpr (RAG) {  // slot pixel -> pixel of the window's own image; only the kept rectangle is stored
           const RaggedWindow& t = g.rwin[n];
           const int y = t.ys + gy, x = t.xs + gx;
-          if (y < t.ky0 || y >= t.ky1 || x < t.kx0 || x >= t.kx1) return;
+          if (y < t.ky0 || y >= t.ky1 || x < t.kx0 || x >= t.kx1) return 0u;
           ohw = (size_t)t.H * t.W;
           oo = (size_t)y * t.W + x;
           o8 = oo * 3;
@@ -420,7 +435,7 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
         } else if (g.tiled) {  // window pixel -> image pixel; the halo around the kept rectangle is not stored
           const TileWindow t = tile_window(g.tiles, g.win0 + n);
           const int y = t.ys + gy, x = t.xs + gx;
-          if (y < t.ky0 || y >= t.ky1 || x < t.kx0 || x >= t.kx1) return;
+          if (y < t.ky0 || y >= t.ky1 || x < t.kx0 || x >= t.kx1) return 0u;
           ohw = (size_t)g.tiles.H * g.tiles.W;
           const size_t ipix = (size_t)y * g.tiles.W + x;
           oo = (size_t)t.img * 3 * ohw + ipix;
@@ -438,6 +453,7 @@ __device__ __forceinline__ void epilogue16(const ConvArgs& g, const float* s_bia
       }
     }
   }
+  return 0u;
 }
 
 // RAG: a pass of a ragged batch (ConvArgs::rwin).  Work item t is pixel tile t / NG, column group t % NG, so the
@@ -451,6 +467,11 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
   static_assert(!OUT8 || EPI == kEpiAct, "fp8 planes are written by the activation epilogue only");
   static_assert(!RAG || EPI == kEpiAct || EPI == kEpiGate, "ragged passes mask activations and store the gate");
   if (g.run_if != nullptr && *reinterpret_cast<const volatile int*>(g.run_if) == 0) return;  // whole grid alike
+  if constexpr (F8IN)  // the producer of this launch's fp8 planes has completed (stream order): check its low end
+    if (g.f8_live_in != nullptr && blockIdx.x == 0 && threadIdx.x == 0) {
+      const unsigned w = atomicAnd(g.f8_live_in, ~g.f8_live_clear);
+      if (w & ~(w >> 1) & g.f8_live_need) atomicOr(g.f8_overflow, 1);
+    }
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* a_stages = smem;
@@ -569,6 +590,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
     }
     pend_a = pend_b = -1;
   };
+  unsigned live = 0u;  // OUT8: ConvArgs::f8_live bits of every value this thread stores
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const bool pair = pair_tile(tile);
 #pragma unroll
@@ -825,7 +847,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
             const float4 x = s[q];
             f[4 * q] = x.x; f[4 * q + 1] = x.y; f[4 * q + 2] = x.z; f[4 * q + 3] = x.w;
           }
-          epilogue16<EPI, OUT8, RAG, C::HI>(g, e_bias, f, c0 + cb, n, gx, gy, valid);
+          live |= epilogue16<EPI, OUT8, RAG, C::HI>(g, e_bias, f, c0 + cb, n, gx, gy, valid);
         }
         wg_bar(1 + wg);
       }
@@ -834,6 +856,10 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmap_in, const ConvArgs g) 
       if (lane == 0)
 #pragma unroll
         for (int s = 0; s < kFuseStages; s++) mbar_arrive(&b_empty[fuse_stage[s]]);
+  }
+  if constexpr (OUT8) {  // the low-end record of what this warp stored: one atomic per warp
+    live = __reduce_or_sync(0xffffffffu, live);
+    if (lane == 0 && live != 0u && g.f8_live != nullptr) atomicOr(g.f8_live, live);
   }
 }
 
